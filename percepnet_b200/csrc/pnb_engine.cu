@@ -368,7 +368,7 @@ extern "C" int pnb_create(pnb_engine **out, int n_streams, int max_frames, const
     if (rp) e->ramp = atoi(rp) != 0;
     const bool worth = (long long)n_streams >= 2048 && max_frames >= 2 * e->chunk && (max_frames + e->chunk - 1) / e->chunk + 5 <= kMaxChunks;
     if (!(ov && atoi(ov) == 0) && (worth || (ov && atoi(ov) == 2)) && max_frames >= 2 * e->chunk)
-      setup_overlap(e, ns && atoi(ns) >= 8 ? atoi(ns) : (e->sm_count * 7 / 16 / 8) * 8);
+      setup_overlap(e, ns && atoi(ns) >= 8 ? atoi(ns) : (e->sm_count * 2 / 3 / 8) * 8);  // 88 of an H100's 132 (DESIGN §4)
   }
   CKD(cudaDeviceSynchronize());
   *out = e;

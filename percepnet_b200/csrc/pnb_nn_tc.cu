@@ -14,19 +14,21 @@
 // Two kernels, both persistent and warp-specialised, one CTA of three warpgroups per SM:
 //   tc_gemm_kernel   one dense layer over all rows (conv1, conv2, fc_gb, fc_rb run once per call over F*S rows)
 //   gru_chain_kernel the five GRUs of all F hops of a call in ONE launch.  A tile (hop, layer, 128 streams,
-//                    32 hidden units) depends only on tiles of the same 128 streams (layer below at this hop,
+//                    64 hidden units) depends only on tiles of the same 128 streams (layer below at this hop,
 //                    own layer at the previous hop), so the recurrence is a per-(layer, row tile) counter that
 //                    the consumer warps bump (release) and the TMA producer polls (acquire) -- no grid barrier,
 //                    no launch boundary between layers or hops.
-// Warpgroup roles per CTA: warpgroup 0 = TMA producer (one thread: cp.async.bulk.tensor, SWIZZLE_128B boxes of 64 k
-// into a ring of stages guarded by full / empty mbarriers), warpgroups 1 and 2 = consumers: each issues wgmma for 64
-// of the tile's 128 rows (m64nNk16, operands from shared memory, fp32 accumulators in registers) and runs the
-// epilogue of its rows.  The producer streams the next tile's operands while the consumers finish the current one.
+// Warpgroup roles per CTA: warpgroup 0 = TMA producer (one thread: cp.async.bulk.tensor into a ring of stages guarded
+// by full / empty mbarriers; dense layers SWIZZLE_128B boxes of 64 k, the chain SWIZZLE_64B boxes of 32 k),
+// warpgroups 1 and 2 = consumers: each issues wgmma for 64 of the tile's 128 rows (m64nNk16, operands from shared
+// memory, fp32 accumulators in registers) and runs the epilogue of its rows.  The producer streams the next tile's
+// operands while the consumers finish the current one.
 //
-// The GRU tile holds, for 32 hidden units, four accumulators per unit (z, r, W_n x, U_n h: nnet.cpp:136-173
-// needs the last two apart), 128 accumulator columns [nx | z | r | nh]; weight rows are packed gate-interleaved per
-// tile (input part [n|z|r], recurrent part [z|r|n]) so that one TMA box brings a tile's rows and ONE N = 96 MMA
-// per product covers either part (at accumulator column 0 and 32 respectively).
+// The GRU tile holds, for 64 hidden units, three accumulators per unit: z and r summed over [x ; h], and the
+// candidate's W_n x and U_n h apart (nnet.cpp:136-173 needs the last two apart) -- 256 accumulator columns in three
+// register blocks nx (64), zr (128), nh (64).  Weight rows are packed [z|r|n] per tile in both parts, so one TMA box
+// brings a tile's rows; per product the input part issues N = 128 into zr and N = 64 into nx, the recurrent part
+// N = 128 into zr and N = 64 into nh.
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -45,8 +47,9 @@ using namespace pnb;
 namespace {
 
 constexpr int TM = 128;   // streams per CTA tile: two consumer warpgroups of 64 rows
-constexpr int BK = 64;    // k per pipeline stage: 128-byte rows, SWIZZLE_128B
-constexpr int HT = 32;    // hidden units per GRU tile
+constexpr int BK = 64;    // k per pipeline stage of the dense layers: 128-byte rows, SWIZZLE_128B
+constexpr int CBK = 32;   // k per pipeline stage of the GRU chain: 64-byte rows, SWIZZLE_64B (five 40 KB stages fit)
+constexpr int HT = 64;    // hidden units per GRU tile
 constexpr int GRU_BN = 3 * HT;  // weight rows per GRU tile (z|r|n)
 constexpr int kConsumerWGs = 2;
 constexpr int kTcThreads = 128 * (1 + kConsumerWGs);
@@ -100,9 +103,12 @@ __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.
 // The high word is a constant; the low word is (address >> 4) | LBO and advances by plain addition, 32 bytes per
 // 16-wide k-step inside the 128-byte row and 1024 bytes per 8 rows (the shared window is < 256 KB, so the 14-bit
 // field never carries).  Tiles are 1024-byte aligned (the swizzle is a function of the address bits).
+// SWIZZLE_64B (the GRU chain): rows of 64 bytes, 8-row groups 512 bytes apart, SBO>>4 = 32, layout = 2; the k-step
+// advance is the same 32 bytes.
 constexpr uint32_t kDescHi = (uint32_t)(1024 >> 4) | (1u << 30);
+constexpr uint32_t kDescHi64 = (uint32_t)(512 >> 4) | (2u << 30);
 __device__ __forceinline__ uint32_t desc_lo(uint32_t saddr) { return ((saddr >> 4) & 0x3FFF) | (1u << 16); }
-__device__ __forceinline__ uint64_t desc64(uint32_t lo) { return ((uint64_t)kDescHi << 32) | lo; }
+__device__ __forceinline__ uint64_t desc64(uint32_t lo, uint32_t hi = kDescHi) { return ((uint64_t)hi << 32) | lo; }
 
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
@@ -115,14 +121,15 @@ __device__ __forceinline__ void acc_fence(float *d) {
   for (int i = 0; i < R; i++) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// D[64 x N] += A[64 x 16] B[N x 16]^T, fp32 accumulators in registers (m64nNk16 fragment: register 4j + q holds row
-// 16 warp + lane/4 + 8 (q/2), column 8j + 2 (lane%4) + q%2)
+// D[64 x N] = (acc ? D : 0) + A[64 x 16] B[N x 16]^T, fp32 accumulators in registers (m64nNk16 fragment: register
+// 4j + q holds row 16 warp + lane/4 + 8 (q/2), column 8j + 2 (lane%4) + q%2).  acc = 0 starts a sum without a
+// zero fill of the registers: a fill that the compiler places while earlier MMAs are in flight serialises them.
 template <int N, bool BF16>
-__device__ __forceinline__ void wgmma(float *d, uint64_t da, uint64_t db);
-#define PNB_WGMMA_PRED "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+__device__ __forceinline__ void wgmma(float *d, uint64_t da, uint64_t db, uint32_t acc = 1);
+#define PNB_WGMMA_PRED(ACC) "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %" #ACC ", 0;\n\t"
 template <>
-__device__ __forceinline__ void wgmma<128, true>(float *d, uint64_t da, uint64_t db) {
-  asm volatile(PNB_WGMMA_PRED
+__device__ __forceinline__ void wgmma<128, true>(float *d, uint64_t da, uint64_t db, uint32_t acc) {
+  asm volatile(PNB_WGMMA_PRED(66)
       "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, "
       "%15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, "
       "%39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, "
@@ -134,31 +141,44 @@ __device__ __forceinline__ void wgmma<128, true>(float *d, uint64_t da, uint64_t
         "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]),
         "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]),
         "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
-      : "l"(da), "l"(db));
+      : "l"(da), "l"(db), "r"(acc));
 }
 template <>
-__device__ __forceinline__ void wgmma<96, false>(float *d, uint64_t da, uint64_t db) {
-  asm volatile(PNB_WGMMA_PRED
-      "wgmma.mma_async.sync.aligned.m64n96k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, "
+__device__ __forceinline__ void wgmma<128, false>(float *d, uint64_t da, uint64_t db, uint32_t acc) {
+  asm volatile(PNB_WGMMA_PRED(66)
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, "
       "%15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, "
-      "%39, %40, %41, %42, %43, %44, %45, %46, %47}, %48, %49, p, 1, 1, 0, 0;\n\t}"
+      "%39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, "
+      "%63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]),
         "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]),
         "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]),
         "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]),
         "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]),
-        "+f"(d[46]), "+f"(d[47])
-      : "l"(da), "l"(db));
+        "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]),
+        "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(da), "l"(db), "r"(acc));
 }
 template <>
-__device__ __forceinline__ void wgmma<48, false>(float *d, uint64_t da, uint64_t db) {
-  asm volatile(PNB_WGMMA_PRED
+__device__ __forceinline__ void wgmma<64, false>(float *d, uint64_t da, uint64_t db, uint32_t acc) {
+  asm volatile(PNB_WGMMA_PRED(34)
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, "
+      "%15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]),
+        "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]),
+        "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]),
+        "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(da), "l"(db), "r"(acc));
+}
+template <>
+__device__ __forceinline__ void wgmma<48, false>(float *d, uint64_t da, uint64_t db, uint32_t acc) {
+  asm volatile(PNB_WGMMA_PRED(26)
       "wgmma.mma_async.sync.aligned.m64n48k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, "
       "%15, %16, %17, %18, %19, %20, %21, %22, %23}, %24, %25, p, 1, 1, 0, 0;\n\t}"
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]),
         "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]),
         "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])
-      : "l"(da), "l"(db));
+      : "l"(da), "l"(db), "r"(acc));
 }
 #undef PNB_WGMMA_PRED
 
@@ -208,10 +228,10 @@ __device__ __forceinline__ void store_split_b2(float v0, float v1, __nv_bfloat16
 }
 
 // ------------------------------------------------------------------------------------------ shared kernel pieces
-template <int BN, int NT = 2>
-struct StageLayout {  // NT terms of A (the tile's 128 rows), then NT terms of the BN rows of B
-  static constexpr int kABytes = TM * BK * 2;
-  static constexpr int kBBytes = BN * BK * 2;
+template <int BN, int NT = 2, int KB = BK>
+struct StageLayout {  // NT terms of A (the tile's 128 rows), then NT terms of the BN rows of B, KB k each
+  static constexpr int kABytes = TM * KB * 2;
+  static constexpr int kBBytes = BN * KB * 2;
   static constexpr int kBytes = NT * (kABytes + kBBytes);
 };
 
@@ -267,23 +287,19 @@ __device__ __forceinline__ void tc_prologue(const SmemCarve &c, const float *tan
 // 16-wide k-steps.  `a_lo` is the descriptor low word of this warpgroup's rows in the stage's first A term, `b_lo` that
 // of the stage's first B term.  Two terms per operand: hi hi, hi lo, lo hi.  Three terms (t0 t1 t2, each 8 bits below
 // the previous): the six products of total order <= 2.
-// PASS < 0: all products of the k-block at once (GRU chain: operands bounded by 1, sums of a few units).
-// PASS >= 0 (dense layers, whose ReLU inputs are unbounded): the K loop runs once per product order, smallest products
-// first (three terms: PASS 0 order 2, PASS 1 order 1, PASS 2 t0 t0; two terms: PASS 1, PASS 2).  The tensor core adds
+// The dense layers' ReLU inputs are unbounded, so the K loop runs once per product order, smallest products first
+// (three terms: PASS 0 order 2, PASS 1 order 1, PASS 2 t0 t0; two terms: PASS 1, PASS 2).  The tensor core adds
 // into the fp32 accumulator with truncation at the accumulator's magnitude, so correction products added to an already
-// large sum lose exactly the bits they were meant to supply; summed among themselves first, they do not.
-template <int BN, int N, bool BF16, int NT, int PASS = -1>
+// large sum lose exactly the bits they were meant to supply; summed among themselves first, they do not.  (The GRU
+// chain, whose operands are bounded by 1, issues all products of a k-block at once: gru_mma_kblock.)
+template <int BN, int N, bool BF16, int NT, int PASS>
 __device__ __forceinline__ void mma_kblock(float *acc, uint32_t a_lo, uint32_t b_lo) {
   using SL = StageLayout<BN, NT>;
   constexpr uint32_t A = SL::kABytes >> 4, B = SL::kBBytes >> 4;
 #pragma unroll
   for (int ks = 0; ks < BK / 16; ks++) {
     const uint32_t a = a_lo + ks * 2, b = b_lo + ks * 2;
-    if (NT == 2 && PASS < 0) {
-      wgmma<N, BF16>(acc, desc64(a), desc64(b));
-      wgmma<N, BF16>(acc, desc64(a), desc64(b + B));
-      wgmma<N, BF16>(acc, desc64(a + A), desc64(b));
-    } else if (NT == 2 && PASS == 1) {
+    if (NT == 2 && PASS == 1) {
       wgmma<N, BF16>(acc, desc64(a), desc64(b + B));
       wgmma<N, BF16>(acc, desc64(a + A), desc64(b));
     } else if (NT == 2) {
@@ -496,7 +512,7 @@ struct ChainLayer {
   int x_row1[2];        // 0: the segment is indexed by hop (conv2 out, slot t); 1: state slots (slot t+1 = after hop t)
   int x_term_rows[2];   // row distance between the two split terms in that buffer
   int h_map, w_map, u_map;
-  int h_kb;             // H / BK
+  int h_kb;             // H / CBK
   int H;
   int tiles_log2;       // log2(H / HT)
   int b_term_rows;      // rows of one term plane of the packed weights
@@ -594,14 +610,39 @@ __device__ __forceinline__ void wait_layer(const ChainArgs &a, int layer, int mp
     if (++spins > (1u << 26)) __trap();  // tens of seconds: a broken schedule becomes a launch error, not a hang
 }
 
-constexpr int GRU_STAGES = 4;
+constexpr int GRU_STAGES = 5;
+using GruStage = StageLayout<GRU_BN, 2, CBK>;  // 2 x 8 KB of A + 2 x 12 KB of B = 40 KB
+// Registers per thread after the producer warpgroup hands its surplus to the consumers (setmaxnreg): the launch
+// gives 168 to each of the 384 threads; 128 x (168 - 40) = 256 x (232 - 168).
+constexpr int kProducerRegs = 40, kConsumerRegs = 232;
+
+// One k-block (CBK = two 16-wide k-steps) of a GRU tile on one consumer warpgroup: per k-step the three products
+// hi hi, hi lo, lo hi of weight rows [z|r] (N = 128) into `zr` and of rows [n] (N = 64) into `n`, the two register
+// blocks alternating so that consecutive MMAs do not wait on each other's accumulators.  zr_acc / n_acc = 0: the
+// k-block starts the block's sum (its first MMA overwrites the registers).
+__device__ __forceinline__ void gru_mma_kblock(float *zr, float *n, uint32_t a_lo, uint32_t b_lo, uint32_t zr_acc, uint32_t n_acc) {
+  constexpr uint32_t A = GruStage::kABytes >> 4, B = GruStage::kBBytes >> 4;
+  constexpr uint32_t BN = (2 * HT * CBK * 2) >> 4;  // the n rows follow the 2 HT rows of [z|r]
+#pragma unroll
+  for (int ks = 0; ks < CBK / 16; ks++) {
+    const uint32_t a = a_lo + ks * 2, b = b_lo + ks * 2;
+    wgmma<128, false>(zr, desc64(a, kDescHi64), desc64(b, kDescHi64), ks ? 1u : zr_acc);
+    wgmma<64, false>(n, desc64(a, kDescHi64), desc64(b + BN, kDescHi64), ks ? 1u : n_acc);
+    wgmma<128, false>(zr, desc64(a, kDescHi64), desc64(b + B, kDescHi64));
+    wgmma<64, false>(n, desc64(a, kDescHi64), desc64(b + B + BN, kDescHi64));
+    wgmma<128, false>(zr, desc64(a + A, kDescHi64), desc64(b, kDescHi64));
+    wgmma<64, false>(n, desc64(a + A, kDescHi64), desc64(b + BN, kDescHi64));
+  }
+}
 
 __global__ void __launch_bounds__(kTcThreads, 1) gru_chain_kernel(const __grid_constant__ ChainArgs args) {
-  using SL = StageLayout<GRU_BN>;
+  using SL = GruStage;
   constexpr int STAGES = GRU_STAGES;
-  // accumulator registers per thread: input part columns [nx | z | r], then recurrent part columns [z | r | nh]
-  // (two separate register blocks: wgmma into overlapping register ranges would serialise the MMA pipeline)
-  constexpr int R = 2 * GRU_BN / 2;
+  // accumulator registers per thread, three blocks: nx = W_n x (64 columns), zr = [z | r] over [x ; h] (128 columns),
+  // nh = U_n h (64 columns).  The blocks never overlap partially: wgmma into partly overlapping register ranges
+  // would serialise the MMA pipeline.
+  constexpr int R = 4 * HT / 2;
+  constexpr int NX = 0, ZR = HT / 2, NH = 3 * HT / 2;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   const SmemCarve c = carve<STAGES, STAGES * SL::kBytes>(smem_raw);
   const int wg = threadIdx.x >> 7;
@@ -612,6 +653,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) gru_chain_kernel(const __grid_c
 
   if (wg == 0) {
     // ===== TMA producer: waits for the rows it is about to read, then streams the tile's operands =====
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kProducerRegs));
     if (threadIdx.x != 0) return;
     Pipe p;
     for (int u = blockIdx.x; u < total_units; u += gridDim.x) {
@@ -634,18 +676,19 @@ __global__ void __launch_bounds__(kTcThreads, 1) gru_chain_kernel(const __grid_c
           const uint32_t fb = c.full + 8 * p.st;
           mbar_expect_tx(fb, SL::kBytes);
           const uint32_t sp = stage0 + p.st * SL::kBytes;
-          tma_load_2d(sp, ma, fb, kb * BK, arow);
-          tma_load_2d(sp + SL::kABytes, ma, fb, kb * BK, aterm + arow);
-          tma_load_2d(sp + 2 * SL::kABytes, mb, fb, bk0 + kb * BK, brow);
-          tma_load_2d(sp + 2 * SL::kABytes + SL::kBBytes, mb, fb, bk0 + kb * BK, L.b_term_rows + brow);
+          tma_load_2d(sp, ma, fb, kb * CBK, arow);
+          tma_load_2d(sp + SL::kABytes, ma, fb, kb * CBK, aterm + arow);
+          tma_load_2d(sp + 2 * SL::kABytes, mb, fb, bk0 + kb * CBK, brow);
+          tma_load_2d(sp + 2 * SL::kABytes + SL::kBBytes, mb, fb, bk0 + kb * CBK, L.b_term_rows + brow);
           p.advance(STAGES);
         }
       }
     }
   } else {
     // ===== consumer warpgroup: MMAs of its 64 streams, then the gate math of nnet.cpp:136-178 (reset_after) =====
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kConsumerRegs));
     const int cw = wg - 1, warp = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
-    const uint32_t a_lo0 = desc_lo(stage0) + (uint32_t)(cw * 64 * 128 >> 4);
+    const uint32_t a_lo0 = desc_lo(stage0) + (uint32_t)(cw * 64 * CBK * 2 >> 4);
     const uint32_t b_lo0 = desc_lo(stage0) + (uint32_t)(2 * SL::kABytes >> 4);
     const float *tbl = c.tbl;
     Pipe p;
@@ -654,23 +697,21 @@ __global__ void __launch_bounds__(kTcThreads, 1) gru_chain_kernel(const __grid_c
       const Unit un = decode_unit(args, u);
       const ChainLayer &L = args.L[un.l];
       const int H = L.H;
-      float acc[R];
-#pragma unroll
-      for (int i = 0; i < R; i++) acc[i] = 0.f;
-      // input part (weight rows [n|z|r]) into acc[0, 48), recurrent part (rows [z|r|n]) into acc[48, 96)
+      float acc[R];  // no zero fill: the first k-block of either part starts its blocks' sums
+      // input part: [z|r] rows into zr, n rows into nx; recurrent part: [z|r] rows into zr, n rows into nh
       int nkb = 0;
       for (int s = 0; s < L.n_x; s++) nkb += L.x_kb[s];
       for (int kb = 0; kb < nkb; kb++) {
         cons.begin(acc, c.full + 8 * p.st, p.ph);
         const uint32_t so = p.st * (SL::kBytes >> 4);
-        mma_kblock<GRU_BN, GRU_BN, false, 2>(acc, a_lo0 + so, b_lo0 + so);
+        gru_mma_kblock(acc + ZR, acc + NX, a_lo0 + so, b_lo0 + so, kb != 0, kb != 0);
         cons.end(acc, c.empty + 8 * p.st);
         p.advance(STAGES);
       }
       for (int kb = 0; kb < L.h_kb; kb++) {
         cons.begin(acc, c.full + 8 * p.st, p.ph);
         const uint32_t so = p.st * (SL::kBytes >> 4);
-        mma_kblock<GRU_BN, GRU_BN, false, 2>(acc + GRU_BN / 2, a_lo0 + so, b_lo0 + so);
+        gru_mma_kblock(acc + ZR, acc + NH, a_lo0 + so, b_lo0 + so, 1u, kb != 0);
         cons.end(acc, c.empty + 8 * p.st);
         p.advance(STAGES);
       }
@@ -696,14 +737,13 @@ __global__ void __launch_bounds__(kTcThreads, 1) gru_chain_kernel(const __grid_c
           float hn[2];
 #pragma unroll
           for (int q = 0; q < 2; q++) {
-            const int i = 4 * j + 2 * h + q;  // fragment register of this (row, unit) inside a 32-column group
-            const float *ax = acc, *ah = acc + GRU_BN / 2;
+            const int i = 4 * j + 2 * h + q;  // fragment register of this (row, unit) inside a 64-column group
             const float4 bb = __ldg(L.bias4 + unit + q);
-            const float z = sigmoid_s(fmaf(ax[HT / 2 + i] + ah[i], sc, bb.x), tbl);
-            const float r = sigmoid_s(fmaf(ax[HT + i] + ah[HT / 2 + i], sc, bb.y), tbl);
-            const float tmp = fmaf(ah[HT + i], sc, bb.w);
+            const float z = sigmoid_s(fmaf(acc[ZR + i], sc, bb.x), tbl);
+            const float r = sigmoid_s(fmaf(acc[ZR + HT / 2 + i], sc, bb.y), tbl);
+            const float tmp = fmaf(acc[NH + i], sc, bb.w);
             float cnd = fmaf(tmp, r, bb.z);
-            cnd = fmaf(ax[i], sc, cnd);
+            cnd = fmaf(acc[NX + i], sc, cnd);
             const float n = tansig_s(cnd, tbl);
             hn[q] = fmaf(z, (q ? ho.y : ho.x) - n, n);  // z h + (1 - z) n
           }
@@ -830,7 +870,8 @@ struct pnb_tc_state {
   int *wide = nullptr;                                   // see kConvTerms
   int tiles_mp = 0;
   // tensor maps
-  CUtensorMap m_fc_all, m_c1_all, m_c2, m_h[5], m_wconv1, m_wconv2, m_w[5], m_u[5], m_wgb, m_wrb;
+  CUtensorMap m_fc_all, m_c1_all, m_c2, m_h[5], m_wconv1, m_wconv2, m_wgb, m_wrb;  // dense layers: 64-k boxes, SW128
+  CUtensorMap m_c2_ch, m_h_ch[5], m_w[5], m_u[5];                                   // GRU chain: 32-k boxes, SW64
 };
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *,
@@ -839,14 +880,16 @@ typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t
 static EncodeTiledFn g_encode = nullptr;
 static std::string g_tc_err;
 
-static int make_map(CUtensorMap *m, const void *base, bool bf16, uint64_t rows, uint64_t cols, uint32_t box_rows) {
+// boxes of box_k x box_rows; the dense layers read 64 k (SWIZZLE_128B), the GRU chain 32 k (SWIZZLE_64B)
+static int make_map(CUtensorMap *m, const void *base, bool bf16, uint64_t rows, uint64_t cols, uint32_t box_rows,
+                    uint32_t box_k = BK, CUtensorMapSwizzle swizzle = CU_TENSOR_MAP_SWIZZLE_128B) {
   cuuint64_t dims[2] = {cols, rows};
   cuuint64_t strides[1] = {cols * 2};
-  cuuint32_t box[2] = {(cuuint32_t)BK, box_rows};
+  cuuint32_t box[2] = {box_k, box_rows};
   cuuint32_t estr[2] = {1, 1};
   CUresult r = g_encode(m, bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2,
                         const_cast<void *>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                        CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+                        swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   return r == CUDA_SUCCESS ? 0 : (int)r;
 }
 
@@ -875,18 +918,16 @@ extern int tc_fail(int code, const char *msg);  // sets pnb_last_error (pnb_engi
     }                                                                                      \
   } while (0)
 
-// GRU weights: reference layout W[j*3H + g*H + i] -> K-major rows ordered [tile][gate][64 units], scaled, split
-// `order` lists the reference gate index (0 z, 1 r, 2 n) of each 64-row group of a tile: input weights are packed
-// [n | z | r], recurrent weights [z | r | n], so that either part is ONE N = 192 MMA onto the accumulator columns
-// [nx | z | r | nh] (at column 0 and at column 64 respectively).
-static void pack_gru(const float *W, int K, int H, float scale, const int order[3], std::vector<__half> &out) {
+// GRU weights: reference layout W[j*3H + g*H + i] -> K-major rows ordered [tile][gate z, r, n][HT units], scaled,
+// split into two fp16 terms.  Input and recurrent weights alike: the first 2 HT rows of a tile are the N = 128 MMA
+// onto the zr accumulators, the last HT rows the N = 64 MMA onto nx (input) or nh (recurrent).
+static void pack_gru(const float *W, int K, int H, float scale, std::vector<__half> &out) {
   const int tiles = H / HT, rows = tiles * GRU_BN;
   out.assign((size_t)2 * rows * K, __float2half(0.f));
   for (int tl = 0; tl < tiles; tl++)
-    for (int gq = 0; gq < 3; gq++)
+    for (int g = 0; g < 3; g++)
       for (int ii = 0; ii < HT; ii++) {
-        const int g = order[gq];
-        const int row = tl * GRU_BN + gq * HT + ii, i = tl * HT + ii;
+        const int row = tl * GRU_BN + g * HT + ii, i = tl * HT + ii;
         for (int j = 0; j < K; j++) {
           float w = W[(size_t)j * 3 * H + g * H + i] * scale;
           __half hi = __float2half_rn(w);
@@ -1010,10 +1051,9 @@ int tc_prepare(pnb_engine *e, const pnb_model *model) {
     float sc = pow2_scale_for(g5[i]->input_weights, (size_t)K * 3 * H, g5[i]->recurrent_weights, (size_t)H * 3 * H, &ex);
     t->scale_gru[i] = ldexpf(1.f, -(10 + ex));
     std::vector<__half> p;
-    const int order_w[3] = {2, 0, 1}, order_u[3] = {0, 1, 2};
-    pack_gru(g5[i]->input_weights, K, H, sc, order_w, p);
+    pack_gru(g5[i]->input_weights, K, H, sc, p);
     TCK(dev_upload(&t->w_gru[i], p));
-    pack_gru(g5[i]->recurrent_weights, H, H, sc, order_u, p);
+    pack_gru(g5[i]->recurrent_weights, H, H, sc, p);
     TCK(dev_upload(&t->u_gru[i], p));
     // nnet.cpp:136-160: z and r start from b + b' (one float add), the candidate keeps b_n and b'_n apart
     const float *b = g5[i]->bias;
@@ -1049,14 +1089,18 @@ int tc_prepare(pnb_engine *e, const pnb_model *model) {
     bad |= make_map(&t->m_h[i], t->h_all[i], false, 2 * (Fm + 1) * S, e->gru[i].H, TM);
   bad |= make_map(&t->m_wconv1, t->w_conv1, true, kConvTerms * 512, 640, DENSE_BN);
   bad |= make_map(&t->m_wconv2, t->w_conv2, true, kConvTerms * 512, 1536, DENSE_BN);
+  // the chain's operands: the same buffers in boxes of 32 k
+  const CUtensorMapSwizzle sw64 = CU_TENSOR_MAP_SWIZZLE_64B;
+  bad |= make_map(&t->m_c2_ch, t->c2_h, false, 2 * Fm * S, 512, TM, CBK, sw64);
   for (int i = 0; i < 5; i++) {
     const int rows = (e->gru[i].H / HT) * GRU_BN;
-    bad |= make_map(&t->m_w[i], t->w_gru[i], false, 2 * rows, e->gru[i].M, GRU_BN);
-    bad |= make_map(&t->m_u[i], t->u_gru[i], false, 2 * rows, e->gru[i].H, GRU_BN);
+    bad |= make_map(&t->m_h_ch[i], t->h_all[i], false, 2 * (Fm + 1) * S, e->gru[i].H, TM, CBK, sw64);
+    bad |= make_map(&t->m_w[i], t->w_gru[i], false, 2 * rows, e->gru[i].M, GRU_BN, CBK, sw64);
+    bad |= make_map(&t->m_u[i], t->u_gru[i], false, 2 * rows, e->gru[i].H, GRU_BN, CBK, sw64);
   }
   if (bad) return tc_fail(PNB_ERR_CUDA, "cuTensorMapEncodeTiled failed");
   TCK(cudaFuncSetAttribute(gru_chain_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                           (int)tc_smem_bytes<GRU_STAGES, GRU_STAGES * StageLayout<GRU_BN>::kBytes>()));
+                           (int)tc_smem_bytes<GRU_STAGES, GRU_STAGES * GruStage::kBytes>()));
   TCK(cudaFuncSetAttribute(tc_gemm_kernel<DENSE_BN, true, DENSE_STAGES, DENSE_STAGES3>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                            (int)dense_smem_bytes<DENSE_BN, DENSE_STAGES, DENSE_STAGES3>()));
   TCK(cudaFuncSetAttribute(tc_gemm_kernel<SMALL_BN, false, SMALL_STAGES, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -1241,15 +1285,15 @@ int tc_gru_chain(pnb_engine *e, int h0, int n, cudaStream_t st) {
   const int S = e->S, Fm = e->Fmax;
   ChainArgs a;
   memset(&a, 0, sizeof a);
-  a.maps[0] = t->m_c2;
-  for (int i = 0; i < 5; i++) { a.maps[1 + i] = t->m_h[i]; a.maps[6 + i] = t->m_w[i]; a.maps[11 + i] = t->m_u[i]; }
+  a.maps[0] = t->m_c2_ch;
+  for (int i = 0; i < 5; i++) { a.maps[1 + i] = t->m_h_ch[i]; a.maps[6 + i] = t->m_w[i]; a.maps[11 + i] = t->m_u[i]; }
   a.S = S; a.F = n; a.t0 = h0; a.tiles_mp = t->tiles_mp; a.cnt = t->cnt; a.tansig = e->tansig();
   const int c2_terms = Fm * S, h_terms = (Fm + 1) * S;
   int unit0 = 0;
   for (int li = 0; li < 5; li++) {
     ChainLayer &L = a.L[li];
     const int H = e->gru[li].H, tiles = H / HT;
-    L.H = H; L.h_kb = H / BK; L.tiles_log2 = __builtin_ctz(tiles);
+    L.H = H; L.h_kb = H / CBK; L.tiles_log2 = __builtin_ctz(tiles);
     L.b_term_rows = tiles * GRU_BN;
     L.h_map = 1 + li; L.w_map = 6 + li; L.u_map = 11 + li;
     L.unit0 = unit0; unit0 += t->tiles_mp * tiles;
@@ -1260,13 +1304,13 @@ int tc_gru_chain(pnb_engine *e, int h0, int n, cudaStream_t st) {
     L.h_hl = t->h_all[li]; L.h_term_rows = h_terms;
     // each GRU consumes the freshly written state (slot t+1) of the layer below (rnn.cpp:58-71, SURVEY.md App. C.10)
     if (li == 0) {          // gru1 <- conv2 out
-      L.n_x = 1; L.x_map[0] = 0; L.x_kb[0] = 512 / BK; L.x_bk0[0] = 0; L.x_row1[0] = 0; L.x_term_rows[0] = c2_terms; L.dep = -1;
+      L.n_x = 1; L.x_map[0] = 0; L.x_kb[0] = 512 / CBK; L.x_bk0[0] = 0; L.x_row1[0] = 0; L.x_term_rows[0] = c2_terms; L.dep = -1;
     } else if (li < 4) {    // gru2 <- gru1, gru3 <- gru2, gru_gb <- gru3
-      L.n_x = 1; L.x_map[0] = li; L.x_kb[0] = 512 / BK; L.x_bk0[0] = 0; L.x_row1[0] = 1; L.x_term_rows[0] = h_terms; L.dep = li - 1;
+      L.n_x = 1; L.x_map[0] = li; L.x_kb[0] = 512 / CBK; L.x_bk0[0] = 0; L.x_row1[0] = 1; L.x_term_rows[0] = h_terms; L.dep = li - 1;
     } else {                // gru_rb <- [gru3 state, conv2 out]
       L.n_x = 2;
-      L.x_map[0] = 3; L.x_kb[0] = 512 / BK; L.x_bk0[0] = 0; L.x_row1[0] = 1; L.x_term_rows[0] = h_terms;
-      L.x_map[1] = 0; L.x_kb[1] = 512 / BK; L.x_bk0[1] = 512; L.x_row1[1] = 0; L.x_term_rows[1] = c2_terms;
+      L.x_map[0] = 3; L.x_kb[0] = 512 / CBK; L.x_bk0[0] = 0; L.x_row1[0] = 1; L.x_term_rows[0] = h_terms;
+      L.x_map[1] = 0; L.x_kb[1] = 512 / CBK; L.x_bk0[1] = 512; L.x_row1[1] = 0; L.x_term_rows[1] = c2_terms;
       L.dep = 2;
     }
   }
@@ -1276,7 +1320,7 @@ int tc_gru_chain(pnb_engine *e, int h0, int n, cudaStream_t st) {
   a.diag = (t->tiles_mp * (512 / HT) < e->tc_sms) ? 1 : 0;
   {
     ProfScope ps(e, PNB_K_TC_GEMM, st);
-    int rc = tc_launch(e, gru_chain_kernel, a, n * unit0, tc_smem_bytes<GRU_STAGES, GRU_STAGES * StageLayout<GRU_BN>::kBytes>(), st);
+    int rc = tc_launch(e, gru_chain_kernel, a, n * unit0, tc_smem_bytes<GRU_STAGES, GRU_STAGES * GruStage::kBytes>(), st);
     if (rc) return rc;
   }
   return 1;

@@ -111,7 +111,9 @@ int pnb_submit_host_f32(pnb_engine *e, const float *in, size_t in_stride, float 
 int pnb_submit_host_i16(pnb_engine *e, const short *in, size_t in_stride, short *out, size_t out_stride, int n_frames);
 int pnb_wait(pnb_engine *e);
 /* Waits for everything enqueued on the engine's internal streams and on `cuda_stream` (the stream the caller passed to
- * pnb_process_device_*), then reports the engine's status: PNB_OK, PNB_ERR_DOMAIN, or PNB_ERR_CUDA. */
+ * pnb_process_device_*), then reports the engine's status: PNB_OK, PNB_ERR_DOMAIN, or PNB_ERR_CUDA -- or, once,
+ * PNB_ERR_ARG when pnb_import_states rejected a blob since the last report.  pnb_wait also waits for the last
+ * pnb_reset_streams / pnb_export_states / pnb_import_states, whichever stream it was issued on. */
 int pnb_check(pnb_engine *e, void *cuda_stream);
 
 /* Device buffers on the engine's device; asynchronous on cuda_stream (a cudaStream_t, NULL = default
@@ -159,6 +161,32 @@ int pnb_train_records_device(pnb_engine *e, const short *d_speech, size_t speech
 size_t pnb_state_size(void);
 int pnb_get_state(pnb_engine *e, int stream, void *dst, size_t dst_bytes);
 int pnb_set_state(pnb_engine *e, int stream, const void *src, size_t src_bytes);
+
+/* Batched stream recycling inside a running engine: a session that ends frees its slot for the next one, a session that
+ * moves to another engine / GPU takes its state along -- without idling the device.  All three are asynchronous on
+ * cuda_stream (a cudaStream_t, NULL = default stream) and never synchronise the host.
+ *   streams      host array of n distinct slots in [0, n_streams); it may be reused as soon as the call returns
+ *   d_blobs      device memory on the engine's device: blob i at d_blobs + i*blob_stride, blob_stride >= pnb_state_size()
+ *                (pointer and stride multiples of 4 bytes); the bytes are those of pnb_get_state / pnb_set_state, so a
+ *                blob may be copied to the host and set with pnb_set_state on any engine, and the reverse
+ * Order: an operation runs after everything already enqueued on cuda_stream and after every call issued earlier on the
+ * engine (plain or submitted, on any stream); every call issued later runs after it.
+ *
+ * pnb_reset_streams: the listed streams get the state of a stream in a freshly created engine (history, overlap-add and
+ *   pitch memory, the live spectrum slots, conv histories and GRU states -- what pnb_reset clears, restricted to them).
+ *   The other streams and the engine's status are not touched.  n = 0 is a no-op.
+ * pnb_export_states: writes the blob of every listed stream (PNB_TRAIN_DATA engines: the signal part, the rest zero).
+ * pnb_import_states: the batched pnb_set_state (any batch size, max_frames or network mode of the exporting engine).
+ *   A tensor-mode engine given an fp32-mode blob splits its conv histories and GRU states on the device exactly as
+ *   pnb_set_state does.  A blob with a wrong magic / version, or (tensor mode) a GRU value outside [-1.0001, 1.0001],
+ *   is not loaded: its stream is left reset and the next synchronising entry point (pnb_wait, pnb_check,
+ *   pnb_process_host_*) returns PNB_ERR_ARG once, naming the lowest rejected slot in pnb_last_error(); unlike
+ *   PNB_ERR_DOMAIN this does not stick.
+ * Refused with PNB_ERR_ARG before anything is enqueued: NULL pointers (for n > 0), a slot out of range or listed twice,
+ * a short or misaligned blob_stride, and an engine poisoned by a failed call. */
+int pnb_reset_streams(pnb_engine *e, const int *streams, int n, void *cuda_stream);
+int pnb_export_states(pnb_engine *e, const int *streams, int n, void *d_blobs, size_t blob_stride, void *cuda_stream);
+int pnb_import_states(pnb_engine *e, const int *streams, int n, const void *d_blobs, size_t blob_stride, void *cuda_stream);
 
 /* The pitch analysis alone (BASELINE.json config 5; needs no engine): for each of n_units pitch buffers of 1728
  * float samples (unit u at d_pitch_buf + u*stride; the reference's st->pitch_buf, src/denoise.cpp:80,405-411) runs

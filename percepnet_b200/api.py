@@ -66,6 +66,9 @@ def load_library() -> C.CDLL:
     L.pnb_state_size.restype = sz
     L.pnb_get_state.argtypes = [vp, i, vp, sz]
     L.pnb_set_state.argtypes = [vp, i, vp, sz]
+    L.pnb_reset_streams.argtypes = [vp, vp, i, vp]
+    L.pnb_export_states.argtypes = [vp, vp, i, vp, sz, vp]
+    L.pnb_import_states.argtypes = [vp, vp, i, vp, sz, vp]
     L.pnb_pitch_only_device.argtypes = [vp, sz, C.c_longlong, vp, vp, vp, vp, vp, vp, vp]
     L.pnb_pitch_only_host.argtypes = [vp, sz, C.c_longlong, vp, vp, vp, vp, vp, vp]
     L.pnb_launch_count.argtypes = [vp]
@@ -88,7 +91,8 @@ def load_library() -> C.CDLL:
 
 EXPORTS = ("pnb_create", "pnb_destroy", "pnb_reset", "pnb_process_host_f32", "pnb_process_host_i16",
            "pnb_model_load_blob", "pnb_model_load_stream", "pnb_model_free", "pnb_train_records_host", "pnb_train_records_device", "pnb_submit_train_records", "pnb_process_device_f32", "pnb_process_device_i16", "pnb_submit_host_f32", "pnb_submit_host_i16", "pnb_submit_device_f32", "pnb_submit_device_i16", "pnb_flush", "pnb_wait", "pnb_check",
-           "pnb_read_tap", "pnb_state_size", "pnb_get_state", "pnb_set_state", "pnb_pitch_only_device", "pnb_pitch_only_host", "pnb_launch_count",
+           "pnb_read_tap", "pnb_state_size", "pnb_get_state", "pnb_set_state",
+           "pnb_reset_streams", "pnb_export_states", "pnb_import_states", "pnb_pitch_only_device", "pnb_pitch_only_host", "pnb_launch_count",
            "pnb_launches_per_call", "pnb_profile_enable", "pnb_profile_read", "pnb_profile_timeline", "pnb_kernel_class_name", "pnb_n_streams", "pnb_overlap_info", "pnb_set_overlap", "pnb_max_frames", "pnb_last_error", "pnb_version")
 
 
@@ -238,6 +242,46 @@ class Engine:
 
     def set_state(self, stream: int, blob: bytes):
         self._ck(self.L.pnb_set_state(self.h, stream, blob, len(blob)), "pnb_set_state")
+
+    # ---- batched stream recycling (asynchronous on `stream`; see pnb_reset_streams in the header) ----------------
+    @staticmethod
+    def _slots(idx):
+        a = np.ascontiguousarray(np.asarray(idx, dtype=np.int64).reshape(-1).astype(np.int32))
+        return a, len(a)
+
+    @property
+    def state_size(self) -> int:
+        return int(self.L.pnb_state_size())
+
+    def reset_streams(self, idx, stream: int = 0):
+        """pnb_reset_streams: the slots in `idx` start over as fresh streams; the others are untouched."""
+        a, n = self._slots(idx)
+        self._ck(self.L.pnb_reset_streams(self.h, a.ctypes.data if n else None, n, stream or None), "pnb_reset_streams")
+
+    def export_states(self, idx, d_blobs, stride: int = 0, stream: int = 0):
+        """pnb_export_states.  d_blobs: a raw device pointer (blob i at d_blobs + i*stride, stride 0 = pnb_state_size()),
+        or None to get a new CUDA uint8 torch tensor [len(idx), pnb_state_size()] back."""
+        a, n = self._slots(idx)
+        out = None
+        if d_blobs is None:
+            import torch
+            out = torch.empty((n, self.state_size), dtype=torch.uint8, device=f"cuda:{self.device}")
+            d_blobs, stride = out.data_ptr(), self.state_size
+        self._ck(self.L.pnb_export_states(self.h, a.ctypes.data if n else None, n, d_blobs or None, stride or self.state_size,
+                                          stream or None), "pnb_export_states")
+        return out
+
+    def import_states(self, idx, d_blobs, stride: int = 0, stream: int = 0):
+        """pnb_import_states.  d_blobs: a raw device pointer (as export_states) or a CUDA uint8 tensor
+        [len(idx), >= pnb_state_size()] whose rows are blobs; the tensor must stay alive until `stream` has run the import."""
+        a, n = self._slots(idx)
+        if not isinstance(d_blobs, int) and d_blobs is not None:
+            t = d_blobs
+            if t.dtype.itemsize != 1 or t.dim() != 2 or t.shape[0] != n or t.stride(1) != 1 or not t.is_cuda:
+                raise PnbError("import_states: blobs must be a CUDA byte tensor [len(idx), pnb_state_size()] with contiguous rows")
+            d_blobs, stride = t.data_ptr(), t.stride(0)
+        self._ck(self.L.pnb_import_states(self.h, a.ctypes.data if n else None, n, d_blobs or None, stride or self.state_size,
+                                          stream or None), "pnb_import_states")
 
     def read_nn_state(self) -> dict:
         """fp32 network state after the last hop: conv2 output and the five GRU states, [S, width]."""

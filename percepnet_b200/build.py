@@ -24,6 +24,7 @@ SOURCES = {
     "pnb_nn_f32.cu": [],
     "pnb_nn_tc.cu": [],
     "pnb_engine.cu": [],
+    "pnb_state.cu": [],
 }
 
 

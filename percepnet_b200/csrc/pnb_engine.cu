@@ -13,6 +13,7 @@
 #include <string.h>
 
 #include <stddef.h>
+#include <stdint.h>
 #include <string>
 #include <vector>
 
@@ -312,9 +313,21 @@ extern "C" int pnb_create(pnb_engine **out, int n_streams, int max_frames, const
   e->pcm_stride = kKeep + line_calls * F * kFrame;
   CKD(dalloc(&e->d_pcm, S * e->pcm_stride));
   CKD(dalloc(&e->d_synth, S * kFrame));
-  CKD(dalloc(&e->d_status, 1));
-  CKD(cudaHostAlloc((void **)&e->h_status, sizeof(int), cudaHostAllocDefault));
-  *e->h_status = 0;
+  CKD(dalloc(&e->d_status, 2));
+  CKD(cudaMemset(e->d_status + 1, 0x7F, sizeof(int)));  // kNoRejectedSlot
+  CKD(cudaHostAlloc((void **)&e->h_status, 2 * sizeof(int), cudaHostAllocDefault));
+  e->h_status[0] = 0;
+  e->h_status[1] = kNoRejectedSlot;
+  // batched stream-state operations: staging of the slot indices, import verdicts, one blob of scratch
+  CKD(cudaEventCreateWithFlags(&e->ev_call, cudaEventDisableTiming));
+  CKD(cudaEventCreateWithFlags(&e->ev_state, cudaEventDisableTiming));
+  for (int k = 0; k < 2; k++) {
+    CKD(cudaEventCreateWithFlags(&e->ev_idx[k], cudaEventDisableTiming));
+    CKD(cudaHostAlloc((void **)&e->h_idx[k], S * sizeof(int), cudaHostAllocDefault));
+    CKD(dalloc(&e->d_idx[k], S, false));
+  }
+  CKD(dalloc(&e->d_ok, S, false));
+  CKD(cudaMalloc(&e->d_blob1, sizeof(StreamState)));
   CKD(dalloc(&e->d_last_period, S));
   CKD(dalloc(&e->d_last_gain, S));
   // per-call buffers
@@ -399,6 +412,15 @@ extern "C" void pnb_destroy(pnb_engine *e) {
   if (e->d_last_period) cudaFree(e->d_last_period);
   if (e->d_status) cudaFree(e->d_status);
   if (e->h_status) cudaFreeHost(e->h_status);
+  for (int k = 0; k < 2; k++) {
+    if (e->h_idx[k]) cudaFreeHost(e->h_idx[k]);
+    if (e->d_idx[k]) cudaFree(e->d_idx[k]);
+    if (e->ev_idx[k]) cudaEventDestroy(e->ev_idx[k]);
+  }
+  if (e->d_ok) cudaFree(e->d_ok);
+  if (e->d_blob1) cudaFree(e->d_blob1);
+  if (e->ev_call) cudaEventDestroy(e->ev_call);
+  if (e->ev_state) cudaEventDestroy(e->ev_state);
   if (e->d_tap_pitch) cudaFree(e->d_tap_pitch);
   if (e->d_tab) cudaFree(e->d_tab);
   if (e->d_hin16) cudaFree(e->d_hin16);
@@ -445,7 +467,9 @@ extern "C" int pnb_reset(pnb_engine *e) {
   CK(cudaMemset(e->d_last_period, 0, S * sizeof(int)));
   CK(cudaMemset(e->d_last_gain, 0, S * sizeof(float)));
   CK(cudaMemset(e->d_status, 0, sizeof(int)));
-  *e->h_status = 0;
+  CK(cudaMemset(e->d_status + 1, 0x7F, sizeof(int)));  // kNoRejectedSlot
+  e->h_status[0] = 0;
+  e->h_status[1] = kNoRejectedSlot;
   e->hop = 0;
   e->poisoned = false;
   e->unjoined = false;      // the device was synchronised above (green-context streams included)
@@ -681,6 +705,16 @@ struct CallLink {
   cudaEvent_t ready = nullptr, done = nullptr;
 };
 
+// End of a call: unless its work is still in flight on the engine's streams (a submitted chunked call, which
+// join_engine_streams covers), it ended in `st`; a later state operation waits for that point.
+static int mark_call_end(pnb_engine *e, cudaStream_t st) {
+  e->state_pending = false;
+  if (e->unjoined) return PNB_OK;
+  CK(cudaEventRecord(e->ev_call, st));
+  e->call_recorded = true;
+  return PNB_OK;
+}
+
 // The caller's stream (or the host, st == nullptr ... not used) catches up with work left in flight by submitted calls.
 static int join_engine_streams(pnb_engine *e, cudaStream_t st) {
   if (!e->unjoined) return PNB_OK;
@@ -740,6 +774,11 @@ static int process_device_enqueue(pnb_engine *e, const float *d_in, const short 
       CK(cudaStreamWaitEvent(sn, e->ev_fork, 0));
       CK(cudaStreamWaitEvent(ss, e->ev_fork, 0));
     }
+    if (e->state_pending) {  // a state operation issued since the last call, possibly on another stream
+      CK(cudaStreamWaitEvent(sd, e->ev_state, 0));
+      CK(cudaStreamWaitEvent(sn, e->ev_state, 0));
+      CK(cudaStreamWaitEvent(ss, e->ev_state, 0));
+    }
     if (lk.ready) CK(cudaStreamWaitEvent(sd, lk.ready, 0));
     const int cur = e->syn_par ^ 1, prv = e->syn_par;
     const int pC = (int)e->prev_start.size();
@@ -797,6 +836,7 @@ static int process_device_enqueue(pnb_engine *e, const float *d_in, const short 
   } else {
     // ---- serial schedule on the caller's stream
     if (lk.ready) CK(cudaStreamWaitEvent(st, lk.ready, 0));
+    if (e->state_pending) CK(cudaStreamWaitEvent(st, e->ev_state, 0));
     { int rc = join_engine_streams(e, st); if (rc) return rc; }
     e->prev_start.clear();
     { ProfScope ps(e, PNB_K_STAGE_IN, st); n += launch_stage_in(line, e->pcm_stride, d_in, d_in16, in_stride, S, F * kFrame, st); }
@@ -825,6 +865,7 @@ static int process_device_enqueue(pnb_engine *e, const float *d_in, const short 
     if (lk.submitted && lk.done) CK(cudaEventRecord(lk.done, st));
   }
   if (d_gr) CK(cudaMemcpyAsync(d_gr, e->d_gr, (size_t)F * S * 68 * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  { int rc = mark_call_end(e, st); if (rc) return rc; }
   CK(cudaGetLastError());
   *n_out = n;
   return PNB_OK;
@@ -883,6 +924,7 @@ extern "C" int pnb_train_records_device(pnb_engine *e, const short *d_speech, si
   const int S = e->S, N = S / 2;
   long long n = 0;
   float *line = e->d_pcm + e->line_off;
+  if (e->state_pending) CK(cudaStreamWaitEvent(st, e->ev_state, 0));
   {
     ProfScope ps(e, PNB_K_STAGE_IN, st);
     n += launch_stage_in(line, e->pcm_stride, nullptr, d_noisy, noisy_stride, N, F * kFrame, st, 1.f);
@@ -900,6 +942,7 @@ extern "C" int pnb_train_records_device(pnb_engine *e, const short *d_speech, si
   l.records = d_records; l.pair_stride = records_stride;
   { ProfScope ps(e, PNB_K_LABELS, st); n += launch_train_labels(l, st); }
   n += advance_line(e, F, st);
+  { int rc = mark_call_end(e, st); if (rc) return rc; }
   CK(cudaGetLastError());
   e->hop += F;
   e->last_frames = F;
@@ -934,7 +977,17 @@ extern "C" int pnb_train_records_host(pnb_engine *e, const short *speech, size_t
 
 // after the stream that carried the status copy was synchronised
 static int report_status(pnb_engine *e) {
-  if (*e->h_status & 1)
+  if (e->h_status[0] & kStatusRejected) {  // reported once: no other stream was affected
+    const int slot = e->h_status[1];
+    launch_state_clear_reject(e->d_status, e->stream);
+    CK(cudaGetLastError());
+    CK(cudaStreamSynchronize(e->stream));
+    e->h_status[0] &= ~kStatusRejected;
+    e->h_status[1] = kNoRejectedSlot;
+    return fail(PNB_ERR_ARG, "pnb_import_states rejected a blob (bad magic / version, or a GRU state outside [-1, 1] for a "
+                             "tensor-mode engine); lowest rejected stream %d, left reset like every rejected one", slot);
+  }
+  if (e->h_status[0] & 1)
     return fail(PNB_ERR_DOMAIN, "tensor path: a pre-activation left the domain of the reference's tansig_approx (|x| >= 8.5e7, "
                                 "src/vec.h:63 is undefined there); results since the last pnb_reset are not the reference's -- "
                                 "use PNB_NN_FP32 for such input");
@@ -964,7 +1017,7 @@ static int process_host(pnb_engine *e, const T *in, size_t in_stride, T *out, si
   if (rc) return rc;
   CK(cudaMemcpy2DAsync(out, out_stride * sizeof(T), *d_out_p, row * sizeof(T), w, S, cudaMemcpyDeviceToHost, e->stream));
   if (gr) CK(cudaMemcpyAsync(gr, e->d_gr, (size_t)F * S * 68 * sizeof(float), cudaMemcpyDeviceToHost, e->stream));
-  CK(cudaMemcpyAsync(e->h_status, e->d_status, sizeof(int), cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaMemcpyAsync(e->h_status, e->d_status, 2 * sizeof(int), cudaMemcpyDeviceToHost, e->stream));
   CK(cudaStreamSynchronize(e->stream));
   return report_status(e);
 }
@@ -1110,7 +1163,8 @@ extern "C" int pnb_wait(pnb_engine *e) {
   CK(cudaSetDevice(e->device));
   if (e->s_in) CK(cudaStreamSynchronize(e->s_in));
   { int rc = drain_engine_streams(e); if (rc) return rc; }
-  CK(cudaMemcpyAsync(e->h_status, e->d_status, sizeof(int), cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaEventSynchronize(e->ev_state));  // the last state operation, whichever stream it was issued on
+  CK(cudaMemcpyAsync(e->h_status, e->d_status, 2 * sizeof(int), cudaMemcpyDeviceToHost, e->stream));
   CK(cudaStreamSynchronize(e->stream));
   if (e->s_out) CK(cudaStreamSynchronize(e->s_out));
   return report_status(e);
@@ -1169,28 +1223,74 @@ extern "C" int pnb_read_tap(pnb_engine *e, int what, void *dst, size_t dst_bytes
 // per-stream state export / import (the reference's DenoiseState + RNNState, src/denoise.cpp:71-85, nnet_data.h:28-38,
 // reduced to what is live: SURVEY.md App. A.2) -- for moving a stream between engines / GPUs at a call boundary
 // ------------------------------------------------------------------------------------------
-namespace {
-struct StreamState {
-  unsigned magic, version;
-  float pcm[kKeep];          // the last 5280 input samples (comb_buf without its newest hop)
-  float synth[kFrame];       // overlap-add memory
-  int last_period;
-  float last_gain;
-  float spec[5][2 * kBins];  // spectra of the last five windowed blocks (analysis spectrum of the next five hops), oldest first
-  float eband[5][kBands];    // their band energies
-  float fc_hist[4][128];     // conv1 input history (last four fc outputs), oldest first
-  float c1_hist[2][512];     // conv2 input history (last two conv1 outputs)
-  float h[4 * 512 + 128];    // gru1, gru2, gru3, gru_gb, gru_rb
-  // tensor-mode engines keep the conv histories as three bf16 terms; the sum above does not always split back into the
-  // same terms (a low term of exactly half an ulp), so the raw terms travel too and a tensor-mode engine restores those
-  unsigned has_terms;
-  unsigned short fc_terms[3][4][128];
-  unsigned short c1_terms[3][2][512];
-};
-constexpr unsigned kStateMagic = 0x53424E50u;  // "PNBS"
-}  // namespace
-
 extern "C" size_t pnb_state_size(void) { return sizeof(StreamState); }
+
+// Enqueues one batched state operation on st (arguments already checked): after every call and state operation issued
+// earlier on the engine, before every one issued later (ev_call / ev_state, see pnb_engine.h).
+static int state_enqueue(pnb_engine *e, int mode, const int *streams, int n, void *d_blobs, size_t blob_stride, cudaStream_t st) {
+  StateArgs a;
+  memset(&a, 0, sizeof a);
+  a.n_seg = state_segs(e, a.seg);
+  if (e->call_recorded) CK(cudaStreamWaitEvent(st, e->ev_call, 0));
+  { int rc = join_engine_streams(e, st); if (rc) return rc; }
+  // the slot indices travel through pinned staging: the caller's array is free again when this returns
+  const int k = e->idx_slot;
+  CK(cudaEventSynchronize(e->ev_idx[k]));  // the copy out of this slot two operations ago has run
+  memcpy(e->h_idx[k], streams, (size_t)n * sizeof(int));
+  CK(cudaMemcpyAsync(e->d_idx[k], e->h_idx[k], (size_t)n * sizeof(int), cudaMemcpyHostToDevice, st));
+  CK(cudaEventRecord(e->ev_idx[k], st));
+  e->idx_slot = k ^ 1;
+  a.n = n; a.streams = e->d_idx[k]; a.blobs = static_cast<char *>(d_blobs); a.blob_stride = blob_stride;
+  a.ok = e->d_ok; a.mode = mode; a.status = e->d_status;
+  a.has_terms = (e->flags & PNB_NN_TENSOR) ? 1u : 0u;
+  a.check_gru = (e->flags & PNB_NN_TENSOR) ? 1 : 0;
+  long long nl = 0;
+  if (mode == kStateImport) nl += launch_state_check(a, st);
+  nl += launch_state_move(a, st);
+  CK(cudaGetLastError());
+  CK(cudaEventRecord(e->ev_state, st));
+  CK(cudaEventRecord(e->ev_call, st));
+  e->call_recorded = true;
+  e->state_pending = true;
+  e->launches += nl;
+  return PNB_OK;
+}
+
+static int state_batch(pnb_engine *e, int mode, const int *streams, int n, void *d_blobs, size_t blob_stride, void *cuda_stream) {
+  if (!e) return fail(PNB_ERR_ARG, "engine is NULL");
+  if (n < 0) return fail(PNB_ERR_ARG, "n = %d is negative", n);
+  if (n == 0) return PNB_OK;
+  if (!streams) return fail(PNB_ERR_ARG, "streams is NULL");
+  if (mode != kStateReset) {
+    if (!d_blobs) return fail(PNB_ERR_ARG, "d_blobs is NULL");
+    if (blob_stride < sizeof(StreamState))
+      return fail(PNB_ERR_ARG, "blob_stride %zu below pnb_state_size() = %zu", blob_stride, sizeof(StreamState));
+    if ((reinterpret_cast<uintptr_t>(d_blobs) | blob_stride) & 3) return fail(PNB_ERR_ARG, "d_blobs and blob_stride must be multiples of 4 bytes");
+  }
+  if (e->poisoned) return fail(PNB_ERR_ARG, "an earlier call failed while enqueuing work; the streams' state is undefined until pnb_reset");
+  if (n > e->S) return fail(PNB_ERR_ARG, "n = %d streams, the engine has %d", n, e->S);
+  std::vector<unsigned char> seen(e->S, 0);
+  for (int i = 0; i < n; i++) {
+    const int s = streams[i];
+    if (s < 0 || s >= e->S) return fail(PNB_ERR_ARG, "streams[%d] = %d outside [0, %d)", i, s, e->S);
+    if (seen[s]) return fail(PNB_ERR_ARG, "stream %d listed twice", s);
+    seen[s] = 1;
+  }
+  CK(cudaSetDevice(e->device));
+  const int rc = state_enqueue(e, mode, streams, n, d_blobs, blob_stride, (cudaStream_t)cuda_stream);
+  if (rc) e->poisoned = true;  // part of the operation may have been enqueued
+  return rc;
+}
+
+extern "C" int pnb_reset_streams(pnb_engine *e, const int *streams, int n, void *cuda_stream) {
+  return state_batch(e, kStateReset, streams, n, nullptr, 0, cuda_stream);
+}
+extern "C" int pnb_export_states(pnb_engine *e, const int *streams, int n, void *d_blobs, size_t blob_stride, void *cuda_stream) {
+  return state_batch(e, kStateExport, streams, n, d_blobs, blob_stride, cuda_stream);
+}
+extern "C" int pnb_import_states(pnb_engine *e, const int *streams, int n, const void *d_blobs, size_t blob_stride, void *cuda_stream) {
+  return state_batch(e, kStateImport, streams, n, const_cast<void *>(d_blobs), blob_stride, cuda_stream);
+}
 
 static int state_args(pnb_engine *e, int stream, const void *buf, size_t bytes) {
   if (!e || !buf) return fail(PNB_ERR_ARG, "NULL argument");
@@ -1200,40 +1300,16 @@ static int state_args(pnb_engine *e, int stream, const void *buf, size_t bytes) 
   return PNB_OK;
 }
 
+// The single-stream host forms: the batched kernels through one blob of device scratch, with the engine idle before
+// and after.
 extern "C" int pnb_get_state(pnb_engine *e, int stream, void *dst, size_t bytes) {
   int rc = state_args(e, stream, dst, bytes);
   if (rc) return rc;
   CK(cudaSetDevice(e->device));
   CK(cudaDeviceSynchronize());
-  StreamState *st = static_cast<StreamState *>(dst);
-  memset(st, 0, sizeof *st);
-  st->magic = kStateMagic; st->version = 1;
-  const size_t s = stream, S = e->S;
-  CK(cudaMemcpy(st->pcm, e->d_pcm + s * e->pcm_stride + e->line_off, kKeep * 4, cudaMemcpyDeviceToHost));
-  CK(cudaMemcpy(st->synth, e->d_synth + s * kFrame, kFrame * 4, cudaMemcpyDeviceToHost));
-  CK(cudaMemcpy(&st->last_period, e->d_last_period + s, 4, cudaMemcpyDeviceToHost));
-  CK(cudaMemcpy(&st->last_gain, e->d_last_gain + s, 4, cudaMemcpyDeviceToHost));
-  for (int k = 0; k < 5; k++) {
-    const long c = e->hop - 5 + k;
-    const size_t slot = (size_t)((c % e->ring + e->ring) % e->ring);
-    CK(cudaMemcpy(st->spec[k], e->d_zring + (slot * S + s) * kBins, kBins * 8, cudaMemcpyDeviceToHost));
-    CK(cudaMemcpy(st->eband[k], e->d_ering + (slot * S + s) * kBands, kBands * 4, cudaMemcpyDeviceToHost));
-  }
-  if (e->flags & PNB_TRAIN_DATA) return PNB_OK;
-  size_t off = 0;
-  for (int li = 0; li < 5; li++) {
-    const size_t H = e->gru[li].H;
-    CK(cudaMemcpy(st->h + off, e->h[li][e->par[li]] + s * H, H * 4, cudaMemcpyDeviceToHost));
-    off += H;
-  }
-  if (e->flags & PNB_NN_TENSOR) {
-    st->has_terms = 1;
-    return tc_get_stream_hist(e, stream, &st->fc_hist[0][0], &st->c1_hist[0][0], &st->fc_terms[0][0][0], &st->c1_terms[0][0][0]);
-  }
-  for (int k = 0; k < 4; k++)   // slots 0..3 / 0..1: the histories, oldest first (nn_chunk_f32's carry)
-    CK(cudaMemcpy(st->fc_hist[k], e->ring_fc + ((size_t)k * S + s) * 128, 128 * 4, cudaMemcpyDeviceToHost));
-  for (int k = 0; k < 2; k++)
-    CK(cudaMemcpy(st->c1_hist[k], e->ring_c1 + ((size_t)k * S + s) * 512, 512 * 4, cudaMemcpyDeviceToHost));
+  if ((rc = state_enqueue(e, kStateExport, &stream, 1, e->d_blob1, sizeof(StreamState), e->stream))) return rc;
+  CK(cudaMemcpyAsync(dst, e->d_blob1, sizeof(StreamState), cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaStreamSynchronize(e->stream));
   return PNB_OK;
 }
 
@@ -1241,38 +1317,16 @@ extern "C" int pnb_set_state(pnb_engine *e, int stream, const void *src, size_t 
   int rc = state_args(e, stream, src, bytes);
   if (rc) return rc;
   const StreamState *st = static_cast<const StreamState *>(src);
-  if (st->magic != kStateMagic || st->version != 1) return fail(PNB_ERR_ARG, "not a pnb_get_state blob (magic/version)");
+  if (st->magic != kStateMagic || st->version != kStateVersion) return fail(PNB_ERR_ARG, "not a pnb_get_state blob (magic/version)");
   if (e->flags & PNB_NN_TENSOR)
     for (size_t i = 0; i < sizeof st->h / sizeof(float); i++)
-      if (!(fabsf(st->h[i]) <= 1.0001f))
+      if (!(fabsf(st->h[i]) <= kStateGruBound))
         return fail(PNB_ERR_ARG, "GRU state value %g outside [-1, 1]: not a state the network can reach", (double)st->h[i]);
   CK(cudaSetDevice(e->device));
   CK(cudaDeviceSynchronize());
-  const size_t s = stream, S = e->S;
-  CK(cudaMemcpy(e->d_pcm + s * e->pcm_stride + e->line_off, st->pcm, kKeep * 4, cudaMemcpyHostToDevice));
-  CK(cudaMemcpy(e->d_synth + s * kFrame, st->synth, kFrame * 4, cudaMemcpyHostToDevice));
-  CK(cudaMemcpy(e->d_last_period + s, &st->last_period, 4, cudaMemcpyHostToDevice));
-  CK(cudaMemcpy(e->d_last_gain + s, &st->last_gain, 4, cudaMemcpyHostToDevice));
-  for (int k = 0; k < 5; k++) {
-    const long c = e->hop - 5 + k;
-    const size_t slot = (size_t)((c % e->ring + e->ring) % e->ring);
-    CK(cudaMemcpy(e->d_zring + (slot * S + s) * kBins, st->spec[k], kBins * 8, cudaMemcpyHostToDevice));
-    CK(cudaMemcpy(e->d_ering + (slot * S + s) * kBands, st->eband[k], kBands * 4, cudaMemcpyHostToDevice));
-  }
-  if (e->flags & PNB_TRAIN_DATA) return PNB_OK;
-  size_t off = 0;
-  for (int li = 0; li < 5; li++) {
-    const size_t H = e->gru[li].H;
-    CK(cudaMemcpy(e->h[li][e->par[li]] + s * H, st->h + off, H * 4, cudaMemcpyHostToDevice));
-    off += H;
-  }
-  if (e->flags & PNB_NN_TENSOR)
-    return tc_set_stream_hist(e, stream, &st->fc_hist[0][0], &st->c1_hist[0][0], st->h,
-                              st->has_terms ? &st->fc_terms[0][0][0] : nullptr, st->has_terms ? &st->c1_terms[0][0][0] : nullptr);
-  for (int k = 0; k < 4; k++)
-    CK(cudaMemcpy(e->ring_fc + ((size_t)k * S + s) * 128, st->fc_hist[k], 128 * 4, cudaMemcpyHostToDevice));
-  for (int k = 0; k < 2; k++)
-    CK(cudaMemcpy(e->ring_c1 + ((size_t)k * S + s) * 512, st->c1_hist[k], 512 * 4, cudaMemcpyHostToDevice));
+  CK(cudaMemcpyAsync(e->d_blob1, src, sizeof(StreamState), cudaMemcpyHostToDevice, e->stream));
+  if ((rc = state_enqueue(e, kStateImport, &stream, 1, e->d_blob1, sizeof(StreamState), e->stream))) return rc;
+  CK(cudaStreamSynchronize(e->stream));
   return PNB_OK;
 }
 

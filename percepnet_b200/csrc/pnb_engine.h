@@ -3,6 +3,7 @@
 #include <stddef.h>
 #include <vector>
 #include "pnb_kernels.h"
+#include "pnb_state.h"
 #include "../../include/percepnet_b200.h"
 #include "../../include/pnb_nnet_layout.h"
 
@@ -90,9 +91,23 @@ struct pnb_engine {
   int last_frames = 0;
   long long launches = 0;
   // status word on the device: bit 0 = an activation left the domain in which the reference's tansig_approx is
-  // defined (tensor path only; reported as PNB_ERR_DOMAIN by the synchronising entry points, cleared by pnb_reset)
-  int *d_status = nullptr;
-  int *h_status = nullptr;  // pinned host copy, refreshed by the synchronising entry points
+  // defined (tensor path only; reported as PNB_ERR_DOMAIN by the synchronising entry points, cleared by pnb_reset);
+  // bit 1 = pnb_import_states rejected a blob, [1] = the lowest rejected slot (reported once, then cleared)
+  int *d_status = nullptr;  // [2]
+  int *h_status = nullptr;  // [2] pinned host copy, refreshed by the synchronising entry points
+
+  // Batched stream-state operations (pnb_reset_streams / pnb_export_states / pnb_import_states).  Every call and state
+  // operation that ends in its caller's stream records ev_call there; a state operation waits for it (and joins the
+  // engine's own streams), and the next call waits for ev_state, whichever stream either was issued on.
+  cudaEvent_t ev_call = nullptr, ev_state = nullptr;
+  bool call_recorded = false;    // ev_call has been recorded at least once
+  bool state_pending = false;    // a state operation was issued after the last call
+  int *h_idx[2] = {nullptr, nullptr};  // [S] pinned staging of the slot indices, double-buffered ...
+  int *d_idx[2] = {nullptr, nullptr};  // [S] ... and their device copies
+  cudaEvent_t ev_idx[2] = {nullptr, nullptr};  // the copy out of h_idx[k] has run
+  int idx_slot = 0;
+  int *d_ok = nullptr;           // [S] import: per-blob verdict of the device-side check
+  void *d_blob1 = nullptr;       // one blob of device scratch: pnb_get_state / pnb_set_state
   // a call failed after it had started to enqueue work: the streams' state is undefined until pnb_reset
   bool poisoned = false;
 
@@ -120,10 +135,8 @@ int tc_gru_chain(pnb_engine *e, int h0, int n, cudaStream_t st);
 int tc_out(pnb_engine *e, int h0, int n, cudaStream_t st);
 int tc_carry(pnb_engine *e, int F, cudaStream_t st);       // once per call, after its last tc_out
 int tc_launches_per_chunk(const pnb_engine *e);
-// pnb_get_state / pnb_set_state: conv histories as fp32 sums and as the raw bf16 term pairs [2 terms][slots][width]
-int tc_get_stream_hist(pnb_engine *e, int s, float *fc_hist, float *c1_hist, unsigned short *fc_terms, unsigned short *c1_terms);
-int tc_set_stream_hist(pnb_engine *e, int s, const float *fc_hist, const float *c1_hist, const float *h,
-                       const unsigned short *fc_terms, const unsigned short *c1_terms);
+// The tensor path's pieces of a stream's state (pnb_state.cu): appended to seg[ns..]; returns the new count
+int tc_state_segs(const pnb_engine *e, pnb::StateSeg *seg, int ns);
 
 // RAII marker used by the launch schedule: records an event pair around a launch when profiling
 struct ProfScope {

@@ -1136,70 +1136,42 @@ int tc_reset(pnb_engine *e) {
   return PNB_OK;
 }
 
-// One stream's conv input history (the last 4 fc outputs, the last 2 conv1 outputs; oldest first) as fp32, for
-// pnb_get_state / pnb_set_state.  Between calls the history sits in hop slots 0..3 / 0..1 as two bf16 terms.
-int tc_get_stream_hist(pnb_engine *e, int s, float *fc_hist, float *c1_hist, unsigned short *fc_terms, unsigned short *c1_terms) {
-  pnb_tc_state *t = e->tc;
+// The tensor path's part of a stream's state: the conv input histories (the last 4 fc / 2 conv1 outputs, oldest first)
+// as the three bf16 term planes of hop slots 0..3 / 0..1, and the fp16 hi / lo terms of the GRU states at slot 0.
+// Export writes the terms and their fp32 sums; import restores the raw terms, or splits blobs without them (fp32-mode
+// engines) with the roundings of store_split_b2 / store_split_h2.
+int tc_state_segs(const pnb_engine *e, StateSeg *seg, int ns) {
+  static_assert(kConvTerms == 3, "StreamState carries three bf16 terms per conv history value");
+  const pnb_tc_state *t = e->tc;
   const size_t S = e->S, Fm = e->Fmax;
-  static_assert(sizeof(__nv_bfloat16) == sizeof(unsigned short), "raw bf16 terms travel as 16-bit words");
-  auto get = [&](const __nv_bfloat16 *base, size_t plane, int slots, int width, float *sum, unsigned short *terms) -> cudaError_t {
+  auto hist = [&](const __nv_bfloat16 *base, size_t plane, int slots, int width, size_t sum_off, size_t terms_off) {
     for (int i = 0; i < slots; i++) {
-      for (int k = 0; k < width; k++) sum[i * width + k] = 0.f;
-      for (int tm = kConvTerms - 1; tm >= 0; tm--) {  // smallest term first: the fp32 sum is then exact up to its last bit
-        __nv_bfloat16 *dst = reinterpret_cast<__nv_bfloat16 *>(terms + ((size_t)tm * slots + i) * width);
-        cudaError_t r = cudaMemcpy(dst, base + (size_t)tm * plane + ((size_t)i * S + s) * width, (size_t)width * 2, cudaMemcpyDeviceToHost);
-        if (r != cudaSuccess) return r;
-        for (int k = 0; k < width; k++) sum[i * width + k] += __bfloat162float(dst[k]);
+      StateSeg g = StateSeg();
+      g.kind = kSegSumBf16; g.eng = (char *)(base + (size_t)i * S * width); g.eng_stride = (size_t)width * 2;
+      g.plane = plane * 2; g.blob_off = (unsigned)(sum_off + (size_t)i * width * 4); g.n = width;
+      seg[ns++] = g;
+      for (int tm = 0; tm < kConvTerms; tm++) {
+        g.kind = kSegTermBf16; g.eng = (char *)(base + (size_t)tm * plane + (size_t)i * S * width); g.plane = 0;
+        g.blob_off = (unsigned)(terms_off + ((size_t)tm * slots + i) * width * 2);
+        g.aux_off = (unsigned)(sum_off + (size_t)i * width * 4); g.term = (short)tm;
+        seg[ns++] = g;
       }
     }
-    return cudaSuccess;
   };
-  TCK(get(t->fc_all, (Fm + 4) * S * 128, 4, 128, fc_hist, fc_terms));
-  TCK(get(t->c1_all, (Fm + 2) * S * 512, 2, 512, c1_hist, c1_terms));
-  return PNB_OK;
-}
-// h: the five GRU states of the stream, concatenated (4 x 512 + 128), already stored as fp32 by the caller.
-// fc_terms / c1_terms (from a tensor-mode engine) are restored verbatim; without them the fp32 values are split.
-int tc_set_stream_hist(pnb_engine *e, int s, const float *fc_hist, const float *c1_hist, const float *h,
-                       const unsigned short *fc_terms, const unsigned short *c1_terms) {
-  pnb_tc_state *t = e->tc;
-  const size_t S = e->S, Fm = e->Fmax;
-  auto put = [&](__nv_bfloat16 *base, size_t plane, int slots, int width, const float *sum, const unsigned short *terms) -> cudaError_t {
-    std::vector<__nv_bfloat16> buf(width);
-    for (int i = 0; i < slots; i++)
-      for (int tm = 0; tm < kConvTerms; tm++) {
-        for (int k = 0; k < width; k++) {
-          if (terms) {
-            buf[k] = reinterpret_cast<const __nv_bfloat16 *>(terms + ((size_t)tm * slots + i) * width)[k];
-          } else {
-            float r = sum[i * width + k];
-            __nv_bfloat16 b = __float2bfloat16_rn(r);
-            for (int q = 0; q < tm; q++) { r -= __bfloat162float(b); b = __float2bfloat16_rn(r); }
-            buf[k] = b;
-          }
-        }
-        cudaError_t r = cudaMemcpy(base + (size_t)tm * plane + ((size_t)i * S + s) * width, buf.data(), (size_t)width * 2, cudaMemcpyHostToDevice);
-        if (r != cudaSuccess) return r;
-      }
-    return cudaSuccess;
-  };
-  TCK(put(t->fc_all, (Fm + 4) * S * 128, 4, 128, fc_hist, fc_terms));
-  TCK(put(t->c1_all, (Fm + 2) * S * 512, 2, 512, c1_hist, c1_terms));
+  hist(t->fc_all, (Fm + 4) * S * 128, 4, 128, offsetof(StreamState, fc_hist), offsetof(StreamState, fc_terms));
+  hist(t->c1_all, (Fm + 2) * S * 512, 2, 512, offsetof(StreamState, c1_hist), offsetof(StreamState, c1_terms));
   size_t off = 0;
   for (int li = 0; li < 5; li++) {
     const size_t H = e->gru[li].H;
-    std::vector<__half> hi(H), lo(H);
-    for (size_t k = 0; k < H; k++) {
-      const float sv = h[off + k] * kActScale;
-      hi[k] = __float2half_rn(sv);
-      lo[k] = __float2half_rn(sv - __half2float(hi[k]));
+    for (int tm = 0; tm < 2; tm++) {
+      StateSeg g = StateSeg();
+      g.kind = kSegSplitF16; g.eng = (char *)(t->h_all[li] + (size_t)tm * (Fm + 1) * S * H); g.eng_stride = H * 2;
+      g.blob_off = (unsigned)(offsetof(StreamState, h) + off * 4); g.n = (unsigned)H; g.scale = kActScale; g.term = (short)tm;
+      seg[ns++] = g;
     }
-    __half *p0 = t->h_all[li] + (size_t)s * H;  // slot 0
-    TCK(cudaMemcpy(p0, hi.data(), H * 2, cudaMemcpyHostToDevice));
-    TCK(cudaMemcpy(p0 + (Fm + 1) * S * H, lo.data(), H * 2, cudaMemcpyHostToDevice));
     off += H;
   }
-  return PNB_OK;
+  return ns;
 }
 
 int tc_launches_per_chunk(const pnb_engine *) { return 6; }  // fc, conv1, conv2, GRU chain, fc_gb, fc_rb (+ 1 carry per call)

@@ -1,0 +1,93 @@
+// pnb_state.h -- the per-stream state blob (pnb_get_state / pnb_export_states) and the descriptors of the kernels that
+// gather it from and scatter it into an engine (pnb_state.cu).  Host and device code share this layout.
+#pragma once
+#include <stddef.h>
+#include "pnb_common.cuh"
+
+struct pnb_engine;
+
+namespace pnb {
+
+// The live part of the reference's DenoiseState + RNNState (src/denoise.cpp:71-85, src/nnet_data.h:28-38; SURVEY.md
+// App. A.2).  A stream moved between engines at a call boundary continues exactly from these bytes.
+struct StreamState {
+  unsigned magic, version;
+  float pcm[kKeep];          // the last 5280 input samples (comb_buf without its newest hop)
+  float synth[kFrame];       // overlap-add memory
+  int last_period;
+  float last_gain;
+  float spec[5][2 * kBins];  // spectra of the last five windowed blocks (analysis spectrum of the next five hops), oldest first
+  float eband[5][kBands];    // their band energies
+  float fc_hist[4][128];     // conv1 input history (last four fc outputs), oldest first
+  float c1_hist[2][512];     // conv2 input history (last two conv1 outputs)
+  float h[4 * 512 + 128];    // gru1, gru2, gru3, gru_gb, gru_rb
+  // tensor-mode engines keep the conv histories as three bf16 terms; the sum above does not always split back into the
+  // same terms (a low term of exactly half an ulp), so the raw terms travel too and a tensor-mode engine restores those
+  unsigned has_terms;
+  unsigned short fc_terms[3][4][128];
+  unsigned short c1_terms[3][2][512];
+};
+constexpr unsigned kStateMagic = 0x53424E50u;  // "PNBS"
+constexpr unsigned kStateVersion = 1;
+constexpr float kStateGruBound = 1.0001f;      // |GRU state| a tensor-mode engine accepts (tanh outputs and their mixes)
+
+// The blob is a wire format: its size and every offset are fixed.
+static_assert(sizeof(StreamState) == 63804, "StreamState is a wire format");
+static_assert(offsetof(StreamState, pcm) == 8 && offsetof(StreamState, synth) == 21128 &&
+              offsetof(StreamState, last_period) == 23048 && offsetof(StreamState, last_gain) == 23052 &&
+              offsetof(StreamState, spec) == 23056 && offsetof(StreamState, eband) == 39056 &&
+              offsetof(StreamState, fc_hist) == 39736 && offsetof(StreamState, c1_hist) == 41784 &&
+              offsetof(StreamState, h) == 45880 && offsetof(StreamState, has_terms) == 54584 &&
+              offsetof(StreamState, fc_terms) == 54588 && offsetof(StreamState, c1_terms) == 57660,
+              "StreamState field offsets are part of the wire format");
+
+// One piece of a stream's state: where it sits in the engine (stream s at eng + s * eng_stride) and in the blob.
+// The kinds say how each direction treats it:
+//   kSegCopy      n 32-bit words, engine <-> blob; reset zeroes the engine side
+//   kSegBlobZero  n words of the blob written as zero on export (parts the engine does not carry)
+//   kSegEngZero   n words of the engine zeroed on reset (engine-side taps that are not part of the blob)
+//   kSegSumBf16   export: n fp32 values = the sum of the three bf16 term planes (`plane` bytes apart), smallest first
+//   kSegTermBf16  term `term` of n bf16 values: export copies it to the blob, import restores it from the blob's raw
+//                 terms or, for a blob without them (has_terms == 0), splits it from the fp32 values at aux_off
+//   kSegSplitF16  import: term `term` (0 hi, 1 lo) of the fp16 split of n fp32 values x kActScale; reset zeroes it
+enum StateSegKind : short { kSegCopy = 0, kSegBlobZero, kSegEngZero, kSegSumBf16, kSegTermBf16, kSegSplitF16 };
+struct StateSeg {
+  char *eng;
+  size_t eng_stride;
+  size_t plane;
+  unsigned blob_off, aux_off;
+  unsigned n;
+  float scale;           // kSegSplitF16: the fp16 activation scale
+  short kind, term;
+};
+constexpr int kMaxStateSegs = 72;  // a tensor-mode engine needs 69
+constexpr int kStateSegMax = 512;  // words / elements per piece: long fields are cut into pieces of at most this
+
+enum StateMode { kStateExport = 0, kStateImport = 1, kStateReset = 2 };
+struct StateArgs {
+  StateSeg seg[kMaxStateSegs];
+  int n_seg;
+  int n;                 // streams in the batch
+  const int *streams;    // [n] engine slots
+  char *blobs;           // blob i at blobs + i * blob_stride (export: written, import: read, reset: null)
+  size_t blob_stride;
+  int *ok;               // [n] import: the verdict of state_check_kernel per blob
+  int mode;
+  unsigned has_terms;    // export: the blob's has_terms
+  // import checks
+  int check_gru;         // tensor-mode engines refuse GRU states outside kStateGruBound
+  int *status;           // the engine's status word [2]: bit 1 of [0] = a blob was rejected, [1] = lowest rejected slot
+};
+
+// Status bit raised when an import rejected a blob (reported once as PNB_ERR_ARG by the synchronising entry points).
+constexpr int kStatusRejected = 2;
+constexpr int kNoRejectedSlot = 0x7F7F7F7F;  // status[1] when nothing was rejected (a byte-wise memset can write it)
+
+// The pieces of a stream's state in engine e at its current hop / line offset / GRU parity (host counters committed
+// when a call is enqueued, so the list is right in stream order); returns their number (<= kMaxStateSegs).
+int state_segs(const pnb_engine *e, StateSeg *seg);
+int launch_state_check(const StateArgs &a, cudaStream_t st);
+int launch_state_move(const StateArgs &a, cudaStream_t st);
+int launch_state_clear_reject(int *status, cudaStream_t st);
+
+}  // namespace pnb

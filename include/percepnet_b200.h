@@ -241,11 +241,11 @@ long long pnb_launch_count(const pnb_engine *e);
  * streams' history back to the start of their rows, at most every call, typically every eighth). */
 int pnb_launches_per_call(const pnb_engine *e, int n_frames);
 
-/* How long calls are scheduled on this engine (PNB_NN_TENSOR engines with many streams): calls of at least two
- * chunks of `chunk_hops` hops run the network of chunk k on `net_sms` SMs while analysis of chunk k+1 and synthesis
- * of chunk k-1 run on the other `dsp_sms` SMs (two green contexts).  net_sms = 0: every call runs its kernels one
- * after the other on all SMs.  Environment: PNB_OVERLAP=0 disables, =2 forces it for small batches; PNB_NET_SMS,
- * PNB_CHUNK tune it (read by pnb_create).  Results do not depend on the schedule. */
+/* How long calls are scheduled on this engine.  net_sms = 0 (the default): every call runs its kernels one after the
+ * other on all SMs.  A PNB_NN_TENSOR engine created with PNB_OVERLAP=2 uses the chunked schedule instead: calls of at
+ * least two chunks of `chunk_hops` hops run the network of chunk k on `net_sms` SMs while analysis of chunk k+1 and
+ * synthesis of chunk k-1 run on the other `dsp_sms` SMs (two green contexts).  Environment (read by pnb_create):
+ * PNB_OVERLAP=2 enables it, PNB_NET_SMS, PNB_CHUNK tune it.  Results do not depend on the schedule. */
 int pnb_overlap_info(const pnb_engine *e, int *net_sms, int *dsp_sms, int *chunk_hops);
 /* on = 0: run every call serially on all SMs (e.g. to time one kernel class alone); on = 1: back to the partition the
  * engine was created with.  Waits for the engine to be idle. */

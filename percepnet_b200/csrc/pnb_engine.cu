@@ -373,14 +373,15 @@ extern "C" int pnb_create(pnb_engine **out, int n_streams, int max_frames, const
   if (flags & PNB_NN_TENSOR) {
     int trc = tc_prepare(e, model);
     if (trc) { pnb_destroy(e); return trc; }
-    // Calls of at least two chunks overlap the DSP kernels with the network on disjoint SMs (pnb_engine.h).
-    // PNB_OVERLAP=0 keeps the serial schedule; PNB_NET_SMS / PNB_CHUNK tune the split and the chunk length.
+    // Every call runs its kernels one after the other on all SMs (the serial schedule): on H100 it is faster than
+    // any measured split of the SMs between the network and the DSP kernels (DESIGN §6).  PNB_OVERLAP=2 sets up the
+    // chunked schedule instead, in which calls of at least two chunks overlap the DSP kernels with the network on
+    // disjoint SMs (pnb_engine.h); PNB_NET_SMS / PNB_CHUNK / PNB_RAMP tune the split and the chunks.
     const char *ov = getenv("PNB_OVERLAP"), *ns = getenv("PNB_NET_SMS"), *ch = getenv("PNB_CHUNK");
     if (ch && atoi(ch) >= 1) e->chunk = atoi(ch);
     const char *rp = getenv("PNB_RAMP");  // 0: all chunks equal (submitted calls overlap each other, so a call's ends need not be short)
     if (rp) e->ramp = atoi(rp) != 0;
-    const bool worth = (long long)n_streams >= 2048 && max_frames >= 2 * e->chunk && (max_frames + e->chunk - 1) / e->chunk + 5 <= kMaxChunks;
-    if (!(ov && atoi(ov) == 0) && (worth || (ov && atoi(ov) == 2)) && max_frames >= 2 * e->chunk)
+    if (ov && atoi(ov) == 2 && max_frames >= 2 * e->chunk && (max_frames + e->chunk - 1) / e->chunk + 5 <= kMaxChunks)
       setup_overlap(e, ns && atoi(ns) >= 8 ? atoi(ns) : (e->sm_count * 2 / 3 / 8) * 8);  // 88 of an H100's 132 (DESIGN §4)
   }
   CKD(cudaDeviceSynchronize());

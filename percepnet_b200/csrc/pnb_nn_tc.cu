@@ -20,15 +20,18 @@
 //                    no launch boundary between layers or hops.
 // Warpgroup roles per CTA: warpgroup 0 = TMA producer (one thread: cp.async.bulk.tensor into a ring of stages guarded
 // by full / empty mbarriers; dense layers SWIZZLE_128B boxes of 64 k, the chain SWIZZLE_64B boxes of 32 k),
-// warpgroups 1 and 2 = consumers: each issues wgmma for 64 of the tile's 128 rows (m64nNk16, operands from shared
-// memory, fp32 accumulators in registers) and runs the epilogue of its rows.  The producer streams the next tile's
+// warpgroups 1 and 2 = consumers: each issues wgmma for 64 of the tile's 128 rows (m64nNk16, fp32 accumulators in
+// registers; the dense layers take both operands from shared memory, the chain loads its activation operand into
+// registers with ldmatrix once per stage) and runs the epilogue of its rows.  The producer streams the next tile's
 // operands while the consumers finish the current one.
 //
 // The GRU tile holds, for 64 hidden units, three accumulators per unit: z and r summed over [x ; h], and the
 // candidate's W_n x and U_n h apart (nnet.cpp:136-173 needs the last two apart) -- 256 accumulator columns in three
 // register blocks nx (64), zr (128), nh (64).  Weight rows are packed [z|r|n] per tile in both parts, so one TMA box
 // brings a tile's rows; per product the input part issues N = 128 into zr and N = 64 into nx, the recurrent part
-// N = 128 into zr and N = 64 into nh.
+// N = 128 into zr and N = 64 into nh.  The six MMAs of a 16-wide k-step read only two 64 x 16 activation blocks (the
+// hi and lo terms), so those are loaded from shared memory into registers once (wgmma's A-from-registers form)
+// instead of being read again by every MMA.
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -144,33 +147,6 @@ __device__ __forceinline__ void wgmma<128, true>(float *d, uint64_t da, uint64_t
       : "l"(da), "l"(db), "r"(acc));
 }
 template <>
-__device__ __forceinline__ void wgmma<128, false>(float *d, uint64_t da, uint64_t db, uint32_t acc) {
-  asm volatile(PNB_WGMMA_PRED(66)
-      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, "
-      "%15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, "
-      "%39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, "
-      "%63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]),
-        "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]),
-        "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]),
-        "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]),
-        "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]),
-        "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]),
-        "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
-      : "l"(da), "l"(db), "r"(acc));
-}
-template <>
-__device__ __forceinline__ void wgmma<64, false>(float *d, uint64_t da, uint64_t db, uint32_t acc) {
-  asm volatile(PNB_WGMMA_PRED(34)
-      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, "
-      "%15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]),
-        "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]),
-        "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]),
-        "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-      : "l"(da), "l"(db), "r"(acc));
-}
-template <>
 __device__ __forceinline__ void wgmma<48, false>(float *d, uint64_t da, uint64_t db, uint32_t acc) {
   asm volatile(PNB_WGMMA_PRED(26)
       "wgmma.mma_async.sync.aligned.m64n48k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, "
@@ -180,7 +156,50 @@ __device__ __forceinline__ void wgmma<48, false>(float *d, uint64_t da, uint64_t
         "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])
       : "l"(da), "l"(db), "r"(acc));
 }
+// The same MMA with A from registers (the GRU chain): a[0..3] is this thread's share of the 64 x 16 A block -- rows
+// 16 warp + lane/4 (+8 in a[1], a[3]), k 2 (lane%4) (+8 in a[2], a[3]), two fp16 per register, as ldmatrix.x4
+// leaves it.  The registers are read asynchronously: they must not be rewritten before the MMA has completed.
+template <int N>
+__device__ __forceinline__ void wgmma_rs(float *d, const uint32_t *a, uint64_t db, uint32_t acc = 1);
+template <>
+__device__ __forceinline__ void wgmma_rs<128>(float *d, const uint32_t *a, uint64_t db, uint32_t acc) {
+  asm volatile(PNB_WGMMA_PRED(69)
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, "
+      "%15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, "
+      "%39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, "
+      "%63}, {%64, %65, %66, %67}, %68, p, 1, 1, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]),
+        "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]),
+        "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]),
+        "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]),
+        "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]),
+        "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]),
+        "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(acc));
+}
+template <>
+__device__ __forceinline__ void wgmma_rs<64>(float *d, const uint32_t *a, uint64_t db, uint32_t acc) {
+  asm volatile(PNB_WGMMA_PRED(37)
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, "
+      "%15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]),
+        "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]),
+        "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]),
+        "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(acc));
+}
 #undef PNB_WGMMA_PRED
+__device__ __forceinline__ void ldsm_x4(uint32_t *r, uint32_t addr) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
+               : "r"(addr)
+               : "memory");
+}
+template <int R>
+__device__ __forceinline__ void reg_fence(uint32_t *r) {  // acc_fence for the A fragments
+#pragma unroll
+  for (int i = 0; i < R; i++) asm volatile("" : "+r"(r[i])::"memory");
+}
 
 // ------------------------------------------------------------------------------------------ activations
 // tansig_approx of vec.h:53-71 on the FMA/ALU pipes only.  The reference forms the table index with
@@ -325,6 +344,10 @@ struct Consumer {
   uint32_t prev_empty = 0;
   __device__ __forceinline__ void begin(float *acc, uint32_t full_bar, uint32_t parity) {
     mbar_wait(full_bar, parity);
+    fence(acc);
+  }
+  // orders the MMAs after every register write before them (accumulators, A fragments loaded after the barrier wait)
+  __device__ __forceinline__ void fence(float *acc) {
     acc_fence<ACC_REGS>(acc);
     wgmma_fence();
   }
@@ -616,23 +639,67 @@ using GruStage = StageLayout<GRU_BN, 2, CBK>;  // 2 x 8 KB of A + 2 x 12 KB of B
 // gives 168 to each of the 384 threads; 128 x (168 - 40) = 256 x (232 - 168).
 constexpr int kProducerRegs = 40, kConsumerRegs = 232;
 
-// One k-block (CBK = two 16-wide k-steps) of a GRU tile on one consumer warpgroup: per k-step the three products
-// hi hi, hi lo, lo hi of weight rows [z|r] (N = 128) into `zr` and of rows [n] (N = 64) into `n`, the two register
-// blocks alternating so that consecutive MMAs do not wait on each other's accumulators.  zr_acc / n_acc = 0: the
-// k-block starts the block's sum (its first MMA overwrites the registers).
-__device__ __forceinline__ void gru_mma_kblock(float *zr, float *n, uint32_t a_lo, uint32_t b_lo, uint32_t zr_acc, uint32_t n_acc) {
-  constexpr uint32_t A = GruStage::kABytes >> 4, B = GruStage::kBBytes >> 4;
+// A fragments of one k-block (CBK = two 16-wide k-steps, both terms of A) for one consumer warp: 16 registers,
+// fa[8 term + 4 ks + i] (wgmma_rs layout).  `a_addr[ks]` is this lane's ldmatrix row address for k-step ks in the first A term of stage
+// 0 (gru_a_addr); `so` the stage's byte offset.
+constexpr int kFragRegs = 2 * (CBK / 16) * 4;
+__device__ __forceinline__ void gru_load_a(uint32_t *fa, const uint32_t *a_addr, uint32_t so) {
+#pragma unroll
+  for (int t = 0; t < 2; t++)
+#pragma unroll
+    for (int ks = 0; ks < CBK / 16; ks++) ldsm_x4(fa + 8 * t + 4 * ks, a_addr[ks] + so + t * GruStage::kABytes);
+}
+// ldmatrix.x4 row addresses: lanes 8m .. 8m+7 address the rows of 8x8 matrix m = (rows +8 (m&1), k +8 (m>>1)) of the
+// warp's 16 rows, which puts the fragment in the order wgmma_rs reads it.  The TMA box wrote the 64-byte rows with
+// SWIZZLE_64B: the 16-byte chunk index XOR address bits 7-8, i.e. XOR (row / 2) % 4 (the stage is 1024-byte aligned).
+__device__ __forceinline__ void gru_a_addr(uint32_t *a_addr, uint32_t stage0, int cw, int warp, int lane) {
+  const int row = cw * 64 + warp * 16 + (lane & 7) + 8 * ((lane >> 3) & 1);
+#pragma unroll
+  for (int ks = 0; ks < CBK / 16; ks++) {
+    const int chunk = 2 * ks + (lane >> 4);
+    a_addr[ks] = stage0 + row * (CBK * 2) + ((chunk ^ ((row >> 1) & 3)) << 4);
+  }
+}
+
+// One k-block of a GRU tile on one consumer warpgroup: per k-step the three products hi hi, hi lo, lo hi of weight
+// rows [z|r] (N = 128) into `zr` and of rows [n] (N = 64) into `n`, the two register blocks alternating so that
+// consecutive MMAs do not wait on each other's accumulators.  A (the activations) comes from the fragments `fa`
+// (gru_load_a), B from the stage.  zr_acc / n_acc = 0: the k-block starts the block's sum (its first MMA overwrites
+// the registers).
+__device__ __forceinline__ void gru_mma_kblock(float *zr, float *n, const uint32_t *fa, uint32_t b_lo, uint32_t zr_acc, uint32_t n_acc) {
+  constexpr uint32_t B = GruStage::kBBytes >> 4;
   constexpr uint32_t BN = (2 * HT * CBK * 2) >> 4;  // the n rows follow the 2 HT rows of [z|r]
 #pragma unroll
   for (int ks = 0; ks < CBK / 16; ks++) {
-    const uint32_t a = a_lo + ks * 2, b = b_lo + ks * 2;
-    wgmma<128, false>(zr, desc64(a, kDescHi64), desc64(b, kDescHi64), ks ? 1u : zr_acc);
-    wgmma<64, false>(n, desc64(a, kDescHi64), desc64(b + BN, kDescHi64), ks ? 1u : n_acc);
-    wgmma<128, false>(zr, desc64(a, kDescHi64), desc64(b + B, kDescHi64));
-    wgmma<64, false>(n, desc64(a, kDescHi64), desc64(b + B + BN, kDescHi64));
-    wgmma<128, false>(zr, desc64(a + A, kDescHi64), desc64(b, kDescHi64));
-    wgmma<64, false>(n, desc64(a + A, kDescHi64), desc64(b + BN, kDescHi64));
+    const uint32_t *hi = fa + 4 * ks, *lo = fa + 8 + 4 * ks;
+    const uint32_t b = b_lo + ks * 2;
+    wgmma_rs<128>(zr, hi, desc64(b, kDescHi64), ks ? 1u : zr_acc);
+    wgmma_rs<64>(n, hi, desc64(b + BN, kDescHi64), ks ? 1u : n_acc);
+    wgmma_rs<128>(zr, hi, desc64(b + B, kDescHi64));
+    wgmma_rs<64>(n, hi, desc64(b + B + BN, kDescHi64));
+    wgmma_rs<128>(zr, lo, desc64(b, kDescHi64));
+    wgmma_rs<64>(n, lo, desc64(b + BN, kDescHi64));
   }
+}
+
+// Consumer side of one k-block of a GRU unit: wait for the stage, load its A fragments into `fa`, issue the MMAs into
+// `zr` and `n` (the nx or nh block of `acc`), free the previous stage.  One k-block stays in flight and reads its
+// fragments asynchronously, so consecutive k-blocks use different `fa`: gru_chain_kernel alternates two, k-blocks
+// in pairs.  Every part of a unit has an even number of k-blocks (inputs are 512 wide, H a multiple of HT).
+constexpr int kChainAccRegs = 4 * HT / 2;  // nx (64 columns), zr (128), nh (64)
+constexpr int NX = 0, ZR = HT / 2, NH = 3 * HT / 2;
+static_assert(512 % (2 * CBK) == 0 && HT % (2 * CBK) == 0, "the chain's k-blocks are consumed in pairs");
+__device__ __forceinline__ void gru_consume_kblock(float *acc, float *n, uint32_t *fa, uint32_t zr_acc, uint32_t n_acc,
+                                                   const uint32_t *a_addr, uint32_t b_lo0, const SmemCarve &c, Pipe &p,
+                                                   Consumer<kChainAccRegs> &cons) {
+  mbar_wait(c.full + 8 * p.st, p.ph);
+  const uint32_t so = p.st * GruStage::kBytes;
+  gru_load_a(fa, a_addr, so);
+  reg_fence<kFragRegs>(fa);
+  cons.fence(acc);
+  gru_mma_kblock(acc + ZR, n, fa, b_lo0 + (so >> 4), zr_acc, n_acc);
+  cons.end(acc, c.empty + 8 * p.st);
+  p.advance(GRU_STAGES);
 }
 
 __global__ void __launch_bounds__(kTcThreads, 1) gru_chain_kernel(const __grid_constant__ ChainArgs args) {
@@ -641,8 +708,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) gru_chain_kernel(const __grid_c
   // accumulator registers per thread, three blocks: nx = W_n x (64 columns), zr = [z | r] over [x ; h] (128 columns),
   // nh = U_n h (64 columns).  The blocks never overlap partially: wgmma into partly overlapping register ranges
   // would serialise the MMA pipeline.
-  constexpr int R = 4 * HT / 2;
-  constexpr int NX = 0, ZR = HT / 2, NH = 3 * HT / 2;
+  constexpr int R = kChainAccRegs;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   const SmemCarve c = carve<STAGES, STAGES * SL::kBytes>(smem_raw);
   const int wg = threadIdx.x >> 7;
@@ -688,8 +754,9 @@ __global__ void __launch_bounds__(kTcThreads, 1) gru_chain_kernel(const __grid_c
     // ===== consumer warpgroup: MMAs of its 64 streams, then the gate math of nnet.cpp:136-178 (reset_after) =====
     asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kConsumerRegs));
     const int cw = wg - 1, warp = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
-    const uint32_t a_lo0 = desc_lo(stage0) + (uint32_t)(cw * 64 * CBK * 2 >> 4);
     const uint32_t b_lo0 = desc_lo(stage0) + (uint32_t)(2 * SL::kABytes >> 4);
+    uint32_t a_addr[CBK / 16];
+    gru_a_addr(a_addr, stage0, cw, warp, lane);
     const float *tbl = c.tbl;
     Pipe p;
     Consumer<R> cons;
@@ -698,22 +765,17 @@ __global__ void __launch_bounds__(kTcThreads, 1) gru_chain_kernel(const __grid_c
       const ChainLayer &L = args.L[un.l];
       const int H = L.H;
       float acc[R];  // no zero fill: the first k-block of either part starts its blocks' sums
+      uint32_t fa0[kFragRegs], fa1[kFragRegs];  // A fragments of the even / odd k-blocks
       // input part: [z|r] rows into zr, n rows into nx; recurrent part: [z|r] rows into zr, n rows into nh
       int nkb = 0;
       for (int s = 0; s < L.n_x; s++) nkb += L.x_kb[s];
-      for (int kb = 0; kb < nkb; kb++) {
-        cons.begin(acc, c.full + 8 * p.st, p.ph);
-        const uint32_t so = p.st * (SL::kBytes >> 4);
-        gru_mma_kblock(acc + ZR, acc + NX, a_lo0 + so, b_lo0 + so, kb != 0, kb != 0);
-        cons.end(acc, c.empty + 8 * p.st);
-        p.advance(STAGES);
+      for (int kb = 0; kb < nkb; kb += 2) {
+        gru_consume_kblock(acc, acc + NX, fa0, kb != 0, kb != 0, a_addr, b_lo0, c, p, cons);
+        gru_consume_kblock(acc, acc + NX, fa1, 1u, 1u, a_addr, b_lo0, c, p, cons);
       }
-      for (int kb = 0; kb < L.h_kb; kb++) {
-        cons.begin(acc, c.full + 8 * p.st, p.ph);
-        const uint32_t so = p.st * (SL::kBytes >> 4);
-        gru_mma_kblock(acc + ZR, acc + NH, a_lo0 + so, b_lo0 + so, 1u, kb != 0);
-        cons.end(acc, c.empty + 8 * p.st);
-        p.advance(STAGES);
+      for (int kb = 0; kb < L.h_kb; kb += 2) {
+        gru_consume_kblock(acc, acc + NH, fa0, 1u, kb != 0, a_addr, b_lo0, c, p, cons);
+        gru_consume_kblock(acc, acc + NH, fa1, 1u, 1u, a_addr, b_lo0, c, p, cons);
       }
       cons.drain(acc);
       // the previous hop's state of these rows is complete (other SMs wrote it): acquire before reading it

@@ -1,6 +1,7 @@
 #!/usr/bin/env python
-"""Launch timeline of two submitted long calls (chunked overlap schedule, calls overlapping each other): prints every launch with its start/end and the busy time
-of the two partitions.  Run on the GPU box: python tools/timeline.py [streams] [frames]"""
+"""Launch timeline of two submitted long calls (calls overlapping each other): prints every launch with its start/end and the busy time
+of the network and DSP kernels.  Run on the GPU box: python tools/timeline.py [streams] [frames]; PNB_OVERLAP=2 for the chunked
+schedule on two SM partitions (the default is the serial schedule)."""
 import json
 import os
 import sys

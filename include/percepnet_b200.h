@@ -91,10 +91,10 @@ int pnb_model_load_blob(const char *path, pnb_model **out);
 int pnb_model_load_stream(void *file, pnb_model **out);
 void pnb_model_free(pnb_model *m);
 
-/* Host buffers (pageable or pinned).  in/out: n_streams rows of n_frames*480 samples, row strides
- * in elements.  in may equal out.  gr (NULL ok) receives the raw network outputs the reference
- * fwrite()s per frame (src/denoise.cpp:533-534) as [n_frames][n_streams][68] = 34 g then 34 r.
- * Blocking: returns when out (and gr) are complete. */
+/* Host buffers (pageable or pinned).  in/out: the active rows (n = pnb_active_streams(e), n_streams unless
+ * pnb_set_active_streams changed it) of n_frames*480 samples, row strides in elements.  in may equal out.  gr (NULL ok)
+ * receives the raw network outputs the reference fwrite()s per frame (src/denoise.cpp:533-534) as [n_frames][n][68] =
+ * 34 g then 34 r.  Blocking: returns when out (and gr) are complete. */
 int pnb_process_host_f32(pnb_engine *e, const float *in, size_t in_stride, float *out, size_t out_stride,
                          int n_frames, float *gr);
 
@@ -103,7 +103,8 @@ int pnb_process_host_f32(pnb_engine *e, const float *in, size_t in_stride, float
 int pnb_process_host_i16(pnb_engine *e, const short *in, size_t in_stride, short *out, size_t out_stride,
                          int n_frames, float *gr);
 
-/* Pipelined host entry for sustained throughput: enqueues host->device copy, processing and device->host copy
+/* Pipelined host entry for sustained throughput (in/out: the active rows, as above): enqueues host->device copy,
+ * processing and device->host copy
  * on internal streams and returns; the copies of neighbouring calls overlap the kernels.  At most two calls are
  * in flight (a third blocks until the oldest completed).  Buffers must stay valid -- and should be pinned --
  * until pnb_wait() returns.  Calls are processed in submission order (the streams' state advances in order). */
@@ -117,13 +118,13 @@ int pnb_wait(pnb_engine *e);
 int pnb_check(pnb_engine *e, void *cuda_stream);
 
 /* Device buffers on the engine's device; asynchronous on cuda_stream (a cudaStream_t, NULL = default
- * stream).  d_gr (NULL ok) as above, in device memory. */
+ * stream).  in/out hold the active rows as above; d_gr (NULL ok) as above, in device memory. */
 int pnb_process_device_f32(pnb_engine *e, const float *d_in, size_t in_stride, float *d_out, size_t out_stride,
                            int n_frames, float *d_gr, void *cuda_stream);
 int pnb_process_device_i16(pnb_engine *e, const short *d_in, size_t in_stride, short *d_out, size_t out_stride,
                            int n_frames, float *d_gr, void *cuda_stream);
 
-/* Submitted twins of pnb_process_device_*: the call starts when cuda_stream reaches this point (its inputs are ready in
+/* Submitted twins of pnb_process_device_* (in/out: the active rows): the call starts when cuda_stream reaches this point (its inputs are ready in
  * that stream's order) but is NOT joined back into it, so a following call's analysis overlaps this call's network and
  * synthesis (the engine orders what they share).  d_out is complete once pnb_flush(e, stream) has made `stream` wait for
  * everything submitted so far, or after pnb_wait / pnb_check on the host.  Calls of one engine are issued in order. */
@@ -187,6 +188,20 @@ int pnb_set_state(pnb_engine *e, int stream, const void *src, size_t src_bytes);
 int pnb_reset_streams(pnb_engine *e, const int *streams, int n, void *cuda_stream);
 int pnb_export_states(pnb_engine *e, const int *streams, int n, void *d_blobs, size_t blob_stride, void *cuda_stream);
 int pnb_import_states(pnb_engine *e, const int *streams, int n, const void *d_blobs, size_t blob_stride, void *cuda_stream);
+
+/* Active range: calls issued after pnb_set_active_streams(e, n, .) advance slots [0, n) only, 1 <= n <= n_streams, and
+ * cost roughly n / n_streams of a full call (rounded up to 128-stream tiles in the network).  A fresh engine, and an
+ * engine after pnb_reset, has n = n_streams.  n is taken when a call is issued: calls already submitted keep theirs.
+ *   Growing n: the entering slots are reset as by pnb_reset_streams, asynchronously on cuda_stream and ordered like
+ *   any state operation.  pnb_import_states after the grow gives an entering slot a state.
+ *   Shrinking n enqueues nothing: the leaving slots lose their state (pnb_export_states them first to keep it).
+ * In and out of every pnb_process_* / pnb_submit_* call hold n rows, gr / d_gr is [n_frames][n][68]; pnb_read_tap keeps
+ * its n_streams layout (rows >= n unspecified).  Live sessions stay packed in [0, n): when the session at slot k ends,
+ * export slot n-1, import it at k, then shrink to n-1.
+ * Refused with PNB_ERR_ARG before anything is enqueued: n outside [1, n_streams], a PNB_TRAIN_DATA engine, a poisoned
+ * engine.  pnb_reset_streams / pnb_export_states / pnb_import_states / pnb_get_state / pnb_set_state refuse slots >= n. */
+int pnb_set_active_streams(pnb_engine *e, int n, void *cuda_stream);
+int pnb_active_streams(const pnb_engine *e);
 
 /* The pitch analysis alone (BASELINE.json config 5; needs no engine): for each of n_units pitch buffers of 1728
  * float samples (unit u at d_pitch_buf + u*stride; the reference's st->pitch_buf, src/denoise.cpp:80,405-411) runs

@@ -69,6 +69,8 @@ def load_library() -> C.CDLL:
     L.pnb_reset_streams.argtypes = [vp, vp, i, vp]
     L.pnb_export_states.argtypes = [vp, vp, i, vp, sz, vp]
     L.pnb_import_states.argtypes = [vp, vp, i, vp, sz, vp]
+    L.pnb_set_active_streams.argtypes = [vp, i, vp]
+    L.pnb_active_streams.argtypes = [vp]
     L.pnb_pitch_only_device.argtypes = [vp, sz, C.c_longlong, vp, vp, vp, vp, vp, vp, vp]
     L.pnb_pitch_only_host.argtypes = [vp, sz, C.c_longlong, vp, vp, vp, vp, vp, vp]
     L.pnb_launch_count.argtypes = [vp]
@@ -92,7 +94,7 @@ def load_library() -> C.CDLL:
 EXPORTS = ("pnb_create", "pnb_destroy", "pnb_reset", "pnb_process_host_f32", "pnb_process_host_i16",
            "pnb_model_load_blob", "pnb_model_load_stream", "pnb_model_free", "pnb_train_records_host", "pnb_train_records_device", "pnb_submit_train_records", "pnb_process_device_f32", "pnb_process_device_i16", "pnb_submit_host_f32", "pnb_submit_host_i16", "pnb_submit_device_f32", "pnb_submit_device_i16", "pnb_flush", "pnb_wait", "pnb_check",
            "pnb_read_tap", "pnb_state_size", "pnb_get_state", "pnb_set_state",
-           "pnb_reset_streams", "pnb_export_states", "pnb_import_states", "pnb_pitch_only_device", "pnb_pitch_only_host", "pnb_launch_count",
+           "pnb_reset_streams", "pnb_export_states", "pnb_import_states", "pnb_set_active_streams", "pnb_active_streams", "pnb_pitch_only_device", "pnb_pitch_only_host", "pnb_launch_count",
            "pnb_launches_per_call", "pnb_profile_enable", "pnb_profile_read", "pnb_profile_timeline", "pnb_kernel_class_name", "pnb_n_streams", "pnb_overlap_info", "pnb_set_overlap", "pnb_max_frames", "pnb_last_error", "pnb_version")
 
 
@@ -169,14 +171,25 @@ class Engine:
     def reset(self):
         self._ck(self.L.pnb_reset(self.h), "pnb_reset")
 
+    @property
+    def active(self) -> int:
+        """Streams the next call advances: slots [0, active) (pnb_active_streams; n_streams unless set_active changed it)."""
+        return int(self.L.pnb_active_streams(self.h))
+
+    def set_active(self, n: int, stream: int = 0):
+        """pnb_set_active_streams: later calls advance slots [0, n) only.  Slots entering the range start as fresh streams
+        (reset asynchronously on `stream`); slots leaving it lose their state."""
+        self._ck(self.L.pnb_set_active_streams(self.h, n, stream or None), "pnb_set_active_streams")
+
     def process(self, x: np.ndarray, want_gr: bool = False):
-        """x: [S, F*480] float32 (C-API scale) or int16 (CLI wire format) host array.
-        Returns (out like x, gr [F, S, 68] or None)."""
-        assert x.ndim == 2 and x.shape[0] == self.n_streams and x.shape[1] % FRAME == 0
+        """x: [active, F*480] float32 (C-API scale) or int16 (CLI wire format) host array.
+        Returns (out like x, gr [F, active, 68] or None)."""
+        n = self.active
+        assert x.ndim == 2 and x.shape[0] == n and x.shape[1] % FRAME == 0
         F = x.shape[1] // FRAME
         x = np.ascontiguousarray(x)
         out = np.empty_like(x)
-        gr = np.empty((F, self.n_streams, 68), np.float32) if want_gr else None
+        gr = np.empty((F, n, 68), np.float32) if want_gr else None
         grp = gr.ctypes.data if want_gr else None
         if x.dtype == np.float32:
             rc = self.L.pnb_process_host_f32(self.h, x.ctypes.data, x.shape[1], out.ctypes.data, x.shape[1], F, grp)
@@ -188,7 +201,7 @@ class Engine:
         return out, gr
 
     def process_stream_chunks(self, x: np.ndarray, want_gr: bool = False):
-        """Any number of hops: walks x in calls of at most max_frames hops."""
+        """Any number of hops: walks x ([active, F*480]) in calls of at most max_frames hops."""
         F = x.shape[1] // FRAME
         outs, grs = [], []
         for t0 in range(0, F, self.max_frames):
@@ -214,9 +227,9 @@ class Engine:
         self._ck(self.L.pnb_flush(self.h, stream or None), "pnb_flush")
 
     def submit(self, x: np.ndarray, out: np.ndarray):
-        """Pipelined host call (pnb_submit_host_*): returns at once; x/out ([S, F*480] float32 or int16, ideally
+        """Pipelined host call (pnb_submit_host_*): returns at once; x/out ([active, F*480] float32 or int16, ideally
         pinned) must stay alive until wait()."""
-        assert x.shape == out.shape and x.dtype == out.dtype and x.shape[0] == self.n_streams
+        assert x.shape == out.shape and x.dtype == out.dtype and x.shape[0] == self.active
         F = x.shape[1] // FRAME
         f = self.L.pnb_submit_host_f32 if x.dtype == np.float32 else self.L.pnb_submit_host_i16
         self._ck(f(self.h, x.ctypes.data, x.strides[0] // x.itemsize, out.ctypes.data, out.strides[0] // out.itemsize, F),

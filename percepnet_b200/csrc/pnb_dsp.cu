@@ -741,7 +741,7 @@ __global__ void __launch_bounds__(AnaCfg<L>::kWarps * 32) analysis_kernel(Analys
 #endif
   for (int t = 0; t < A.n_frames; t++) {
     const float *line = row + (size_t)t * kFrame;  // line[j] == reference comb_buf[j] at this hop
-    const size_t fs = (size_t)t * A.n_streams + s;
+    const size_t fs = (size_t)t * A.stride + s;
 
     // ---- pre-pass, once per group of kAcHops hops: the five autocorrelations pitch_downsample needs
     // (pitch.cpp:182 -> celt_lpc.cpp:198-279).  Inside a hop only five lanes can work on them (one strictly
@@ -803,7 +803,7 @@ __global__ void __launch_bounds__(AnaCfg<L>::kWarps * 32) analysis_kernel(Analys
     }
     ANA_TICK(0);
     {
-      float2 *Zg = A.zring + ((size_t)slot_new * A.n_streams + s) * kBins;
+      float2 *Zg = A.zring + ((size_t)slot_new * A.stride + s) * kBins;
       for (int k = lane; k < kBins; k += L) {
         float2 x = W.fft[fpos(k)];
         Zg[k] = x;
@@ -813,14 +813,14 @@ __global__ void __launch_bounds__(AnaCfg<L>::kWarps * 32) analysis_kernel(Analys
         xo[k] = B.omf[k] * e;
       }
       band_pool_warp<L>(W.xc, xo, W.Ey, B.border, lane, mask);
-      float *Eg = A.ering + ((size_t)slot_new * A.n_streams + s) * kBands;
-      const float *Eo = A.ering + ((size_t)slot_x * A.n_streams + s) * kBands;
+      float *Eg = A.ering + ((size_t)slot_new * A.stride + s) * kBands;
+      const float *Eo = A.ering + ((size_t)slot_x * A.stride + s) * kBands;
       for (int b = lane; b < kBands; b += L) {
         Eg[b] = W.Ey[b];
         W.Ex[b] = Eo[b];  // written five hops ago (by this lane group, or by the previous call)
       }
     }
-    const float2 *Xg = A.zring + ((size_t)slot_x * A.n_streams + s) * kBins;
+    const float2 *Xg = A.zring + ((size_t)slot_x * A.stride + s) * kBins;
     __syncwarp(mask);
     ANA_TICK(1);
 
@@ -949,7 +949,7 @@ __global__ void __launch_bounds__(kSynWarps * 32) synthesis_kernel(SynthesisArgs
   for (int i = 0; i < 15; i++) mem[i] = A.synth_mem[(size_t)s * kFrame + lane + 32 * i];
 
   for (int t = 0; t < A.n_frames; t++) {
-    const size_t fs = (size_t)t * A.n_streams + s;
+    const size_t fs = (size_t)t * A.stride + s;
     const float *gr = A.gr + fs * 68;
     for (int b = lane; b < kBands; b += 32) {
       float g = gr[b], r = gr[kBands + b];
@@ -981,7 +981,7 @@ __global__ void __launch_bounds__(kSynWarps * 32) synthesis_kernel(SynthesisArgs
     const bool silence = A.silence[fs] != 0;
     const long c = A.hop0 + t;
     const int slot_x = (int)(((c - 5) % A.ring + A.ring) % A.ring);
-    const float2 *Xg = A.zring + ((size_t)slot_x * A.n_streams + s) * kBins, *Pg = A.P + fs * kBins;
+    const float2 *Xg = A.zring + ((size_t)slot_x * A.stride + s) * kBins, *Pg = A.P + fs * kBins;
     // bins 0..399 and their mirror images; everything from 400 to 560 is zero (SURVEY.md App. C.1)
     {
       const float *frac = B.frac, *omf = B.omf;

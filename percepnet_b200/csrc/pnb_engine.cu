@@ -253,6 +253,7 @@ extern "C" int pnb_create(pnb_engine **out, int n_streams, int max_frames, const
 
   pnb_engine *e = new pnb_engine();
   e->S = n_streams;
+  e->n_active = n_streams;
   e->Fmax = max_frames;
   e->device = device;
   e->flags = flags;
@@ -472,6 +473,7 @@ extern "C" int pnb_reset(pnb_engine *e) {
   e->h_status[0] = 0;
   e->h_status[1] = kNoRejectedSlot;
   e->hop = 0;
+  e->n_active = e->S;
   e->poisoned = false;
   e->unjoined = false;      // the device was synchronised above (green-context streams included)
   e->prev_start.clear();
@@ -574,17 +576,19 @@ static GemmSeg seg(const float *A, int lda, const float *B, int ldb, int K) {
 }
 
 // The network of hops [h0, h0 + n) of a call (n <= e->f32_chunk) in fp32 FMA (rnn.cpp:42-81): the non-recurrent layers
-// once over all n S rows, the five GRUs of all n hops in one persistent launch, the output layers over n S rows, and the
-// carry that moves the conv histories and the states back to the front of their slot buffers.
+// once over the active rows of all n hop slots, the five GRUs of all n hops in one persistent launch, the output layers
+// over the same rows, and the carry that moves the conv histories and the states back to the front of their slot buffers.
 static int nn_chunk_f32(pnb_engine *e, int h0, int n, cudaStream_t st) {
-  const int S = e->S, rows = n * S;
+  const int S = e->S, na = e->n_active;
+  // all streams active: the rows of the n slots are one flat range; otherwise the first na rows of each slot
+  const int rows = na == S ? n * S : na, slots = na == S ? 1 : n;
   const float *tbl = e->tansig();
   int nl = 0;
   // fc -> slots 4.. (slots 0..3 hold the last four hops' outputs)
-  { ProfScope ps(e, PNB_K_FC, st); nl += launch_fc_f32(e->d_feat + (size_t)h0 * S * kFeat, e->fc.W, e->fc.b, e->ring_fc + (size_t)4 * S * 128, rows, 70, 128, st); }
+  { ProfScope ps(e, PNB_K_FC, st); nl += launch_fc_f32(e->d_feat + (size_t)h0 * S * kFeat, e->fc.W, e->fc.b, e->ring_fc + (size_t)4 * S * 128, rows, 70, 128, slots, S, st); }
   GemmArgs g;
   memset(&g, 0, sizeof g);
-  g.M = rows; g.tansig = tbl;
+  g.M = rows; g.n_slots = slots; g.slot_stride = S; g.tansig = tbl;
   // conv1: tap q of hop t reads fc slot t + q (oldest first, nnet.cpp:182-200; weights [tap][c][n]) -> c1 slots 2..
   for (int q = 0; q < 5; q++) g.seg[q] = seg(e->ring_fc + (size_t)q * S * 128, 128, e->conv1.W + (size_t)q * 128 * 512, 512, 128);
   g.n_seg = 5; g.N = 512; g.C = e->ring_c1 + (size_t)2 * S * 512; g.ldc = 512; g.bias = e->conv1.b; g.act = e->act_conv1;
@@ -596,7 +600,8 @@ static int nn_chunk_f32(pnb_engine *e, int h0, int n, cudaStream_t st) {
   // stacked GRUs: each consumes the freshly updated state of the one below (SURVEY.md App. C.10)
   F32ChainArgs a;
   memset(&a, 0, sizeof a);
-  a.S = S; a.n_rb = e->f32_rb; a.cnt = e->f32_cnt; a.tansig = tbl;
+  const int n_rb = (int)(((size_t)na + 16 * e->f32_rt - 1) / (16 * e->f32_rt));  // stream blocks of the active streams
+  a.S = S; a.n = na; a.n_rb = n_rb; a.cnt = e->f32_cnt; a.tansig = tbl;
   for (int li = 0; li < 5; li++) {
     F32ChainLayer &L = a.L[li];
     const int H = e->gru[li].H;
@@ -621,7 +626,7 @@ static int nn_chunk_f32(pnb_engine *e, int h0, int n, cudaStream_t st) {
         if (t < 0 || t >= n) continue;
         a.lh[k] = (unsigned char)((t << 3) | li);
         a.lh_unit0[k] = unit;
-        unit += e->f32_rb * (e->gru[li].H / 32);
+        unit += n_rb * (e->gru[li].H / 32);
         k++;
       }
     a.lh_unit0[k] = unit;
@@ -645,13 +650,15 @@ static int nn_chunk_f32(pnb_engine *e, int h0, int n, cudaStream_t st) {
   F32CarryArgs c;
   memset(&c, 0, sizeof c);
   int ns = 0;
-  auto cseg = [&](float *base, size_t slot_floats, int n_slots, int from) {
-    c.seg[ns++] = F32CarrySeg{reinterpret_cast<float4 *>(base), reinterpret_cast<const float4 *>(base + (size_t)from * slot_floats), slot_floats / 4, n_slots};
+  auto cseg = [&](float *base, size_t width, int n_slots, int from) {  // the active rows of n_slots slots of [S][width]
+    c.seg[ns++] = F32CarrySeg{reinterpret_cast<float4 *>(base), reinterpret_cast<const float4 *>(base + (size_t)from * S * width),
+                              (size_t)na * width / 4, (size_t)S * width / 4, n_slots};
   };
-  cseg(e->ring_fc, (size_t)S * 128, 4, n);
-  cseg(e->ring_c1, (size_t)S * 512, 2, n);
-  for (int li = 0; li < 5; li++) cseg(e->h[li][0], (size_t)S * e->gru[li].H, 1, n);
-  c.seg[ns++] = F32CarrySeg{reinterpret_cast<float4 *>(e->c2), reinterpret_cast<const float4 *>(e->c2_all + (size_t)(n - 1) * S * 512), (size_t)S * 512 / 4, 1};
+  cseg(e->ring_fc, 128, 4, n);
+  cseg(e->ring_c1, 512, 2, n);
+  for (int li = 0; li < 5; li++) cseg(e->h[li][0], e->gru[li].H, 1, n);
+  c.seg[ns++] = F32CarrySeg{reinterpret_cast<float4 *>(e->c2), reinterpret_cast<const float4 *>(e->c2_all + (size_t)(n - 1) * S * 512),
+                            (size_t)na * 512 / 4, (size_t)S * 512 / 4, 1};
   c.n_seg = ns; c.cnt = e->f32_cnt; c.n_cnt = 5 * e->f32_rb;
   { ProfScope ps(e, PNB_K_F32_CARRY, st); nl += launch_f32_carry(c, st); }
   return nl;
@@ -664,7 +671,7 @@ static int advance_line(pnb_engine *e, int F, cudaStream_t st) {
   e->line_off += (size_t)F * kFrame;
   if (e->line_off + kKeep + (size_t)e->Fmax * kFrame <= e->pcm_stride) return 0;
   ProfScope ps(e, PNB_K_SLIDE, st);
-  int n = launch_slide_history(e->d_pcm, e->pcm_stride, e->S, (int)e->line_off, st);
+  int n = launch_slide_history(e->d_pcm, e->pcm_stride, e->n_active, (int)e->line_off, st);  // inactive rows: no state to keep
   e->line_off = 0;
   return n;
 }
@@ -675,7 +682,7 @@ static AnalysisArgs analysis_args(pnb_engine *e, int h0, int n) {
   const size_t S = e->S, o = (size_t)h0 * S;
   AnalysisArgs a;
   a.pcm = e->d_pcm + e->line_off + (size_t)h0 * kFrame;  // this chunk's [history | new hops] window of every row
-  a.pcm_stride = e->pcm_stride; a.n_streams = e->S; a.n_frames = n; a.tab = e->d_tab;
+  a.pcm_stride = e->pcm_stride; a.n_streams = e->n_active; a.stride = e->S; a.n_frames = n; a.tab = e->d_tab;
   a.feat = e->d_feat + o * kFeat; a.zring = e->d_zring; a.ering = e->d_ering; a.ring = e->ring; a.hop0 = e->hop + h0;
   a.P = e->d_P ? e->d_P + o * kBins : nullptr; a.Ex = e->d_Ex + o * kBands; a.raw = nullptr; a.silence = e->d_sil + o;
   a.last_period = e->d_last_period; a.last_gain = e->d_last_gain;
@@ -687,7 +694,7 @@ static SynthesisArgs synthesis_args(pnb_engine *e, int h0, int n, float *d_out, 
   const size_t S = e->S, o = (size_t)h0 * S;
   SynthesisArgs s;
   s.zring = e->d_zring; s.ring = e->ring; s.hop0 = e->hop + h0; s.P = e->d_P + o * kBins; s.gr = e->d_gr + o * 68;
-  s.Ex = e->d_Ex + o * kBands; s.silence = e->d_sil + o; s.n_streams = e->S; s.n_frames = n;
+  s.Ex = e->d_Ex + o * kBands; s.silence = e->d_sil + o; s.n_streams = e->n_active; s.stride = e->S; s.n_frames = n;
   s.tab = e->d_tab; s.synth_mem = e->d_synth;
   s.out = d_out ? d_out + (size_t)h0 * kFrame : nullptr;
   s.out16 = d_out16 ? d_out16 + (size_t)h0 * kFrame : nullptr;
@@ -742,7 +749,7 @@ static int drain_engine_streams(pnb_engine *e) {  // host-side
 static int process_device_enqueue(pnb_engine *e, const float *d_in, const short *d_in16, size_t in_stride, float *d_out,
                                   short *d_out16, size_t out_stride, int F, float *d_gr, cudaStream_t st, const CallLink &lk,
                                   long long *n_out) {
-  const int S = e->S;
+  const int S = e->S, na = e->n_active;  // the call advances streams [0, na); per-call buffers keep the stride S
   long long n = 0;
   float *line = e->d_pcm + e->line_off;
   const bool tensor = (e->flags & PNB_NN_TENSOR) != 0;
@@ -798,7 +805,7 @@ static int process_device_enqueue(pnb_engine *e, const float *d_in, const short 
       {
         ProfScope ps(e, PNB_K_STAGE_IN, sd);
         n += launch_stage_in(line + (size_t)h0 * kFrame, e->pcm_stride, d_in ? d_in + (size_t)h0 * kFrame : nullptr,
-                             d_in16 ? d_in16 + (size_t)h0 * kFrame : nullptr, in_stride, S, nh * kFrame, sd);
+                             d_in16 ? d_in16 + (size_t)h0 * kFrame : nullptr, in_stride, na, nh * kFrame, sd);
       }
       { ProfScope ps(e, PNB_K_ANALYSIS, sd); n += launch_analysis(analysis_args(e, h0, nh), sd); }
       n += tc_fc(e, h0, nh, sd);  // CUDA-core work: with the DSP kernels
@@ -840,7 +847,7 @@ static int process_device_enqueue(pnb_engine *e, const float *d_in, const short 
     if (e->state_pending) CK(cudaStreamWaitEvent(st, e->ev_state, 0));
     { int rc = join_engine_streams(e, st); if (rc) return rc; }
     e->prev_start.clear();
-    { ProfScope ps(e, PNB_K_STAGE_IN, st); n += launch_stage_in(line, e->pcm_stride, d_in, d_in16, in_stride, S, F * kFrame, st); }
+    { ProfScope ps(e, PNB_K_STAGE_IN, st); n += launch_stage_in(line, e->pcm_stride, d_in, d_in16, in_stride, na, F * kFrame, st); }
     { ProfScope ps(e, PNB_K_ANALYSIS, st); n += launch_analysis(analysis_args(e, 0, F), st); }
     CK(cudaGetLastError());
     if (tensor) {
@@ -865,7 +872,9 @@ static int process_device_enqueue(pnb_engine *e, const float *d_in, const short 
     n += advance_line(e, F, st);
     if (lk.submitted && lk.done) CK(cudaEventRecord(lk.done, st));
   }
-  if (d_gr) CK(cudaMemcpyAsync(d_gr, e->d_gr, (size_t)F * S * 68 * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  if (d_gr)  // [F][na][68] from the [F][S][68] buffer
+    CK(cudaMemcpy2DAsync(d_gr, (size_t)na * 68 * sizeof(float), e->d_gr, (size_t)S * 68 * sizeof(float), (size_t)na * 68 * sizeof(float), F,
+                         cudaMemcpyDeviceToDevice, st));
   { int rc = mark_call_end(e, st); if (rc) return rc; }
   CK(cudaGetLastError());
   *n_out = n;
@@ -932,7 +941,7 @@ extern "C" int pnb_train_records_device(pnb_engine *e, const short *d_speech, si
     n += launch_stage_in(line + (size_t)N * e->pcm_stride, e->pcm_stride, nullptr, d_speech, speech_stride, N, F * kFrame, st, 1.f);
   }
   AnalysisArgs a;
-  a.pcm = line; a.pcm_stride = e->pcm_stride; a.n_streams = S; a.n_frames = F; a.tab = e->d_tab;
+  a.pcm = line; a.pcm_stride = e->pcm_stride; a.n_streams = S; a.stride = S; a.n_frames = F; a.tab = e->d_tab;
   a.feat = e->d_feat; a.zring = e->d_zring; a.ering = e->d_ering; a.ring = e->ring; a.hop0 = e->hop;
   a.P = nullptr; a.Ex = e->d_Ex; a.raw = e->d_raw; a.silence = e->d_sil;
   a.last_period = e->d_last_period; a.last_gain = e->d_last_gain;
@@ -1009,15 +1018,18 @@ static int process_host(pnb_engine *e, const T *in, size_t in_stride, T *out, si
   if (!*d_in_p) CK(cudaMalloc((void **)d_in_p, S * row * sizeof(T)));
   if (!*d_out_p) CK(cudaMalloc((void **)d_out_p, S * row * sizeof(T)));
   const size_t w = (size_t)F * kFrame * sizeof(T);
-  CK(cudaMemcpy2DAsync(*d_in_p, row * sizeof(T), in, in_stride * sizeof(T), w, S, cudaMemcpyHostToDevice, e->stream));
+  const size_t na = e->n_active;  // the rows of in / out / gr
+  CK(cudaMemcpy2DAsync(*d_in_p, row * sizeof(T), in, in_stride * sizeof(T), w, na, cudaMemcpyHostToDevice, e->stream));
   int rc;
   if (sizeof(T) == 4)
     rc = process_device(e, (const float *)*d_in_p, nullptr, row, (float *)*d_out_p, nullptr, row, F, nullptr, e->stream);
   else
     rc = process_device(e, nullptr, (const short *)*d_in_p, row, nullptr, (short *)*d_out_p, row, F, nullptr, e->stream);
   if (rc) return rc;
-  CK(cudaMemcpy2DAsync(out, out_stride * sizeof(T), *d_out_p, row * sizeof(T), w, S, cudaMemcpyDeviceToHost, e->stream));
-  if (gr) CK(cudaMemcpyAsync(gr, e->d_gr, (size_t)F * S * 68 * sizeof(float), cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaMemcpy2DAsync(out, out_stride * sizeof(T), *d_out_p, row * sizeof(T), w, na, cudaMemcpyDeviceToHost, e->stream));
+  if (gr)
+    CK(cudaMemcpy2DAsync(gr, na * 68 * sizeof(float), e->d_gr, S * 68 * sizeof(float), na * 68 * sizeof(float), F, cudaMemcpyDeviceToHost,
+                         e->stream));
   CK(cudaMemcpyAsync(e->h_status, e->d_status, 2 * sizeof(int), cudaMemcpyDeviceToHost, e->stream));
   CK(cudaStreamSynchronize(e->stream));
   return report_status(e);
@@ -1067,8 +1079,8 @@ static int submit_host(pnb_engine *e, const T *in, size_t in_stride, T *out, siz
   }
   const int k = (int)(e->submitted & 1);
   if (e->submitted >= 2) CK(cudaEventSynchronize(e->ev_out[k]));  // the slot's previous round trip is complete
-  const size_t w = (size_t)F * kFrame * sizeof(T);
-  CK(cudaMemcpy2DAsync(e->pipe_in[k], row * sizeof(T), in, in_stride * sizeof(T), w, S, cudaMemcpyHostToDevice, e->s_in));
+  const size_t w = (size_t)F * kFrame * sizeof(T), na = e->n_active;  // the rows of in / out
+  CK(cudaMemcpy2DAsync(e->pipe_in[k], row * sizeof(T), in, in_stride * sizeof(T), w, na, cudaMemcpyHostToDevice, e->s_in));
   CK(cudaEventRecord(e->ev_in[k], e->s_in));
   CallLink lk;  // starts when the copy has landed, not joined into any stream: the next call's analysis may overlap this call's tail
   lk.submitted = true; lk.ready = e->ev_in[k]; lk.done = e->ev_cmp[k];
@@ -1079,7 +1091,7 @@ static int submit_host(pnb_engine *e, const T *in, size_t in_stride, T *out, siz
     rc = process_device(e, nullptr, (const short *)e->pipe_in[k], row, nullptr, (short *)e->pipe_out[k], row, F, nullptr, e->stream, lk);
   if (rc) return rc;
   CK(cudaStreamWaitEvent(e->s_out, e->ev_cmp[k], 0));
-  CK(cudaMemcpy2DAsync(out, out_stride * sizeof(T), e->pipe_out[k], row * sizeof(T), w, S, cudaMemcpyDeviceToHost, e->s_out));
+  CK(cudaMemcpy2DAsync(out, out_stride * sizeof(T), e->pipe_out[k], row * sizeof(T), w, na, cudaMemcpyDeviceToHost, e->s_out));
   CK(cudaEventRecord(e->ev_out[k], e->s_out));
   e->submitted++;
   return PNB_OK;
@@ -1274,6 +1286,7 @@ static int state_batch(pnb_engine *e, int mode, const int *streams, int n, void 
   for (int i = 0; i < n; i++) {
     const int s = streams[i];
     if (s < 0 || s >= e->S) return fail(PNB_ERR_ARG, "streams[%d] = %d outside [0, %d)", i, s, e->S);
+    if (s >= e->n_active) return fail(PNB_ERR_ARG, "streams[%d] = %d outside the active range [0, %d)", i, s, e->n_active);
     if (seen[s]) return fail(PNB_ERR_ARG, "stream %d listed twice", s);
     seen[s] = 1;
   }
@@ -1293,9 +1306,29 @@ extern "C" int pnb_import_states(pnb_engine *e, const int *streams, int n, const
   return state_batch(e, kStateImport, streams, n, const_cast<void *>(d_blobs), blob_stride, cuda_stream);
 }
 
+// Active range: calls advance slots [0, n).  Growing it resets the entering slots like pnb_reset_streams (ordered like
+// any state operation); shrinking it enqueues nothing, the leaving slots' state is simply no longer kept.
+extern "C" int pnb_set_active_streams(pnb_engine *e, int n, void *cuda_stream) {
+  if (!e) return fail(PNB_ERR_ARG, "engine is NULL");
+  if (e->flags & PNB_TRAIN_DATA) return fail(PNB_ERR_ARG, "PNB_TRAIN_DATA engines always advance all their streams");
+  if (n < 1 || n > e->S) return fail(PNB_ERR_ARG, "active streams %d outside [1, %d]", n, e->S);
+  if (e->poisoned) return fail(PNB_ERR_ARG, "an earlier call failed while enqueuing work; the streams' state is undefined until pnb_reset");
+  if (n > e->n_active) {
+    std::vector<int> entering(n - e->n_active);
+    for (int i = 0; i < n - e->n_active; i++) entering[i] = e->n_active + i;
+    CK(cudaSetDevice(e->device));
+    const int rc = state_enqueue(e, kStateReset, entering.data(), (int)entering.size(), nullptr, 0, (cudaStream_t)cuda_stream);
+    if (rc) { e->poisoned = true; return rc; }
+  }
+  e->n_active = n;
+  return PNB_OK;
+}
+extern "C" int pnb_active_streams(const pnb_engine *e) { return e ? e->n_active : 0; }
+
 static int state_args(pnb_engine *e, int stream, const void *buf, size_t bytes) {
   if (!e || !buf) return fail(PNB_ERR_ARG, "NULL argument");
   if (stream < 0 || stream >= e->S) return fail(PNB_ERR_ARG, "stream %d outside [0, %d)", stream, e->S);
+  if (stream >= e->n_active) return fail(PNB_ERR_ARG, "stream %d outside the active range [0, %d)", stream, e->n_active);
   if (bytes < sizeof(StreamState)) return fail(PNB_ERR_ARG, "state buffer of %zu bytes, need pnb_state_size() = %zu", bytes, sizeof(StreamState));
   if (e->poisoned) return fail(PNB_ERR_CUDA, "engine state is undefined after a failed call; pnb_reset it");
   return PNB_OK;

@@ -11,6 +11,9 @@ struct pnb_tc_state;  // tensor-core path (pnb_nn_tc.cu)
 
 struct pnb_engine {
   int S = 0, Fmax = 0, device = 0, sm_count = 0;
+  // Active range (pnb_set_active_streams): a call advances slots [0, n_active) only.  Per-stream buffers keep the stride
+  // S (slot s of hop slot t at row t*S + s), so the active rows of every hop slot are a contiguous prefix.
+  int n_active = 0;
   unsigned flags = 0;
   cudaStream_t stream = nullptr;  // used by the host-buffer entry points
   pnb::Tables *d_tab = nullptr;

@@ -8,7 +8,8 @@ namespace pnb {
 struct AnalysisArgs {
   const float *pcm;        // [S][pcm_stride]: 5280 samples of history, then the call's hops
   size_t pcm_stride;
-  int n_streams, n_frames;
+  int n_streams, n_frames; // streams analysed: rows [0, n_streams)
+  int stride;              // S: rows per hop slot of the per-call buffers and the ring (>= n_streams)
   const Tables *tab;
   float *feat;             // [F][S][70]
   float2 *zring;           // [ring][S][400] spectra of the windowed blocks, slot = hop % ring (carried state)
@@ -33,7 +34,8 @@ struct SynthesisArgs {
   const float *gr;         // [F][S][68]
   const float *Ex;         // [F][S][34] (post-filter only)
   const unsigned char *silence;
-  int n_streams, n_frames;
+  int n_streams, n_frames; // streams synthesised: rows [0, n_streams)
+  int stride;              // S: rows per hop slot of the per-call buffers and the ring (>= n_streams)
   const Tables *tab;
   float *synth_mem;        // [S][480] carried state
   float *out;              // float output rows or null
@@ -79,7 +81,8 @@ int launch_slide_history(float *pcm, size_t pcm_stride, int n_streams, int n_sam
 // ---- network, fp32 FMA path (pnb_nn_f32.cu) ---------------------------------------------
 // One contraction  C[M x N] = epilogue( sum_seg A_seg[M x K_seg] * B_seg[K_seg x N] ).
 // A segments are activation matrices (row = stream), B segments are slices of the reference's
-// input-major weight arrays (row = input j, column = output i: W[j*ldb + i]).
+// input-major weight arrays (row = input j, column = output i: W[j*ldb + i]).  With an active range the rows are the
+// first M of each of n_slots hop slots.
 struct GemmSeg {
   const float *A;
   int lda;
@@ -90,7 +93,9 @@ struct GemmSeg {
 struct GemmArgs {
   GemmSeg seg[5];
   int n_seg;
-  int M, N;
+  int M, N;           // M: rows per hop slot (all n_slots x M rows when n_slots = 1 and the rows are one flat range)
+  int n_slots;        // hop slots; the rows of slot k start at row k * slot_stride of A and C
+  int slot_stride;
   float *C;
   int ldc;
   const float *bias;  // null -> raw sums
@@ -99,9 +104,10 @@ struct GemmArgs {
 };
 int launch_gemm_f32(const GemmArgs &g, cudaStream_t st);
 
-// fc: features [M x 70] -> [M x 128], relu (nnet.cpp:105 on the `fc` layer)
-int launch_fc_f32(const float *feat, const float *W, const float *bias, float *out, int M, int K, int N,
-                  cudaStream_t st);
+// fc: features [M x 70] -> [M x 128], relu (nnet.cpp:105 on the `fc` layer), on M rows of each of n_slots hop slots
+// slot_stride rows apart
+int launch_fc_f32(const float *feat, const float *W, const float *bias, float *out, int M, int K, int N, int n_slots,
+                  size_t slot_stride, cudaStream_t st);
 
 // The five GRUs of a chunk of hops in one persistent fp32 launch (pnb_nn_f32.cu).  Slot buffers: hop t of the chunk
 // reads state slot t and writes slot t+1; inputs are conv2's output slot t or the layer below's slot t+1.
@@ -117,14 +123,14 @@ struct F32ChainLayer {
 constexpr int kF32ChainMaxHops = 32;  // hops per launch of the fp32 chain (longer chunks amortise the ramp diagonals)
 struct F32ChainArgs {
   F32ChainLayer L[5];
-  int S, n_rb, n_units, n_lh;
+  int S, n, n_rb, n_units, n_lh;               // S: rows per slot; n: active streams [0, n); n_rb: their stream blocks
   unsigned char lh[5 * kF32ChainMaxHops];      // (hop << 3) | layer in anti-diagonal order
   int lh_unit0[5 * kF32ChainMaxHops + 1];      // first unit of every entry; [n_lh] = n_units
   unsigned *cnt;                               // [5][n_rb] finished tiles per (layer, stream block), zero at launch
   const float *tansig;
 };
 int launch_gru_chain_f32(const F32ChainArgs &a, int rows_per_thread, int sm_count, cudaStream_t st);
-struct F32CarrySeg { float4 *dst; const float4 *src; size_t slot4; int n_slots; };  // n_slots slots of slot4 float4s
+struct F32CarrySeg { float4 *dst; const float4 *src; size_t slot4, stride4; int n_slots; };  // first slot4 float4s of n_slots slots stride4 apart
 struct F32CarryArgs { F32CarrySeg seg[12]; int n_seg; unsigned *cnt; int n_cnt; };
 int launch_f32_carry(const F32CarryArgs &a, cudaStream_t st);
 

@@ -53,7 +53,10 @@ __global__ void __launch_bounds__(256) gemm_f32_kernel(GemmArgs g) {
   __shared__ __align__(16) float As[2][BK][BM + APAD];
   __shared__ __align__(16) float Bs[2][BK][BN];
   const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
-  const int m0 = blockIdx.y * BM, n0 = blockIdx.x * BN;
+  // row tiles per hop slot; rows [m_lim - M, m_lim) are the slot's (one flat range when n_slots = 1)
+  const int tiles_slot = (int)(gridDim.y / (unsigned)g.n_slots), slot = blockIdx.y / tiles_slot;
+  const int m0 = slot * g.slot_stride + (blockIdx.y - slot * tiles_slot) * BM, n0 = blockIdx.x * BN;
+  const int m_lim = slot * g.slot_stride + g.M;
 
   f32x2 acc[8][2];  // 8 rows x 2 pairs of columns
 #pragma unroll
@@ -71,9 +74,9 @@ __global__ void __launch_bounds__(256) gemm_f32_kernel(GemmArgs g) {
   auto fetch = [&](int sg, int k0) {
     const GemmSeg &S = g.seg[sg];
     int r0 = m0 + a_row, r1 = r0 + 64;
-    ra0 = r0 < g.M ? *reinterpret_cast<const float4 *>(S.A + (size_t)r0 * S.lda + k0 + a_kq)
+    ra0 = r0 < m_lim ? *reinterpret_cast<const float4 *>(S.A + (size_t)r0 * S.lda + k0 + a_kq)
                    : make_float4(0.f, 0.f, 0.f, 0.f);
-    ra1 = r1 < g.M ? *reinterpret_cast<const float4 *>(S.A + (size_t)r1 * S.lda + k0 + a_kq)
+    ra1 = r1 < m_lim ? *reinterpret_cast<const float4 *>(S.A + (size_t)r1 * S.lda + k0 + a_kq)
                    : make_float4(0.f, 0.f, 0.f, 0.f);
     const float *bp = S.B + (size_t)(k0 + b_k) * S.ldb + n0 + b_n;
     if (VEC_B) {
@@ -126,7 +129,7 @@ __global__ void __launch_bounds__(256) gemm_f32_kernel(GemmArgs g) {
 #pragma unroll
   for (int i = 0; i < 8; i++) {
     int r = m0 + ty * 8 + i;
-    if (r >= g.M) continue;
+    if (r >= m_lim) continue;
     const float2 p0 = unpack2(acc[i][0]), p1 = unpack2(acc[i][1]);
     const float accv[4] = {p0.x, p0.y, p1.x, p1.y};
 #pragma unroll
@@ -141,7 +144,7 @@ __global__ void __launch_bounds__(256) gemm_f32_kernel(GemmArgs g) {
 }
 
 int launch_gemm_f32(const GemmArgs &g, cudaStream_t st) {
-  dim3 grid((g.N + BN - 1) / BN, (g.M + BM - 1) / BM);
+  dim3 grid((g.N + BN - 1) / BN, g.n_slots * ((g.M + BM - 1) / BM));
   bool vec = true;
   for (int i = 0; i < g.n_seg; i++)
     if ((g.seg[i].ldb & 3) || (reinterpret_cast<uintptr_t>(g.seg[i].B) & 15)) vec = false;
@@ -154,9 +157,11 @@ int launch_gemm_f32(const GemmArgs &g, cudaStream_t st) {
 // weight row W[j*128 + i] is coalesced over i.
 __global__ void __launch_bounds__(128) fc_f32_kernel(const float *__restrict__ feat, const float *__restrict__ W,
                                                      const float *__restrict__ bias, float *__restrict__ out,
-                                                     int M, int K, int N) {
+                                                     int M, int K, int N, size_t slot_stride) {
   __shared__ float f[4][72];
   const int r0 = blockIdx.x * 4;
+  feat += blockIdx.y * slot_stride * K;  // hop slot blockIdx.y
+  out += blockIdx.y * slot_stride * N;
   for (int i = threadIdx.x; i < 4 * K; i += blockDim.x) {
     int rr = i / K, kk = i % K;
     f[rr][kk] = (r0 + rr < M) ? feat[(size_t)(r0 + rr) * K + kk] : 0.f;
@@ -177,9 +182,9 @@ __global__ void __launch_bounds__(128) fc_f32_kernel(const float *__restrict__ f
     if (r0 + rr < M) out[(size_t)(r0 + rr) * N + n] = a[rr] < 0.f ? 0.f : a[rr];
 }
 
-int launch_fc_f32(const float *feat, const float *W, const float *bias, float *out, int M, int K, int N,
-                  cudaStream_t st) {
-  fc_f32_kernel<<<(M + 3) / 4, 128, 0, st>>>(feat, W, bias, out, M, K, N);
+int launch_fc_f32(const float *feat, const float *W, const float *bias, float *out, int M, int K, int N, int n_slots,
+                  size_t slot_stride, cudaStream_t st) {
+  fc_f32_kernel<<<dim3((M + 3) / 4, n_slots), 128, 0, st>>>(feat, W, bias, out, M, K, N, slot_stride);
   return 1;
 }
 
@@ -309,7 +314,7 @@ __global__ void __launch_bounds__(CH_THREADS, RT == 8 ? 2 : 4) gru_chain_f32_ker
       constexpr int CPR = CH_BK / 4;
       for (int c = tid; c < BM * CPR; c += CH_THREADS) {
         const int r = c / CPR, q = c - r * CPR;
-        const bool ok = m0 + r < S;
+        const bool ok = m0 + r < args.n;
         cp_async16(&sm.A[st][r][q * 4], Ab + (size_t)(ok ? m0 + r : 0) * lda + k0 + q * 4, ok);
       }
       // B: CH_BK k-rows x 3 gates x 8 chunks
@@ -352,7 +357,7 @@ __global__ void __launch_bounds__(CH_THREADS, RT == 8 ? 2 : 4) gru_chain_f32_ker
 #pragma unroll
       for (int i = 0; i < RT; i++) {
         const int m = m0 + ty + 16 * i;
-        if (m >= S) continue;
+        if (m >= args.n) continue;
         const float2 ho = __ldcg(reinterpret_cast<const float2 *>(h_old + (size_t)m * H + j));
         const float2 sz = unpack2(az[i]), sr = unpack2(ar[i]), snx = unpack2(anx[i]), snh = unpack2(anh[i]);
         float out[2];
@@ -378,14 +383,15 @@ __global__ void __launch_bounds__(CH_THREADS, RT == 8 ? 2 : 4) gru_chain_f32_ker
   }
 }
 
-// End of a chunk of n hops: the last 4 fc / 2 conv1 slots and the last state slot move to the front, conv2's output of
-// the last hop is kept for the tap, the chain's counters return to zero.  A thread owns the same element of every slot.
+// End of a chunk of n hops: the last 4 fc / 2 conv1 slots and the last state slot move to the front (the active rows
+// of each), conv2's output of the last hop is kept for the tap, the chain's counters return to zero.  A thread owns the
+// same element of every slot.
 __global__ void f32_carry_kernel(F32CarryArgs a) {
   const size_t tid = (size_t)blockIdx.x * blockDim.x + threadIdx.x, stride = (size_t)gridDim.x * blockDim.x;
   for (int sg = 0; sg < a.n_seg; sg++) {
     const F32CarrySeg &g = a.seg[sg];
     for (size_t i = tid; i < g.slot4; i += stride)
-      for (int q = 0; q < g.n_slots; q++) g.dst[(size_t)q * g.slot4 + i] = g.src[(size_t)q * g.slot4 + i];
+      for (int q = 0; q < g.n_slots; q++) g.dst[(size_t)q * g.stride4 + i] = g.src[(size_t)q * g.stride4 + i];
   }
   for (size_t i = tid; i < (size_t)a.n_cnt; i += stride) a.cnt[i] = 0u;
 }

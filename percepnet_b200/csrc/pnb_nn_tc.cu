@@ -379,8 +379,10 @@ struct TcArgs {
   CUtensorMap maps[8];
   TcSeg seg[5];
   int n_seg;
-  int M;                // rows
-  int tiles_m, tiles_n; // tile grid; a CTA walks tiles blockIdx.x, blockIdx.x + gridDim.x, ...
+  int M;                // rows per hop slot: rows [k slot_stride, k slot_stride + M) of slot k (one slot: a flat range)
+  int slot_stride;      // row distance between hop slots (unused with one slot)
+  int tiles_slot;       // row tiles per hop slot: tiles never straddle two slots
+  int tiles_m, tiles_n; // tile grid (tiles_m = slots x tiles_slot); a CTA walks tiles blockIdx.x, blockIdx.x + gridDim.x, ...
   int b_term_rows;      // row distance between the split terms inside a packed weight matrix
   float out_scale;      // 2^-(activation scale + weight scale)
   const float *tansig;  // 201-entry table (global)
@@ -399,13 +401,21 @@ struct TcArgs {
   int out_plane_rows;   // rows per term plane of out_h / out_b
 };
 
+// First row of row tile mt, and the end of its hop slot's rows in *lim
+__device__ __forceinline__ int dense_tile_row0(const TcArgs &args, int mt, int *lim) {
+  const int slot = mt / args.tiles_slot;
+  *lim = slot * args.slot_stride + args.M;
+  return slot * args.slot_stride + (mt - slot * args.tiles_slot) * TM;
+}
+
 // ===== TMA producer (one thread): the tile's A rows and B rows, one pass over K per product order =====
 template <int BN, int NT, int STAGES>
 __device__ __forceinline__ void dense_producer(const TcArgs &args, const SmemCarve &c, uint32_t stage0, int total_tiles) {
   using SL = StageLayout<BN, NT>;
   Pipe p;
   for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-    const int n_tile = tile % args.tiles_n, m0 = (tile / args.tiles_n) * TM;
+    int lim;
+    const int n_tile = tile % args.tiles_n, m0 = dense_tile_row0(args, tile / args.tiles_n, &lim);
     // one pass over K per product order (see mma_kblock); with q passes still to go after this one, the pass needs
     // the first q + 1 terms of either operand
     for (int pass = 0; pass < NT; pass++) {
@@ -447,7 +457,8 @@ __device__ __forceinline__ void dense_consumer(const TcArgs &args, const SmemCar
   Pipe p;
   Consumer<R> cons;
   for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-    const int n_tile = tile % args.tiles_n, m0 = (tile / args.tiles_n) * TM;
+    int lim;  // rows from lim on (padding up to the tile's end) are computed but neither stored nor checked
+    const int n_tile = tile % args.tiles_n, m0 = dense_tile_row0(args, tile / args.tiles_n, &lim);
     float acc[R];
 #pragma unroll
     for (int i = 0; i < R; i++) acc[i] = 0.f;
@@ -470,7 +481,7 @@ __device__ __forceinline__ void dense_consumer(const TcArgs &args, const SmemCar
 #pragma unroll
     for (int h = 0; h < 2; h++) {  // the thread's two rows of the fragment
       const int row = m0 + wg * 64 + warp * 16 + (lane >> 2) + 8 * h;
-      if (row >= args.M) continue;
+      if (row >= lim) continue;
       const size_t orow = (size_t)args.out_row0 + row;
 #pragma unroll
       for (int j = 0; j < BN / 8; j++) {
@@ -551,9 +562,10 @@ struct ChainLayer {
 struct ChainArgs {
   CUtensorMap maps[16];  // 0: conv2 out, 1..5: state slots of the five GRUs, 6..10: input weights, 11..15: recurrent weights
   ChainLayer L[5];
-  int S, F;              // streams; hops this launch covers
+  int S, F;              // rows per hop slot of the buffers; hops this launch covers
+  int n;                 // active streams: rows [0, n) of every slot
   int t0;                // first hop of this launch inside the call (slot / counter arithmetic is per call)
-  int tiles_mp;          // row tiles (128 streams each)
+  int tiles_mp;          // row tiles of the active streams (128 streams each)
   int units_per_hop;
   int diag;              // unit order: 0 = hop-major (layer by layer inside a hop), 1 = anti-diagonals (few streams)
   unsigned *cnt;         // [5][tiles_mp] consumer-warp completions, zero at launch
@@ -788,7 +800,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) gru_chain_kernel(const __grid_c
 #pragma unroll
       for (int h = 0; h < 2; h++) {  // the thread's two rows of the fragment
         const int row = un.mp * TM + cw * 64 + warp * 16 + (lane >> 2) + 8 * h;
-        if (row >= S) continue;
+        if (row >= args.n) continue;
         const float *h_old = L.h32[pold] + (size_t)row * H;
         float *h_new = L.h32[pold ^ 1] + (size_t)row * H;
         __half *ph = L.h_hl + ((size_t)(un.t + 1) * S + row) * H;
@@ -833,13 +845,16 @@ constexpr int kConvTerms = 3;
 // fc 70 -> 128 relu in fp32 FMA (0.1 % of the MACs; K = 70 is no tensor-core shape), emitting the three bf16
 // terms conv1 consumes.  One block per 16 rows, one thread per output: the 16 feature rows sit in shared memory and are
 // read four k at a time (one broadcast 128-bit load per row and four FMAs), the weight column comes through L1.
-// Every output is bias + sum over ascending k, one fmaf per term, like the fp32 path's fc kernel.
+// Every output is bias + sum over ascending k, one fmaf per term, like the fp32 path's fc kernel.  grid.y walks hop slots
+// of M rows each, slot_stride rows apart (one slot: M is all rows of the call's hops).
 constexpr int FC_ROWS = 16;
 __global__ void __launch_bounds__(128) fc_split_kernel(const float *__restrict__ feat, const float *__restrict__ W,
                                                        const float *__restrict__ bias, __nv_bfloat16 *__restrict__ out,
-                                                       int M, size_t plane_rows) {
+                                                       int M, size_t plane_rows, size_t slot_stride) {
   __shared__ __align__(16) float f[FC_ROWS][72];
   const int r0 = blockIdx.x * FC_ROWS;
+  feat += blockIdx.y * slot_stride * 70;  // hop slot blockIdx.y: M rows of it
+  out += blockIdx.y * slot_stride * 128;
   for (int i = threadIdx.x; i < FC_ROWS * 72; i += blockDim.x) {
     const int rr = i / 72, kk = i - rr * 72;
     f[rr][kk] = (kk < 70 && r0 + rr < M) ? feat[(size_t)(r0 + rr) * 70 + kk] : 0.f;
@@ -886,11 +901,12 @@ __global__ void __launch_bounds__(128) fc_split_kernel(const float *__restrict__
 }
 
 // End-of-call bookkeeping in one launch: the hop slots the next call reads first (last 4 fc / 2 conv1 outputs,
-// last GRU states) move to the front of their buffers, and the chain's dependency counters return to zero.
+// last GRU states) move to the front of their buffers, and the chain's dependency counters return to zero.  Only the
+// active streams' rows move: they are the first rows of every slot.
 // A segment shifts `n_slots` slots down by `shift` slots.  One thread owns the same element of every slot and walks
 // the slots in ascending order, so a slot that is both source and destination (shift < n_slots) is read before it is
 // overwritten -- by the same thread, no cross-thread ordering needed.
-struct CarrySeg { uint4 *base; size_t slot16; int n_slots, shift; };
+struct CarrySeg { uint4 *base; size_t slot16, stride16; int n_slots, shift; };  // the first slot16 of each stride16
 struct CarryArgs {
   CarrySeg seg[16];
   int n_seg;
@@ -902,7 +918,7 @@ __global__ void __launch_bounds__(256) tc_carry_kernel(const __grid_constant__ C
   for (int s = 0; s < a.n_seg; s++) {
     const CarrySeg sg = a.seg[s];
     for (size_t i = tid; i < sg.slot16; i += nth)
-      for (int k = 0; k < sg.n_slots; k++) sg.base[(size_t)k * sg.slot16 + i] = sg.base[(size_t)(k + sg.shift) * sg.slot16 + i];
+      for (int k = 0; k < sg.n_slots; k++) sg.base[(size_t)k * sg.stride16 + i] = sg.base[(size_t)(k + sg.shift) * sg.stride16 + i];
   }
   for (size_t i = tid; i < (size_t)a.n_cnt; i += nth) a.cnt[i] = 0u;
 }
@@ -1246,10 +1262,16 @@ static int tc_launch(pnb_engine *e, K kernel, const A &a, int units, size_t smem
   TCK(cudaGetLastError());
   return PNB_OK;
 }
+// A dense layer over the active rows of `slots` hop slots.  With every stream active the rows are one flat range of
+// slots x S; otherwise each slot has its own ceil(n / 128) row tiles.
 template <int BN, bool BF16, int ST2, int ST3>
-static int tc_launch_dense(pnb_engine *e, TcArgs &a, int rows, int tiles_n, cudaStream_t st) {
-  a.M = rows;
-  a.tiles_m = (rows + TM - 1) / TM;
+static int tc_launch_dense(pnb_engine *e, TcArgs &a, int slots, int tiles_n, cudaStream_t st) {
+  const int n = e->n_active;
+  if (n == e->S) {
+    a.M = slots * n; a.slot_stride = 0; a.tiles_slot = (a.M + TM - 1) / TM; a.tiles_m = a.tiles_slot;
+  } else {
+    a.M = n; a.slot_stride = e->S; a.tiles_slot = (n + TM - 1) / TM; a.tiles_m = slots * a.tiles_slot;
+  }
   a.tiles_n = tiles_n;
   a.status = e->d_status;
   return tc_launch(e, tc_gemm_kernel<BN, BF16, ST2, ST3>, a, a.tiles_m * a.tiles_n, dense_smem_bytes<BN, ST2, ST3>(), st);
@@ -1269,17 +1291,17 @@ static TcSeg mkseg(int a_map, int b_map, int K, int a_k0, int b_k0, int a_row0, 
 int tc_fc(pnb_engine *e, int h0, int n, cudaStream_t st) {
   // fc (fp32 FMA on the CUDA cores: it runs with the DSP kernels when the schedule is split) -> bf16 terms at slots 4 + h0 ..
   pnb_tc_state *t = e->tc;
-  const int S = e->S, Fm = e->Fmax, rows = n * S;
+  const int S = e->S, Fm = e->Fmax, na = e->n_active;
+  const int rows = na == S ? n * S : na, slots = na == S ? 1 : n;  // per grid.y slot
   ProfScope ps(e, PNB_K_TC_AUX, st);
-  fc_split_kernel<<<(rows + FC_ROWS - 1) / FC_ROWS, 128, 0, st>>>(e->d_feat + (size_t)h0 * S * kFeat, e->fc.W, e->fc.b,
-                                                  t->fc_all + (size_t)(4 + h0) * S * 128, rows, (size_t)(Fm + 4) * S);
+  fc_split_kernel<<<dim3((rows + FC_ROWS - 1) / FC_ROWS, slots), 128, 0, st>>>(e->d_feat + (size_t)h0 * S * kFeat, e->fc.W, e->fc.b,
+                                                  t->fc_all + (size_t)(4 + h0) * S * 128, rows, (size_t)(Fm + 4) * S, (size_t)S);
   return 1;
 }
 int tc_front(pnb_engine *e, int h0, int n, int F, cudaStream_t st) {
   pnb_tc_state *t = e->tc;
   const int S = e->S, Fm = e->Fmax;
   const float *tbl = e->tansig();
-  const int rows = n * S;
   int nl = 0, rc;
   TcArgs a;
   // conv1: tap q of hop t reads fc slot t + q (oldest first, nnet.cpp:182-200); output -> c1 slots 2 + t
@@ -1292,7 +1314,7 @@ int tc_front(pnb_engine *e, int h0, int n, int F, cudaStream_t st) {
   a.out_b = t->c1_all; a.out_row0 = (2 + h0) * S; a.out_plane_rows = (Fm + 2) * S; a.out_terms = kConvTerms; a.wide = t->wide;
   {
     ProfScope ps(e, PNB_K_TC_GEMM, st);
-    if ((rc = tc_launch_dense<DENSE_BN, true, DENSE_STAGES, DENSE_STAGES3>(e, a, rows, 512 / DENSE_BN, st))) return rc;
+    if ((rc = tc_launch_dense<DENSE_BN, true, DENSE_STAGES, DENSE_STAGES3>(e, a, n, 512 / DENSE_BN, st))) return rc;
     nl++;
   }
   // conv2: three taps -> tanh -> fp16 terms (gru1 / gru_rb / fc_gb inputs); fp32 copy of the call's last hop
@@ -1306,7 +1328,7 @@ int tc_front(pnb_engine *e, int h0, int n, int F, cudaStream_t st) {
   a.out_h = t->c2_h; a.out_row0 = h0 * S; a.out_plane_rows = Fm * S; a.wide = t->wide;
   {
     ProfScope ps(e, PNB_K_TC_GEMM, st);
-    if ((rc = tc_launch_dense<DENSE_BN, true, DENSE_STAGES, DENSE_STAGES3>(e, a, rows, 512 / DENSE_BN, st))) return rc;
+    if ((rc = tc_launch_dense<DENSE_BN, true, DENSE_STAGES, DENSE_STAGES3>(e, a, n, 512 / DENSE_BN, st))) return rc;
     nl++;
   }
   return nl;
@@ -1321,7 +1343,8 @@ int tc_gru_chain(pnb_engine *e, int h0, int n, cudaStream_t st) {
   memset(&a, 0, sizeof a);
   a.maps[0] = t->m_c2_ch;
   for (int i = 0; i < 5; i++) { a.maps[1 + i] = t->m_h_ch[i]; a.maps[6 + i] = t->m_w[i]; a.maps[11 + i] = t->m_u[i]; }
-  a.S = S; a.F = n; a.t0 = h0; a.tiles_mp = t->tiles_mp; a.cnt = t->cnt; a.tansig = e->tansig();
+  // only the active streams' row tiles are units; the counters of the others stay zero
+  a.S = S; a.n = e->n_active; a.F = n; a.t0 = h0; a.tiles_mp = (e->n_active + TM - 1) / TM; a.cnt = t->cnt; a.tansig = e->tansig();
   const int c2_terms = Fm * S, h_terms = (Fm + 1) * S;
   int unit0 = 0;
   for (int li = 0; li < 5; li++) {
@@ -1330,7 +1353,7 @@ int tc_gru_chain(pnb_engine *e, int h0, int n, cudaStream_t st) {
     L.H = H; L.h_kb = H / CBK; L.tiles_log2 = __builtin_ctz(tiles);
     L.b_term_rows = tiles * GRU_BN;
     L.h_map = 1 + li; L.w_map = 6 + li; L.u_map = 11 + li;
-    L.unit0 = unit0; unit0 += t->tiles_mp * tiles;
+    L.unit0 = unit0; unit0 += a.tiles_mp * tiles;
     L.par0 = e->par[li];
     L.scale = t->scale_gru[li];
     L.bias4 = t->bias4[li];
@@ -1351,7 +1374,7 @@ int tc_gru_chain(pnb_engine *e, int h0, int n, cudaStream_t st) {
   a.units_per_hop = unit0;
   // with many streams one layer-hop fills the machine and hop-major order keeps a layer's fresh output in L2 for the
   // layer above; with few, only the anti-diagonal order exposes enough independent units
-  a.diag = (t->tiles_mp * (512 / HT) < e->tc_sms) ? 1 : 0;
+  a.diag = (a.tiles_mp * (512 / HT) < e->tc_sms) ? 1 : 0;
   {
     ProfScope ps(e, PNB_K_TC_GEMM, st);
     int rc = tc_launch(e, gru_chain_kernel, a, n * unit0, tc_smem_bytes<GRU_STAGES, GRU_STAGES * GruStage::kBytes>(), st);
@@ -1365,7 +1388,7 @@ int tc_out(pnb_engine *e, int h0, int n, cudaStream_t st) {
   pnb_tc_state *t = e->tc;
   const int S = e->S, Fm = e->Fmax;
   const float *tbl = e->tansig();
-  const int rows = n * S, h_terms = (Fm + 1) * S;
+  const int h_terms = (Fm + 1) * S;
   int nl = 0, rc;
   TcArgs a;
   memset(&a, 0, sizeof a);
@@ -1378,7 +1401,7 @@ int tc_out(pnb_engine *e, int h0, int n, cudaStream_t st) {
   a.bias = t->bias_pad + 1024; a.act = PNB_ACT_SIGMOID; a.N = 34; a.ldc = 68; a.out_f32 = e->d_gr + (size_t)h0 * S * 68;
   {
     ProfScope ps(e, PNB_K_TC_GEMM, st);
-    if ((rc = tc_launch_dense<SMALL_BN, false, SMALL_STAGES, 0>(e, a, rows, 1, st))) return rc;
+    if ((rc = tc_launch_dense<SMALL_BN, false, SMALL_STAGES, 0>(e, a, n, 1, st))) return rc;
     nl++;
   }
   memset(&a, 0, sizeof a);
@@ -1389,7 +1412,7 @@ int tc_out(pnb_engine *e, int h0, int n, cudaStream_t st) {
   a.bias = t->bias_pad + 1072; a.act = PNB_ACT_SIGMOID; a.N = 34; a.ldc = 68; a.out_f32 = e->d_gr + (size_t)h0 * S * 68 + 34;
   {
     ProfScope ps(e, PNB_K_TC_GEMM, st);
-    if ((rc = tc_launch_dense<SMALL_BN, false, SMALL_STAGES, 0>(e, a, rows, 1, st))) return rc;
+    if ((rc = tc_launch_dense<SMALL_BN, false, SMALL_STAGES, 0>(e, a, n, 1, st))) return rc;
     nl++;
   }
   return nl;
@@ -1399,7 +1422,7 @@ int tc_out(pnb_engine *e, int h0, int n, cudaStream_t st) {
 // dependency counters return to zero (one launch), and the fp32 state parity advances by F.
 int tc_carry(pnb_engine *e, int F, cudaStream_t st) {
   pnb_tc_state *t = e->tc;
-  const int S = e->S, Fm = e->Fmax;
+  const int S = e->S, Fm = e->Fmax, na = e->n_active;
   const int h_terms = (Fm + 1) * S;
   CarryArgs ca;
   memset(&ca, 0, sizeof ca);
@@ -1408,14 +1431,14 @@ int tc_carry(pnb_engine *e, int F, cudaStream_t st) {
   for (int tm = 0; tm < kConvTerms; tm++) {
     __nv_bfloat16 *bf = t->fc_all + (size_t)tm * (Fm + 4) * S * 128;
     __nv_bfloat16 *bc = t->c1_all + (size_t)tm * (Fm + 2) * S * 512;
-    ca.seg[ns++] = CarrySeg{reinterpret_cast<uint4 *>(bf), (size_t)S * 128 * 2 / 16, 4, F};
-    ca.seg[ns++] = CarrySeg{reinterpret_cast<uint4 *>(bc), (size_t)S * 512 * 2 / 16, 2, F};
+    ca.seg[ns++] = CarrySeg{reinterpret_cast<uint4 *>(bf), (size_t)na * 128 * 2 / 16, (size_t)S * 128 * 2 / 16, 4, F};
+    ca.seg[ns++] = CarrySeg{reinterpret_cast<uint4 *>(bc), (size_t)na * 512 * 2 / 16, (size_t)S * 512 * 2 / 16, 2, F};
   }
   for (int li = 0; li < 5; li++) {
     const size_t H = e->gru[li].H;
     for (int tm = 0; tm < 2; tm++) {
       __half *base = t->h_all[li] + (size_t)tm * h_terms * H;
-      ca.seg[ns++] = CarrySeg{reinterpret_cast<uint4 *>(base), (size_t)S * H * 2 / 16, 1, F};
+      ca.seg[ns++] = CarrySeg{reinterpret_cast<uint4 *>(base), (size_t)na * H * 2 / 16, (size_t)S * H * 2 / 16, 1, F};
     }
   }
   ca.n_seg = ns;

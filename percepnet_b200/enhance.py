@@ -11,7 +11,9 @@ stores the per-frame g[34], r[34] the reference dumps to feature_test.raw (denoi
 
 Weights come from a binary weight file (percepnet_b200.weights.PackedModel.save_blob; INTEGRATION.md 3) -- the
 reference binary has them compiled in.  ``--seed N`` uses the synthetic random-init model instead (tests, benches).
-All files of a list run as independent streams of one engine, padded to the longest file of their batch.
+All files of a list run as independent streams of one engine.  Within a batch the files are sorted longest first, and
+each call advances only the files that still have frames (the engine's active range), so the padding behind a file
+that has ended is not processed.
 There is no CPU path: without the CUDA library / a GPU this exits with an error.
 """
 from __future__ import annotations
@@ -41,16 +43,19 @@ def run_jobs(jobs, model, nn: str = "tensor", batch: int = 4096, chunk: int = 10
         for row, k in enumerate(group):
             x[row, :nfr[row] * FRAME] = np.fromfile(jobs[k][0], dtype="<i2", count=nfr[row] * FRAME)
         eng = api.Engine(S, min(chunk, Fmax), model, flags, device=device)
-        outs, grs = [], []
         want_gr = gr_paths is not None and any(gr_paths[k] for k in group)
+        out = np.zeros_like(x)
+        gr = np.zeros((Fmax, S, 68), np.float32) if want_gr else None              # [F, S, 68]
         for t0 in range(0, Fmax, chunk):
             t1 = min(Fmax, t0 + chunk)
-            o, g = eng.process(np.ascontiguousarray(x[:, t0 * FRAME:t1 * FRAME]), want_gr=want_gr)
-            outs.append(o)
-            grs.append(g)
+            n = sum(1 for f in nfr if f > t0)   # rows [0, n): the files (longest first) that still have frames
+            if n != eng.active:
+                eng.set_active(n)               # only shrinks: the files that left have ended
+            o, g = eng.process(np.ascontiguousarray(x[:n, t0 * FRAME:t1 * FRAME]), want_gr=want_gr)
+            out[:n, t0 * FRAME:t1 * FRAME] = o
+            if want_gr:
+                gr[t0:t1, :n] = g
         eng.close()
-        out = np.concatenate(outs, axis=1)
-        gr = np.concatenate(grs, axis=0) if want_gr else None                       # [F, S, 68]
         for row, k in enumerate(group):
             n = nfr[row]
             out[row, FRAME:n * FRAME].astype("<i2").tofile(jobs[k][1])            # first frame dropped, main.cpp:37-38

@@ -1,11 +1,13 @@
 #!/usr/bin/env python
-"""Session churn in a running engine: stream states moved per second by pnb_export_states + pnb_import_states, and
-serving throughput while slots are reset or moved between calls.  One JSON line, in the style of bench.py's paths.
+"""Session churn in a running engine: stream states moved per second by pnb_export_states + pnb_import_states,
+serving throughput while slots are reset or moved between calls, and serving throughput at partial occupancy (the
+engine's active range, pnb_set_active_streams).  One JSON line, in the style of bench.py's paths.
 
   python tools/bench_churn.py [--streams S] [--frames F] [--steps K] [--warmup W] [--nn tensor|fp32] [--churn 0.01]
+                              [--active 0.25,0.5,0.75,1.0]
 
 Defaults: 16 384 streams on the tensor path, calls of 10 hops (a 100 ms serving cadence), 1 % of the slots churned
-before every call.  The card's name and power limit are read in the same run.  The inputs, clock sampling and peak
+before every call, occupancy sweep over a quarter, half, three quarters and all of the slots.  The card's name and power limit are read in the same run.  The inputs, clock sampling and peak
 figures are bench.py's own (imported, not changed).
 """
 from __future__ import annotations
@@ -163,7 +165,52 @@ def run_churn(args):
             torch.cuda.synchronize()
             fps[kind].append(S * F * K / (evs[0].elapsed_time(evs[1]) * 1e-3))
     eng.check(st)
+
+    # ---- occupancy: calls advance only the first n = fraction x S slots; fractions alternated over three runs
+    fracs = [float(f) for f in args.active.split(",") if f.strip()]
+    occ = {f: {"n": max(1, min(S, int(round(f * S)))), "fps": [], "ms": []} for f in fracs}
+    for _ in range(3):
+        for f in fracs:
+            n = occ[f]["n"]
+            eng.set_active(n, stream=st)                   # a grow resets the entering slots (not timed)
+            for _ in range(2):
+                call(i)
+                i += 1
+            eng.flush(st)
+            evs[0].record(stream)
+            for _ in range(K):
+                call(i)
+                i += 1
+            eng.flush(st)
+            evs[1].record(stream)
+            torch.cuda.synchronize()
+            ms = evs[0].elapsed_time(evs[1])
+            occ[f]["fps"].append(n * F * K / (ms * 1e-3))
+            occ[f]["ms"].append(ms / K)
+    for f in fracs:                                        # per-class kernel time of one profiled call
+        eng.set_active(occ[f]["n"], stream=st)
+        call(i)
+        i += 1
+        eng.flush(st)
+        torch.cuda.synchronize()
+        eng.profile(True)
+        call(i)
+        i += 1
+        eng.flush(st)
+        occ[f]["kernel_ms"] = {k: round(v[0], 4) for k, v in eng.profile_read().items()}
+        eng.profile(False)
+    eng.check(st)
     eng.close()
+    full_ms = float(np.median(occ[max(fracs)]["ms"]))
+    occupancy = {"runs_per_fraction": 3, "calls_per_run": K, "note": (
+        "frames/s of live streams (n x hops / s) and ms per call of back-to-back pnb_submit_device_f32 calls after "
+        "pnb_set_active_streams(n); fractions alternated in one process, median of three runs; kernel_ms: per-class "
+        "device time of one profiled call (pnb_profile_read); ms_vs_largest: ms per call relative to the largest fraction")}
+    for f in fracs:
+        o = occ[f]
+        ms = float(np.median(o["ms"]))
+        occupancy[f"{f:g}"] = {"active": o["n"], "fps": float(np.median(o["fps"])), "fps_runs": [round(x) for x in o["fps"]],
+                               "ms_per_call": ms, "ms_vs_largest": ms / full_ms, "kernel_ms": o["kernel_ms"]}
     serving = {k: {"value": float(np.median(v)), "runs": [round(x) for x in v]} for k, v in fps.items()}
     serving["calls_per_run"] = K
     serving["churn"] = args.churn
@@ -177,7 +224,7 @@ def run_churn(args):
         "config": {"workload": f"export + import of all {S} streams per repetition ({nn_mode} engine, {F}-hop calls)",
                    "streams": S, "frames_per_call": F, "nn": nn_mode, "schedule": ov,
                    "repetitions": reps, "export_ms": exp_ms / reps, "import_ms": imp_ms / reps},
-        "card": card, "clocks": clocks, "roofline": roof, "serving": serving}))
+        "card": card, "clocks": clocks, "roofline": roof, "serving": serving, "occupancy": occupancy}))
     return 0
 
 
@@ -189,6 +236,7 @@ def main():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--nn", default="tensor", choices=["tensor", "fp32"])
     ap.add_argument("--churn", type=float, default=0.01, help="fraction of the slots reset / moved before every call")
+    ap.add_argument("--active", default="0.25,0.5,0.75,1.0", help="occupancy sweep: fractions of the slots the calls advance")
     return run_churn(ap.parse_args())
 
 

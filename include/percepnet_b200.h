@@ -110,24 +110,26 @@ int pnb_process_host_i16(pnb_engine *e, const short *in, size_t in_stride, short
  * until pnb_wait() returns.  Calls are processed in submission order (the streams' state advances in order). */
 int pnb_submit_host_f32(pnb_engine *e, const float *in, size_t in_stride, float *out, size_t out_stride, int n_frames);
 int pnb_submit_host_i16(pnb_engine *e, const short *in, size_t in_stride, short *out, size_t out_stride, int n_frames);
+/* Waits on the host for every call and state operation issued on the engine, on any stream, then reports the engine's
+ * status: PNB_OK, PNB_ERR_DOMAIN, or PNB_ERR_CUDA -- or, once, PNB_ERR_ARG when pnb_import_states rejected a blob since
+ * the last report. */
 int pnb_wait(pnb_engine *e);
-/* Waits for everything enqueued on the engine's internal streams and on `cuda_stream` (the stream the caller passed to
- * pnb_process_device_*), then reports the engine's status: PNB_OK, PNB_ERR_DOMAIN, or PNB_ERR_CUDA -- or, once,
- * PNB_ERR_ARG when pnb_import_states rejected a blob since the last report.  pnb_wait also waits for the last
- * pnb_reset_streams / pnb_export_states / pnb_import_states, whichever stream it was issued on. */
+/* pnb_wait, after everything enqueued on `cuda_stream` so far has run. */
 int pnb_check(pnb_engine *e, void *cuda_stream);
 
 /* Device buffers on the engine's device; asynchronous on cuda_stream (a cudaStream_t, NULL = default
- * stream).  in/out hold the active rows as above; d_gr (NULL ok) as above, in device memory. */
+ * stream).  in/out hold the active rows as above; d_gr (NULL ok) as above, in device memory.
+ * Order: the calls and state operations of one engine run in the order they are issued, on whatever streams they are
+ * issued on.  A call starts after everything enqueued on its cuda_stream before it and after the engine's previous call
+ * or state operation; d_out (and d_gr) are complete in cuda_stream's order behind it. */
 int pnb_process_device_f32(pnb_engine *e, const float *d_in, size_t in_stride, float *d_out, size_t out_stride,
                            int n_frames, float *d_gr, void *cuda_stream);
 int pnb_process_device_i16(pnb_engine *e, const short *d_in, size_t in_stride, short *d_out, size_t out_stride,
                            int n_frames, float *d_gr, void *cuda_stream);
 
-/* Submitted twins of pnb_process_device_* (in/out: the active rows): the call starts when cuda_stream reaches this point (its inputs are ready in
- * that stream's order) but is NOT joined back into it, so a following call's analysis overlaps this call's network and
- * synthesis (the engine orders what they share).  d_out is complete once pnb_flush(e, stream) has made `stream` wait for
- * everything submitted so far, or after pnb_wait / pnb_check on the host.  Calls of one engine are issued in order. */
+/* pnb_process_device_* without d_gr.  pnb_flush(e, stream) makes `stream` wait for every call and state operation
+ * issued on the engine so far, on any stream: d_out is then complete in that stream's order, and on the host after
+ * pnb_wait / pnb_check. */
 int pnb_submit_device_f32(pnb_engine *e, const float *d_in, size_t in_stride, float *d_out, size_t out_stride,
                           int n_frames, void *cuda_stream);
 int pnb_submit_device_i16(pnb_engine *e, const short *d_in, size_t in_stride, short *d_out, size_t out_stride,
@@ -171,7 +173,7 @@ int pnb_set_state(pnb_engine *e, int stream, const void *src, size_t src_bytes);
  *                (pointer and stride multiples of 4 bytes); the bytes are those of pnb_get_state / pnb_set_state, so a
  *                blob may be copied to the host and set with pnb_set_state on any engine, and the reverse
  * Order: an operation runs after everything already enqueued on cuda_stream and after every call issued earlier on the
- * engine (plain or submitted, on any stream); every call issued later runs after it.
+ * engine, on any stream; every call issued later runs after it.
  *
  * pnb_reset_streams: the listed streams get the state of a stream in a freshly created engine (history, overlap-add and
  *   pitch memory, the live spectrum slots, conv histories and GRU states -- what pnb_reset clears, restricted to them).
@@ -246,7 +248,7 @@ enum {
 int pnb_profile_enable(pnb_engine *e, int on);
 int pnb_profile_read(pnb_engine *e, double *ms, long long *counts);
 /* The same records as a timeline: launch i of the profiled calls as (class, start ms, end ms) relative to the first
- * launch, in launch order (launches on different internal streams overlap).  Returns the count written (<= cap). */
+ * launch, in launch order.  Returns the count written (<= cap). */
 int pnb_profile_timeline(pnb_engine *e, int *cls, double *t0_ms, double *t1_ms, int cap);
 const char *pnb_kernel_class_name(int cls);
 
@@ -255,16 +257,6 @@ long long pnb_launch_count(const pnb_engine *e);
 /* Kernel launches one pnb_process_* call with n_frames hops issues (one more on the calls that also move the
  * streams' history back to the start of their rows, at most every call, typically every eighth). */
 int pnb_launches_per_call(const pnb_engine *e, int n_frames);
-
-/* How long calls are scheduled on this engine.  net_sms = 0 (the default): every call runs its kernels one after the
- * other on all SMs.  A PNB_NN_TENSOR engine created with PNB_OVERLAP=2 uses the chunked schedule instead: calls of at
- * least two chunks of `chunk_hops` hops run the network of chunk k on `net_sms` SMs while analysis of chunk k+1 and
- * synthesis of chunk k-1 run on the other `dsp_sms` SMs (two green contexts).  Environment (read by pnb_create):
- * PNB_OVERLAP=2 enables it, PNB_NET_SMS, PNB_CHUNK tune it.  Results do not depend on the schedule. */
-int pnb_overlap_info(const pnb_engine *e, int *net_sms, int *dsp_sms, int *chunk_hops);
-/* on = 0: run every call serially on all SMs (e.g. to time one kernel class alone); on = 1: back to the partition the
- * engine was created with.  Waits for the engine to be idle. */
-int pnb_set_overlap(pnb_engine *e, int on);
 int pnb_n_streams(const pnb_engine *e);
 int pnb_max_frames(const pnb_engine *e);
 const char *pnb_last_error(void);

@@ -77,8 +77,6 @@ def load_library() -> C.CDLL:
     L.pnb_launch_count.restype = C.c_longlong
     L.pnb_launches_per_call.argtypes = [vp, i]
     L.pnb_n_streams.argtypes = [vp]
-    L.pnb_overlap_info.argtypes = [vp, vp, vp, vp]
-    L.pnb_set_overlap.argtypes = [vp, i]
     L.pnb_max_frames.argtypes = [vp]
     L.pnb_profile_enable.argtypes = [vp, i]
     L.pnb_profile_read.argtypes = [vp, vp, vp]
@@ -95,7 +93,7 @@ EXPORTS = ("pnb_create", "pnb_destroy", "pnb_reset", "pnb_process_host_f32", "pn
            "pnb_model_load_blob", "pnb_model_load_stream", "pnb_model_free", "pnb_train_records_host", "pnb_train_records_device", "pnb_submit_train_records", "pnb_process_device_f32", "pnb_process_device_i16", "pnb_submit_host_f32", "pnb_submit_host_i16", "pnb_submit_device_f32", "pnb_submit_device_i16", "pnb_flush", "pnb_wait", "pnb_check",
            "pnb_read_tap", "pnb_state_size", "pnb_get_state", "pnb_set_state",
            "pnb_reset_streams", "pnb_export_states", "pnb_import_states", "pnb_set_active_streams", "pnb_active_streams", "pnb_pitch_only_device", "pnb_pitch_only_host", "pnb_launch_count",
-           "pnb_launches_per_call", "pnb_profile_enable", "pnb_profile_read", "pnb_profile_timeline", "pnb_kernel_class_name", "pnb_n_streams", "pnb_overlap_info", "pnb_set_overlap", "pnb_max_frames", "pnb_last_error", "pnb_version")
+           "pnb_launches_per_call", "pnb_profile_enable", "pnb_profile_read", "pnb_profile_timeline", "pnb_kernel_class_name", "pnb_n_streams", "pnb_max_frames", "pnb_last_error", "pnb_version")
 
 
 def pitch_only_device(d_buf: int, stride: int, n_units: int, d_period: int, d_corr: int, d_gain: int, d_lag: int = 0,
@@ -219,7 +217,7 @@ class Engine:
 
     def submit_device(self, d_in: int, in_stride: int, d_out: int, out_stride: int, n_frames: int, stream: int = 0,
                       int16: bool = False):
-        """pnb_submit_device_*: like process_device but not joined into `stream`; flush(stream) or wait() completes it."""
+        """pnb_submit_device_*: process_device without g/r; flush(other_stream) or wait() orders other work behind it."""
         f = self.L.pnb_submit_device_i16 if int16 else self.L.pnb_submit_device_f32
         self._ck(f(self.h, d_in, in_stride, d_out, out_stride, n_frames, stream or None), "pnb_submit_device")
 
@@ -346,13 +344,10 @@ class Engine:
             self._ck(n, "pnb_profile_timeline")
         return [(self.L.pnb_kernel_class_name(cls[k]).decode(), t0[k], t1[k]) for k in range(n)]
 
-    def set_overlap(self, on: bool):
-        self._ck(self.L.pnb_set_overlap(self.h, 1 if on else 0), "pnb_set_overlap")
-
     def overlap_info(self) -> dict:
-        a, b, c = C.c_int(), C.c_int(), C.c_int()
-        self._ck(self.L.pnb_overlap_info(self.h, C.byref(a), C.byref(b), C.byref(c)), "pnb_overlap_info")
-        return {"net_sms": a.value, "dsp_sms": b.value, "chunk_hops": c.value}
+        """Every call runs its kernels one after the other on all SMs; no SM partition exists.  Kept as this constant
+        because bench.py reports it as the schedule."""
+        return {"net_sms": 0, "dsp_sms": 0, "chunk_hops": 0}
 
     @property
     def launches(self) -> int:

@@ -5,7 +5,6 @@
 //   stage_in -> analysis (all F hops; one warp per stream) -> F x network step -> synthesis -> slide history
 // The network step is the only part that is sequential in time across the batch; analysis and synthesis
 // need no network state, so hops are processed F at a time.
-#include <cuda.h>
 #include <math.h>
 #include <stdarg.h>
 #include <stdio.h>
@@ -136,90 +135,6 @@ static int check_model(const pnb_model *m) {
   return PNB_OK;
 }
 
-constexpr int kMaxChunks = 512;  // chunks one call may be cut into (chunked overlap schedule)
-
-// ------------------------------------------------------------------------------------------
-// SM partition (driver green contexts, reached through the runtime's entry-point query: no libcuda link)
-// ------------------------------------------------------------------------------------------
-namespace {
-struct GreenApi {
-  CUresult (*DeviceGet)(CUdevice *, int) = nullptr;
-  CUresult (*DeviceGetDevResource)(CUdevice, CUdevResource *, CUdevResourceType) = nullptr;
-  CUresult (*DevSmResourceSplitByCount)(CUdevResource *, unsigned int *, const CUdevResource *, CUdevResource *, unsigned int, unsigned int) = nullptr;
-  CUresult (*DevResourceGenerateDesc)(CUdevResourceDesc *, CUdevResource *, unsigned int) = nullptr;
-  CUresult (*GreenCtxCreate)(CUgreenCtx *, CUdevResourceDesc, CUdevice, unsigned int) = nullptr;
-  CUresult (*GreenCtxStreamCreate)(CUstream *, CUgreenCtx, unsigned int, int) = nullptr;
-  CUresult (*GreenCtxDestroy)(CUgreenCtx) = nullptr;
-  bool ok = false;
-};
-const GreenApi &green_api() {
-  static GreenApi g = [] {
-    GreenApi a;
-    auto get = [](const char *name, void **fn) {
-      cudaDriverEntryPointQueryResult qr;
-      return cudaGetDriverEntryPoint(name, fn, cudaEnableDefault, &qr) == cudaSuccess && *fn != nullptr;
-    };
-    a.ok = get("cuDeviceGet", (void **)&a.DeviceGet) && get("cuDeviceGetDevResource", (void **)&a.DeviceGetDevResource) &&
-           get("cuDevSmResourceSplitByCount", (void **)&a.DevSmResourceSplitByCount) &&
-           get("cuDevResourceGenerateDesc", (void **)&a.DevResourceGenerateDesc) && get("cuGreenCtxCreate", (void **)&a.GreenCtxCreate) &&
-           get("cuGreenCtxStreamCreate", (void **)&a.GreenCtxStreamCreate) && get("cuGreenCtxDestroy", (void **)&a.GreenCtxDestroy);
-    return a;
-  }();
-  return g;
-}
-}  // namespace
-
-// Splits the device's SMs into a share for the network kernels and the rest for the DSP kernels and creates one stream
-// in each.  Best effort: on any failure the engine simply keeps the serial schedule (net_sms stays 0).
-static void setup_overlap(pnb_engine *e, int want_net_sms) {
-  const GreenApi &G = green_api();
-  if (!G.ok) return;
-  CUdevice dev;
-  CUdevResource all, grp, rem;
-  unsigned int ngrp = 1;
-  CUdevResourceDesc d_net = nullptr, d_dsp = nullptr;
-  CUgreenCtx g_net = nullptr, g_dsp = nullptr;
-  CUstream s_net = nullptr, s_dsp = nullptr, s_syn = nullptr;
-  if (G.DeviceGet(&dev, e->device) != CUDA_SUCCESS) return;
-  if (G.DeviceGetDevResource(dev, &all, CU_DEV_RESOURCE_TYPE_SM) != CUDA_SUCCESS) return;
-  // default granularity: 8 SMs (keeps whole GPCs' cluster scheduling); PNB_SPLIT_FINE=1 asks for 2-SM (TPC) granularity,
-  // enough for the CTA pairs of the network kernels
-  const char *fine = getenv("PNB_SPLIT_FINE");
-  const unsigned split_flags = (fine && atoi(fine) != 0) ? CU_DEV_SM_RESOURCE_SPLIT_IGNORE_SM_COSCHEDULING : 0;
-  if (G.DevSmResourceSplitByCount(&grp, &ngrp, &all, &rem, split_flags, (unsigned)want_net_sms) != CUDA_SUCCESS || ngrp != 1) return;
-  if (grp.sm.smCount < 8 || rem.sm.smCount < 8) return;
-  if (G.DevResourceGenerateDesc(&d_net, &grp, 1) != CUDA_SUCCESS || G.DevResourceGenerateDesc(&d_dsp, &rem, 1) != CUDA_SUCCESS) return;
-  if (G.GreenCtxCreate(&g_net, d_net, dev, CU_GREEN_CTX_DEFAULT_STREAM) != CUDA_SUCCESS) return;
-  if (G.GreenCtxCreate(&g_dsp, d_dsp, dev, CU_GREEN_CTX_DEFAULT_STREAM) != CUDA_SUCCESS) { G.GreenCtxDestroy(g_net); return; }
-  if (G.GreenCtxStreamCreate(&s_net, g_net, CU_STREAM_NON_BLOCKING, 0) != CUDA_SUCCESS ||
-      G.GreenCtxStreamCreate(&s_dsp, g_dsp, CU_STREAM_NON_BLOCKING, 0) != CUDA_SUCCESS ||
-      G.GreenCtxStreamCreate(&s_syn, g_dsp, CU_STREAM_NON_BLOCKING, 0) != CUDA_SUCCESS) {
-    if (s_net) cudaStreamDestroy((cudaStream_t)s_net);
-    if (s_dsp) cudaStreamDestroy((cudaStream_t)s_dsp);
-    G.GreenCtxDestroy(g_net); G.GreenCtxDestroy(g_dsp);
-    return;
-  }
-  bool ev_ok = cudaEventCreateWithFlags(&e->ev_fork, cudaEventDisableTiming) == cudaSuccess &&
-               cudaEventCreateWithFlags(&e->ev_join_net, cudaEventDisableTiming) == cudaSuccess &&
-               cudaEventCreateWithFlags(&e->ev_join_dsp, cudaEventDisableTiming) == cudaSuccess &&
-               cudaEventCreateWithFlags(&e->ev_join_syn, cudaEventDisableTiming) == cudaSuccess;
-  const int nchunks = (e->Fmax + e->chunk - 1) / e->chunk + 5;  // + the short chunks at both ends of a call
-  e->ev_ana.assign(nchunks, nullptr);
-  e->ev_net.assign(nchunks, nullptr);
-  e->ev_syn[0].assign(nchunks, nullptr);
-  e->ev_syn[1].assign(nchunks, nullptr);
-  for (int k = 0; k < nchunks && ev_ok; k++)
-    ev_ok = cudaEventCreateWithFlags(&e->ev_ana[k], cudaEventDisableTiming) == cudaSuccess &&
-            cudaEventCreateWithFlags(&e->ev_net[k], cudaEventDisableTiming) == cudaSuccess &&
-            cudaEventCreateWithFlags(&e->ev_syn[0][k], cudaEventDisableTiming) == cudaSuccess &&
-            cudaEventCreateWithFlags(&e->ev_syn[1][k], cudaEventDisableTiming) == cudaSuccess;
-  e->green_net = g_net; e->green_dsp = g_dsp;
-  e->s_net = (cudaStream_t)s_net; e->s_dsp = (cudaStream_t)s_dsp; e->s_syn = (cudaStream_t)s_syn;
-  if (!ev_ok) return;  // net_sms stays 0: the serial schedule; pnb_destroy releases what was created
-  e->net_sms = (int)grp.sm.smCount;
-  e->dsp_sms = (int)rem.sm.smCount;
-}
-
 extern "C" int pnb_create(pnb_engine **out, int n_streams, int max_frames, const pnb_model *model, unsigned flags,
                           int device) {
   if (!out) return fail(PNB_ERR_ARG, "out is NULL");
@@ -321,7 +236,6 @@ extern "C" int pnb_create(pnb_engine **out, int n_streams, int max_frames, const
   e->h_status[1] = kNoRejectedSlot;
   // batched stream-state operations: staging of the slot indices, import verdicts, one blob of scratch
   CKD(cudaEventCreateWithFlags(&e->ev_call, cudaEventDisableTiming));
-  CKD(cudaEventCreateWithFlags(&e->ev_state, cudaEventDisableTiming));
   for (int k = 0; k < 2; k++) {
     CKD(cudaEventCreateWithFlags(&e->ev_idx[k], cudaEventDisableTiming));
     CKD(cudaHostAlloc((void **)&e->h_idx[k], S * sizeof(int), cudaHostAllocDefault));
@@ -370,20 +284,9 @@ extern "C" int pnb_create(pnb_engine **out, int n_streams, int max_frames, const
     for (int i = 0; i < 5; i++) CKD(dalloc(&e->h[i][0], (C + 1) * S * e->gru[i].H));
     CKD(dalloc(&e->f32_cnt, (size_t)5 * e->f32_rb));
   }
-  e->tc_sms = e->sm_count;
   if (flags & PNB_NN_TENSOR) {
     int trc = tc_prepare(e, model);
     if (trc) { pnb_destroy(e); return trc; }
-    // Every call runs its kernels one after the other on all SMs (the serial schedule): on H100 it is faster than
-    // any measured split of the SMs between the network and the DSP kernels (DESIGN §6).  PNB_OVERLAP=2 sets up the
-    // chunked schedule instead, in which calls of at least two chunks overlap the DSP kernels with the network on
-    // disjoint SMs (pnb_engine.h); PNB_NET_SMS / PNB_CHUNK / PNB_RAMP tune the split and the chunks.
-    const char *ov = getenv("PNB_OVERLAP"), *ns = getenv("PNB_NET_SMS"), *ch = getenv("PNB_CHUNK");
-    if (ch && atoi(ch) >= 1) e->chunk = atoi(ch);
-    const char *rp = getenv("PNB_RAMP");  // 0: all chunks equal (submitted calls overlap each other, so a call's ends need not be short)
-    if (rp) e->ramp = atoi(rp) != 0;
-    if (ov && atoi(ov) == 2 && max_frames >= 2 * e->chunk && (max_frames + e->chunk - 1) / e->chunk + 5 <= kMaxChunks)
-      setup_overlap(e, ns && atoi(ns) >= 8 ? atoi(ns) : (e->sm_count * 2 / 3 / 8) * 8);  // 88 of an H100's 132 (DESIGN §4)
   }
   CKD(cudaDeviceSynchronize());
   *out = e;
@@ -422,7 +325,6 @@ extern "C" void pnb_destroy(pnb_engine *e) {
   if (e->d_ok) cudaFree(e->d_ok);
   if (e->d_blob1) cudaFree(e->d_blob1);
   if (e->ev_call) cudaEventDestroy(e->ev_call);
-  if (e->ev_state) cudaEventDestroy(e->ev_state);
   if (e->d_tap_pitch) cudaFree(e->d_tap_pitch);
   if (e->d_tab) cudaFree(e->d_tab);
   if (e->d_hin16) cudaFree(e->d_hin16);
@@ -436,19 +338,6 @@ extern "C" void pnb_destroy(pnb_engine *e) {
   }
   if (e->s_in) cudaStreamDestroy(e->s_in);
   if (e->s_out) cudaStreamDestroy(e->s_out);
-  for (cudaEvent_t ev : e->ev_ana) if (ev) cudaEventDestroy(ev);
-  for (cudaEvent_t ev : e->ev_net) if (ev) cudaEventDestroy(ev);
-  for (int p = 0; p < 2; p++)
-    for (cudaEvent_t ev : e->ev_syn[p]) if (ev) cudaEventDestroy(ev);
-  if (e->ev_fork) cudaEventDestroy(e->ev_fork);
-  if (e->ev_join_net) cudaEventDestroy(e->ev_join_net);
-  if (e->ev_join_dsp) cudaEventDestroy(e->ev_join_dsp);
-  if (e->ev_join_syn) cudaEventDestroy(e->ev_join_syn);
-  if (e->s_net) cudaStreamDestroy(e->s_net);
-  if (e->s_dsp) cudaStreamDestroy(e->s_dsp);
-  if (e->s_syn) cudaStreamDestroy(e->s_syn);
-  if (e->green_net) green_api().GreenCtxDestroy((CUgreenCtx)e->green_net);
-  if (e->green_dsp) green_api().GreenCtxDestroy((CUgreenCtx)e->green_dsp);
   for (auto &r : e->prof_pending) { cudaEventDestroy(r.a); cudaEventDestroy(r.b); }
   for (auto ev : e->prof_pool) cudaEventDestroy(ev);
   if (e->stream) cudaStreamDestroy(e->stream);
@@ -475,8 +364,6 @@ extern "C" int pnb_reset(pnb_engine *e) {
   e->hop = 0;
   e->n_active = e->S;
   e->poisoned = false;
-  e->unjoined = false;      // the device was synchronised above (green-context streams included)
-  e->prev_start.clear();
   if (e->flags & PNB_TRAIN_DATA) {
     CK(cudaDeviceSynchronize());
     return PNB_OK;
@@ -676,202 +563,62 @@ static int advance_line(pnb_engine *e, int F, cudaStream_t st) {
   return n;
 }
 
-// Enqueues one call.  Host-side stream state (hop counter, line offset, GRU buffer parity) is committed only after
-// every launch was accepted; a failure in between leaves work half-enqueued, so the engine is poisoned until pnb_reset.
-static AnalysisArgs analysis_args(pnb_engine *e, int h0, int n) {
-  const size_t S = e->S, o = (size_t)h0 * S;
+static AnalysisArgs analysis_args(pnb_engine *e, int F) {
   AnalysisArgs a;
-  a.pcm = e->d_pcm + e->line_off + (size_t)h0 * kFrame;  // this chunk's [history | new hops] window of every row
-  a.pcm_stride = e->pcm_stride; a.n_streams = e->n_active; a.stride = e->S; a.n_frames = n; a.tab = e->d_tab;
-  a.feat = e->d_feat + o * kFeat; a.zring = e->d_zring; a.ering = e->d_ering; a.ring = e->ring; a.hop0 = e->hop + h0;
-  a.P = e->d_P ? e->d_P + o * kBins : nullptr; a.Ex = e->d_Ex + o * kBands; a.raw = nullptr; a.silence = e->d_sil + o;
+  a.pcm = e->d_pcm + e->line_off;  // this call's [history | new hops] window of every row
+  a.pcm_stride = e->pcm_stride; a.n_streams = e->n_active; a.stride = e->S; a.n_frames = F; a.tab = e->d_tab;
+  a.feat = e->d_feat; a.zring = e->d_zring; a.ering = e->d_ering; a.ring = e->ring; a.hop0 = e->hop;
+  a.P = e->d_P; a.Ex = e->d_Ex; a.raw = nullptr; a.silence = e->d_sil;
   a.last_period = e->d_last_period; a.last_gain = e->d_last_gain;
-  a.tap_pitch = e->d_tap_pitch ? e->d_tap_pitch + o * 4 : nullptr;
-  a.tap_pitchf = e->d_tap_pitchf ? e->d_tap_pitchf + o * 2 : nullptr;
+  a.tap_pitch = e->d_tap_pitch; a.tap_pitchf = e->d_tap_pitchf;
   return a;
 }
-static SynthesisArgs synthesis_args(pnb_engine *e, int h0, int n, float *d_out, short *d_out16, size_t out_stride) {
-  const size_t S = e->S, o = (size_t)h0 * S;
+static SynthesisArgs synthesis_args(pnb_engine *e, int F, float *d_out, short *d_out16, size_t out_stride) {
   SynthesisArgs s;
-  s.zring = e->d_zring; s.ring = e->ring; s.hop0 = e->hop + h0; s.P = e->d_P + o * kBins; s.gr = e->d_gr + o * 68;
-  s.Ex = e->d_Ex + o * kBands; s.silence = e->d_sil + o; s.n_streams = e->n_active; s.stride = e->S; s.n_frames = n;
+  s.zring = e->d_zring; s.ring = e->ring; s.hop0 = e->hop; s.P = e->d_P; s.gr = e->d_gr;
+  s.Ex = e->d_Ex; s.silence = e->d_sil; s.n_streams = e->n_active; s.stride = e->S; s.n_frames = F;
   s.tab = e->d_tab; s.synth_mem = e->d_synth;
-  s.out = d_out ? d_out + (size_t)h0 * kFrame : nullptr;
-  s.out16 = d_out16 ? d_out16 + (size_t)h0 * kFrame : nullptr;
-  s.out_stride = out_stride;
+  s.out = d_out; s.out16 = d_out16; s.out_stride = out_stride;
   s.postfilter = (e->flags & PNB_POSTFILTER) ? 1 : 0;
-  s.tap_g = e->d_tap_g ? e->d_tap_g + o * kBands : nullptr;
+  s.tap_g = e->d_tap_g;
   return s;
 }
 
-// How a call is tied to the caller: a plain call forks from the caller's stream and joins back into it; a submitted
-// call (pnb_submit_*) starts when `ready` fires (or at the current end of the caller's stream when it is null), records
-// `done` behind its last synthesis and is NOT joined into any stream, so that the next call's analysis can start
-// while this call's network and synthesis are still running.
-struct CallLink {
-  bool submitted = false;
-  cudaEvent_t ready = nullptr, done = nullptr;
-};
-
-// End of a call: unless its work is still in flight on the engine's streams (a submitted chunked call, which
-// join_engine_streams covers), it ended in `st`; a later state operation waits for that point.
+// Ordering of an engine's work (see pnb_engine.h): every call and state operation makes its stream wait for the last
+// one before its first launch, and marks its own end behind its last launch.
+static int wait_last_call(pnb_engine *e, cudaStream_t st) {
+  if (e->call_recorded) CK(cudaStreamWaitEvent(st, e->ev_call, 0));
+  return PNB_OK;
+}
 static int mark_call_end(pnb_engine *e, cudaStream_t st) {
-  e->state_pending = false;
-  if (e->unjoined) return PNB_OK;
   CK(cudaEventRecord(e->ev_call, st));
   e->call_recorded = true;
   return PNB_OK;
 }
 
-// The caller's stream (or the host, st == nullptr ... not used) catches up with work left in flight by submitted calls.
-static int join_engine_streams(pnb_engine *e, cudaStream_t st) {
-  if (!e->unjoined) return PNB_OK;
-  CK(cudaEventRecord(e->ev_join_net, e->s_net));
-  CK(cudaEventRecord(e->ev_join_dsp, e->s_dsp));
-  CK(cudaEventRecord(e->ev_join_syn, e->s_syn));
-  CK(cudaStreamWaitEvent(st, e->ev_join_net, 0));
-  CK(cudaStreamWaitEvent(st, e->ev_join_dsp, 0));
-  CK(cudaStreamWaitEvent(st, e->ev_join_syn, 0));
-  e->unjoined = false;
-  return PNB_OK;
-}
-static int drain_engine_streams(pnb_engine *e) {  // host-side
-  if (!e->unjoined) return PNB_OK;
-  CK(cudaStreamSynchronize(e->s_dsp));
-  CK(cudaStreamSynchronize(e->s_net));
-  CK(cudaStreamSynchronize(e->s_syn));
-  e->unjoined = false;
-  return PNB_OK;
-}
-
-// Enqueues one call.  Host-side stream state (hop counter, line offset, GRU buffer parity) is committed only after
+// Enqueues one call on st.  Host-side stream state (hop counter, line offset, GRU buffer parity) is committed only after
 // every launch was accepted; a failure in between leaves work half-enqueued, so the engine is poisoned until pnb_reset.
 static int process_device_enqueue(pnb_engine *e, const float *d_in, const short *d_in16, size_t in_stride, float *d_out,
-                                  short *d_out16, size_t out_stride, int F, float *d_gr, cudaStream_t st, const CallLink &lk,
-                                  long long *n_out) {
+                                  short *d_out16, size_t out_stride, int F, float *d_gr, cudaStream_t st, long long *n_out) {
   const int S = e->S, na = e->n_active;  // the call advances streams [0, na); per-call buffers keep the stride S
   long long n = 0;
-  float *line = e->d_pcm + e->line_off;
-  const bool tensor = (e->flags & PNB_NN_TENSOR) != 0;
-  if (tensor && e->net_sms > 0 && F >= 2 * e->chunk) {
-    // ---- chunked schedule: s_dsp runs stage-in + analysis + fc of chunk k+1 and s_syn the synthesis of chunk k-1 (both
-    // on the DSP partition) while s_net runs the network of chunk k on its own SMs
-    cudaStream_t sd = e->s_dsp, sn = e->s_net, ss = e->s_syn;
-    // chunk lengths: short at both ends (the first analysis and the last network chunk run with the other partition
-    // idle unless calls overlap), e->chunk in between
-    int len[kMaxChunks], start[kMaxChunks + 1], C = 0;
-    {
-      int left = F, head[2] = {e->chunk / 4 > 0 ? e->chunk / 4 : 1, e->chunk / 2 > 0 ? e->chunk / 2 : 1};
-      if (!e->ramp) {
-        while (left > 0) { len[C] = left < e->chunk ? left : e->chunk; left -= len[C++]; }
-      }
-      const int tail_total = head[0] + head[1];
-      for (int i = 0; i < 2 && left > tail_total + e->chunk; i++) { len[C++] = head[i]; left -= head[i]; }
-      while (left > tail_total + e->chunk) { len[C++] = e->chunk; left -= e->chunk; }
-      if (left > tail_total) { len[C++] = left - tail_total; left = tail_total; }
-      if (left > head[0]) { len[C++] = left - head[0]; left = head[0]; }
-      if (left > 0) len[C++] = left;
-      start[0] = 0;
-      for (int k = 0; k < C; k++) start[k + 1] = start[k] + len[k];
-    }
-    // start of the call: the caller's stream unless a ready event was given; when the previous call did not run on the
-    // engine's streams (first call, serial schedule) the caller's stream is what orders this call behind it
-    if (!lk.ready || e->prev_start.empty()) {
-      CK(cudaEventRecord(e->ev_fork, st));
-      CK(cudaStreamWaitEvent(sd, e->ev_fork, 0));
-      CK(cudaStreamWaitEvent(sn, e->ev_fork, 0));
-      CK(cudaStreamWaitEvent(ss, e->ev_fork, 0));
-    }
-    if (e->state_pending) {  // a state operation issued since the last call, possibly on another stream
-      CK(cudaStreamWaitEvent(sd, e->ev_state, 0));
-      CK(cudaStreamWaitEvent(sn, e->ev_state, 0));
-      CK(cudaStreamWaitEvent(ss, e->ev_state, 0));
-    }
-    if (lk.ready) CK(cudaStreamWaitEvent(sd, lk.ready, 0));
-    const int cur = e->syn_par ^ 1, prv = e->syn_par;
-    const int pC = (int)e->prev_start.size();
-    e->tc_sms = e->net_sms;
-    for (int k = 0; k < C; k++) {
-      const int h0 = start[k], nh = len[k], h1 = h0 + nh;
-      if (pC) {
-        // What this chunk overwrites was last read by the previous call: hop slots [h0, h1) of the per-call buffers and
-        // the ring slots behind them by its synthesis of the same hops, fc slots [h0+4, h1+4) by its conv1 of hops
-        // < h1+4 (and by its carry, which runs before the last chunk's network-done event).  The synthesis of the last
-        // previous chunk that starts before hop h1+4 is behind all of them.
-        int j = 0;
-        while (j + 1 < pC && e->prev_start[j + 1] < h1 + 4) j++;
-        CK(cudaStreamWaitEvent(sd, e->ev_syn[prv][j], 0));
-      }
-      {
-        ProfScope ps(e, PNB_K_STAGE_IN, sd);
-        n += launch_stage_in(line + (size_t)h0 * kFrame, e->pcm_stride, d_in ? d_in + (size_t)h0 * kFrame : nullptr,
-                             d_in16 ? d_in16 + (size_t)h0 * kFrame : nullptr, in_stride, na, nh * kFrame, sd);
-      }
-      { ProfScope ps(e, PNB_K_ANALYSIS, sd); n += launch_analysis(analysis_args(e, h0, nh), sd); }
-      n += tc_fc(e, h0, nh, sd);  // CUDA-core work: with the DSP kernels
-      CK(cudaEventRecord(e->ev_ana[k], sd));
-      CK(cudaStreamWaitEvent(sn, e->ev_ana[k], 0));
-      int q = tc_front(e, h0, nh, F, sn);
-      if (q < 0) { e->tc_sms = e->sm_count; return q; }
-      n += q;
-      if ((q = tc_gru_chain(e, h0, nh, sn)) < 0) { e->tc_sms = e->sm_count; return q; }
-      n += q;
-      if ((q = tc_out(e, h0, nh, sn)) < 0) { e->tc_sms = e->sm_count; return q; }
-      n += q;
-      if (k == C - 1) {  // the carry reads the call's last fc / conv1 / state slots: before the event the next call waits for
-        if ((q = tc_carry(e, F, sn)) < 0) { e->tc_sms = e->sm_count; return q; }
-        n += q;
-      }
-      CK(cudaEventRecord(e->ev_net[k], sn));
-      CK(cudaStreamWaitEvent(ss, e->ev_net[k], 0));
-      {
-        ProfScope ps(e, PNB_K_SYNTHESIS, ss);
-        n += launch_synthesis(synthesis_args(e, h0, nh, d_out, d_out16, out_stride), ss);
-      }
-      CK(cudaEventRecord(e->ev_syn[cur][k], ss));
-    }
-    e->tc_sms = e->sm_count;
-    n += advance_line(e, F, sd);
-    e->prev_start.assign(start, start + C);
-    e->syn_par = cur;
-    e->unjoined = true;
-    if (lk.submitted) {
-      if (lk.done) CK(cudaEventRecord(lk.done, ss));
-    } else {
-      int rc = join_engine_streams(e, st);
-      if (rc) return rc;
-    }
+  { int rc = wait_last_call(e, st); if (rc) return rc; }
+  { ProfScope ps(e, PNB_K_STAGE_IN, st); n += launch_stage_in(e->d_pcm + e->line_off, e->pcm_stride, d_in, d_in16, in_stride, na, F * kFrame, st); }
+  { ProfScope ps(e, PNB_K_ANALYSIS, st); n += launch_analysis(analysis_args(e, F), st); }
+  CK(cudaGetLastError());
+  if (e->flags & PNB_NN_TENSOR) {
+    const int q = tc_network(e, F, st);
+    if (q < 0) return q;
+    n += q;
   } else {
-    // ---- serial schedule on the caller's stream
-    if (lk.ready) CK(cudaStreamWaitEvent(st, lk.ready, 0));
-    if (e->state_pending) CK(cudaStreamWaitEvent(st, e->ev_state, 0));
-    { int rc = join_engine_streams(e, st); if (rc) return rc; }
-    e->prev_start.clear();
-    { ProfScope ps(e, PNB_K_STAGE_IN, st); n += launch_stage_in(line, e->pcm_stride, d_in, d_in16, in_stride, na, F * kFrame, st); }
-    { ProfScope ps(e, PNB_K_ANALYSIS, st); n += launch_analysis(analysis_args(e, 0, F), st); }
-    CK(cudaGetLastError());
-    if (tensor) {
-      n += tc_fc(e, 0, F, st);
-      int k = tc_front(e, 0, F, F, st);
-      if (k < 0) return k;
-      n += k;
-      if ((k = tc_gru_chain(e, 0, F, st)) < 0) return k;
-      n += k;
-      if ((k = tc_out(e, 0, F, st)) < 0) return k;
-      n += k;
-      if ((k = tc_carry(e, F, st)) < 0) return k;
-      n += k;
-    } else {
-      for (int h0 = 0; h0 < F; h0 += e->f32_chunk) {
-        const int q = nn_chunk_f32(e, h0, F - h0 < e->f32_chunk ? F - h0 : e->f32_chunk, st);
-        if (q < 0) return q;
-        n += q;
-      }
+    for (int h0 = 0; h0 < F; h0 += e->f32_chunk) {
+      const int q = nn_chunk_f32(e, h0, F - h0 < e->f32_chunk ? F - h0 : e->f32_chunk, st);
+      if (q < 0) return q;
+      n += q;
     }
-    { ProfScope ps(e, PNB_K_SYNTHESIS, st); n += launch_synthesis(synthesis_args(e, 0, F, d_out, d_out16, out_stride), st); }
-    n += advance_line(e, F, st);
-    if (lk.submitted && lk.done) CK(cudaEventRecord(lk.done, st));
   }
+  { ProfScope ps(e, PNB_K_SYNTHESIS, st); n += launch_synthesis(synthesis_args(e, F, d_out, d_out16, out_stride), st); }
+  n += advance_line(e, F, st);
   if (d_gr)  // [F][na][68] from the [F][S][68] buffer
     CK(cudaMemcpy2DAsync(d_gr, (size_t)na * 68 * sizeof(float), e->d_gr, (size_t)S * 68 * sizeof(float), (size_t)na * 68 * sizeof(float), F,
                          cudaMemcpyDeviceToDevice, st));
@@ -882,8 +629,7 @@ static int process_device_enqueue(pnb_engine *e, const float *d_in, const short 
 }
 
 static int process_device(pnb_engine *e, const float *d_in, const short *d_in16, size_t in_stride, float *d_out,
-                          short *d_out16, size_t out_stride, int F, float *d_gr, cudaStream_t st,
-                          const CallLink &lk = CallLink()) {
+                          short *d_out16, size_t out_stride, int F, float *d_gr, cudaStream_t st) {
   if (!e) return fail(PNB_ERR_ARG, "engine is NULL");
   if (e->flags & PNB_TRAIN_DATA) return fail(PNB_ERR_ARG, "engine was created with PNB_TRAIN_DATA: use pnb_train_records_*");
   if (e->poisoned) return fail(PNB_ERR_CUDA, "an earlier call failed while enqueuing work; the streams' state is undefined until pnb_reset");
@@ -893,8 +639,7 @@ static int process_device(pnb_engine *e, const float *d_in, const short *d_in16,
     return fail(PNB_ERR_ARG, "row stride smaller than n_frames*480");
   CK(cudaSetDevice(e->device));
   long long n = 0;
-  if (lk.submitted && d_gr) return fail(PNB_ERR_ARG, "submitted calls do not copy g/r out");
-  const int rc = process_device_enqueue(e, d_in, d_in16, in_stride, d_out, d_out16, out_stride, F, d_gr, st, lk, &n);
+  const int rc = process_device_enqueue(e, d_in, d_in16, in_stride, d_out, d_out16, out_stride, F, d_gr, st, &n);
   if (rc) {
     e->poisoned = true;
     return rc;
@@ -934,7 +679,7 @@ extern "C" int pnb_train_records_device(pnb_engine *e, const short *d_speech, si
   const int S = e->S, N = S / 2;
   long long n = 0;
   float *line = e->d_pcm + e->line_off;
-  if (e->state_pending) CK(cudaStreamWaitEvent(st, e->ev_state, 0));
+  { int rc = wait_last_call(e, st); if (rc) return rc; }
   {
     ProfScope ps(e, PNB_K_STAGE_IN, st);
     n += launch_stage_in(line, e->pcm_stride, nullptr, d_noisy, noisy_stride, N, F * kFrame, st, 1.f);
@@ -1082,14 +827,14 @@ static int submit_host(pnb_engine *e, const T *in, size_t in_stride, T *out, siz
   const size_t w = (size_t)F * kFrame * sizeof(T), na = e->n_active;  // the rows of in / out
   CK(cudaMemcpy2DAsync(e->pipe_in[k], row * sizeof(T), in, in_stride * sizeof(T), w, na, cudaMemcpyHostToDevice, e->s_in));
   CK(cudaEventRecord(e->ev_in[k], e->s_in));
-  CallLink lk;  // starts when the copy has landed, not joined into any stream: the next call's analysis may overlap this call's tail
-  lk.submitted = true; lk.ready = e->ev_in[k]; lk.done = e->ev_cmp[k];
+  CK(cudaStreamWaitEvent(e->stream, e->ev_in[k], 0));
   int rc;
   if (sizeof(T) == 4)
-    rc = process_device(e, (const float *)e->pipe_in[k], nullptr, row, (float *)e->pipe_out[k], nullptr, row, F, nullptr, e->stream, lk);
+    rc = process_device(e, (const float *)e->pipe_in[k], nullptr, row, (float *)e->pipe_out[k], nullptr, row, F, nullptr, e->stream);
   else
-    rc = process_device(e, nullptr, (const short *)e->pipe_in[k], row, nullptr, (short *)e->pipe_out[k], row, F, nullptr, e->stream, lk);
+    rc = process_device(e, nullptr, (const short *)e->pipe_in[k], row, nullptr, (short *)e->pipe_out[k], row, F, nullptr, e->stream);
   if (rc) return rc;
+  CK(cudaEventRecord(e->ev_cmp[k], e->stream));
   CK(cudaStreamWaitEvent(e->s_out, e->ev_cmp[k], 0));
   CK(cudaMemcpy2DAsync(out, out_stride * sizeof(T), e->pipe_out[k], row * sizeof(T), w, na, cudaMemcpyDeviceToHost, e->s_out));
   CK(cudaEventRecord(e->ev_out[k], e->s_out));
@@ -1151,32 +896,26 @@ extern "C" int pnb_submit_train_records(pnb_engine *e, const short *speech, size
   return PNB_OK;
 }
 
-// Device-buffer twins of pnb_submit_host_*: the call starts when `cuda_stream` reaches this point (the inputs are ready in
-// its order) and is not joined back; pnb_flush makes a stream wait for everything submitted, pnb_wait the host.
+// pnb_process_device_* without g/r; both names are part of the ABI.
 extern "C" int pnb_submit_device_f32(pnb_engine *e, const float *d_in, size_t in_stride, float *d_out, size_t out_stride,
                                      int n_frames, void *cuda_stream) {
-  CallLink lk;
-  lk.submitted = true;
-  return process_device(e, d_in, nullptr, in_stride, d_out, nullptr, out_stride, n_frames, nullptr, (cudaStream_t)cuda_stream, lk);
+  return pnb_process_device_f32(e, d_in, in_stride, d_out, out_stride, n_frames, nullptr, cuda_stream);
 }
 extern "C" int pnb_submit_device_i16(pnb_engine *e, const short *d_in, size_t in_stride, short *d_out, size_t out_stride,
                                      int n_frames, void *cuda_stream) {
-  CallLink lk;
-  lk.submitted = true;
-  return process_device(e, nullptr, d_in, in_stride, nullptr, d_out, out_stride, n_frames, nullptr, (cudaStream_t)cuda_stream, lk);
+  return pnb_process_device_i16(e, d_in, in_stride, d_out, out_stride, n_frames, nullptr, cuda_stream);
 }
 extern "C" int pnb_flush(pnb_engine *e, void *cuda_stream) {
   if (!e) return fail(PNB_ERR_ARG, "engine is NULL");
   CK(cudaSetDevice(e->device));
-  return join_engine_streams(e, (cudaStream_t)cuda_stream);
+  return wait_last_call(e, (cudaStream_t)cuda_stream);
 }
 
 extern "C" int pnb_wait(pnb_engine *e) {
   if (!e) return fail(PNB_ERR_ARG, "engine is NULL");
   CK(cudaSetDevice(e->device));
   if (e->s_in) CK(cudaStreamSynchronize(e->s_in));
-  { int rc = drain_engine_streams(e); if (rc) return rc; }
-  CK(cudaEventSynchronize(e->ev_state));  // the last state operation, whichever stream it was issued on
+  { int rc = wait_last_call(e, e->stream); if (rc) return rc; }  // the status covers every call, on any stream
   CK(cudaMemcpyAsync(e->h_status, e->d_status, 2 * sizeof(int), cudaMemcpyDeviceToHost, e->stream));
   CK(cudaStreamSynchronize(e->stream));
   if (e->s_out) CK(cudaStreamSynchronize(e->s_out));
@@ -1239,13 +978,12 @@ extern "C" int pnb_read_tap(pnb_engine *e, int what, void *dst, size_t dst_bytes
 extern "C" size_t pnb_state_size(void) { return sizeof(StreamState); }
 
 // Enqueues one batched state operation on st (arguments already checked): after every call and state operation issued
-// earlier on the engine, before every one issued later (ev_call / ev_state, see pnb_engine.h).
+// earlier on the engine, before every one issued later (ev_call, see pnb_engine.h).
 static int state_enqueue(pnb_engine *e, int mode, const int *streams, int n, void *d_blobs, size_t blob_stride, cudaStream_t st) {
   StateArgs a;
   memset(&a, 0, sizeof a);
   a.n_seg = state_segs(e, a.seg);
-  if (e->call_recorded) CK(cudaStreamWaitEvent(st, e->ev_call, 0));
-  { int rc = join_engine_streams(e, st); if (rc) return rc; }
+  { int rc = wait_last_call(e, st); if (rc) return rc; }
   // the slot indices travel through pinned staging: the caller's array is free again when this returns
   const int k = e->idx_slot;
   CK(cudaEventSynchronize(e->ev_idx[k]));  // the copy out of this slot two operations ago has run
@@ -1261,10 +999,7 @@ static int state_enqueue(pnb_engine *e, int mode, const int *streams, int n, voi
   if (mode == kStateImport) nl += launch_state_check(a, st);
   nl += launch_state_move(a, st);
   CK(cudaGetLastError());
-  CK(cudaEventRecord(e->ev_state, st));
-  CK(cudaEventRecord(e->ev_call, st));
-  e->call_recorded = true;
-  e->state_pending = true;
+  { int rc = mark_call_end(e, st); if (rc) return rc; }
   e->launches += nl;
   return PNB_OK;
 }
@@ -1494,33 +1229,8 @@ extern "C" long long pnb_launch_count(const pnb_engine *e) { return e ? e->launc
 extern "C" int pnb_launches_per_call(const pnb_engine *e, int n_frames) {
   if (!e) return 0;
   // without the history move of advance_line (at most one more launch per call)
-  if (e->flags & PNB_NN_TENSOR) {
-    const int C = (e->net_sms > 0 && n_frames >= 2 * e->chunk) ? (n_frames + e->chunk - 1) / e->chunk + 4 : 1;  // upper bound
-    return 1 + C * (2 + tc_launches_per_chunk(e)) + 1;  // stage_in + per chunk (analysis, network, synthesis) + carry
-  }
+  if (e->flags & PNB_NN_TENSOR) return 10;  // stage_in, analysis, fc, conv1, conv2, GRU chain, fc_gb, fc_rb, carry, synthesis
   return 3 + 7 * ((n_frames + e->f32_chunk - 1) / e->f32_chunk);  // stage_in, analysis, synthesis + per chunk: fc, conv1, conv2, GRU chain, fc_gb, fc_rb, carry
-}
-// Runtime switch for the chunked overlap schedule (an engine created without it cannot turn it on): profiling a
-// kernel class alone on all SMs needs the serial schedule.
-extern "C" int pnb_set_overlap(pnb_engine *e, int on) {
-  if (!e) return fail(PNB_ERR_ARG, "engine is NULL");
-  if (!e->s_net) return on ? fail(PNB_ERR_ARG, "this engine was created without an SM partition") : PNB_OK;
-  CK(cudaSetDevice(e->device));
-  CK(cudaDeviceSynchronize());
-  if (on) {
-    if (e->net_sms == 0) { e->net_sms = e->saved_net_sms; }
-  } else if (e->net_sms) {
-    e->saved_net_sms = e->net_sms;
-    e->net_sms = 0;
-  }
-  return PNB_OK;
-}
-extern "C" int pnb_overlap_info(const pnb_engine *e, int *net_sms, int *dsp_sms, int *chunk_hops) {
-  if (!e) return fail(PNB_ERR_ARG, "engine is NULL");
-  if (net_sms) *net_sms = e->net_sms;
-  if (dsp_sms) *dsp_sms = e->dsp_sms;
-  if (chunk_hops) *chunk_hops = e->chunk;
-  return PNB_OK;
 }
 extern "C" int pnb_n_streams(const pnb_engine *e) { return e ? e->S : 0; }
 extern "C" int pnb_max_frames(const pnb_engine *e) { return e ? e->Fmax : 0; }

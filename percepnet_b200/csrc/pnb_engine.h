@@ -73,24 +73,6 @@ struct pnb_engine {
   long long submitted = 0;
 
   pnb_tc_state *tc = nullptr;
-  int tc_sms = 0;  // SMs the persistent network kernels may occupy (all of them, or the network's share of a partition)
-  // Overlap of the DSP kernels with the network inside long calls (tensor mode): the call is cut into chunks of hops,
-  // analysis / synthesis of neighbouring chunks run on s_dsp while the network of a chunk runs on s_net, each stream
-  // in its own green context = its own disjoint set of SMs.  The network phase alone is capped by the board's power
-  // limit (it clocks down to ~1.4 GHz) while the DSP phase leaves that budget unused; side by side they even out.
-  void *green_net = nullptr, *green_dsp = nullptr;  // CUgreenCtx
-  cudaStream_t s_net = nullptr, s_dsp = nullptr, s_syn = nullptr;  // s_syn: synthesis, in the DSP partition
-  int net_sms = 0, dsp_sms = 0, chunk = 8, saved_net_sms = 0;
-  bool ramp = true;              // short chunks at both ends of a call (PNB_RAMP=0: all chunks equal)
-  cudaEvent_t ev_fork = nullptr, ev_join_net = nullptr, ev_join_dsp = nullptr, ev_join_syn = nullptr;
-  std::vector<cudaEvent_t> ev_ana, ev_net;
-  // Calls overlap each other as well (pnb_submit_*): the analysis of call i+1 starts while the network and synthesis
-  // of call i are still running.  What call i+1 overwrites (hop-slot buffers, spectrum ring, fc slots) is guarded by
-  // the synthesis-done events of call i, kept per chunk and double-buffered by call parity.
-  std::vector<cudaEvent_t> ev_syn[2];
-  std::vector<int> prev_start;   // first hop of every chunk of the previous chunked call (empty: it was not chunked)
-  int syn_par = 0;               // which ev_syn[] the previous chunked call recorded into
-  bool unjoined = false;         // submitted work is in flight on the engine's own streams, not joined into any caller stream
   int last_frames = 0;
   long long launches = 0;
   // status word on the device: bit 0 = an activation left the domain in which the reference's tansig_approx is
@@ -99,12 +81,13 @@ struct pnb_engine {
   int *d_status = nullptr;  // [2]
   int *h_status = nullptr;  // [2] pinned host copy, refreshed by the synchronising entry points
 
-  // Batched stream-state operations (pnb_reset_streams / pnb_export_states / pnb_import_states).  Every call and state
-  // operation that ends in its caller's stream records ev_call there; a state operation waits for it (and joins the
-  // engine's own streams), and the next call waits for ev_state, whichever stream either was issued on.
-  cudaEvent_t ev_call = nullptr, ev_state = nullptr;
+  // Ordering: every call (process, submit, train records) and every state operation (pnb_reset_streams /
+  // pnb_export_states / pnb_import_states) makes the stream it is issued on wait for ev_call before its first launch and
+  // records ev_call there after its last.  Each waits for the one before, so ev_call stands for everything issued
+  // earlier on the engine, whichever stream it went to; pnb_flush and pnb_wait wait for it too.
+  cudaEvent_t ev_call = nullptr;
   bool call_recorded = false;    // ev_call has been recorded at least once
-  bool state_pending = false;    // a state operation was issued after the last call
+  // batched stream-state operations: staging of the slot indices, import verdicts, one blob of scratch
   int *h_idx[2] = {nullptr, nullptr};  // [S] pinned staging of the slot indices, double-buffered ...
   int *d_idx[2] = {nullptr, nullptr};  // [S] ... and their device copies
   cudaEvent_t ev_idx[2] = {nullptr, nullptr};  // the copy out of h_idx[k] has run
@@ -131,13 +114,8 @@ struct pnb_engine {
 int tc_prepare(pnb_engine *e, const pnb_model *model);
 void tc_release(pnb_engine *e);
 int tc_reset(pnb_engine *e);
-// the network of hops [h0, h0+n) of a call of F hops: hop-parallel front, the GRU chain, hop-parallel output layers
-int tc_fc(pnb_engine *e, int h0, int n, cudaStream_t st);
-int tc_front(pnb_engine *e, int h0, int n, int F, cudaStream_t st);
-int tc_gru_chain(pnb_engine *e, int h0, int n, cudaStream_t st);
-int tc_out(pnb_engine *e, int h0, int n, cudaStream_t st);
-int tc_carry(pnb_engine *e, int F, cudaStream_t st);       // once per call, after its last tc_out
-int tc_launches_per_chunk(const pnb_engine *e);
+// the network of a call of F hops: hop-parallel front, the GRU chain, hop-parallel output layers, carry
+int tc_network(pnb_engine *e, int F, cudaStream_t st);
 // The tensor path's pieces of a stream's state (pnb_state.cu): appended to seg[ns..]; returns the new count
 int tc_state_segs(const pnb_engine *e, pnb::StateSeg *seg, int ns);
 

@@ -562,9 +562,8 @@ struct ChainLayer {
 struct ChainArgs {
   CUtensorMap maps[16];  // 0: conv2 out, 1..5: state slots of the five GRUs, 6..10: input weights, 11..15: recurrent weights
   ChainLayer L[5];
-  int S, F;              // rows per hop slot of the buffers; hops this launch covers
+  int S, F;              // rows per hop slot of the buffers; hops of the call
   int n;                 // active streams: rows [0, n) of every slot
-  int t0;                // first hop of this launch inside the call (slot / counter arithmetic is per call)
   int tiles_mp;          // row tiles of the active streams (128 streams each)
   int units_per_hop;
   int diag;              // unit order: 0 = hop-major (layer by layer inside a hop), 1 = anti-diagonals (few streams)
@@ -616,7 +615,6 @@ __device__ __forceinline__ Unit decode_unit_diag(const ChainArgs &a, int u) {
     }
   }
   const int sh = a.L[x.l].tiles_log2;
-  x.t += a.t0;
   x.mp = r >> sh;
   x.nt = r & ((1 << sh) - 1);
   return x;
@@ -624,9 +622,8 @@ __device__ __forceinline__ Unit decode_unit_diag(const ChainArgs &a, int u) {
 __device__ __forceinline__ Unit decode_unit(const ChainArgs &a, int u) {
   if (a.diag) return decode_unit_diag(a, u);
   Unit x;
-  const int tl = u / a.units_per_hop;
-  int r = u - tl * a.units_per_hop;
-  x.t = a.t0 + tl;
+  x.t = u / a.units_per_hop;
+  int r = u - x.t * a.units_per_hop;
   x.l = 0;
 #pragma unroll
   for (int i = 1; i < 5; i++) x.l = (r >= a.L[i].unit0) ? i : x.l;
@@ -1252,11 +1249,9 @@ int tc_state_segs(const pnb_engine *e, StateSeg *seg, int ns) {
   return ns;
 }
 
-int tc_launches_per_chunk(const pnb_engine *) { return 6; }  // fc, conv1, conv2, GRU chain, fc_gb, fc_rb (+ 1 carry per call)
-
 template <typename K, typename A>
 static int tc_launch(pnb_engine *e, K kernel, const A &a, int units, size_t smem, cudaStream_t st) {
-  int grid = units < e->tc_sms ? units : e->tc_sms;  // persistent: one CTA per SM of the network's share
+  int grid = units < e->sm_count ? units : e->sm_count;  // persistent: one CTA per SM
   if (grid < 1) grid = 1;
   kernel<<<grid, kTcThreads, smem, st>>>(a);
   TCK(cudaGetLastError());
@@ -1284,51 +1279,47 @@ static TcSeg mkseg(int a_map, int b_map, int K, int a_k0, int b_k0, int a_row0, 
   return s;
 }
 
-// ---- the network of hops [h0, h0 + n) of a call of F hops, in three phases -----------------------------------
-// The non-recurrent front (rnn.cpp:50-52 on n S rows): fc (tc_fc) -> conv1 -> conv2 (tc_front).  Hop t of the call lives in slot t of the
-// per-call buffers, so a phase can be run for any hop range once the earlier hops' phases are enqueued.
-// Returns the number of launches or a negative error.
-int tc_fc(pnb_engine *e, int h0, int n, cudaStream_t st) {
-  // fc (fp32 FMA on the CUDA cores: it runs with the DSP kernels when the schedule is split) -> bf16 terms at slots 4 + h0 ..
+// ---- the network of a call of F hops, in phases; each returns its number of launches or a negative error ------------
+// The non-recurrent front (rnn.cpp:50-52 on F S rows): fc -> conv1 -> conv2.  Hop t of the call lives in slot t of the
+// per-call buffers.
+static int tc_front(pnb_engine *e, int F, cudaStream_t st) {
   pnb_tc_state *t = e->tc;
   const int S = e->S, Fm = e->Fmax, na = e->n_active;
-  const int rows = na == S ? n * S : na, slots = na == S ? 1 : n;  // per grid.y slot
-  ProfScope ps(e, PNB_K_TC_AUX, st);
-  fc_split_kernel<<<dim3((rows + FC_ROWS - 1) / FC_ROWS, slots), 128, 0, st>>>(e->d_feat + (size_t)h0 * S * kFeat, e->fc.W, e->fc.b,
-                                                  t->fc_all + (size_t)(4 + h0) * S * 128, rows, (size_t)(Fm + 4) * S, (size_t)S);
-  return 1;
-}
-int tc_front(pnb_engine *e, int h0, int n, int F, cudaStream_t st) {
-  pnb_tc_state *t = e->tc;
-  const int S = e->S, Fm = e->Fmax;
   const float *tbl = e->tansig();
   int nl = 0, rc;
+  {  // fc (fp32 FMA on the CUDA cores) -> bf16 terms at slots 4 ..
+    const int rows = na == S ? F * S : na, slots = na == S ? 1 : F;  // per grid.y slot
+    ProfScope ps(e, PNB_K_TC_AUX, st);
+    fc_split_kernel<<<dim3((rows + FC_ROWS - 1) / FC_ROWS, slots), 128, 0, st>>>(e->d_feat, e->fc.W, e->fc.b,
+                                                    t->fc_all + (size_t)4 * S * 128, rows, (size_t)(Fm + 4) * S, (size_t)S);
+    nl++;
+  }
   TcArgs a;
   // conv1: tap q of hop t reads fc slot t + q (oldest first, nnet.cpp:182-200); output -> c1 slots 2 + t
   memset(&a, 0, sizeof a);
   a.maps[0] = t->m_fc_all;
   a.maps[1] = t->m_wconv1;
-  for (int q = 0; q < 5; q++) a.seg[q] = mkseg(0, 1, 128, 0, q * 128, (h0 + q) * S, (Fm + 4) * S);
+  for (int q = 0; q < 5; q++) a.seg[q] = mkseg(0, 1, 128, 0, q * 128, q * S, (Fm + 4) * S);
   a.n_seg = 5; a.b_term_rows = 512; a.out_scale = 1.f; a.tansig = tbl;
   a.bias = t->bias_pad; a.act = PNB_ACT_RELU; a.N = 512;
-  a.out_b = t->c1_all; a.out_row0 = (2 + h0) * S; a.out_plane_rows = (Fm + 2) * S; a.out_terms = kConvTerms; a.wide = t->wide;
+  a.out_b = t->c1_all; a.out_row0 = 2 * S; a.out_plane_rows = (Fm + 2) * S; a.out_terms = kConvTerms; a.wide = t->wide;
   {
     ProfScope ps(e, PNB_K_TC_GEMM, st);
-    if ((rc = tc_launch_dense<DENSE_BN, true, DENSE_STAGES, DENSE_STAGES3>(e, a, n, 512 / DENSE_BN, st))) return rc;
+    if ((rc = tc_launch_dense<DENSE_BN, true, DENSE_STAGES, DENSE_STAGES3>(e, a, F, 512 / DENSE_BN, st))) return rc;
     nl++;
   }
   // conv2: three taps -> tanh -> fp16 terms (gru1 / gru_rb / fc_gb inputs); fp32 copy of the call's last hop
   memset(&a, 0, sizeof a);
   a.maps[0] = t->m_c1_all;
   a.maps[1] = t->m_wconv2;
-  for (int q = 0; q < 3; q++) a.seg[q] = mkseg(0, 1, 512, 0, q * 512, (h0 + q) * S, (Fm + 2) * S);
+  for (int q = 0; q < 3; q++) a.seg[q] = mkseg(0, 1, 512, 0, q * 512, q * S, (Fm + 2) * S);
   a.n_seg = 3; a.b_term_rows = 512; a.out_scale = 1.f; a.tansig = tbl;
   a.bias = t->bias_pad + 512; a.act = PNB_ACT_TANH; a.N = 512;
-  if (h0 + n == F) { a.out_f32 = e->c2; a.ldc = 512; a.f32_row0 = (n - 1) * S; }
-  a.out_h = t->c2_h; a.out_row0 = h0 * S; a.out_plane_rows = Fm * S; a.wide = t->wide;
+  a.out_f32 = e->c2; a.ldc = 512; a.f32_row0 = (F - 1) * S;
+  a.out_h = t->c2_h; a.out_row0 = 0; a.out_plane_rows = Fm * S; a.wide = t->wide;
   {
     ProfScope ps(e, PNB_K_TC_GEMM, st);
-    if ((rc = tc_launch_dense<DENSE_BN, true, DENSE_STAGES, DENSE_STAGES3>(e, a, n, 512 / DENSE_BN, st))) return rc;
+    if ((rc = tc_launch_dense<DENSE_BN, true, DENSE_STAGES, DENSE_STAGES3>(e, a, F, 512 / DENSE_BN, st))) return rc;
     nl++;
   }
   return nl;
@@ -1336,7 +1327,7 @@ int tc_front(pnb_engine *e, int h0, int n, int F, cudaStream_t st) {
 
 // The recurrent part: five GRUs per hop (rnn.cpp:58-71) in one persistent launch.  State slot t holds the state
 // BEFORE hop t of the call; the fp32 state ping-pongs by hop, starting from e->par (the call's first hop).
-int tc_gru_chain(pnb_engine *e, int h0, int n, cudaStream_t st) {
+static int tc_gru_chain(pnb_engine *e, int F, cudaStream_t st) {
   pnb_tc_state *t = e->tc;
   const int S = e->S, Fm = e->Fmax;
   ChainArgs a;
@@ -1344,7 +1335,7 @@ int tc_gru_chain(pnb_engine *e, int h0, int n, cudaStream_t st) {
   a.maps[0] = t->m_c2_ch;
   for (int i = 0; i < 5; i++) { a.maps[1 + i] = t->m_h_ch[i]; a.maps[6 + i] = t->m_w[i]; a.maps[11 + i] = t->m_u[i]; }
   // only the active streams' row tiles are units; the counters of the others stay zero
-  a.S = S; a.n = e->n_active; a.F = n; a.t0 = h0; a.tiles_mp = (e->n_active + TM - 1) / TM; a.cnt = t->cnt; a.tansig = e->tansig();
+  a.S = S; a.n = e->n_active; a.F = F; a.tiles_mp = (e->n_active + TM - 1) / TM; a.cnt = t->cnt; a.tansig = e->tansig();
   const int c2_terms = Fm * S, h_terms = (Fm + 1) * S;
   int unit0 = 0;
   for (int li = 0; li < 5; li++) {
@@ -1374,17 +1365,17 @@ int tc_gru_chain(pnb_engine *e, int h0, int n, cudaStream_t st) {
   a.units_per_hop = unit0;
   // with many streams one layer-hop fills the machine and hop-major order keeps a layer's fresh output in L2 for the
   // layer above; with few, only the anti-diagonal order exposes enough independent units
-  a.diag = (a.tiles_mp * (512 / HT) < e->tc_sms) ? 1 : 0;
+  a.diag = (a.tiles_mp * (512 / HT) < e->sm_count) ? 1 : 0;
   {
     ProfScope ps(e, PNB_K_TC_GEMM, st);
-    int rc = tc_launch(e, gru_chain_kernel, a, n * unit0, tc_smem_bytes<GRU_STAGES, GRU_STAGES * GruStage::kBytes>(), st);
+    int rc = tc_launch(e, gru_chain_kernel, a, F * unit0, tc_smem_bytes<GRU_STAGES, GRU_STAGES * GruStage::kBytes>(), st);
     if (rc) return rc;
   }
   return 1;
 }
 
 // The two 34-wide output layers (rnn.cpp:73-80; N padded to 48, fp16 two-term split, sigmoid epilogue).
-int tc_out(pnb_engine *e, int h0, int n, cudaStream_t st) {
+static int tc_out(pnb_engine *e, int F, cudaStream_t st) {
   pnb_tc_state *t = e->tc;
   const int S = e->S, Fm = e->Fmax;
   const float *tbl = e->tansig();
@@ -1395,24 +1386,24 @@ int tc_out(pnb_engine *e, int h0, int n, cudaStream_t st) {
   a.maps[0] = t->m_c2;
   for (int q = 0; q < 4; q++) a.maps[1 + q] = t->m_h[q];
   a.maps[5] = t->m_wgb;
-  a.seg[0] = mkseg(0, 5, 512, 0, 0, h0 * S, Fm * S);
-  for (int q = 1; q < 5; q++) a.seg[q] = mkseg(q, 5, 512, 0, q * 512, (h0 + 1) * S, h_terms);  // state after hop t = slot t+1
+  a.seg[0] = mkseg(0, 5, 512, 0, 0, 0, Fm * S);
+  for (int q = 1; q < 5; q++) a.seg[q] = mkseg(q, 5, 512, 0, q * 512, S, h_terms);  // state after hop t = slot t+1
   a.n_seg = 5; a.b_term_rows = SMALL_BN; a.out_scale = t->scale_gb; a.tansig = tbl;
-  a.bias = t->bias_pad + 1024; a.act = PNB_ACT_SIGMOID; a.N = 34; a.ldc = 68; a.out_f32 = e->d_gr + (size_t)h0 * S * 68;
+  a.bias = t->bias_pad + 1024; a.act = PNB_ACT_SIGMOID; a.N = 34; a.ldc = 68; a.out_f32 = e->d_gr;
   {
     ProfScope ps(e, PNB_K_TC_GEMM, st);
-    if ((rc = tc_launch_dense<SMALL_BN, false, SMALL_STAGES, 0>(e, a, n, 1, st))) return rc;
+    if ((rc = tc_launch_dense<SMALL_BN, false, SMALL_STAGES, 0>(e, a, F, 1, st))) return rc;
     nl++;
   }
   memset(&a, 0, sizeof a);
   a.maps[0] = t->m_h[4];
   a.maps[1] = t->m_wrb;
-  a.seg[0] = mkseg(0, 1, 128, 0, 0, (h0 + 1) * S, h_terms);
+  a.seg[0] = mkseg(0, 1, 128, 0, 0, S, h_terms);
   a.n_seg = 1; a.b_term_rows = SMALL_BN; a.out_scale = t->scale_rb; a.tansig = tbl;
-  a.bias = t->bias_pad + 1072; a.act = PNB_ACT_SIGMOID; a.N = 34; a.ldc = 68; a.out_f32 = e->d_gr + (size_t)h0 * S * 68 + 34;
+  a.bias = t->bias_pad + 1072; a.act = PNB_ACT_SIGMOID; a.N = 34; a.ldc = 68; a.out_f32 = e->d_gr + 34;
   {
     ProfScope ps(e, PNB_K_TC_GEMM, st);
-    if ((rc = tc_launch_dense<SMALL_BN, false, SMALL_STAGES, 0>(e, a, n, 1, st))) return rc;
+    if ((rc = tc_launch_dense<SMALL_BN, false, SMALL_STAGES, 0>(e, a, F, 1, st))) return rc;
     nl++;
   }
   return nl;
@@ -1420,7 +1411,7 @@ int tc_out(pnb_engine *e, int h0, int n, cudaStream_t st) {
 
 // End of a call of F hops: the last 4 fc / 2 conv1 hop slots and the last state slot move to the front, the chain's
 // dependency counters return to zero (one launch), and the fp32 state parity advances by F.
-int tc_carry(pnb_engine *e, int F, cudaStream_t st) {
+static int tc_carry(pnb_engine *e, int F, cudaStream_t st) {
   pnb_tc_state *t = e->tc;
   const int S = e->S, Fm = e->Fmax, na = e->n_active;
   const int h_terms = (Fm + 1) * S;
@@ -1444,9 +1435,19 @@ int tc_carry(pnb_engine *e, int F, cudaStream_t st) {
   ca.n_seg = ns;
   {
     ProfScope ps(e, PNB_K_TC_AUX, st);
-    tc_carry_kernel<<<2 * e->tc_sms, 256, 0, st>>>(ca);
+    tc_carry_kernel<<<2 * e->sm_count, 256, 0, st>>>(ca);
   }
   if (F & 1)
     for (int li = 0; li < 5; li++) e->par[li] ^= 1;
   return 1;
+}
+
+int tc_network(pnb_engine *e, int F, cudaStream_t st) {
+  int n = 0;
+  for (int (*phase)(pnb_engine *, int, cudaStream_t) : {tc_front, tc_gru_chain, tc_out, tc_carry}) {
+    const int q = phase(e, F, st);
+    if (q < 0) return q;
+    n += q;
+  }
+  return n;
 }

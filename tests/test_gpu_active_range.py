@@ -6,16 +6,17 @@ import ctypes
 import numpy as np
 import pytest
 
-from test_gpu_lifecycle import OVERLAP, SERIAL, _engine, _signal
+from test_gpu_lifecycle import _engine, _ops_stream, _signal
 from test_gpu_parity import api  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
 HOP = 480
 FM = 16
-# (id, network mode, streams, environment at pnb_create); 1000 is not a multiple of the 128-row tile
-CONFIGS = [("fp32-1000", "fp32", 1000, {}), ("fp32-2048", "fp32", 2048, {}), ("tensor-1000", "tensor", 1000, SERIAL),
-           ("tensor-2048", "tensor", 2048, SERIAL), ("tensor-1000-overlap", "tensor", 1000, OVERLAP)]
+# (id, network mode, streams, overlap); 1000 is not a multiple of the 128-row tile.  overlap: the state operations (the
+# resets of a grow included) go to a non-blocking stream of their own, beside the streams the calls run on.
+CONFIGS = [("fp32-1000", "fp32", 1000, False), ("fp32-2048", "fp32", 2048, False), ("tensor-1000", "tensor", 1000, False),
+           ("tensor-2048", "tensor", 2048, False), ("tensor-1000-overlap", "tensor", 1000, True)]
 IDS = [c[0] for c in CONFIGS]
 
 
@@ -33,16 +34,16 @@ def _to_i16(x):
     return np.clip(np.rint(x * 16384.0), -32768, 32767).astype(np.int16)
 
 
-def _resize(a, b, n_old, n):
+def _resize(a, b, n_old, n, stream=0):
     """a goes to n active slots; its full-range twin b resets the slots that enter."""
-    a.set_active(n)
+    a.set_active(n, stream)
     if n > n_old:
-        b.reset_streams(np.arange(n_old, n))
+        b.reset_streams(np.arange(n_old, n), stream)
 
 
 def _twins(api, model0, cfg):
-    _, mode, S, env = cfg
-    return _engine(api, model0, S, mode, env, Fm=FM), _engine(api, model0, S, mode, env, Fm=FM)
+    _, mode, S, _ = cfg
+    return _engine(api, model0, S, mode, Fm=FM), _engine(api, model0, S, mode, Fm=FM)
 
 
 @pytest.mark.parametrize("dtype", ["f32", "i16"])
@@ -54,9 +55,10 @@ def test_host_calls_match_full_range_twin(api, model0, cfg, dtype):
     if dtype == "i16":
         x = _to_i16(x)
     a, b = _twins(api, model0, cfg)
+    ops = _ops_stream(cfg)
     n_old, t = S, 0
     for n, F in sched:
-        _resize(a, b, n_old, n)
+        _resize(a, b, n_old, n, ops)
         assert a.active == n and b.active == S
         xc = np.ascontiguousarray(x[:, t * HOP:(t + F) * HOP])
         out_a, gr_a = a.process(xc[:n], want_gr=True)
@@ -79,11 +81,10 @@ def test_device_calls_match_full_range_twin(api, model0, cfg):
     x = torch.from_numpy(_inputs(S, sum(f for _, f in sched), 12)).cuda()
     a, b = _twins(api, model0, cfg)
     st = torch.cuda.current_stream().cuda_stream
+    ops = _ops_stream(cfg, st)
     n_old, t = S, 0
     for n, F in sched:
-        a.set_active(n, st)
-        if n > n_old:
-            b.reset_streams(np.arange(n_old, n), st)
+        _resize(a, b, n_old, n, ops)
         xa = x[:n, t * HOP:(t + F) * HOP].contiguous()
         xb = x[:, t * HOP:(t + F) * HOP].contiguous()
         oa, ob = torch.empty_like(xa), torch.empty_like(xb)
@@ -109,12 +110,11 @@ def test_submitted_calls_with_mixed_ranges_match_twin(api, model0, cfg):
     x = torch.from_numpy(_to_i16(_inputs(S, sum(f for _, f in sched), 13))).cuda()
     a, b = _twins(api, model0, cfg)
     st = torch.cuda.current_stream().cuda_stream
+    ops = _ops_stream(cfg, st)
     pending = []
     n_old, t = S, 0
     for k, (n, F) in enumerate(sched):
-        a.set_active(n, st)
-        if n > n_old:
-            b.reset_streams(np.arange(n_old, n), st)
+        _resize(a, b, n_old, n, ops)
         xa = x[:n, t * HOP:(t + F) * HOP].contiguous()
         xb = x[:, t * HOP:(t + F) * HOP].contiguous()
         oa, ob = torch.empty_like(xa), torch.empty_like(xb)
@@ -145,7 +145,7 @@ def test_compaction_keeps_live_streams_exact(api, model0, cfg):
     x = _inputs(S, F * (rounds + 1), 14)
     a, b = _twins(api, model0, cfg)
     rng = np.random.RandomState(3)
-    st = torch.cuda.current_stream().cuda_stream
+    st = _ops_stream(cfg, torch.cuda.current_stream().cuda_stream)
     blob = torch.empty((1, a.state_size), dtype=torch.uint8, device="cuda")
     n = S
     for r in range(rounds + 1):
@@ -173,7 +173,7 @@ def test_compaction_keeps_live_streams_exact(api, model0, cfg):
 def test_refused_arguments_leave_engine_usable(api, model0, mode):
     import torch
     S, n = 270, 200
-    e = _engine(api, model0, S, mode, SERIAL, Fm=8)   # 8 hops: output hop t carries input hop t-6
+    e = _engine(api, model0, S, mode, Fm=8)   # 8 hops: output hop t carries input hop t-6
     L, h = e.L, e.h
     assert L.pnb_active_streams(h) == S
     for bad in (0, -1, S + 1):

@@ -1,9 +1,6 @@
 """Stream slots recycled inside a running engine: pnb_reset_streams / pnb_export_states / pnb_import_states.  A reset slot
 is a fresh stream, an exported and imported stream continues bit for bit, the operations keep stream order with the
 calls around them, and bad blobs or arguments touch no other stream."""
-import contextlib
-import os
-
 import numpy as np
 import pytest
 
@@ -12,35 +9,25 @@ from test_gpu_parity import GR_RTOL, _inputs, api  # noqa: F401
 pytestmark = pytest.mark.gpu
 
 F = 8
-OVERLAP = {"PNB_OVERLAP": "2", "PNB_CHUNK": "4", "PNB_NET_SMS": "64"}   # calls of 8 hops: two chunks of 4
-SERIAL = {"PNB_OVERLAP": "0"}
-# (id, network mode, streams, environment at pnb_create); 270 is not a multiple of the 256-row tile pair
-CONFIGS = [("fp32-270", "fp32", 270, {}), ("tensor-270", "tensor", 270, SERIAL),
-           ("tensor-2048-overlap", "tensor", 2048, OVERLAP)]
+# (id, network mode, streams, overlap); 270 is not a multiple of the 256-row tile pair.  overlap: the state operations go
+# to a non-blocking stream of their own, which nothing but the engine orders with the streams its calls run on.
+CONFIGS = [("fp32-270", "fp32", 270, False), ("tensor-270", "tensor", 270, False),
+           ("tensor-2048-overlap", "tensor", 2048, True)]
 HOP = 480
 
 
-@contextlib.contextmanager
-def _env(env):
-    old = {k: os.environ.get(k) for k in env}
-    os.environ.update(env)
-    try:
-        yield
-    finally:
-        for k, v in old.items():
-            if v is None:
-                os.environ.pop(k, None)
-            else:
-                os.environ[k] = v
+def _ops_stream(cfg, default=0):
+    """The stream a config issues its state operations on."""
+    import torch
+    return torch.cuda.Stream().cuda_stream if cfg[3] else default
 
 
 def _flags(api, mode):
     return api.NN_FP32 if mode == "fp32" else api.NN_TENSOR
 
 
-def _engine(api, model, S, mode, env, Fm=F, flags=None):
-    with _env(env):
-        return api.Engine(S, Fm, model, _flags(api, mode) if flags is None else flags)
+def _engine(api, model, S, mode, Fm=F, flags=None):
+    return api.Engine(S, Fm, model, _flags(api, mode) if flags is None else flags)
 
 
 def _signal(S, n_calls, seed):
@@ -58,9 +45,9 @@ def _call(x, k):
     return np.ascontiguousarray(x[:, k * F * HOP:(k + 1) * F * HOP])
 
 
-def _blob_rows(api, e, idx):
+def _blob_rows(api, e, idx, stream=0):
     import torch
-    t = e.export_states(idx, None)
+    t = e.export_states(idx, None, stream=stream)
     torch.cuda.synchronize()
     return t.cpu().numpy()
 
@@ -68,13 +55,13 @@ def _blob_rows(api, e, idx):
 # ---------------------------------------------------------------------------------------------- 1
 @pytest.mark.parametrize("cfg", CONFIGS, ids=[c[0] for c in CONFIGS])
 def test_batched_export_matches_single_stream_export(api, model0, cfg):
-    _, mode, S, env = cfg
+    _, mode, S, _ = cfg
     x = _signal(S, 2, 1)
-    e = _engine(api, model0, S, mode, env)
+    e = _engine(api, model0, S, mode)
     e.process(_call(x, 0))
     e.process(_call(x, 1))
     idx = [0, 1, 137, S - 1]
-    got = _blob_rows(api, e, idx)
+    got = _blob_rows(api, e, idx, _ops_stream(cfg))
     assert got.shape == (4, e.state_size)
     for i, s in enumerate(idx):
         assert got[i].tobytes() == e.get_state(s), s
@@ -99,19 +86,19 @@ def test_batched_export_matches_single_stream_export_traindata(api):
 # ---------------------------------------------------------------------------------------------- 2
 @pytest.mark.parametrize("cfg", CONFIGS, ids=[c[0] for c in CONFIGS])
 def test_reset_stream_equals_fresh_stream(api, model0, cfg):
-    _, mode, S, env = cfg
+    _, mode, S, _ = cfg
     x = _signal(S, 4, 2)
     z = _signal(S, 2, 3)
     R = [0, 5, S - 1]
     y = x.copy()
     y[R, 2 * F * HOP:] = z[R]                      # from the third call on, the reset slots carry a new session
-    a = _engine(api, model0, S, mode, env)           # reset after two calls
-    b = _engine(api, model0, S, mode, env)           # no reset
-    c = _engine(api, model0, S, mode, env)           # fresh engine fed the new sessions
+    a = _engine(api, model0, S, mode)              # reset after two calls
+    b = _engine(api, model0, S, mode)              # no reset
+    c = _engine(api, model0, S, mode)              # fresh engine fed the new sessions
     for k in range(2):
         a.process(_call(y, k))
         b.process(_call(x, k))
-    a.reset_streams(R)                             # default stream; the next host call runs on the engine's own
+    a.reset_streams(R, stream=_ops_stream(cfg))    # the next host call runs on the engine's own stream
     for k in (2, 3):
         out_a, gr_a = a.process(_call(y, k), want_gr=True)
         out_b, gr_b = b.process(_call(x, k), want_gr=True)
@@ -126,24 +113,24 @@ def test_reset_stream_equals_fresh_stream(api, model0, cfg):
 
 
 # ---------------------------------------------------------------------------------------------- 3
-PAIRS = [("fp32-fp32", "fp32", "fp32", 300, {}), ("tensor-tensor", "tensor", "tensor", 2048, OVERLAP),
-         ("fp32-tensor", "fp32", "tensor", 2048, OVERLAP)]
+PAIRS = [("fp32-fp32", "fp32", "fp32", 300), ("tensor-tensor", "tensor", "tensor", 2048),
+         ("fp32-tensor", "fp32", "tensor", 2048)]
 
 
 @pytest.mark.parametrize("pair", PAIRS, ids=[p[0] for p in PAIRS])
 def test_import_moves_streams_exactly(api, model0, pair):
     import torch
-    _, mode_a, mode_b, S_b, env_b = pair
+    _, mode_a, mode_b, S_b = pair
     S_a = 270
     x = _signal(S_a, 3, 4)
     other = _signal(S_b, 1, 5) * np.float32(0.5)
-    a = _engine(api, model0, S_a, mode_a, SERIAL)
+    a = _engine(api, model0, S_a, mode_a)
     for k in range(2):
         a.process(_call(x, k))
     src, dst = [3, 100, S_a - 1], [S_b - 1, 0, 7]
     blobs = a.export_states(src, None)
     want, want_gr = a.process(_call(x, 2), want_gr=True)
-    b = _engine(api, model0, S_b, mode_b, env_b, Fm=10)  # other batch size, max_frames, hop count
+    b = _engine(api, model0, S_b, mode_b, Fm=10)  # other batch size, max_frames, hop count
     b.process(np.ascontiguousarray(other))
     b.import_states(dst, blobs)
     y = np.zeros((S_b, F * HOP), np.float32)
@@ -168,11 +155,11 @@ def test_device_blob_and_host_blob_interchange(api, model0):
     """A blob exported on the device is a pnb_set_state blob, and a pnb_get_state blob imports on the device."""
     import torch
     x = _signal(270, 2, 6)
-    a = _engine(api, model0, 270, "tensor", SERIAL)
+    a = _engine(api, model0, 270, "tensor")
     a.process(_call(x, 0))
     dev = a.export_states([11], None)[0].cpu().numpy().tobytes()
     host = a.get_state(12)
-    b = _engine(api, model0, 64, "tensor", SERIAL)
+    b = _engine(api, model0, 64, "tensor")
     b.set_state(3, dev)
     t = torch.from_numpy(np.frombuffer(host, np.uint8).copy()).cuda()[None]
     b.import_states([4], t)
@@ -184,10 +171,10 @@ def test_device_blob_and_host_blob_interchange(api, model0):
 
 
 # ---------------------------------------------------------------------------------------------- 4
-ORDER_CONFIGS = [("fp32-270", "fp32", 270, {}), ("tensor-2048-overlap", "tensor", 2048, OVERLAP)]
+ORDER_CONFIGS = [("fp32-270", "fp32", 270, False), ("tensor-2048-overlap", "tensor", 2048, True)]
 
 
-def _order_sequence(api, e, x, st, submitted):
+def _order_sequence(api, e, x, st, submitted, ops_st=None):
     """calls interleaved with reset / export / import; returns (outputs, exported blobs) as device tensors"""
     import torch
     S = e.n_streams
@@ -205,7 +192,7 @@ def _order_sequence(api, e, x, st, submitted):
             torch.cuda.synchronize()
 
     def op(fn, *args):
-        fn(*args, stream=st)
+        fn(*args, stream=st if ops_st is None else ops_st)
         if not submitted:
             torch.cuda.synchronize()
     call(0)
@@ -228,15 +215,15 @@ def _order_sequence(api, e, x, st, submitted):
 @pytest.mark.parametrize("cfg", ORDER_CONFIGS, ids=[c[0] for c in ORDER_CONFIGS])
 def test_state_operations_keep_stream_order(api, model0, cfg):
     import torch
-    _, mode, S, env = cfg
+    _, mode, S, _ = cfg
     x = _signal(S, 4, 7)
-    ref_e = _engine(api, model0, S, mode, SERIAL)
+    ref_e = _engine(api, model0, S, mode)
     ref = _order_sequence(api, ref_e, x, torch.cuda.current_stream().cuda_stream, submitted=False)
     ref_e.close()
-    e = _engine(api, model0, S, mode, env)
+    e = _engine(api, model0, S, mode)
     side = torch.cuda.Stream()
     with torch.cuda.stream(side):
-        got = _order_sequence(api, e, x, side.cuda_stream, submitted=True)
+        got = _order_sequence(api, e, x, side.cuda_stream, submitted=True, ops_st=_ops_stream(cfg, None))
     e.close()
     assert np.array_equal(ref[0], got[0])
     assert np.array_equal(ref[1], got[1])
@@ -247,26 +234,28 @@ def test_state_operations_keep_stream_order(api, model0, cfg):
 @pytest.mark.parametrize("cfg", CONFIGS, ids=[c[0] for c in CONFIGS])
 def test_bad_blobs_are_rejected(api, model0, cfg):
     import torch
-    _, mode, S, env = cfg
+    _, mode, S, _ = cfg
+    ops = _ops_stream(cfg)
     x = _signal(S, 2, 8)
-    e = _engine(api, model0, S, mode, env)
+    e = _engine(api, model0, S, mode)
     e.process(_call(x, 0))
     e.process(_call(x, 1))
-    fresh_e = _engine(api, model0, 16, mode, SERIAL)
+    fresh_e = _engine(api, model0, 16, mode)
     fresh = _blob_rows(api, fresh_e, [0])[0]
     fresh_e.close()
-    good = e.export_states([1, 2, 3], None)
+    good = e.export_states([1, 2, 3], None, stream=ops)
+    torch.cuda.synchronize()
     bad = good.clone()
     bad[0, 0] ^= 0xFF                                                   # magic
     h0 = 45880                                                          # offsetof(StreamState, h)
     bad[1, h0:h0 + 4] = torch.from_numpy(np.frombuffer(np.float32(2.0).tobytes(), np.uint8).copy()).cuda()
-    before = _blob_rows(api, e, np.arange(S))
+    before = _blob_rows(api, e, np.arange(S), ops)
     dst = [12, 10, 11]
-    e.import_states(dst, bad)
+    e.import_states(dst, bad, stream=ops)
     with pytest.raises(api.PnbError, match=r"stream 10\b" if mode == "tensor" else r"stream 12\b"):
         e.check()
     e.check()                                                           # reported once
-    after = _blob_rows(api, e, np.arange(S))
+    after = _blob_rows(api, e, np.arange(S), ops)
     assert after[12].tobytes() == fresh.tobytes()                       # bad magic: left fresh
     if mode == "tensor":
         assert after[10].tobytes() == fresh.tobytes()                   # GRU value 2.0: left fresh
@@ -280,7 +269,7 @@ def test_bad_blobs_are_rejected(api, model0, cfg):
 
 def test_rejection_names_lowest_slot(api, model0):
     import torch
-    e = _engine(api, model0, 270, "tensor", SERIAL)
+    e = _engine(api, model0, 270, "tensor")
     b = torch.zeros((2, e.state_size), dtype=torch.uint8, device="cuda")
     e.import_states([200, 30], b)
     with pytest.raises(api.PnbError, match=r"stream 30\b"):
@@ -293,10 +282,10 @@ def test_rejection_names_lowest_slot(api, model0):
 @pytest.mark.parametrize("cfg", CONFIGS[:2], ids=[c[0] for c in CONFIGS[:2]])
 def test_bad_arguments_are_refused(api, model0, cfg):
     import torch
-    _, mode, S, env = cfg
+    _, mode, S, _ = cfg
     x = _signal(S, 2, 9)
-    e = _engine(api, model0, S, mode, env)
-    ref = _engine(api, model0, S, mode, env)
+    e = _engine(api, model0, S, mode)
+    ref = _engine(api, model0, S, mode)
     out0 = e.process(_call(x, 0))[0]
     assert np.array_equal(out0, ref.process(_call(x, 0))[0])
     blobs = e.export_states([0, 1], None)

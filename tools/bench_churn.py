@@ -78,7 +78,6 @@ def run_churn(args):
     nn_mode = "fp32" if args.nn == "fp32" else "tensor"
     flags = api.NN_FP32 if nn_mode == "fp32" else api.NN_TENSOR
     eng = api.Engine(S, F, synth_model(0), flags)
-    ov = eng.overlap_info()
     n_buf = 3
     bufs = make_step_inputs(S, F, n_buf, 0, device)
     outs = [torch.empty_like(b) for b in bufs]
@@ -222,7 +221,7 @@ def run_churn(args):
         "metric": "stream_states_moved_per_sec", "value": value, "unit": "states/s", "n_gpus": 1, "steps": reps,
         "warmup": W, "higher_is_better": True, "dtype": "bytes (fp32 / bf16 / fp16 state as stored)", "data": "synthetic",
         "config": {"workload": f"export + import of all {S} streams per repetition ({nn_mode} engine, {F}-hop calls)",
-                   "streams": S, "frames_per_call": F, "nn": nn_mode, "schedule": ov,
+                   "streams": S, "frames_per_call": F, "nn": nn_mode,
                    "repetitions": reps, "export_ms": exp_ms / reps, "import_ms": imp_ms / reps},
         "card": card, "clocks": clocks, "roofline": roof, "serving": serving, "occupancy": occupancy}))
     return 0

@@ -4,9 +4,9 @@
     compute-sanitizer --tool racecheck python tools/sanitizer_smoke.py
 
 Exercises the fp32 path, the tensor path (one CTA pair's worth of streams), the post-filter, the int16 entry,
-the pipelined host entry, the training-data generator, the persistent fp32 GRU chain (both block sizes), the chunked
-overlap schedule with submitted calls, state export / import and the pitch-only kernel on tiny batches; prints a
-checksum per leg."""
+the pipelined host entry, the training-data generator, the persistent fp32 GRU chain (both block sizes), submitted
+calls on the chain's anti-diagonal unit order, state export / import and the pitch-only kernel on tiny batches; prints
+a checksum per leg."""
 import os
 import sys
 
@@ -19,7 +19,7 @@ from percepnet_b200.weights import synth_model  # noqa: E402
 
 
 def main():
-    legs = sys.argv[1:] or ["fp32", "tensor", "train", "fp32chain", "overlap", "pitch"]
+    legs = sys.argv[1:] or ["fp32", "tensor", "train", "fp32chain", "submit", "pitch"]
     m = synth_model(0)
     if "fp32" in legs:
         x = synth_pcm(5, 4, seed=3)
@@ -46,8 +46,7 @@ def main():
             e.set_state(0, blob)
             print("fp32chain", S, float(np.abs(o1).sum()), float(np.abs(o2).sum()), len(blob))
             e.close()
-    if "overlap" in legs:    # chunked schedule on the SM partition, submitted calls overlapping each other, anti-diagonal unit order
-        os.environ.update({"PNB_OVERLAP": "2", "PNB_CHUNK": "2", "PNB_NET_SMS": "64"})
+    if "submit" in legs:     # pipelined host calls in flight together, anti-diagonal unit order (few streams)
         S, F = 300, 6
         x = synth_pcm(S, 3 * F, seed=8)
         e = api.Engine(S, F, m, api.NN_TENSOR | api.CONV_WIDE)
@@ -55,10 +54,8 @@ def main():
         for k in range(3):
             e.submit(np.ascontiguousarray(x[:, k * F * 480:(k + 1) * F * 480]), outs[k])
         e.wait()
-        print("overlap", e.overlap_info(), [float(np.abs(o).sum()) for o in outs])
+        print("submit", [float(np.abs(o).sum()) for o in outs])
         e.close()
-        for k in ("PNB_OVERLAP", "PNB_CHUNK", "PNB_NET_SMS"):
-            os.environ.pop(k)
     if "pitch" in legs:
         buf = synth_pcm(40, 4, seed=12)[:, :1728].copy()
         r = api.pitch_only(buf, np.zeros(40, np.int32), np.zeros(40, np.float32))

@@ -1,7 +1,6 @@
 #!/usr/bin/env python
-"""Launch timeline of two submitted long calls (calls overlapping each other): prints every launch with its start/end and the busy time
-of the network and DSP kernels.  Run on the GPU box: python tools/timeline.py [streams] [frames]; PNB_OVERLAP=2 for the chunked
-schedule on two SM partitions (the default is the serial schedule)."""
+"""Launch timeline of two submitted long calls: prints every launch with its start/end and the busy time of the network
+and DSP kernels.  Run on the GPU box: python tools/timeline.py [streams] [frames]."""
 import json
 import os
 import sys
@@ -29,7 +28,7 @@ def main():
     eng.profile(True)
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record(st)
-    for i in range(2):   # two submitted calls: the second call's analysis overlaps the first call's network tail
+    for i in range(2):
         eng.submit_device(bufs[i].data_ptr(), bufs[i].stride(0), outs[i].data_ptr(), outs[i].stride(0), F, stream=st.cuda_stream)
     eng.flush(st.cuda_stream)
     e1.record(st)
@@ -39,7 +38,7 @@ def main():
     net = {"tc_gemm_kernel", "tc_aux_kernel"}
     rows = [{"k": k, "t0": round(a, 3), "t1": round(b, 3), "part": "net" if k in net else "dsp"} for k, a, b in tl]
     busy = {"net": sum(r["t1"] - r["t0"] for r in rows if r["part"] == "net"), "dsp": sum(r["t1"] - r["t0"] for r in rows if r["part"] == "dsp")}
-    print(json.dumps({"two_calls_ms": e0.elapsed_time(e1), "span_ms": max(r["t1"] for r in rows), "busy_ms": busy, "info": eng.overlap_info(), "launches": rows}))
+    print(json.dumps({"two_calls_ms": e0.elapsed_time(e1), "span_ms": max(r["t1"] for r in rows), "busy_ms": busy, "launches": rows}))
     eng.close()
 
 

@@ -300,8 +300,7 @@ extern "C" void pnb_destroy(pnb_engine *e) {
   tc_release(e);
   float *fl[] = {e->fc.W, e->fc.b, e->conv1.W, e->conv1.b, e->conv2.W, e->conv2.b, e->fc_gb.W, e->fc_gb.b,
                  e->fc_rb.W, e->fc_rb.b, e->d_pcm, e->d_synth, e->d_last_gain, e->d_feat, e->d_Ex, e->d_gr,
-                 e->d_tap_pitchf, e->d_tap_g, e->ring_fc, e->ring_c1, e->c2, e->c2_all, e->d_hin, e->d_hout,
-                 e->d_raw, e->d_records};
+                 e->d_tap_pitchf, e->d_tap_g, e->ring_fc, e->ring_c1, e->c2, e->c2_all, e->d_raw};
   for (float *p : fl) if (p) cudaFree(p);
   for (int i = 0; i < 5; i++) {
     if (e->gru[i].W) cudaFree(e->gru[i].W);
@@ -327,11 +326,9 @@ extern "C" void pnb_destroy(pnb_engine *e) {
   if (e->ev_call) cudaEventDestroy(e->ev_call);
   if (e->d_tap_pitch) cudaFree(e->d_tap_pitch);
   if (e->d_tab) cudaFree(e->d_tab);
-  if (e->d_hin16) cudaFree(e->d_hin16);
-  if (e->d_hout16) cudaFree(e->d_hout16);
   for (int k = 0; k < 2; k++) {
-    if (e->pipe_in[k]) cudaFree(e->pipe_in[k]);
-    if (e->pipe_out[k]) cudaFree(e->pipe_out[k]);
+    if (e->stage[k].in) cudaFree(e->stage[k].in);
+    if (e->stage[k].out) cudaFree(e->stage[k].out);
     if (e->ev_in[k]) cudaEventDestroy(e->ev_in[k]);
     if (e->ev_cmp[k]) cudaEventDestroy(e->ev_cmp[k]);
     if (e->ev_out[k]) cudaEventDestroy(e->ev_out[k]);
@@ -596,58 +593,89 @@ static int mark_call_end(pnb_engine *e, cudaStream_t st) {
   return PNB_OK;
 }
 
-// Enqueues one call on st.  Host-side stream state (hop counter, line offset, GRU buffer parity) is committed only after
-// every launch was accepted; a failure in between leaves work half-enqueued, so the engine is poisoned until pnb_reset.
-static int process_device_enqueue(pnb_engine *e, const float *d_in, const short *d_in16, size_t in_stride, float *d_out,
-                                  short *d_out16, size_t out_stride, int F, float *d_gr, cudaStream_t st, long long *n_out) {
-  const int S = e->S, na = e->n_active;  // the call advances streams [0, na); per-call buffers keep the stride S
-  long long n = 0;
-  { int rc = wait_last_call(e, st); if (rc) return rc; }
-  { ProfScope ps(e, PNB_K_STAGE_IN, st); n += launch_stage_in(e->d_pcm + e->line_off, e->pcm_stride, d_in, d_in16, in_stride, na, F * kFrame, st); }
-  { ProfScope ps(e, PNB_K_ANALYSIS, st); n += launch_analysis(analysis_args(e, F), st); }
-  CK(cudaGetLastError());
-  if (e->flags & PNB_NN_TENSOR) {
-    const int q = tc_network(e, F, st);
-    if (q < 0) return q;
-    n += q;
-  } else {
-    for (int h0 = 0; h0 < F; h0 += e->f32_chunk) {
-      const int q = nn_chunk_f32(e, h0, F - h0 < e->f32_chunk ? F - h0 : e->f32_chunk, st);
-      if (q < 0) return q;
-      n += q;
-    }
-  }
-  { ProfScope ps(e, PNB_K_SYNTHESIS, st); n += launch_synthesis(synthesis_args(e, F, d_out, d_out16, out_stride), st); }
-  n += advance_line(e, F, st);
-  if (d_gr)  // [F][na][68] from the [F][S][68] buffer
-    CK(cudaMemcpy2DAsync(d_gr, (size_t)na * 68 * sizeof(float), e->d_gr, (size_t)S * 68 * sizeof(float), (size_t)na * 68 * sizeof(float), F,
-                         cudaMemcpyDeviceToDevice, st));
-  { int rc = mark_call_end(e, st); if (rc) return rc; }
-  CK(cudaGetLastError());
-  *n_out = n;
+// What every call checks before it allocates or enqueues anything: an engine of the call's family (training records
+// or enhancement) that no failed call has poisoned, 1 <= F <= Fmax, its buffers (`buffers`: none is NULL), and two
+// row strides of at least F hops.
+static int check_call(const pnb_engine *e, bool train, bool buffers, int F, size_t stride_a, size_t stride_b) {
+  if (!e) return fail(PNB_ERR_ARG, "engine is NULL");
+  if (train && !(e->flags & PNB_TRAIN_DATA)) return fail(PNB_ERR_ARG, "engine was not created with PNB_TRAIN_DATA");
+  if (!train && (e->flags & PNB_TRAIN_DATA))
+    return fail(PNB_ERR_ARG, "engine was created with PNB_TRAIN_DATA: use pnb_train_records_* / pnb_submit_train_records");
+  if (e->poisoned) return fail(PNB_ERR_CUDA, "an earlier call failed while enqueuing work; the streams' state is undefined until pnb_reset");
+  if (F < 1 || F > e->Fmax) return fail(PNB_ERR_ARG, "n_frames %d outside [1, %d]", F, e->Fmax);
+  if (!buffers) return fail(PNB_ERR_ARG, train ? "speech/noisy/records pointer is NULL" : "input/output pointer is NULL");
+  if (stride_a < (size_t)F * kFrame || stride_b < (size_t)F * kFrame) return fail(PNB_ERR_ARG, "row stride smaller than n_frames*480");
+  return PNB_OK;
+}
+static int check_train(const pnb_engine *e, const short *speech, size_t speech_stride, const short *noisy, size_t noisy_stride,
+                       int F, const float *records, size_t records_stride) {
+  const int rc = check_call(e, true, speech && noisy && records, F, speech_stride, noisy_stride);
+  if (rc) return rc;
+  if (records_stride < (size_t)F * PNB_RECORD_FLOATS) return fail(PNB_ERR_ARG, "records_stride smaller than n_frames*138");
   return PNB_OK;
 }
 
-static int process_device(pnb_engine *e, const float *d_in, const short *d_in16, size_t in_stride, float *d_out,
-                          short *d_out16, size_t out_stride, int F, float *d_gr, cudaStream_t st) {
-  if (!e) return fail(PNB_ERR_ARG, "engine is NULL");
-  if (e->flags & PNB_TRAIN_DATA) return fail(PNB_ERR_ARG, "engine was created with PNB_TRAIN_DATA: use pnb_train_records_*");
-  if (e->poisoned) return fail(PNB_ERR_CUDA, "an earlier call failed while enqueuing work; the streams' state is undefined until pnb_reset");
-  if (F < 1 || F > e->Fmax) return fail(PNB_ERR_ARG, "n_frames %d outside [1, %d]", F, e->Fmax);
-  if ((!d_in && !d_in16) || (!d_out && !d_out16)) return fail(PNB_ERR_ARG, "input/output pointer is NULL");
-  if (in_stride < (size_t)F * kFrame || out_stride < (size_t)F * kFrame)
-    return fail(PNB_ERR_ARG, "row stride smaller than n_frames*480");
-  CK(cudaSetDevice(e->device));
-  long long n = 0;
-  const int rc = process_device_enqueue(e, d_in, d_in16, in_stride, d_out, d_out16, out_stride, F, d_gr, st, &n);
-  if (rc) {
+// The call's own launches, in ev_call's order; returns their count or a negative error.
+template <typename Launches>
+static int enqueue_ordered(pnb_engine *e, cudaStream_t st, Launches launches) {
+  { int rc = wait_last_call(e, st); if (rc) return rc; }
+  const int n = launches();
+  if (n < 0) return n;
+  { int rc = mark_call_end(e, st); if (rc) return rc; }
+  CK(cudaGetLastError());
+  return n;
+}
+// Enqueues one call of F hops on st (arguments already checked) and commits the hop counter, last_frames and the launch
+// count when all of it was accepted.  The enqueue itself moves host-side stream state (advance_line the line offset,
+// the tensor carry the GRU buffer parity), so a failure after it started leaves the streams' state undefined: the
+// engine is poisoned, and refuses calls until pnb_reset.
+template <typename Launches>
+static int enqueue_call(pnb_engine *e, int F, cudaStream_t st, Launches launches) {
+  const int n = enqueue_ordered(e, st, launches);
+  if (n < 0) {
     e->poisoned = true;
-    return rc;
+    return n;
   }
   e->hop += F;
   e->last_frames = F;
   e->launches += n;
   return PNB_OK;
+}
+
+// One enhancement call on st (arguments already checked).
+static int enqueue_enhance(pnb_engine *e, const float *d_in, const short *d_in16, size_t in_stride, float *d_out,
+                           short *d_out16, size_t out_stride, int F, float *d_gr, cudaStream_t st) {
+  return enqueue_call(e, F, st, [&]() -> int {
+    const int S = e->S, na = e->n_active;  // the call advances streams [0, na); per-call buffers keep the stride S
+    int n = 0;
+    { ProfScope ps(e, PNB_K_STAGE_IN, st); n += launch_stage_in(e->d_pcm + e->line_off, e->pcm_stride, d_in, d_in16, in_stride, na, F * kFrame, st); }
+    { ProfScope ps(e, PNB_K_ANALYSIS, st); n += launch_analysis(analysis_args(e, F), st); }
+    CK(cudaGetLastError());
+    if (e->flags & PNB_NN_TENSOR) {
+      const int q = tc_network(e, F, st);
+      if (q < 0) return q;
+      n += q;
+    } else {
+      for (int h0 = 0; h0 < F; h0 += e->f32_chunk) {
+        const int q = nn_chunk_f32(e, h0, F - h0 < e->f32_chunk ? F - h0 : e->f32_chunk, st);
+        if (q < 0) return q;
+        n += q;
+      }
+    }
+    { ProfScope ps(e, PNB_K_SYNTHESIS, st); n += launch_synthesis(synthesis_args(e, F, d_out, d_out16, out_stride), st); }
+    n += advance_line(e, F, st);
+    if (d_gr)  // [F][na][68] from the [F][S][68] buffer
+      CK(cudaMemcpy2DAsync(d_gr, (size_t)na * 68 * sizeof(float), e->d_gr, (size_t)S * 68 * sizeof(float), (size_t)na * 68 * sizeof(float), F,
+                           cudaMemcpyDeviceToDevice, st));
+    return n;
+  });
+}
+
+static int process_device(pnb_engine *e, const float *d_in, const short *d_in16, size_t in_stride, float *d_out,
+                          short *d_out16, size_t out_stride, int F, float *d_gr, cudaStream_t st) {
+  { int rc = check_call(e, false, (d_in || d_in16) && (d_out || d_out16), F, in_stride, out_stride); if (rc) return rc; }
+  CK(cudaSetDevice(e->device));
+  return enqueue_enhance(e, d_in, d_in16, in_stride, d_out, d_out16, out_stride, F, d_gr, st);
 }
 
 extern "C" int pnb_process_device_f32(pnb_engine *e, const float *d_in, size_t in_stride, float *d_out,
@@ -664,70 +692,134 @@ extern "C" int pnb_process_device_i16(pnb_engine *e, const short *d_in, size_t i
 // ------------------------------------------------------------------------------------------
 // training-data generator (row f1): stage both files of every pair, analysis over 2N streams, labels
 // ------------------------------------------------------------------------------------------
+// One training-record call on st (arguments already checked).
+static int enqueue_records(pnb_engine *e, const short *d_speech, size_t speech_stride, const short *d_noisy,
+                           size_t noisy_stride, int F, float *d_records, size_t records_stride, cudaStream_t st) {
+  return enqueue_call(e, F, st, [&]() -> int {
+    const int N = e->S / 2;
+    float *line = e->d_pcm + e->line_off;
+    int n = 0;
+    {
+      ProfScope ps(e, PNB_K_STAGE_IN, st);
+      n += launch_stage_in(line, e->pcm_stride, nullptr, d_noisy, noisy_stride, N, F * kFrame, st, 1.f);
+      n += launch_stage_in(line + (size_t)N * e->pcm_stride, e->pcm_stride, nullptr, d_speech, speech_stride, N, F * kFrame, st, 1.f);
+    }
+    AnalysisArgs a = analysis_args(e, F);  // all S streams: the active range of a training-data engine is always S
+    a.raw = e->d_raw;
+    { ProfScope ps(e, PNB_K_ANALYSIS, st); n += launch_analysis(a, st); }
+    LabelArgs l;
+    l.feat = e->d_feat; l.raw = e->d_raw; l.Ex = e->d_Ex; l.tab = e->d_tab; l.n_pairs = N; l.n_frames = F;
+    l.records = d_records; l.pair_stride = records_stride;
+    { ProfScope ps(e, PNB_K_LABELS, st); n += launch_train_labels(l, st); }
+    n += advance_line(e, F, st);
+    return n;
+  });
+}
+
 extern "C" int pnb_train_records_device(pnb_engine *e, const short *d_speech, size_t speech_stride,
                                         const short *d_noisy, size_t noisy_stride, int F, float *d_records,
                                         size_t records_stride, void *cuda_stream) {
-  if (!e) return fail(PNB_ERR_ARG, "engine is NULL");
-  if (!(e->flags & PNB_TRAIN_DATA)) return fail(PNB_ERR_ARG, "engine was not created with PNB_TRAIN_DATA");
-  if (F < 1 || F > e->Fmax) return fail(PNB_ERR_ARG, "n_frames %d outside [1, %d]", F, e->Fmax);
-  if (!d_speech || !d_noisy || !d_records) return fail(PNB_ERR_ARG, "speech/noisy/records pointer is NULL");
-  if (speech_stride < (size_t)F * kFrame || noisy_stride < (size_t)F * kFrame)
-    return fail(PNB_ERR_ARG, "row stride smaller than n_frames*480");
-  if (records_stride < (size_t)F * PNB_RECORD_FLOATS) return fail(PNB_ERR_ARG, "records_stride smaller than n_frames*138");
+  { int rc = check_train(e, d_speech, speech_stride, d_noisy, noisy_stride, F, d_records, records_stride); if (rc) return rc; }
   CK(cudaSetDevice(e->device));
-  cudaStream_t st = (cudaStream_t)cuda_stream;
-  const int S = e->S, N = S / 2;
-  long long n = 0;
-  float *line = e->d_pcm + e->line_off;
-  { int rc = wait_last_call(e, st); if (rc) return rc; }
-  {
-    ProfScope ps(e, PNB_K_STAGE_IN, st);
-    n += launch_stage_in(line, e->pcm_stride, nullptr, d_noisy, noisy_stride, N, F * kFrame, st, 1.f);
-    n += launch_stage_in(line + (size_t)N * e->pcm_stride, e->pcm_stride, nullptr, d_speech, speech_stride, N, F * kFrame, st, 1.f);
-  }
-  AnalysisArgs a;
-  a.pcm = line; a.pcm_stride = e->pcm_stride; a.n_streams = S; a.stride = S; a.n_frames = F; a.tab = e->d_tab;
-  a.feat = e->d_feat; a.zring = e->d_zring; a.ering = e->d_ering; a.ring = e->ring; a.hop0 = e->hop;
-  a.P = nullptr; a.Ex = e->d_Ex; a.raw = e->d_raw; a.silence = e->d_sil;
-  a.last_period = e->d_last_period; a.last_gain = e->d_last_gain;
-  a.tap_pitch = e->d_tap_pitch; a.tap_pitchf = e->d_tap_pitchf;
-  { ProfScope ps(e, PNB_K_ANALYSIS, st); n += launch_analysis(a, st); }
-  LabelArgs l;
-  l.feat = e->d_feat; l.raw = e->d_raw; l.Ex = e->d_Ex; l.tab = e->d_tab; l.n_pairs = N; l.n_frames = F;
-  l.records = d_records; l.pair_stride = records_stride;
-  { ProfScope ps(e, PNB_K_LABELS, st); n += launch_train_labels(l, st); }
-  n += advance_line(e, F, st);
-  { int rc = mark_call_end(e, st); if (rc) return rc; }
-  CK(cudaGetLastError());
-  e->hop += F;
-  e->last_frames = F;
-  e->launches += n;
+  return enqueue_records(e, d_speech, speech_stride, d_noisy, noisy_stride, F, d_records, records_stride, (cudaStream_t)cuda_stream);
+}
+
+// ------------------------------------------------------------------------------------------
+// host-buffer calls: device staging, and the pipeline in which the H2D of call i+1 and the D2H of call i-1 overlap the
+// kernels of call i
+// ------------------------------------------------------------------------------------------
+// Buffers of at least `bytes`: a slot grows, never shrinks.  The slot is idle when this runs.
+static int grow(void **buf, size_t *cap, size_t bytes) {
+  if (*cap >= bytes) return PNB_OK;
+  if (*buf) CK(cudaFree(*buf));
+  *buf = nullptr;
+  *cap = 0;
+  CK(cudaMalloc(buf, bytes));
+  *cap = bytes;
   return PNB_OK;
 }
 
-extern "C" int pnb_train_records_host(pnb_engine *e, const short *speech, size_t speech_stride, const short *noisy,
-                                      size_t noisy_stride, int F, float *records, size_t records_stride) {
-  if (!e) return fail(PNB_ERR_ARG, "engine is NULL");
-  if (!(e->flags & PNB_TRAIN_DATA)) return fail(PNB_ERR_ARG, "engine was not created with PNB_TRAIN_DATA");
-  if (!speech || !noisy || !records) return fail(PNB_ERR_ARG, "speech/noisy/records pointer is NULL");
-  if (F < 1 || F > e->Fmax) return fail(PNB_ERR_ARG, "n_frames %d outside [1, %d]", F, e->Fmax);
-  if (speech_stride < (size_t)F * kFrame || noisy_stride < (size_t)F * kFrame)
-    return fail(PNB_ERR_ARG, "row stride smaller than n_frames*480");
-  if (records_stride < (size_t)F * PNB_RECORD_FLOATS) return fail(PNB_ERR_ARG, "records_stride smaller than n_frames*138");
+// The staging slot of a host-buffer call: k = submitted & 1, the slot the next pipelined call takes.  Only pipelined
+// calls advance `submitted`, so a blocking call borrows that slot, and an engine that only makes blocking calls uses
+// slot 0 alone.  Creates the copy streams and their events for the first pipelined call: blocking calls do not use
+// them, and with them created a blocking 16-stream tensor engine took about 15 us (4 %) longer per call (H100 80GB HBM3,
+// 700 W).  Waits until the slot's last pipelined round trip is complete, and grows its buffers to in_bytes / out_bytes.
+// Callers size them for an Fmax-hop call, so a slot grows at most once however f32, int16, blocking and pipelined calls
+// mix.  Returns k or a negative error.
+static int staging_slot(pnb_engine *e, bool pipelined, size_t in_bytes, size_t out_bytes) {
+  if (pipelined && !e->s_in) {
+    CK(cudaStreamCreateWithFlags(&e->s_in, cudaStreamNonBlocking));
+    CK(cudaStreamCreateWithFlags(&e->s_out, cudaStreamNonBlocking));
+    for (int k = 0; k < 2; k++) {
+      CK(cudaEventCreateWithFlags(&e->ev_in[k], cudaEventDisableTiming));
+      CK(cudaEventCreateWithFlags(&e->ev_cmp[k], cudaEventDisableTiming));
+      CK(cudaEventCreateWithFlags(&e->ev_out[k], cudaEventDisableTiming));
+    }
+  }
+  const int k = (int)(e->submitted & 1);
+  if (e->submitted >= 2) CK(cudaEventSynchronize(e->ev_out[k]));  // the slot's last pipelined round trip is complete
+  pnb_engine::Staging &s = e->stage[k];
+  { int rc = grow(&s.in, &s.in_bytes, in_bytes); if (rc) return rc; }
+  { int rc = grow(&s.out, &s.out_bytes, out_bytes); if (rc) return rc; }
+  return k;
+}
+
+// One round trip through staging slot k: h2d(stream) copies the input into the slot, call() enqueues the call on the
+// engine's stream, d2h(stream) copies the output back.  Pipelined, the copies go to s_in / s_out, the slot's events
+// order them with the call, and the round trip is left in flight.  Blocking, all of it goes to the engine's stream, for
+// the caller to synchronise.
+template <typename H2D, typename Call, typename D2H>
+static int round_trip(pnb_engine *e, int k, bool pipelined, H2D h2d, Call call, D2H d2h) {
+  CK(h2d(pipelined ? e->s_in : e->stream));
+  if (pipelined) {
+    CK(cudaEventRecord(e->ev_in[k], e->s_in));
+    CK(cudaStreamWaitEvent(e->stream, e->ev_in[k], 0));
+  }
+  { int rc = call(); if (rc) return rc; }
+  if (pipelined) {
+    CK(cudaEventRecord(e->ev_cmp[k], e->stream));
+    CK(cudaStreamWaitEvent(e->s_out, e->ev_cmp[k], 0));
+  }
+  CK(d2h(pipelined ? e->s_out : e->stream));
+  if (pipelined) {
+    CK(cudaEventRecord(e->ev_out[k], e->s_out));
+    e->submitted++;
+  }
+  return PNB_OK;
+}
+
+// pnb_train_records_host (blocking) and pnb_submit_train_records (pipelined)
+static int records_host(pnb_engine *e, const short *speech, size_t speech_stride, const short *noisy, size_t noisy_stride,
+                        int F, float *records, size_t records_stride, bool pipelined) {
+  { int rc = check_train(e, speech, speech_stride, noisy, noisy_stride, F, records, records_stride); if (rc) return rc; }
   CK(cudaSetDevice(e->device));
   const size_t N = e->S / 2, row = (size_t)e->Fmax * kFrame, rrow = (size_t)e->Fmax * PNB_RECORD_FLOATS;
-  if (!e->d_hin16) CK(cudaMalloc((void **)&e->d_hin16, 2 * N * row * sizeof(short)));
-  if (!e->d_records) CK(cudaMalloc((void **)&e->d_records, N * rrow * sizeof(float)));
   const size_t w = (size_t)F * kFrame * sizeof(short);
-  short *d_noisy = e->d_hin16, *d_speech = e->d_hin16 + N * row;
-  CK(cudaMemcpy2DAsync(d_noisy, row * 2, noisy, noisy_stride * 2, w, N, cudaMemcpyHostToDevice, e->stream));
-  CK(cudaMemcpy2DAsync(d_speech, row * 2, speech, speech_stride * 2, w, N, cudaMemcpyHostToDevice, e->stream));
-  int rc = pnb_train_records_device(e, d_speech, row, d_noisy, row, F, e->d_records, rrow, e->stream);
-  if (rc) return rc;
-  CK(cudaMemcpy2DAsync(records, records_stride * 4, e->d_records, rrow * 4, (size_t)F * PNB_RECORD_FLOATS * 4, N,
-                       cudaMemcpyDeviceToHost, e->stream));
+  const int k = staging_slot(e, pipelined, 2 * N * row * sizeof(short), N * rrow * sizeof(float));
+  if (k < 0) return k;
+  short *d_noisy = (short *)e->stage[k].in, *d_speech = d_noisy + N * row;
+  float *d_rec = (float *)e->stage[k].out;
+  const int rc = round_trip(e, k, pipelined,
+      [&](cudaStream_t s) {
+        const cudaError_t ce = cudaMemcpy2DAsync(d_noisy, row * 2, noisy, noisy_stride * 2, w, N, cudaMemcpyHostToDevice, s);
+        return ce != cudaSuccess ? ce : cudaMemcpy2DAsync(d_speech, row * 2, speech, speech_stride * 2, w, N, cudaMemcpyHostToDevice, s);
+      },
+      [&] { return enqueue_records(e, d_speech, row, d_noisy, row, F, d_rec, rrow, e->stream); },
+      [&](cudaStream_t s) {
+        return cudaMemcpy2DAsync(records, records_stride * 4, d_rec, rrow * 4, (size_t)F * PNB_RECORD_FLOATS * 4, N,
+                                 cudaMemcpyDeviceToHost, s);
+      });
+  if (rc || pipelined) return rc;
   CK(cudaStreamSynchronize(e->stream));
   return PNB_OK;
+}
+extern "C" int pnb_train_records_host(pnb_engine *e, const short *speech, size_t speech_stride, const short *noisy,
+                                      size_t noisy_stride, int F, float *records, size_t records_stride) {
+  return records_host(e, speech, speech_stride, noisy, noisy_stride, F, records, records_stride, false);
+}
+extern "C" int pnb_submit_train_records(pnb_engine *e, const short *speech, size_t speech_stride, const short *noisy,
+                                        size_t noisy_stride, int F, float *records, size_t records_stride) {
+  return records_host(e, speech, speech_stride, noisy, noisy_stride, F, records, records_stride, true);
 }
 
 // after the stream that carried the status copy was synchronised
@@ -749,29 +841,25 @@ static int report_status(pnb_engine *e) {
   return PNB_OK;
 }
 
+// pnb_process_host_* (blocking) and pnb_submit_host_* (pipelined).  The blocking form then copies g/r and the status
+// word back on the engine's stream too, and synchronises it once.
 template <typename T>
-static int process_host(pnb_engine *e, const T *in, size_t in_stride, T *out, size_t out_stride, int F, float *gr,
-                        T **d_in_p, T **d_out_p) {
-  if (!e) return fail(PNB_ERR_ARG, "engine is NULL");
-  if (e->flags & PNB_TRAIN_DATA) return fail(PNB_ERR_ARG, "engine was created with PNB_TRAIN_DATA: use pnb_train_records_*");
-  if (!in || !out) return fail(PNB_ERR_ARG, "input/output pointer is NULL");
-  if (F < 1 || F > e->Fmax) return fail(PNB_ERR_ARG, "n_frames %d outside [1, %d]", F, e->Fmax);
-  if (in_stride < (size_t)F * kFrame || out_stride < (size_t)F * kFrame)
-    return fail(PNB_ERR_ARG, "row stride smaller than n_frames*480");
+static int host_call(pnb_engine *e, const T *in, size_t in_stride, T *out, size_t out_stride, int F, float *gr, bool pipelined) {
+  { int rc = check_call(e, false, in && out, F, in_stride, out_stride); if (rc) return rc; }
   CK(cudaSetDevice(e->device));
-  const size_t S = e->S, row = (size_t)e->Fmax * kFrame;
-  if (!*d_in_p) CK(cudaMalloc((void **)d_in_p, S * row * sizeof(T)));
-  if (!*d_out_p) CK(cudaMalloc((void **)d_out_p, S * row * sizeof(T)));
-  const size_t w = (size_t)F * kFrame * sizeof(T);
+  const size_t S = e->S, row = (size_t)e->Fmax * kFrame, w = (size_t)F * kFrame * sizeof(T);
   const size_t na = e->n_active;  // the rows of in / out / gr
-  CK(cudaMemcpy2DAsync(*d_in_p, row * sizeof(T), in, in_stride * sizeof(T), w, na, cudaMemcpyHostToDevice, e->stream));
-  int rc;
-  if (sizeof(T) == 4)
-    rc = process_device(e, (const float *)*d_in_p, nullptr, row, (float *)*d_out_p, nullptr, row, F, nullptr, e->stream);
-  else
-    rc = process_device(e, nullptr, (const short *)*d_in_p, row, nullptr, (short *)*d_out_p, row, F, nullptr, e->stream);
-  if (rc) return rc;
-  CK(cudaMemcpy2DAsync(out, out_stride * sizeof(T), *d_out_p, row * sizeof(T), w, na, cudaMemcpyDeviceToHost, e->stream));
+  const int k = staging_slot(e, pipelined, S * row * sizeof(T), S * row * sizeof(T));
+  if (k < 0) return k;
+  T *d_in = (T *)e->stage[k].in, *d_out = (T *)e->stage[k].out;
+  const int rc = round_trip(e, k, pipelined,
+      [&](cudaStream_t s) { return cudaMemcpy2DAsync(d_in, row * sizeof(T), in, in_stride * sizeof(T), w, na, cudaMemcpyHostToDevice, s); },
+      [&] {
+        return sizeof(T) == 4 ? enqueue_enhance(e, (const float *)d_in, nullptr, row, (float *)d_out, nullptr, row, F, nullptr, e->stream)
+                              : enqueue_enhance(e, nullptr, (const short *)d_in, row, nullptr, (short *)d_out, row, F, nullptr, e->stream);
+      },
+      [&](cudaStream_t s) { return cudaMemcpy2DAsync(out, out_stride * sizeof(T), d_out, row * sizeof(T), w, na, cudaMemcpyDeviceToHost, s); });
+  if (rc || pipelined) return rc;
   if (gr)
     CK(cudaMemcpy2DAsync(gr, na * 68 * sizeof(float), e->d_gr, S * 68 * sizeof(float), na * 68 * sizeof(float), F, cudaMemcpyDeviceToHost,
                          e->stream));
@@ -782,118 +870,19 @@ static int process_host(pnb_engine *e, const T *in, size_t in_stride, T *out, si
 
 extern "C" int pnb_process_host_f32(pnb_engine *e, const float *in, size_t in_stride, float *out, size_t out_stride,
                                     int n_frames, float *gr) {
-  return process_host<float>(e, in, in_stride, out, out_stride, n_frames, gr, &e->d_hin, &e->d_hout);
+  return host_call<float>(e, in, in_stride, out, out_stride, n_frames, gr, false);
 }
 extern "C" int pnb_process_host_i16(pnb_engine *e, const short *in, size_t in_stride, short *out, size_t out_stride,
                                     int n_frames, float *gr) {
-  return process_host<short>(e, in, in_stride, out, out_stride, n_frames, gr, &e->d_hin16, &e->d_hout16);
-}
-
-// ------------------------------------------------------------------------------------------
-// pipelined host entry: H2D of call i+1 and D2H of call i-1 overlap the kernels of call i
-// ------------------------------------------------------------------------------------------
-template <typename T>
-static int submit_host(pnb_engine *e, const T *in, size_t in_stride, T *out, size_t out_stride, int F) {
-  if (!e) return fail(PNB_ERR_ARG, "engine is NULL");
-  if (e->flags & PNB_TRAIN_DATA) return fail(PNB_ERR_ARG, "engine was created with PNB_TRAIN_DATA: use pnb_submit_train_records");
-  if (!in || !out) return fail(PNB_ERR_ARG, "input/output pointer is NULL");
-  if (F < 1 || F > e->Fmax) return fail(PNB_ERR_ARG, "n_frames %d outside [1, %d]", F, e->Fmax);
-  if (in_stride < (size_t)F * kFrame || out_stride < (size_t)F * kFrame)
-    return fail(PNB_ERR_ARG, "row stride smaller than n_frames*480");
-  CK(cudaSetDevice(e->device));
-  const size_t S = e->S, row = (size_t)e->Fmax * kFrame;
-  if (!e->s_in) {
-    CK(cudaStreamCreateWithFlags(&e->s_in, cudaStreamNonBlocking));
-    CK(cudaStreamCreateWithFlags(&e->s_out, cudaStreamNonBlocking));
-    for (int k = 0; k < 2; k++) {
-      CK(cudaEventCreateWithFlags(&e->ev_in[k], cudaEventDisableTiming));
-      CK(cudaEventCreateWithFlags(&e->ev_cmp[k], cudaEventDisableTiming));
-      CK(cudaEventCreateWithFlags(&e->ev_out[k], cudaEventDisableTiming));
-    }
-  }
-  if (e->pipe_elem != sizeof(T)) {
-    CK(cudaDeviceSynchronize());
-    for (int k = 0; k < 2; k++) {
-      if (e->pipe_in[k]) cudaFree(e->pipe_in[k]);
-      if (e->pipe_out[k]) cudaFree(e->pipe_out[k]);
-      CK(cudaMalloc(&e->pipe_in[k], S * row * sizeof(T)));
-      CK(cudaMalloc(&e->pipe_out[k], S * row * sizeof(T)));
-    }
-    e->pipe_elem = sizeof(T);
-    e->submitted = 0;
-  }
-  const int k = (int)(e->submitted & 1);
-  if (e->submitted >= 2) CK(cudaEventSynchronize(e->ev_out[k]));  // the slot's previous round trip is complete
-  const size_t w = (size_t)F * kFrame * sizeof(T), na = e->n_active;  // the rows of in / out
-  CK(cudaMemcpy2DAsync(e->pipe_in[k], row * sizeof(T), in, in_stride * sizeof(T), w, na, cudaMemcpyHostToDevice, e->s_in));
-  CK(cudaEventRecord(e->ev_in[k], e->s_in));
-  CK(cudaStreamWaitEvent(e->stream, e->ev_in[k], 0));
-  int rc;
-  if (sizeof(T) == 4)
-    rc = process_device(e, (const float *)e->pipe_in[k], nullptr, row, (float *)e->pipe_out[k], nullptr, row, F, nullptr, e->stream);
-  else
-    rc = process_device(e, nullptr, (const short *)e->pipe_in[k], row, nullptr, (short *)e->pipe_out[k], row, F, nullptr, e->stream);
-  if (rc) return rc;
-  CK(cudaEventRecord(e->ev_cmp[k], e->stream));
-  CK(cudaStreamWaitEvent(e->s_out, e->ev_cmp[k], 0));
-  CK(cudaMemcpy2DAsync(out, out_stride * sizeof(T), e->pipe_out[k], row * sizeof(T), w, na, cudaMemcpyDeviceToHost, e->s_out));
-  CK(cudaEventRecord(e->ev_out[k], e->s_out));
-  e->submitted++;
-  return PNB_OK;
+  return host_call<short>(e, in, in_stride, out, out_stride, n_frames, gr, false);
 }
 extern "C" int pnb_submit_host_f32(pnb_engine *e, const float *in, size_t in_stride, float *out, size_t out_stride,
                                    int n_frames) {
-  return submit_host<float>(e, in, in_stride, out, out_stride, n_frames);
+  return host_call<float>(e, in, in_stride, out, out_stride, n_frames, nullptr, true);
 }
 extern "C" int pnb_submit_host_i16(pnb_engine *e, const short *in, size_t in_stride, short *out, size_t out_stride,
                                    int n_frames) {
-  return submit_host<short>(e, in, in_stride, out, out_stride, n_frames);
-}
-// pipelined twin of pnb_train_records_host: same slots, streams and events as submit_host
-extern "C" int pnb_submit_train_records(pnb_engine *e, const short *speech, size_t speech_stride, const short *noisy,
-                                        size_t noisy_stride, int F, float *records, size_t records_stride) {
-  if (!e) return fail(PNB_ERR_ARG, "engine is NULL");
-  if (!(e->flags & PNB_TRAIN_DATA)) return fail(PNB_ERR_ARG, "engine was not created with PNB_TRAIN_DATA");
-  if (!speech || !noisy || !records) return fail(PNB_ERR_ARG, "speech/noisy/records pointer is NULL");
-  if (F < 1 || F > e->Fmax) return fail(PNB_ERR_ARG, "n_frames %d outside [1, %d]", F, e->Fmax);
-  if (speech_stride < (size_t)F * kFrame || noisy_stride < (size_t)F * kFrame)
-    return fail(PNB_ERR_ARG, "row stride smaller than n_frames*480");
-  if (records_stride < (size_t)F * PNB_RECORD_FLOATS) return fail(PNB_ERR_ARG, "records_stride smaller than n_frames*138");
-  CK(cudaSetDevice(e->device));
-  const size_t N = e->S / 2, row = (size_t)e->Fmax * kFrame, rrow = (size_t)e->Fmax * PNB_RECORD_FLOATS;
-  if (!e->s_in) {
-    CK(cudaStreamCreateWithFlags(&e->s_in, cudaStreamNonBlocking));
-    CK(cudaStreamCreateWithFlags(&e->s_out, cudaStreamNonBlocking));
-    for (int k = 0; k < 2; k++) {
-      CK(cudaEventCreateWithFlags(&e->ev_in[k], cudaEventDisableTiming));
-      CK(cudaEventCreateWithFlags(&e->ev_cmp[k], cudaEventDisableTiming));
-      CK(cudaEventCreateWithFlags(&e->ev_out[k], cudaEventDisableTiming));
-    }
-  }
-  if (!e->pipe_in[0]) {
-    for (int k = 0; k < 2; k++) {
-      CK(cudaMalloc(&e->pipe_in[k], 2 * N * row * sizeof(short)));
-      CK(cudaMalloc(&e->pipe_out[k], N * rrow * sizeof(float)));
-    }
-    e->submitted = 0;
-  }
-  const int k = (int)(e->submitted & 1);
-  if (e->submitted >= 2) CK(cudaEventSynchronize(e->ev_out[k]));  // the slot's previous round trip is complete
-  short *d_noisy = (short *)e->pipe_in[k], *d_speech = d_noisy + N * row;
-  const size_t w = (size_t)F * kFrame * sizeof(short);
-  CK(cudaMemcpy2DAsync(d_noisy, row * 2, noisy, noisy_stride * 2, w, N, cudaMemcpyHostToDevice, e->s_in));
-  CK(cudaMemcpy2DAsync(d_speech, row * 2, speech, speech_stride * 2, w, N, cudaMemcpyHostToDevice, e->s_in));
-  CK(cudaEventRecord(e->ev_in[k], e->s_in));
-  CK(cudaStreamWaitEvent(e->stream, e->ev_in[k], 0));
-  int rc = pnb_train_records_device(e, d_speech, row, d_noisy, row, F, (float *)e->pipe_out[k], rrow, e->stream);
-  if (rc) return rc;
-  CK(cudaEventRecord(e->ev_cmp[k], e->stream));
-  CK(cudaStreamWaitEvent(e->s_out, e->ev_cmp[k], 0));
-  CK(cudaMemcpy2DAsync(records, records_stride * 4, e->pipe_out[k], rrow * 4, (size_t)F * PNB_RECORD_FLOATS * 4, N,
-                       cudaMemcpyDeviceToHost, e->s_out));
-  CK(cudaEventRecord(e->ev_out[k], e->s_out));
-  e->submitted++;
-  return PNB_OK;
+  return host_call<short>(e, in, in_stride, out, out_stride, n_frames, nullptr, true);
 }
 
 // pnb_process_device_* without g/r; both names are part of the ABI.

@@ -42,7 +42,6 @@ struct pnb_engine {
   float2 *d_P = nullptr;
   float *d_Ex = nullptr;
   float *d_raw = nullptr;     // [F][S][68] training-data mode only
-  float *d_records = nullptr; // [S/2][Fmax][138] staging of pnb_train_records_host
   unsigned char *d_sil = nullptr;
   float *d_gr = nullptr;
   int *d_tap_pitch = nullptr;
@@ -61,16 +60,16 @@ struct pnb_engine {
   int f32_rt = 8, f32_rb = 0;   // rows per thread of the chain kernel (8: 128-stream blocks, 1: 16-stream blocks); stream blocks
   long hop = 0;  // hops processed since reset
 
-  // staging for the host-buffer entry points
-  float *d_hin = nullptr, *d_hout = nullptr;
-  short *d_hin16 = nullptr, *d_hout16 = nullptr;
-
-  // pipelined host entry (pnb_submit_host_*): two slots of device staging, three streams
+  // Device staging of the host-buffer calls (pnb_process_host_*, pnb_submit_host_*, pnb_train_records_host,
+  // pnb_submit_train_records): two slots, each an input and an output buffer, allocated on first use and only ever
+  // grown.  Pipelined calls take slot submitted & 1 and copy on s_in / s_out (created for the first of them), ordered
+  // with the call on `stream` by the slot's events; blocking calls borrow the slot the next pipelined call will take and
+  // run on `stream` alone.
+  struct Staging { void *in = nullptr, *out = nullptr; size_t in_bytes = 0, out_bytes = 0; };
+  Staging stage[2];
   cudaStream_t s_in = nullptr, s_out = nullptr;
-  void *pipe_in[2] = {nullptr, nullptr}, *pipe_out[2] = {nullptr, nullptr};
-  size_t pipe_elem = 0;  // element size the staging was allocated for
   cudaEvent_t ev_in[2] = {nullptr, nullptr}, ev_cmp[2] = {nullptr, nullptr}, ev_out[2] = {nullptr, nullptr};
-  long long submitted = 0;
+  long long submitted = 0;  // pipelined calls so far
 
   pnb_tc_state *tc = nullptr;
   int last_frames = 0;

@@ -227,6 +227,20 @@ class Oracle:
     def sigmoid(self, x):
         return np.array([self.lib.pn_oracle_sigmoid(float(v)) for v in np.asarray(x, np.float32).ravel()], np.float32)
 
+    def _vec(self, fn, x):
+        a = np.ascontiguousarray(x, np.float32)
+        y = np.empty_like(a)
+        fn.argtypes = [F32P, F32P, C.c_long]
+        fn(a.ctypes.data_as(F32P), y.ctypes.data_as(F32P), a.size)
+        return y
+
+    def tansig_n(self, x):
+        """tansig_approx (vec.h:53-71) of every element, same shape; one call for the whole array."""
+        return self._vec(self.lib.pn_oracle_tansig_n, x)
+
+    def sigmoid_n(self, x):
+        return self._vec(self.lib.pn_oracle_sigmoid_n, x)
+
     def dense_layer(self, layer, x, n_out):
         x, xp = _f(x)
         out = np.empty(n_out, np.float32)
@@ -262,12 +276,17 @@ class Oracle:
                                        gain.ctypes.data_as(F32P), n_threads)
         return T, corr, gain
 
-    def rnn_f64(self, model, features):
+    NN_STATE = 512 + 1024 + 4 * 512 + 128  # [conv1 mem 4 x 128][conv2 mem 2 x 512][gru1 gru2 gru3 gru_gb][gru_rb]
+
+    def rnn_f64(self, model, features, state=None):
         """features [F, 70] of one stream -> (g [F, 34], r [F, 34] in float64, max |pre-activation| per frame):
-        the network in double precision from a zero state (pn_oracle_compute_rnn_f64)."""
+        the network in double precision (pn_oracle_compute_rnn_f64) from `state` ([NN_STATE], the conv memories
+        oldest first, then the five GRU states; not modified), or from a zero state."""
         feats = np.ascontiguousarray(features, dtype=np.float32)
         F = feats.shape[0]
-        st = np.zeros(512 + 1024 + 4 * 512 + 128, np.float64)
+        st = np.zeros(self.NN_STATE, np.float64)
+        if state is not None:
+            st[:] = np.asarray(state, np.float64).reshape(self.NN_STATE)
         g, r, mp = np.empty((F, 34), np.float64), np.empty((F, 34), np.float64), np.empty(F, np.float64)
         D = C.POINTER(C.c_double)
         self.lib.pn_oracle_compute_rnn_f64.restype = C.c_double

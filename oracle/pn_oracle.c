@@ -545,6 +545,15 @@ float pn_oracle_tansig(float x) { /* vec.h:53-71 */
   return sign * y;
 }
 float pn_oracle_sigmoid(float x) { return .5f + .5f * pn_oracle_tansig(.5f * x); } /* vec.h:73-76 */
+/* the two above over n values in one call (tests evaluate millions) */
+void pn_oracle_tansig_n(const float *x, float *y, long n) {
+  long i;
+  for (i = 0; i < n; i++) y[i] = pn_oracle_tansig(x[i]);
+}
+void pn_oracle_sigmoid_n(const float *x, float *y, long n) {
+  long i;
+  for (i = 0; i < n; i++) y[i] = pn_oracle_sigmoid(x[i]);
+}
 
 static void activate(float *v, int n, int act) { /* nnet.cpp:74-103 */
   int i;

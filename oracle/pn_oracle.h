@@ -83,6 +83,8 @@ void pn_oracle_erb_borders(int *out34);                                   /* erb
 void pn_oracle_tables(float *half_window480, float *comb_window7);        /* denoise.cpp:186-214     */
 float pn_oracle_tansig(float x);                                          /* vec.h:53-71             */
 float pn_oracle_sigmoid(float x);                                         /* vec.h:73-76             */
+void pn_oracle_tansig_n(const float *x, float *y, long n);                /* the same, n values      */
+void pn_oracle_sigmoid_n(const float *x, float *y, long n);
 void pn_oracle_fft960(const float *in_ri, float *out_ri);                 /* kiss_fft.cpp:566-586    */
 void pn_oracle_band_energy(float *bandE, const float *X_ri);              /* denoise.cpp:89-123      */
 void pn_oracle_band_corr(float *bandE, const float *X_ri, const float *P_ri); /* denoise.cpp:125-160 */

@@ -205,6 +205,47 @@ int pnb_import_states(pnb_engine *e, const int *streams, int n, const void *d_bl
 int pnb_set_active_streams(pnb_engine *e, int n, void *cuda_stream);
 int pnb_active_streams(const pnb_engine *e);
 
+/* Session pool: calls advance any listed subset of sessions, and sessions that sit a call out keep their state.
+ * A session is a logical stream id in [0, capacity); each session is either resident in a slot of the engine or parked
+ * as a blob (the bytes of pnb_export_states) in engine-owned device memory.  Only sessions that change membership
+ * between two calls move: a session listed in consecutive calls stays in its slot, one that skips a call is parked once
+ * and unparked once; listing the same set in another order moves nothing.
+ *
+ * pnb_sessions_reserve: the first call puts the engine in session mode and resets it (every session starts fresh); a
+ *   later call with a larger n_sessions grows the parking area (pnb_state_size() bytes, rounded up to 16, per session)
+ *   and keeps every session's state; a smaller or equal one is a no-op.  Waits for the engine to be idle.  Refused on
+ *   PNB_TRAIN_DATA engines and on an engine poisoned by a failed call.
+ * pnb_process_sessions_*: advances exactly the n listed sessions (distinct ids, 1 <= n <= n_streams) by n_frames hops;
+ *   row i of in / out and gr[t][i] belong to ids[i], in list order; every session not listed keeps its state.  ids is
+ *   host memory, reusable when the call returns.  The device forms are asynchronous and ordered like pnb_process_device_*
+ *   (d_gr NULL ok); the host forms block like pnb_process_host_* (gr NULL ok).
+ * pnb_reset_sessions: the listed sessions start over as fresh streams (the session-level pnb_reset_streams).
+ * pnb_export_sessions / pnb_import_sessions: the blobs of pnb_export_states / pnb_import_states (same d_blobs and
+ *   blob_stride rules, n <= capacity), so a session moves between pooled engines, plain engines (pnb_set_state) and
+ *   the host.  An import is checked like pnb_import_states: a rejected blob leaves its session fresh, and the next
+ *   synchronising entry point returns PNB_ERR_ARG once, naming the lowest rejected session id.
+ *   The three are asynchronous on cuda_stream and ordered with the calls like the slot-level state operations.
+ * pnb_session_stats: out[0] parks, out[1] unparks (fresh starts included), out[2] relocations (a listed session moved
+ *   from a slot >= n to a free slot < n), counted since pnb_sessions_reserve.  A test and measurement hook.
+ * In session mode pnb_process_* / pnb_submit_*, pnb_set_active_streams, pnb_reset_streams, pnb_export_states,
+ * pnb_import_states, pnb_get_state and pnb_set_state return PNB_ERR_ARG before anything is enqueued; pnb_reset makes
+ * every session fresh and keeps session mode.  The session calls refuse, before any state changes: a call before
+ * pnb_sessions_reserve, NULL pointers, ids out of range or listed twice, n out of range, short strides, and n_frames
+ * outside [1, max_frames].  A call that fails after it started to enqueue work poisons the engine, as the other calls. */
+int pnb_sessions_reserve(pnb_engine *e, int n_sessions);
+int pnb_process_sessions_device_f32(pnb_engine *e, const int *ids, int n, const float *d_in, size_t in_stride,
+                                    float *d_out, size_t out_stride, int n_frames, float *d_gr, void *cuda_stream);
+int pnb_process_sessions_device_i16(pnb_engine *e, const int *ids, int n, const short *d_in, size_t in_stride,
+                                    short *d_out, size_t out_stride, int n_frames, float *d_gr, void *cuda_stream);
+int pnb_process_sessions_host_f32(pnb_engine *e, const int *ids, int n, const float *in, size_t in_stride, float *out,
+                                  size_t out_stride, int n_frames, float *gr);
+int pnb_process_sessions_host_i16(pnb_engine *e, const int *ids, int n, const short *in, size_t in_stride, short *out,
+                                  size_t out_stride, int n_frames, float *gr);
+int pnb_reset_sessions(pnb_engine *e, const int *ids, int n, void *cuda_stream);
+int pnb_export_sessions(pnb_engine *e, const int *ids, int n, void *d_blobs, size_t blob_stride, void *cuda_stream);
+int pnb_import_sessions(pnb_engine *e, const int *ids, int n, const void *d_blobs, size_t blob_stride, void *cuda_stream);
+int pnb_session_stats(const pnb_engine *e, long long *out);
+
 /* The pitch analysis alone (BASELINE.json config 5; needs no engine): for each of n_units pitch buffers of 1728
  * float samples (unit u at d_pitch_buf + u*stride; the reference's st->pitch_buf, src/denoise.cpp:80,405-411) runs
  * pitch_downsample, pitch_search and remove_doubling (src/pitch.cpp:148-216, 283-386, 423-527) exactly as the hot path

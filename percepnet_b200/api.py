@@ -71,6 +71,15 @@ def load_library() -> C.CDLL:
     L.pnb_import_states.argtypes = [vp, vp, i, vp, sz, vp]
     L.pnb_set_active_streams.argtypes = [vp, i, vp]
     L.pnb_active_streams.argtypes = [vp]
+    L.pnb_sessions_reserve.argtypes = [vp, i]
+    L.pnb_process_sessions_device_f32.argtypes = [vp, vp, i, vp, sz, vp, sz, i, vp, vp]
+    L.pnb_process_sessions_device_i16.argtypes = [vp, vp, i, vp, sz, vp, sz, i, vp, vp]
+    L.pnb_process_sessions_host_f32.argtypes = [vp, vp, i, vp, sz, vp, sz, i, vp]
+    L.pnb_process_sessions_host_i16.argtypes = [vp, vp, i, vp, sz, vp, sz, i, vp]
+    L.pnb_reset_sessions.argtypes = [vp, vp, i, vp]
+    L.pnb_export_sessions.argtypes = [vp, vp, i, vp, sz, vp]
+    L.pnb_import_sessions.argtypes = [vp, vp, i, vp, sz, vp]
+    L.pnb_session_stats.argtypes = [vp, vp]
     L.pnb_pitch_only_device.argtypes = [vp, sz, C.c_longlong, vp, vp, vp, vp, vp, vp, vp]
     L.pnb_pitch_only_host.argtypes = [vp, sz, C.c_longlong, vp, vp, vp, vp, vp, vp]
     L.pnb_launch_count.argtypes = [vp]
@@ -92,7 +101,10 @@ def load_library() -> C.CDLL:
 EXPORTS = ("pnb_create", "pnb_destroy", "pnb_reset", "pnb_process_host_f32", "pnb_process_host_i16",
            "pnb_model_load_blob", "pnb_model_load_stream", "pnb_model_free", "pnb_train_records_host", "pnb_train_records_device", "pnb_submit_train_records", "pnb_process_device_f32", "pnb_process_device_i16", "pnb_submit_host_f32", "pnb_submit_host_i16", "pnb_submit_device_f32", "pnb_submit_device_i16", "pnb_flush", "pnb_wait", "pnb_check",
            "pnb_read_tap", "pnb_state_size", "pnb_get_state", "pnb_set_state",
-           "pnb_reset_streams", "pnb_export_states", "pnb_import_states", "pnb_set_active_streams", "pnb_active_streams", "pnb_pitch_only_device", "pnb_pitch_only_host", "pnb_launch_count",
+           "pnb_reset_streams", "pnb_export_states", "pnb_import_states", "pnb_set_active_streams", "pnb_active_streams",
+           "pnb_sessions_reserve", "pnb_process_sessions_device_f32", "pnb_process_sessions_device_i16",
+           "pnb_process_sessions_host_f32", "pnb_process_sessions_host_i16", "pnb_reset_sessions", "pnb_export_sessions",
+           "pnb_import_sessions", "pnb_session_stats", "pnb_pitch_only_device", "pnb_pitch_only_host", "pnb_launch_count",
            "pnb_launches_per_call", "pnb_profile_enable", "pnb_profile_read", "pnb_profile_timeline", "pnb_kernel_class_name", "pnb_n_streams", "pnb_max_frames", "pnb_last_error", "pnb_version")
 
 
@@ -286,13 +298,82 @@ class Engine:
         """pnb_import_states.  d_blobs: a raw device pointer (as export_states) or a CUDA uint8 tensor
         [len(idx), >= pnb_state_size()] whose rows are blobs; the tensor must stay alive until `stream` has run the import."""
         a, n = self._slots(idx)
+        d_blobs, stride = self._blob_rows(d_blobs, stride, n, "import_states")
+        self._ck(self.L.pnb_import_states(self.h, a.ctypes.data if n else None, n, d_blobs or None, stride or self.state_size,
+                                          stream or None), "pnb_import_states")
+
+    @staticmethod
+    def _blob_rows(d_blobs, stride, n, what):
         if not isinstance(d_blobs, int) and d_blobs is not None:
             t = d_blobs
             if t.dtype.itemsize != 1 or t.dim() != 2 or t.shape[0] != n or t.stride(1) != 1 or not t.is_cuda:
-                raise PnbError("import_states: blobs must be a CUDA byte tensor [len(idx), pnb_state_size()] with contiguous rows")
+                raise PnbError(f"{what}: blobs must be a CUDA byte tensor [len(idx), pnb_state_size()] with contiguous rows")
             d_blobs, stride = t.data_ptr(), t.stride(0)
-        self._ck(self.L.pnb_import_states(self.h, a.ctypes.data if n else None, n, d_blobs or None, stride or self.state_size,
-                                          stream or None), "pnb_import_states")
+        return d_blobs, stride
+
+    # ---- session pool (see pnb_sessions_reserve in the header) ---------------------------------------------------------
+    def reserve_sessions(self, n_sessions: int):
+        """pnb_sessions_reserve: session mode with sessions [0, n_sessions), all fresh (the first call resets the engine);
+        a later, larger call grows the pool and keeps every session's state."""
+        self._ck(self.L.pnb_sessions_reserve(self.h, n_sessions), "pnb_sessions_reserve")
+
+    def process_sessions(self, ids, x: np.ndarray, want_gr: bool = False):
+        """pnb_process_sessions_host_*: advances exactly the listed sessions.  x: [len(ids), F*480] float32 or int16 host
+        array, row i for ids[i].  Returns (out like x, gr [F, len(ids), 68] or None)."""
+        a, n = self._slots(ids)
+        assert x.ndim == 2 and x.shape[0] == n and x.shape[1] % FRAME == 0
+        F = x.shape[1] // FRAME
+        x = np.ascontiguousarray(x)
+        out = np.empty_like(x)
+        gr = np.empty((F, n, 68), np.float32) if want_gr else None
+        grp = gr.ctypes.data if want_gr else None
+        if x.dtype == np.float32:
+            f = self.L.pnb_process_sessions_host_f32
+        elif x.dtype == np.int16:
+            f = self.L.pnb_process_sessions_host_i16
+        else:
+            raise TypeError("x must be float32 or int16")
+        self._ck(f(self.h, a.ctypes.data, n, x.ctypes.data, x.shape[1], out.ctypes.data, x.shape[1], F, grp),
+                 "pnb_process_sessions_host")
+        return out, gr
+
+    def process_sessions_device(self, ids, d_in: int, in_stride: int, d_out: int, out_stride: int, n_frames: int,
+                                d_gr: int = 0, stream: int = 0, int16: bool = False):
+        """pnb_process_sessions_device_*: raw device pointers, row i of in / out and d_gr[t][i] for ids[i]."""
+        a, n = self._slots(ids)
+        f = self.L.pnb_process_sessions_device_i16 if int16 else self.L.pnb_process_sessions_device_f32
+        self._ck(f(self.h, a.ctypes.data, n, d_in, in_stride, d_out, out_stride, n_frames, d_gr or None, stream or None),
+                 "pnb_process_sessions_device")
+
+    def reset_sessions(self, ids, stream: int = 0):
+        """pnb_reset_sessions: the listed sessions start over as fresh streams."""
+        a, n = self._slots(ids)
+        self._ck(self.L.pnb_reset_sessions(self.h, a.ctypes.data if n else None, n, stream or None), "pnb_reset_sessions")
+
+    def export_sessions(self, ids, d_blobs, stride: int = 0, stream: int = 0):
+        """pnb_export_sessions, with the conventions of export_states (None: returns a new CUDA uint8 tensor)."""
+        a, n = self._slots(ids)
+        out = None
+        if d_blobs is None:
+            import torch
+            out = torch.empty((n, self.state_size), dtype=torch.uint8, device=f"cuda:{self.device}")
+            d_blobs, stride = out.data_ptr(), self.state_size
+        self._ck(self.L.pnb_export_sessions(self.h, a.ctypes.data if n else None, n, d_blobs or None,
+                                            stride or self.state_size, stream or None), "pnb_export_sessions")
+        return out
+
+    def import_sessions(self, ids, d_blobs, stride: int = 0, stream: int = 0):
+        """pnb_import_sessions, with the conventions of import_states (a raw pointer or a CUDA uint8 tensor of blob rows)."""
+        a, n = self._slots(ids)
+        d_blobs, stride = self._blob_rows(d_blobs, stride, n, "import_sessions")
+        self._ck(self.L.pnb_import_sessions(self.h, a.ctypes.data if n else None, n, d_blobs or None,
+                                            stride or self.state_size, stream or None), "pnb_import_sessions")
+
+    def session_stats(self) -> dict:
+        """pnb_session_stats: cumulative {parks, unparks, relocations} of the session pool."""
+        c = (C.c_longlong * 3)()
+        self._ck(self.L.pnb_session_stats(self.h, c), "pnb_session_stats")
+        return {"parks": int(c[0]), "unparks": int(c[1]), "relocations": int(c[2])}
 
     def read_nn_state(self) -> dict:
         """fp32 network state after the last hop: conv2 output and the five GRU states, [S, width]."""

@@ -943,6 +943,7 @@ __global__ void __launch_bounds__(kSynWarps * 32) synthesis_kernel(SynthesisArgs
   const int s = blockIdx.x * kSynWarps + wib;
   if (s >= A.n_streams) return;
   SynWarpSmem &W = Wall[wib];
+  const int orow = A.row ? A.row[s] : s;  // output row of slot s
 
   float mem[15];  // overlap-add memory: samples lane + 32 i  (denoise.cpp:75,357-358)
 #pragma unroll
@@ -1012,8 +1013,8 @@ __global__ void __launch_bounds__(kSynWarps * 32) synthesis_kernel(SynthesisArgs
       });
     }
     // time samples are read back reversed and rescaled (denoise.cpp:318-323), windowed, overlap-added
-    float *outp = A.out ? A.out + (size_t)s * A.out_stride + (size_t)t * kFrame : nullptr;
-    short *outs = A.out16 ? A.out16 + (size_t)s * A.out_stride + (size_t)t * kFrame : nullptr;
+    float *outp = A.out ? A.out + (size_t)orow * A.out_stride + (size_t)t * kFrame : nullptr;
+    short *outs = A.out16 ? A.out16 + (size_t)orow * A.out_stride + (size_t)t * kFrame : nullptr;
 #pragma unroll
     for (int i = 0; i < 15; i++) {
       int n = lane + 32 * i;
@@ -1036,13 +1037,14 @@ __global__ void __launch_bounds__(kSynWarps * 32) synthesis_kernel(SynthesisArgs
 // staging: append the new hops to each stream's PCM line / slide the history forward
 // ------------------------------------------------------------------------------------------
 __global__ void stage_in_kernel(float *pcm, size_t pcm_stride, const float *in, const short *in16, size_t in_stride,
-                                int n_streams, int n_samples, float i16_div) {
+                                int n_streams, int n_samples, float i16_div, const int *row) {
   const int s = blockIdx.x;  // streams on grid.x (no 65535 limit), chunks of the row on grid.y
+  const size_t r = row ? row[s] : s;  // input row of slot s
   float *dst = pcm + (size_t)s * pcm_stride + kKeep;
   for (int i = blockIdx.y * blockDim.x + threadIdx.x; i < n_samples; i += gridDim.y * blockDim.x) {
     float v;
-    if (in) v = in[(size_t)s * in_stride + i];
-    else v = ((float)in16[(size_t)s * in_stride + i]) / i16_div;  // main.cpp:34 (32768) / denoise.cpp:681 (NORM_RATIO 1)
+    if (in) v = in[r * in_stride + i];
+    else v = ((float)in16[r * in_stride + i]) / i16_div;  // main.cpp:34 (32768) / denoise.cpp:681 (NORM_RATIO 1)
     dst[i] = v;
   }
 }
@@ -1211,9 +1213,9 @@ int launch_synthesis(const SynthesisArgs &a, cudaStream_t st) {
   return 1;
 }
 int launch_stage_in(float *pcm, size_t pcm_stride, const float *in, const short *in16, size_t in_stride,
-                    int n_streams, int n_samples, cudaStream_t st, float i16_div) {
+                    int n_streams, int n_samples, cudaStream_t st, float i16_div, const int *row) {
   dim3 grid(n_streams, (n_samples + 1023) / 1024 > 8 ? 8 : (n_samples + 1023) / 1024);
-  stage_in_kernel<<<grid, 256, 0, st>>>(pcm, pcm_stride, in, in16, in_stride, n_streams, n_samples, i16_div);
+  stage_in_kernel<<<grid, 256, 0, st>>>(pcm, pcm_stride, in, in16, in_stride, n_streams, n_samples, i16_div, row);
   return 1;
 }
 int launch_slide_history(float *pcm, size_t pcm_stride, int n_streams, int n_samples, cudaStream_t st) {

@@ -241,7 +241,9 @@ extern "C" int pnb_create(pnb_engine **out, int n_streams, int max_frames, const
     CKD(cudaHostAlloc((void **)&e->h_idx[k], S * sizeof(int), cudaHostAllocDefault));
     CKD(dalloc(&e->d_idx[k], S, false));
   }
+  e->idx_cap = S;
   CKD(dalloc(&e->d_ok, S, false));
+  e->ok_cap = S;
   CKD(cudaMalloc(&e->d_blob1, sizeof(StreamState)));
   CKD(dalloc(&e->d_last_period, S));
   CKD(dalloc(&e->d_last_gain, S));
@@ -323,6 +325,8 @@ extern "C" void pnb_destroy(pnb_engine *e) {
   }
   if (e->d_ok) cudaFree(e->d_ok);
   if (e->d_blob1) cudaFree(e->d_blob1);
+  if (e->d_park) cudaFree(e->d_park);
+  if (e->d_sgr) cudaFree(e->d_sgr);
   if (e->ev_call) cudaEventDestroy(e->ev_call);
   if (e->d_tap_pitch) cudaFree(e->d_tap_pitch);
   if (e->d_tab) cudaFree(e->d_tab);
@@ -361,6 +365,10 @@ extern "C" int pnb_reset(pnb_engine *e) {
   e->hop = 0;
   e->n_active = e->S;
   e->poisoned = false;
+  if (e->sessions) {  // every session fresh: all parked, every blob marked fresh
+    CK(cudaMemset(e->d_park, 0, (size_t)e->pool.capacity() * kParkStride));
+    e->pool.init(e->S, e->pool.capacity());
+  }
   if (e->flags & PNB_TRAIN_DATA) {
     CK(cudaDeviceSynchronize());
     return PNB_OK;
@@ -578,6 +586,7 @@ static SynthesisArgs synthesis_args(pnb_engine *e, int F, float *d_out, short *d
   s.out = d_out; s.out16 = d_out16; s.out_stride = out_stride;
   s.postfilter = (e->flags & PNB_POSTFILTER) ? 1 : 0;
   s.tap_g = e->d_tap_g;
+  s.row = nullptr;
   return s;
 }
 
@@ -642,13 +651,69 @@ static int enqueue_call(pnb_engine *e, int F, cudaStream_t st, Launches launches
   return PNB_OK;
 }
 
-// One enhancement call on st (arguments already checked).
+// The n ints at src through the pinned, event-guarded index staging, copied on st; *dst: their device copy, valid for
+// the work enqueued on st behind it (the caller's array is free again when this returns).
+static int stage_ints(pnb_engine *e, const int *src, size_t n, cudaStream_t st, const int **dst) {
+  const int k = e->idx_slot;
+  CK(cudaEventSynchronize(e->ev_idx[k]));  // the copy out of this slot two operations ago has run
+  memcpy(e->h_idx[k], src, n * sizeof(int));
+  CK(cudaMemcpyAsync(e->d_idx[k], e->h_idx[k], n * sizeof(int), cudaMemcpyHostToDevice, st));
+  CK(cudaEventRecord(e->ev_idx[k], st));
+  e->idx_slot = k ^ 1;
+  *dst = e->d_idx[k];
+  return PNB_OK;
+}
+
+// The state-operation arguments of a session pool: the pieces of a slot at the counters committed by the last call.
+static StateArgs session_args(pnb_engine *e) {
+  StateArgs a;
+  memset(&a, 0, sizeof a);
+  a.n_seg = state_segs(e, a.seg);
+  a.park = e->d_park;
+  a.park_stride = kParkStride;
+  a.ok = e->d_ok;
+  a.status = e->d_status;
+  a.has_terms = (e->flags & PNB_NN_TENSOR) ? 1u : 0u;
+  a.check_gru = (e->flags & PNB_NN_TENSOR) ? 1 : 0;
+  return a;
+}
+
+// A session call's residency plan, applied (pnb_session_plan.h), its upload (row map, then the moves), and its state
+// launch when membership changed.  Sets the active range to the list; *d_row: the row map on the device.  Returns the
+// number of launches or a negative error.
+static int enqueue_plan(pnb_engine *e, const int *ids, int k, cudaStream_t st, const int **d_row) {
+  StateArgs a = session_args(e);  // before the plan: parking reads the pieces where the last call left them
+  e->pool.plan(ids, k, e->plan_row, e->plan_moves);
+  e->n_active = k;
+  const size_t k4 = ((size_t)k + 3) & ~(size_t)3;  // the moves start 16-byte aligned
+  std::vector<int> &up = e->plan_up;
+  up.assign(e->plan_row.begin(), e->plan_row.end());
+  up.resize(k4, 0);
+  const int *mv = reinterpret_cast<const int *>(e->plan_moves.data());
+  up.insert(up.end(), mv, mv + 4 * e->plan_moves.size());
+  const int *d = nullptr;
+  { int rc = stage_ints(e, up.data(), up.size(), st, &d); if (rc) return rc; }
+  *d_row = d;
+  if (e->plan_moves.empty()) return 0;
+  a.n = (int)e->plan_moves.size();
+  a.moves = d + k4;
+  return launch_session_move(a, st);
+}
+
+// One enhancement call on st (arguments already checked).  With a session list (ids, n_ids) the call first applies its
+// residency plan, and reads input row / writes output row and g/r row row[p] for slot p.
 static int enqueue_enhance(pnb_engine *e, const float *d_in, const short *d_in16, size_t in_stride, float *d_out,
-                           short *d_out16, size_t out_stride, int F, float *d_gr, cudaStream_t st) {
+                           short *d_out16, size_t out_stride, int F, float *d_gr, cudaStream_t st, const int *ids = nullptr,
+                           int n_ids = 0) {
   return enqueue_call(e, F, st, [&]() -> int {
-    const int S = e->S, na = e->n_active;  // the call advances streams [0, na); per-call buffers keep the stride S
     int n = 0;
-    { ProfScope ps(e, PNB_K_STAGE_IN, st); n += launch_stage_in(e->d_pcm + e->line_off, e->pcm_stride, d_in, d_in16, in_stride, na, F * kFrame, st); }
+    const int *row = nullptr;
+    if (ids) {
+      n = enqueue_plan(e, ids, n_ids, st, &row);
+      if (n < 0) return n;
+    }
+    const int S = e->S, na = e->n_active;  // the call advances streams [0, na); per-call buffers keep the stride S
+    { ProfScope ps(e, PNB_K_STAGE_IN, st); n += launch_stage_in(e->d_pcm + e->line_off, e->pcm_stride, d_in, d_in16, in_stride, na, F * kFrame, st, 32768.f, row); }
     { ProfScope ps(e, PNB_K_ANALYSIS, st); n += launch_analysis(analysis_args(e, F), st); }
     CK(cudaGetLastError());
     if (e->flags & PNB_NN_TENSOR) {
@@ -662,18 +727,44 @@ static int enqueue_enhance(pnb_engine *e, const float *d_in, const short *d_in16
         n += q;
       }
     }
-    { ProfScope ps(e, PNB_K_SYNTHESIS, st); n += launch_synthesis(synthesis_args(e, F, d_out, d_out16, out_stride), st); }
+    {
+      SynthesisArgs sa = synthesis_args(e, F, d_out, d_out16, out_stride);
+      sa.row = row;
+      ProfScope ps(e, PNB_K_SYNTHESIS, st);
+      n += launch_synthesis(sa, st);
+    }
     n += advance_line(e, F, st);
-    if (d_gr)  // [F][na][68] from the [F][S][68] buffer
+    if (d_gr && row)  // [F][na][68] in list order
+      n += launch_gr_gather(e->d_gr, d_gr, row, na, S, F, st);
+    else if (d_gr)  // [F][na][68] from the [F][S][68] buffer
       CK(cudaMemcpy2DAsync(d_gr, (size_t)na * 68 * sizeof(float), e->d_gr, (size_t)S * 68 * sizeof(float), (size_t)na * 68 * sizeof(float), F,
                            cudaMemcpyDeviceToDevice, st));
     return n;
   });
 }
 
+// The slot-level entry points of an engine in session mode: refused before anything is enqueued.
+static int refuse_in_session_mode() {
+  return fail(PNB_ERR_ARG, "engine is in session mode (pnb_sessions_reserve): slots are the pool's; use the *_sessions entry points");
+}
+
+// A session list: after pnb_sessions_reserve, n in [1, n_max], distinct ids in [0, capacity).
+static int check_ids(pnb_engine *e, const int *ids, int n, int n_max) {
+  if (!e->sessions) return fail(PNB_ERR_ARG, "no session pool: call pnb_sessions_reserve first");
+  if (!ids) return fail(PNB_ERR_ARG, "ids is NULL");
+  if (n < 1 || n > n_max) return fail(PNB_ERR_ARG, "n = %d sessions outside [1, %d]", n, n_max);
+  const int cap = e->pool.capacity();
+  for (int i = 0; i < n; i++)
+    if (ids[i] < 0 || ids[i] >= cap) return fail(PNB_ERR_ARG, "ids[%d] = %d outside [0, %d)", i, ids[i], cap);
+  const int d = e->pool.duplicate(ids, n);
+  if (d >= 0) return fail(PNB_ERR_ARG, "session %d listed twice (ids[%d])", ids[d], d);
+  return PNB_OK;
+}
+
 static int process_device(pnb_engine *e, const float *d_in, const short *d_in16, size_t in_stride, float *d_out,
                           short *d_out16, size_t out_stride, int F, float *d_gr, cudaStream_t st) {
   { int rc = check_call(e, false, (d_in || d_in16) && (d_out || d_out16), F, in_stride, out_stride); if (rc) return rc; }
+  if (e->sessions) return refuse_in_session_mode();
   CK(cudaSetDevice(e->device));
   return enqueue_enhance(e, d_in, d_in16, in_stride, d_out, d_out16, out_stride, F, d_gr, st);
 }
@@ -831,6 +922,9 @@ static int report_status(pnb_engine *e) {
     CK(cudaStreamSynchronize(e->stream));
     e->h_status[0] &= ~kStatusRejected;
     e->h_status[1] = kNoRejectedSlot;
+    if (e->sessions)
+      return fail(PNB_ERR_ARG, "pnb_import_sessions rejected a blob (bad magic / version, or a GRU state outside [-1, 1] for a "
+                               "tensor-mode engine); lowest rejected session %d, left fresh like every rejected one", slot);
     return fail(PNB_ERR_ARG, "pnb_import_states rejected a blob (bad magic / version, or a GRU state outside [-1, 1] for a "
                              "tensor-mode engine); lowest rejected stream %d, left reset like every rejected one", slot);
   }
@@ -841,26 +935,34 @@ static int report_status(pnb_engine *e) {
   return PNB_OK;
 }
 
-// pnb_process_host_* (blocking) and pnb_submit_host_* (pipelined).  The blocking form then copies g/r and the status
-// word back on the engine's stream too, and synchronises it once.
+// pnb_process_host_* (blocking) and pnb_submit_host_* (pipelined); with a session list (ids, n_ids) the blocking
+// pnb_process_sessions_host_*.  The blocking form then copies g/r and the status word back on the engine's stream too,
+// and synchronises it once.
 template <typename T>
-static int host_call(pnb_engine *e, const T *in, size_t in_stride, T *out, size_t out_stride, int F, float *gr, bool pipelined) {
+static int host_call(pnb_engine *e, const T *in, size_t in_stride, T *out, size_t out_stride, int F, float *gr, bool pipelined,
+                     const int *ids = nullptr, int n_ids = 0) {
   { int rc = check_call(e, false, in && out, F, in_stride, out_stride); if (rc) return rc; }
+  if (!ids && e->sessions) return refuse_in_session_mode();
+  if (ids) { int rc = check_ids(e, ids, n_ids, e->S); if (rc) return rc; }
   CK(cudaSetDevice(e->device));
   const size_t S = e->S, row = (size_t)e->Fmax * kFrame, w = (size_t)F * kFrame * sizeof(T);
-  const size_t na = e->n_active;  // the rows of in / out / gr
+  const size_t na = ids ? n_ids : e->n_active;  // the rows of in / out / gr
   const int k = staging_slot(e, pipelined, S * row * sizeof(T), S * row * sizeof(T));
   if (k < 0) return k;
+  if (ids && gr) { int rc = grow((void **)&e->d_sgr, &e->sgr_bytes, (size_t)e->Fmax * S * 68 * sizeof(float)); if (rc) return rc; }
+  float *d_gr = ids && gr ? e->d_sgr : nullptr;  // session calls gather g/r in list order on the device
   T *d_in = (T *)e->stage[k].in, *d_out = (T *)e->stage[k].out;
   const int rc = round_trip(e, k, pipelined,
       [&](cudaStream_t s) { return cudaMemcpy2DAsync(d_in, row * sizeof(T), in, in_stride * sizeof(T), w, na, cudaMemcpyHostToDevice, s); },
       [&] {
-        return sizeof(T) == 4 ? enqueue_enhance(e, (const float *)d_in, nullptr, row, (float *)d_out, nullptr, row, F, nullptr, e->stream)
-                              : enqueue_enhance(e, nullptr, (const short *)d_in, row, nullptr, (short *)d_out, row, F, nullptr, e->stream);
+        return sizeof(T) == 4 ? enqueue_enhance(e, (const float *)d_in, nullptr, row, (float *)d_out, nullptr, row, F, d_gr, e->stream, ids, n_ids)
+                              : enqueue_enhance(e, nullptr, (const short *)d_in, row, nullptr, (short *)d_out, row, F, d_gr, e->stream, ids, n_ids);
       },
       [&](cudaStream_t s) { return cudaMemcpy2DAsync(out, out_stride * sizeof(T), d_out, row * sizeof(T), w, na, cudaMemcpyDeviceToHost, s); });
   if (rc || pipelined) return rc;
-  if (gr)
+  if (gr && d_gr)
+    CK(cudaMemcpyAsync(gr, d_gr, (size_t)F * na * 68 * sizeof(float), cudaMemcpyDeviceToHost, e->stream));
+  else if (gr)
     CK(cudaMemcpy2DAsync(gr, na * 68 * sizeof(float), e->d_gr, S * 68 * sizeof(float), na * 68 * sizeof(float), F, cudaMemcpyDeviceToHost,
                          e->stream));
   CK(cudaMemcpyAsync(e->h_status, e->d_status, 2 * sizeof(int), cudaMemcpyDeviceToHost, e->stream));
@@ -974,13 +1076,8 @@ static int state_enqueue(pnb_engine *e, int mode, const int *streams, int n, voi
   a.n_seg = state_segs(e, a.seg);
   { int rc = wait_last_call(e, st); if (rc) return rc; }
   // the slot indices travel through pinned staging: the caller's array is free again when this returns
-  const int k = e->idx_slot;
-  CK(cudaEventSynchronize(e->ev_idx[k]));  // the copy out of this slot two operations ago has run
-  memcpy(e->h_idx[k], streams, (size_t)n * sizeof(int));
-  CK(cudaMemcpyAsync(e->d_idx[k], e->h_idx[k], (size_t)n * sizeof(int), cudaMemcpyHostToDevice, st));
-  CK(cudaEventRecord(e->ev_idx[k], st));
-  e->idx_slot = k ^ 1;
-  a.n = n; a.streams = e->d_idx[k]; a.blobs = static_cast<char *>(d_blobs); a.blob_stride = blob_stride;
+  { int rc = stage_ints(e, streams, (size_t)n, st, &a.streams); if (rc) return rc; }
+  a.n = n; a.blobs = static_cast<char *>(d_blobs); a.blob_stride = blob_stride;
   a.ok = e->d_ok; a.mode = mode; a.status = e->d_status;
   a.has_terms = (e->flags & PNB_NN_TENSOR) ? 1u : 0u;
   a.check_gru = (e->flags & PNB_NN_TENSOR) ? 1 : 0;
@@ -995,6 +1092,7 @@ static int state_enqueue(pnb_engine *e, int mode, const int *streams, int n, voi
 
 static int state_batch(pnb_engine *e, int mode, const int *streams, int n, void *d_blobs, size_t blob_stride, void *cuda_stream) {
   if (!e) return fail(PNB_ERR_ARG, "engine is NULL");
+  if (e->sessions) return refuse_in_session_mode();
   if (n < 0) return fail(PNB_ERR_ARG, "n = %d is negative", n);
   if (n == 0) return PNB_OK;
   if (!streams) return fail(PNB_ERR_ARG, "streams is NULL");
@@ -1035,6 +1133,7 @@ extern "C" int pnb_import_states(pnb_engine *e, const int *streams, int n, const
 extern "C" int pnb_set_active_streams(pnb_engine *e, int n, void *cuda_stream) {
   if (!e) return fail(PNB_ERR_ARG, "engine is NULL");
   if (e->flags & PNB_TRAIN_DATA) return fail(PNB_ERR_ARG, "PNB_TRAIN_DATA engines always advance all their streams");
+  if (e->sessions) return refuse_in_session_mode();
   if (n < 1 || n > e->S) return fail(PNB_ERR_ARG, "active streams %d outside [1, %d]", n, e->S);
   if (e->poisoned) return fail(PNB_ERR_ARG, "an earlier call failed while enqueuing work; the streams' state is undefined until pnb_reset");
   if (n > e->n_active) {
@@ -1051,6 +1150,7 @@ extern "C" int pnb_active_streams(const pnb_engine *e) { return e ? e->n_active 
 
 static int state_args(pnb_engine *e, int stream, const void *buf, size_t bytes) {
   if (!e || !buf) return fail(PNB_ERR_ARG, "NULL argument");
+  if (e->sessions) return refuse_in_session_mode();
   if (stream < 0 || stream >= e->S) return fail(PNB_ERR_ARG, "stream %d outside [0, %d)", stream, e->S);
   if (stream >= e->n_active) return fail(PNB_ERR_ARG, "stream %d outside the active range [0, %d)", stream, e->n_active);
   if (bytes < sizeof(StreamState)) return fail(PNB_ERR_ARG, "state buffer of %zu bytes, need pnb_state_size() = %zu", bytes, sizeof(StreamState));
@@ -1086,6 +1186,166 @@ extern "C" int pnb_set_state(pnb_engine *e, int stream, const void *src, size_t 
   if ((rc = state_enqueue(e, kStateImport, &stream, 1, e->d_blob1, sizeof(StreamState), e->stream))) return rc;
   CK(cudaStreamSynchronize(e->stream));
   return PNB_OK;
+}
+
+// ------------------------------------------------------------------------------------------
+// session pool: sessions [0, capacity) over the engine's slots; a call advances any listed subset (pnb_session_plan.h)
+// ------------------------------------------------------------------------------------------
+// Grows both buffer pairs (pinned and device) of the index staging to at least n ints; the engine is idle.
+static int grow_ints(pnb_engine *e, size_t n) {
+  if (n > e->idx_cap) {
+    for (int k = 0; k < 2; k++) {
+      int *h = nullptr, *d = nullptr;
+      CK(cudaHostAlloc((void **)&h, n * sizeof(int), cudaHostAllocDefault));
+      CK(cudaMalloc((void **)&d, n * sizeof(int)));
+      cudaFreeHost(e->h_idx[k]);
+      cudaFree(e->d_idx[k]);
+      e->h_idx[k] = h;
+      e->d_idx[k] = d;
+    }
+    e->idx_cap = n;
+  }
+  return PNB_OK;
+}
+
+extern "C" int pnb_sessions_reserve(pnb_engine *e, int n_sessions) {
+  if (!e) return fail(PNB_ERR_ARG, "engine is NULL");
+  if (e->flags & PNB_TRAIN_DATA) return fail(PNB_ERR_ARG, "PNB_TRAIN_DATA engines have no session pool");
+  if (e->poisoned) return fail(PNB_ERR_ARG, "an earlier call failed while enqueuing work; the streams' state is undefined until pnb_reset");
+  if (n_sessions < 1) return fail(PNB_ERR_ARG, "n_sessions = %d, need >= 1", n_sessions);
+  if (e->sessions && n_sessions <= e->pool.capacity()) return PNB_OK;  // the pool never shrinks
+  CK(cudaSetDevice(e->device));
+  CK(cudaDeviceSynchronize());
+  const size_t cap = (size_t)n_sessions, wide = cap > (size_t)e->S ? cap : (size_t)e->S;
+  // staging: a call's row map and moves (<= 5 S + 3 ints), an export's moves, ids and rows (<= 6 n)
+  { int rc = grow_ints(e, 6 * wide + 4); if (rc) return rc; }
+  if (wide > e->ok_cap) {
+    int *ok = nullptr;
+    CK(cudaMalloc((void **)&ok, wide * sizeof(int)));
+    cudaFree(e->d_ok);
+    e->d_ok = ok;
+    e->ok_cap = wide;
+  }
+  char *park = nullptr;
+  cudaError_t ce = cudaMalloc((void **)&park, cap * kParkStride);
+  if (ce != cudaSuccess)
+    return fail(ce == cudaErrorMemoryAllocation ? PNB_ERR_ALLOC : PNB_ERR_CUDA, "parking area of %zu sessions: %s", cap,
+                cudaGetErrorString(ce));
+  if (e->sessions) {  // grow: the parked sessions keep their blobs, the new ones start fresh
+    const size_t old = (size_t)e->pool.capacity() * kParkStride;
+    CK(cudaMemcpy(park, e->d_park, old, cudaMemcpyDeviceToDevice));
+    CK(cudaMemset(park + old, 0, cap * kParkStride - old));
+    CK(cudaFree(e->d_park));
+    e->d_park = park;
+    e->pool.grow((int)cap);
+    return PNB_OK;
+  }
+  e->d_park = park;
+  e->sessions = true;
+  e->pool.init(e->S, (int)cap);
+  return pnb_reset(e);
+}
+
+extern "C" int pnb_session_stats(const pnb_engine *e, long long *out) {
+  if (!e || !out) return fail(PNB_ERR_ARG, "NULL argument");
+  out[0] = e->pool.parks;
+  out[1] = e->pool.unparks;
+  out[2] = e->pool.relocations;
+  return PNB_OK;
+}
+
+static int process_sessions_device(pnb_engine *e, const int *ids, int n, const float *d_in, const short *d_in16, size_t in_stride,
+                                   float *d_out, short *d_out16, size_t out_stride, int F, float *d_gr, cudaStream_t st) {
+  { int rc = check_call(e, false, (d_in || d_in16) && (d_out || d_out16), F, in_stride, out_stride); if (rc) return rc; }
+  { int rc = check_ids(e, ids, n, e->S); if (rc) return rc; }
+  CK(cudaSetDevice(e->device));
+  return enqueue_enhance(e, d_in, d_in16, in_stride, d_out, d_out16, out_stride, F, d_gr, st, ids, n);
+}
+extern "C" int pnb_process_sessions_device_f32(pnb_engine *e, const int *ids, int n, const float *d_in, size_t in_stride,
+                                               float *d_out, size_t out_stride, int n_frames, float *d_gr, void *cuda_stream) {
+  return process_sessions_device(e, ids, n, d_in, nullptr, in_stride, d_out, nullptr, out_stride, n_frames, d_gr,
+                                 (cudaStream_t)cuda_stream);
+}
+extern "C" int pnb_process_sessions_device_i16(pnb_engine *e, const int *ids, int n, const short *d_in, size_t in_stride,
+                                               short *d_out, size_t out_stride, int n_frames, float *d_gr, void *cuda_stream) {
+  return process_sessions_device(e, ids, n, nullptr, d_in, in_stride, nullptr, d_out, out_stride, n_frames, d_gr,
+                                 (cudaStream_t)cuda_stream);
+}
+extern "C" int pnb_process_sessions_host_f32(pnb_engine *e, const int *ids, int n, const float *in, size_t in_stride, float *out,
+                                             size_t out_stride, int n_frames, float *gr) {
+  if (!e) return fail(PNB_ERR_ARG, "engine is NULL");
+  return host_call<float>(e, in, in_stride, out, out_stride, n_frames, gr, false, ids, n);
+}
+extern "C" int pnb_process_sessions_host_i16(pnb_engine *e, const int *ids, int n, const short *in, size_t in_stride, short *out,
+                                             size_t out_stride, int n_frames, float *gr) {
+  if (!e) return fail(PNB_ERR_ARG, "engine is NULL");
+  return host_call<short>(e, in, in_stride, out, out_stride, n_frames, gr, false, ids, n);
+}
+
+// pnb_reset_sessions / pnb_export_sessions / pnb_import_sessions.  A reset or an import takes the listed sessions out
+// of their slots (the slot's content is abandoned) and rewrites their parking blobs; the next call that lists them
+// unparks them.  An export writes resident sessions from their slots (session_move_kernel) and parked ones from their
+// parking blobs (session_blob_kernel); nothing moves.
+static int session_batch(pnb_engine *e, int mode, const int *ids, int n, void *d_blobs, size_t blob_stride, void *cuda_stream) {
+  if (!e) return fail(PNB_ERR_ARG, "engine is NULL");
+  if (e->poisoned) return fail(PNB_ERR_ARG, "an earlier call failed while enqueuing work; the streams' state is undefined until pnb_reset");
+  if (n == 0 && e->sessions) return PNB_OK;
+  if (mode != kStateReset) {
+    if (!d_blobs) return fail(PNB_ERR_ARG, "d_blobs is NULL");
+    if (blob_stride < sizeof(StreamState))
+      return fail(PNB_ERR_ARG, "blob_stride %zu below pnb_state_size() = %zu", blob_stride, sizeof(StreamState));
+    if ((reinterpret_cast<uintptr_t>(d_blobs) | blob_stride) & 3) return fail(PNB_ERR_ARG, "d_blobs and blob_stride must be multiples of 4 bytes");
+  }
+  { int rc = check_ids(e, ids, n, e->pool.capacity()); if (rc) return rc; }
+  CK(cudaSetDevice(e->device));
+  const cudaStream_t st = (cudaStream_t)cuda_stream;
+  const int rc = [&]() -> int {
+    { int rc = wait_last_call(e, st); if (rc) return rc; }
+    StateArgs a = session_args(e);
+    a.blobs = static_cast<char *>(d_blobs);
+    a.blob_stride = blob_stride;
+    a.mode = mode;
+    long long nl = 0;
+    std::vector<int> &up = e->plan_up;
+    up.clear();
+    if (mode == kStateExport) {  // [moves of the resident ones][ids of the parked ones][their rows]
+      std::vector<int> parked, rows;
+      for (int i = 0; i < n; i++) {
+        const int s = e->pool.where[ids[i]];
+        if (s >= 0) up.insert(up.end(), {s, i, kFillNone, -1});
+        else { parked.push_back(ids[i]); rows.push_back(i); }
+      }
+      const int r = (int)up.size() / 4, p = (int)parked.size();
+      up.insert(up.end(), parked.begin(), parked.end());
+      up.insert(up.end(), rows.begin(), rows.end());
+      const int *d = nullptr;
+      { int rc = stage_ints(e, up.data(), up.size(), st, &d); if (rc) return rc; }
+      if (r) { a.n = r; a.moves = d; nl += launch_session_move(a, st); }
+      if (p) { a.n = p; a.streams = d + 4 * r; a.rows = d + 4 * r + p; a.blobs = static_cast<char *>(d_blobs); nl += launch_session_blob(a, st); }
+    } else {
+      for (int i = 0; i < n; i++) e->pool.evict(ids[i]);
+      const int *d = nullptr;
+      { int rc = stage_ints(e, ids, (size_t)n, st, &d); if (rc) return rc; }
+      a.n = n; a.streams = d;
+      if (mode == kStateImport) nl += launch_state_check(a, st);  // reports session ids: a.streams are the ids
+      nl += launch_session_blob(a, st);
+    }
+    CK(cudaGetLastError());
+    { int rc = mark_call_end(e, st); if (rc) return rc; }
+    e->launches += nl;
+    return PNB_OK;
+  }();
+  if (rc) e->poisoned = true;  // part of the operation may have been enqueued
+  return rc;
+}
+extern "C" int pnb_reset_sessions(pnb_engine *e, const int *ids, int n, void *cuda_stream) {
+  return session_batch(e, kStateReset, ids, n, nullptr, 0, cuda_stream);
+}
+extern "C" int pnb_export_sessions(pnb_engine *e, const int *ids, int n, void *d_blobs, size_t blob_stride, void *cuda_stream) {
+  return session_batch(e, kStateExport, ids, n, d_blobs, blob_stride, cuda_stream);
+}
+extern "C" int pnb_import_sessions(pnb_engine *e, const int *ids, int n, const void *d_blobs, size_t blob_stride, void *cuda_stream) {
+  return session_batch(e, kStateImport, ids, n, const_cast<void *>(d_blobs), blob_stride, cuda_stream);
 }
 
 // ------------------------------------------------------------------------------------------

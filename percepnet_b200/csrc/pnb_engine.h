@@ -3,6 +3,7 @@
 #include <stddef.h>
 #include <vector>
 #include "pnb_kernels.h"
+#include "pnb_session_plan.h"
 #include "pnb_state.h"
 #include "../../include/percepnet_b200.h"
 #include "../../include/pnb_nnet_layout.h"
@@ -76,7 +77,8 @@ struct pnb_engine {
   long long launches = 0;
   // status word on the device: bit 0 = an activation left the domain in which the reference's tansig_approx is
   // defined (tensor path only; reported as PNB_ERR_DOMAIN by the synchronising entry points, cleared by pnb_reset);
-  // bit 1 = pnb_import_states rejected a blob, [1] = the lowest rejected slot (reported once, then cleared)
+  // bit 1 = pnb_import_states rejected a blob, [1] = the lowest rejected slot (reported once, then cleared; in session
+  // mode pnb_import_sessions raises it and [1] is the lowest rejected session id)
   int *d_status = nullptr;  // [2]
   int *h_status = nullptr;  // [2] pinned host copy, refreshed by the synchronising entry points
 
@@ -87,14 +89,26 @@ struct pnb_engine {
   cudaEvent_t ev_call = nullptr;
   bool call_recorded = false;    // ev_call has been recorded at least once
   // batched stream-state operations: staging of the slot indices, import verdicts, one blob of scratch
-  int *h_idx[2] = {nullptr, nullptr};  // [S] pinned staging of the slot indices, double-buffered ...
-  int *d_idx[2] = {nullptr, nullptr};  // [S] ... and their device copies
+  int *h_idx[2] = {nullptr, nullptr};  // [idx_cap] pinned staging of the slot indices (session calls: row map and moves),
+  int *d_idx[2] = {nullptr, nullptr};  // double-buffered, and their device copies
   cudaEvent_t ev_idx[2] = {nullptr, nullptr};  // the copy out of h_idx[k] has run
   int idx_slot = 0;
-  int *d_ok = nullptr;           // [S] import: per-blob verdict of the device-side check
+  size_t idx_cap = 0;            // ints: S, more in session mode
+  int *d_ok = nullptr;           // [ok_cap] import: per-blob verdict of the device-side check
+  size_t ok_cap = 0;
   void *d_blob1 = nullptr;       // one blob of device scratch: pnb_get_state / pnb_set_state
   // a call failed after it had started to enqueue work: the streams' state is undefined until pnb_reset
   bool poisoned = false;
+
+  // Session pool (pnb_sessions_reserve): sessions [0, capacity) are resident in a slot or parked as a blob in d_park.
+  // The host-side plan says which; every session call applies its plan when it is enqueued, like hop / line_off / par.
+  bool sessions = false;
+  pnb::SessionPool pool;
+  char *d_park = nullptr;        // [capacity][kParkStride] parking blobs; magic 0 = a fresh (or rejected) session
+  float *d_sgr = nullptr;        // pnb_process_sessions_host_*: g/r of the call in list order, grown on first use
+  size_t sgr_bytes = 0;
+  std::vector<int> plan_row, plan_up;       // scratch of a session call: row map, and what is uploaded
+  std::vector<pnb::SessionMove> plan_moves;
 
   // optional per-kernel-class timing (pnb_profile_enable): CUDA events around every launch
   bool profiling = false;

@@ -43,6 +43,7 @@ struct SynthesisArgs {
   size_t out_stride;
   int postfilter;
   float *tap_g;            // [F][S][34] or null: the band gains as applied (after the optional post-filter)
+  const int *row;          // [n_streams] output row of each slot (session calls), or null: row s
 };
 
 // training-data records (train(), denoise.cpp:600-787): streams [0,N) are the noisy signals, [N,2N) the clean ones
@@ -74,8 +75,9 @@ int launch_pitch_only(const PitchOnlyArgs &a, cudaStream_t st);
 cudaError_t dsp_configure();
 int launch_analysis(const AnalysisArgs &a, cudaStream_t st);
 int launch_synthesis(const SynthesisArgs &a, cudaStream_t st);
+// row: [n_streams] input row of each slot (session calls), or null: row s
 int launch_stage_in(float *pcm, size_t pcm_stride, const float *in, const short *in16, size_t in_stride,
-                    int n_streams, int n_samples, cudaStream_t st, float i16_div = 32768.f);
+                    int n_streams, int n_samples, cudaStream_t st, float i16_div = 32768.f, const int *row = nullptr);
 int launch_slide_history(float *pcm, size_t pcm_stride, int n_streams, int n_samples, cudaStream_t st);
 
 // ---- network, fp32 FMA path (pnb_nn_f32.cu) ---------------------------------------------

@@ -1,6 +1,8 @@
 // pnb_state.cu -- batched per-stream state movement: the gather (export) and scatter (import, reset) kernels behind
 // pnb_export_states / pnb_import_states / pnb_reset_streams, and the one table that says where a stream's state lives
-// in an engine (state_segs).  pnb_get_state / pnb_set_state are the n = 1 case of the same kernels.
+// in an engine (state_segs).  pnb_get_state / pnb_set_state are the n = 1 case of the same kernels.  The session pool
+// (pnb_process_sessions_*) parks, unparks and relocates sessions with the same pieces (session_move_kernel) and keeps
+// its parking blobs with session_blob_kernel.
 //
 // A stream's state is a list of pieces (StateSeg): the history line at line_off, the overlap-add memory, pitch
 // continuity, the five live spectrum ring slots, and the network's conv histories and GRU states (fp32, or the tensor
@@ -48,23 +50,16 @@ __global__ void __launch_bounds__(256) state_check_kernel(const __grid_constant_
   }
 }
 
-// Warp w of the grid moves piece (w mod n_seg) of stream (w / n_seg).
-__global__ void __launch_bounds__(256) state_move_kernel(const __grid_constant__ StateArgs a) {
-  const unsigned lane = threadIdx.x & 31;
-  const long long task = (long long)blockIdx.x * kWarpsPerBlock + (threadIdx.x >> 5);
-  if (task >= (long long)a.n * a.n_seg) return;
-  const int i = (int)(task / a.n_seg), j = (int)(task - (long long)i * a.n_seg);
-  const StateSeg &g = a.seg[j];
-  char *eng = g.eng + (size_t)a.streams[i] * g.eng_stride;
-  char *blob = a.blobs ? a.blobs + (size_t)i * a.blob_stride : nullptr;
-  int mode = a.mode;
-  if (mode == kStateImport && !a.ok[i]) mode = kStateReset;  // a rejected blob leaves its stream fresh
+// One piece g of one stream: engine side at `eng`, blob at `blob` (null for a reset); `first`: the stream's first piece,
+// whose warp writes the blob's header on export.
+__device__ __forceinline__ void move_piece(int mode, const StateSeg &g, char *eng, char *blob, bool first, unsigned has_terms,
+                                           unsigned lane) {
   const unsigned n = g.n;
-  if (mode == kStateExport && j == 0 && lane == 0) {
+  if (mode == kStateExport && first && lane == 0) {
     StreamState *b = reinterpret_cast<StreamState *>(blob);
     b->magic = kStateMagic;
     b->version = kStateVersion;
-    b->has_terms = a.has_terms;
+    b->has_terms = has_terms;
   }
   switch (g.kind) {
     case kSegCopy: {
@@ -133,6 +128,120 @@ __global__ void __launch_bounds__(256) state_move_kernel(const __grid_constant__
   }
 }
 
+// Warp w of the grid moves piece (w mod n_seg) of stream (w / n_seg).
+__global__ void __launch_bounds__(256) state_move_kernel(const __grid_constant__ StateArgs a) {
+  const unsigned lane = threadIdx.x & 31;
+  const long long task = (long long)blockIdx.x * kWarpsPerBlock + (threadIdx.x >> 5);
+  if (task >= (long long)a.n * a.n_seg) return;
+  const int i = (int)(task / a.n_seg), j = (int)(task - (long long)i * a.n_seg);
+  const StateSeg &g = a.seg[j];
+  char *eng = g.eng + (size_t)a.streams[i] * g.eng_stride;
+  char *blob = a.blobs ? a.blobs + (size_t)i * a.blob_stride : nullptr;
+  int mode = a.mode;
+  if (mode == kStateImport && !a.ok[i]) mode = kStateReset;  // a rejected blob leaves its stream fresh
+  move_piece(mode, g, eng, blob, j == 0, a.has_terms, lane);
+}
+
+// The engine-side bytes of piece g, raw, from slot src to slot dst (a session moved between slots): the bf16 term
+// planes and fp16 GRU terms as they are, never through the blob's sums.
+__device__ __forceinline__ void relocate_piece(const StateSeg &g, char *dst, const char *src, unsigned lane) {
+  switch (g.kind) {
+    case kSegCopy:
+    case kSegEngZero:
+      copy_words(reinterpret_cast<unsigned *>(dst), reinterpret_cast<const unsigned *>(src), g.n, lane);
+      break;
+    case kSegTermBf16:
+    case kSegSplitF16:
+      for (unsigned k = lane; k < g.n; k += 32)
+        reinterpret_cast<unsigned short *>(dst)[k] = reinterpret_cast<const unsigned short *>(src)[k];
+      break;
+    default:
+      break;
+  }
+}
+
+// The state launch of a session call (pnb_session_plan.h): warp w handles piece (w mod n_seg) of move (w / n_seg).  It
+// first parks the slot's occupant (export of the piece to that session's blob), then fills the piece from the entering
+// session's blob (import; reset when the blob is marked fresh or rejected), or from the relocation source slot.  Parking
+// and filling one piece in one warp, in that order, is what keeps the launch race-free.  The three bf16 term planes of a
+// conv history are read by the sum piece as well, so the warp of the sum piece handles the whole group (the sum and its
+// three terms, the next three pieces) and the warps of the term pieces do nothing.  With a.blobs set (export of resident
+// sessions to the caller's blobs) `park` is the row of the caller's blob and nothing is filled.
+__global__ void __launch_bounds__(256) session_move_kernel(const __grid_constant__ StateArgs a) {
+  const unsigned lane = threadIdx.x & 31;
+  const long long task = (long long)blockIdx.x * kWarpsPerBlock + (threadIdx.x >> 5);
+  if (task >= (long long)a.n * a.n_seg) return;
+  const int i = (int)(task / a.n_seg), j = (int)(task - (long long)i * a.n_seg);
+  if (a.seg[j].kind == kSegTermBf16) return;  // handled with its sum piece
+  const int4 mv = reinterpret_cast<const int4 *>(a.moves)[i];
+  const int group = a.seg[j].kind == kSegSumBf16 ? 4 : 1;
+  const size_t slot = (size_t)mv.x;
+  if (mv.y >= 0) {
+    char *blob = a.blobs ? a.blobs + (size_t)mv.y * a.blob_stride : a.park + (size_t)mv.y * a.park_stride;
+    for (int q = 0; q < group; q++) {
+      const StateSeg &g = a.seg[j + q];
+      move_piece(kStateExport, g, g.eng + slot * g.eng_stride, blob, j == 0, a.has_terms, lane);
+    }
+  }
+  if (mv.z == kFillBlob) {
+    char *blob = a.park + (size_t)mv.w * a.park_stride;
+    const StreamState *b = reinterpret_cast<const StreamState *>(blob);
+    const int mode = b->magic == kStateMagic && b->version == kStateVersion ? kStateImport : kStateReset;
+    for (int q = 0; q < group; q++) {
+      const StateSeg &g = a.seg[j + q];
+      move_piece(mode, g, g.eng + slot * g.eng_stride, blob, false, a.has_terms, lane);
+    }
+  } else if (mv.z == kFillSlot) {
+    for (int q = 0; q < group; q++) {
+      const StateSeg &g = a.seg[j + q];
+      relocate_piece(g, g.eng + slot * g.eng_stride, g.eng + (size_t)mv.w * g.eng_stride, lane);
+    }
+  }
+}
+
+// Parking blobs of the listed sessions (a.streams: session ids), one block per session:
+//   import  the caller's blob i becomes the session's parking blob when state_check_kernel accepted it; a rejected one
+//           marks the parking blob fresh (magic 0), so the session is unparked as a reset stream
+//   export  the parking blob is written to the caller's blob a.rows[i] (i when null); a blob marked fresh is written as
+//           the blob of a fresh stream (zeros under the header)
+//   reset   marks the parking blob fresh
+__global__ void __launch_bounds__(256) session_blob_kernel(const __grid_constant__ StateArgs a) {
+  const int i = blockIdx.x;
+  unsigned *park = reinterpret_cast<unsigned *>(a.park + (size_t)a.streams[i] * a.park_stride);
+  constexpr unsigned kWords = sizeof(StreamState) / 4;
+  if (a.mode == kStateReset || (a.mode == kStateImport && !a.ok[i])) {
+    if (threadIdx.x == 0) park[0] = 0u;
+    return;
+  }
+  const int r = a.rows ? a.rows[i] : i;
+  unsigned *user = reinterpret_cast<unsigned *>(a.blobs + (size_t)r * a.blob_stride);
+  if (a.mode == kStateImport) {
+    for (unsigned k = threadIdx.x; k < kWords; k += blockDim.x) park[k] = user[k];
+    return;
+  }
+  const StreamState *b = reinterpret_cast<const StreamState *>(park);
+  const bool fresh = !(b->magic == kStateMagic && b->version == kStateVersion);
+  for (unsigned k = threadIdx.x; k < kWords; k += blockDim.x) user[k] = fresh ? 0u : park[k];
+  if (fresh && threadIdx.x == 0) {
+    StreamState *u = reinterpret_cast<StreamState *>(user);
+    u->magic = kStateMagic;
+    u->version = kStateVersion;
+    u->has_terms = a.has_terms;
+  }
+}
+
+// g/r of a session call in list order: dst[t][row[p]][:] = src[t][p][:] for the k computed slots
+__global__ void gr_gather_kernel(const float *__restrict__ src, float *__restrict__ dst, const int *__restrict__ row, int k,
+                                 int S, int F) {
+  const long long total = (long long)F * k * 68;
+  for (long long x = (long long)blockIdx.x * blockDim.x + threadIdx.x; x < total; x += (long long)gridDim.x * blockDim.x) {
+    const int c = (int)(x % 68);
+    const long long tp = x / 68;
+    const int p = (int)(tp % k), t = (int)(tp / k);
+    dst[((size_t)t * k + row[p]) * 68 + c] = src[((size_t)t * S + p) * 68 + c];
+  }
+}
+
 __global__ void state_clear_reject_kernel(int *status) {
   atomicAnd(status, ~kStatusRejected);
   status[1] = kNoRejectedSlot;
@@ -198,6 +307,21 @@ int launch_state_check(const StateArgs &a, cudaStream_t st) {
 int launch_state_move(const StateArgs &a, cudaStream_t st) {
   const long long warps = (long long)a.n * a.n_seg;
   state_move_kernel<<<(unsigned)((warps + kWarpsPerBlock - 1) / kWarpsPerBlock), 32 * kWarpsPerBlock, 0, st>>>(a);
+  return 1;
+}
+int launch_session_move(const StateArgs &a, cudaStream_t st) {
+  const long long warps = (long long)a.n * a.n_seg;
+  session_move_kernel<<<(unsigned)((warps + kWarpsPerBlock - 1) / kWarpsPerBlock), 32 * kWarpsPerBlock, 0, st>>>(a);
+  return 1;
+}
+int launch_session_blob(const StateArgs &a, cudaStream_t st) {
+  session_blob_kernel<<<a.n, 256, 0, st>>>(a);
+  return 1;
+}
+int launch_gr_gather(const float *src, float *dst, const int *row, int k, int S, int F, cudaStream_t st) {
+  const long long total = (long long)F * k * 68;
+  const long long blocks = (total + 255) / 256;
+  gr_gather_kernel<<<(unsigned)(blocks < 4096 ? blocks : 4096), 256, 0, st>>>(src, dst, row, k, S, F);
   return 1;
 }
 int launch_state_clear_reject(int *status, cudaStream_t st) {

@@ -77,6 +77,11 @@ struct StateArgs {
   // import checks
   int check_gru;         // tensor-mode engines refuse GRU states outside kStateGruBound
   int *status;           // the engine's status word [2]: bit 1 of [0] = a blob was rejected, [1] = lowest rejected slot
+  // session pool (session_move_kernel / session_blob_kernel): streams are then session ids
+  const int *moves;      // [n][4] SessionMove (pnb_session_plan.h)
+  const int *rows;       // session_blob_kernel export: caller's blob of entry i (null = i)
+  char *park;            // parking blob of session s at park + s * park_stride
+  size_t park_stride;
 };
 
 // Status bit raised when an import rejected a blob (reported once as PNB_ERR_ARG by the synchronising entry points).
@@ -89,5 +94,12 @@ int state_segs(const pnb_engine *e, StateSeg *seg);
 int launch_state_check(const StateArgs &a, cudaStream_t st);
 int launch_state_move(const StateArgs &a, cudaStream_t st);
 int launch_state_clear_reject(int *status, cudaStream_t st);
+// session pool: the state launch of a call (a.n moves), the parking-blob operations (a.n sessions), and the g/r of a
+// call in list order ([F][k][68] from the engine's [F][S][68])
+int launch_session_move(const StateArgs &a, cudaStream_t st);
+int launch_session_blob(const StateArgs &a, cudaStream_t st);
+int launch_gr_gather(const float *src, float *dst, const int *row, int k, int S, int F, cudaStream_t st);
+// Parking blobs are engine-owned: padded to 16 bytes
+constexpr size_t kParkStride = (sizeof(StreamState) + 15) / 16 * 16;
 
 }  // namespace pnb

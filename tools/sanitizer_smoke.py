@@ -5,8 +5,9 @@
 
 Exercises the fp32 path, the tensor path (one CTA pair's worth of streams), the post-filter, the int16 entry,
 the pipelined host entry, the training-data generator, the persistent fp32 GRU chain (both block sizes), submitted
-calls on the chain's anti-diagonal unit order, state export / import and the pitch-only kernel on tiny batches; prints
-a checksum per leg."""
+calls on the chain's anti-diagonal unit order, state export / import, a session-pool schedule (parks, unparks,
+relocations, fresh starts, session export / import / reset) and the pitch-only kernel on tiny batches; prints a checksum
+per leg."""
 import os
 import sys
 
@@ -19,7 +20,7 @@ from percepnet_b200.weights import synth_model  # noqa: E402
 
 
 def main():
-    legs = sys.argv[1:] or ["fp32", "tensor", "train", "fp32chain", "submit", "pitch"]
+    legs = sys.argv[1:] or ["fp32", "tensor", "train", "fp32chain", "submit", "sessions", "pitch"]
     m = synth_model(0)
     if "fp32" in legs:
         x = synth_pcm(5, 4, seed=3)
@@ -56,6 +57,25 @@ def main():
         e.wait()
         print("submit", [float(np.abs(o).sum()) for o in outs])
         e.close()
+    if "sessions" in legs:   # session pool on both network modes: every kind of move, list sizes across a row tile
+        for flags in (api.NN_FP32, api.NN_TENSOR):
+            S, N, F = 130, 400, 2
+            e = api.Engine(S, F, m, flags)
+            e.reserve_sessions(N)
+            rng = np.random.RandomState(13)
+            x = synth_pcm(S, F, seed=14)
+            sums = []
+            for c, k in enumerate((129, 130, 1, 128, 130, 64)):
+                ids = rng.choice(N if c > 2 else 200, size=k, replace=False).astype(np.int32)
+                if c == 3:
+                    e.reset_sessions(ids[:3])
+                    blobs = e.export_sessions(ids[3:9], None)
+                    e.import_sessions(ids[9:15], blobs)
+                o, gr = e.process_sessions(ids, x[:k], want_gr=True)
+                sums.append(float(np.abs(o).sum()) + float(gr.sum()))
+            e.wait()
+            print("sessions", flags, sums, e.session_stats())
+            e.close()
     if "pitch" in legs:
         buf = synth_pcm(40, 4, seed=12)[:, :1728].copy()
         r = api.pitch_only(buf, np.zeros(40, np.int32), np.zeros(40, np.float32))

@@ -241,6 +241,25 @@ int pnb_process_sessions_host_f32(pnb_engine *e, const int *ids, int n, const fl
                                   size_t out_stride, int n_frames, float *gr);
 int pnb_process_sessions_host_i16(pnb_engine *e, const int *ids, int n, const short *in, size_t in_stride, short *out,
                                   size_t out_stride, int n_frames, float *gr);
+/* Ragged session calls: session ids[i] advances by its own hops[i] hops, 1 <= hops[i] <= max_frames (hops is host
+ * memory, reusable when the call returns); the call is F = max(hops) hops long.  Row strides must be at least F*480;
+ * input row i is read for its first hops[i]*480 samples only (the host forms copy F*480 samples of every row, the
+ * rest is ignored); output row i holds hops[i] hops of output followed by zeros up to F*480; gr / d_gr is [F][n][68]
+ * with gr[t][i] = 0 for t >= hops[i].  Each session ends in the state of its own hops[i] hops and continues bit for bit
+ * like a plain engine fed the same hops back to back; sessions not listed keep their state.  Residency, ordering,
+ * blocking, poisoning and error codes are those of pnb_process_sessions_*, which refuse the same arguments; a ragged
+ * call also refuses hops == NULL and any hops[i] outside [1, max_frames], with PNB_ERR_ARG before anything changes.
+ * When every hops[i] == F the call is pnb_process_sessions_*(..., F, ...): the same launches, the same results.  A
+ * call with a shorter session adds one launch (the fix-up that moves the early finishers' state to the call's end).
+ * PNB_KEEP_TAPS taps of the hops a session did not run are unspecified. */
+int pnb_process_sessions_ragged_device_f32(pnb_engine *e, const int *ids, const int *hops, int n, const float *d_in,
+                                           size_t in_stride, float *d_out, size_t out_stride, float *d_gr, void *cuda_stream);
+int pnb_process_sessions_ragged_device_i16(pnb_engine *e, const int *ids, const int *hops, int n, const short *d_in,
+                                           size_t in_stride, short *d_out, size_t out_stride, float *d_gr, void *cuda_stream);
+int pnb_process_sessions_ragged_host_f32(pnb_engine *e, const int *ids, const int *hops, int n, const float *in,
+                                         size_t in_stride, float *out, size_t out_stride, float *gr);
+int pnb_process_sessions_ragged_host_i16(pnb_engine *e, const int *ids, const int *hops, int n, const short *in,
+                                         size_t in_stride, short *out, size_t out_stride, float *gr);
 int pnb_reset_sessions(pnb_engine *e, const int *ids, int n, void *cuda_stream);
 int pnb_export_sessions(pnb_engine *e, const int *ids, int n, void *d_blobs, size_t blob_stride, void *cuda_stream);
 int pnb_import_sessions(pnb_engine *e, const int *ids, int n, const void *d_blobs, size_t blob_stride, void *cuda_stream);
@@ -296,7 +315,8 @@ const char *pnb_kernel_class_name(int cls);
 /* Number of kernels this library has launched on behalf of e since creation. */
 long long pnb_launch_count(const pnb_engine *e);
 /* Kernel launches one pnb_process_* call with n_frames hops issues (one more on the calls that also move the
- * streams' history back to the start of their rows, at most every call, typically every eighth). */
+ * streams' history back to the start of their rows, at most every call, typically every eighth; one more on a ragged
+ * session call in which some session runs fewer than n_frames = max(hops) hops). */
 int pnb_launches_per_call(const pnb_engine *e, int n_frames);
 int pnb_n_streams(const pnb_engine *e);
 int pnb_max_frames(const pnb_engine *e);

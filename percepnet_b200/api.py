@@ -76,6 +76,10 @@ def load_library() -> C.CDLL:
     L.pnb_process_sessions_device_i16.argtypes = [vp, vp, i, vp, sz, vp, sz, i, vp, vp]
     L.pnb_process_sessions_host_f32.argtypes = [vp, vp, i, vp, sz, vp, sz, i, vp]
     L.pnb_process_sessions_host_i16.argtypes = [vp, vp, i, vp, sz, vp, sz, i, vp]
+    L.pnb_process_sessions_ragged_device_f32.argtypes = [vp, vp, vp, i, vp, sz, vp, sz, vp, vp]
+    L.pnb_process_sessions_ragged_device_i16.argtypes = [vp, vp, vp, i, vp, sz, vp, sz, vp, vp]
+    L.pnb_process_sessions_ragged_host_f32.argtypes = [vp, vp, vp, i, vp, sz, vp, sz, vp]
+    L.pnb_process_sessions_ragged_host_i16.argtypes = [vp, vp, vp, i, vp, sz, vp, sz, vp]
     L.pnb_reset_sessions.argtypes = [vp, vp, i, vp]
     L.pnb_export_sessions.argtypes = [vp, vp, i, vp, sz, vp]
     L.pnb_import_sessions.argtypes = [vp, vp, i, vp, sz, vp]
@@ -103,7 +107,9 @@ EXPORTS = ("pnb_create", "pnb_destroy", "pnb_reset", "pnb_process_host_f32", "pn
            "pnb_read_tap", "pnb_state_size", "pnb_get_state", "pnb_set_state",
            "pnb_reset_streams", "pnb_export_states", "pnb_import_states", "pnb_set_active_streams", "pnb_active_streams",
            "pnb_sessions_reserve", "pnb_process_sessions_device_f32", "pnb_process_sessions_device_i16",
-           "pnb_process_sessions_host_f32", "pnb_process_sessions_host_i16", "pnb_reset_sessions", "pnb_export_sessions",
+           "pnb_process_sessions_host_f32", "pnb_process_sessions_host_i16", "pnb_process_sessions_ragged_device_f32",
+           "pnb_process_sessions_ragged_device_i16", "pnb_process_sessions_ragged_host_f32",
+           "pnb_process_sessions_ragged_host_i16", "pnb_reset_sessions", "pnb_export_sessions",
            "pnb_import_sessions", "pnb_session_stats", "pnb_pitch_only_device", "pnb_pitch_only_host", "pnb_launch_count",
            "pnb_launches_per_call", "pnb_profile_enable", "pnb_profile_read", "pnb_profile_timeline", "pnb_kernel_class_name", "pnb_n_streams", "pnb_max_frames", "pnb_last_error", "pnb_version")
 
@@ -317,9 +323,11 @@ class Engine:
         a later, larger call grows the pool and keeps every session's state."""
         self._ck(self.L.pnb_sessions_reserve(self.h, n_sessions), "pnb_sessions_reserve")
 
-    def process_sessions(self, ids, x: np.ndarray, want_gr: bool = False):
+    def process_sessions(self, ids, x: np.ndarray, want_gr: bool = False, hops=None):
         """pnb_process_sessions_host_*: advances exactly the listed sessions.  x: [len(ids), F*480] float32 or int16 host
-        array, row i for ids[i].  Returns (out like x, gr [F, len(ids), 68] or None)."""
+        array, row i for ids[i].  Returns (out like x, gr [F, len(ids), 68] or None).
+        hops: None, or one hop count per session (pnb_process_sessions_ragged_host_*): session ids[i] advances by
+        hops[i], F = max(hops) must be x's width in hops, and row i of out / gr[:, i] is zero after hops[i] hops."""
         a, n = self._slots(ids)
         assert x.ndim == 2 and x.shape[0] == n and x.shape[1] % FRAME == 0
         F = x.shape[1] // FRAME
@@ -327,23 +335,39 @@ class Engine:
         out = np.empty_like(x)
         gr = np.empty((F, n, 68), np.float32) if want_gr else None
         grp = gr.ctypes.data if want_gr else None
-        if x.dtype == np.float32:
-            f = self.L.pnb_process_sessions_host_f32
-        elif x.dtype == np.int16:
-            f = self.L.pnb_process_sessions_host_i16
-        else:
+        if x.dtype not in (np.float32, np.int16):
             raise TypeError("x must be float32 or int16")
-        self._ck(f(self.h, a.ctypes.data, n, x.ctypes.data, x.shape[1], out.ctypes.data, x.shape[1], F, grp),
-                 "pnb_process_sessions_host")
+        i16 = x.dtype == np.int16
+        if hops is None:
+            f = self.L.pnb_process_sessions_host_i16 if i16 else self.L.pnb_process_sessions_host_f32
+            self._ck(f(self.h, a.ctypes.data, n, x.ctypes.data, x.shape[1], out.ctypes.data, x.shape[1], F, grp),
+                     "pnb_process_sessions_host")
+            return out, gr
+        hp, nh = self._slots(hops)
+        if nh != n or int(hp.max(initial=0)) != F:
+            raise PnbError("process_sessions: hops needs one entry per session, and x must be max(hops) hops wide")
+        f = self.L.pnb_process_sessions_ragged_host_i16 if i16 else self.L.pnb_process_sessions_ragged_host_f32
+        self._ck(f(self.h, a.ctypes.data, hp.ctypes.data, n, x.ctypes.data, x.shape[1], out.ctypes.data, x.shape[1], grp),
+                 "pnb_process_sessions_ragged_host")
         return out, gr
 
-    def process_sessions_device(self, ids, d_in: int, in_stride: int, d_out: int, out_stride: int, n_frames: int,
-                                d_gr: int = 0, stream: int = 0, int16: bool = False):
-        """pnb_process_sessions_device_*: raw device pointers, row i of in / out and d_gr[t][i] for ids[i]."""
+    def process_sessions_device(self, ids, d_in: int, in_stride: int, d_out: int, out_stride: int, n_frames: int = 0,
+                                d_gr: int = 0, stream: int = 0, int16: bool = False, hops=None):
+        """pnb_process_sessions_device_*: raw device pointers, row i of in / out and d_gr[t][i] for ids[i].
+        hops: None, or one hop count per session (pnb_process_sessions_ragged_device_*; n_frames is then max(hops) and
+        need not be given)."""
         a, n = self._slots(ids)
-        f = self.L.pnb_process_sessions_device_i16 if int16 else self.L.pnb_process_sessions_device_f32
-        self._ck(f(self.h, a.ctypes.data, n, d_in, in_stride, d_out, out_stride, n_frames, d_gr or None, stream or None),
-                 "pnb_process_sessions_device")
+        if hops is None:
+            f = self.L.pnb_process_sessions_device_i16 if int16 else self.L.pnb_process_sessions_device_f32
+            self._ck(f(self.h, a.ctypes.data, n, d_in, in_stride, d_out, out_stride, n_frames, d_gr or None, stream or None),
+                     "pnb_process_sessions_device")
+            return
+        hp, nh = self._slots(hops)
+        if nh != n or (n_frames and int(hp.max(initial=0)) != n_frames):
+            raise PnbError("process_sessions_device: hops needs one entry per session, and n_frames (if given) = max(hops)")
+        f = self.L.pnb_process_sessions_ragged_device_i16 if int16 else self.L.pnb_process_sessions_ragged_device_f32
+        self._ck(f(self.h, a.ctypes.data, hp.ctypes.data, n, d_in, in_stride, d_out, out_stride, d_gr or None,
+                   stream or None), "pnb_process_sessions_ragged_device")
 
     def reset_sessions(self, ids, stream: int = 0):
         """pnb_reset_sessions: the listed sessions start over as fresh streams."""

@@ -733,13 +733,16 @@ __global__ void __launch_bounds__(AnaCfg<L>::kWarps * 32) analysis_kernel(Analys
   const float *row = A.pcm + (size_t)s * A.pcm_stride;
   int last_period = A.last_period[s];
   float last_gain = A.last_gain[s];
+  // a ragged call's slot walks its own hops: with two streams per warp the lane groups then run different trip counts,
+  // which is safe because every barrier and shuffle inside the hop loop is masked to the group
+  const int n_frames = A.hops ? A.hops[s] : A.n_frames;
 
 #ifdef PNB_ANA_TIMING
   unsigned long long ana_acc[16];
   for (int i = 0; i < 16; i++) ana_acc[i] = 0;
   long long ana_t0 = clock64();
 #endif
-  for (int t = 0; t < A.n_frames; t++) {
+  for (int t = 0; t < n_frames; t++) {
     const float *line = row + (size_t)t * kFrame;  // line[j] == reference comb_buf[j] at this hop
     const size_t fs = (size_t)t * A.stride + s;
 
@@ -750,7 +753,7 @@ __global__ void __launch_bounds__(AnaCfg<L>::kWarps * 32) analysis_kernel(Analys
     // of the whole group is laid out once in the scratch line and ONE LANE PER HOP runs the five sums of its hop,
     // sharing every loaded sample between the lags.  Same products, same order of additions as the reference.
     if (t % kAcHops == 0) {
-      const int G = (A.n_frames - t < kAcHops) ? A.n_frames - t : kAcHops;
+      const int G = (n_frames - t < kAcHops) ? n_frames - t : kAcHops;
       float *D = reinterpret_cast<float *>(W.fft);
       const float *src = line + kOffPitch;
       const int nD = kLp + 240 * (G - 1);
@@ -949,7 +952,8 @@ __global__ void __launch_bounds__(kSynWarps * 32) synthesis_kernel(SynthesisArgs
 #pragma unroll
   for (int i = 0; i < 15; i++) mem[i] = A.synth_mem[(size_t)s * kFrame + lane + 32 * i];
 
-  for (int t = 0; t < A.n_frames; t++) {
+  const int n_frames = A.hops ? A.hops[s] : A.n_frames;  // a ragged call's slot: its own hops, zeros after them
+  for (int t = 0; t < n_frames; t++) {
     const size_t fs = (size_t)t * A.stride + s;
     const float *gr = A.gr + fs * 68;
     for (int b = lane; b < kBands; b += 32) {
@@ -1029,6 +1033,14 @@ __global__ void __launch_bounds__(kSynWarps * 32) synthesis_kernel(SynthesisArgs
     }
     __syncwarp();
   }
+  for (int t = n_frames; t < A.n_frames; t++) {
+    float *outp = A.out ? A.out + (size_t)orow * A.out_stride + (size_t)t * kFrame : nullptr;
+    short *outs = A.out16 ? A.out16 + (size_t)orow * A.out_stride + (size_t)t * kFrame : nullptr;
+    for (int n = lane; n < kFrame; n += 32) {
+      if (outp) outp[n] = 0.f;
+      if (outs) outs[n] = 0;
+    }
+  }
 #pragma unroll
   for (int i = 0; i < 15; i++) A.synth_mem[(size_t)s * kFrame + lane + 32 * i] = mem[i];
 }
@@ -1037,11 +1049,12 @@ __global__ void __launch_bounds__(kSynWarps * 32) synthesis_kernel(SynthesisArgs
 // staging: append the new hops to each stream's PCM line / slide the history forward
 // ------------------------------------------------------------------------------------------
 __global__ void stage_in_kernel(float *pcm, size_t pcm_stride, const float *in, const short *in16, size_t in_stride,
-                                int n_streams, int n_samples, float i16_div, const int *row) {
+                                int n_streams, int n_samples, float i16_div, const int *row, const int *hops) {
   const int s = blockIdx.x;  // streams on grid.x (no 65535 limit), chunks of the row on grid.y
   const size_t r = row ? row[s] : s;  // input row of slot s
+  const int n = hops ? hops[s] * kFrame : n_samples;  // a ragged call reads only the slot's own hops
   float *dst = pcm + (size_t)s * pcm_stride + kKeep;
-  for (int i = blockIdx.y * blockDim.x + threadIdx.x; i < n_samples; i += gridDim.y * blockDim.x) {
+  for (int i = blockIdx.y * blockDim.x + threadIdx.x; i < n; i += gridDim.y * blockDim.x) {
     float v;
     if (in) v = in[r * in_stride + i];
     else v = ((float)in16[r * in_stride + i]) / i16_div;  // main.cpp:34 (32768) / denoise.cpp:681 (NORM_RATIO 1)
@@ -1213,9 +1226,9 @@ int launch_synthesis(const SynthesisArgs &a, cudaStream_t st) {
   return 1;
 }
 int launch_stage_in(float *pcm, size_t pcm_stride, const float *in, const short *in16, size_t in_stride,
-                    int n_streams, int n_samples, cudaStream_t st, float i16_div, const int *row) {
+                    int n_streams, int n_samples, cudaStream_t st, float i16_div, const int *row, const int *hops) {
   dim3 grid(n_streams, (n_samples + 1023) / 1024 > 8 ? 8 : (n_samples + 1023) / 1024);
-  stage_in_kernel<<<grid, 256, 0, st>>>(pcm, pcm_stride, in, in16, in_stride, n_streams, n_samples, i16_div, row);
+  stage_in_kernel<<<grid, 256, 0, st>>>(pcm, pcm_stride, in, in16, in_stride, n_streams, n_samples, i16_div, row, hops);
   return 1;
 }
 int launch_slide_history(float *pcm, size_t pcm_stride, int n_streams, int n_samples, cudaStream_t st) {

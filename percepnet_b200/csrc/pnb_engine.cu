@@ -470,7 +470,8 @@ static GemmSeg seg(const float *A, int lda, const float *B, int ldb, int K) {
 // The network of hops [h0, h0 + n) of a call (n <= e->f32_chunk) in fp32 FMA (rnn.cpp:42-81): the non-recurrent layers
 // once over the active rows of all n hop slots, the five GRUs of all n hops in one persistent launch, the output layers
 // over the same rows, and the carry that moves the conv histories and the states back to the front of their slot buffers.
-static int nn_chunk_f32(pnb_engine *e, int h0, int n, cudaStream_t st) {
+// hops: the per-slot hops of a ragged call (device), or null.
+static int nn_chunk_f32(pnb_engine *e, int h0, int n, const int *hops, cudaStream_t st) {
   const int S = e->S, na = e->n_active;
   // all streams active: the rows of the n slots are one flat range; otherwise the first na rows of each slot
   const int rows = na == S ? n * S : na, slots = na == S ? 1 : n;
@@ -538,20 +539,21 @@ static int nn_chunk_f32(pnb_engine *e, int h0, int n, cudaStream_t st) {
   g.seg[0] = seg(e->h[4][0] + (size_t)S * 128, 128, e->fc_rb.W, 34, 128);
   g.n_seg = 1; g.N = 34; g.C = gr + 34; g.ldc = 68; g.bias = e->fc_rb.b; g.act = e->act_rb;
   { ProfScope ps(e, PNB_K_GEMM_F32, st); nl += launch_gemm_f32(g, st); }
-  // carry
+  // carry; in a ragged call a row that stopped inside the chunk takes its own last hop's slots, one that stopped in an
+  // earlier chunk keeps its front slots
   F32CarryArgs c;
   memset(&c, 0, sizeof c);
   int ns = 0;
-  auto cseg = [&](float *base, size_t width, int n_slots, int from) {  // the active rows of n_slots slots of [S][width]
-    c.seg[ns++] = F32CarrySeg{reinterpret_cast<float4 *>(base), reinterpret_cast<const float4 *>(base + (size_t)from * S * width),
-                              (size_t)na * width / 4, (size_t)S * width / 4, n_slots};
+  auto cseg = [&](float *dst, const float *src, size_t width, int n_slots, int from) {  // the active rows of n_slots slots of [S][width]
+    c.seg[ns++] = F32CarrySeg{reinterpret_cast<float4 *>(dst), reinterpret_cast<const float4 *>(src), (size_t)na * width / 4,
+                              (size_t)S * width / 4, width / 4, n_slots, from};
   };
-  cseg(e->ring_fc, 128, 4, n);
-  cseg(e->ring_c1, 512, 2, n);
-  for (int li = 0; li < 5; li++) cseg(e->h[li][0], e->gru[li].H, 1, n);
-  c.seg[ns++] = F32CarrySeg{reinterpret_cast<float4 *>(e->c2), reinterpret_cast<const float4 *>(e->c2_all + (size_t)(n - 1) * S * 512),
-                            (size_t)na * 512 / 4, (size_t)S * 512 / 4, 1};
+  cseg(e->ring_fc, e->ring_fc, 128, 4, n);
+  cseg(e->ring_c1, e->ring_c1, 512, 2, n);
+  for (int li = 0; li < 5; li++) cseg(e->h[li][0], e->h[li][0], e->gru[li].H, 1, n);
+  cseg(e->c2, e->c2_all, 512, 1, n - 1);
   c.n_seg = ns; c.cnt = e->f32_cnt; c.n_cnt = 5 * e->f32_rb;
+  c.hops = hops; c.h0 = h0; c.n = n;
   { ProfScope ps(e, PNB_K_F32_CARRY, st); nl += launch_f32_carry(c, st); }
   return nl;
 }
@@ -576,6 +578,7 @@ static AnalysisArgs analysis_args(pnb_engine *e, int F) {
   a.P = e->d_P; a.Ex = e->d_Ex; a.raw = nullptr; a.silence = e->d_sil;
   a.last_period = e->d_last_period; a.last_gain = e->d_last_gain;
   a.tap_pitch = e->d_tap_pitch; a.tap_pitchf = e->d_tap_pitchf;
+  a.hops = nullptr;
   return a;
 }
 static SynthesisArgs synthesis_args(pnb_engine *e, int F, float *d_out, short *d_out16, size_t out_stride) {
@@ -587,6 +590,7 @@ static SynthesisArgs synthesis_args(pnb_engine *e, int F, float *d_out, short *d
   s.postfilter = (e->flags & PNB_POSTFILTER) ? 1 : 0;
   s.tap_g = e->d_tap_g;
   s.row = nullptr;
+  s.hops = nullptr;
   return s;
 }
 
@@ -678,10 +682,19 @@ static StateArgs session_args(pnb_engine *e) {
   return a;
 }
 
-// A session call's residency plan, applied (pnb_session_plan.h), its upload (row map, then the moves), and its state
-// launch when membership changed.  Sets the active range to the list; *d_row: the row map on the device.  Returns the
-// number of launches or a negative error.
-static int enqueue_plan(pnb_engine *e, const int *ids, int k, cudaStream_t st, const int **d_row) {
+// The per-slot part of a ragged session call on the device: hops[p] of slot p, and the slots that stop before the
+// call's last hop.  All null / 0 for every other call.
+struct RaggedSlots {
+  const int *hops = nullptr;
+  const int *slots = nullptr;
+  int n_short = 0;
+};
+
+// A session call's residency plan, applied (pnb_session_plan.h), its upload (row map, then the moves, then for a ragged
+// call the hops of every slot and the slots with fewer than F), and its state launch when membership changed.  Sets the
+// active range to the list; *d_row: the row map on the device.  Returns the number of launches or a negative error.
+static int enqueue_plan(pnb_engine *e, const int *ids, int k, const int *hops, int F, cudaStream_t st, const int **d_row,
+                        RaggedSlots *rg) {
   StateArgs a = session_args(e);  // before the plan: parking reads the pieces where the last call left them
   e->pool.plan(ids, k, e->plan_row, e->plan_moves);
   e->n_active = k;
@@ -691,9 +704,20 @@ static int enqueue_plan(pnb_engine *e, const int *ids, int k, cudaStream_t st, c
   up.resize(k4, 0);
   const int *mv = reinterpret_cast<const int *>(e->plan_moves.data());
   up.insert(up.end(), mv, mv + 4 * e->plan_moves.size());
+  const size_t at_hops = up.size();
+  if (hops) {  // slot p runs the hops of its list row; then the slots that stop early
+    for (int p = 0; p < k; p++) up.push_back(hops[e->plan_row[p]]);
+    for (int p = 0; p < k; p++)
+      if (hops[e->plan_row[p]] < F) up.push_back(p);
+  }
   const int *d = nullptr;
   { int rc = stage_ints(e, up.data(), up.size(), st, &d); if (rc) return rc; }
   *d_row = d;
+  if (hops) {
+    rg->hops = d + at_hops;
+    rg->slots = d + at_hops + k;
+    rg->n_short = (int)(up.size() - at_hops - k);
+  }
   if (e->plan_moves.empty()) return 0;
   a.n = (int)e->plan_moves.size();
   a.moves = d + k4;
@@ -701,28 +725,36 @@ static int enqueue_plan(pnb_engine *e, const int *ids, int k, cudaStream_t st, c
 }
 
 // One enhancement call on st (arguments already checked).  With a session list (ids, n_ids) the call first applies its
-// residency plan, and reads input row / writes output row and g/r row row[p] for slot p.
+// residency plan, and reads input row / writes output row and g/r row row[p] for slot p.  With hops (host, list order;
+// a ragged call, F = the largest) slot p runs the hops of its list row, and the slots that stop early are moved to the
+// counters of hop F after synthesis.
 static int enqueue_enhance(pnb_engine *e, const float *d_in, const short *d_in16, size_t in_stride, float *d_out,
                            short *d_out16, size_t out_stride, int F, float *d_gr, cudaStream_t st, const int *ids = nullptr,
-                           int n_ids = 0) {
+                           int n_ids = 0, const int *hops = nullptr) {
   return enqueue_call(e, F, st, [&]() -> int {
     int n = 0;
     const int *row = nullptr;
+    RaggedSlots rg;
     if (ids) {
-      n = enqueue_plan(e, ids, n_ids, st, &row);
+      n = enqueue_plan(e, ids, n_ids, hops, F, st, &row, &rg);
       if (n < 0) return n;
     }
     const int S = e->S, na = e->n_active;  // the call advances streams [0, na); per-call buffers keep the stride S
-    { ProfScope ps(e, PNB_K_STAGE_IN, st); n += launch_stage_in(e->d_pcm + e->line_off, e->pcm_stride, d_in, d_in16, in_stride, na, F * kFrame, st, 32768.f, row); }
-    { ProfScope ps(e, PNB_K_ANALYSIS, st); n += launch_analysis(analysis_args(e, F), st); }
+    { ProfScope ps(e, PNB_K_STAGE_IN, st); n += launch_stage_in(e->d_pcm + e->line_off, e->pcm_stride, d_in, d_in16, in_stride, na, F * kFrame, st, 32768.f, row, rg.hops); }
+    {
+      AnalysisArgs aa = analysis_args(e, F);
+      aa.hops = rg.hops;
+      ProfScope ps(e, PNB_K_ANALYSIS, st);
+      n += launch_analysis(aa, st);
+    }
     CK(cudaGetLastError());
     if (e->flags & PNB_NN_TENSOR) {
-      const int q = tc_network(e, F, st);
+      const int q = tc_network(e, F, rg.hops, st);
       if (q < 0) return q;
       n += q;
     } else {
       for (int h0 = 0; h0 < F; h0 += e->f32_chunk) {
-        const int q = nn_chunk_f32(e, h0, F - h0 < e->f32_chunk ? F - h0 : e->f32_chunk, st);
+        const int q = nn_chunk_f32(e, h0, F - h0 < e->f32_chunk ? F - h0 : e->f32_chunk, rg.hops, st);
         if (q < 0) return q;
         n += q;
       }
@@ -730,12 +762,17 @@ static int enqueue_enhance(pnb_engine *e, const float *d_in, const short *d_in16
     {
       SynthesisArgs sa = synthesis_args(e, F, d_out, d_out16, out_stride);
       sa.row = row;
+      sa.hops = rg.hops;
       ProfScope ps(e, PNB_K_SYNTHESIS, st);
       n += launch_synthesis(sa, st);
     }
+    if (rg.n_short) {  // before the slide: it moves the window the counters of hop F point at
+      ProfScope ps(e, PNB_K_SLIDE, st);
+      n += launch_ragged_carry(e, F, rg.hops, rg.slots, rg.n_short, st);
+    }
     n += advance_line(e, F, st);
     if (d_gr && row)  // [F][na][68] in list order
-      n += launch_gr_gather(e->d_gr, d_gr, row, na, S, F, st);
+      n += launch_gr_gather(e->d_gr, d_gr, row, na, S, F, st, rg.hops);
     else if (d_gr)  // [F][na][68] from the [F][S][68] buffer
       CK(cudaMemcpy2DAsync(d_gr, (size_t)na * 68 * sizeof(float), e->d_gr, (size_t)S * 68 * sizeof(float), (size_t)na * 68 * sizeof(float), F,
                            cudaMemcpyDeviceToDevice, st));
@@ -759,6 +796,30 @@ static int check_ids(pnb_engine *e, const int *ids, int n, int n_max) {
   const int d = e->pool.duplicate(ids, n);
   if (d >= 0) return fail(PNB_ERR_ARG, "session %d listed twice (ids[%d])", ids[d], d);
   return PNB_OK;
+}
+
+// Every session call's check (pnb_process_sessions_* and pnb_process_sessions_ragged_*): check_call and the list.  A
+// ragged call (ragged) checks its hop counts first, because their largest is the call's length *F; when every session
+// runs *F hops, *hops becomes null and the call is the plain session call of *F hops.
+static int check_sessions(pnb_engine *e, bool buffers, const int *ids, int n, bool ragged, const int **hops, int *F,
+                          size_t in_stride, size_t out_stride) {
+  if (ragged) {
+    if (!e) return fail(PNB_ERR_ARG, "engine is NULL");
+    { int rc = check_ids(e, ids, n, e->S); if (rc) return rc; }
+    const int *h = *hops;
+    if (!h) return fail(PNB_ERR_ARG, "hops is NULL");
+    int mx = 0;
+    for (int i = 0; i < n; i++) {
+      if (h[i] < 1 || h[i] > e->Fmax) return fail(PNB_ERR_ARG, "hops[%d] = %d outside [1, %d]", i, h[i], e->Fmax);
+      mx = h[i] > mx ? h[i] : mx;
+    }
+    bool uniform = true;
+    for (int i = 0; i < n; i++) uniform = uniform && h[i] == mx;
+    *F = mx;
+    if (uniform) *hops = nullptr;
+  }
+  { int rc = check_call(e, false, buffers, *F, in_stride, out_stride); if (rc) return rc; }
+  return ragged ? PNB_OK : check_ids(e, ids, n, e->S);
 }
 
 static int process_device(pnb_engine *e, const float *d_in, const short *d_in16, size_t in_stride, float *d_out,
@@ -935,28 +996,34 @@ static int report_status(pnb_engine *e) {
   return PNB_OK;
 }
 
-// pnb_process_host_* (blocking) and pnb_submit_host_* (pipelined); with a session list (ids, n_ids) the blocking
-// pnb_process_sessions_host_*.  The blocking form then copies g/r and the status word back on the engine's stream too,
-// and synchronises it once.
+// pnb_process_host_* (blocking) and pnb_submit_host_* (pipelined); with `sessions` the blocking
+// pnb_process_sessions_host_* of the list (ids, n_ids), and with `ragged` too pnb_process_sessions_ragged_host_* (hops;
+// F is then the largest).  The blocking form then copies g/r and the status word back on the engine's stream too, and
+// synchronises it once.  Rows travel F hops wide: a ragged call's input beyond a row's hops is copied but not read.
 template <typename T>
 static int host_call(pnb_engine *e, const T *in, size_t in_stride, T *out, size_t out_stride, int F, float *gr, bool pipelined,
-                     const int *ids = nullptr, int n_ids = 0) {
-  { int rc = check_call(e, false, in && out, F, in_stride, out_stride); if (rc) return rc; }
-  if (!ids && e->sessions) return refuse_in_session_mode();
-  if (ids) { int rc = check_ids(e, ids, n_ids, e->S); if (rc) return rc; }
+                     bool sessions = false, const int *ids = nullptr, int n_ids = 0, bool ragged = false,
+                     const int *hops = nullptr) {
+  if (sessions) {
+    int rc = check_sessions(e, in && out, ids, n_ids, ragged, &hops, &F, in_stride, out_stride);
+    if (rc) return rc;
+  } else {
+    { int rc = check_call(e, false, in && out, F, in_stride, out_stride); if (rc) return rc; }
+    if (e->sessions) return refuse_in_session_mode();
+  }
   CK(cudaSetDevice(e->device));
   const size_t S = e->S, row = (size_t)e->Fmax * kFrame, w = (size_t)F * kFrame * sizeof(T);
-  const size_t na = ids ? n_ids : e->n_active;  // the rows of in / out / gr
+  const size_t na = sessions ? n_ids : e->n_active;  // the rows of in / out / gr
   const int k = staging_slot(e, pipelined, S * row * sizeof(T), S * row * sizeof(T));
   if (k < 0) return k;
-  if (ids && gr) { int rc = grow((void **)&e->d_sgr, &e->sgr_bytes, (size_t)e->Fmax * S * 68 * sizeof(float)); if (rc) return rc; }
-  float *d_gr = ids && gr ? e->d_sgr : nullptr;  // session calls gather g/r in list order on the device
+  if (sessions && gr) { int rc = grow((void **)&e->d_sgr, &e->sgr_bytes, (size_t)e->Fmax * S * 68 * sizeof(float)); if (rc) return rc; }
+  float *d_gr = sessions && gr ? e->d_sgr : nullptr;  // session calls gather g/r in list order on the device
   T *d_in = (T *)e->stage[k].in, *d_out = (T *)e->stage[k].out;
   const int rc = round_trip(e, k, pipelined,
       [&](cudaStream_t s) { return cudaMemcpy2DAsync(d_in, row * sizeof(T), in, in_stride * sizeof(T), w, na, cudaMemcpyHostToDevice, s); },
       [&] {
-        return sizeof(T) == 4 ? enqueue_enhance(e, (const float *)d_in, nullptr, row, (float *)d_out, nullptr, row, F, d_gr, e->stream, ids, n_ids)
-                              : enqueue_enhance(e, nullptr, (const short *)d_in, row, nullptr, (short *)d_out, row, F, d_gr, e->stream, ids, n_ids);
+        return sizeof(T) == 4 ? enqueue_enhance(e, (const float *)d_in, nullptr, row, (float *)d_out, nullptr, row, F, d_gr, e->stream, ids, n_ids, hops)
+                              : enqueue_enhance(e, nullptr, (const short *)d_in, row, nullptr, (short *)d_out, row, F, d_gr, e->stream, ids, n_ids, hops);
       },
       [&](cudaStream_t s) { return cudaMemcpy2DAsync(out, out_stride * sizeof(T), d_out, row * sizeof(T), w, na, cudaMemcpyDeviceToHost, s); });
   if (rc || pipelined) return rc;
@@ -1217,8 +1284,9 @@ extern "C" int pnb_sessions_reserve(pnb_engine *e, int n_sessions) {
   CK(cudaSetDevice(e->device));
   CK(cudaDeviceSynchronize());
   const size_t cap = (size_t)n_sessions, wide = cap > (size_t)e->S ? cap : (size_t)e->S;
-  // staging: a call's row map and moves (<= 5 S + 3 ints), an export's moves, ids and rows (<= 6 n)
-  { int rc = grow_ints(e, 6 * wide + 4); if (rc) return rc; }
+  // staging: a call's row map, moves, and for a ragged call slot hops and short slots (<= 7 S + 3 ints), an export's
+  // moves, ids and rows (<= 6 n)
+  { int rc = grow_ints(e, 7 * wide + 4); if (rc) return rc; }
   if (wide > e->ok_cap) {
     int *ok = nullptr;
     CK(cudaMalloc((void **)&ok, wide * sizeof(int)));
@@ -1255,11 +1323,11 @@ extern "C" int pnb_session_stats(const pnb_engine *e, long long *out) {
 }
 
 static int process_sessions_device(pnb_engine *e, const int *ids, int n, const float *d_in, const short *d_in16, size_t in_stride,
-                                   float *d_out, short *d_out16, size_t out_stride, int F, float *d_gr, cudaStream_t st) {
-  { int rc = check_call(e, false, (d_in || d_in16) && (d_out || d_out16), F, in_stride, out_stride); if (rc) return rc; }
-  { int rc = check_ids(e, ids, n, e->S); if (rc) return rc; }
+                                   float *d_out, short *d_out16, size_t out_stride, int F, float *d_gr, cudaStream_t st,
+                                   bool ragged = false, const int *hops = nullptr) {
+  { int rc = check_sessions(e, (d_in || d_in16) && (d_out || d_out16), ids, n, ragged, &hops, &F, in_stride, out_stride); if (rc) return rc; }
   CK(cudaSetDevice(e->device));
-  return enqueue_enhance(e, d_in, d_in16, in_stride, d_out, d_out16, out_stride, F, d_gr, st, ids, n);
+  return enqueue_enhance(e, d_in, d_in16, in_stride, d_out, d_out16, out_stride, F, d_gr, st, ids, n, hops);
 }
 extern "C" int pnb_process_sessions_device_f32(pnb_engine *e, const int *ids, int n, const float *d_in, size_t in_stride,
                                                float *d_out, size_t out_stride, int n_frames, float *d_gr, void *cuda_stream) {
@@ -1274,12 +1342,34 @@ extern "C" int pnb_process_sessions_device_i16(pnb_engine *e, const int *ids, in
 extern "C" int pnb_process_sessions_host_f32(pnb_engine *e, const int *ids, int n, const float *in, size_t in_stride, float *out,
                                              size_t out_stride, int n_frames, float *gr) {
   if (!e) return fail(PNB_ERR_ARG, "engine is NULL");
-  return host_call<float>(e, in, in_stride, out, out_stride, n_frames, gr, false, ids, n);
+  return host_call<float>(e, in, in_stride, out, out_stride, n_frames, gr, false, true, ids, n);
 }
 extern "C" int pnb_process_sessions_host_i16(pnb_engine *e, const int *ids, int n, const short *in, size_t in_stride, short *out,
                                              size_t out_stride, int n_frames, float *gr) {
   if (!e) return fail(PNB_ERR_ARG, "engine is NULL");
-  return host_call<short>(e, in, in_stride, out, out_stride, n_frames, gr, false, ids, n);
+  return host_call<short>(e, in, in_stride, out, out_stride, n_frames, gr, false, true, ids, n);
+}
+
+// Ragged session calls: session ids[i] advances by hops[i]; the call is max(hops) hops long (check_sessions).
+extern "C" int pnb_process_sessions_ragged_device_f32(pnb_engine *e, const int *ids, const int *hops, int n, const float *d_in,
+                                                      size_t in_stride, float *d_out, size_t out_stride, float *d_gr,
+                                                      void *cuda_stream) {
+  return process_sessions_device(e, ids, n, d_in, nullptr, in_stride, d_out, nullptr, out_stride, 0, d_gr,
+                                 (cudaStream_t)cuda_stream, true, hops);
+}
+extern "C" int pnb_process_sessions_ragged_device_i16(pnb_engine *e, const int *ids, const int *hops, int n, const short *d_in,
+                                                      size_t in_stride, short *d_out, size_t out_stride, float *d_gr,
+                                                      void *cuda_stream) {
+  return process_sessions_device(e, ids, n, nullptr, d_in, in_stride, nullptr, d_out, out_stride, 0, d_gr,
+                                 (cudaStream_t)cuda_stream, true, hops);
+}
+extern "C" int pnb_process_sessions_ragged_host_f32(pnb_engine *e, const int *ids, const int *hops, int n, const float *in,
+                                                    size_t in_stride, float *out, size_t out_stride, float *gr) {
+  return host_call<float>(e, in, in_stride, out, out_stride, 0, gr, false, true, ids, n, true, hops);
+}
+extern "C" int pnb_process_sessions_ragged_host_i16(pnb_engine *e, const int *ids, const int *hops, int n, const short *in,
+                                                    size_t in_stride, short *out, size_t out_stride, float *gr) {
+  return host_call<short>(e, in, in_stride, out, out_stride, 0, gr, false, true, ids, n, true, hops);
 }
 
 // pnb_reset_sessions / pnb_export_sessions / pnb_import_sessions.  A reset or an import takes the listed sessions out
@@ -1477,7 +1567,8 @@ extern "C" int pnb_pitch_only_host(const float *pitch_buf, size_t stride, long l
 extern "C" long long pnb_launch_count(const pnb_engine *e) { return e ? e->launches : 0; }
 extern "C" int pnb_launches_per_call(const pnb_engine *e, int n_frames) {
   if (!e) return 0;
-  // without the history move of advance_line (at most one more launch per call)
+  // without the history move of advance_line (at most one more launch per call), and without the fix-up of a ragged
+  // session call in which a session runs fewer hops than the call (one more launch)
   if (e->flags & PNB_NN_TENSOR) return 10;  // stage_in, analysis, fc, conv1, conv2, GRU chain, fc_gb, fc_rb, carry, synthesis
   return 3 + 7 * ((n_frames + e->f32_chunk - 1) / e->f32_chunk);  // stage_in, analysis, synthesis + per chunk: fc, conv1, conv2, GRU chain, fc_gb, fc_rb, carry
 }

@@ -127,8 +127,9 @@ struct pnb_engine {
 int tc_prepare(pnb_engine *e, const pnb_model *model);
 void tc_release(pnb_engine *e);
 int tc_reset(pnb_engine *e);
-// the network of a call of F hops: hop-parallel front, the GRU chain, hop-parallel output layers, carry
-int tc_network(pnb_engine *e, int F, cudaStream_t st);
+// the network of a call of F hops: hop-parallel front, the GRU chain, hop-parallel output layers, carry; hops: the
+// per-slot hops of a ragged session call (device), or null
+int tc_network(pnb_engine *e, int F, const int *hops, cudaStream_t st);
 // The tensor path's pieces of a stream's state (pnb_state.cu): appended to seg[ns..]; returns the new count
 int tc_state_segs(const pnb_engine *e, pnb::StateSeg *seg, int ns);
 

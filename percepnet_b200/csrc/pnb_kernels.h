@@ -24,6 +24,7 @@ struct AnalysisArgs {
   float *last_gain;        // [S]
   int *tap_pitch;          // [F][S][4] or null
   float *tap_pitchf;       // [F][S][2] or null
+  const int *hops;         // [n_streams] hops of each slot (ragged session calls, each <= n_frames), or null: n_frames
 };
 
 struct SynthesisArgs {
@@ -44,6 +45,8 @@ struct SynthesisArgs {
   int postfilter;
   float *tap_g;            // [F][S][34] or null: the band gains as applied (after the optional post-filter)
   const int *row;          // [n_streams] output row of each slot (session calls), or null: row s
+  const int *hops;         // [n_streams] hops of each slot (ragged session calls), or null: n_frames; hops [hops[s],
+                           // n_frames) of a slot's output row are written as zeros
 };
 
 // training-data records (train(), denoise.cpp:600-787): streams [0,N) are the noisy signals, [N,2N) the clean ones
@@ -75,9 +78,11 @@ int launch_pitch_only(const PitchOnlyArgs &a, cudaStream_t st);
 cudaError_t dsp_configure();
 int launch_analysis(const AnalysisArgs &a, cudaStream_t st);
 int launch_synthesis(const SynthesisArgs &a, cudaStream_t st);
-// row: [n_streams] input row of each slot (session calls), or null: row s
+// row: [n_streams] input row of each slot (session calls), or null: row s.  hops: [n_streams] hops of each slot (ragged
+// session calls), or null: slot s copies hops[s] * 480 samples instead of n_samples
 int launch_stage_in(float *pcm, size_t pcm_stride, const float *in, const short *in16, size_t in_stride,
-                    int n_streams, int n_samples, cudaStream_t st, float i16_div = 32768.f, const int *row = nullptr);
+                    int n_streams, int n_samples, cudaStream_t st, float i16_div = 32768.f, const int *row = nullptr,
+                    const int *hops = nullptr);
 int launch_slide_history(float *pcm, size_t pcm_stride, int n_streams, int n_samples, cudaStream_t st);
 
 // ---- network, fp32 FMA path (pnb_nn_f32.cu) ---------------------------------------------
@@ -132,8 +137,19 @@ struct F32ChainArgs {
   const float *tansig;
 };
 int launch_gru_chain_f32(const F32ChainArgs &a, int rows_per_thread, int sm_count, cudaStream_t st);
-struct F32CarrySeg { float4 *dst; const float4 *src; size_t slot4, stride4; int n_slots; };  // first slot4 float4s of n_slots slots stride4 apart
-struct F32CarryArgs { F32CarrySeg seg[12]; int n_seg; unsigned *cnt; int n_cnt; };
+// The first slot4 float4s of n_slots slots stride4 apart, from slots from.. of src (slot 0 of the source buffer) to
+// dst; row4: float4s per row.  In a ragged call (hops) a row that stops after hop h of the call takes its slots from
+// from - (n - clamp(h - h0, 0, n)) on instead (it stopped that many slots before the chunk's end), and nothing moves
+// when that is below 0 or the row is already in place.
+struct F32CarrySeg { float4 *dst; const float4 *src; size_t slot4, stride4, row4; int n_slots, from; };
+struct F32CarryArgs {
+  F32CarrySeg seg[12];
+  int n_seg;
+  unsigned *cnt;
+  int n_cnt;
+  const int *hops;  // [active streams] hops of each row in a ragged call, or null
+  int h0, n;        // the chunk: hops [h0, h0 + n) of the call
+};
 int launch_f32_carry(const F32CarryArgs &a, cudaStream_t st);
 
 }  // namespace pnb

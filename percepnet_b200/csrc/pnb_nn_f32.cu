@@ -385,13 +385,22 @@ __global__ void __launch_bounds__(CH_THREADS, RT == 8 ? 2 : 4) gru_chain_f32_ker
 
 // End of a chunk of n hops: the last 4 fc / 2 conv1 slots and the last state slot move to the front (the active rows
 // of each), conv2's output of the last hop is kept for the tap, the chain's counters return to zero.  A thread owns the
-// same element of every slot.
+// same element of every slot and walks the slots upwards, so a slot that is both source and destination is read before
+// it is overwritten.  In a ragged call each row takes the slots of its own last hop (F32CarrySeg).
 __global__ void f32_carry_kernel(F32CarryArgs a) {
   const size_t tid = (size_t)blockIdx.x * blockDim.x + threadIdx.x, stride = (size_t)gridDim.x * blockDim.x;
   for (int sg = 0; sg < a.n_seg; sg++) {
     const F32CarrySeg &g = a.seg[sg];
-    for (size_t i = tid; i < g.slot4; i += stride)
-      for (int q = 0; q < g.n_slots; q++) g.dst[(size_t)q * g.stride4 + i] = g.src[(size_t)q * g.stride4 + i];
+    for (size_t i = tid; i < g.slot4; i += stride) {
+      int from = g.from;
+      if (a.hops) {
+        const int done = min(max(a.hops[i / g.row4] - a.h0, 0), a.n);  // hops of this chunk the row ran
+        from -= a.n - done;
+        if (from < 0 || (from == 0 && (const float4 *)g.dst == g.src)) continue;
+      }
+      const float4 *src = g.src + (size_t)from * g.stride4;
+      for (int q = 0; q < g.n_slots; q++) g.dst[(size_t)q * g.stride4 + i] = src[(size_t)q * g.stride4 + i];
+    }
   }
   for (size_t i = tid; i < (size_t)a.n_cnt; i += stride) a.cnt[i] = 0u;
 }

@@ -395,16 +395,20 @@ struct TcArgs {
   int ldc;              // row stride of out_f32
   float *out_f32;       // [M][ldc] or null
   int f32_row0;         // only rows >= f32_row0 are written to out_f32, at row - f32_row0
+  const int *hops;      // ragged calls (per-slot tiling): [M] hops of each row of a slot, or null.  Row r of hop slot t is
+                        // computed but neither checked nor stored when t >= hops[r]; out_f32 takes row r of slot
+                        // hops[r] - 1, at r
   __half *out_h;        // fp16 two-term split [2][out_plane_rows][N] (x 2^10) or null
   __nv_bfloat16 *out_b; // bf16 two-term split [2][out_plane_rows][N] or null
   int out_row0;         // first row written inside a term plane of out_h / out_b
   int out_plane_rows;   // rows per term plane of out_h / out_b
 };
 
-// First row of row tile mt, and the end of its hop slot's rows in *lim
-__device__ __forceinline__ int dense_tile_row0(const TcArgs &args, int mt, int *lim) {
+// First row of row tile mt, the end of its hop slot's rows in *lim, and the hop slot in *slot_out
+__device__ __forceinline__ int dense_tile_row0(const TcArgs &args, int mt, int *lim, int *slot_out = nullptr) {
   const int slot = mt / args.tiles_slot;
   *lim = slot * args.slot_stride + args.M;
+  if (slot_out) *slot_out = slot;
   return slot * args.slot_stride + (mt - slot * args.tiles_slot) * TM;
 }
 
@@ -457,8 +461,8 @@ __device__ __forceinline__ void dense_consumer(const TcArgs &args, const SmemCar
   Pipe p;
   Consumer<R> cons;
   for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-    int lim;  // rows from lim on (padding up to the tile's end) are computed but neither stored nor checked
-    const int n_tile = tile % args.tiles_n, m0 = dense_tile_row0(args, tile / args.tiles_n, &lim);
+    int lim, slot;  // rows from lim on (padding up to the tile's end) are computed but neither stored nor checked
+    const int n_tile = tile % args.tiles_n, m0 = dense_tile_row0(args, tile / args.tiles_n, &lim, &slot);
     float acc[R];
 #pragma unroll
     for (int i = 0; i < R; i++) acc[i] = 0.f;
@@ -482,6 +486,13 @@ __device__ __forceinline__ void dense_consumer(const TcArgs &args, const SmemCar
     for (int h = 0; h < 2; h++) {  // the thread's two rows of the fragment
       const int row = m0 + wg * 64 + warp * 16 + (lane >> 2) + 8 * h;
       if (row >= lim) continue;
+      const int r = row - slot * args.slot_stride;  // the row inside its hop slot
+      int f32_at = row - args.f32_row0;              // out_f32 row, or < 0
+      if (args.hops) {                               // a ragged call: the row's frozen hops are padding too
+        const int hr = __ldg(args.hops + r);
+        if (slot >= hr) continue;
+        f32_at = slot == hr - 1 ? r : -1;
+      }
       const size_t orow = (size_t)args.out_row0 + row;
 #pragma unroll
       for (int j = 0; j < BN / 8; j++) {
@@ -497,8 +508,8 @@ __device__ __forceinline__ void dense_consumer(const TcArgs &args, const SmemCar
           else if (act == PNB_ACT_SIGMOID) { v[q] = sigmoid_s(x, tbl); bad |= fabsf(x) >= 2.f * kTanhDomain; }
           else v[q] = x;
         }
-        if (args.out_f32 && row >= args.f32_row0) {
-          float *op = args.out_f32 + (size_t)(row - args.f32_row0) * args.ldc + col;
+        if (args.out_f32 && f32_at >= 0) {
+          float *op = args.out_f32 + (size_t)f32_at * args.ldc + col;
           op[0] = v[0];
           op[1] = v[1];
         }
@@ -567,6 +578,8 @@ struct ChainArgs {
   int tiles_mp;          // row tiles of the active streams (128 streams each)
   int units_per_hop;
   int diag;              // unit order: 0 = hop-major (layer by layer inside a hop), 1 = anti-diagonals (few streams)
+  const int *hops;       // ragged calls: [n] hops of each row, or null.  Hop t of row r with t >= hops[r] is computed
+                         // but stores nothing: its last real state stays in the fp32 buffer of parity par0 + hops[r]
   unsigned *cnt;         // [5][tiles_mp] consumer-warp completions, zero at launch
   const float *tansig;
 };
@@ -797,7 +810,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) gru_chain_kernel(const __grid_c
 #pragma unroll
       for (int h = 0; h < 2; h++) {  // the thread's two rows of the fragment
         const int row = un.mp * TM + cw * 64 + warp * 16 + (lane >> 2) + 8 * h;
-        if (row >= args.n) continue;
+        if (row >= args.n || (args.hops && un.t >= __ldg(args.hops + row))) continue;
         const float *h_old = L.h32[pold] + (size_t)row * H;
         float *h_new = L.h32[pold ^ 1] + (size_t)row * H;
         __half *ph = L.h_hl + ((size_t)(un.t + 1) * S + row) * H;
@@ -900,22 +913,26 @@ __global__ void __launch_bounds__(128) fc_split_kernel(const float *__restrict__
 // End-of-call bookkeeping in one launch: the hop slots the next call reads first (last 4 fc / 2 conv1 outputs,
 // last GRU states) move to the front of their buffers, and the chain's dependency counters return to zero.  Only the
 // active streams' rows move: they are the first rows of every slot.
-// A segment shifts `n_slots` slots down by `shift` slots.  One thread owns the same element of every slot and walks
-// the slots in ascending order, so a slot that is both source and destination (shift < n_slots) is read before it is
-// overwritten -- by the same thread, no cross-thread ordering needed.
-struct CarrySeg { uint4 *base; size_t slot16, stride16; int n_slots, shift; };  // the first slot16 of each stride16
+// A segment shifts `n_slots` slots down by `shift` slots (in a ragged call, the row's own hops: the slots of its last
+// hop).  One thread owns the same element of every slot and walks the slots in ascending order, so a slot that is both
+// source and destination (shift < n_slots) is read before it is overwritten -- by the same thread, no cross-thread
+// ordering needed.
+struct CarrySeg { uint4 *base; size_t slot16, stride16, row16; int n_slots, shift; };  // the first slot16 of each stride16; row16 per row
 struct CarryArgs {
   CarrySeg seg[16];
   int n_seg;
   unsigned *cnt;
   int n_cnt;
+  const int *hops;  // ragged calls: [active streams] hops of each row, or null
 };
 __global__ void __launch_bounds__(256) tc_carry_kernel(const __grid_constant__ CarryArgs a) {
   const size_t tid = (size_t)blockIdx.x * blockDim.x + threadIdx.x, nth = (size_t)gridDim.x * blockDim.x;
   for (int s = 0; s < a.n_seg; s++) {
     const CarrySeg sg = a.seg[s];
-    for (size_t i = tid; i < sg.slot16; i += nth)
-      for (int k = 0; k < sg.n_slots; k++) sg.base[(size_t)k * sg.stride16 + i] = sg.base[(size_t)(k + sg.shift) * sg.stride16 + i];
+    for (size_t i = tid; i < sg.slot16; i += nth) {
+      const int shift = a.hops ? a.hops[i / sg.row16] : sg.shift;
+      for (int k = 0; k < sg.n_slots; k++) sg.base[(size_t)k * sg.stride16 + i] = sg.base[(size_t)(k + shift) * sg.stride16 + i];
+    }
   }
   for (size_t i = tid; i < (size_t)a.n_cnt; i += nth) a.cnt[i] = 0u;
 }
@@ -1258,11 +1275,12 @@ static int tc_launch(pnb_engine *e, K kernel, const A &a, int units, size_t smem
   return PNB_OK;
 }
 // A dense layer over the active rows of `slots` hop slots.  With every stream active the rows are one flat range of
-// slots x S; otherwise each slot has its own ceil(n / 128) row tiles.
+// slots x S; otherwise, and whenever the epilogue needs each row's hop slot (a.hops), each slot has its own
+// ceil(n / 128) row tiles.
 template <int BN, bool BF16, int ST2, int ST3>
 static int tc_launch_dense(pnb_engine *e, TcArgs &a, int slots, int tiles_n, cudaStream_t st) {
   const int n = e->n_active;
-  if (n == e->S) {
+  if (n == e->S && !a.hops) {
     a.M = slots * n; a.slot_stride = 0; a.tiles_slot = (a.M + TM - 1) / TM; a.tiles_m = a.tiles_slot;
   } else {
     a.M = n; a.slot_stride = e->S; a.tiles_slot = (n + TM - 1) / TM; a.tiles_m = slots * a.tiles_slot;
@@ -1282,7 +1300,7 @@ static TcSeg mkseg(int a_map, int b_map, int K, int a_k0, int b_k0, int a_row0, 
 // ---- the network of a call of F hops, in phases; each returns its number of launches or a negative error ------------
 // The non-recurrent front (rnn.cpp:50-52 on F S rows): fc -> conv1 -> conv2.  Hop t of the call lives in slot t of the
 // per-call buffers.
-static int tc_front(pnb_engine *e, int F, cudaStream_t st) {
+static int tc_front(pnb_engine *e, int F, const int *hops, cudaStream_t st) {
   pnb_tc_state *t = e->tc;
   const int S = e->S, Fm = e->Fmax, na = e->n_active;
   const float *tbl = e->tansig();
@@ -1308,7 +1326,8 @@ static int tc_front(pnb_engine *e, int F, cudaStream_t st) {
     if ((rc = tc_launch_dense<DENSE_BN, true, DENSE_STAGES, DENSE_STAGES3>(e, a, F, 512 / DENSE_BN, st))) return rc;
     nl++;
   }
-  // conv2: three taps -> tanh -> fp16 terms (gru1 / gru_rb / fc_gb inputs); fp32 copy of the call's last hop
+  // conv2: three taps -> tanh -> fp16 terms (gru1 / gru_rb / fc_gb inputs); fp32 copy of the call's last hop (of each
+  // row's last hop in a ragged call, whose frozen hops neither store nor raise the domain bit)
   memset(&a, 0, sizeof a);
   a.maps[0] = t->m_c1_all;
   a.maps[1] = t->m_wconv2;
@@ -1317,6 +1336,7 @@ static int tc_front(pnb_engine *e, int F, cudaStream_t st) {
   a.bias = t->bias_pad + 512; a.act = PNB_ACT_TANH; a.N = 512;
   a.out_f32 = e->c2; a.ldc = 512; a.f32_row0 = (F - 1) * S;
   a.out_h = t->c2_h; a.out_row0 = 0; a.out_plane_rows = Fm * S; a.wide = t->wide;
+  a.hops = hops;
   {
     ProfScope ps(e, PNB_K_TC_GEMM, st);
     if ((rc = tc_launch_dense<DENSE_BN, true, DENSE_STAGES, DENSE_STAGES3>(e, a, F, 512 / DENSE_BN, st))) return rc;
@@ -1327,7 +1347,7 @@ static int tc_front(pnb_engine *e, int F, cudaStream_t st) {
 
 // The recurrent part: five GRUs per hop (rnn.cpp:58-71) in one persistent launch.  State slot t holds the state
 // BEFORE hop t of the call; the fp32 state ping-pongs by hop, starting from e->par (the call's first hop).
-static int tc_gru_chain(pnb_engine *e, int F, cudaStream_t st) {
+static int tc_gru_chain(pnb_engine *e, int F, const int *hops, cudaStream_t st) {
   pnb_tc_state *t = e->tc;
   const int S = e->S, Fm = e->Fmax;
   ChainArgs a;
@@ -1336,6 +1356,7 @@ static int tc_gru_chain(pnb_engine *e, int F, cudaStream_t st) {
   for (int i = 0; i < 5; i++) { a.maps[1 + i] = t->m_h_ch[i]; a.maps[6 + i] = t->m_w[i]; a.maps[11 + i] = t->m_u[i]; }
   // only the active streams' row tiles are units; the counters of the others stay zero
   a.S = S; a.n = e->n_active; a.F = F; a.tiles_mp = (e->n_active + TM - 1) / TM; a.cnt = t->cnt; a.tansig = e->tansig();
+  a.hops = hops;
   const int c2_terms = Fm * S, h_terms = (Fm + 1) * S;
   int unit0 = 0;
   for (int li = 0; li < 5; li++) {
@@ -1375,7 +1396,7 @@ static int tc_gru_chain(pnb_engine *e, int F, cudaStream_t st) {
 }
 
 // The two 34-wide output layers (rnn.cpp:73-80; N padded to 48, fp16 two-term split, sigmoid epilogue).
-static int tc_out(pnb_engine *e, int F, cudaStream_t st) {
+static int tc_out(pnb_engine *e, int F, const int *, cudaStream_t st) {
   pnb_tc_state *t = e->tc;
   const int S = e->S, Fm = e->Fmax;
   const float *tbl = e->tansig();
@@ -1409,27 +1430,29 @@ static int tc_out(pnb_engine *e, int F, cudaStream_t st) {
   return nl;
 }
 
-// End of a call of F hops: the last 4 fc / 2 conv1 hop slots and the last state slot move to the front, the chain's
-// dependency counters return to zero (one launch), and the fp32 state parity advances by F.
-static int tc_carry(pnb_engine *e, int F, cudaStream_t st) {
+// End of a call of F hops: the last 4 fc / 2 conv1 hop slots and the last state slot move to the front (in a ragged
+// call those of each row's own last hop), the chain's dependency counters return to zero (one launch), and the fp32
+// state parity advances by F.  A ragged call's rows that stopped early hold their fp32 state at parity par0 + hops:
+// the call's fix-up moves it (pnb_state.cu, ragged_carry_kernel).
+static int tc_carry(pnb_engine *e, int F, const int *hops, cudaStream_t st) {
   pnb_tc_state *t = e->tc;
   const int S = e->S, Fm = e->Fmax, na = e->n_active;
   const int h_terms = (Fm + 1) * S;
   CarryArgs ca;
   memset(&ca, 0, sizeof ca);
-  ca.cnt = t->cnt; ca.n_cnt = 5 * t->tiles_mp;
+  ca.cnt = t->cnt; ca.n_cnt = 5 * t->tiles_mp; ca.hops = hops;
   int ns = 0;
   for (int tm = 0; tm < kConvTerms; tm++) {
     __nv_bfloat16 *bf = t->fc_all + (size_t)tm * (Fm + 4) * S * 128;
     __nv_bfloat16 *bc = t->c1_all + (size_t)tm * (Fm + 2) * S * 512;
-    ca.seg[ns++] = CarrySeg{reinterpret_cast<uint4 *>(bf), (size_t)na * 128 * 2 / 16, (size_t)S * 128 * 2 / 16, 4, F};
-    ca.seg[ns++] = CarrySeg{reinterpret_cast<uint4 *>(bc), (size_t)na * 512 * 2 / 16, (size_t)S * 512 * 2 / 16, 2, F};
+    ca.seg[ns++] = CarrySeg{reinterpret_cast<uint4 *>(bf), (size_t)na * 128 * 2 / 16, (size_t)S * 128 * 2 / 16, 128 * 2 / 16, 4, F};
+    ca.seg[ns++] = CarrySeg{reinterpret_cast<uint4 *>(bc), (size_t)na * 512 * 2 / 16, (size_t)S * 512 * 2 / 16, 512 * 2 / 16, 2, F};
   }
   for (int li = 0; li < 5; li++) {
     const size_t H = e->gru[li].H;
     for (int tm = 0; tm < 2; tm++) {
       __half *base = t->h_all[li] + (size_t)tm * h_terms * H;
-      ca.seg[ns++] = CarrySeg{reinterpret_cast<uint4 *>(base), (size_t)na * H * 2 / 16, (size_t)S * H * 2 / 16, 1, F};
+      ca.seg[ns++] = CarrySeg{reinterpret_cast<uint4 *>(base), (size_t)na * H * 2 / 16, (size_t)S * H * 2 / 16, H * 2 / 16, 1, F};
     }
   }
   ca.n_seg = ns;
@@ -1442,10 +1465,10 @@ static int tc_carry(pnb_engine *e, int F, cudaStream_t st) {
   return 1;
 }
 
-int tc_network(pnb_engine *e, int F, cudaStream_t st) {
+int tc_network(pnb_engine *e, int F, const int *hops, cudaStream_t st) {
   int n = 0;
-  for (int (*phase)(pnb_engine *, int, cudaStream_t) : {tc_front, tc_gru_chain, tc_out, tc_carry}) {
-    const int q = phase(e, F, st);
+  for (int (*phase)(pnb_engine *, int, const int *, cudaStream_t) : {tc_front, tc_gru_chain, tc_out, tc_carry}) {
+    const int q = phase(e, F, hops, st);
     if (q < 0) return q;
     n += q;
   }

@@ -11,6 +11,7 @@
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 #include <stdint.h>
+#include <string.h>
 
 #include "pnb_engine.h"
 #include "pnb_state.h"
@@ -230,16 +231,80 @@ __global__ void __launch_bounds__(256) session_blob_kernel(const __grid_constant
   }
 }
 
-// g/r of a session call in list order: dst[t][row[p]][:] = src[t][p][:] for the k computed slots
+// g/r of a session call in list order: dst[t][row[p]][:] = src[t][p][:] for the k computed slots (zeros for the hops
+// a ragged call's slot did not run)
 __global__ void gr_gather_kernel(const float *__restrict__ src, float *__restrict__ dst, const int *__restrict__ row, int k,
-                                 int S, int F) {
+                                 int S, int F, const int *__restrict__ hops) {
   const long long total = (long long)F * k * 68;
   for (long long x = (long long)blockIdx.x * blockDim.x + threadIdx.x; x < total; x += (long long)gridDim.x * blockDim.x) {
     const int c = (int)(x % 68);
     const long long tp = x / 68;
     const int p = (int)(tp % k), t = (int)(tp / k);
-    dst[((size_t)t * k + row[p]) * 68 + c] = src[((size_t)t * S + p) * 68 + c];
+    dst[((size_t)t * k + row[p]) * 68 + c] = (hops && t >= hops[p]) ? 0.f : src[((size_t)t * S + p) * 68 + c];
   }
+}
+
+// The pieces of a slot's state that move with the engine's counters (see state_segs): the history window at line_off,
+// the five live spectrum ring slots at hop, and (tensor path) the fp32 GRU states at parity par.
+struct RaggedArgs {
+  float *pcm;
+  size_t pcm_stride, line_off;  // the call's window: line_off + h * 480 after h hops
+  float2 *zring;                // [ring][S][400]
+  float *ering;                 // [ring][S][34]
+  int ring, S, F;
+  long hop0;                    // hop counter at the call's start
+  int n_gru;                    // 5 on tensor engines (ping-pong fp32 states), 0 on fp32 engines (states carried by slot)
+  float *h[5][2];
+  int H[5], par[5];             // parity after the call
+  const int *hops, *slots;      // [S] hops per slot; [gridDim.x] the slots that stopped early
+};
+
+// One block per slot that stopped after h < F hops.  Each piece is read completely before it is written, so the
+// overlapping source and destination ranges (F - h < 11 hops of history, F - h < 5 ring slots) need no second buffer:
+// the history window goes through registers between two block barriers, and each thread owns one word of every ring
+// slot and walks the five slots from the newest down, reading a slot before it writes the one it shadows.
+constexpr int kRaggedThreads = 256;
+__global__ void __launch_bounds__(kRaggedThreads) ragged_carry_kernel(const __grid_constant__ RaggedArgs a) {
+  const int p = a.slots[blockIdx.x], h = a.hops[p], d = a.F - h;
+  const unsigned tid = threadIdx.x;
+  {
+    float *line = a.pcm + (size_t)p * a.pcm_stride + a.line_off;
+    constexpr int kPer = (kKeep + kRaggedThreads - 1) / kRaggedThreads;
+    float keep[kPer];
+#pragma unroll
+    for (int i = 0; i < kPer; i++) {
+      const int j = tid + kRaggedThreads * i;
+      keep[i] = j < kKeep ? line[(size_t)h * kFrame + j] : 0.f;
+    }
+    __syncthreads();
+#pragma unroll
+    for (int i = 0; i < kPer; i++) {
+      const int j = tid + kRaggedThreads * i;
+      if (j < kKeep) line[(size_t)a.F * kFrame + j] = keep[i];
+    }
+  }
+  {
+    const int R = a.ring;
+    const long base = a.hop0 + h - 5;  // live slot k after h hops: base + k; after F hops: base + d + k
+    constexpr unsigned kZ = 2 * kBins;
+    for (unsigned w = tid; w < kZ + kBands; w += kRaggedThreads)
+      for (int k = 4; k >= 0; k--) {
+        const size_t src = (size_t)(((base + k) % R + R) % R), dst = (size_t)(((base + d + k) % R + R) % R);
+        if (w < kZ) {
+          float *z = reinterpret_cast<float *>(a.zring);
+          z[(dst * a.S + p) * kZ + w] = z[(src * a.S + p) * kZ + w];
+        } else {
+          a.ering[(dst * a.S + p) * kBands + (w - kZ)] = a.ering[(src * a.S + p) * kBands + (w - kZ)];
+        }
+      }
+  }
+  if (d & 1)
+    for (int li = 0; li < a.n_gru; li++) {
+      const size_t H = a.H[li];
+      const float *src = a.h[li][a.par[li] ^ 1] + (size_t)p * H;
+      float *dst = a.h[li][a.par[li]] + (size_t)p * H;
+      for (unsigned k = tid; k < H; k += kRaggedThreads) dst[k] = src[k];
+    }
 }
 
 __global__ void state_clear_reject_kernel(int *status) {
@@ -318,10 +383,27 @@ int launch_session_blob(const StateArgs &a, cudaStream_t st) {
   session_blob_kernel<<<a.n, 256, 0, st>>>(a);
   return 1;
 }
-int launch_gr_gather(const float *src, float *dst, const int *row, int k, int S, int F, cudaStream_t st) {
+int launch_gr_gather(const float *src, float *dst, const int *row, int k, int S, int F, cudaStream_t st, const int *hops) {
   const long long total = (long long)F * k * 68;
   const long long blocks = (total + 255) / 256;
-  gr_gather_kernel<<<(unsigned)(blocks < 4096 ? blocks : 4096), 256, 0, st>>>(src, dst, row, k, S, F);
+  gr_gather_kernel<<<(unsigned)(blocks < 4096 ? blocks : 4096), 256, 0, st>>>(src, dst, row, k, S, F, hops);
+  return 1;
+}
+
+// Beside state_segs: the same places, at the counters of the call's start (history, ring) and end (GRU parity).
+int launch_ragged_carry(const pnb_engine *e, int F, const int *d_hops, const int *d_slots, int n, cudaStream_t st) {
+  RaggedArgs a;
+  memset(&a, 0, sizeof a);
+  a.pcm = e->d_pcm; a.pcm_stride = e->pcm_stride; a.line_off = e->line_off;
+  a.zring = e->d_zring; a.ering = e->d_ering; a.ring = e->ring; a.S = e->S; a.F = F; a.hop0 = e->hop;
+  if (e->flags & PNB_NN_TENSOR) {
+    a.n_gru = 5;
+    for (int li = 0; li < 5; li++) {
+      a.h[li][0] = e->h[li][0]; a.h[li][1] = e->h[li][1]; a.H[li] = e->gru[li].H; a.par[li] = e->par[li];
+    }
+  }
+  a.hops = d_hops; a.slots = d_slots;
+  ragged_carry_kernel<<<n, kRaggedThreads, 0, st>>>(a);
   return 1;
 }
 int launch_state_clear_reject(int *status, cudaStream_t st) {

@@ -98,7 +98,14 @@ int launch_state_clear_reject(int *status, cudaStream_t st);
 // call in list order ([F][k][68] from the engine's [F][S][68])
 int launch_session_move(const StateArgs &a, cudaStream_t st);
 int launch_session_blob(const StateArgs &a, cudaStream_t st);
-int launch_gr_gather(const float *src, float *dst, const int *row, int k, int S, int F, cudaStream_t st);
+// hops: [k] hops of each slot in a ragged call (entries t >= hops[p] are written as zeros), or null
+int launch_gr_gather(const float *src, float *dst, const int *row, int k, int S, int F, cudaStream_t st,
+                     const int *hops = nullptr);
+// The fix-up of a ragged session call (pnb_process_sessions_ragged_*), enqueued after synthesis and before the history
+// slide, with the engine's hop counter and line offset still those of the call's start and its GRU parity already that
+// of its end.  The n slots at d_slots stopped after hops[p] < F hops; the pieces of their state that sit where the
+// counters say (state_segs) move from where hop hops[p] left them to where hop F would have put them.  One launch.
+int launch_ragged_carry(const pnb_engine *e, int F, const int *d_hops, const int *d_slots, int n, cudaStream_t st);
 // Parking blobs are engine-owned: padded to 16 bytes
 constexpr size_t kParkStride = (sizeof(StreamState) + 15) / 16 * 16;
 

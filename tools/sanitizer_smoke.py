@@ -6,8 +6,8 @@
 Exercises the fp32 path, the tensor path (one CTA pair's worth of streams), the post-filter, the int16 entry,
 the pipelined host entry, the training-data generator, the persistent fp32 GRU chain (both block sizes), submitted
 calls on the chain's anti-diagonal unit order, state export / import, a session-pool schedule (parks, unparks,
-relocations, fresh starts, session export / import / reset) and the pitch-only kernel on tiny batches; prints a checksum
-per leg."""
+relocations, fresh starts, session export / import / reset), ragged session calls (sessions that stop early, across the
+history slide and the fp32 network's 32-hop chunk) and the pitch-only kernel on tiny batches; prints a checksum per leg."""
 import os
 import sys
 
@@ -20,7 +20,7 @@ from percepnet_b200.weights import synth_model  # noqa: E402
 
 
 def main():
-    legs = sys.argv[1:] or ["fp32", "tensor", "train", "fp32chain", "submit", "sessions", "pitch"]
+    legs = sys.argv[1:] or ["fp32", "tensor", "train", "fp32chain", "submit", "sessions", "ragged", "pitch"]
     m = synth_model(0)
     if "fp32" in legs:
         x = synth_pcm(5, 4, seed=3)
@@ -75,6 +75,23 @@ def main():
                 sums.append(float(np.abs(o).sum()) + float(gr.sum()))
             e.wait()
             print("sessions", flags, sums, e.session_stats())
+            e.close()
+    if "ragged" in legs:     # ragged session calls on both network modes; max_frames 33 crosses the fp32 32-hop chunk
+        for flags in (api.NN_FP32, api.NN_TENSOR):
+            S, N, F = 130, 300, 33
+            e = api.Engine(S, F, m, flags)
+            e.reserve_sessions(N)
+            rng = np.random.RandomState(15)
+            x = synth_pcm(S, F, seed=16)
+            sums = []
+            for c, k in enumerate((129, 130, 1, 128, 130, 64)):
+                ids = rng.choice(N, size=k, replace=False).astype(np.int32)
+                hops = rng.randint(1, F + 1, size=k).astype(np.int32)
+                w = int(hops.max())
+                o, gr = e.process_sessions(ids, np.ascontiguousarray(x[:k, :w * 480]), want_gr=True, hops=hops)
+                sums.append(float(np.abs(o).sum()) + float(gr.sum()))
+            e.wait()
+            print("ragged", flags, sums)
             e.close()
     if "pitch" in legs:
         buf = synth_pcm(40, 4, seed=12)[:, :1728].copy()

@@ -81,6 +81,10 @@ int pnb_create(pnb_engine **out, int n_streams, int max_frames_per_call, const p
                unsigned flags, int device);   /* device: CUDA ordinal, or -1 = the calling thread's current device */
 void pnb_destroy(pnb_engine *e);
 int pnb_reset(pnb_engine *e);
+/* The CUDA ordinal pnb_create(..., device) would use (device -1 = the calling thread's current device), or the negative
+ * error code pnb_create would return for it (PNB_ERR_NO_DEVICE, PNB_ERR_CUDA, PNB_ERR_ARG).  Creates nothing; lets a
+ * host key per-device resources without linking the CUDA runtime itself. */
+int pnb_resolve_device(int device);
 
 /* Binary weight file (percepnet_b200.weights.PackedModel.save_blob): the arrays of the generated nnet_data.cpp
  * as raw float32, 32 MB instead of 180 MB of C source and no 46 s compile.  The returned model owns its arrays;

@@ -51,6 +51,7 @@ def load_library() -> C.CDLL:
     L.pnb_destroy.argtypes = [vp]
     L.pnb_destroy.restype = None
     L.pnb_reset.argtypes = [vp]
+    L.pnb_resolve_device.argtypes = [i]
     L.pnb_process_host_f32.argtypes = [vp, vp, sz, vp, sz, i, vp]
     L.pnb_process_host_i16.argtypes = [vp, vp, sz, vp, sz, i, vp]
     L.pnb_process_device_f32.argtypes = [vp, vp, sz, vp, sz, i, vp, vp]
@@ -102,7 +103,7 @@ def load_library() -> C.CDLL:
     return L
 
 
-EXPORTS = ("pnb_create", "pnb_destroy", "pnb_reset", "pnb_process_host_f32", "pnb_process_host_i16",
+EXPORTS = ("pnb_create", "pnb_destroy", "pnb_reset", "pnb_resolve_device", "pnb_process_host_f32", "pnb_process_host_i16",
            "pnb_model_load_blob", "pnb_model_load_stream", "pnb_model_free", "pnb_train_records_host", "pnb_train_records_device", "pnb_submit_train_records", "pnb_process_device_f32", "pnb_process_device_i16", "pnb_submit_host_f32", "pnb_submit_host_i16", "pnb_submit_device_f32", "pnb_submit_device_i16", "pnb_flush", "pnb_wait", "pnb_check",
            "pnb_read_tap", "pnb_state_size", "pnb_get_state", "pnb_set_state",
            "pnb_reset_streams", "pnb_export_states", "pnb_import_states", "pnb_set_active_streams", "pnb_active_streams",

@@ -68,9 +68,10 @@ def build(force: bool = False, verbose: bool = False) -> str:
             sys.stderr.write(log[-1])
             raise RuntimeError("link failed")
     shim_src = os.path.join(CSRC, "rnnoise_shim.cpp")
-    if force or _newer([shim_src, LIB], SHIM):
+    if force or _newer([shim_src, os.path.join(CSRC, "pnb_shim_batcher.h"), LIB, __file__], SHIM):
         cxx = "/usr/bin/g++" if os.path.exists("/usr/bin/g++") else "g++"
-        cmd = [cxx, "-O2", "-std=c++11", "-fPIC", "-shared", "-o", SHIM, shim_src, "-L" + HERE,
+        # -pthread: pooled handles (PNB_SHIM_POOL) batch frames of concurrent threads under std::mutex
+        cmd = [cxx, "-O2", "-std=c++11", "-pthread", "-fPIC", "-shared", "-o", SHIM, shim_src, "-L" + HERE,
                "-lpercepnet_b200", "-Wl,-rpath,$ORIGIN"]
         r = subprocess.run(cmd, capture_output=True, text=True)
         log.append(f"$ {' '.join(cmd)}\n{r.stdout}{r.stderr}")

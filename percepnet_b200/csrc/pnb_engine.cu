@@ -135,6 +135,20 @@ static int check_model(const pnb_model *m) {
   return PNB_OK;
 }
 
+extern "C" int pnb_resolve_device(int device) {
+  int ndev = 0;
+  cudaError_t ce = cudaGetDeviceCount(&ndev);
+  if (ce != cudaSuccess || ndev == 0)
+    return fail(PNB_ERR_NO_DEVICE, "no CUDA device available (%s); this library has no CPU path",
+                ce == cudaSuccess ? "device count 0" : cudaGetErrorString(ce));
+  if (device == -1) {  // the calling thread's current device
+    ce = cudaGetDevice(&device);
+    if (ce != cudaSuccess) return fail(PNB_ERR_CUDA, "cudaGetDevice failed: %s", cudaGetErrorString(ce));
+  }
+  if (device < 0 || device >= ndev) return fail(PNB_ERR_ARG, "device %d out of range (have %d)", device, ndev);
+  return device;
+}
+
 extern "C" int pnb_create(pnb_engine **out, int n_streams, int max_frames, const pnb_model *model, unsigned flags,
                           int device) {
   if (!out) return fail(PNB_ERR_ARG, "out is NULL");
@@ -149,16 +163,8 @@ extern "C" int pnb_create(pnb_engine **out, int n_streams, int max_frames, const
     return fail(PNB_ERR_ARG, "PNB_TRAIN_DATA runs no network: combine it only with PNB_KEEP_TAPS");
   int rc = train_mode ? 0 : check_model(model);
   if (rc) return rc;
-  int ndev = 0;
-  cudaError_t ce = cudaGetDeviceCount(&ndev);
-  if (ce != cudaSuccess || ndev == 0)
-    return fail(PNB_ERR_NO_DEVICE, "no CUDA device available (%s); this library has no CPU path",
-                ce == cudaSuccess ? "device count 0" : cudaGetErrorString(ce));
-  if (device == -1) {  // the calling thread's current device
-    ce = cudaGetDevice(&device);
-    if (ce != cudaSuccess) return fail(PNB_ERR_CUDA, "cudaGetDevice failed: %s", cudaGetErrorString(ce));
-  }
-  if (device < 0 || device >= ndev) return fail(PNB_ERR_ARG, "device %d out of range (have %d)", device, ndev);
+  device = pnb_resolve_device(device);
+  if (device < 0) return device;
   CK(cudaSetDevice(device));
   cudaDeviceProp prop;
   CK(cudaGetDeviceProperties(&prop, device));

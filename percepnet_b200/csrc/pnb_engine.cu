@@ -37,7 +37,7 @@ static int fail(int code, const char *fmt, ...) {
     if (_e != cudaSuccess) return fail(PNB_ERR_CUDA, "%s failed: %s (%s:%d)", #call, cudaGetErrorString(_e), __FILE__, __LINE__); \
   } while (0)
 
-int tc_fail(int code, const char *msg) { return fail(code, "%s", msg); }
+int engine_fail(int code, const char *msg) { return fail(code, "%s", msg); }
 
 extern "C" const char *pnb_last_error(void) { return g_err.c_str(); }
 extern "C" const char *pnb_version(void) { return "percepnet_b200 0.1 (sm_90a)"; }
@@ -99,17 +99,11 @@ static void build_tables(Tables &t) {
 }
 
 // ------------------------------------------------------------------------------------------
-template <typename T>
-static cudaError_t dalloc(T **p, size_t n, bool zero = true) {
-  cudaError_t e = cudaMalloc((void **)p, n * sizeof(T));
-  if (e != cudaSuccess) return e;
-  if (zero) return cudaMemset(*p, 0, n * sizeof(T));
-  return cudaSuccess;
-}
-static cudaError_t upload(float **dst, const float *src, size_t n) {
-  cudaError_t e = cudaMalloc((void **)dst, n * sizeof(float));
-  if (e != cudaSuccess) return e;
-  return cudaMemcpy(*dst, src, n * sizeof(float), cudaMemcpyHostToDevice);
+cudaError_t engine_buffer(pnb_engine *e, void **p, size_t bytes, bool zero_on_reset, const void *src) {
+  cudaError_t r = cudaMalloc(p, bytes);
+  if (r != cudaSuccess) return r;
+  e->buffers.push_back({*p, bytes, zero_on_reset});
+  return src ? cudaMemcpy(*p, src, bytes, cudaMemcpyHostToDevice) : cudaMemset(*p, 0, bytes);
 }
 
 static int check_model(const pnb_model *m) {
@@ -195,37 +189,13 @@ extern "C" int pnb_create(pnb_engine **out, int n_streams, int max_frames, const
   {
     Tables *t = new Tables();
     build_tables(*t);
-    cudaError_t r = cudaMalloc((void **)&e->d_tab, sizeof(Tables));
-    if (r == cudaSuccess) r = cudaMemcpy(e->d_tab, t, sizeof(Tables), cudaMemcpyHostToDevice);
+    cudaError_t r = engine_upload(e, &e->d_tab, t, 1);
     delete t;
     CKD(r);
   }
-  // weights, in the reference's layout (SURVEY.md App. B)
-  if (!train_mode) {
-  CKD(upload(&e->fc.W, model->fc->input_weights, 70 * 128));
-  CKD(upload(&e->fc.b, model->fc->bias, 128));
-  CKD(upload(&e->conv1.W, model->conv1->input_weights, 5 * 128 * 512));
-  CKD(upload(&e->conv1.b, model->conv1->bias, 512));
-  CKD(upload(&e->conv2.W, model->conv2->input_weights, 3 * 512 * 512));
-  CKD(upload(&e->conv2.b, model->conv2->bias, 512));
-  const pnb_gru_layer *g5[5] = {model->gru1, model->gru2, model->gru3, model->gru_gb, model->gru_rb};
-  for (int i = 0; i < 5; i++) {
-    int M = g5[i]->nb_inputs, H = g5[i]->nb_neurons;
-    e->gru[i].M = M;
-    e->gru[i].H = H;
-    CKD(upload(&e->gru[i].W, g5[i]->input_weights, (size_t)M * 3 * H));
-    CKD(upload(&e->gru[i].U, g5[i]->recurrent_weights, (size_t)H * 3 * H));
-    CKD(upload(&e->gru[i].b, g5[i]->bias, 6 * (size_t)H));
-  }
-  CKD(upload(&e->fc_gb.W, model->fc_gb->input_weights, 2560 * 34));
-  CKD(upload(&e->fc_gb.b, model->fc_gb->bias, 34));
-  CKD(upload(&e->fc_rb.W, model->fc_rb->input_weights, 128 * 34));
-  CKD(upload(&e->fc_rb.b, model->fc_rb->bias, 34));
-  e->act_fc = model->fc->activation;
-  e->act_conv1 = model->conv1->activation;
-  e->act_conv2 = model->conv2->activation;
-  e->act_gb = model->fc_gb->activation;
-  e->act_rb = model->fc_rb->activation;
+  if (!train_mode) {  // both paths run fc from the reference's layout (SURVEY.md App. B)
+    CKD(engine_upload(e, &e->fc.W, model->fc->input_weights, 70 * 128));
+    CKD(engine_upload(e, &e->fc.b, model->fc->bias, 128));
   }
 
   // stream state
@@ -233,68 +203,46 @@ extern "C" int pnb_create(pnb_engine **out, int n_streams, int max_frames, const
   // when one call already carries many hops (the move is then amortised over those hops anyway)
   const size_t line_calls = F >= 128 ? 1 : (128 / F > (size_t)kLineCalls ? (size_t)kLineCalls : 128 / F);
   e->pcm_stride = kKeep + line_calls * F * kFrame;
-  CKD(dalloc(&e->d_pcm, S * e->pcm_stride));
-  CKD(dalloc(&e->d_synth, S * kFrame));
-  CKD(dalloc(&e->d_status, 2));
+  CKD(engine_alloc(e, &e->d_pcm, S * e->pcm_stride, kStreamState));
+  CKD(engine_alloc(e, &e->d_synth, S * kFrame, kStreamState));
+  CKD(engine_alloc(e, &e->d_status, 2, kScratch));  // pnb_reset sets it itself
   CKD(cudaMemset(e->d_status + 1, 0x7F, sizeof(int)));  // kNoRejectedSlot
   CKD(cudaHostAlloc((void **)&e->h_status, 2 * sizeof(int), cudaHostAllocDefault));
   e->h_status[0] = 0;
   e->h_status[1] = kNoRejectedSlot;
-  // batched stream-state operations: staging of the slot indices, import verdicts, one blob of scratch
+  // batched stream-state operations: staging of the slot indices, import verdicts (both grown by the session pool),
+  // one blob of scratch
   CKD(cudaEventCreateWithFlags(&e->ev_call, cudaEventDisableTiming));
   for (int k = 0; k < 2; k++) {
     CKD(cudaEventCreateWithFlags(&e->ev_idx[k], cudaEventDisableTiming));
     CKD(cudaHostAlloc((void **)&e->h_idx[k], S * sizeof(int), cudaHostAllocDefault));
-    CKD(dalloc(&e->d_idx[k], S, false));
+    CKD(cudaMalloc((void **)&e->d_idx[k], S * sizeof(int)));
   }
   e->idx_cap = S;
-  CKD(dalloc(&e->d_ok, S, false));
+  CKD(cudaMalloc((void **)&e->d_ok, S * sizeof(int)));
   e->ok_cap = S;
-  CKD(cudaMalloc(&e->d_blob1, sizeof(StreamState)));
-  CKD(dalloc(&e->d_last_period, S));
-  CKD(dalloc(&e->d_last_gain, S));
+  CKD(engine_buffer(e, &e->d_blob1, sizeof(StreamState), kScratch, nullptr));
+  CKD(engine_alloc(e, &e->d_last_period, S, kStreamState));
+  CKD(engine_alloc(e, &e->d_last_gain, S, kStreamState));
   // per-call buffers
-  CKD(dalloc(&e->d_feat, F * S * kFeat));
+  CKD(engine_alloc(e, &e->d_feat, F * S * kFeat, kScratch));
   e->ring = (int)F + 5;
-  CKD(dalloc(&e->d_zring, (size_t)e->ring * S * kBins));
-  CKD(dalloc(&e->d_ering, (size_t)e->ring * S * kBands));
-  if (!train_mode) CKD(dalloc(&e->d_P, F * S * kBins));
-  CKD(dalloc(&e->d_Ex, F * S * kBands));
-  CKD(dalloc(&e->d_sil, F * S));
-  if (!train_mode) CKD(dalloc(&e->d_gr, F * S * 68));
-  if (train_mode) CKD(dalloc(&e->d_raw, F * S * 68));
+  CKD(engine_alloc(e, &e->d_zring, (size_t)e->ring * S * kBins, kStreamState));
+  CKD(engine_alloc(e, &e->d_ering, (size_t)e->ring * S * kBands, kStreamState));
+  if (!train_mode) CKD(engine_alloc(e, &e->d_P, F * S * kBins, kScratch));
+  CKD(engine_alloc(e, &e->d_Ex, F * S * kBands, kScratch));
+  CKD(engine_alloc(e, &e->d_sil, F * S, kScratch));
+  if (!train_mode) CKD(engine_alloc(e, &e->d_gr, F * S * 68, kScratch));
+  if (train_mode) CKD(engine_alloc(e, &e->d_raw, F * S * 68, kScratch));
   if (flags & PNB_KEEP_TAPS) {
-    CKD(dalloc(&e->d_tap_pitch, F * S * 4));
-    CKD(dalloc(&e->d_tap_pitchf, F * S * 2));
-    if (!train_mode) CKD(dalloc(&e->d_tap_g, F * S * kBands));
+    CKD(engine_alloc(e, &e->d_tap_pitch, F * S * 4, kScratch));
+    CKD(engine_alloc(e, &e->d_tap_pitchf, F * S * 2, kScratch));
+    if (!train_mode) CKD(engine_alloc(e, &e->d_tap_g, F * S * kBands, kScratch));
   }
-  if (train_mode) {
-    CKD(cudaDeviceSynchronize());
-    *out = e;
-    return PNB_OK;
-  }
-  // network state; the conv rings and gate sums are scratch of the fp32 path only
-  CKD(dalloc(&e->c2, S * 512));
-  if (flags & PNB_NN_TENSOR) {
-    for (int i = 0; i < 5; i++)
-      for (int p = 0; p < 2; p++) CKD(dalloc(&e->h[i][p], S * e->gru[i].H));
-  } else {
-    // fp32 path: hop-slot buffers of one chunk of at most f32_chunk = min(max_frames, 32) hops.  Slot 0.. of the fc / conv1 buffers hold
-    // the conv histories (oldest first), slot 0 of every state buffer the state before the chunk's first hop; the
-    // chunk's carry moves the last slots back there, so between calls the state lives at the front (par stays 0).
-    e->f32_chunk = max_frames < kF32ChainMaxHops ? max_frames : kF32ChainMaxHops;
-    const size_t C = e->f32_chunk;
-    e->f32_rt = S <= 64 ? 1 : 8;
-    e->f32_rb = (int)((S + 16 * e->f32_rt - 1) / (16 * e->f32_rt));
-    CKD(dalloc(&e->ring_fc, (C + 4) * S * 128));
-    CKD(dalloc(&e->ring_c1, (C + 2) * S * 512));
-    CKD(dalloc(&e->c2_all, C * S * 512));
-    for (int i = 0; i < 5; i++) CKD(dalloc(&e->h[i][0], (C + 1) * S * e->gru[i].H));
-    CKD(dalloc(&e->f32_cnt, (size_t)5 * e->f32_rb));
-  }
-  if (flags & PNB_NN_TENSOR) {
-    int trc = tc_prepare(e, model);
-    if (trc) { pnb_destroy(e); return trc; }
+  if (!train_mode) {
+    CKD(engine_alloc(e, &e->c2, S * 512, kStreamState));
+    const int rc = (flags & PNB_NN_TENSOR) ? tc_prepare(e, model) : f32_prepare(e, model);
+    if (rc) { pnb_destroy(e); return rc; }
   }
   CKD(cudaDeviceSynchronize());
   *out = e;
@@ -305,24 +253,7 @@ extern "C" void pnb_destroy(pnb_engine *e) {
   if (!e) return;
   cudaSetDevice(e->device);
   cudaDeviceSynchronize();
-  tc_release(e);
-  float *fl[] = {e->fc.W, e->fc.b, e->conv1.W, e->conv1.b, e->conv2.W, e->conv2.b, e->fc_gb.W, e->fc_gb.b,
-                 e->fc_rb.W, e->fc_rb.b, e->d_pcm, e->d_synth, e->d_last_gain, e->d_feat, e->d_Ex, e->d_gr,
-                 e->d_tap_pitchf, e->d_tap_g, e->ring_fc, e->ring_c1, e->c2, e->c2_all, e->d_raw};
-  for (float *p : fl) if (p) cudaFree(p);
-  for (int i = 0; i < 5; i++) {
-    if (e->gru[i].W) cudaFree(e->gru[i].W);
-    if (e->gru[i].U) cudaFree(e->gru[i].U);
-    if (e->gru[i].b) cudaFree(e->gru[i].b);
-    for (int p = 0; p < 2; p++) if (e->h[i][p]) cudaFree(e->h[i][p]);
-  }
-  if (e->f32_cnt) cudaFree(e->f32_cnt);
-  if (e->d_zring) cudaFree(e->d_zring);
-  if (e->d_ering) cudaFree(e->d_ering);
-  if (e->d_P) cudaFree(e->d_P);
-  if (e->d_sil) cudaFree(e->d_sil);
-  if (e->d_last_period) cudaFree(e->d_last_period);
-  if (e->d_status) cudaFree(e->d_status);
+  for (const auto &b : e->buffers) cudaFree(b.p);
   if (e->h_status) cudaFreeHost(e->h_status);
   for (int k = 0; k < 2; k++) {
     if (e->h_idx[k]) cudaFreeHost(e->h_idx[k]);
@@ -330,12 +261,9 @@ extern "C" void pnb_destroy(pnb_engine *e) {
     if (e->ev_idx[k]) cudaEventDestroy(e->ev_idx[k]);
   }
   if (e->d_ok) cudaFree(e->d_ok);
-  if (e->d_blob1) cudaFree(e->d_blob1);
   if (e->d_park) cudaFree(e->d_park);
   if (e->d_sgr) cudaFree(e->d_sgr);
   if (e->ev_call) cudaEventDestroy(e->ev_call);
-  if (e->d_tap_pitch) cudaFree(e->d_tap_pitch);
-  if (e->d_tab) cudaFree(e->d_tab);
   for (int k = 0; k < 2; k++) {
     if (e->stage[k].in) cudaFree(e->stage[k].in);
     if (e->stage[k].out) cudaFree(e->stage[k].out);
@@ -356,14 +284,9 @@ extern "C" int pnb_reset(pnb_engine *e) {
   CK(cudaSetDevice(e->device));
   cudaDeviceSynchronize();  // a poisoned engine may carry a sticky launch error of its own; the memsets below report a dead context
   cudaGetLastError();
-  const size_t S = e->S;
-  CK(cudaMemset(e->d_pcm, 0, S * e->pcm_stride * sizeof(float)));
+  for (const auto &b : e->buffers)
+    if (b.zero_on_reset) CK(cudaMemset(b.p, 0, b.bytes));
   e->line_off = 0;
-  CK(cudaMemset(e->d_synth, 0, S * kFrame * sizeof(float)));
-  CK(cudaMemset(e->d_zring, 0, (size_t)e->ring * S * kBins * sizeof(float2)));
-  CK(cudaMemset(e->d_ering, 0, (size_t)e->ring * S * kBands * sizeof(float)));
-  CK(cudaMemset(e->d_last_period, 0, S * sizeof(int)));
-  CK(cudaMemset(e->d_last_gain, 0, S * sizeof(float)));
   CK(cudaMemset(e->d_status, 0, sizeof(int)));
   CK(cudaMemset(e->d_status + 1, 0x7F, sizeof(int)));  // kNoRejectedSlot
   e->h_status[0] = 0;
@@ -375,20 +298,7 @@ extern "C" int pnb_reset(pnb_engine *e) {
     CK(cudaMemset(e->d_park, 0, (size_t)e->pool.capacity() * kParkStride));
     e->pool.init(e->S, e->pool.capacity());
   }
-  if (e->flags & PNB_TRAIN_DATA) {
-    CK(cudaDeviceSynchronize());
-    return PNB_OK;
-  }
-  if (e->ring_fc) CK(cudaMemset(e->ring_fc, 0, (size_t)(e->f32_chunk + 4) * S * 128 * sizeof(float)));
-  if (e->ring_c1) CK(cudaMemset(e->ring_c1, 0, (size_t)(e->f32_chunk + 2) * S * 512 * sizeof(float)));
-  if (e->f32_cnt) CK(cudaMemset(e->f32_cnt, 0, (size_t)5 * e->f32_rb * sizeof(unsigned)));
-  CK(cudaMemset(e->c2, 0, S * 512 * sizeof(float)));
-  for (int i = 0; i < 5; i++)
-    for (int p = 0; p < 2; p++)
-      if (e->h[i][p]) CK(cudaMemset(e->h[i][p], 0, (size_t)((e->flags & PNB_NN_TENSOR) ? 1 : e->f32_chunk + 1) * S * e->gru[i].H * sizeof(float)));
   for (int i = 0; i < 5; i++) e->par[i] = 0;
-  int trc = tc_reset(e);
-  if (trc) return trc;
   CK(cudaDeviceSynchronize());
   return PNB_OK;
 }
@@ -462,106 +372,6 @@ extern "C" const char *pnb_kernel_class_name(int cls) {
   static const char *names[PNB_NUM_KERNEL_CLASSES] = {"stage_in_kernel", "analysis_kernel", "fc_f32_kernel",
       "gemm_f32_kernel", "f32_carry_kernel", "synthesis_kernel", "slide_history_kernel", "tc_gemm_kernel", "tc_aux_kernel", "train_labels_kernel"};
   return (cls >= 0 && cls < PNB_NUM_KERNEL_CLASSES) ? names[cls] : "?";
-}
-
-// ------------------------------------------------------------------------------------------
-// one network step in fp32 (rnn.cpp:42-81), hop index `c` counted since reset
-// ------------------------------------------------------------------------------------------
-static GemmSeg seg(const float *A, int lda, const float *B, int ldb, int K) {
-  GemmSeg s;
-  s.A = A; s.lda = lda; s.B = B; s.ldb = ldb; s.K = K;
-  return s;
-}
-
-// The network of hops [h0, h0 + n) of a call (n <= e->f32_chunk) in fp32 FMA (rnn.cpp:42-81): the non-recurrent layers
-// once over the active rows of all n hop slots, the five GRUs of all n hops in one persistent launch, the output layers
-// over the same rows, and the carry that moves the conv histories and the states back to the front of their slot buffers.
-// hops: the per-slot hops of a ragged call (device), or null.
-static int nn_chunk_f32(pnb_engine *e, int h0, int n, const int *hops, cudaStream_t st) {
-  const int S = e->S, na = e->n_active;
-  // all streams active: the rows of the n slots are one flat range; otherwise the first na rows of each slot
-  const int rows = na == S ? n * S : na, slots = na == S ? 1 : n;
-  const float *tbl = e->tansig();
-  int nl = 0;
-  // fc -> slots 4.. (slots 0..3 hold the last four hops' outputs)
-  { ProfScope ps(e, PNB_K_FC, st); nl += launch_fc_f32(e->d_feat + (size_t)h0 * S * kFeat, e->fc.W, e->fc.b, e->ring_fc + (size_t)4 * S * 128, rows, 70, 128, slots, S, st); }
-  GemmArgs g;
-  memset(&g, 0, sizeof g);
-  g.M = rows; g.n_slots = slots; g.slot_stride = S; g.tansig = tbl;
-  // conv1: tap q of hop t reads fc slot t + q (oldest first, nnet.cpp:182-200; weights [tap][c][n]) -> c1 slots 2..
-  for (int q = 0; q < 5; q++) g.seg[q] = seg(e->ring_fc + (size_t)q * S * 128, 128, e->conv1.W + (size_t)q * 128 * 512, 512, 128);
-  g.n_seg = 5; g.N = 512; g.C = e->ring_c1 + (size_t)2 * S * 512; g.ldc = 512; g.bias = e->conv1.b; g.act = e->act_conv1;
-  { ProfScope ps(e, PNB_K_GEMM_F32, st); nl += launch_gemm_f32(g, st); }
-  for (int q = 0; q < 3; q++) g.seg[q] = seg(e->ring_c1 + (size_t)q * S * 512, 512, e->conv2.W + (size_t)q * 512 * 512, 512, 512);
-  g.n_seg = 3; g.N = 512; g.C = e->c2_all; g.ldc = 512; g.bias = e->conv2.b; g.act = e->act_conv2;
-  { ProfScope ps(e, PNB_K_GEMM_F32, st); nl += launch_gemm_f32(g, st); }
-
-  // stacked GRUs: each consumes the freshly updated state of the one below (SURVEY.md App. C.10)
-  F32ChainArgs a;
-  memset(&a, 0, sizeof a);
-  const int n_rb = (int)(((size_t)na + 16 * e->f32_rt - 1) / (16 * e->f32_rt));  // stream blocks of the active streams
-  a.S = S; a.n = na; a.n_rb = n_rb; a.cnt = e->f32_cnt; a.tansig = tbl;
-  for (int li = 0; li < 5; li++) {
-    F32ChainLayer &L = a.L[li];
-    const int H = e->gru[li].H;
-    L.H = H; L.W = e->gru[li].W; L.U = e->gru[li].U; L.bias = e->gru[li].b; L.ldw = 3 * H; L.h = e->h[li][0];
-    if (li == 0) {          // gru1 <- conv2 out
-      L.n_x = 1; L.dep = -1; L.x[0] = e->c2_all; L.x_ld[0] = 512; L.x_K[0] = 512; L.x_slot1[0] = 0; L.x_slot_stride[0] = (size_t)S * 512;
-    } else if (li < 4) {    // gru2 <- gru1, gru3 <- gru2, gru_gb <- gru3
-      L.n_x = 1; L.dep = li - 1; L.x[0] = e->h[li - 1][0]; L.x_ld[0] = 512; L.x_K[0] = 512; L.x_slot1[0] = 1; L.x_slot_stride[0] = (size_t)S * 512;
-    } else {                // gru_rb <- [gru3 state, conv2 out] (rnn.cpp:69-71)
-      L.n_x = 2; L.dep = 2;
-      L.x[0] = e->h[2][0]; L.x_ld[0] = 512; L.x_K[0] = 512; L.x_slot1[0] = 1; L.x_slot_stride[0] = (size_t)S * 512; L.w_row0[0] = 0;
-      L.x[1] = e->c2_all;  L.x_ld[1] = 512; L.x_K[1] = 512; L.x_slot1[1] = 0; L.x_slot_stride[1] = (size_t)S * 512; L.w_row0[1] = 512;
-    }
-  }
-  {
-    // anti-diagonal order: (t, l) sits on diagonal t + depth(l); everything it needs is on an earlier one
-    static const int depth[5] = {0, 1, 2, 3, 3};
-    int k = 0, unit = 0;
-    for (int d = 0; d < n + 3; d++)
-      for (int li = 0; li < 5; li++) {
-        const int t = d - depth[li];
-        if (t < 0 || t >= n) continue;
-        a.lh[k] = (unsigned char)((t << 3) | li);
-        a.lh_unit0[k] = unit;
-        unit += n_rb * (e->gru[li].H / 32);
-        k++;
-      }
-    a.lh_unit0[k] = unit;
-    a.n_lh = k; a.n_units = unit;
-  }
-  {
-    ProfScope ps(e, PNB_K_GEMM_F32, st);
-    if (launch_gru_chain_f32(a, e->f32_rt, e->sm_count, st) < 0) return fail(PNB_ERR_CUDA, "cannot configure the fp32 GRU chain kernel");
-    nl++;
-  }
-  // fc_gb on [conv2, gru1, gru2, gru3, gru_gb] (rnn.cpp:73-78), fc_rb on gru_rb (rnn.cpp:80); state after hop t = slot t+1
-  float *gr = e->d_gr + (size_t)h0 * S * 68;
-  g.seg[0] = seg(e->c2_all, 512, e->fc_gb.W, 34, 512);
-  for (int q = 1; q < 5; q++) g.seg[q] = seg(e->h[q - 1][0] + (size_t)S * 512, 512, e->fc_gb.W + (size_t)q * 512 * 34, 34, 512);
-  g.n_seg = 5; g.N = 34; g.C = gr; g.ldc = 68; g.bias = e->fc_gb.b; g.act = e->act_gb;
-  { ProfScope ps(e, PNB_K_GEMM_F32, st); nl += launch_gemm_f32(g, st); }
-  g.seg[0] = seg(e->h[4][0] + (size_t)S * 128, 128, e->fc_rb.W, 34, 128);
-  g.n_seg = 1; g.N = 34; g.C = gr + 34; g.ldc = 68; g.bias = e->fc_rb.b; g.act = e->act_rb;
-  { ProfScope ps(e, PNB_K_GEMM_F32, st); nl += launch_gemm_f32(g, st); }
-  // carry; in a ragged call a row that stopped inside the chunk takes its own last hop's slots, one that stopped in an
-  // earlier chunk keeps its front slots
-  F32CarryArgs c;
-  memset(&c, 0, sizeof c);
-  int ns = 0;
-  auto cseg = [&](float *dst, const float *src, size_t width, int n_slots, int from) {  // the active rows of n_slots slots of [S][width]
-    c.seg[ns++] = F32CarrySeg{reinterpret_cast<float4 *>(dst), reinterpret_cast<const float4 *>(src), (size_t)na * width / 4,
-                              (size_t)S * width / 4, width / 4, n_slots, from};
-  };
-  cseg(e->ring_fc, e->ring_fc, 128, 4, n);
-  cseg(e->ring_c1, e->ring_c1, 512, 2, n);
-  for (int li = 0; li < 5; li++) cseg(e->h[li][0], e->h[li][0], e->gru[li].H, 1, n);
-  cseg(e->c2, e->c2_all, 512, 1, n - 1);
-  c.n_seg = ns; c.cnt = e->f32_cnt; c.n_cnt = 5 * e->f32_rb;
-  c.hops = hops; c.h0 = h0; c.n = n;
-  { ProfScope ps(e, PNB_K_F32_CARRY, st); nl += launch_f32_carry(c, st); }
-  return nl;
 }
 
 // ------------------------------------------------------------------------------------------
@@ -754,16 +564,10 @@ static int enqueue_enhance(pnb_engine *e, const float *d_in, const short *d_in16
       n += launch_analysis(aa, st);
     }
     CK(cudaGetLastError());
-    if (e->flags & PNB_NN_TENSOR) {
-      const int q = tc_network(e, F, rg.hops, st);
+    {
+      const int q = (e->flags & PNB_NN_TENSOR) ? tc_network(e, F, rg.hops, st) : f32_network(e, F, rg.hops, st);
       if (q < 0) return q;
       n += q;
-    } else {
-      for (int h0 = 0; h0 < F; h0 += e->f32_chunk) {
-        const int q = nn_chunk_f32(e, h0, F - h0 < e->f32_chunk ? F - h0 : e->f32_chunk, rg.hops, st);
-        if (q < 0) return q;
-        n += q;
-      }
     }
     {
       SynthesisArgs sa = synthesis_args(e, F, d_out, d_out16, out_stride);
@@ -1124,7 +928,7 @@ extern "C" int pnb_read_tap(pnb_engine *e, int what, void *dst, size_t dst_bytes
     case PNB_TAP_NN_C2: src = e->c2; bytes = (size_t)e->S * 512 * 4; break;
     case PNB_TAP_NN_H0: case PNB_TAP_NN_H0 + 1: case PNB_TAP_NN_H0 + 2: case PNB_TAP_NN_H0 + 3: case PNB_TAP_NN_H0 + 4: {
       int li = what - PNB_TAP_NN_H0;
-      src = e->h[li][e->par[li]]; bytes = (size_t)e->S * e->gru[li].H * 4; break;
+      src = e->h[li][e->par[li]]; bytes = (size_t)e->S * kGruH[li] * 4; break;
     }
     default: return fail(PNB_ERR_ARG, "unknown tap %d", what);
   }
@@ -1573,10 +1377,9 @@ extern "C" int pnb_pitch_only_host(const float *pitch_buf, size_t stride, long l
 extern "C" long long pnb_launch_count(const pnb_engine *e) { return e ? e->launches : 0; }
 extern "C" int pnb_launches_per_call(const pnb_engine *e, int n_frames) {
   if (!e) return 0;
-  // without the history move of advance_line (at most one more launch per call), and without the fix-up of a ragged
-  // session call in which a session runs fewer hops than the call (one more launch)
-  if (e->flags & PNB_NN_TENSOR) return 10;  // stage_in, analysis, fc, conv1, conv2, GRU chain, fc_gb, fc_rb, carry, synthesis
-  return 3 + 7 * ((n_frames + e->f32_chunk - 1) / e->f32_chunk);  // stage_in, analysis, synthesis + per chunk: fc, conv1, conv2, GRU chain, fc_gb, fc_rb, carry
+  // stage_in, analysis, the network, synthesis; without the history move of advance_line (at most one more launch per
+  // call), and without the fix-up of a ragged session call in which a session runs fewer hops than the call (one more)
+  return 3 + ((e->flags & PNB_NN_TENSOR) ? tc_network_launches(e, n_frames) : f32_network_launches(e, n_frames));
 }
 extern "C" int pnb_n_streams(const pnb_engine *e) { return e ? e->S : 0; }
 extern "C" int pnb_max_frames(const pnb_engine *e) { return e ? e->Fmax : 0; }

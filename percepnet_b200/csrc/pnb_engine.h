@@ -1,6 +1,7 @@
 // pnb_engine.h -- the engine object behind the opaque pnb_engine handle.
 #pragma once
 #include <stddef.h>
+#include <memory>
 #include <vector>
 #include "pnb_kernels.h"
 #include "pnb_session_plan.h"
@@ -8,7 +9,10 @@
 #include "../../include/percepnet_b200.h"
 #include "../../include/pnb_nnet_layout.h"
 
-struct pnb_tc_state;  // tensor-core path (pnb_nn_tc.cu)
+struct pnb_tc_state;   // tensor-core path (pnb_nn_tc.cu)
+struct pnb_f32_state;  // fp32 FMA path (pnb_nn_f32.cu)
+
+constexpr int kGruH[5] = {512, 512, 512, 512, 128};  // hidden sizes of gru1..3, gru_gb, gru_rb (check_model)
 
 struct pnb_engine {
   int S = 0, Fmax = 0, device = 0, sm_count = 0;
@@ -19,10 +23,11 @@ struct pnb_engine {
   cudaStream_t stream = nullptr;  // used by the host-buffer entry points
   pnb::Tables *d_tab = nullptr;
 
-  // weights in the reference's layout (SURVEY.md App. B)
-  struct { float *W = nullptr, *b = nullptr; } fc, conv1, conv2, fc_gb, fc_rb;
-  struct { float *W = nullptr, *U = nullptr, *b = nullptr; int M = 0, H = 0; } gru[5];  // gru1..3, gru_gb, gru_rb
-  int act_fc = 0, act_conv1 = 0, act_conv2 = 0, act_gb = 0, act_rb = 0;
+  // every device buffer whose size is fixed at pnb_create (engine_buffer)
+  struct Buffer { void *p; size_t bytes; bool zero_on_reset; };
+  std::vector<Buffer> buffers;
+
+  struct { float *W = nullptr, *b = nullptr; } fc;  // the fc layer in the reference's layout (SURVEY.md App. B)
 
   // per-stream signal state
   // [S][5280 + c*Fmax*480], c <= kLineCalls: each stream's history line.  A call appends its hops behind the history and
@@ -49,16 +54,11 @@ struct pnb_engine {
   float *d_tap_pitchf = nullptr;
   float *d_tap_g = nullptr;   // [F][S][34] gains as applied (PNB_KEEP_TAPS)
 
-  // network state (fp32 path): conv rings, GRU states (ping-pong), scratch sums
-  float *ring_fc = nullptr;  // [chunk+4][S][128] fc outputs: slots 0..3 the last four hops (oldest first), 4.. the chunk's
-  float *ring_c1 = nullptr;  // [chunk+2][S][512] conv1 outputs, likewise
+  // network state both paths share: conv2's output of the last hop and the GRU states in fp32, whose layout each path's
+  // prepare hook sets (tensor: [S][H] ping-pong by hop parity par; fp32: h[l][0] only, its hop slots [chunk+1][S][H])
   float *c2 = nullptr;       // [S][512]
   float *h[5][2] = {{nullptr, nullptr}, {nullptr, nullptr}, {nullptr, nullptr}, {nullptr, nullptr}, {nullptr, nullptr}};
   int par[5] = {0, 0, 0, 0, 0};
-  float *c2_all = nullptr;   // fp32 path: [chunk][S][512] conv2 outputs of a chunk of hops
-  unsigned *f32_cnt = nullptr;  // fp32 path: [5][f32_rb] dependency counters of the persistent GRU chain
-  int f32_chunk = 8;            // hops per chunk of the fp32 network = min(max_frames, kF32ChainMaxHops)
-  int f32_rt = 8, f32_rb = 0;   // rows per thread of the chain kernel (8: 128-stream blocks, 1: 16-stream blocks); stream blocks
   long hop = 0;  // hops processed since reset
 
   // Device staging of the host-buffer calls (pnb_process_host_*, pnb_submit_host_*, pnb_train_records_host,
@@ -72,7 +72,10 @@ struct pnb_engine {
   cudaEvent_t ev_in[2] = {nullptr, nullptr}, ev_cmp[2] = {nullptr, nullptr}, ev_out[2] = {nullptr, nullptr};
   long long submitted = 0;  // pipelined calls so far
 
-  pnb_tc_state *tc = nullptr;
+  // the network path's own buffers and packed weights; shared_ptr because its deleter is bound in the path's file,
+  // where the type is complete
+  std::shared_ptr<pnb_tc_state> tc;
+  std::shared_ptr<pnb_f32_state> f32;
   int last_frames = 0;
   long long launches = 0;
   // status word on the device: bit 0 = an activation left the domain in which the reference's tansig_approx is
@@ -123,15 +126,36 @@ struct pnb_engine {
   }
 };
 
-// tensor-core path hooks (pnb_nn_tc.cu); return PNB_OK / negative error; the call phases return their launch count
+// A zeroed device buffer (engine_alloc: of n T) whose size is fixed for the engine's life: pnb_destroy frees it, and
+// pnb_reset zeroes it again when zero_on_reset (stream state).  engine_upload fills it from host memory instead; it is
+// never reset.
+cudaError_t engine_buffer(pnb_engine *e, void **p, size_t bytes, bool zero_on_reset, const void *src);
+template <typename T>
+cudaError_t engine_alloc(pnb_engine *e, T **p, size_t n, bool zero_on_reset) {
+  return engine_buffer(e, reinterpret_cast<void **>(p), n * sizeof(T), zero_on_reset, nullptr);
+}
+template <typename T>
+cudaError_t engine_upload(pnb_engine *e, T **p, const T *src, size_t n) {
+  return engine_buffer(e, reinterpret_cast<void **>(p), n * sizeof(T), false, src);
+}
+constexpr bool kStreamState = true, kScratch = false;  // engine_alloc's zero_on_reset
+// Sets pnb_last_error to msg; returns code.
+int engine_fail(int code, const char *msg);
+
+// The network paths' hooks, tensor-core (tc_*, pnb_nn_tc.cu) and fp32 FMA (f32_*, pnb_nn_f32.cu).  Return PNB_OK /
+// a negative error; the network hooks return their launch count.
+// prepare: the path's weights and buffers, and the GRU states e->h in its layout
 int tc_prepare(pnb_engine *e, const pnb_model *model);
-void tc_release(pnb_engine *e);
-int tc_reset(pnb_engine *e);
-// the network of a call of F hops: hop-parallel front, the GRU chain, hop-parallel output layers, carry; hops: the
-// per-slot hops of a ragged session call (device), or null
+int f32_prepare(pnb_engine *e, const pnb_model *model);
+// the network of a call of F hops; hops: the per-slot hops of a ragged session call (device), or null
 int tc_network(pnb_engine *e, int F, const int *hops, cudaStream_t st);
-// The tensor path's pieces of a stream's state (pnb_state.cu): appended to seg[ns..]; returns the new count
+int f32_network(pnb_engine *e, int F, const int *hops, cudaStream_t st);
+// launches of the network of a call of F hops
+int tc_network_launches(const pnb_engine *e, int F);
+int f32_network_launches(const pnb_engine *e, int F);
+// the path's pieces of a stream's state (state_segs, pnb_state.cu): appended to seg[ns..]; returns the new count
 int tc_state_segs(const pnb_engine *e, pnb::StateSeg *seg, int ns);
+int f32_state_segs(const pnb_engine *e, pnb::StateSeg *seg, int ns);
 
 // RAII marker used by the launch schedule: records an event pair around a launch when profiling
 struct ProfScope {

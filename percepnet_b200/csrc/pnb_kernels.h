@@ -85,71 +85,4 @@ int launch_stage_in(float *pcm, size_t pcm_stride, const float *in, const short 
                     const int *hops = nullptr);
 int launch_slide_history(float *pcm, size_t pcm_stride, int n_streams, int n_samples, cudaStream_t st);
 
-// ---- network, fp32 FMA path (pnb_nn_f32.cu) ---------------------------------------------
-// One contraction  C[M x N] = epilogue( sum_seg A_seg[M x K_seg] * B_seg[K_seg x N] ).
-// A segments are activation matrices (row = stream), B segments are slices of the reference's
-// input-major weight arrays (row = input j, column = output i: W[j*ldb + i]).  With an active range the rows are the
-// first M of each of n_slots hop slots.
-struct GemmSeg {
-  const float *A;
-  int lda;
-  const float *B;
-  int ldb;
-  int K;  // multiple of 16
-};
-struct GemmArgs {
-  GemmSeg seg[5];
-  int n_seg;
-  int M, N;           // M: rows per hop slot (all n_slots x M rows when n_slots = 1 and the rows are one flat range)
-  int n_slots;        // hop slots; the rows of slot k start at row k * slot_stride of A and C
-  int slot_stride;
-  float *C;
-  int ldc;
-  const float *bias;  // null -> raw sums
-  int act;            // PNB_ACT_* applied when bias != null
-  const float *tansig;
-};
-int launch_gemm_f32(const GemmArgs &g, cudaStream_t st);
-
-// fc: features [M x 70] -> [M x 128], relu (nnet.cpp:105 on the `fc` layer), on M rows of each of n_slots hop slots
-// slot_stride rows apart
-int launch_fc_f32(const float *feat, const float *W, const float *bias, float *out, int M, int K, int N, int n_slots,
-                  size_t slot_stride, cudaStream_t st);
-
-// The five GRUs of a chunk of hops in one persistent fp32 launch (pnb_nn_f32.cu).  Slot buffers: hop t of the chunk
-// reads state slot t and writes slot t+1; inputs are conv2's output slot t or the layer below's slot t+1.
-struct F32ChainLayer {
-  int H, n_x, dep;            // hidden size; input segments (1 or 2); layer whose fresh state is the input (-1: conv2 out)
-  const float *x[2];          // input buffers [slots][S][x_ld]
-  int x_ld[2], x_K[2], x_slot1[2];
-  size_t x_slot_stride[2];    // floats per hop slot of the input buffer
-  const float *W, *U, *bias;  // reference layout: W [K_in][3H], U [H][3H], bias [6H]
-  int ldw, w_row0[2];         // 3H; first row of W for each input segment
-  float *h;                   // [(n+1) slots][S][H]
-};
-constexpr int kF32ChainMaxHops = 32;  // hops per launch of the fp32 chain (longer chunks amortise the ramp diagonals)
-struct F32ChainArgs {
-  F32ChainLayer L[5];
-  int S, n, n_rb, n_units, n_lh;               // S: rows per slot; n: active streams [0, n); n_rb: their stream blocks
-  unsigned char lh[5 * kF32ChainMaxHops];      // (hop << 3) | layer in anti-diagonal order
-  int lh_unit0[5 * kF32ChainMaxHops + 1];      // first unit of every entry; [n_lh] = n_units
-  unsigned *cnt;                               // [5][n_rb] finished tiles per (layer, stream block), zero at launch
-  const float *tansig;
-};
-int launch_gru_chain_f32(const F32ChainArgs &a, int rows_per_thread, int sm_count, cudaStream_t st);
-// The first slot4 float4s of n_slots slots stride4 apart, from slots from.. of src (slot 0 of the source buffer) to
-// dst; row4: float4s per row.  In a ragged call (hops) a row that stops after hop h of the call takes its slots from
-// from - (n - clamp(h - h0, 0, n)) on instead (it stopped that many slots before the chunk's end), and nothing moves
-// when that is below 0 or the row is already in place.
-struct F32CarrySeg { float4 *dst; const float4 *src; size_t slot4, stride4, row4; int n_slots, from; };
-struct F32CarryArgs {
-  F32CarrySeg seg[12];
-  int n_seg;
-  unsigned *cnt;
-  int n_cnt;
-  const int *hops;  // [active streams] hops of each row in a ragged call, or null
-  int h0, n;        // the chunk: hops [h0, h0 + n) of the call
-};
-int launch_f32_carry(const F32CarryArgs &a, cudaStream_t st);
-
 }  // namespace pnb

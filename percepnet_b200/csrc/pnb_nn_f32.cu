@@ -6,11 +6,73 @@
 // weight tile is reused across 128 streams from shared memory; activations use the reference's
 // tansig table approximation (vec.h:53-76).  Per chunk of hops: fc, conv1, conv2 over all rows of the chunk
 // (gemm_f32_kernel), the five GRUs of all its hops in one persistent launch (gru_chain_f32_kernel), the output layers,
-// and a carry; the schedule is nn_chunk_f32 in pnb_engine.cu.
-#include "pnb_kernels.h"
-#include "../../include/pnb_nnet_layout.h"
+// and a carry.  The host side at the end of the file is the path's part of the engine: its weights and buffers
+// (pnb_f32_state), and the hooks the engine calls (f32_prepare, f32_network, f32_state_segs).
+#include <string.h>
+
+#include <string>
+
+#include "pnb_engine.h"
 
 namespace pnb {
+
+// One contraction  C[M x N] = epilogue( sum_seg A_seg[M x K_seg] * B_seg[K_seg x N] ).
+// A segments are activation matrices (row = stream), B segments are slices of the reference's
+// input-major weight arrays (row = input j, column = output i: W[j*ldb + i]).  With an active range the rows are the
+// first M of each of n_slots hop slots.
+struct GemmSeg {
+  const float *A;
+  int lda;
+  const float *B;
+  int ldb;
+  int K;  // multiple of 16
+};
+struct GemmArgs {
+  GemmSeg seg[5];
+  int n_seg;
+  int M, N;           // M: rows per hop slot (all n_slots x M rows when n_slots = 1 and the rows are one flat range)
+  int n_slots;        // hop slots; the rows of slot k start at row k * slot_stride of A and C
+  int slot_stride;
+  float *C;
+  int ldc;
+  const float *bias;  // null -> raw sums
+  int act;            // PNB_ACT_* applied when bias != null
+  const float *tansig;
+};
+
+// The five GRUs of a chunk of hops in one persistent fp32 launch.  Slot buffers: hop t of the chunk
+// reads state slot t and writes slot t+1; inputs are conv2's output slot t or the layer below's slot t+1.
+struct F32ChainLayer {
+  int H, n_x, dep;            // hidden size; input segments (1 or 2); layer whose fresh state is the input (-1: conv2 out)
+  const float *x[2];          // input buffers [slots][S][x_ld]
+  int x_ld[2], x_K[2], x_slot1[2];
+  size_t x_slot_stride[2];    // floats per hop slot of the input buffer
+  const float *W, *U, *bias;  // reference layout: W [K_in][3H], U [H][3H], bias [6H]
+  int ldw, w_row0[2];         // 3H; first row of W for each input segment
+  float *h;                   // [(n+1) slots][S][H]
+};
+constexpr int kF32ChainMaxHops = 32;  // hops per launch of the fp32 chain (longer chunks amortise the ramp diagonals)
+struct F32ChainArgs {
+  F32ChainLayer L[5];
+  int S, n, n_rb, n_units, n_lh;               // S: rows per slot; n: active streams [0, n); n_rb: their stream blocks
+  unsigned char lh[5 * kF32ChainMaxHops];      // (hop << 3) | layer in anti-diagonal order
+  int lh_unit0[5 * kF32ChainMaxHops + 1];      // first unit of every entry; [n_lh] = n_units
+  unsigned *cnt;                               // [5][n_rb] finished tiles per (layer, stream block), zero at launch
+  const float *tansig;
+};
+// The first slot4 float4s of n_slots slots stride4 apart, from slots from.. of src (slot 0 of the source buffer) to
+// dst; row4: float4s per row.  In a ragged call (hops) a row that stops after hop h of the call takes its slots from
+// from - (n - clamp(h - h0, 0, n)) on instead (it stopped that many slots before the chunk's end), and nothing moves
+// when that is below 0 or the row is already in place.
+struct F32CarrySeg { float4 *dst; const float4 *src; size_t slot4, stride4, row4; int n_slots, from; };
+struct F32CarryArgs {
+  F32CarrySeg seg[12];
+  int n_seg;
+  unsigned *cnt;
+  int n_cnt;
+  const int *hops;  // [active streams] hops of each row in a ragged call, or null
+  int h0, n;        // the chunk: hops [h0, h0 + n) of the call
+};
 
 __device__ __forceinline__ float tansig_approx(float x, const float *__restrict__ tbl) {  // vec.h:53-71
   float sign = 1.f;
@@ -437,3 +499,189 @@ int launch_f32_carry(const F32CarryArgs &a, cudaStream_t st) {
 }
 
 }  // namespace pnb
+
+// ------------------------------------------------------------------------------------------ host state
+using namespace pnb;
+
+struct pnb_f32_state {
+  // weights in the reference's layout (SURVEY.md App. B); fc is the engine's, the tensor path reads it too
+  struct { float *W = nullptr, *b = nullptr; } conv1, conv2, fc_gb, fc_rb;
+  struct { float *W = nullptr, *U = nullptr, *b = nullptr; } gru[5];  // gru1..3, gru_gb, gru_rb
+  // Hop-slot buffers of one chunk of at most chunk_hops(e) hops.  Slots 0.. of the fc / conv1 buffers hold the conv
+  // histories (oldest first), slot 0 of every GRU state buffer e->h[l][0] ([chunk+1][S][H]) the state before the
+  // chunk's first hop; the chunk's carry moves the last slots back there, so between calls the state lives at the front
+  // (par stays 0).
+  float *ring_fc = nullptr;  // [chunk+4][S][128] fc outputs: slots 0..3 the last four hops (oldest first), 4.. the chunk's
+  float *ring_c1 = nullptr;  // [chunk+2][S][512] conv1 outputs, likewise
+  float *c2_all = nullptr;   // [chunk][S][512] conv2 outputs of the chunk
+  unsigned *cnt = nullptr;   // [5][rb] dependency counters of the persistent GRU chain
+  int rt = 8, rb = 0;        // rows per thread of the chain kernel (8: 128-stream blocks, 1: 16-stream blocks); stream blocks
+};
+
+// hops per chunk of the network
+static int chunk_hops(const pnb_engine *e) { return e->Fmax < kF32ChainMaxHops ? e->Fmax : kF32ChainMaxHops; }
+
+#define FCK(call)                                                                                                   \
+  do {                                                                                                              \
+    cudaError_t _e = (call);                                                                                        \
+    if (_e != cudaSuccess)                                                                                          \
+      return engine_fail(_e == cudaErrorMemoryAllocation ? PNB_ERR_ALLOC : PNB_ERR_CUDA,                            \
+                         (std::string(#call) + " failed: " + cudaGetErrorString(_e)).c_str());                      \
+  } while (0)
+
+int f32_prepare(pnb_engine *e, const pnb_model *model) {
+  e->f32 = std::make_shared<pnb_f32_state>();
+  pnb_f32_state &f = *e->f32;
+  FCK(engine_upload(e, &f.conv1.W, model->conv1->input_weights, 5 * 128 * 512));
+  FCK(engine_upload(e, &f.conv1.b, model->conv1->bias, 512));
+  FCK(engine_upload(e, &f.conv2.W, model->conv2->input_weights, 3 * 512 * 512));
+  FCK(engine_upload(e, &f.conv2.b, model->conv2->bias, 512));
+  const pnb_gru_layer *g5[5] = {model->gru1, model->gru2, model->gru3, model->gru_gb, model->gru_rb};
+  for (int i = 0; i < 5; i++) {
+    const size_t M = g5[i]->nb_inputs, H = kGruH[i];
+    FCK(engine_upload(e, &f.gru[i].W, g5[i]->input_weights, M * 3 * H));
+    FCK(engine_upload(e, &f.gru[i].U, g5[i]->recurrent_weights, H * 3 * H));
+    FCK(engine_upload(e, &f.gru[i].b, g5[i]->bias, 6 * H));
+  }
+  FCK(engine_upload(e, &f.fc_gb.W, model->fc_gb->input_weights, 2560 * 34));
+  FCK(engine_upload(e, &f.fc_gb.b, model->fc_gb->bias, 34));
+  FCK(engine_upload(e, &f.fc_rb.W, model->fc_rb->input_weights, 128 * 34));
+  FCK(engine_upload(e, &f.fc_rb.b, model->fc_rb->bias, 34));
+  const size_t S = e->S, C = chunk_hops(e);
+  f.rt = S <= 64 ? 1 : 8;
+  f.rb = (int)((S + 16 * f.rt - 1) / (16 * f.rt));
+  FCK(engine_alloc(e, &f.ring_fc, (C + 4) * S * 128, kStreamState));
+  FCK(engine_alloc(e, &f.ring_c1, (C + 2) * S * 512, kStreamState));
+  FCK(engine_alloc(e, &f.c2_all, C * S * 512, kScratch));
+  for (int i = 0; i < 5; i++) FCK(engine_alloc(e, &e->h[i][0], (C + 1) * S * kGruH[i], kStreamState));
+  FCK(engine_alloc(e, &f.cnt, (size_t)5 * f.rb, kStreamState));
+  return PNB_OK;
+}
+
+static GemmSeg seg(const float *A, int lda, const float *B, int ldb, int K) {
+  GemmSeg s;
+  s.A = A; s.lda = lda; s.B = B; s.ldb = ldb; s.K = K;
+  return s;
+}
+
+// The network of hops [h0, h0 + n) of a call (n <= chunk_hops(e)) in fp32 FMA (rnn.cpp:42-81): the non-recurrent layers
+// once over the active rows of all n hop slots, the five GRUs of all n hops in one persistent launch, the output layers
+// over the same rows, and the carry that moves the conv histories and the states back to the front of their slot buffers.
+// hops: the per-slot hops of a ragged call (device), or null.
+static int run_chunk(pnb_engine *e, int h0, int n, const int *hops, cudaStream_t st) {
+  const pnb_f32_state &f = *e->f32;
+  const int S = e->S, na = e->n_active;
+  // all streams active: the rows of the n slots are one flat range; otherwise the first na rows of each slot
+  const int rows = na == S ? n * S : na, slots = na == S ? 1 : n;
+  const float *tbl = e->tansig();
+  int nl = 0;
+  // fc -> slots 4.. (slots 0..3 hold the last four hops' outputs)
+  { ProfScope ps(e, PNB_K_FC, st); nl += launch_fc_f32(e->d_feat + (size_t)h0 * S * kFeat, e->fc.W, e->fc.b, f.ring_fc + (size_t)4 * S * 128, rows, 70, 128, slots, S, st); }
+  GemmArgs g;
+  memset(&g, 0, sizeof g);
+  g.M = rows; g.n_slots = slots; g.slot_stride = S; g.tansig = tbl;
+  // conv1: tap q of hop t reads fc slot t + q (oldest first, nnet.cpp:182-200; weights [tap][c][n]) -> c1 slots 2..
+  for (int q = 0; q < 5; q++) g.seg[q] = seg(f.ring_fc + (size_t)q * S * 128, 128, f.conv1.W + (size_t)q * 128 * 512, 512, 128);
+  g.n_seg = 5; g.N = 512; g.C = f.ring_c1 + (size_t)2 * S * 512; g.ldc = 512; g.bias = f.conv1.b; g.act = PNB_ACT_RELU;
+  { ProfScope ps(e, PNB_K_GEMM_F32, st); nl += launch_gemm_f32(g, st); }
+  for (int q = 0; q < 3; q++) g.seg[q] = seg(f.ring_c1 + (size_t)q * S * 512, 512, f.conv2.W + (size_t)q * 512 * 512, 512, 512);
+  g.n_seg = 3; g.N = 512; g.C = f.c2_all; g.ldc = 512; g.bias = f.conv2.b; g.act = PNB_ACT_TANH;
+  { ProfScope ps(e, PNB_K_GEMM_F32, st); nl += launch_gemm_f32(g, st); }
+
+  // stacked GRUs: each consumes the freshly updated state of the one below (SURVEY.md App. C.10)
+  F32ChainArgs a;
+  memset(&a, 0, sizeof a);
+  const int n_rb = (int)(((size_t)na + 16 * f.rt - 1) / (16 * f.rt));  // stream blocks of the active streams
+  a.S = S; a.n = na; a.n_rb = n_rb; a.cnt = f.cnt; a.tansig = tbl;
+  for (int li = 0; li < 5; li++) {
+    F32ChainLayer &L = a.L[li];
+    const int H = kGruH[li];
+    L.H = H; L.W = f.gru[li].W; L.U = f.gru[li].U; L.bias = f.gru[li].b; L.ldw = 3 * H; L.h = e->h[li][0];
+    if (li == 0) {          // gru1 <- conv2 out
+      L.n_x = 1; L.dep = -1; L.x[0] = f.c2_all; L.x_ld[0] = 512; L.x_K[0] = 512; L.x_slot1[0] = 0; L.x_slot_stride[0] = (size_t)S * 512;
+    } else if (li < 4) {    // gru2 <- gru1, gru3 <- gru2, gru_gb <- gru3
+      L.n_x = 1; L.dep = li - 1; L.x[0] = e->h[li - 1][0]; L.x_ld[0] = 512; L.x_K[0] = 512; L.x_slot1[0] = 1; L.x_slot_stride[0] = (size_t)S * 512;
+    } else {                // gru_rb <- [gru3 state, conv2 out] (rnn.cpp:69-71)
+      L.n_x = 2; L.dep = 2;
+      L.x[0] = e->h[2][0]; L.x_ld[0] = 512; L.x_K[0] = 512; L.x_slot1[0] = 1; L.x_slot_stride[0] = (size_t)S * 512; L.w_row0[0] = 0;
+      L.x[1] = f.c2_all;  L.x_ld[1] = 512; L.x_K[1] = 512; L.x_slot1[1] = 0; L.x_slot_stride[1] = (size_t)S * 512; L.w_row0[1] = 512;
+    }
+  }
+  {
+    // anti-diagonal order: (t, l) sits on diagonal t + depth(l); everything it needs is on an earlier one
+    static const int depth[5] = {0, 1, 2, 3, 3};
+    int k = 0, unit = 0;
+    for (int d = 0; d < n + 3; d++)
+      for (int li = 0; li < 5; li++) {
+        const int t = d - depth[li];
+        if (t < 0 || t >= n) continue;
+        a.lh[k] = (unsigned char)((t << 3) | li);
+        a.lh_unit0[k] = unit;
+        unit += n_rb * (kGruH[li] / 32);
+        k++;
+      }
+    a.lh_unit0[k] = unit;
+    a.n_lh = k; a.n_units = unit;
+  }
+  {
+    ProfScope ps(e, PNB_K_GEMM_F32, st);
+    if (launch_gru_chain_f32(a, f.rt, e->sm_count, st) < 0) return engine_fail(PNB_ERR_CUDA, "cannot configure the fp32 GRU chain kernel");
+    nl++;
+  }
+  // fc_gb on [conv2, gru1, gru2, gru3, gru_gb] (rnn.cpp:73-78), fc_rb on gru_rb (rnn.cpp:80); state after hop t = slot t+1
+  float *gr = e->d_gr + (size_t)h0 * S * 68;
+  g.seg[0] = seg(f.c2_all, 512, f.fc_gb.W, 34, 512);
+  for (int q = 1; q < 5; q++) g.seg[q] = seg(e->h[q - 1][0] + (size_t)S * 512, 512, f.fc_gb.W + (size_t)q * 512 * 34, 34, 512);
+  g.n_seg = 5; g.N = 34; g.C = gr; g.ldc = 68; g.bias = f.fc_gb.b; g.act = PNB_ACT_SIGMOID;
+  { ProfScope ps(e, PNB_K_GEMM_F32, st); nl += launch_gemm_f32(g, st); }
+  g.seg[0] = seg(e->h[4][0] + (size_t)S * 128, 128, f.fc_rb.W, 34, 128);
+  g.n_seg = 1; g.N = 34; g.C = gr + 34; g.ldc = 68; g.bias = f.fc_rb.b; g.act = PNB_ACT_SIGMOID;
+  { ProfScope ps(e, PNB_K_GEMM_F32, st); nl += launch_gemm_f32(g, st); }
+  // carry; in a ragged call a row that stopped inside the chunk takes its own last hop's slots, one that stopped in an
+  // earlier chunk keeps its front slots
+  F32CarryArgs c;
+  memset(&c, 0, sizeof c);
+  int ns = 0;
+  auto cseg = [&](float *dst, const float *src, size_t width, int n_slots, int from) {  // the active rows of n_slots slots of [S][width]
+    c.seg[ns++] = F32CarrySeg{reinterpret_cast<float4 *>(dst), reinterpret_cast<const float4 *>(src), (size_t)na * width / 4,
+                              (size_t)S * width / 4, width / 4, n_slots, from};
+  };
+  cseg(f.ring_fc, f.ring_fc, 128, 4, n);
+  cseg(f.ring_c1, f.ring_c1, 512, 2, n);
+  for (int li = 0; li < 5; li++) cseg(e->h[li][0], e->h[li][0], kGruH[li], 1, n);
+  cseg(e->c2, f.c2_all, 512, 1, n - 1);
+  c.n_seg = ns; c.cnt = f.cnt; c.n_cnt = 5 * f.rb;
+  c.hops = hops; c.h0 = h0; c.n = n;
+  { ProfScope ps(e, PNB_K_F32_CARRY, st); nl += launch_f32_carry(c, st); }
+  return nl;
+}
+
+// The network of a call of F hops: chunks of up to chunk_hops(e) hops, in order.
+int f32_network(pnb_engine *e, int F, const int *hops, cudaStream_t st) {
+  const int C = chunk_hops(e);
+  int nl = 0;
+  for (int h0 = 0; h0 < F; h0 += C) {
+    const int q = run_chunk(e, h0, F - h0 < C ? F - h0 : C, hops, st);
+    if (q < 0) return q;
+    nl += q;
+  }
+  return nl;
+}
+
+int f32_network_launches(const pnb_engine *e, int F) {
+  const int C = chunk_hops(e);
+  return 7 * ((F + C - 1) / C);  // per chunk: fc, conv1, conv2, GRU chain, fc_gb, fc_rb, carry
+}
+
+// The fp32 path's part of a stream's state: the conv histories at slots 0..3 / 0..1 of the hop-slot buffers (where
+// run_chunk's carry leaves them); the blob's bf16 term planes, which only tensor engines fill, are written as zeros.
+int f32_state_segs(const pnb_engine *e, StateSeg *seg, int ns) {
+  const pnb_f32_state &f = *e->f32;
+  const size_t S = e->S;
+  for (int k = 0; k < 4; k++)
+    add_words(seg, ns, kSegCopy, f.ring_fc + (size_t)k * S * 128, 128 * 4, offsetof(StreamState, fc_hist) + (size_t)k * 128 * 4, 128);
+  for (int k = 0; k < 2; k++)
+    add_words(seg, ns, kSegCopy, f.ring_c1 + (size_t)k * S * 512, 512 * 4, offsetof(StreamState, c1_hist) + (size_t)k * 512 * 4, 512);
+  add_words(seg, ns, kSegBlobZero, nullptr, 0, offsetof(StreamState, fc_terms), (sizeof(StreamState) - offsetof(StreamState, fc_terms)) / 4);
+  return ns;
+}

@@ -999,14 +999,12 @@ static float pow2_scale_for(const float *a, size_t na, const float *b, size_t nb
   return ldexpf(1.f, e);
 }
 
-extern int tc_fail(int code, const char *msg);  // sets pnb_last_error (pnb_engine.cu)
-
 #define TCK(call)                                                                          \
   do {                                                                                     \
     cudaError_t _e = (call);                                                               \
     if (_e != cudaSuccess) {                                                               \
       g_tc_err = std::string(#call) + ": " + cudaGetErrorString(_e);                       \
-      return tc_fail(PNB_ERR_CUDA, g_tc_err.c_str());                                      \
+      return engine_fail(PNB_ERR_CUDA, g_tc_err.c_str());                                      \
     }                                                                                      \
   } while (0)
 
@@ -1074,25 +1072,12 @@ static double max_preact(const float *W, int K, int N, int ld, const float *U, i
   return mx;
 }
 
-template <typename T>
-static cudaError_t dev_upload(T **dst, const std::vector<T> &src) {
-  cudaError_t e = cudaMalloc((void **)dst, src.size() * sizeof(T));
-  if (e != cudaSuccess) return e;
-  return cudaMemcpy(*dst, src.data(), src.size() * sizeof(T), cudaMemcpyHostToDevice);
-}
-template <typename T>
-static cudaError_t dev_zeros(T **dst, size_t n) {
-  cudaError_t e = cudaMalloc((void **)dst, n * sizeof(T));
-  if (e != cudaSuccess) return e;
-  return cudaMemset(*dst, 0, n * sizeof(T));
-}
-
 int tc_prepare(pnb_engine *e, const pnb_model *model) {
   if (!g_encode) {
     void *fn = nullptr;
     cudaDriverEntryPointQueryResult qr;
     cudaError_t r = cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qr);
-    if (r != cudaSuccess || !fn) return tc_fail(PNB_ERR_CUDA, "cuTensorMapEncodeTiled is not available from the driver");
+    if (r != cudaSuccess || !fn) return engine_fail(PNB_ERR_CUDA, "cuTensorMapEncodeTiled is not available from the driver");
     g_encode = (EncodeTiledFn)fn;
   }
   const pnb_gru_layer *g5[5] = {model->gru1, model->gru2, model->gru3, model->gru_gb, model->gru_rb};
@@ -1111,31 +1096,32 @@ int tc_prepare(pnb_engine *e, const pnb_model *model) {
     v = max_preact(model->fc_rb->input_weights, 128, 34, 34, nullptr, 0, model->fc_rb->bias, nullptr);
     if (!(v <= mx)) mx = v;
     if (!(mx < kTanhDomain))
-      return tc_fail(PNB_ERR_ARG, "PNB_NN_TENSOR: a GRU / output layer can form pre-activations >= 8.5e7 (or NaN), outside the "
+      return engine_fail(PNB_ERR_ARG, "PNB_NN_TENSOR: a GRU / output layer can form pre-activations >= 8.5e7 (or NaN), outside the "
                                   "domain of the reference's tansig_approx; use PNB_NN_FP32 for this model");
   }
-  pnb_tc_state *t = new pnb_tc_state();
-  e->tc = t;
+  e->tc = std::make_shared<pnb_tc_state>();
+  pnb_tc_state *t = e->tc.get();
   const size_t S = e->S;
   const size_t Fm = e->Fmax;
-  TCK(dev_zeros(&t->fc_all, kConvTerms * (Fm + 4) * S * 128));
-  TCK(dev_zeros(&t->c1_all, kConvTerms * (Fm + 2) * S * 512));
-  TCK(dev_zeros(&t->wide, 1));
+  for (int i = 0; i < 5; i++)
+    for (int p = 0; p < 2; p++) TCK(engine_alloc(e, &e->h[i][p], S * kGruH[i], kStreamState));
+  TCK(engine_alloc(e, &t->fc_all, kConvTerms * (Fm + 4) * S * 128, kStreamState));
+  TCK(engine_alloc(e, &t->c1_all, kConvTerms * (Fm + 2) * S * 512, kStreamState));
   {
     int w = (e->flags & PNB_CONV_WIDE) ? 1 : 0;
     if (const char *ct = getenv("PNB_CONV_TERMS")) w = atoi(ct) == 3 ? 1 : atoi(ct) == 2 ? 0 : w;  // experiments
-    TCK(cudaMemcpy(t->wide, &w, sizeof w, cudaMemcpyHostToDevice));
+    TCK(engine_upload(e, &t->wide, &w, 1));
   }
-  TCK(dev_zeros(&t->c2_h, 2 * Fm * S * 512));
-  for (int i = 0; i < 5; i++) TCK(dev_zeros(&t->h_all[i], 2 * (Fm + 1) * S * e->gru[i].H));
+  TCK(engine_alloc(e, &t->c2_h, 2 * Fm * S * 512, kStreamState));
+  for (int i = 0; i < 5; i++) TCK(engine_alloc(e, &t->h_all[i], 2 * (Fm + 1) * S * kGruH[i], kStreamState));
   t->tiles_mp = (int)((S + TM - 1) / TM);
-  TCK(dev_zeros(&t->cnt, (size_t)5 * t->tiles_mp));
+  TCK(engine_alloc(e, &t->cnt, (size_t)5 * t->tiles_mp, kStreamState));
   {
     std::vector<__nv_bfloat16> p;
     pack_dense_b3(model->conv1->input_weights, 640, 512, p);
-    TCK(dev_upload(&t->w_conv1, p));
+    TCK(engine_upload(e, &t->w_conv1, p.data(), p.size()));
     pack_dense_b3(model->conv2->input_weights, 1536, 512, p);
-    TCK(dev_upload(&t->w_conv2, p));
+    TCK(engine_upload(e, &t->w_conv2, p.data(), p.size()));
   }
   for (int i = 0; i < 5; i++) {
     const int K = g5[i]->nb_inputs, H = g5[i]->nb_neurons;
@@ -1144,14 +1130,14 @@ int tc_prepare(pnb_engine *e, const pnb_model *model) {
     t->scale_gru[i] = ldexpf(1.f, -(10 + ex));
     std::vector<__half> p;
     pack_gru(g5[i]->input_weights, K, H, sc, p);
-    TCK(dev_upload(&t->w_gru[i], p));
+    TCK(engine_upload(e, &t->w_gru[i], p.data(), p.size()));
     pack_gru(g5[i]->recurrent_weights, H, H, sc, p);
-    TCK(dev_upload(&t->u_gru[i], p));
+    TCK(engine_upload(e, &t->u_gru[i], p.data(), p.size()));
     // nnet.cpp:136-160: z and r start from b + b' (one float add), the candidate keeps b_n and b'_n apart
     const float *b = g5[i]->bias;
     std::vector<float4> b4(H);
     for (int j = 0; j < H; j++) b4[j] = make_float4(b[j] + b[3 * H + j], b[H + j] + b[4 * H + j], b[2 * H + j], b[5 * H + j]);
-    TCK(dev_upload(&t->bias4[i], b4));
+    TCK(engine_upload(e, &t->bias4[i], b4.data(), b4.size()));
   }
   {
     int ex;
@@ -1159,17 +1145,17 @@ int tc_prepare(pnb_engine *e, const pnb_model *model) {
     float sc = pow2_scale_for(model->fc_gb->input_weights, (size_t)2560 * 34, nullptr, 0, &ex);
     t->scale_gb = ldexpf(1.f, -(10 + ex));
     pack_small_h2(model->fc_gb->input_weights, 2560, 34, sc, p);
-    TCK(dev_upload(&t->w_gb, p));
+    TCK(engine_upload(e, &t->w_gb, p.data(), p.size()));
     sc = pow2_scale_for(model->fc_rb->input_weights, (size_t)128 * 34, nullptr, 0, &ex);
     t->scale_rb = ldexpf(1.f, -(10 + ex));
     pack_small_h2(model->fc_rb->input_weights, 128, 34, sc, p);
-    TCK(dev_upload(&t->w_rb, p));
+    TCK(engine_upload(e, &t->w_rb, p.data(), p.size()));
     std::vector<float> bp(512 + 512 + 48 + 48, 0.f);
     memcpy(bp.data(), model->conv1->bias, 512 * 4);
     memcpy(bp.data() + 512, model->conv2->bias, 512 * 4);
     memcpy(bp.data() + 1024, model->fc_gb->bias, 34 * 4);
     memcpy(bp.data() + 1072, model->fc_rb->bias, 34 * 4);
-    TCK(dev_upload(&t->bias_pad, bp));
+    TCK(engine_upload(e, &t->bias_pad, bp.data(), bp.size()));
   }
   int bad = 0;
   bad |= make_map(&t->m_wgb, t->w_gb, false, 2 * SMALL_BN, 2560, SMALL_BN);
@@ -1178,19 +1164,19 @@ int tc_prepare(pnb_engine *e, const pnb_model *model) {
   bad |= make_map(&t->m_c1_all, t->c1_all, true, kConvTerms * (Fm + 2) * S, 512, TM);
   bad |= make_map(&t->m_c2, t->c2_h, false, 2 * Fm * S, 512, TM);
   for (int i = 0; i < 5; i++)
-    bad |= make_map(&t->m_h[i], t->h_all[i], false, 2 * (Fm + 1) * S, e->gru[i].H, TM);
+    bad |= make_map(&t->m_h[i], t->h_all[i], false, 2 * (Fm + 1) * S, kGruH[i], TM);
   bad |= make_map(&t->m_wconv1, t->w_conv1, true, kConvTerms * 512, 640, DENSE_BN);
   bad |= make_map(&t->m_wconv2, t->w_conv2, true, kConvTerms * 512, 1536, DENSE_BN);
   // the chain's operands: the same buffers in boxes of 32 k
   const CUtensorMapSwizzle sw64 = CU_TENSOR_MAP_SWIZZLE_64B;
   bad |= make_map(&t->m_c2_ch, t->c2_h, false, 2 * Fm * S, 512, TM, CBK, sw64);
   for (int i = 0; i < 5; i++) {
-    const int rows = (e->gru[i].H / HT) * GRU_BN;
-    bad |= make_map(&t->m_h_ch[i], t->h_all[i], false, 2 * (Fm + 1) * S, e->gru[i].H, TM, CBK, sw64);
-    bad |= make_map(&t->m_w[i], t->w_gru[i], false, 2 * rows, e->gru[i].M, GRU_BN, CBK, sw64);
-    bad |= make_map(&t->m_u[i], t->u_gru[i], false, 2 * rows, e->gru[i].H, GRU_BN, CBK, sw64);
+    const int rows = (kGruH[i] / HT) * GRU_BN;
+    bad |= make_map(&t->m_h_ch[i], t->h_all[i], false, 2 * (Fm + 1) * S, kGruH[i], TM, CBK, sw64);
+    bad |= make_map(&t->m_w[i], t->w_gru[i], false, 2 * rows, g5[i]->nb_inputs, GRU_BN, CBK, sw64);
+    bad |= make_map(&t->m_u[i], t->u_gru[i], false, 2 * rows, kGruH[i], GRU_BN, CBK, sw64);
   }
-  if (bad) return tc_fail(PNB_ERR_CUDA, "cuTensorMapEncodeTiled failed");
+  if (bad) return engine_fail(PNB_ERR_CUDA, "cuTensorMapEncodeTiled failed");
   TCK(cudaFuncSetAttribute(gru_chain_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                            (int)tc_smem_bytes<GRU_STAGES, GRU_STAGES * GruStage::kBytes>()));
   TCK(cudaFuncSetAttribute(tc_gemm_kernel<DENSE_BN, true, DENSE_STAGES, DENSE_STAGES3>, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -1200,41 +1186,13 @@ int tc_prepare(pnb_engine *e, const pnb_model *model) {
   return PNB_OK;
 }
 
-void tc_release(pnb_engine *e) {
-  pnb_tc_state *t = e->tc;
-  if (!t) return;
-  void *ptrs[] = {t->fc_all, t->c1_all, t->c2_h, t->w_conv1, t->w_conv2, t->w_gb, t->w_rb, t->bias_pad, t->cnt, t->wide};
-  for (void *p : ptrs) if (p) cudaFree(p);
-  for (int i = 0; i < 5; i++) {
-    if (t->h_all[i]) cudaFree(t->h_all[i]);
-    if (t->w_gru[i]) cudaFree(t->w_gru[i]);
-    if (t->u_gru[i]) cudaFree(t->u_gru[i]);
-    if (t->bias4[i]) cudaFree(t->bias4[i]);
-  }
-  delete t;
-  e->tc = nullptr;
-}
-
-int tc_reset(pnb_engine *e) {
-  pnb_tc_state *t = e->tc;
-  if (!t) return PNB_OK;
-  const size_t S = e->S;
-  const size_t Fm = e->Fmax;
-  TCK(cudaMemset(t->fc_all, 0, kConvTerms * (Fm + 4) * S * 128 * 2));
-  TCK(cudaMemset(t->c1_all, 0, kConvTerms * (Fm + 2) * S * 512 * 2));
-  TCK(cudaMemset(t->c2_h, 0, 2 * Fm * S * 512 * 2));
-  for (int i = 0; i < 5; i++) TCK(cudaMemset(t->h_all[i], 0, 2 * (Fm + 1) * S * e->gru[i].H * 2));
-  TCK(cudaMemset(t->cnt, 0, (size_t)5 * t->tiles_mp * sizeof(unsigned)));
-  return PNB_OK;
-}
-
 // The tensor path's part of a stream's state: the conv input histories (the last 4 fc / 2 conv1 outputs, oldest first)
 // as the three bf16 term planes of hop slots 0..3 / 0..1, and the fp16 hi / lo terms of the GRU states at slot 0.
 // Export writes the terms and their fp32 sums; import restores the raw terms, or splits blobs without them (fp32-mode
 // engines) with the roundings of store_split_b2 / store_split_h2.
 int tc_state_segs(const pnb_engine *e, StateSeg *seg, int ns) {
   static_assert(kConvTerms == 3, "StreamState carries three bf16 terms per conv history value");
-  const pnb_tc_state *t = e->tc;
+  const pnb_tc_state *t = e->tc.get();
   const size_t S = e->S, Fm = e->Fmax;
   auto hist = [&](const __nv_bfloat16 *base, size_t plane, int slots, int width, size_t sum_off, size_t terms_off) {
     for (int i = 0; i < slots; i++) {
@@ -1254,7 +1212,7 @@ int tc_state_segs(const pnb_engine *e, StateSeg *seg, int ns) {
   hist(t->c1_all, (Fm + 2) * S * 512, 2, 512, offsetof(StreamState, c1_hist), offsetof(StreamState, c1_terms));
   size_t off = 0;
   for (int li = 0; li < 5; li++) {
-    const size_t H = e->gru[li].H;
+    const size_t H = kGruH[li];
     for (int tm = 0; tm < 2; tm++) {
       StateSeg g = StateSeg();
       g.kind = kSegSplitF16; g.eng = (char *)(t->h_all[li] + (size_t)tm * (Fm + 1) * S * H); g.eng_stride = H * 2;
@@ -1301,7 +1259,7 @@ static TcSeg mkseg(int a_map, int b_map, int K, int a_k0, int b_k0, int a_row0, 
 // The non-recurrent front (rnn.cpp:50-52 on F S rows): fc -> conv1 -> conv2.  Hop t of the call lives in slot t of the
 // per-call buffers.
 static int tc_front(pnb_engine *e, int F, const int *hops, cudaStream_t st) {
-  pnb_tc_state *t = e->tc;
+  pnb_tc_state *t = e->tc.get();
   const int S = e->S, Fm = e->Fmax, na = e->n_active;
   const float *tbl = e->tansig();
   int nl = 0, rc;
@@ -1348,7 +1306,7 @@ static int tc_front(pnb_engine *e, int F, const int *hops, cudaStream_t st) {
 // The recurrent part: five GRUs per hop (rnn.cpp:58-71) in one persistent launch.  State slot t holds the state
 // BEFORE hop t of the call; the fp32 state ping-pongs by hop, starting from e->par (the call's first hop).
 static int tc_gru_chain(pnb_engine *e, int F, const int *hops, cudaStream_t st) {
-  pnb_tc_state *t = e->tc;
+  pnb_tc_state *t = e->tc.get();
   const int S = e->S, Fm = e->Fmax;
   ChainArgs a;
   memset(&a, 0, sizeof a);
@@ -1361,7 +1319,7 @@ static int tc_gru_chain(pnb_engine *e, int F, const int *hops, cudaStream_t st) 
   int unit0 = 0;
   for (int li = 0; li < 5; li++) {
     ChainLayer &L = a.L[li];
-    const int H = e->gru[li].H, tiles = H / HT;
+    const int H = kGruH[li], tiles = H / HT;
     L.H = H; L.h_kb = H / CBK; L.tiles_log2 = __builtin_ctz(tiles);
     L.b_term_rows = tiles * GRU_BN;
     L.h_map = 1 + li; L.w_map = 6 + li; L.u_map = 11 + li;
@@ -1397,7 +1355,7 @@ static int tc_gru_chain(pnb_engine *e, int F, const int *hops, cudaStream_t st) 
 
 // The two 34-wide output layers (rnn.cpp:73-80; N padded to 48, fp16 two-term split, sigmoid epilogue).
 static int tc_out(pnb_engine *e, int F, const int *, cudaStream_t st) {
-  pnb_tc_state *t = e->tc;
+  pnb_tc_state *t = e->tc.get();
   const int S = e->S, Fm = e->Fmax;
   const float *tbl = e->tansig();
   const int h_terms = (Fm + 1) * S;
@@ -1435,7 +1393,7 @@ static int tc_out(pnb_engine *e, int F, const int *, cudaStream_t st) {
 // state parity advances by F.  A ragged call's rows that stopped early hold their fp32 state at parity par0 + hops:
 // the call's fix-up moves it (pnb_state.cu, ragged_carry_kernel).
 static int tc_carry(pnb_engine *e, int F, const int *hops, cudaStream_t st) {
-  pnb_tc_state *t = e->tc;
+  pnb_tc_state *t = e->tc.get();
   const int S = e->S, Fm = e->Fmax, na = e->n_active;
   const int h_terms = (Fm + 1) * S;
   CarryArgs ca;
@@ -1449,7 +1407,7 @@ static int tc_carry(pnb_engine *e, int F, const int *hops, cudaStream_t st) {
     ca.seg[ns++] = CarrySeg{reinterpret_cast<uint4 *>(bc), (size_t)na * 512 * 2 / 16, (size_t)S * 512 * 2 / 16, 512 * 2 / 16, 2, F};
   }
   for (int li = 0; li < 5; li++) {
-    const size_t H = e->gru[li].H;
+    const size_t H = kGruH[li];
     for (int tm = 0; tm < 2; tm++) {
       __half *base = t->h_all[li] + (size_t)tm * h_terms * H;
       ca.seg[ns++] = CarrySeg{reinterpret_cast<uint4 *>(base), (size_t)na * H * 2 / 16, (size_t)S * H * 2 / 16, H * 2 / 16, 1, F};
@@ -1474,3 +1432,5 @@ int tc_network(pnb_engine *e, int F, const int *hops, cudaStream_t st) {
   }
   return n;
 }
+
+int tc_network_launches(const pnb_engine *, int) { return 7; }  // fc, conv1, conv2, GRU chain, fc_gb, fc_rb, carry

@@ -1,6 +1,7 @@
 // pnb_state.cu -- batched per-stream state movement: the gather (export) and scatter (import, reset) kernels behind
 // pnb_export_states / pnb_import_states / pnb_reset_streams, and the one table that says where a stream's state lives
-// in an engine (state_segs).  pnb_get_state / pnb_set_state are the n = 1 case of the same kernels.  The session pool
+// in an engine (state_segs, which takes the network path's own pieces from tc_state_segs / f32_state_segs).
+// pnb_get_state / pnb_set_state are the n = 1 case of the same kernels.  The session pool
 // (pnb_process_sessions_*) parks, unparks and relocates sessions with the same pieces (session_move_kernel) and keeps
 // its parking blobs with session_blob_kernel.
 //
@@ -312,19 +313,6 @@ __global__ void state_clear_reject_kernel(int *status) {
   status[1] = kNoRejectedSlot;
 }
 
-// n 32-bit words of one field, cut into pieces of at most kStateSegMax words
-void add_words(StateSeg *seg, int &ns, short kind, void *eng, size_t eng_stride, size_t blob_off, size_t n) {
-  for (size_t k = 0; k < n; k += kStateSegMax) {
-    StateSeg &g = seg[ns++];
-    g = StateSeg();
-    g.kind = kind;
-    g.eng = eng ? static_cast<char *>(eng) + 4 * k : nullptr;
-    g.eng_stride = eng_stride;
-    g.blob_off = (unsigned)(blob_off + 4 * k);
-    g.n = (unsigned)(n - k < (size_t)kStateSegMax ? n - k : (size_t)kStateSegMax);
-  }
-}
-
 }  // namespace
 
 int state_segs(const pnb_engine *e, StateSeg *seg) {
@@ -350,19 +338,12 @@ int state_segs(const pnb_engine *e, StateSeg *seg) {
   // GRU states in fp32 (both paths), at the parity the next call starts from
   size_t off = 0;
   for (int li = 0; li < 5; li++) {
-    const size_t H = e->gru[li].H;
+    const size_t H = kGruH[li];
     add_words(seg, ns, kSegCopy, e->h[li][e->par[li]], H * 4, offsetof(StreamState, h) + off * 4, H);
     off += H;
   }
   add_words(seg, ns, kSegEngZero, e->c2, 512 * 4, 0, 512);  // the conv2 tap (PNB_TAP_NN_C2) of a fresh stream
-  if (e->flags & PNB_NN_TENSOR) return tc_state_segs(e, seg, ns);
-  // fp32 path: the conv histories at slots 0..3 / 0..1 of the hop-slot buffers (nn_chunk_f32's carry)
-  for (int k = 0; k < 4; k++)
-    add_words(seg, ns, kSegCopy, e->ring_fc + (size_t)k * S * 128, 128 * 4, offsetof(StreamState, fc_hist) + (size_t)k * 128 * 4, 128);
-  for (int k = 0; k < 2; k++)
-    add_words(seg, ns, kSegCopy, e->ring_c1 + (size_t)k * S * 512, 512 * 4, offsetof(StreamState, c1_hist) + (size_t)k * 512 * 4, 512);
-  add_words(seg, ns, kSegBlobZero, nullptr, 0, offsetof(StreamState, fc_terms), (sizeof(StreamState) - offsetof(StreamState, fc_terms)) / 4);
-  return ns;
+  return (e->flags & PNB_NN_TENSOR) ? tc_state_segs(e, seg, ns) : f32_state_segs(e, seg, ns);
 }
 
 int launch_state_check(const StateArgs &a, cudaStream_t st) {
@@ -399,7 +380,7 @@ int launch_ragged_carry(const pnb_engine *e, int F, const int *d_hops, const int
   if (e->flags & PNB_NN_TENSOR) {
     a.n_gru = 5;
     for (int li = 0; li < 5; li++) {
-      a.h[li][0] = e->h[li][0]; a.h[li][1] = e->h[li][1]; a.H[li] = e->gru[li].H; a.par[li] = e->par[li];
+      a.h[li][0] = e->h[li][0]; a.h[li][1] = e->h[li][1]; a.H[li] = kGruH[li]; a.par[li] = e->par[li];
     }
   }
   a.hops = d_hops; a.slots = d_slots;

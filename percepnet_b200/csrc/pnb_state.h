@@ -63,6 +63,19 @@ struct StateSeg {
 constexpr int kMaxStateSegs = 72;  // a tensor-mode engine needs 69
 constexpr int kStateSegMax = 512;  // words / elements per piece: long fields are cut into pieces of at most this
 
+// Appends the pieces of n 32-bit words of one field, cut into pieces of at most kStateSegMax words
+inline void add_words(StateSeg *seg, int &ns, short kind, void *eng, size_t eng_stride, size_t blob_off, size_t n) {
+  for (size_t k = 0; k < n; k += kStateSegMax) {
+    StateSeg &g = seg[ns++];
+    g = StateSeg();
+    g.kind = kind;
+    g.eng = eng ? static_cast<char *>(eng) + 4 * k : nullptr;
+    g.eng_stride = eng_stride;
+    g.blob_off = (unsigned)(blob_off + 4 * k);
+    g.n = (unsigned)(n - k < (size_t)kStateSegMax ? n - k : (size_t)kStateSegMax);
+  }
+}
+
 enum StateMode { kStateExport = 0, kStateImport = 1, kStateReset = 2 };
 struct StateArgs {
   StateSeg seg[kMaxStateSegs];

@@ -1,6 +1,6 @@
 """The persistent GRU chain kernels walk their units in an order in which everything a unit waits for has a smaller
 index (round-robin over co-resident blocks then cannot deadlock).  This restates the two orders the kernels use --
-hop-major and anti-diagonal (pnb_nn_tc.cu decode_unit / decode_unit_diag, pnb_engine.cu nn_chunk_f32's table) -- and checks
+hop-major and anti-diagonal (pnb_nn_tc.cu decode_unit / decode_unit_diag, pnb_nn_f32.cu run_chunk's table) -- and checks
 the property, the coverage (every unit exactly once) and the closed-form decode against the table."""
 import itertools
 
@@ -10,7 +10,7 @@ DEPTH = (0, 1, 2, 3, 3)          # gru1, gru2, gru3, gru_gb, gru_rb (gru_rb read
 DEP = (-1, 0, 1, 2, 2)           # layer whose fresh state is a layer's input (-1: conv2 output, ready before the launch)
 
 
-def diag_table(n_hops, units):   # nn_chunk_f32: entries (t, l) sorted by diagonal, then layer
+def diag_table(n_hops, units):   # run_chunk: entries (t, l) sorted by diagonal, then layer
     order = []
     for d in range(n_hops + 3):
         for l in range(5):

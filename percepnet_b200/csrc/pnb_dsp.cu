@@ -58,16 +58,16 @@ struct FftTw {            // per-block tables in shared memory
 //           through shared memory), does radix-4 m=1 and radix-4 m=4 in registers, stores 128 contiguous bytes
 //   pass B: radix-4 m=16 then radix-3 m=64 on the 12 elements {192 n0 + 64 r + 16 q + j}
 //   pass C: radix-5 m=192
-// L lanes (32 or 16) cooperate on one transform; `mask` names them, `lane` is the index within the group.
-template <bool kAllOutputs, int L, class Load>
-__device__ __forceinline__ void fft960_warp(float2 *f, const FftTw &T, int lane, unsigned mask, Load load) {
-  __syncwarp(mask);
+// The 32 lanes of a warp cooperate on one transform.
+template <bool kAllOutputs, class Load>
+__device__ __forceinline__ void fft960_warp(float2 *f, const FftTw &T, int lane, Load load) {
+  __syncwarp();
   {  // ---------------- pass A ----------------
     const float2 t1a = T.tw[60], t1b = T.tw[120], t1c = T.tw[180];    // j = 1: tw[60 j], tw[120 j], tw[180 j]
     const float2 t2a = T.tw[120], t2b = T.tw[240], t2c = T.tw[360];   // j = 2
     const float2 t3a = T.tw[180], t3b = T.tw[360], t3c = T.tw[540];   // j = 3
     const float2 t0 = T.tw[0];
-    for (int b = lane; b < 60; b += L) {
+    for (int b = lane; b < 60; b += 32) {
       const int n0 = b / 12, n1 = (b >> 2) % 3, n2 = b & 3;
       const int ibase = n0 + 5 * n1 + 15 * n2;
       float2 v[16];
@@ -109,10 +109,10 @@ __device__ __forceinline__ void fft960_warp(float2 *f, const FftTw &T, int lane,
       for (int k = 0; k < 8; k++) dst[k] = make_float4(v[2 * k].x, v[2 * k].y, v[2 * k + 1].x, v[2 * k + 1].y);
     }
   }
-  __syncwarp(mask);
+  __syncwarp();
   {  // ---------------- pass B ----------------
     const float w3i = T.tw[320].y;  // epi3, kiss_fft.cpp:194
-    for (int g = lane; g < 80; g += L) {
+    for (int g = lane; g < 80; g += 32) {
       const int n0 = g >> 4, jj = g & 15;
       const int e0 = 192 * n0 + jj;
       float2 v[3][4];
@@ -153,10 +153,10 @@ __device__ __forceinline__ void fft960_warp(float2 *f, const FftTw &T, int lane,
         for (int q = 0; q < 4; q++) f[fpos(e0 + 64 * r + 16 * q)] = v[r][q];
     }
   }
-  __syncwarp(mask);
+  __syncwarp();
   {  // ---------------- pass C: radix-5, m = 192 (kiss_fft.cpp:232-305); ya = tw[192], yb = tw[384] ----------------
     const float2 ya = T.tw[192], yb = T.tw[384];
-    for (int u = lane; u < 192; u += L) {
+    for (int u = lane; u < 192; u += 32) {
       float2 z0 = f[fpos(u)];
       float2 z1 = cmul(f[fpos(u + 192)], T.tw5[0][u]);
       float2 z2 = cmul(f[fpos(u + 384)], T.tw5[1][u]);
@@ -175,7 +175,7 @@ __device__ __forceinline__ void fft960_warp(float2 *f, const FftTw &T, int lane,
       if (kAllOutputs) f[fpos(u + 576)] = csub(p, q);
     }
   }
-  __syncwarp(mask);
+  __syncwarp();
 }
 
 // ERB band pooling (denoise.cpp:89-123 / 125-160): v[bin] is |X|^2 or Re(X conj P) for bins 0..399.
@@ -206,23 +206,19 @@ __device__ __forceinline__ void band_acc(int b, const float *vf, const float *vo
   out[b] = acc;
   if (kDual) out2[b] = acc2;
 }
-template <int L, bool kDual = false>
+template <bool kDual = false>
 __device__ void band_pool_warp(const float *vf, const float *vo, float *out, const short *border, int lane,
-                               unsigned mask, const float *vf2 = nullptr, const float *vo2 = nullptr,
-                               float *out2 = nullptr) {
+                               const float *vf2 = nullptr, const float *vo2 = nullptr, float *out2 = nullptr) {
   // vf[k] = frac[k] * v[k] and vo[k] = (1 - frac[k]) * v[k] were formed by the caller (the very products the
   // reference adds, denoise.cpp:102-103), so the serial part is one load and one add per bin.
-  // Accumulators 32 and 33 are the longest chains (96 and 51 adds) and 0 and 1 the shortest (2 and 4): with a
-  // warp per stream, lane j takes accumulator j+2 and lanes 0/1 then add the two short ones, so the critical
-  // path is one long chain instead of two.
-  __syncwarp(mask);
-  if (L == 32) {
-    band_acc<kDual>(lane + 2, vf, vo, out, vf2, vo2, out2, border);
-    if (lane < 2) band_acc<kDual>(lane, vf, vo, out, vf2, vo2, out2, border);
-  } else {
-    for (int b = lane; b < kBands; b += L) band_acc<kDual>(b, vf, vo, out, vf2, vo2, out2, border);
-  }
-  __syncwarp(mask);
+  // Accumulators 32 and 33 are the longest chains (96 and 51 adds) and 0 and 1 the shortest (2 and 4): lane j
+  // takes accumulator j+2 and lanes 0/1 then add the two short ones, so the critical path is one long chain
+  // instead of two.
+  static_assert(kBands == 34, "one accumulator per lane plus two short ones on lanes 0 and 1");
+  __syncwarp();
+  band_acc<kDual>(lane + 2, vf, vo, out, vf2, vo2, out2, border);
+  if (lane < 2) band_acc<kDual>(lane, vf, vo, out, vf2, vo2, out2, border);
+  __syncwarp();
 }
 
 // Sequential dot product s + sum_j a[j] b[j] (ascending j, multiply then add -- the reference's order) with the
@@ -276,22 +272,22 @@ __device__ __forceinline__ void energy_chain(float *d, int n4, float syy) {
   }
 }
 
-// lanes hold candidates in ascending lag order (lane order); wlane = lane id within the warp
-__device__ __forceinline__ void best2_rounds(Best2 &S, bool alive, float num, float e, int idx, unsigned mask, int wlane) {
+// lanes hold candidates in ascending lag order (lane order)
+__device__ __forceinline__ void best2_rounds(Best2 &S, bool alive, float num, float e, int idx, int lane) {
   while (true) {
     const bool pass = alive && (num * S.den1 > S.num1 * e);
-    const unsigned m = __ballot_sync(mask, pass);
+    const unsigned m = __ballot_sync(0xffffffffu, pass);
     if (!m) break;
     const int f = __ffs(m) - 1;
-    const float nf = __shfl_sync(mask, num, f), ef = __shfl_sync(mask, e, f);
-    const int jf = __shfl_sync(mask, idx, f);
+    const float nf = __shfl_sync(0xffffffffu, num, f), ef = __shfl_sync(0xffffffffu, e, f);
+    const int jf = __shfl_sync(0xffffffffu, idx, f);
     if (nf * S.den0 > S.num0 * ef) {
       S.num1 = S.num0; S.den1 = S.den0; S.b1 = S.b0;
       S.num0 = nf; S.den0 = ef; S.b0 = jf;
     } else {
       S.num1 = nf; S.den1 = ef; S.b1 = jf;
     }
-    alive = alive && (wlane > f);
+    alive = alive && (lane > f);
   }
 }
 
@@ -328,18 +324,6 @@ struct BlockSmem {
   float comb_w[8];
 };
 
-// One stream is owned by a group of L lanes: L = 32 (a warp per stream) or L = 16 (two streams per warp).  The
-// serial stretches of the pitch analysis keep only a handful of lanes busy, so with L = 16 every such instruction
-// (and shared-memory wavefront) serves two streams.
-template <int L>
-struct AnaCfg {
-  static constexpr int kStreamsPerWarp = 32 / L;
-  static constexpr int kWarps = (L == 32) ? 8 : 4;             // 8 streams per block either way
-  static constexpr int kStreamsPerBlock = kWarps * kStreamsPerWarp;
-  static constexpr int kLagsPerLane = (L == 32) ? 5 : 10;       // coarse search: adjacent lags per lane
-  static constexpr int kLagLanes = (L == 32) ? 30 : 15;         // lanes that own lags; the next lane accumulates Syy
-};
-
 // Per-section cycle accounting of the analysis kernel (debug builds only: -DPNB_ANA_TIMING).  Lane 0 of every
 // warp samples clock64() at the section boundaries and the deltas are summed into g_ana_cycles.
 #ifdef PNB_ANA_TIMING
@@ -371,19 +355,18 @@ struct PitchResult {
 #define ANA_TIMER_PARAMS
 #define ANA_TIMER_ARGS
 #endif
-template <int L, bool kInlineAc = false>
+template <bool kInlineAc = false>
 __device__ __forceinline__ PitchResult pitch_stage(WarpSmem &W, const float *src, const float *acp, int last_period,
-                                                   float last_gain, int lane, int wlane, unsigned mask ANA_TIMER_PARAMS) {
-  using CF = AnaCfg<L>;
+                                                   float last_gain, int lane ANA_TIMER_PARAMS) {
   // ---- pitch_downsample (pitch.cpp:148-216) ----
   {
-    for (int i = lane; i < kLp; i += L) {
+    for (int i = lane; i < kLp; i += 32) {
       float v;
       if (i == 0) v = .5f * (.5f * src[1] + src[0]);
       else v = .5f * (.5f * (src[2 * i - 1] + src[2 * i + 1]) + src[2 * i]);
       W.p.lp[i] = v;
     }
-    __syncwarp(mask);
+    __syncwarp();
     ANA_TICK(2);
     // autocorrelation, 5 lags (celt_lpc.cpp:198-279): the analysis kernel computes them for a whole group of hops in
     // its pre-pass; a caller without one (kInlineAc) has lane k run the strictly sequential sum of lag k here
@@ -395,7 +378,7 @@ __device__ __forceinline__ PitchResult pitch_stage(WarpSmem &W, const float *src
         for (int i = lane + 860; i < kLp; i++) d = d + lp[i] * lp[i - lane];  // the tail, summed apart (:253-256)
         W.ac_pre[lane] = a + d;
       }
-      __syncwarp(mask);
+      __syncwarp();
       acp = W.ac_pre;
     }
     const float ac0 = acp[0], ac1 = acp[1], ac2 = acp[2], ac3 = acp[3], ac4 = acp[4];
@@ -431,15 +414,16 @@ __device__ __forceinline__ PitchResult pitch_stage(WarpSmem &W, const float *src
       fir3 = lpc[3] + .8f * lpc[2];
       fir4 = .8f * lpc[3];
     }
-    fir0 = __shfl_sync(mask, fir0, 0, L);
-    fir1 = __shfl_sync(mask, fir1, 0, L);
-    fir2 = __shfl_sync(mask, fir2, 0, L);
-    fir3 = __shfl_sync(mask, fir3, 0, L);
-    fir4 = __shfl_sync(mask, fir4, 0, L);
+    fir0 = __shfl_sync(0xffffffffu, fir0, 0);
+    fir1 = __shfl_sync(0xffffffffu, fir1, 0);
+    fir2 = __shfl_sync(0xffffffffu, fir2, 0);
+    fir3 = __shfl_sync(0xffffffffu, fir3, 0);
+    fir4 = __shfl_sync(0xffffffffu, fir4, 0);
     ANA_TICK(4);
     // 5-tap FIR in place with zero history (pitch.cpp:106-145,154), walked from the end so the taps
     // still see unfiltered samples
-    for (int base = kLp - L; base >= 0; base -= L) {
+    static_assert(kLp % 32 == 0, "the FIR walk covers [0, kLp) in whole warps");
+    for (int base = kLp - 32; base >= 0; base -= 32) {
       int i = base + lane;
       float x0 = W.p.lp[i];
       float m0 = i >= 1 ? W.p.lp[i - 1] : 0.f, m1 = i >= 2 ? W.p.lp[i - 2] : 0.f, m2 = i >= 3 ? W.p.lp[i - 3] : 0.f,
@@ -450,10 +434,10 @@ __device__ __forceinline__ PitchResult pitch_stage(WarpSmem &W, const float *src
       sum = sum + fir2 * m2;
       sum = sum + fir3 * m3;
       sum = sum + fir4 * m4;
-      __syncwarp(mask);
+      __syncwarp();
       W.p.lp[i] = sum;
       W.p.sq[i] = sum * sum;
-      __syncwarp(mask);
+      __syncwarp();
     }
   }
 
@@ -468,10 +452,13 @@ __device__ __forceinline__ PitchResult pitch_stage(WarpSmem &W, const float *src
     // j exactly like the reference (pitch.cpp:218-281).  The lane after the lag lanes accumulates the energy
     // Syy = 1 + sum y4[j]^2 of find_best_pitch (pitch.cpp:54,69-70) through the same code shape (lag 0 of y on y).
     {
-      constexpr int NL = CF::kLagsPerLane;
-      const bool syy_lane = (lane == CF::kLagLanes);
+      constexpr int NL = 5;          // adjacent lags per lag lane
+      constexpr int kLagLanes = 30;  // lanes that own lags
+      static_assert(kLagLanes * NL >= 147, "the lag lanes cover every coarse lag");
+      static_assert(kLagLanes < 32, "the lane after the lag lanes accumulates Syy");
+      const bool syy_lane = (lane == kLagLanes);
       const float *xb = syy_lane ? W.p.lp : W.p.lp + 384;
-      const int L0 = (lane < CF::kLagLanes) ? NL * lane : 0;
+      const int L0 = (lane < kLagLanes) ? NL * lane : 0;
       const float *yb = W.p.lp + 2 * L0;
       float acc[NL], w[NL];
 #pragma unroll
@@ -486,41 +473,41 @@ __device__ __forceinline__ PitchResult pitch_stage(WarpSmem &W, const float *src
           w[u] = yb[2 * (j + u + NL)];
         }
       }
-      if (lane < CF::kLagLanes) {
+      if (lane < kLagLanes) {
 #pragma unroll
         for (int q = 0; q < NL; q++)
           if (L0 + q < 147) W.xc[L0 + q] = acc[q];
       }
       // energy deltas of the coarse scan: y4[i+240]^2 - y4[i]^2 (pitch.cpp:101)
-      for (int i = lane; i < 147; i += L) {
+      for (int i = lane; i < 147; i += 32) {
         W.p.yy[i] = W.p.sq[2 * (i + 240)] - W.p.sq[2 * i];
       }
-      float syy_c = __shfl_sync(mask, acc[0], CF::kLagLanes, L);
-      __syncwarp(mask);
+      float syy_c = __shfl_sync(0xffffffffu, acc[0], kLagLanes);
+      __syncwarp();
       ANA_TICK(6);
       if (lane == 0) energy_chain(W.p.yy, 148, syy_c);
-      __syncwarp(mask);
+      __syncwarp();
       {
         Best2 S = best2_init();
-        for (int base = 0; base < 147; base += L) {
+        for (int base = 0; base < 147; base += 32) {
           const int i = base + lane;
           const bool valid = i < 147;
           const float xv = valid ? W.xc[i] : 0.f, ev = valid ? W.p.yy[i] : 1.f;
           const float c = xv * 1e-12f;
-          best2_rounds(S, valid && xv > 0.f, c * c, ev, i, mask, wlane);
+          best2_rounds(S, valid && xv > 0.f, c * c, ev, i, lane);
         }
         b0 = S.b0; b1 = S.b1;
       }
-      __syncwarp(mask);
+      __syncwarp();
       ANA_TICK(7);
     }
     // fine: at most ten lags around 2*b0 and 2*b1 (pitch.cpp:344-361); lane 10 accumulates Syy of the
     // second find_best_pitch, lane 11 the xx of remove_doubling (pitch.cpp:448)
-    for (int i = lane; i < 294; i += L) {
+    for (int i = lane; i < 294; i += 32) {
       W.xc[i] = 0.f;
       W.p.yy[i] = W.p.sq[i + 480] - W.p.sq[i];  // energy deltas of the fine scan
     }
-    __syncwarp(mask);
+    __syncwarp();
     int fl = -1;
     if (lane < 5) fl = 2 * b0 - 2 + lane;
     else if (lane < 10) fl = 2 * b1 - 2 + (lane - 5);
@@ -536,9 +523,9 @@ __device__ __forceinline__ PitchResult pitch_stage(WarpSmem &W, const float *src
       if (n) sacc = seq_dot4(a, b, 480, sacc);
     }
     if (fine_ok) W.xc[fl] = (-1.f > sacc) ? -1.f : sacc;
-    float syy_f = __shfl_sync(mask, sacc, 10, L);
-    float xx = __shfl_sync(mask, sacc, 11, L);
-    __syncwarp(mask);
+    float syy_f = __shfl_sync(0xffffffffu, sacc, 10);
+    float xx = __shfl_sync(0xffffffffu, sacc, 11);
+    __syncwarp();
     ANA_TICK(8);
     int off = 0;
     float corr = 0.f;
@@ -561,13 +548,13 @@ __device__ __forceinline__ PitchResult pitch_stage(WarpSmem &W, const float *src
       hiB = hiB < loB ? loB : hiB;
       hiB = hiB > 294 ? 294 : hiB;
       if (lane == 0) energy_chain(W.p.yy, (hiB + 3) & ~3, syy_f);
-      __syncwarp(mask);
+      __syncwarp();
       const int idx = lane < 5 ? loA + lane : loB + (lane - 5);
       const bool valid = lane < 5 ? idx < hiA : (lane < 10 && idx < hiB);
       const float xv = valid ? W.xc[idx] : 0.f, ev = valid ? W.p.yy[idx] : 1.f;
       const float c = xv * 1e-12f;
       Best2 S = best2_init();
-      best2_rounds(S, valid && xv > 0.f, c * c, ev, idx, mask, wlane);
+      best2_rounds(S, valid && xv > 0.f, c * c, ev, idx, lane);
       c0 = S.b0;
     }
     if (lane == 0) {
@@ -579,9 +566,9 @@ __device__ __forceinline__ PitchResult pitch_stage(WarpSmem &W, const float *src
       pitch_lag = 2 * c0 - off;
       corr = W.xc[c0];
     }
-    pitch_lag = __shfl_sync(mask, pitch_lag, 0, L);
-    pitch_corr = __shfl_sync(mask, corr, 0, L);
-    __syncwarp(mask);  // the scan's energy deltas in W.p.yy are dead; the yy table is built next
+    pitch_lag = __shfl_sync(0xffffffffu, pitch_lag, 0);
+    pitch_corr = __shfl_sync(0xffffffffu, corr, 0);
+    __syncwarp();  // the scan's energy deltas in W.p.yy are dead; the yy table is built next
     ANA_TICK(9);
 
     // ---- remove_doubling (pitch.cpp:423-527) with maxperiod 384, minperiod 30, N 480 ----
@@ -593,9 +580,8 @@ __device__ __forceinline__ PitchResult pitch_stage(WarpSmem &W, const float *src
     // 32 roles: 0: xy at T0; 1: the yy_lookup recurrence; 2..29: candidate (k, which) = (2 + (role-2)/2, (role-2)&1);
     // 30, 31: xy at T0-1 and T0+1, the neighbours the final refinement needs when no sub-harmonic replaces T0
     // (the usual outcome) -- they ride along in lanes that would idle, and the extra pass below is skipped
-#pragma unroll 1
-    for (int rbase = 0; rbase < 32; rbase += L) {
-      const int role = rbase + lane;
+    {
+      const int role = lane;
       int lag = -1;
       if (role == 0) lag = T0;
       else if (role == 30) lag = T0 - 1;
@@ -610,10 +596,10 @@ __device__ __forceinline__ PitchResult pitch_stage(WarpSmem &W, const float *src
         }
       }
       // all lanes meet here before the 480-step loops: without it the lanes whose lag needed no division run the
-      // dot loop ahead of the candidate lanes and the loop is executed once per group
-      __syncwarp(mask);
+      // dot loop ahead of the candidate lanes and the loop is executed once per diverged set of lanes
+      __syncwarp();
       // the energy table is read only at the lags of roles 0 and 2..29 (T0, T1, T1b): the recurrence stops there
-      const int max_lag = (L == 32) ? __reduce_max_sync(mask, role < 30 ? lag : -1) : 384;  // (all roles in one pass)
+      const int max_lag = __reduce_max_sync(0xffffffffu, role < 30 ? lag : -1);
       if (role == 1) {
         // yy_lookup recurrence (pitch.cpp:449-455), strictly sequential; operands fetched four at a time.
         // Table entry i is stored at W.p.yy[i + 3] so that groups of four are 16-byte aligned.
@@ -635,7 +621,7 @@ __device__ __forceinline__ PitchResult pitch_stage(WarpSmem &W, const float *src
         W.p.cand_xy[role] = d;
       }
     }
-    __syncwarp(mask);
+    __syncwarp();
     ANA_TICK(10);
     int Tsel = T0;
     float g = 0.f, best_xy = 0.f, best_yy = 0.f;
@@ -671,7 +657,7 @@ __device__ __forceinline__ PitchResult pitch_stage(WarpSmem &W, const float *src
         if (g1 > thresh) { best_xy = xy; best_yy = yy; Tsel = T1; g = g1; }
       }
     }
-    Tsel = __shfl_sync(mask, Tsel, 0, L);
+    Tsel = __shfl_sync(0xffffffffu, Tsel, 0);
     ANA_TICK(11);
     // final +-1 refinement: three dot products around the selected period (pitch.cpp:512-513)
     {
@@ -681,7 +667,7 @@ __device__ __forceinline__ PitchResult pitch_stage(WarpSmem &W, const float *src
       } else {
         float d = 0.f;
         if (lane < 3) d = seq_dot4(x, x - (Tsel + lane - 1), 480, 0.f);
-        x0 = __shfl_sync(mask, d, 0, L); x1 = __shfl_sync(mask, d, 1, L); x2 = __shfl_sync(mask, d, 2, L);
+        x0 = __shfl_sync(0xffffffffu, d, 0); x1 = __shfl_sync(0xffffffffu, d, 1); x2 = __shfl_sync(0xffffffffu, d, 2);
       }
       int Tout = 0;
       float pg = 0.f;
@@ -697,8 +683,8 @@ __device__ __forceinline__ PitchResult pitch_stage(WarpSmem &W, const float *src
         Tout = 2 * Tsel + o2;
         if (Tout < kMinPeriod) Tout = kMinPeriod;
       }
-      T = __shfl_sync(mask, Tout, 0, L);
-      gain = __shfl_sync(mask, pg, 0, L);
+      T = __shfl_sync(0xffffffffu, Tout, 0);
+      gain = __shfl_sync(0xffffffffu, pg, 0);
     }
     ANA_TICK(12);
   }
@@ -707,15 +693,13 @@ __device__ __forceinline__ PitchResult pitch_stage(WarpSmem &W, const float *src
   return res;
 }
 
-template <int L>
-__global__ void __launch_bounds__(AnaCfg<L>::kWarps * 32) analysis_kernel(AnalysisArgs A) {
-  using CF = AnaCfg<L>;
+constexpr int kAnaWarps = 8;  // one stream per warp
+
+__global__ void __launch_bounds__(kAnaWarps * 32) analysis_kernel(AnalysisArgs A) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   BlockSmem &B = *reinterpret_cast<BlockSmem *>(smem_raw);
   WarpSmem *Wall = reinterpret_cast<WarpSmem *>(smem_raw + ((sizeof(BlockSmem) + 15) / 16) * 16);
-  const int wlane = threadIdx.x & 31, wib = threadIdx.x >> 5;
-  const int lane = wlane % L, sub = wlane / L;  // lane within the stream's group, group within the warp
-  const unsigned mask = (L == 32) ? 0xffffffffu : (0xffffu << (16 * sub));
+  const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
   const Tables *T = A.tab;
   for (int i = threadIdx.x; i < kWin; i += blockDim.x) B.ft.tw[i] = T->tw[i];
   for (int i = threadIdx.x; i < 4 * 192; i += blockDim.x) B.ft.tw5[i / 192][i % 192] = T->tw[(i / 192 + 1) * (i % 192)];
@@ -725,16 +709,15 @@ __global__ void __launch_bounds__(AnaCfg<L>::kWarps * 32) analysis_kernel(Analys
   if (threadIdx.x < 8) B.comb_w[threadIdx.x] = T->comb_w[threadIdx.x];
   __syncthreads();
 
-  const int sl = wib * CF::kStreamsPerWarp + sub;  // stream slot within the block
-  const int s = blockIdx.x * CF::kStreamsPerBlock + sl;
+  const int s = blockIdx.x * kAnaWarps + wib;
   if (s >= A.n_streams) return;
-  WarpSmem &W = Wall[sl];
+  WarpSmem &W = Wall[wib];
   float *xo = reinterpret_cast<float *>(&W.fft[448]);
   const float *row = A.pcm + (size_t)s * A.pcm_stride;
   int last_period = A.last_period[s];
   float last_gain = A.last_gain[s];
-  // a ragged call's slot walks its own hops: with two streams per warp the lane groups then run different trip counts,
-  // which is safe because every barrier and shuffle inside the hop loop is masked to the group
+  // a ragged call's slot walks its own hops: the trip count is uniform across the warp because the warp owns one
+  // stream, so every full-warp barrier and shuffle in the hop loop is reached by all 32 lanes
   const int n_frames = A.hops ? A.hops[s] : A.n_frames;
 
 #ifdef PNB_ANA_TIMING
@@ -757,8 +740,8 @@ __global__ void __launch_bounds__(AnaCfg<L>::kWarps * 32) analysis_kernel(Analys
       float *D = reinterpret_cast<float *>(W.fft);
       const float *src = line + kOffPitch;
       const int nD = kLp + 240 * (G - 1);
-      for (int i = lane; i < nD; i += L) D[i] = .5f * (.5f * (src[2 * i - 1] + src[2 * i + 1]) + src[2 * i]);
-      __syncwarp(mask);
+      for (int i = lane; i < nD; i += 32) D[i] = .5f * (.5f * (src[2 * i - 1] + src[2 * i + 1]) + src[2 * i]);
+      __syncwarp();
       if (lane < G) {
         const float *Dh = D + 240 * lane, *sh = src + kFrame * lane;
         float4 c = *reinterpret_cast<const float4 *>(Dh), n = *reinterpret_cast<const float4 *>(Dh + 4);
@@ -785,7 +768,7 @@ __global__ void __launch_bounds__(AnaCfg<L>::kWarps * 32) analysis_kernel(Analys
         float *o = W.ac_pre + 5 * lane;
         o[0] = a0 + d0; o[1] = a1 + d1; o[2] = a2 + d2; o[3] = a3 + d3; o[4] = a4 + 0.f;
       }
-      __syncwarp(mask);
+      __syncwarp();
     }
 
     // ---- one transform per hop.  The look-ahead window of hop c (denoise.cpp:498-506: the newest 960
@@ -798,7 +781,7 @@ __global__ void __launch_bounds__(AnaCfg<L>::kWarps * 32) analysis_kernel(Analys
       const float *src = line + kOffLook;
       const float *hw = B.hw;
       // window (denoise.cpp:282-289), real -> complex, 1/960 (kiss_fft.cpp:582-583)
-      fft960_warp<false, L>(W.fft, B.ft, lane, mask, [&](int i) {
+      fft960_warp<false>(W.fft, B.ft, lane, [&](int i) {
         float w = hw[i < kFrame ? i : kWin - 1 - i];
         float v = src[i] * w;
         return make_float2((1.f / kWin) * v, 0.f);
@@ -807,7 +790,7 @@ __global__ void __launch_bounds__(AnaCfg<L>::kWarps * 32) analysis_kernel(Analys
     ANA_TICK(0);
     {
       float2 *Zg = A.zring + ((size_t)slot_new * A.stride + s) * kBins;
-      for (int k = lane; k < kBins; k += L) {
+      for (int k = lane; k < kBins; k += 32) {
         float2 x = W.fft[fpos(k)];
         Zg[k] = x;
         float e = x.x * x.x;
@@ -815,33 +798,33 @@ __global__ void __launch_bounds__(AnaCfg<L>::kWarps * 32) analysis_kernel(Analys
         W.xc[k] = B.frac[k] * e;
         xo[k] = B.omf[k] * e;
       }
-      band_pool_warp<L>(W.xc, xo, W.Ey, B.border, lane, mask);
+      band_pool_warp(W.xc, xo, W.Ey, B.border, lane);
       float *Eg = A.ering + ((size_t)slot_new * A.stride + s) * kBands;
       const float *Eo = A.ering + ((size_t)slot_x * A.stride + s) * kBands;
-      for (int b = lane; b < kBands; b += L) {
+      for (int b = lane; b < kBands; b += 32) {
         Eg[b] = W.Ey[b];
-        W.Ex[b] = Eo[b];  // written five hops ago (by this lane group, or by the previous call)
+        W.Ex[b] = Eo[b];  // written five hops ago (by this lane, or by the previous call)
       }
     }
     const float2 *Xg = A.zring + ((size_t)slot_x * A.stride + s) * kBins;
-    __syncwarp(mask);
+    __syncwarp();
     ANA_TICK(1);
 
     // ---- pitch_downsample, pitch_search, remove_doubling (pitch.cpp:148-216, 283-386, 423-527) ----
-    const PitchResult pr = pitch_stage<L>(W, line + kOffPitch, W.ac_pre + 5 * (t % kAcHops), last_period, last_gain, lane,
-                                          wlane, mask ANA_TIMER_ARGS);
+    const PitchResult pr =
+        pitch_stage(W, line + kOffPitch, W.ac_pre + 5 * (t % kAcHops), last_period, last_gain, lane ANA_TIMER_ARGS);
     const int pitch_lag = pr.pitch_lag, T = pr.T;
     const float pitch_corr = pr.pitch_corr, gain = pr.gain;
     last_period = T;
     last_gain = gain;
 
     // ---- comb-filtered block, its spectrum P and the band statistics (denoise.cpp:416-427) ----
-    __syncwarp(mask);  // the pitch scratch is dead from here on; its storage becomes the FFT line again
+    __syncwarp();  // the pitch scratch is dead from here on; its storage becomes the FFT line again
     {
       const float *hw = B.hw;
       const float *cw = B.comb_w;
       const float *ctr = line + kOffAnalysis;
-      fft960_warp<false, L>(W.fft, B.ft, lane, mask, [&](int i) {
+      fft960_warp<false>(W.fft, B.ft, lane, [&](int i) {
         float p = 0.f;
 #pragma unroll
         for (int k = -3; k <= 3; k++) p = p + ctr[i - T * k] * cw[k + 3];
@@ -851,7 +834,7 @@ __global__ void __launch_bounds__(AnaCfg<L>::kWarps * 32) analysis_kernel(Analys
       });
       ANA_TICK(13);
       float2 *Pg = A.P ? A.P + fs * kBins : nullptr;
-      for (int k = lane; k < kBins; k += L) {
+      for (int k = lane; k < kBins; k += 32) {
         float2 p = W.fft[fpos(k)], x = Xg[k];
         if (Pg) Pg[k] = p;
         float e = p.x * p.x;
@@ -864,14 +847,14 @@ __global__ void __launch_bounds__(AnaCfg<L>::kWarps * 32) analysis_kernel(Analys
         xo[kBins + k] = fr * c;       // the line's tail (fft[448..1080)) holds three 400-float arrays
         xo[2 * kBins + k] = om * c;
       }
-      band_pool_warp<L, true>(W.xc, xo, W.Ep, B.border, lane, mask, xo + kBins, xo + 2 * kBins, W.Exp);
+      band_pool_warp<true>(W.xc, xo, W.Ep, B.border, lane, xo + kBins, xo + 2 * kBins, W.Exp);
     }
 
     ANA_TICK(14);
     // ---- features (denoise.cpp:427-433, 487-496, 528-530) ----
     {
       float *F = A.feat + fs * kFeat;
-      for (int b = lane; b < kBands; b += L) {
+      for (int b = lane; b < kBands; b += 32) {
         float prod = W.Ex[b] * W.Ep[b];                       // float product, then double (H4)
         double v = (double)W.Exp[b] / sqrt(1e-15 + (double)prod);
         v = fmax(0.0, v);
@@ -897,9 +880,9 @@ __global__ void __launch_bounds__(AnaCfg<L>::kWarps * 32) analysis_kernel(Analys
           A.tap_pitchf[fs * 2 + 1] = gain;
         }
       }
-      if (A.Ex) for (int b = lane; b < kBands; b += L) A.Ex[fs * kBands + b] = W.Ex[b];
+      if (A.Ex) for (int b = lane; b < kBands; b += 32) A.Ex[fs * kBands + b] = W.Ex[b];
     }
-    __syncwarp(mask);
+    __syncwarp();
     ANA_TICK(15);
   }
 #ifdef PNB_ANA_TIMING
@@ -992,7 +975,7 @@ __global__ void __launch_bounds__(kSynWarps * 32) synthesis_kernel(SynthesisArgs
       const float *frac = B.frac, *omf = B.omf;
       const short *band_of = B.band_of;
       const float *gg = W.g, *rr = W.r, *ir = W.ir;
-      fft960_warp<true, 32>(W.fft, B.ft, lane, 0xffffffffu, [&](int i) {
+      fft960_warp<true>(W.fft, B.ft, lane, [&](int i) {
         int k = i <= kFrame ? i : kWin - i;
         float2 v = make_float2(0.f, 0.f);
         if (k < kBins) {
@@ -1097,8 +1080,8 @@ __global__ void __launch_bounds__(kPitchWarps * 32) pitch_only_kernel(PitchOnlyA
   unsigned long long ana_acc[16];
   long long ana_t0 = clock64();
 #endif
-  const PitchResult r = pitch_stage<32, true>(W, A.buf + (size_t)s * A.stride, nullptr, A.prev_period ? A.prev_period[s] : 0,
-                                              A.prev_gain ? A.prev_gain[s] : 0.f, lane, lane, 0xffffffffu ANA_TIMER_ARGS);
+  const PitchResult r = pitch_stage<true>(W, A.buf + (size_t)s * A.stride, nullptr, A.prev_period ? A.prev_period[s] : 0,
+                                          A.prev_gain ? A.prev_gain[s] : 0.f, lane ANA_TIMER_ARGS);
   if (lane == 0) {
     A.T[s] = r.T;
     A.gain[s] = r.gain;
@@ -1108,24 +1091,20 @@ __global__ void __launch_bounds__(kPitchWarps * 32) pitch_only_kernel(PitchOnlyA
 }
 
 // ---------------------------------------------------------------------------------- launchers
-template <int L>
-static size_t analysis_smem_bytes() {
-  return ((sizeof(BlockSmem) + 15) / 16) * 16 + AnaCfg<L>::kStreamsPerBlock * sizeof(WarpSmem);
-}
+static size_t analysis_smem_bytes() { return ((sizeof(BlockSmem) + 15) / 16) * 16 + kAnaWarps * sizeof(WarpSmem); }
 static size_t synthesis_smem_bytes() { return ((sizeof(SynBlockSmem) + 15) / 16) * 16 + kSynWarps * sizeof(SynWarpSmem); }
 
 cudaError_t dsp_configure() {
-  // a warp per stream; the two-streams-per-warp variant (L = 16) fits only 8 warps per SM and is no longer instantiated
-  cudaError_t e = cudaFuncSetAttribute(analysis_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       (int)analysis_smem_bytes<32>());
+  cudaError_t e = cudaFuncSetAttribute(analysis_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       (int)analysis_smem_bytes());
   if (e != cudaSuccess) return e;
   return cudaFuncSetAttribute(synthesis_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                               (int)synthesis_smem_bytes());
 }
 
 int launch_analysis(const AnalysisArgs &a, cudaStream_t st) {
-  dim3 grid((a.n_streams + AnaCfg<32>::kStreamsPerBlock - 1) / AnaCfg<32>::kStreamsPerBlock);
-  analysis_kernel<32><<<grid, AnaCfg<32>::kWarps * 32, analysis_smem_bytes<32>(), st>>>(a);
+  dim3 grid((a.n_streams + kAnaWarps - 1) / kAnaWarps);
+  analysis_kernel<<<grid, kAnaWarps * 32, analysis_smem_bytes(), st>>>(a);
   return 1;
 }
 // ------------------------------------------------------------------------------------------

@@ -89,3 +89,18 @@ def test_hop_major_order_is_topological(n_hops):
             assert idx[(t, DEP[l])] + units[DEP[l]] <= lo
         if t > 0:
             assert idx[(t - 1, l)] + units[l] <= lo
+
+
+def chain_is_diagonal(n_active, sm):         # tc_gru_chain: a.diag = (tiles_mp * (512 / HT) < sm_count), HT = 64
+    return -(-n_active // 128) * (512 // 64) < sm
+
+
+@pytest.mark.parametrize("sm,first", [(132, 2049), (114, 1793), (128, 1921), (136, 2049), (8, 1)])
+def test_first_hop_major_size(sm, first):
+    """tests/util.first_hop_major, which the GPU tests size their hop-major cases with, is the chain's switch: H100 SXM
+    (132 SMs) and PCIe (114 SMs), and SM counts on and next to a multiple of 8."""
+    from util import first_hop_major
+    assert first_hop_major(sm) == first
+    assert not chain_is_diagonal(first, sm)
+    assert first == 1 or chain_is_diagonal(first - 1, sm)
+    assert not chain_is_diagonal(16384, sm)

@@ -8,7 +8,9 @@ states; `read_nn_state()["c2"]` gives the conv2 output and `gr` the fc_gb / fc_r
 exactly these fp32 values (for a tensor engine the exported values are the sums of the 16-bit terms the MMAs read), wired
 as compute_rnn (rnn.cpp:42-81): gru1 <- c2, gru2 <- gru1, gru3 <- gru2, gru_gb <- gru3, gru_rb <- [gru3 ; c2],
 fc_gb <- [c2 ; gru1 ; gru2 ; gru3 ; gru_gb], fc_rb <- gru_rb.  Multi-hop calls are tied bit for bit to 1-hop calls by
-test_gpu_submit's test_call_granularity_does_not_change_the_output, so checking 1-hop calls covers the chain.
+test_gpu_isolation's test_call_granularity_does_not_change_the_output, at 9 streams (the GRU chain's anti-diagonal unit
+order) and at util.first_hop_major streams (its hop-major order), so checking 1-hop calls covers the chain in both orders;
+the cases below run both orders too (the "-hm" cases are hop-major).
 
 The bound.  For a layer with pre-activation y = b + sum_k w_k x_k (float64 from the fp32 operands) and
 A = sum_k |w_k| |x_k|, the engine's fp32 pre-activation lies in [y - B, y + B] with
@@ -610,6 +612,7 @@ def signals(oracle, m, S, F, seed):
 
 
 WARM, HOPS = 3, 3
+HM = "first_hop_major"
 CASES = [  # (id, S, n active, mode, model)
     ("tc-1", 1, 1, "bf16x2", "model0"), ("tc-127", 127, 127, "bf16x2", "model0"),
     ("tc-129", 129, 129, "bf16x2", "model0"), ("tc-1000", 1000, 1000, "bf16x2", "model0"),
@@ -620,7 +623,18 @@ CASES = [  # (id, S, n active, mode, model)
     ("tc-hot", 129, 129, "bf16x2", "model_hot"), ("wide-hot", 129, 129, "bf16x3", "model_hot"),
     ("tc-third", 129, 129, "bf16x2", "third"), ("wide-third", 129, 129, "bf16x3", "third"),
     ("fp32-third", 65, 65, "fp32", "third"),
+    # hop-major chain order: HM + k stands for util.first_hop_major + k rows, resolved on the device the test runs on
+    ("tc-hm", (HM, 0), (HM, 0), "bf16x2", "model0"), ("wide-hm", (HM, 0), (HM, 0), "bf16x3", "model0"),
+    ("tc-active-hm", (HM, 255), (HM, 0), "bf16x2", "model0"),
 ]
+
+
+def _rows(v):
+    """a CASES size: an int, or (HM, k) = first_hop_major + k"""
+    if isinstance(v, int):
+        return v
+    from util import device_first_hop_major
+    return device_first_hop_major() + v[1]
 
 
 def _model(name, model0, model_hot):
@@ -664,6 +678,7 @@ def run_case(api, oracle, ar, m, S, n, mode, seed, inject_rows=True):
 @pytest.mark.parametrize("case", CASES, ids=[c[0] for c in CASES])
 def test_every_layer_within_its_bound(api, oracle, actrange, model0, model_hot, case, capsys):
     cid, S, n, mode, mname = case
+    S, n = _rows(S), _rows(n)
     m = _model(mname, model0, model_hot)
     reps = run_case(api, oracle, actrange, m, S, n, mode, seed=len(cid) + S)
     with capsys.disabled():

@@ -180,6 +180,40 @@ def test_ragged_pool_matches_twin(api, model0, mode, dtype):
     assert slides >= 1
 
 
+def _schedule_hop_major(seed, h, S, N, n_calls=10):
+    """Like _schedule, with list sizes h - 1 / h / S (h = first_hop_major: the chain's anti-diagonal order, then
+    hop-major) so consecutive calls change order, F in {1, 4, 9}, resets before call 5."""
+    rng = np.random.RandomState(seed)
+    sizes = [h - 1, h, S] * (n_calls // 3 + 1)
+    rng.shuffle(sizes)
+    out = []
+    for c, k in enumerate(sizes[:n_calls]):
+        ids = rng.choice(N, size=k, replace=False).astype(np.int32)
+        F = int(rng.choice([1, 4, 9]))
+        kind = c % 4
+        if kind == 2:
+            hops = np.full(k, F, np.int32)
+        elif kind == 3:
+            hops = np.ones(k, np.int32)
+        else:
+            hops = rng.randint(1, F + 1, size=k).astype(np.int32)
+        hops[rng.randint(k)] = F
+        resets = rng.choice(N, size=4, replace=False) if c == 5 else np.empty(0, np.int64)
+        out.append((ids, hops, resets))
+    return out
+
+
+def test_ragged_pool_matches_twin_hop_major(api, model0):
+    """A tensor pool of first_hop_major + 255 slots and 300 more sessions: list sizes on both sides of the chain's
+    switch to hop-major order, so frozen rows (hops beyond a session's count store nothing) and session moves run in
+    both orders and calls change order.  Outputs, g/r and final states equal the twin's."""
+    from util import device_first_hop_major
+    h = device_first_hop_major()
+    S = h + 255
+    N = S + 300
+    _run_pool(api, model0, "tensor", "f32", S, N, 9, _schedule_hop_major(19, h, S, N), 37)
+
+
 def test_fp32_chunks(api, model0):
     """An fp32 pool with max_frames = 40: hop counts 1, 31, 32, 33 and 40 straddle the 32-hop chunk of the fp32 network."""
     rng = np.random.RandomState(5)

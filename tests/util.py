@@ -19,6 +19,34 @@ def digest(*arrays):
     return h.hexdigest()
 
 
+def first_hop_major(sm):
+    """Fewest active streams whose GRU chain walks its units in hop-major order on a device with `sm` SMs.
+    tc_gru_chain (pnb_nn_tc.cu) picks anti-diagonal order while ceil(n / 128) * (512 / 64) < sm, so the first
+    hop-major size starts the row tile that brings the count to ceil(sm / 8) (132 SMs: 2 049, 114 SMs: 1 793)."""
+    return 128 * (-(-sm // 8) - 1) + 1
+
+
+def device_first_hop_major():
+    """first_hop_major of cuda:0."""
+    import torch
+    return first_hop_major(torch.cuda.get_device_properties(0).multi_processor_count)
+
+
+def crowd(n_streams, n_frames, seed, n_base=32):
+    """[n_streams, n_frames*480] float32 of distinct rows made cheaply: n_base synthetic streams, each row one of them
+    at its own level and shifted by its own whole number of hops."""
+    from percepnet_b200.synth import synth_pcm
+    base = synth_pcm(n_base, n_frames, seed=seed)
+    rng = np.random.RandomState(seed)
+    rows = rng.randint(0, n_base, n_streams)
+    level = (0.25 + rng.rand(n_streams)).astype(np.float32)
+    shift = rng.randint(0, n_frames, n_streams) * 480
+    out = np.empty((n_streams, base.shape[1]), np.float32)
+    for i in range(n_streams):
+        out[i] = np.roll(base[rows[i]], shift[i]) * level[i]
+    return out
+
+
 def bits(a):
     return np.ascontiguousarray(a, dtype=np.float32).view(np.int32)
 

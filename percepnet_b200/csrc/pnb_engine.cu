@@ -540,23 +540,40 @@ static int enqueue_plan(pnb_engine *e, const int *ids, int k, const int *hops, i
   return launch_session_move(a, st);
 }
 
-// One enhancement call on st (arguments already checked).  With a session list (ids, n_ids) the call first applies its
-// residency plan, and reads input row / writes output row and g/r row row[p] for slot p.  With hops (host, list order;
-// a ragged call, F = the largest) slot p runs the hops of its list row, and the slots that stop early are moved to the
-// counters of hop F after synthesis.
-static int enqueue_enhance(pnb_engine *e, const float *d_in, const short *d_in16, size_t in_stride, float *d_out,
-                           short *d_out16, size_t out_stride, int F, float *d_gr, cudaStream_t st, const int *ids = nullptr,
-                           int n_ids = 0, const int *hops = nullptr) {
+// One enhancement call as its entry point received it: rows of float samples, or of int16 samples (i16), in and out, in
+// host or device memory by entry point.
+struct Call {
+  enum Kind { kSlots, kSessions, kRagged } kind;
+  const void *in;
+  size_t in_stride;
+  void *out;
+  size_t out_stride;
+  bool i16;
+  int F;           // hops; a ragged call's is max(hops), set by check_enhance
+  float *gr;       // g/r destination [F][rows][68], or null
+  const int *ids;  // session and ragged calls: the session list (host), n_ids long
+  int n_ids;
+  const int *hops;  // ragged calls: each listed session's hops (host); null once check_enhance finds them all equal to F
+};
+
+// One enhancement call on st, its buffers on the device (arguments already checked).  A session call first applies its
+// residency plan, and reads input row / writes output row and g/r row row[p] for slot p.  With hops (a ragged call)
+// slot p runs the hops of its list row, and the slots that stop early are moved to the counters of hop F after
+// synthesis.
+static int enqueue_enhance(pnb_engine *e, const Call &c, cudaStream_t st) {
+  const int F = c.F;
   return enqueue_call(e, F, st, [&]() -> int {
     int n = 0;
     const int *row = nullptr;
     RaggedSlots rg;
-    if (ids) {
-      n = enqueue_plan(e, ids, n_ids, hops, F, st, &row, &rg);
+    if (c.ids) {
+      n = enqueue_plan(e, c.ids, c.n_ids, c.hops, F, st, &row, &rg);
       if (n < 0) return n;
     }
     const int S = e->S, na = e->n_active;  // the call advances streams [0, na); per-call buffers keep the stride S
-    { ProfScope ps(e, PNB_K_STAGE_IN, st); n += launch_stage_in(e->d_pcm + e->line_off, e->pcm_stride, d_in, d_in16, in_stride, na, F * kFrame, st, 32768.f, row, rg.hops); }
+    const float *in = c.i16 ? nullptr : static_cast<const float *>(c.in);
+    const short *in16 = c.i16 ? static_cast<const short *>(c.in) : nullptr;
+    { ProfScope ps(e, PNB_K_STAGE_IN, st); n += launch_stage_in(e->d_pcm + e->line_off, e->pcm_stride, in, in16, c.in_stride, na, F * kFrame, st, 32768.f, row, rg.hops); }
     {
       AnalysisArgs aa = analysis_args(e, F);
       aa.hops = rg.hops;
@@ -570,7 +587,8 @@ static int enqueue_enhance(pnb_engine *e, const float *d_in, const short *d_in16
       n += q;
     }
     {
-      SynthesisArgs sa = synthesis_args(e, F, d_out, d_out16, out_stride);
+      SynthesisArgs sa = synthesis_args(e, F, c.i16 ? nullptr : static_cast<float *>(c.out),
+                                        c.i16 ? static_cast<short *>(c.out) : nullptr, c.out_stride);
       sa.row = row;
       sa.hops = rg.hops;
       ProfScope ps(e, PNB_K_SYNTHESIS, st);
@@ -581,10 +599,10 @@ static int enqueue_enhance(pnb_engine *e, const float *d_in, const short *d_in16
       n += launch_ragged_carry(e, F, rg.hops, rg.slots, rg.n_short, st);
     }
     n += advance_line(e, F, st);
-    if (d_gr && row)  // [F][na][68] in list order
-      n += launch_gr_gather(e->d_gr, d_gr, row, na, S, F, st, rg.hops);
-    else if (d_gr)  // [F][na][68] from the [F][S][68] buffer
-      CK(cudaMemcpy2DAsync(d_gr, (size_t)na * 68 * sizeof(float), e->d_gr, (size_t)S * 68 * sizeof(float), (size_t)na * 68 * sizeof(float), F,
+    if (c.gr && row)  // [F][na][68] in list order
+      n += launch_gr_gather(e->d_gr, c.gr, row, na, S, F, st, rg.hops);
+    else if (c.gr)  // [F][na][68] from the [F][S][68] buffer
+      CK(cudaMemcpy2DAsync(c.gr, (size_t)na * 68 * sizeof(float), e->d_gr, (size_t)S * 68 * sizeof(float), (size_t)na * 68 * sizeof(float), F,
                            cudaMemcpyDeviceToDevice, st));
     return n;
   });
@@ -595,60 +613,74 @@ static int refuse_in_session_mode() {
   return fail(PNB_ERR_ARG, "engine is in session mode (pnb_sessions_reserve): slots are the pool's; use the *_sessions entry points");
 }
 
+// The entries of a slot or session list, the argument `name`: each in [0, end) and in the active range [0, active) (a
+// session list passes active = end), none listed twice.  Repeats are found with the session pool's scratch, which is -1
+// everywhere between calls; a slot list of an engine without a pool grows it to the number of slots.
+static int check_list(pnb_engine *e, const int *list, int n, int end, int active, const char *name) {
+  for (int i = 0; i < n; i++) {
+    if (list[i] < 0 || list[i] >= end) return fail(PNB_ERR_ARG, "%s[%d] = %d outside [0, %d)", name, i, list[i], end);
+    if (list[i] >= active) return fail(PNB_ERR_ARG, "%s[%d] = %d outside the active range [0, %d)", name, i, list[i], active);
+  }
+  if (e->pool.listed.size() < (size_t)end) e->pool.listed.resize(end, -1);
+  const int d = e->pool.duplicate(list, n);
+  if (d >= 0) return fail(PNB_ERR_ARG, "%s[%d] = %d listed twice", name, d, list[d]);
+  return PNB_OK;
+}
+
 // A session list: after pnb_sessions_reserve, n in [1, n_max], distinct ids in [0, capacity).
 static int check_ids(pnb_engine *e, const int *ids, int n, int n_max) {
   if (!e->sessions) return fail(PNB_ERR_ARG, "no session pool: call pnb_sessions_reserve first");
   if (!ids) return fail(PNB_ERR_ARG, "ids is NULL");
   if (n < 1 || n > n_max) return fail(PNB_ERR_ARG, "n = %d sessions outside [1, %d]", n, n_max);
-  const int cap = e->pool.capacity();
-  for (int i = 0; i < n; i++)
-    if (ids[i] < 0 || ids[i] >= cap) return fail(PNB_ERR_ARG, "ids[%d] = %d outside [0, %d)", i, ids[i], cap);
-  const int d = e->pool.duplicate(ids, n);
-  if (d >= 0) return fail(PNB_ERR_ARG, "session %d listed twice (ids[%d])", ids[d], d);
+  return check_list(e, ids, n, e->pool.capacity(), e->pool.capacity(), "ids");
+}
+
+// Every refusal of an enhancement call, before anything changes.  A slot call: check_call, then session mode.  A session
+// call: check_call, then the list.  A ragged call checks the list and its hop counts first, because their largest is
+// the call's length F; when every session runs F hops, hops becomes null and the call is the plain session call.
+static int check_enhance(pnb_engine *e, Call &c) {
+  if (c.kind == Call::kRagged) {
+    if (!e) return fail(PNB_ERR_ARG, "engine is NULL");
+    { int rc = check_ids(e, c.ids, c.n_ids, e->S); if (rc) return rc; }
+    if (!c.hops) return fail(PNB_ERR_ARG, "hops is NULL");
+    c.F = 0;
+    for (int i = 0; i < c.n_ids; i++) {
+      if (c.hops[i] < 1 || c.hops[i] > e->Fmax) return fail(PNB_ERR_ARG, "hops[%d] = %d outside [1, %d]", i, c.hops[i], e->Fmax);
+      c.F = c.hops[i] > c.F ? c.hops[i] : c.F;
+    }
+    bool uniform = true;
+    for (int i = 0; i < c.n_ids; i++) uniform = uniform && c.hops[i] == c.F;
+    if (uniform) c.hops = nullptr;
+  }
+  { int rc = check_call(e, false, c.in && c.out, c.F, c.in_stride, c.out_stride); if (rc) return rc; }
+  if (c.kind == Call::kSessions) return check_ids(e, c.ids, c.n_ids, e->S);
+  if (c.kind == Call::kSlots && e->sessions) return refuse_in_session_mode();
   return PNB_OK;
 }
 
-// Every session call's check (pnb_process_sessions_* and pnb_process_sessions_ragged_*): check_call and the list.  A
-// ragged call (ragged) checks its hop counts first, because their largest is the call's length *F; when every session
-// runs *F hops, *hops becomes null and the call is the plain session call of *F hops.
-static int check_sessions(pnb_engine *e, bool buffers, const int *ids, int n, bool ragged, const int **hops, int *F,
-                          size_t in_stride, size_t out_stride) {
-  if (ragged) {
-    if (!e) return fail(PNB_ERR_ARG, "engine is NULL");
-    { int rc = check_ids(e, ids, n, e->S); if (rc) return rc; }
-    const int *h = *hops;
-    if (!h) return fail(PNB_ERR_ARG, "hops is NULL");
-    int mx = 0;
-    for (int i = 0; i < n; i++) {
-      if (h[i] < 1 || h[i] > e->Fmax) return fail(PNB_ERR_ARG, "hops[%d] = %d outside [1, %d]", i, h[i], e->Fmax);
-      mx = h[i] > mx ? h[i] : mx;
-    }
-    bool uniform = true;
-    for (int i = 0; i < n; i++) uniform = uniform && h[i] == mx;
-    *F = mx;
-    if (uniform) *hops = nullptr;
-  }
-  { int rc = check_call(e, false, buffers, *F, in_stride, out_stride); if (rc) return rc; }
-  return ragged ? PNB_OK : check_ids(e, ids, n, e->S);
-}
-
-static int process_device(pnb_engine *e, const float *d_in, const short *d_in16, size_t in_stride, float *d_out,
-                          short *d_out16, size_t out_stride, int F, float *d_gr, cudaStream_t st) {
-  { int rc = check_call(e, false, (d_in || d_in16) && (d_out || d_out16), F, in_stride, out_stride); if (rc) return rc; }
-  if (e->sessions) return refuse_in_session_mode();
+// pnb_process_device_*, pnb_submit_device_* and the device forms of the session calls.
+static int device_call(pnb_engine *e, Call c, cudaStream_t st) {
+  { int rc = check_enhance(e, c); if (rc) return rc; }
   CK(cudaSetDevice(e->device));
-  return enqueue_enhance(e, d_in, d_in16, in_stride, d_out, d_out16, out_stride, F, d_gr, st);
+  return enqueue_enhance(e, c, st);
 }
 
 extern "C" int pnb_process_device_f32(pnb_engine *e, const float *d_in, size_t in_stride, float *d_out,
                                       size_t out_stride, int n_frames, float *d_gr, void *cuda_stream) {
-  return process_device(e, d_in, nullptr, in_stride, d_out, nullptr, out_stride, n_frames, d_gr,
-                        (cudaStream_t)cuda_stream);
+  return device_call(e, {Call::kSlots, d_in, in_stride, d_out, out_stride, false, n_frames, d_gr}, (cudaStream_t)cuda_stream);
 }
 extern "C" int pnb_process_device_i16(pnb_engine *e, const short *d_in, size_t in_stride, short *d_out,
                                       size_t out_stride, int n_frames, float *d_gr, void *cuda_stream) {
-  return process_device(e, nullptr, d_in, in_stride, nullptr, d_out, out_stride, n_frames, d_gr,
-                        (cudaStream_t)cuda_stream);
+  return device_call(e, {Call::kSlots, d_in, in_stride, d_out, out_stride, true, n_frames, d_gr}, (cudaStream_t)cuda_stream);
+}
+// pnb_process_device_* without g/r; both names are part of the ABI.
+extern "C" int pnb_submit_device_f32(pnb_engine *e, const float *d_in, size_t in_stride, float *d_out, size_t out_stride,
+                                     int n_frames, void *cuda_stream) {
+  return device_call(e, {Call::kSlots, d_in, in_stride, d_out, out_stride, false, n_frames, nullptr}, (cudaStream_t)cuda_stream);
+}
+extern "C" int pnb_submit_device_i16(pnb_engine *e, const short *d_in, size_t in_stride, short *d_out, size_t out_stride,
+                                     int n_frames, void *cuda_stream) {
+  return device_call(e, {Call::kSlots, d_in, in_stride, d_out, out_stride, true, n_frames, nullptr}, (cudaStream_t)cuda_stream);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -806,41 +838,32 @@ static int report_status(pnb_engine *e) {
   return PNB_OK;
 }
 
-// pnb_process_host_* (blocking) and pnb_submit_host_* (pipelined); with `sessions` the blocking
-// pnb_process_sessions_host_* of the list (ids, n_ids), and with `ragged` too pnb_process_sessions_ragged_host_* (hops;
-// F is then the largest).  The blocking form then copies g/r and the status word back on the engine's stream too, and
+// pnb_process_host_*, pnb_process_sessions_host_*, pnb_process_sessions_ragged_host_* (blocking) and pnb_submit_host_*
+// (pipelined).  The blocking form then copies g/r and the status word back on the engine's stream too, and
 // synchronises it once.  Rows travel F hops wide: a ragged call's input beyond a row's hops is copied but not read.
-template <typename T>
-static int host_call(pnb_engine *e, const T *in, size_t in_stride, T *out, size_t out_stride, int F, float *gr, bool pipelined,
-                     bool sessions = false, const int *ids = nullptr, int n_ids = 0, bool ragged = false,
-                     const int *hops = nullptr) {
-  if (sessions) {
-    int rc = check_sessions(e, in && out, ids, n_ids, ragged, &hops, &F, in_stride, out_stride);
-    if (rc) return rc;
-  } else {
-    { int rc = check_call(e, false, in && out, F, in_stride, out_stride); if (rc) return rc; }
-    if (e->sessions) return refuse_in_session_mode();
-  }
+static int host_call(pnb_engine *e, Call c, bool pipelined) {
+  { int rc = check_enhance(e, c); if (rc) return rc; }
   CK(cudaSetDevice(e->device));
-  const size_t S = e->S, row = (size_t)e->Fmax * kFrame, w = (size_t)F * kFrame * sizeof(T);
-  const size_t na = sessions ? n_ids : e->n_active;  // the rows of in / out / gr
-  const int k = staging_slot(e, pipelined, S * row * sizeof(T), S * row * sizeof(T));
+  const size_t es = c.i16 ? sizeof(short) : sizeof(float);
+  const size_t S = e->S, row = (size_t)e->Fmax * kFrame, w = (size_t)c.F * kFrame * es;
+  const size_t na = c.ids ? c.n_ids : e->n_active;  // the rows of in / out / gr
+  const int k = staging_slot(e, pipelined, S * row * es, S * row * es);
   if (k < 0) return k;
-  if (sessions && gr) { int rc = grow((void **)&e->d_sgr, &e->sgr_bytes, (size_t)e->Fmax * S * 68 * sizeof(float)); if (rc) return rc; }
-  float *d_gr = sessions && gr ? e->d_sgr : nullptr;  // session calls gather g/r in list order on the device
-  T *d_in = (T *)e->stage[k].in, *d_out = (T *)e->stage[k].out;
+  if (c.ids && c.gr) { int rc = grow((void **)&e->d_sgr, &e->sgr_bytes, (size_t)e->Fmax * S * 68 * sizeof(float)); if (rc) return rc; }
+  Call d = c;  // the call on staging slot k
+  d.in = e->stage[k].in;
+  d.out = e->stage[k].out;
+  d.in_stride = d.out_stride = row;
+  d.gr = c.ids && c.gr ? e->d_sgr : nullptr;  // session calls gather g/r in list order on the device
   const int rc = round_trip(e, k, pipelined,
-      [&](cudaStream_t s) { return cudaMemcpy2DAsync(d_in, row * sizeof(T), in, in_stride * sizeof(T), w, na, cudaMemcpyHostToDevice, s); },
-      [&] {
-        return sizeof(T) == 4 ? enqueue_enhance(e, (const float *)d_in, nullptr, row, (float *)d_out, nullptr, row, F, d_gr, e->stream, ids, n_ids, hops)
-                              : enqueue_enhance(e, nullptr, (const short *)d_in, row, nullptr, (short *)d_out, row, F, d_gr, e->stream, ids, n_ids, hops);
-      },
-      [&](cudaStream_t s) { return cudaMemcpy2DAsync(out, out_stride * sizeof(T), d_out, row * sizeof(T), w, na, cudaMemcpyDeviceToHost, s); });
+      [&](cudaStream_t s) { return cudaMemcpy2DAsync(e->stage[k].in, row * es, c.in, c.in_stride * es, w, na, cudaMemcpyHostToDevice, s); },
+      [&] { return enqueue_enhance(e, d, e->stream); },
+      [&](cudaStream_t s) { return cudaMemcpy2DAsync(c.out, c.out_stride * es, e->stage[k].out, row * es, w, na, cudaMemcpyDeviceToHost, s); });
   if (rc || pipelined) return rc;
-  if (gr && d_gr)
-    CK(cudaMemcpyAsync(gr, d_gr, (size_t)F * na * 68 * sizeof(float), cudaMemcpyDeviceToHost, e->stream));
-  else if (gr)
-    CK(cudaMemcpy2DAsync(gr, na * 68 * sizeof(float), e->d_gr, S * 68 * sizeof(float), na * 68 * sizeof(float), F, cudaMemcpyDeviceToHost,
+  if (d.gr)
+    CK(cudaMemcpyAsync(c.gr, d.gr, (size_t)c.F * na * 68 * sizeof(float), cudaMemcpyDeviceToHost, e->stream));
+  else if (c.gr)
+    CK(cudaMemcpy2DAsync(c.gr, na * 68 * sizeof(float), e->d_gr, S * 68 * sizeof(float), na * 68 * sizeof(float), c.F, cudaMemcpyDeviceToHost,
                          e->stream));
   CK(cudaMemcpyAsync(e->h_status, e->d_status, 2 * sizeof(int), cudaMemcpyDeviceToHost, e->stream));
   CK(cudaStreamSynchronize(e->stream));
@@ -849,30 +872,21 @@ static int host_call(pnb_engine *e, const T *in, size_t in_stride, T *out, size_
 
 extern "C" int pnb_process_host_f32(pnb_engine *e, const float *in, size_t in_stride, float *out, size_t out_stride,
                                     int n_frames, float *gr) {
-  return host_call<float>(e, in, in_stride, out, out_stride, n_frames, gr, false);
+  return host_call(e, {Call::kSlots, in, in_stride, out, out_stride, false, n_frames, gr}, false);
 }
 extern "C" int pnb_process_host_i16(pnb_engine *e, const short *in, size_t in_stride, short *out, size_t out_stride,
                                     int n_frames, float *gr) {
-  return host_call<short>(e, in, in_stride, out, out_stride, n_frames, gr, false);
+  return host_call(e, {Call::kSlots, in, in_stride, out, out_stride, true, n_frames, gr}, false);
 }
 extern "C" int pnb_submit_host_f32(pnb_engine *e, const float *in, size_t in_stride, float *out, size_t out_stride,
                                    int n_frames) {
-  return host_call<float>(e, in, in_stride, out, out_stride, n_frames, nullptr, true);
+  return host_call(e, {Call::kSlots, in, in_stride, out, out_stride, false, n_frames, nullptr}, true);
 }
 extern "C" int pnb_submit_host_i16(pnb_engine *e, const short *in, size_t in_stride, short *out, size_t out_stride,
                                    int n_frames) {
-  return host_call<short>(e, in, in_stride, out, out_stride, n_frames, nullptr, true);
+  return host_call(e, {Call::kSlots, in, in_stride, out, out_stride, true, n_frames, nullptr}, true);
 }
 
-// pnb_process_device_* without g/r; both names are part of the ABI.
-extern "C" int pnb_submit_device_f32(pnb_engine *e, const float *d_in, size_t in_stride, float *d_out, size_t out_stride,
-                                     int n_frames, void *cuda_stream) {
-  return pnb_process_device_f32(e, d_in, in_stride, d_out, out_stride, n_frames, nullptr, cuda_stream);
-}
-extern "C" int pnb_submit_device_i16(pnb_engine *e, const short *d_in, size_t in_stride, short *d_out, size_t out_stride,
-                                     int n_frames, void *cuda_stream) {
-  return pnb_process_device_i16(e, d_in, in_stride, d_out, out_stride, n_frames, nullptr, cuda_stream);
-}
 extern "C" int pnb_flush(pnb_engine *e, void *cuda_stream) {
   if (!e) return fail(PNB_ERR_ARG, "engine is NULL");
   CK(cudaSetDevice(e->device));
@@ -967,28 +981,25 @@ static int state_enqueue(pnb_engine *e, int mode, const int *streams, int n, voi
   return PNB_OK;
 }
 
+// The blobs of a batched state operation: not NULL, blob_stride at least pnb_state_size(), both 4-byte aligned.
+static int check_blobs(const void *d_blobs, size_t blob_stride) {
+  if (!d_blobs) return fail(PNB_ERR_ARG, "d_blobs is NULL");
+  if (blob_stride < sizeof(StreamState))
+    return fail(PNB_ERR_ARG, "blob_stride %zu below pnb_state_size() = %zu", blob_stride, sizeof(StreamState));
+  if ((reinterpret_cast<uintptr_t>(d_blobs) | blob_stride) & 3) return fail(PNB_ERR_ARG, "d_blobs and blob_stride must be multiples of 4 bytes");
+  return PNB_OK;
+}
+
 static int state_batch(pnb_engine *e, int mode, const int *streams, int n, void *d_blobs, size_t blob_stride, void *cuda_stream) {
   if (!e) return fail(PNB_ERR_ARG, "engine is NULL");
   if (e->sessions) return refuse_in_session_mode();
   if (n < 0) return fail(PNB_ERR_ARG, "n = %d is negative", n);
   if (n == 0) return PNB_OK;
   if (!streams) return fail(PNB_ERR_ARG, "streams is NULL");
-  if (mode != kStateReset) {
-    if (!d_blobs) return fail(PNB_ERR_ARG, "d_blobs is NULL");
-    if (blob_stride < sizeof(StreamState))
-      return fail(PNB_ERR_ARG, "blob_stride %zu below pnb_state_size() = %zu", blob_stride, sizeof(StreamState));
-    if ((reinterpret_cast<uintptr_t>(d_blobs) | blob_stride) & 3) return fail(PNB_ERR_ARG, "d_blobs and blob_stride must be multiples of 4 bytes");
-  }
+  if (mode != kStateReset) { int rc = check_blobs(d_blobs, blob_stride); if (rc) return rc; }
   if (e->poisoned) return fail(PNB_ERR_ARG, "an earlier call failed while enqueuing work; the streams' state is undefined until pnb_reset");
   if (n > e->S) return fail(PNB_ERR_ARG, "n = %d streams, the engine has %d", n, e->S);
-  std::vector<unsigned char> seen(e->S, 0);
-  for (int i = 0; i < n; i++) {
-    const int s = streams[i];
-    if (s < 0 || s >= e->S) return fail(PNB_ERR_ARG, "streams[%d] = %d outside [0, %d)", i, s, e->S);
-    if (s >= e->n_active) return fail(PNB_ERR_ARG, "streams[%d] = %d outside the active range [0, %d)", i, s, e->n_active);
-    if (seen[s]) return fail(PNB_ERR_ARG, "stream %d listed twice", s);
-    seen[s] = 1;
-  }
+  { int rc = check_list(e, streams, n, e->S, e->n_active, "streams"); if (rc) return rc; }
   CK(cudaSetDevice(e->device));
   const int rc = state_enqueue(e, mode, streams, n, d_blobs, blob_stride, (cudaStream_t)cuda_stream);
   if (rc) e->poisoned = true;  // part of the operation may have been enqueued
@@ -1028,8 +1039,7 @@ extern "C" int pnb_active_streams(const pnb_engine *e) { return e ? e->n_active 
 static int state_args(pnb_engine *e, int stream, const void *buf, size_t bytes) {
   if (!e || !buf) return fail(PNB_ERR_ARG, "NULL argument");
   if (e->sessions) return refuse_in_session_mode();
-  if (stream < 0 || stream >= e->S) return fail(PNB_ERR_ARG, "stream %d outside [0, %d)", stream, e->S);
-  if (stream >= e->n_active) return fail(PNB_ERR_ARG, "stream %d outside the active range [0, %d)", stream, e->n_active);
+  { int rc = check_list(e, &stream, 1, e->S, e->n_active, "stream"); if (rc) return rc; }
   if (bytes < sizeof(StreamState)) return fail(PNB_ERR_ARG, "state buffer of %zu bytes, need pnb_state_size() = %zu", bytes, sizeof(StreamState));
   if (e->poisoned) return fail(PNB_ERR_CUDA, "engine state is undefined after a failed call; pnb_reset it");
   return PNB_OK;
@@ -1132,54 +1142,41 @@ extern "C" int pnb_session_stats(const pnb_engine *e, long long *out) {
   return PNB_OK;
 }
 
-static int process_sessions_device(pnb_engine *e, const int *ids, int n, const float *d_in, const short *d_in16, size_t in_stride,
-                                   float *d_out, short *d_out16, size_t out_stride, int F, float *d_gr, cudaStream_t st,
-                                   bool ragged = false, const int *hops = nullptr) {
-  { int rc = check_sessions(e, (d_in || d_in16) && (d_out || d_out16), ids, n, ragged, &hops, &F, in_stride, out_stride); if (rc) return rc; }
-  CK(cudaSetDevice(e->device));
-  return enqueue_enhance(e, d_in, d_in16, in_stride, d_out, d_out16, out_stride, F, d_gr, st, ids, n, hops);
-}
 extern "C" int pnb_process_sessions_device_f32(pnb_engine *e, const int *ids, int n, const float *d_in, size_t in_stride,
                                                float *d_out, size_t out_stride, int n_frames, float *d_gr, void *cuda_stream) {
-  return process_sessions_device(e, ids, n, d_in, nullptr, in_stride, d_out, nullptr, out_stride, n_frames, d_gr,
-                                 (cudaStream_t)cuda_stream);
+  return device_call(e, {Call::kSessions, d_in, in_stride, d_out, out_stride, false, n_frames, d_gr, ids, n}, (cudaStream_t)cuda_stream);
 }
 extern "C" int pnb_process_sessions_device_i16(pnb_engine *e, const int *ids, int n, const short *d_in, size_t in_stride,
                                                short *d_out, size_t out_stride, int n_frames, float *d_gr, void *cuda_stream) {
-  return process_sessions_device(e, ids, n, nullptr, d_in, in_stride, nullptr, d_out, out_stride, n_frames, d_gr,
-                                 (cudaStream_t)cuda_stream);
+  return device_call(e, {Call::kSessions, d_in, in_stride, d_out, out_stride, true, n_frames, d_gr, ids, n}, (cudaStream_t)cuda_stream);
 }
 extern "C" int pnb_process_sessions_host_f32(pnb_engine *e, const int *ids, int n, const float *in, size_t in_stride, float *out,
                                              size_t out_stride, int n_frames, float *gr) {
-  if (!e) return fail(PNB_ERR_ARG, "engine is NULL");
-  return host_call<float>(e, in, in_stride, out, out_stride, n_frames, gr, false, true, ids, n);
+  return host_call(e, {Call::kSessions, in, in_stride, out, out_stride, false, n_frames, gr, ids, n}, false);
 }
 extern "C" int pnb_process_sessions_host_i16(pnb_engine *e, const int *ids, int n, const short *in, size_t in_stride, short *out,
                                              size_t out_stride, int n_frames, float *gr) {
-  if (!e) return fail(PNB_ERR_ARG, "engine is NULL");
-  return host_call<short>(e, in, in_stride, out, out_stride, n_frames, gr, false, true, ids, n);
+  return host_call(e, {Call::kSessions, in, in_stride, out, out_stride, true, n_frames, gr, ids, n}, false);
 }
 
-// Ragged session calls: session ids[i] advances by hops[i]; the call is max(hops) hops long (check_sessions).
+// Ragged session calls: session ids[i] advances by hops[i]; the call is max(hops) hops long (check_enhance).
 extern "C" int pnb_process_sessions_ragged_device_f32(pnb_engine *e, const int *ids, const int *hops, int n, const float *d_in,
                                                       size_t in_stride, float *d_out, size_t out_stride, float *d_gr,
                                                       void *cuda_stream) {
-  return process_sessions_device(e, ids, n, d_in, nullptr, in_stride, d_out, nullptr, out_stride, 0, d_gr,
-                                 (cudaStream_t)cuda_stream, true, hops);
+  return device_call(e, {Call::kRagged, d_in, in_stride, d_out, out_stride, false, 0, d_gr, ids, n, hops}, (cudaStream_t)cuda_stream);
 }
 extern "C" int pnb_process_sessions_ragged_device_i16(pnb_engine *e, const int *ids, const int *hops, int n, const short *d_in,
                                                       size_t in_stride, short *d_out, size_t out_stride, float *d_gr,
                                                       void *cuda_stream) {
-  return process_sessions_device(e, ids, n, nullptr, d_in, in_stride, nullptr, d_out, out_stride, 0, d_gr,
-                                 (cudaStream_t)cuda_stream, true, hops);
+  return device_call(e, {Call::kRagged, d_in, in_stride, d_out, out_stride, true, 0, d_gr, ids, n, hops}, (cudaStream_t)cuda_stream);
 }
 extern "C" int pnb_process_sessions_ragged_host_f32(pnb_engine *e, const int *ids, const int *hops, int n, const float *in,
                                                     size_t in_stride, float *out, size_t out_stride, float *gr) {
-  return host_call<float>(e, in, in_stride, out, out_stride, 0, gr, false, true, ids, n, true, hops);
+  return host_call(e, {Call::kRagged, in, in_stride, out, out_stride, false, 0, gr, ids, n, hops}, false);
 }
 extern "C" int pnb_process_sessions_ragged_host_i16(pnb_engine *e, const int *ids, const int *hops, int n, const short *in,
                                                     size_t in_stride, short *out, size_t out_stride, float *gr) {
-  return host_call<short>(e, in, in_stride, out, out_stride, 0, gr, false, true, ids, n, true, hops);
+  return host_call(e, {Call::kRagged, in, in_stride, out, out_stride, true, 0, gr, ids, n, hops}, false);
 }
 
 // pnb_reset_sessions / pnb_export_sessions / pnb_import_sessions.  A reset or an import takes the listed sessions out
@@ -1190,12 +1187,7 @@ static int session_batch(pnb_engine *e, int mode, const int *ids, int n, void *d
   if (!e) return fail(PNB_ERR_ARG, "engine is NULL");
   if (e->poisoned) return fail(PNB_ERR_ARG, "an earlier call failed while enqueuing work; the streams' state is undefined until pnb_reset");
   if (n == 0 && e->sessions) return PNB_OK;
-  if (mode != kStateReset) {
-    if (!d_blobs) return fail(PNB_ERR_ARG, "d_blobs is NULL");
-    if (blob_stride < sizeof(StreamState))
-      return fail(PNB_ERR_ARG, "blob_stride %zu below pnb_state_size() = %zu", blob_stride, sizeof(StreamState));
-    if ((reinterpret_cast<uintptr_t>(d_blobs) | blob_stride) & 3) return fail(PNB_ERR_ARG, "d_blobs and blob_stride must be multiples of 4 bytes");
-  }
+  if (mode != kStateReset) { int rc = check_blobs(d_blobs, blob_stride); if (rc) return rc; }
   { int rc = check_ids(e, ids, n, e->pool.capacity()); if (rc) return rc; }
   CK(cudaSetDevice(e->device));
   const cudaStream_t st = (cudaStream_t)cuda_stream;

@@ -298,7 +298,6 @@ extern "C" int pnb_reset(pnb_engine *e) {
     CK(cudaMemset(e->d_park, 0, (size_t)e->pool.capacity() * kParkStride));
     e->pool.init(e->S, e->pool.capacity());
   }
-  for (int i = 0; i < 5; i++) e->par[i] = 0;
   CK(cudaDeviceSynchronize());
   return PNB_OK;
 }
@@ -455,9 +454,9 @@ static int enqueue_ordered(pnb_engine *e, cudaStream_t st, Launches launches) {
   return n;
 }
 // Enqueues one call of F hops on st (arguments already checked) and commits the hop counter, last_frames and the launch
-// count when all of it was accepted.  The enqueue itself moves host-side stream state (advance_line the line offset,
-// the tensor carry the GRU buffer parity), so a failure after it started leaves the streams' state undefined: the
-// engine is poisoned, and refuses calls until pnb_reset.
+// count when all of it was accepted.  The enqueue itself moves host-side stream state (advance_line the line offset),
+// so a failure after it started leaves the streams' state undefined: the engine is poisoned, and refuses calls until
+// pnb_reset.
 template <typename Launches>
 static int enqueue_call(pnb_engine *e, int F, cudaStream_t st, Launches launches) {
   const int n = enqueue_ordered(e, st, launches);
@@ -942,7 +941,7 @@ extern "C" int pnb_read_tap(pnb_engine *e, int what, void *dst, size_t dst_bytes
     case PNB_TAP_NN_C2: src = e->c2; bytes = (size_t)e->S * 512 * 4; break;
     case PNB_TAP_NN_H0: case PNB_TAP_NN_H0 + 1: case PNB_TAP_NN_H0 + 2: case PNB_TAP_NN_H0 + 3: case PNB_TAP_NN_H0 + 4: {
       int li = what - PNB_TAP_NN_H0;
-      src = e->h[li][e->par[li]]; bytes = (size_t)e->S * kGruH[li] * 4; break;
+      src = e->h[li]; bytes = (size_t)e->S * kGruH[li] * 4; break;
     }
     default: return fail(PNB_ERR_ARG, "unknown tap %d", what);
   }

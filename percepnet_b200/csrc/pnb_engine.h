@@ -54,11 +54,10 @@ struct pnb_engine {
   float *d_tap_pitchf = nullptr;
   float *d_tap_g = nullptr;   // [F][S][34] gains as applied (PNB_KEEP_TAPS)
 
-  // network state both paths share: conv2's output of the last hop and the GRU states in fp32, whose layout each path's
-  // prepare hook sets (tensor: [S][H] ping-pong by hop parity par; fp32: h[l][0] only, its hop slots [chunk+1][S][H])
+  // network state both paths share: conv2's output of the last hop and the GRU states in fp32, whose rows [0, S) hold
+  // the state between calls (tensor: [S][H], updated in place; fp32: the front of its hop slots [chunk+1][S][H])
   float *c2 = nullptr;       // [S][512]
-  float *h[5][2] = {{nullptr, nullptr}, {nullptr, nullptr}, {nullptr, nullptr}, {nullptr, nullptr}, {nullptr, nullptr}};
-  int par[5] = {0, 0, 0, 0, 0};
+  float *h[5] = {};
   long hop = 0;  // hops processed since reset
 
   // Device staging of the host-buffer calls (pnb_process_host_*, pnb_submit_host_*, pnb_train_records_host,
@@ -104,7 +103,7 @@ struct pnb_engine {
   bool poisoned = false;
 
   // Session pool (pnb_sessions_reserve): sessions [0, capacity) are resident in a slot or parked as a blob in d_park.
-  // The host-side plan says which; every session call applies its plan when it is enqueued, like hop / line_off / par.
+  // The host-side plan says which; every session call applies its plan when it is enqueued, like hop / line_off.
   bool sessions = false;
   pnb::SessionPool pool;
   char *d_park = nullptr;        // [capacity][kParkStride] parking blobs; magic 0 = a fresh (or rejected) session

@@ -12,6 +12,7 @@
 
 #include <string>
 
+#include "pnb_chain.cuh"
 #include "pnb_engine.h"
 
 namespace pnb {
@@ -43,7 +44,7 @@ struct GemmArgs {
 // The five GRUs of a chunk of hops in one persistent fp32 launch.  Slot buffers: hop t of the chunk
 // reads state slot t and writes slot t+1; inputs are conv2's output slot t or the layer below's slot t+1.
 struct F32ChainLayer {
-  int H, n_x, dep;            // hidden size; input segments (1 or 2); layer whose fresh state is the input (-1: conv2 out)
+  int H, n_x, dep;            // hidden size; input segments (1 or 2); chain_dep of the layer
   const float *x[2];          // input buffers [slots][S][x_ld]
   int x_ld[2], x_K[2], x_slot1[2];
   size_t x_slot_stride[2];    // floats per hop slot of the input buffer
@@ -54,24 +55,10 @@ struct F32ChainLayer {
 constexpr int kF32ChainMaxHops = 32;  // hops per launch of the fp32 chain (longer chunks amortise the ramp diagonals)
 struct F32ChainArgs {
   F32ChainLayer L[5];
-  int S, n, n_rb, n_units, n_lh;               // S: rows per slot; n: active streams [0, n); n_rb: their stream blocks
-  unsigned char lh[5 * kF32ChainMaxHops];      // (hop << 3) | layer in anti-diagonal order
-  int lh_unit0[5 * kF32ChainMaxHops + 1];      // first unit of every entry; [n_lh] = n_units
-  unsigned *cnt;                               // [5][n_rb] finished tiles per (layer, stream block), zero at launch
+  ChainOrder order;  // anti-diagonal: the chunk's hops of the active streams' blocks, 32-unit tiles
+  int S, n;          // rows per slot; active streams [0, n)
+  unsigned *cnt;     // [5][order.n_rb] finished tiles per (layer, stream block), zero at launch
   const float *tansig;
-};
-// The first slot4 float4s of n_slots slots stride4 apart, from slots from.. of src (slot 0 of the source buffer) to
-// dst; row4: float4s per row.  In a ragged call (hops) a row that stops after hop h of the call takes its slots from
-// from - (n - clamp(h - h0, 0, n)) on instead (it stopped that many slots before the chunk's end), and nothing moves
-// when that is below 0 or the row is already in place.
-struct F32CarrySeg { float4 *dst; const float4 *src; size_t slot4, stride4, row4; int n_slots, from; };
-struct F32CarryArgs {
-  F32CarrySeg seg[12];
-  int n_seg;
-  unsigned *cnt;
-  int n_cnt;
-  const int *hops;  // [active streams] hops of each row in a ragged call, or null
-  int h0, n;        // the chunk: hops [h0, h0 + n) of the call
 };
 
 __device__ __forceinline__ float tansig_approx(float x, const float *__restrict__ tbl) {  // vec.h:53-71
@@ -258,10 +245,8 @@ int launch_fc_f32(const float *feat, const float *W, const float *bias, float *o
 // [x ; h], then the gate math and the state update in the same thread -- no pre-activation ever goes to memory.
 // State slot t of h_all[l] is the state BEFORE hop t of the chunk, slot t+1 the state after it: a layer reads slot t of
 // its own buffer and slot t+1 of the layer below (the freshly updated state, rnn.cpp:58-71), so nothing is overwritten
-// inside a launch.  A unit depends only on units of the same stream block: all tiles of (t, l-1) and of (t-1, l).  Each
-// (layer, stream block) has a completion counter (red.release / ld.acquire); units are walked in anti-diagonal order
-// (t + l ascending), where every dependency lies on an earlier diagonal, by a grid that is fully co-resident -- so the
-// waits are short, there is no grid barrier and no launch boundary between layers or hops.
+// inside a launch.  Dependencies, counters and the unit order are the tensor chain's (pnb_chain.cuh), always in
+// anti-diagonal order.
 // The accumulation order of every sum (ascending k, x segments first, then h, one FMA per term) is the one the
 // per-layer kernels above use.
 // ------------------------------------------------------------------------------------------------------------------
@@ -277,14 +262,6 @@ __device__ __forceinline__ void cp_async16(void *smem, const void *gmem, bool va
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 template <int N>
 __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
-__device__ __forceinline__ unsigned ld_acquire_gpu_u32(const unsigned *p) {
-  unsigned v;
-  asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-  return v;
-}
-__device__ __forceinline__ void red_release_gpu_add_u32(unsigned *p, unsigned v) {
-  asm volatile("red.release.gpu.global.add.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
-}
 
 template <int RT>  // rows per thread: 8 (128-stream blocks) or 1 (16-stream blocks, for a handful of streams)
 struct ChainSmem {
@@ -326,31 +303,19 @@ __global__ void __launch_bounds__(CH_THREADS, RT == 8 ? 2 : 4) gru_chain_f32_ker
   extern __shared__ __align__(16) unsigned char chain_smem_raw[];
   SM &sm = *reinterpret_cast<SM *>(chain_smem_raw);
   const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
-  const int S = args.S;
+  const int S = args.S, n_rb = args.order.n_rb;
 
-  for (int u = blockIdx.x; u < args.n_units; u += gridDim.x) {
-    // ---- which unit: anti-diagonal order, the (hop, layer) entries and their first units come from the host
-    int e = 0;
-    while (u >= args.lh_unit0[e + 1]) e++;
-    const int t = args.lh[e] >> 3, l = args.lh[e] & 7;
+  for (int u = blockIdx.x; u < args.order.units(); u += gridDim.x) {
+    const ChainUnit un = chain_decode(args.order, u);
+    const int t = un.t, l = un.l, rb = un.rb;
     const F32ChainLayer &L = args.L[l];
     const int tiles = L.H / CH_HT;
-    const int local = u - args.lh_unit0[e];
-    const int rb = local / tiles, j0 = (local - rb * tiles) * CH_HT, m0 = rb * BM;
+    const int j0 = un.tile * CH_HT, m0 = rb * BM;
 
     // ---- dependencies (one thread polls; the barrier publishes the result to the block)
     if (tid == 0) {
-      unsigned spins = 0;
-      if (L.dep >= 0) {
-        const unsigned want = (unsigned)(t + 1) * (unsigned)(args.L[L.dep].H / CH_HT);
-        while (ld_acquire_gpu_u32(args.cnt + L.dep * args.n_rb + rb) < want)
-          if (++spins > (1u << 26)) __trap();  // a broken schedule becomes a launch error, not a hang
-      }
-      if (t > 0) {
-        const unsigned want = (unsigned)t * (unsigned)tiles;
-        while (ld_acquire_gpu_u32(args.cnt + l * args.n_rb + rb) < want)
-          if (++spins > (1u << 26)) __trap();
-      }
+      if (L.dep >= 0) chain_wait(args.cnt + L.dep * n_rb + rb, (unsigned)(t + 1) * (unsigned)(args.L[L.dep].H / CH_HT));
+      if (t > 0) chain_wait(args.cnt + l * n_rb + rb, (unsigned)t * (unsigned)tiles);
     }
     __syncthreads();
 
@@ -440,31 +405,9 @@ __global__ void __launch_bounds__(CH_THREADS, RT == 8 ? 2 : 4) gru_chain_f32_ker
     __syncthreads();  // every thread's stores are issued (and the tile buffers are free for the next unit)
     if (tid == 0) {
       __threadfence();
-      red_release_gpu_add_u32(args.cnt + l * args.n_rb + rb, 1u);
+      red_release_gpu_add(args.cnt + l * n_rb + rb, 1u);
     }
   }
-}
-
-// End of a chunk of n hops: the last 4 fc / 2 conv1 slots and the last state slot move to the front (the active rows
-// of each), conv2's output of the last hop is kept for the tap, the chain's counters return to zero.  A thread owns the
-// same element of every slot and walks the slots upwards, so a slot that is both source and destination is read before
-// it is overwritten.  In a ragged call each row takes the slots of its own last hop (F32CarrySeg).
-__global__ void f32_carry_kernel(F32CarryArgs a) {
-  const size_t tid = (size_t)blockIdx.x * blockDim.x + threadIdx.x, stride = (size_t)gridDim.x * blockDim.x;
-  for (int sg = 0; sg < a.n_seg; sg++) {
-    const F32CarrySeg &g = a.seg[sg];
-    for (size_t i = tid; i < g.slot4; i += stride) {
-      int from = g.from;
-      if (a.hops) {
-        const int done = min(max(a.hops[i / g.row4] - a.h0, 0), a.n);  // hops of this chunk the row ran
-        from -= a.n - done;
-        if (from < 0 || (from == 0 && (const float4 *)g.dst == g.src)) continue;
-      }
-      const float4 *src = g.src + (size_t)from * g.stride4;
-      for (int q = 0; q < g.n_slots; q++) g.dst[(size_t)q * g.stride4 + i] = src[(size_t)q * g.stride4 + i];
-    }
-  }
-  for (size_t i = tid; i < (size_t)a.n_cnt; i += stride) a.cnt[i] = 0u;
 }
 }  // namespace
 
@@ -487,14 +430,9 @@ int launch_gru_chain_f32(const F32ChainArgs &a, int rt, int sm_count, cudaStream
   }
   // the dependency waits need every block of the grid resident: never more blocks than fit at once
   int grid = occ * sm_count;
-  if (grid > a.n_units) grid = a.n_units;
+  if (grid > a.order.units()) grid = a.order.units();
   if (rt == 8) gru_chain_f32_kernel<8><<<grid, CH_THREADS, smem, st>>>(a);
   else gru_chain_f32_kernel<1><<<grid, CH_THREADS, smem, st>>>(a);
-  return 1;
-}
-
-int launch_f32_carry(const F32CarryArgs &a, cudaStream_t st) {
-  f32_carry_kernel<<<264, 256, 0, st>>>(a);  // two blocks per SM of an H100 SXM
   return 1;
 }
 
@@ -508,9 +446,8 @@ struct pnb_f32_state {
   struct { float *W = nullptr, *b = nullptr; } conv1, conv2, fc_gb, fc_rb;
   struct { float *W = nullptr, *U = nullptr, *b = nullptr; } gru[5];  // gru1..3, gru_gb, gru_rb
   // Hop-slot buffers of one chunk of at most chunk_hops(e) hops.  Slots 0.. of the fc / conv1 buffers hold the conv
-  // histories (oldest first), slot 0 of every GRU state buffer e->h[l][0] ([chunk+1][S][H]) the state before the
-  // chunk's first hop; the chunk's carry moves the last slots back there, so between calls the state lives at the front
-  // (par stays 0).
+  // histories (oldest first), slot 0 of every GRU state buffer e->h[l] ([chunk+1][S][H]) the state before the chunk's
+  // first hop; the chunk's carry moves the last slots back there, so between calls the state lives at the front.
   float *ring_fc = nullptr;  // [chunk+4][S][128] fc outputs: slots 0..3 the last four hops (oldest first), 4.. the chunk's
   float *ring_c1 = nullptr;  // [chunk+2][S][512] conv1 outputs, likewise
   float *c2_all = nullptr;   // [chunk][S][512] conv2 outputs of the chunk
@@ -553,7 +490,7 @@ int f32_prepare(pnb_engine *e, const pnb_model *model) {
   FCK(engine_alloc(e, &f.ring_fc, (C + 4) * S * 128, kStreamState));
   FCK(engine_alloc(e, &f.ring_c1, (C + 2) * S * 512, kStreamState));
   FCK(engine_alloc(e, &f.c2_all, C * S * 512, kScratch));
-  for (int i = 0; i < 5; i++) FCK(engine_alloc(e, &e->h[i][0], (C + 1) * S * kGruH[i], kStreamState));
+  for (int i = 0; i < 5; i++) FCK(engine_alloc(e, &e->h[i], (C + 1) * S * kGruH[i], kStreamState));
   FCK(engine_alloc(e, &f.cnt, (size_t)5 * f.rb, kStreamState));
   return PNB_OK;
 }
@@ -592,36 +529,22 @@ static int run_chunk(pnb_engine *e, int h0, int n, const int *hops, cudaStream_t
   F32ChainArgs a;
   memset(&a, 0, sizeof a);
   const int n_rb = (int)(((size_t)na + 16 * f.rt - 1) / (16 * f.rt));  // stream blocks of the active streams
-  a.S = S; a.n = na; a.n_rb = n_rb; a.cnt = f.cnt; a.tansig = tbl;
+  a.order = chain_order(n, n_rb, CH_HT, 1);
+  a.S = S; a.n = na; a.cnt = f.cnt; a.tansig = tbl;
   for (int li = 0; li < 5; li++) {
     F32ChainLayer &L = a.L[li];
     const int H = kGruH[li];
-    L.H = H; L.W = f.gru[li].W; L.U = f.gru[li].U; L.bias = f.gru[li].b; L.ldw = 3 * H; L.h = e->h[li][0];
+    L.H = H; L.W = f.gru[li].W; L.U = f.gru[li].U; L.bias = f.gru[li].b; L.ldw = 3 * H; L.h = e->h[li];
+    L.dep = chain_dep(li);
     if (li == 0) {          // gru1 <- conv2 out
-      L.n_x = 1; L.dep = -1; L.x[0] = f.c2_all; L.x_ld[0] = 512; L.x_K[0] = 512; L.x_slot1[0] = 0; L.x_slot_stride[0] = (size_t)S * 512;
+      L.n_x = 1; L.x[0] = f.c2_all; L.x_ld[0] = 512; L.x_K[0] = 512; L.x_slot1[0] = 0; L.x_slot_stride[0] = (size_t)S * 512;
     } else if (li < 4) {    // gru2 <- gru1, gru3 <- gru2, gru_gb <- gru3
-      L.n_x = 1; L.dep = li - 1; L.x[0] = e->h[li - 1][0]; L.x_ld[0] = 512; L.x_K[0] = 512; L.x_slot1[0] = 1; L.x_slot_stride[0] = (size_t)S * 512;
+      L.n_x = 1; L.x[0] = e->h[li - 1]; L.x_ld[0] = 512; L.x_K[0] = 512; L.x_slot1[0] = 1; L.x_slot_stride[0] = (size_t)S * 512;
     } else {                // gru_rb <- [gru3 state, conv2 out] (rnn.cpp:69-71)
-      L.n_x = 2; L.dep = 2;
-      L.x[0] = e->h[2][0]; L.x_ld[0] = 512; L.x_K[0] = 512; L.x_slot1[0] = 1; L.x_slot_stride[0] = (size_t)S * 512; L.w_row0[0] = 0;
+      L.n_x = 2;
+      L.x[0] = e->h[2]; L.x_ld[0] = 512; L.x_K[0] = 512; L.x_slot1[0] = 1; L.x_slot_stride[0] = (size_t)S * 512; L.w_row0[0] = 0;
       L.x[1] = f.c2_all;  L.x_ld[1] = 512; L.x_K[1] = 512; L.x_slot1[1] = 0; L.x_slot_stride[1] = (size_t)S * 512; L.w_row0[1] = 512;
     }
-  }
-  {
-    // anti-diagonal order: (t, l) sits on diagonal t + depth(l); everything it needs is on an earlier one
-    static const int depth[5] = {0, 1, 2, 3, 3};
-    int k = 0, unit = 0;
-    for (int d = 0; d < n + 3; d++)
-      for (int li = 0; li < 5; li++) {
-        const int t = d - depth[li];
-        if (t < 0 || t >= n) continue;
-        a.lh[k] = (unsigned char)((t << 3) | li);
-        a.lh_unit0[k] = unit;
-        unit += n_rb * (kGruH[li] / 32);
-        k++;
-      }
-    a.lh_unit0[k] = unit;
-    a.n_lh = k; a.n_units = unit;
   }
   {
     ProfScope ps(e, PNB_K_GEMM_F32, st);
@@ -631,28 +554,23 @@ static int run_chunk(pnb_engine *e, int h0, int n, const int *hops, cudaStream_t
   // fc_gb on [conv2, gru1, gru2, gru3, gru_gb] (rnn.cpp:73-78), fc_rb on gru_rb (rnn.cpp:80); state after hop t = slot t+1
   float *gr = e->d_gr + (size_t)h0 * S * 68;
   g.seg[0] = seg(f.c2_all, 512, f.fc_gb.W, 34, 512);
-  for (int q = 1; q < 5; q++) g.seg[q] = seg(e->h[q - 1][0] + (size_t)S * 512, 512, f.fc_gb.W + (size_t)q * 512 * 34, 34, 512);
+  for (int q = 1; q < 5; q++) g.seg[q] = seg(e->h[q - 1] + (size_t)S * 512, 512, f.fc_gb.W + (size_t)q * 512 * 34, 34, 512);
   g.n_seg = 5; g.N = 34; g.C = gr; g.ldc = 68; g.bias = f.fc_gb.b; g.act = PNB_ACT_SIGMOID;
   { ProfScope ps(e, PNB_K_GEMM_F32, st); nl += launch_gemm_f32(g, st); }
-  g.seg[0] = seg(e->h[4][0] + (size_t)S * 128, 128, f.fc_rb.W, 34, 128);
+  g.seg[0] = seg(e->h[4] + (size_t)S * 128, 128, f.fc_rb.W, 34, 128);
   g.n_seg = 1; g.N = 34; g.C = gr + 34; g.ldc = 68; g.bias = f.fc_rb.b; g.act = PNB_ACT_SIGMOID;
   { ProfScope ps(e, PNB_K_GEMM_F32, st); nl += launch_gemm_f32(g, st); }
-  // carry; in a ragged call a row that stopped inside the chunk takes its own last hop's slots, one that stopped in an
-  // earlier chunk keeps its front slots
-  F32CarryArgs c;
+  // carry: the last 4 fc / 2 conv1 slots and the last state slot move to the front, conv2's output of the last hop is
+  // kept for the tap.  In a ragged call a row that stopped inside the chunk takes its own last hop's slots, one that
+  // stopped in an earlier chunk keeps its front slots
+  SlotCarry c;
   memset(&c, 0, sizeof c);
-  int ns = 0;
-  auto cseg = [&](float *dst, const float *src, size_t width, int n_slots, int from) {  // the active rows of n_slots slots of [S][width]
-    c.seg[ns++] = F32CarrySeg{reinterpret_cast<float4 *>(dst), reinterpret_cast<const float4 *>(src), (size_t)na * width / 4,
-                              (size_t)S * width / 4, width / 4, n_slots, from};
-  };
-  cseg(f.ring_fc, f.ring_fc, 128, 4, n);
-  cseg(f.ring_c1, f.ring_c1, 512, 2, n);
-  for (int li = 0; li < 5; li++) cseg(e->h[li][0], e->h[li][0], kGruH[li], 1, n);
-  cseg(e->c2, f.c2_all, 512, 1, n - 1);
-  c.n_seg = ns; c.cnt = f.cnt; c.n_cnt = 5 * f.rb;
-  c.hops = hops; c.h0 = h0; c.n = n;
-  { ProfScope ps(e, PNB_K_F32_CARRY, st); nl += launch_f32_carry(c, st); }
+  c.hops = hops; c.h0 = h0; c.n = n; c.cnt = f.cnt; c.n_cnt = 5 * f.rb;
+  add_carry_seg(c, f.ring_fc, f.ring_fc, 128 * 4, na, S, 4, n);
+  add_carry_seg(c, f.ring_c1, f.ring_c1, 512 * 4, na, S, 2, n);
+  for (int li = 0; li < 5; li++) add_carry_seg(c, e->h[li], e->h[li], kGruH[li] * 4, na, S, 1, n);
+  add_carry_seg(c, e->c2, f.c2_all, 512 * 4, na, S, 1, n - 1);
+  { ProfScope ps(e, PNB_K_F32_CARRY, st); nl += launch_slot_carry(c, e->sm_count, st); }
   return nl;
 }
 

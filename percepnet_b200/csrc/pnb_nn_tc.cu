@@ -43,6 +43,7 @@
 #include <vector>
 
 #include "../../include/percepnet_b200.h"
+#include "pnb_chain.cuh"
 #include "pnb_engine.h"
 
 using namespace pnb;
@@ -90,14 +91,6 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap *map
       "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(x), "r"(y),
       "l"(0x1000000000000000ull)  // EVICT_NORMAL
       : "memory");
-}
-__device__ __forceinline__ unsigned ld_acquire_gpu(const unsigned *p) {
-  unsigned v;
-  asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-  return v;
-}
-__device__ __forceinline__ void red_release_gpu_add(unsigned *p, unsigned v) {
-  asm volatile("red.release.gpu.global.add.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
 }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async;" ::: "memory"); }
 
@@ -559,100 +552,29 @@ struct ChainLayer {
   int h_map, w_map, u_map;
   int h_kb;             // H / CBK
   int H;
-  int tiles_log2;       // log2(H / HT)
   int b_term_rows;      // rows of one term plane of the packed weights
-  int dep;              // layer whose output at the same hop is this layer's input (-1: produced before the launch)
-  int unit0;            // first unit of this layer inside a hop
-  int par0;             // which fp32 state buffer holds the state before hop 0
+  int dep;              // chain_dep of this layer
   float scale;          // 2^-(10 + weight scale)
   const float4 *bias4;  // per unit {b_z + b'_z, b_r + b'_r, b_n, b'_n}
-  float *h32[2];        // fp32 state, ping-pong by hop
+  float *h32;           // fp32 state [S][H], updated in place
   __half *h_hl;         // fp16 terms [2][(Fmax+1) S][H]
   int h_term_rows;      // (Fmax+1) S
 };
 struct ChainArgs {
   CUtensorMap maps[16];  // 0: conv2 out, 1..5: state slots of the five GRUs, 6..10: input weights, 11..15: recurrent weights
   ChainLayer L[5];
-  int S, F;              // rows per hop slot of the buffers; hops of the call
+  ChainOrder order;      // F hops of the row tiles of the active streams (128 streams each), 64-unit tiles
+  int S;                 // rows per hop slot of the buffers
   int n;                 // active streams: rows [0, n) of every slot
-  int tiles_mp;          // row tiles of the active streams (128 streams each)
-  int units_per_hop;
-  int diag;              // unit order: 0 = hop-major (layer by layer inside a hop), 1 = anti-diagonals (few streams)
   const int *hops;       // ragged calls: [n] hops of each row, or null.  Hop t of row r with t >= hops[r] is computed
-                         // but stores nothing: its last real state stays in the fp32 buffer of parity par0 + hops[r]
-  unsigned *cnt;         // [5][tiles_mp] consumer-warp completions, zero at launch
+                         // but stores nothing: the fp32 state keeps that of the row's last hop
+  unsigned *cnt;         // [5][order.n_rb] consumer-warp completions, zero at launch
   const float *tansig;
 };
 
-struct Unit { int t, l, mp, nt; };
-// Anti-diagonal unit order (small batches): (hop t, layer l) sits on diagonal t + depth(l), depth = 0,1,2,3,3 (gru_rb reads
-// gru3 like gru_gb does).  Everything a unit waits for lies on an earlier diagonal, and a diagonal holds up to five
-// layer-hops of mutually independent units -- with few streams one layer-hop alone cannot occupy the CTAs.
-__device__ __forceinline__ int diag_size(const ChainArgs &a, int d) {
-  int n = 0;
-#pragma unroll
-  for (int l = 0; l < 5; l++) {
-    const int t = d - (l < 4 ? l : 3);
-    n += (t >= 0 && t < a.F) ? (a.tiles_mp << a.L[l].tiles_log2) : 0;
-  }
-  return n;
-}
-__device__ __forceinline__ Unit decode_unit_diag(const ChainArgs &a, int u) {
-  int d = 0, r = u;
-  bool found = false;
-  for (; d < 3 && !found; d++) {  // ramp-up diagonals
-    const int sz = diag_size(a, d);
-    if (r < sz) { found = true; break; }
-    r -= sz;
-  }
-  if (!found && a.F > 3) {        // full diagonals 3 .. F-1 all hold units_per_hop units
-    const int q = r / a.units_per_hop;
-    if (q < a.F - 3) { d = 3 + q; r -= q * a.units_per_hop; found = true; }
-    else { r -= (a.F - 3) * a.units_per_hop; d = a.F; }
-  }
-  for (; !found; d++) {           // ramp-down diagonals
-    const int sz = diag_size(a, d);
-    if (r < sz) break;
-    r -= sz;
-  }
-  Unit x;
-  x.l = 0; x.t = 0;
-  bool hit = false;
-#pragma unroll
-  for (int l = 0; l < 5; l++) {
-    const int t = d - (l < 4 ? l : 3);
-    const int nl = (t >= 0 && t < a.F) ? (a.tiles_mp << a.L[l].tiles_log2) : 0;
-    if (!hit) {
-      if (r < nl) { x.l = l; x.t = t; hit = true; }
-      else r -= nl;
-    }
-  }
-  const int sh = a.L[x.l].tiles_log2;
-  x.mp = r >> sh;
-  x.nt = r & ((1 << sh) - 1);
-  return x;
-}
-__device__ __forceinline__ Unit decode_unit(const ChainArgs &a, int u) {
-  if (a.diag) return decode_unit_diag(a, u);
-  Unit x;
-  x.t = u / a.units_per_hop;
-  int r = u - x.t * a.units_per_hop;
-  x.l = 0;
-#pragma unroll
-  for (int i = 1; i < 5; i++) x.l = (r >= a.L[i].unit0) ? i : x.l;
-  r -= a.L[x.l].unit0;
-  const int sh = a.L[x.l].tiles_log2;
-  x.mp = r >> sh;
-  x.nt = r & ((1 << sh) - 1);
-  return x;
-}
 // all consumer warps of every tile of (layer, row tile) have finished `hops` hops
-__device__ __forceinline__ void wait_layer(const ChainArgs &a, int layer, int mp, int hops) {
-  const unsigned target = (unsigned)hops * kPubWarps << a.L[layer].tiles_log2;
-  const unsigned *p = a.cnt + layer * a.tiles_mp + mp;
-  unsigned spins = 0;
-  while (ld_acquire_gpu(p) < target)
-    if (++spins > (1u << 26)) __trap();  // tens of seconds: a broken schedule becomes a launch error, not a hang
+__device__ __forceinline__ void wait_layer(const ChainArgs &a, int layer, int rb, int hops) {
+  chain_wait(a.cnt + layer * a.order.n_rb + rb, (unsigned)hops * kPubWarps << a.order.tiles_log2[layer]);
 }
 
 constexpr int GRU_STAGES = 5;
@@ -734,7 +656,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) gru_chain_kernel(const __grid_c
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   const SmemCarve c = carve<STAGES, STAGES * SL::kBytes>(smem_raw);
   const int wg = threadIdx.x >> 7;
-  const int total_units = args.F * args.units_per_hop;
+  const int total_units = args.order.units();
   const int S = args.S;
   tc_prologue<STAGES>(c, args.tansig);
   const uint32_t stage0 = smem_u32(c.stages);
@@ -745,13 +667,13 @@ __global__ void __launch_bounds__(kTcThreads, 1) gru_chain_kernel(const __grid_c
     if (threadIdx.x != 0) return;
     Pipe p;
     for (int u = blockIdx.x; u < total_units; u += gridDim.x) {
-      const Unit un = decode_unit(args, u);
+      const ChainUnit un = chain_decode(args.order, u);
       const ChainLayer &L = args.L[un.l];
-      if (L.dep >= 0) wait_layer(args, L.dep, un.mp, un.t + 1);  // input: layer below, this hop
-      if (un.t > 0) wait_layer(args, un.l, un.mp, un.t);        // own state after the previous hop
+      if (L.dep >= 0) wait_layer(args, L.dep, un.rb, un.t + 1);  // input: layer below, this hop
+      if (un.t > 0) wait_layer(args, un.l, un.rb, un.t);        // own state after the previous hop
       fence_proxy_async();  // the rows were written with st.global by other SMs; TMA reads them through the async proxy
-      const int m0 = un.mp * TM;
-      const int brow = un.nt * GRU_BN;
+      const int m0 = un.rb * TM;
+      const int brow = un.tile * GRU_BN;
       for (int s = 0; s <= L.n_x; s++) {
         const bool rec = s == L.n_x;
         const CUtensorMap *ma = &args.maps[rec ? L.h_map : L.x_map[s]], *mb = &args.maps[rec ? L.u_map : L.w_map];
@@ -783,7 +705,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) gru_chain_kernel(const __grid_c
     Pipe p;
     Consumer<R> cons;
     for (int u = blockIdx.x; u < total_units; u += gridDim.x) {
-      const Unit un = decode_unit(args, u);
+      const ChainUnit un = chain_decode(args.order, u);
       const ChainLayer &L = args.L[un.l];
       const int H = L.H;
       float acc[R];  // no zero fill: the first k-block of either part starts its blocks' sums
@@ -800,24 +722,24 @@ __global__ void __launch_bounds__(kTcThreads, 1) gru_chain_kernel(const __grid_c
         gru_consume_kblock(acc, acc + NH, fa1, 1u, 1u, a_addr, b_lo0, c, p, cons);
       }
       cons.drain(acc);
-      // the previous hop's state of these rows is complete (other SMs wrote it): acquire before reading it
+      // the previous hop's state of these rows is complete (other SMs wrote it): acquire before reading it.  The fp32
+      // state is updated in place: this thread alone reads and writes these (row, unit) pairs at this hop, and whoever
+      // touches them at the next hop waits for this unit's counter bump first.
       if (un.t > 0) {
-        if (lane == 0) wait_layer(args, un.l, un.mp, un.t);
+        if (lane == 0) wait_layer(args, un.l, un.rb, un.t);
         __syncwarp();
       }
-      const int pold = (L.par0 + un.t) & 1;
       const float sc = L.scale;
 #pragma unroll
       for (int h = 0; h < 2; h++) {  // the thread's two rows of the fragment
-        const int row = un.mp * TM + cw * 64 + warp * 16 + (lane >> 2) + 8 * h;
+        const int row = un.rb * TM + cw * 64 + warp * 16 + (lane >> 2) + 8 * h;
         if (row >= args.n || (args.hops && un.t >= __ldg(args.hops + row))) continue;
-        const float *h_old = L.h32[pold] + (size_t)row * H;
-        float *h_new = L.h32[pold ^ 1] + (size_t)row * H;
+        float *h32 = L.h32 + (size_t)row * H;
         __half *ph = L.h_hl + ((size_t)(un.t + 1) * S + row) * H;
 #pragma unroll
         for (int j = 0; j < HT / 8; j++) {
-          const int unit = un.nt * HT + 8 * j + 2 * (lane & 3);
-          const float2 ho = __ldcg(reinterpret_cast<const float2 *>(h_old + unit));
+          const int unit = un.tile * HT + 8 * j + 2 * (lane & 3);
+          const float2 ho = __ldcg(reinterpret_cast<const float2 *>(h32 + unit));
           float hn[2];
 #pragma unroll
           for (int q = 0; q < 2; q++) {
@@ -831,7 +753,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) gru_chain_kernel(const __grid_c
             const float n = tansig_s(cnd, tbl);
             hn[q] = fmaf(z, (q ? ho.y : ho.x) - n, n);  // z h + (1 - z) n
           }
-          *reinterpret_cast<float2 *>(h_new + unit) = make_float2(hn[0], hn[1]);
+          *reinterpret_cast<float2 *>(h32 + unit) = make_float2(hn[0], hn[1]);
           store_split_h2(hn[0], hn[1], ph + unit, ph + (size_t)L.h_term_rows * H + unit);
         }
       }
@@ -839,7 +761,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) gru_chain_kernel(const __grid_c
       __syncwarp();
       if (lane == 0) {
         __threadfence();
-        red_release_gpu_add(args.cnt + un.l * args.tiles_mp + un.mp, 1u);
+        red_release_gpu_add(args.cnt + un.l * args.order.n_rb + un.rb, 1u);
       }
     }
   }
@@ -908,33 +830,6 @@ __global__ void __launch_bounds__(128) fc_split_kernel(const float *__restrict__
     size_t o = (size_t)(r0 + rr) * 128 + n;
     out[o] = t0; out[plane + o] = t1; out[2 * plane + o] = t2;
   }
-}
-
-// End-of-call bookkeeping in one launch: the hop slots the next call reads first (last 4 fc / 2 conv1 outputs,
-// last GRU states) move to the front of their buffers, and the chain's dependency counters return to zero.  Only the
-// active streams' rows move: they are the first rows of every slot.
-// A segment shifts `n_slots` slots down by `shift` slots (in a ragged call, the row's own hops: the slots of its last
-// hop).  One thread owns the same element of every slot and walks the slots in ascending order, so a slot that is both
-// source and destination (shift < n_slots) is read before it is overwritten -- by the same thread, no cross-thread
-// ordering needed.
-struct CarrySeg { uint4 *base; size_t slot16, stride16, row16; int n_slots, shift; };  // the first slot16 of each stride16; row16 per row
-struct CarryArgs {
-  CarrySeg seg[16];
-  int n_seg;
-  unsigned *cnt;
-  int n_cnt;
-  const int *hops;  // ragged calls: [active streams] hops of each row, or null
-};
-__global__ void __launch_bounds__(256) tc_carry_kernel(const __grid_constant__ CarryArgs a) {
-  const size_t tid = (size_t)blockIdx.x * blockDim.x + threadIdx.x, nth = (size_t)gridDim.x * blockDim.x;
-  for (int s = 0; s < a.n_seg; s++) {
-    const CarrySeg sg = a.seg[s];
-    for (size_t i = tid; i < sg.slot16; i += nth) {
-      const int shift = a.hops ? a.hops[i / sg.row16] : sg.shift;
-      for (int k = 0; k < sg.n_slots; k++) sg.base[(size_t)k * sg.stride16 + i] = sg.base[(size_t)(k + shift) * sg.stride16 + i];
-    }
-  }
-  for (size_t i = tid; i < (size_t)a.n_cnt; i += nth) a.cnt[i] = 0u;
 }
 
 }  // namespace
@@ -1103,8 +998,7 @@ int tc_prepare(pnb_engine *e, const pnb_model *model) {
   pnb_tc_state *t = e->tc.get();
   const size_t S = e->S;
   const size_t Fm = e->Fmax;
-  for (int i = 0; i < 5; i++)
-    for (int p = 0; p < 2; p++) TCK(engine_alloc(e, &e->h[i][p], S * kGruH[i], kStreamState));
+  for (int i = 0; i < 5; i++) TCK(engine_alloc(e, &e->h[i], S * kGruH[i], kStreamState));
   TCK(engine_alloc(e, &t->fc_all, kConvTerms * (Fm + 4) * S * 128, kStreamState));
   TCK(engine_alloc(e, &t->c1_all, kConvTerms * (Fm + 2) * S * 512, kStreamState));
   {
@@ -1304,7 +1198,7 @@ static int tc_front(pnb_engine *e, int F, const int *hops, cudaStream_t st) {
 }
 
 // The recurrent part: five GRUs per hop (rnn.cpp:58-71) in one persistent launch.  State slot t holds the state
-// BEFORE hop t of the call; the fp32 state ping-pongs by hop, starting from e->par (the call's first hop).
+// BEFORE hop t of the call; the fp32 state e->h is updated in place.
 static int tc_gru_chain(pnb_engine *e, int F, const int *hops, cudaStream_t st) {
   pnb_tc_state *t = e->tc.get();
   const int S = e->S, Fm = e->Fmax;
@@ -1312,42 +1206,39 @@ static int tc_gru_chain(pnb_engine *e, int F, const int *hops, cudaStream_t st) 
   memset(&a, 0, sizeof a);
   a.maps[0] = t->m_c2_ch;
   for (int i = 0; i < 5; i++) { a.maps[1 + i] = t->m_h_ch[i]; a.maps[6 + i] = t->m_w[i]; a.maps[11 + i] = t->m_u[i]; }
-  // only the active streams' row tiles are units; the counters of the others stay zero
-  a.S = S; a.n = e->n_active; a.F = F; a.tiles_mp = (e->n_active + TM - 1) / TM; a.cnt = t->cnt; a.tansig = e->tansig();
+  // only the active streams' row tiles are units; the counters of the others stay zero.  With many streams one
+  // layer-hop fills the machine and hop-major order keeps a layer's fresh output in L2 for the layer above; with few,
+  // only the anti-diagonal order exposes enough independent units
+  const int tiles_mp = (e->n_active + TM - 1) / TM;
+  a.order = chain_order(F, tiles_mp, HT, (tiles_mp * (512 / HT) < e->sm_count) ? 1 : 0);
+  a.S = S; a.n = e->n_active; a.cnt = t->cnt; a.tansig = e->tansig();
   a.hops = hops;
   const int c2_terms = Fm * S, h_terms = (Fm + 1) * S;
-  int unit0 = 0;
   for (int li = 0; li < 5; li++) {
     ChainLayer &L = a.L[li];
     const int H = kGruH[li], tiles = H / HT;
-    L.H = H; L.h_kb = H / CBK; L.tiles_log2 = __builtin_ctz(tiles);
+    L.H = H; L.h_kb = H / CBK;
     L.b_term_rows = tiles * GRU_BN;
     L.h_map = 1 + li; L.w_map = 6 + li; L.u_map = 11 + li;
-    L.unit0 = unit0; unit0 += a.tiles_mp * tiles;
-    L.par0 = e->par[li];
+    L.dep = chain_dep(li);
     L.scale = t->scale_gru[li];
     L.bias4 = t->bias4[li];
-    L.h32[0] = e->h[li][0]; L.h32[1] = e->h[li][1];
+    L.h32 = e->h[li];
     L.h_hl = t->h_all[li]; L.h_term_rows = h_terms;
     // each GRU consumes the freshly written state (slot t+1) of the layer below (rnn.cpp:58-71, SURVEY.md App. C.10)
     if (li == 0) {          // gru1 <- conv2 out
-      L.n_x = 1; L.x_map[0] = 0; L.x_kb[0] = 512 / CBK; L.x_bk0[0] = 0; L.x_row1[0] = 0; L.x_term_rows[0] = c2_terms; L.dep = -1;
+      L.n_x = 1; L.x_map[0] = 0; L.x_kb[0] = 512 / CBK; L.x_bk0[0] = 0; L.x_row1[0] = 0; L.x_term_rows[0] = c2_terms;
     } else if (li < 4) {    // gru2 <- gru1, gru3 <- gru2, gru_gb <- gru3
-      L.n_x = 1; L.x_map[0] = li; L.x_kb[0] = 512 / CBK; L.x_bk0[0] = 0; L.x_row1[0] = 1; L.x_term_rows[0] = h_terms; L.dep = li - 1;
+      L.n_x = 1; L.x_map[0] = li; L.x_kb[0] = 512 / CBK; L.x_bk0[0] = 0; L.x_row1[0] = 1; L.x_term_rows[0] = h_terms;
     } else {                // gru_rb <- [gru3 state, conv2 out]
       L.n_x = 2;
       L.x_map[0] = 3; L.x_kb[0] = 512 / CBK; L.x_bk0[0] = 0; L.x_row1[0] = 1; L.x_term_rows[0] = h_terms;
       L.x_map[1] = 0; L.x_kb[1] = 512 / CBK; L.x_bk0[1] = 512; L.x_row1[1] = 0; L.x_term_rows[1] = c2_terms;
-      L.dep = 2;
     }
   }
-  a.units_per_hop = unit0;
-  // with many streams one layer-hop fills the machine and hop-major order keeps a layer's fresh output in L2 for the
-  // layer above; with few, only the anti-diagonal order exposes enough independent units
-  a.diag = (a.tiles_mp * (512 / HT) < e->sm_count) ? 1 : 0;
   {
     ProfScope ps(e, PNB_K_TC_GEMM, st);
-    int rc = tc_launch(e, gru_chain_kernel, a, F * unit0, tc_smem_bytes<GRU_STAGES, GRU_STAGES * GruStage::kBytes>(), st);
+    int rc = tc_launch(e, gru_chain_kernel, a, a.order.units(), tc_smem_bytes<GRU_STAGES, GRU_STAGES * GruStage::kBytes>(), st);
     if (rc) return rc;
   }
   return 1;
@@ -1389,38 +1280,25 @@ static int tc_out(pnb_engine *e, int F, const int *, cudaStream_t st) {
 }
 
 // End of a call of F hops: the last 4 fc / 2 conv1 hop slots and the last state slot move to the front (in a ragged
-// call those of each row's own last hop), the chain's dependency counters return to zero (one launch), and the fp32
-// state parity advances by F.  A ragged call's rows that stopped early hold their fp32 state at parity par0 + hops:
-// the call's fix-up moves it (pnb_state.cu, ragged_carry_kernel).
+// call those of each row's own last hop), and the chain's dependency counters return to zero, in one launch.
 static int tc_carry(pnb_engine *e, int F, const int *hops, cudaStream_t st) {
   pnb_tc_state *t = e->tc.get();
   const int S = e->S, Fm = e->Fmax, na = e->n_active;
-  const int h_terms = (Fm + 1) * S;
-  CarryArgs ca;
-  memset(&ca, 0, sizeof ca);
-  ca.cnt = t->cnt; ca.n_cnt = 5 * t->tiles_mp; ca.hops = hops;
-  int ns = 0;
+  SlotCarry c;
+  memset(&c, 0, sizeof c);
+  c.hops = hops; c.h0 = 0; c.n = F; c.cnt = t->cnt; c.n_cnt = 5 * t->tiles_mp;
   for (int tm = 0; tm < kConvTerms; tm++) {
-    __nv_bfloat16 *bf = t->fc_all + (size_t)tm * (Fm + 4) * S * 128;
-    __nv_bfloat16 *bc = t->c1_all + (size_t)tm * (Fm + 2) * S * 512;
-    ca.seg[ns++] = CarrySeg{reinterpret_cast<uint4 *>(bf), (size_t)na * 128 * 2 / 16, (size_t)S * 128 * 2 / 16, 128 * 2 / 16, 4, F};
-    ca.seg[ns++] = CarrySeg{reinterpret_cast<uint4 *>(bc), (size_t)na * 512 * 2 / 16, (size_t)S * 512 * 2 / 16, 512 * 2 / 16, 2, F};
+    __nv_bfloat16 *bf = t->fc_all + (size_t)tm * (Fm + 4) * S * 128, *bc = t->c1_all + (size_t)tm * (Fm + 2) * S * 512;
+    add_carry_seg(c, bf, bf, 128 * 2, na, S, 4, F);
+    add_carry_seg(c, bc, bc, 512 * 2, na, S, 2, F);
   }
-  for (int li = 0; li < 5; li++) {
-    const size_t H = kGruH[li];
+  for (int li = 0; li < 5; li++)
     for (int tm = 0; tm < 2; tm++) {
-      __half *base = t->h_all[li] + (size_t)tm * h_terms * H;
-      ca.seg[ns++] = CarrySeg{reinterpret_cast<uint4 *>(base), (size_t)na * H * 2 / 16, (size_t)S * H * 2 / 16, H * 2 / 16, 1, F};
+      __half *b = t->h_all[li] + (size_t)tm * (Fm + 1) * S * kGruH[li];
+      add_carry_seg(c, b, b, kGruH[li] * 2, na, S, 1, F);
     }
-  }
-  ca.n_seg = ns;
-  {
-    ProfScope ps(e, PNB_K_TC_AUX, st);
-    tc_carry_kernel<<<2 * e->sm_count, 256, 0, st>>>(ca);
-  }
-  if (F & 1)
-    for (int li = 0; li < 5; li++) e->par[li] ^= 1;
-  return 1;
+  ProfScope ps(e, PNB_K_TC_AUX, st);
+  return launch_slot_carry(c, e->sm_count, st);
 }
 
 int tc_network(pnb_engine *e, int F, const int *hops, cudaStream_t st) {

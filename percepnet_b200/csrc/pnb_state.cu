@@ -3,7 +3,9 @@
 // in an engine (state_segs, which takes the network path's own pieces from tc_state_segs / f32_state_segs).
 // pnb_get_state / pnb_set_state are the n = 1 case of the same kernels.  The session pool
 // (pnb_process_sessions_*) parks, unparks and relocates sessions with the same pieces (session_move_kernel) and keeps
-// its parking blobs with session_blob_kernel.
+// its parking blobs with session_blob_kernel.  The carries that put the state back in place after a call are here
+// too: the network paths' end-of-chunk carry of their hop-slot buffers (slot_carry_kernel) and a ragged call's fix-up
+// of the pieces that follow the engine's counters (ragged_carry_kernel).
 //
 // A stream's state is a list of pieces (StateSeg): the history line at line_off, the overlap-add memory, pitch
 // continuity, the five live spectrum ring slots, and the network's conv histories and GRU states (fp32, or the tensor
@@ -245,8 +247,8 @@ __global__ void gr_gather_kernel(const float *__restrict__ src, float *__restric
   }
 }
 
-// The pieces of a slot's state that move with the engine's counters (see state_segs): the history window at line_off,
-// the five live spectrum ring slots at hop, and (tensor path) the fp32 GRU states at parity par.
+// The pieces of a slot's state that move with the engine's counters (see state_segs): the history window at line_off
+// and the five live spectrum ring slots at hop.
 struct RaggedArgs {
   float *pcm;
   size_t pcm_stride, line_off;  // the call's window: line_off + h * 480 after h hops
@@ -254,9 +256,6 @@ struct RaggedArgs {
   float *ering;                 // [ring][S][34]
   int ring, S, F;
   long hop0;                    // hop counter at the call's start
-  int n_gru;                    // 5 on tensor engines (ping-pong fp32 states), 0 on fp32 engines (states carried by slot)
-  float *h[5][2];
-  int H[5], par[5];             // parity after the call
   const int *hops, *slots;      // [S] hops per slot; [gridDim.x] the slots that stopped early
 };
 
@@ -299,13 +298,24 @@ __global__ void __launch_bounds__(kRaggedThreads) ragged_carry_kernel(const __gr
         }
       }
   }
-  if (d & 1)
-    for (int li = 0; li < a.n_gru; li++) {
-      const size_t H = a.H[li];
-      const float *src = a.h[li][a.par[li] ^ 1] + (size_t)p * H;
-      float *dst = a.h[li][a.par[li]] + (size_t)p * H;
-      for (unsigned k = tid; k < H; k += kRaggedThreads) dst[k] = src[k];
+}
+
+__global__ void __launch_bounds__(256) slot_carry_kernel(const __grid_constant__ SlotCarry a) {
+  const size_t tid = (size_t)blockIdx.x * blockDim.x + threadIdx.x, nth = (size_t)gridDim.x * blockDim.x;
+  for (int s = 0; s < a.n_seg; s++) {
+    const SlotSeg g = a.seg[s];
+    for (size_t i = tid; i < g.slot; i += nth) {
+      int from = g.from;
+      if (a.hops) {
+        const int done = min(max(a.hops[i / g.row] - a.h0, 0), a.n);  // hops of this chunk the row ran
+        from -= a.n - done;
+        if (from < 0 || (from == 0 && g.dst == g.src)) continue;
+      }
+      const uint4 *src = g.src + (size_t)from * g.stride;
+      for (int q = 0; q < g.n_slots; q++) g.dst[(size_t)q * g.stride + i] = src[(size_t)q * g.stride + i];
     }
+  }
+  for (size_t i = tid; i < (size_t)a.n_cnt; i += nth) a.cnt[i] = 0u;
 }
 
 __global__ void state_clear_reject_kernel(int *status) {
@@ -335,11 +345,11 @@ int state_segs(const pnb_engine *e, StateSeg *seg) {
     add_words(seg, ns, kSegBlobZero, nullptr, 0, offsetof(StreamState, fc_terms), (sizeof(StreamState) - offsetof(StreamState, fc_terms)) / 4);
     return ns;
   }
-  // GRU states in fp32 (both paths), at the parity the next call starts from
+  // GRU states in fp32 (both paths)
   size_t off = 0;
   for (int li = 0; li < 5; li++) {
     const size_t H = kGruH[li];
-    add_words(seg, ns, kSegCopy, e->h[li][e->par[li]], H * 4, offsetof(StreamState, h) + off * 4, H);
+    add_words(seg, ns, kSegCopy, e->h[li], H * 4, offsetof(StreamState, h) + off * 4, H);
     off += H;
   }
   add_words(seg, ns, kSegEngZero, e->c2, 512 * 4, 0, 512);  // the conv2 tap (PNB_TAP_NN_C2) of a fresh stream
@@ -371,20 +381,18 @@ int launch_gr_gather(const float *src, float *dst, const int *row, int k, int S,
   return 1;
 }
 
-// Beside state_segs: the same places, at the counters of the call's start (history, ring) and end (GRU parity).
+// Beside state_segs: the same places, at the counters of the call's start.
 int launch_ragged_carry(const pnb_engine *e, int F, const int *d_hops, const int *d_slots, int n, cudaStream_t st) {
   RaggedArgs a;
   memset(&a, 0, sizeof a);
   a.pcm = e->d_pcm; a.pcm_stride = e->pcm_stride; a.line_off = e->line_off;
   a.zring = e->d_zring; a.ering = e->d_ering; a.ring = e->ring; a.S = e->S; a.F = F; a.hop0 = e->hop;
-  if (e->flags & PNB_NN_TENSOR) {
-    a.n_gru = 5;
-    for (int li = 0; li < 5; li++) {
-      a.h[li][0] = e->h[li][0]; a.h[li][1] = e->h[li][1]; a.H[li] = kGruH[li]; a.par[li] = e->par[li];
-    }
-  }
   a.hops = d_hops; a.slots = d_slots;
   ragged_carry_kernel<<<n, kRaggedThreads, 0, st>>>(a);
+  return 1;
+}
+int launch_slot_carry(const SlotCarry &c, int sm_count, cudaStream_t st) {
+  slot_carry_kernel<<<2 * sm_count, 256, 0, st>>>(c);
   return 1;
 }
 int launch_state_clear_reject(int *status, cudaStream_t st) {

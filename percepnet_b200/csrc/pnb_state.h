@@ -101,8 +101,8 @@ struct StateArgs {
 constexpr int kStatusRejected = 2;
 constexpr int kNoRejectedSlot = 0x7F7F7F7F;  // status[1] when nothing was rejected (a byte-wise memset can write it)
 
-// The pieces of a stream's state in engine e at its current hop / line offset / GRU parity (host counters committed
-// when a call is enqueued, so the list is right in stream order); returns their number (<= kMaxStateSegs).
+// The pieces of a stream's state in engine e at its current hop / line offset (host counters committed when a call is
+// enqueued, so the list is right in stream order); returns their number (<= kMaxStateSegs).
 int state_segs(const pnb_engine *e, StateSeg *seg);
 int launch_state_check(const StateArgs &a, cudaStream_t st);
 int launch_state_move(const StateArgs &a, cudaStream_t st);
@@ -115,10 +115,33 @@ int launch_session_blob(const StateArgs &a, cudaStream_t st);
 int launch_gr_gather(const float *src, float *dst, const int *row, int k, int S, int F, cudaStream_t st,
                      const int *hops = nullptr);
 // The fix-up of a ragged session call (pnb_process_sessions_ragged_*), enqueued after synthesis and before the history
-// slide, with the engine's hop counter and line offset still those of the call's start and its GRU parity already that
-// of its end.  The n slots at d_slots stopped after hops[p] < F hops; the pieces of their state that sit where the
-// counters say (state_segs) move from where hop hops[p] left them to where hop F would have put them.  One launch.
+// slide, with the engine's hop counter and line offset still those of the call's start.  The n slots at d_slots stopped
+// after hops[p] < F hops; the pieces of their state that sit where the counters say (state_segs) move from where hop
+// hops[p] left them to where hop F would have put them.  One launch.
 int launch_ragged_carry(const pnb_engine *e, int F, const int *d_hops, const int *d_slots, int n, cudaStream_t st);
+
+// The carry at the end of a network chunk of n hops (hops [h0, h0 + n) of the call), both network paths: the hop slots
+// the next chunk reads first move to the front of their buffers, and the chain's counters return to zero.  Segment g
+// moves the first `slot` 16-byte words of n_slots slots, `stride` words apart, from slots from.. of src to slots 0.. of
+// dst.  In a ragged call a row (`row` words) that stopped after hop hops[row] takes its slots from
+// from - (n - clamp(hops[row] - h0, 0, n)) on instead, and nothing moves when that is below 0 or the row is already in
+// place.  A thread owns the same word of every slot and walks the slots upwards, so a slot that is both source and
+// destination is read before it is overwritten.
+struct SlotSeg { uint4 *dst; const uint4 *src; size_t slot, stride, row; int n_slots, from; };
+struct SlotCarry {
+  SlotSeg seg[16];
+  int n_seg;
+  const int *hops;  // [active streams] hops of each row in a ragged call, or null
+  int h0, n;
+  unsigned *cnt;    // [n_cnt] counters to zero
+  int n_cnt;
+};
+// Appends the segment of the first n_rows rows (row_bytes each, a multiple of 16) of n_slots slots of S rows
+inline void add_carry_seg(SlotCarry &c, void *dst, const void *src, size_t row_bytes, int n_rows, int S, int n_slots, int from) {
+  c.seg[c.n_seg++] = SlotSeg{static_cast<uint4 *>(dst), static_cast<const uint4 *>(src), n_rows * row_bytes / 16,
+                             S * row_bytes / 16, row_bytes / 16, n_slots, from};
+}
+int launch_slot_carry(const SlotCarry &c, int sm_count, cudaStream_t st);
 // Parking blobs are engine-owned: padded to 16 bytes
 constexpr size_t kParkStride = (sizeof(StreamState) + 15) / 16 * 16;
 

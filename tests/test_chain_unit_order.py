@@ -1,16 +1,17 @@
 """The persistent GRU chain kernels walk their units in an order in which everything a unit waits for has a smaller
-index (round-robin over co-resident blocks then cannot deadlock).  This restates the two orders the kernels use --
-hop-major and anti-diagonal (pnb_nn_tc.cu decode_unit / decode_unit_diag, pnb_nn_f32.cu run_chunk's table) -- and checks
-the property, the coverage (every unit exactly once) and the closed-form decode against the table."""
+index (round-robin over co-resident blocks then cannot deadlock).  Both chains take the order from ChainOrder
+(pnb_chain.cuh): hop-major, or anti-diagonal, which the fp32 chain always uses.  This defines the anti-diagonal order
+as a table, restates the closed-form decode both kernels run (chain_decode_diag) and checks the property, the coverage
+(every unit exactly once) and the decode against the table; and it checks the property for the hop-major order."""
 import itertools
 
 import pytest
 
-DEPTH = (0, 1, 2, 3, 3)          # gru1, gru2, gru3, gru_gb, gru_rb (gru_rb reads gru3 like gru_gb does)
-DEP = (-1, 0, 1, 2, 2)           # layer whose fresh state is a layer's input (-1: conv2 output, ready before the launch)
+DEP = (-1, 0, 1, 2, 2)           # chain_dep: layer whose fresh state is a layer's input (-1: conv2 output, ready before the launch)
+DEPTH = tuple(d + 1 for d in DEP)  # (0, 1, 2, 3, 3) for gru1, gru2, gru3, gru_gb, gru_rb (gru_rb reads gru3 like gru_gb does)
 
 
-def diag_table(n_hops, units):   # run_chunk: entries (t, l) sorted by diagonal, then layer
+def diag_table(n_hops, units):   # the definition: entries (t, l) sorted by diagonal, then layer
     order = []
     for d in range(n_hops + 3):
         for l in range(5):
@@ -24,7 +25,7 @@ def diag_table(n_hops, units):   # run_chunk: entries (t, l) sorted by diagonal,
     return order, first, u
 
 
-def decode_diag_closed_form(u, n_hops, units):   # decode_unit_diag
+def decode_diag_closed_form(u, n_hops, units):   # chain_decode_diag
     per_hop = sum(units)
 
     def size(d):

@@ -159,6 +159,34 @@ int pnb_train_records_device(pnb_engine *e, const short *d_speech, size_t speech
                              size_t noisy_stride, int n_frames, float *d_records, size_t records_stride,
                              void *cuda_stream);
 
+/* The network alone: the batched compute_rnn (src/rnnoise.h:68, src/rnn.cpp:42) on caller-supplied inputs, to score a
+ * model on features or training records exactly as the engine runs it.
+ *   format       PNB_RNN_FEATURES: 70 floats per hop, the network input as create_features makes it
+ *                (src/denoise.cpp:487-496, = PNB_TAP_FEATURES).  PNB_RNN_RECORDS: 138 floats per hop, a record of
+ *                train() / pnb_train_records_*; the device takes features = {30*rec[0..67], rec[68], rec[69]} (one fp32
+ *                multiply, as create_features and rnn_train.py's CppRawListDataset scale them) and ignores the labels
+ *                rec[70..137].
+ *   in / d_in    the active rows [0, n) (n = pnb_active_streams(e)), stream-major: row i holds n_frames consecutive hops,
+ *                at in + i*in_stride, in_stride >= n_frames * (70 or 138) floats.
+ *   gr / d_gr    row i receives n_frames x 68 floats (34 g then 34 r per hop) at gr + i*gr_stride, gr_stride >=
+ *                n_frames*68.  Unlike the [n_frames][n][68] g/r of pnb_process_*, hop t of row i lines up with the
+ *                labels rec[t][70..137] of the same record row.
+ * A call advances the network state of every active slot (conv histories, GRU states, conv2 output) by n_frames hops,
+ * computing compute_rnn once per hop in order, exactly as a pnb_process_* call does after its analysis.  It does not
+ * touch the slot's signal state (history, overlap-add memory, pitch memory, spectra), so between two pnb_process_*
+ * calls it is the batched compute_rnn(&st->rnn, ...) on a DenoiseState between two frames.  PNB_TAP_FEATURES and
+ * PNB_TAP_GR read the call; the other per-frame taps are unspecified after it.  Ordering and blocking are those of
+ * pnb_process_device_* / pnb_process_host_*; on a PNB_NN_TENSOR engine, features that drive a pre-activation out of the
+ * domain raise PNB_ERR_DOMAIN the same way (features are not otherwise validated).  Refused with PNB_ERR_ARG before
+ * anything is enqueued: NULL pointers, format not 0 or 1, n_frames outside [1, max_frames], short strides, a
+ * PNB_TRAIN_DATA engine, an engine in session mode; a poisoned engine returns PNB_ERR_CUDA.  A call issues the
+ * network's launches plus two. */
+enum { PNB_RNN_FEATURES = 0, PNB_RNN_RECORDS = 1 };
+int pnb_compute_rnn_device(pnb_engine *e, int format, const float *d_in, size_t in_stride, int n_frames,
+                           float *d_gr, size_t gr_stride, void *cuda_stream);
+int pnb_compute_rnn_host(pnb_engine *e, int format, const float *in, size_t in_stride, int n_frames,
+                         float *gr, size_t gr_stride);
+
 /* Per-stream state for migration between engines / GPUs (the live part of the reference's DenoiseState + RNNState,
  * src/denoise.cpp:71-85, src/nnet_data.h:28-38): input history, overlap-add memory, pitch continuity, the spectra the
  * next five hops will analyse, conv histories and GRU states -- pnb_state_size() bytes, a flat host blob.

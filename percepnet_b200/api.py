@@ -20,6 +20,7 @@ LIB_PATH = os.path.join(HERE, "libpercepnet_b200.so")
 FRAME = 480
 NN_FP32, NN_TENSOR, POSTFILTER, KEEP_TAPS, TRAIN_DATA, CONV_WIDE = 0, 1, 2, 4, 8, 16
 RECORD = 138
+RNN_FEATURES, RNN_RECORDS = 0, 1   # pnb_compute_rnn_* formats: 70 features or 138 record floats per hop
 TAPS = {"features": (0, np.float32, 70), "pitch": (1, np.int32, 4), "pitchf": (2, np.float32, 2),
         "X": (3, np.float32, 800), "P": (4, np.float32, 800), "Ex": (5, np.float32, 34), "gr": (6, np.float32, 68),
         "g_used": (13, np.float32, 34)}
@@ -60,6 +61,8 @@ def load_library() -> C.CDLL:
     L.pnb_submit_host_i16.argtypes = [vp, vp, sz, vp, sz, i]
     L.pnb_submit_device_f32.argtypes = [vp, vp, sz, vp, sz, i, vp]
     L.pnb_submit_device_i16.argtypes = [vp, vp, sz, vp, sz, i, vp]
+    L.pnb_compute_rnn_device.argtypes = [vp, i, vp, sz, i, vp, sz, vp]
+    L.pnb_compute_rnn_host.argtypes = [vp, i, vp, sz, i, vp, sz]
     L.pnb_flush.argtypes = [vp, vp]
     L.pnb_wait.argtypes = [vp]
     L.pnb_check.argtypes = [vp, vp]
@@ -105,6 +108,7 @@ def load_library() -> C.CDLL:
 
 EXPORTS = ("pnb_create", "pnb_destroy", "pnb_reset", "pnb_resolve_device", "pnb_process_host_f32", "pnb_process_host_i16",
            "pnb_model_load_blob", "pnb_model_load_stream", "pnb_model_free", "pnb_train_records_host", "pnb_train_records_device", "pnb_submit_train_records", "pnb_process_device_f32", "pnb_process_device_i16", "pnb_submit_host_f32", "pnb_submit_host_i16", "pnb_submit_device_f32", "pnb_submit_device_i16", "pnb_flush", "pnb_wait", "pnb_check",
+           "pnb_compute_rnn_device", "pnb_compute_rnn_host",
            "pnb_read_tap", "pnb_state_size", "pnb_get_state", "pnb_set_state",
            "pnb_reset_streams", "pnb_export_states", "pnb_import_states", "pnb_set_active_streams", "pnb_active_streams",
            "pnb_sessions_reserve", "pnb_process_sessions_device_f32", "pnb_process_sessions_device_i16",
@@ -239,6 +243,29 @@ class Engine:
         """pnb_submit_device_*: process_device without g/r; flush(other_stream) or wait() orders other work behind it."""
         f = self.L.pnb_submit_device_i16 if int16 else self.L.pnb_submit_device_f32
         self._ck(f(self.h, d_in, in_stride, d_out, out_stride, n_frames, stream or None), "pnb_submit_device")
+
+    def compute_rnn(self, x: np.ndarray) -> np.ndarray:
+        """pnb_compute_rnn_host: the network alone.  x: [active, F, 70] float32 features (as create_features makes them)
+        or [active, F, 138] float32 training records (scaled x30 on the device like rnn_train.py's CppRawListDataset;
+        the labels are ignored); the last dimension selects the format.  Advances the slots' network state by F hops
+        and leaves their signal state alone.  Returns g/r [active, F, 68], hop t of row i beside record t's labels."""
+        n = self.active
+        if x.dtype != np.float32:
+            raise TypeError("x must be float32")
+        assert x.ndim == 3 and x.shape[0] == n and x.shape[2] in (70, RECORD), "x must be [active, F, 70 | 138]"
+        F, W = x.shape[1], x.shape[2]
+        x = np.ascontiguousarray(x)
+        gr = np.empty((n, F, 68), np.float32)
+        fmt = RNN_FEATURES if W == 70 else RNN_RECORDS
+        self._ck(self.L.pnb_compute_rnn_host(self.h, fmt, x.ctypes.data, F * W, F, gr.ctypes.data, F * 68),
+                 "pnb_compute_rnn_host")
+        return gr
+
+    def compute_rnn_device(self, format: int, d_in: int, in_stride: int, n_frames: int, d_gr: int, gr_stride: int,
+                           stream: int = 0):
+        """pnb_compute_rnn_device on raw device pointers (format RNN_FEATURES or RNN_RECORDS; strides in floats)."""
+        self._ck(self.L.pnb_compute_rnn_device(self.h, format, d_in or None, in_stride, n_frames, d_gr or None, gr_stride,
+                                               stream or None), "pnb_compute_rnn_device")
 
     def flush(self, stream: int = 0):
         self._ck(self.L.pnb_flush(self.h, stream or None), "pnb_flush")

@@ -25,6 +25,7 @@ SOURCES = {
     "pnb_nn_tc.cu": [],
     "pnb_engine.cu": [],
     "pnb_state.cu": [],
+    "pnb_rnn_io.cu": [],
 }
 
 

@@ -4,7 +4,9 @@
 // Schedule of one pnb_process_* call with F hops on S streams:
 //   stage_in -> analysis (all F hops; one warp per stream) -> F x network step -> synthesis -> slide history
 // The network step is the only part that is sequential in time across the batch; analysis and synthesis
-// need no network state, so hops are processed F at a time.
+// need no network state, so hops are processed F at a time.  A network-only call (pnb_compute_rnn_*) is
+//   features_stage -> F x network step -> gr_store
+// on caller-supplied features or training records.
 #include <math.h>
 #include <stdarg.h>
 #include <stdio.h>
@@ -423,8 +425,9 @@ static int mark_call_end(pnb_engine *e, cudaStream_t st) {
 
 // What every call checks before it allocates or enqueues anything: an engine of the call's family (training records
 // or enhancement) that no failed call has poisoned, 1 <= F <= Fmax, its buffers (`buffers`: none is NULL), and two
-// row strides of at least F hops.
-static int check_call(const pnb_engine *e, bool train, bool buffers, int F, size_t stride_a, size_t stride_b) {
+// row strides of at least F hops (of width_a / width_b values each: 480 samples unless a network call says otherwise).
+static int check_call(const pnb_engine *e, bool train, bool buffers, int F, size_t stride_a, size_t stride_b,
+                      size_t width_a = kFrame, size_t width_b = kFrame) {
   if (!e) return fail(PNB_ERR_ARG, "engine is NULL");
   if (train && !(e->flags & PNB_TRAIN_DATA)) return fail(PNB_ERR_ARG, "engine was not created with PNB_TRAIN_DATA");
   if (!train && (e->flags & PNB_TRAIN_DATA))
@@ -432,7 +435,8 @@ static int check_call(const pnb_engine *e, bool train, bool buffers, int F, size
   if (e->poisoned) return fail(PNB_ERR_CUDA, "an earlier call failed while enqueuing work; the streams' state is undefined until pnb_reset");
   if (F < 1 || F > e->Fmax) return fail(PNB_ERR_ARG, "n_frames %d outside [1, %d]", F, e->Fmax);
   if (!buffers) return fail(PNB_ERR_ARG, train ? "speech/noisy/records pointer is NULL" : "input/output pointer is NULL");
-  if (stride_a < (size_t)F * kFrame || stride_b < (size_t)F * kFrame) return fail(PNB_ERR_ARG, "row stride smaller than n_frames*480");
+  if (stride_a < (size_t)F * width_a) return fail(PNB_ERR_ARG, "row stride smaller than n_frames*%zu", width_a);
+  if (stride_b < (size_t)F * width_b) return fail(PNB_ERR_ARG, "row stride smaller than n_frames*%zu", width_b);
   return PNB_OK;
 }
 static int check_train(const pnb_engine *e, const short *speech, size_t speech_stride, const short *noisy, size_t noisy_stride,
@@ -453,18 +457,18 @@ static int enqueue_ordered(pnb_engine *e, cudaStream_t st, Launches launches) {
   CK(cudaGetLastError());
   return n;
 }
-// Enqueues one call of F hops on st (arguments already checked) and commits the hop counter, last_frames and the launch
-// count when all of it was accepted.  The enqueue itself moves host-side stream state (advance_line the line offset),
-// so a failure after it started leaves the streams' state undefined: the engine is poisoned, and refuses calls until
-// pnb_reset.
+// Enqueues one call of F hops on st (arguments already checked) and commits the hop counter (unless the call leaves the
+// signal state alone: `signal` false, a network call), last_frames and the launch count when all of it was accepted.
+// The enqueue itself moves host-side stream state (advance_line the line offset), so a failure after it started leaves
+// the streams' state undefined: the engine is poisoned, and refuses calls until pnb_reset.
 template <typename Launches>
-static int enqueue_call(pnb_engine *e, int F, cudaStream_t st, Launches launches) {
+static int enqueue_call(pnb_engine *e, int F, cudaStream_t st, Launches launches, bool signal = true) {
   const int n = enqueue_ordered(e, st, launches);
   if (n < 0) {
     e->poisoned = true;
     return n;
   }
-  e->hop += F;
+  if (signal) e->hop += F;
   e->last_frames = F;
   e->launches += n;
   return PNB_OK;
@@ -540,9 +544,10 @@ static int enqueue_plan(pnb_engine *e, const int *ids, int k, const int *hops, i
 }
 
 // One enhancement call as its entry point received it: rows of float samples, or of int16 samples (i16), in and out, in
-// host or device memory by entry point.
+// host or device memory by entry point.  A network call (kNetwork, pnb_compute_rnn_*) reads rows of features or
+// training records (format) and writes rows of g/r to out instead.
 struct Call {
-  enum Kind { kSlots, kSessions, kRagged } kind;
+  enum Kind { kSlots, kSessions, kRagged, kNetwork } kind;
   const void *in;
   size_t in_stride;
   void *out;
@@ -553,13 +558,41 @@ struct Call {
   const int *ids;  // session and ragged calls: the session list (host), n_ids long
   int n_ids;
   const int *hops;  // ragged calls: each listed session's hops (host); null once check_enhance finds them all equal to F
+  int format;       // network calls: PNB_RNN_FEATURES or PNB_RNN_RECORDS
+  // values per hop of an input / output row: 480 samples, or a network call's 70 features / 138 record floats and 68 g/r
+  size_t in_width() const { return kind != kNetwork ? kFrame : format == PNB_RNN_RECORDS ? PNB_RECORD_FLOATS : kFeat; }
+  size_t out_width() const { return kind != kNetwork ? kFrame : 68; }
 };
+
+// A network call on st (arguments already checked): the caller's rows into the features buffer, the network hook, its
+// g/r out to the caller's rows.  The signal state (history line, overlap-add, pitch memory, spectrum ring, hop
+// counter, line offset) is not touched.
+static int enqueue_network(pnb_engine *e, const Call &c, cudaStream_t st) {
+  const int F = c.F;
+  return enqueue_call(e, F, st, [&]() -> int {
+    const int S = e->S, na = e->n_active;
+    int n = 0;
+    {
+      ProfScope ps(e, PNB_K_STAGE_IN, st);
+      n += launch_features_stage(e->d_feat, static_cast<const float *>(c.in), c.in_stride, (int)c.in_width(), na, S, F, st);
+    }
+    CK(cudaGetLastError());
+    {
+      const int q = (e->flags & PNB_NN_TENSOR) ? tc_network(e, F, nullptr, st) : f32_network(e, F, nullptr, st);
+      if (q < 0) return q;
+      n += q;
+    }
+    { ProfScope ps(e, PNB_K_STAGE_IN, st); n += launch_gr_store(e->d_gr, static_cast<float *>(c.out), c.out_stride, na, S, F, st); }
+    return n;
+  }, false);
+}
 
 // One enhancement call on st, its buffers on the device (arguments already checked).  A session call first applies its
 // residency plan, and reads input row / writes output row and g/r row row[p] for slot p.  With hops (a ragged call)
 // slot p runs the hops of its list row, and the slots that stop early are moved to the counters of hop F after
 // synthesis.
 static int enqueue_enhance(pnb_engine *e, const Call &c, cudaStream_t st) {
+  if (c.kind == Call::kNetwork) return enqueue_network(e, c, st);
   const int F = c.F;
   return enqueue_call(e, F, st, [&]() -> int {
     int n = 0;
@@ -634,9 +667,10 @@ static int check_ids(pnb_engine *e, const int *ids, int n, int n_max) {
   return check_list(e, ids, n, e->pool.capacity(), e->pool.capacity(), "ids");
 }
 
-// Every refusal of an enhancement call, before anything changes.  A slot call: check_call, then session mode.  A session
-// call: check_call, then the list.  A ragged call checks the list and its hop counts first, because their largest is
-// the call's length F; when every session runs F hops, hops becomes null and the call is the plain session call.
+// Every refusal of an enhancement call, before anything changes.  A slot call: check_call, then session mode.  A network
+// call: check_call with its row widths, then its format, then session mode.  A session call: check_call, then the list.
+// A ragged call checks the list and its hop counts first, because their largest is the call's length F; when every
+// session runs F hops, hops becomes null and the call is the plain session call.
 static int check_enhance(pnb_engine *e, Call &c) {
   if (c.kind == Call::kRagged) {
     if (!e) return fail(PNB_ERR_ARG, "engine is NULL");
@@ -651,9 +685,11 @@ static int check_enhance(pnb_engine *e, Call &c) {
     for (int i = 0; i < c.n_ids; i++) uniform = uniform && c.hops[i] == c.F;
     if (uniform) c.hops = nullptr;
   }
-  { int rc = check_call(e, false, c.in && c.out, c.F, c.in_stride, c.out_stride); if (rc) return rc; }
+  { int rc = check_call(e, false, c.in && c.out, c.F, c.in_stride, c.out_stride, c.in_width(), c.out_width()); if (rc) return rc; }
   if (c.kind == Call::kSessions) return check_ids(e, c.ids, c.n_ids, e->S);
-  if (c.kind == Call::kSlots && e->sessions) return refuse_in_session_mode();
+  if (c.kind == Call::kNetwork && c.format != PNB_RNN_FEATURES && c.format != PNB_RNN_RECORDS)
+    return fail(PNB_ERR_ARG, "format %d is neither PNB_RNN_FEATURES (0) nor PNB_RNN_RECORDS (1)", c.format);
+  if ((c.kind == Call::kSlots || c.kind == Call::kNetwork) && e->sessions) return refuse_in_session_mode();
   return PNB_OK;
 }
 
@@ -837,14 +873,17 @@ static int report_status(pnb_engine *e) {
   return PNB_OK;
 }
 
-// pnb_process_host_*, pnb_process_sessions_host_*, pnb_process_sessions_ragged_host_* (blocking) and pnb_submit_host_*
-// (pipelined).  The blocking form then copies g/r and the status word back on the engine's stream too, and
-// synchronises it once.  Rows travel F hops wide: a ragged call's input beyond a row's hops is copied but not read.
+// pnb_process_host_*, pnb_process_sessions_host_*, pnb_process_sessions_ragged_host_*, pnb_compute_rnn_host (blocking)
+// and pnb_submit_host_* (pipelined).  The blocking form then copies g/r and the status word back on the engine's stream
+// too, and synchronises it once.  Rows travel F hops wide: a ragged call's input beyond a row's hops is copied but not
+// read.  A network call's rows (in_width / out_width floats per hop) fit the slot sized for float PCM.
 static int host_call(pnb_engine *e, Call c, bool pipelined) {
   { int rc = check_enhance(e, c); if (rc) return rc; }
   CK(cudaSetDevice(e->device));
   const size_t es = c.i16 ? sizeof(short) : sizeof(float);
-  const size_t S = e->S, row = (size_t)e->Fmax * kFrame, w = (size_t)c.F * kFrame * es;
+  const size_t S = e->S, row = (size_t)e->Fmax * kFrame;
+  const size_t row_in = (size_t)e->Fmax * c.in_width(), row_out = (size_t)e->Fmax * c.out_width();  // staged row strides
+  const size_t w_in = (size_t)c.F * c.in_width() * es, w_out = (size_t)c.F * c.out_width() * es;
   const size_t na = c.ids ? c.n_ids : e->n_active;  // the rows of in / out / gr
   const int k = staging_slot(e, pipelined, S * row * es, S * row * es);
   if (k < 0) return k;
@@ -852,12 +891,13 @@ static int host_call(pnb_engine *e, Call c, bool pipelined) {
   Call d = c;  // the call on staging slot k
   d.in = e->stage[k].in;
   d.out = e->stage[k].out;
-  d.in_stride = d.out_stride = row;
+  d.in_stride = row_in;
+  d.out_stride = row_out;
   d.gr = c.ids && c.gr ? e->d_sgr : nullptr;  // session calls gather g/r in list order on the device
   const int rc = round_trip(e, k, pipelined,
-      [&](cudaStream_t s) { return cudaMemcpy2DAsync(e->stage[k].in, row * es, c.in, c.in_stride * es, w, na, cudaMemcpyHostToDevice, s); },
+      [&](cudaStream_t s) { return cudaMemcpy2DAsync(e->stage[k].in, row_in * es, c.in, c.in_stride * es, w_in, na, cudaMemcpyHostToDevice, s); },
       [&] { return enqueue_enhance(e, d, e->stream); },
-      [&](cudaStream_t s) { return cudaMemcpy2DAsync(c.out, c.out_stride * es, e->stage[k].out, row * es, w, na, cudaMemcpyDeviceToHost, s); });
+      [&](cudaStream_t s) { return cudaMemcpy2DAsync(c.out, c.out_stride * es, e->stage[k].out, row_out * es, w_out, na, cudaMemcpyDeviceToHost, s); });
   if (rc || pipelined) return rc;
   if (d.gr)
     CK(cudaMemcpyAsync(c.gr, d.gr, (size_t)c.F * na * 68 * sizeof(float), cudaMemcpyDeviceToHost, e->stream));
@@ -884,6 +924,20 @@ extern "C" int pnb_submit_host_f32(pnb_engine *e, const float *in, size_t in_str
 extern "C" int pnb_submit_host_i16(pnb_engine *e, const short *in, size_t in_stride, short *out, size_t out_stride,
                                    int n_frames) {
   return host_call(e, {Call::kSlots, in, in_stride, out, out_stride, true, n_frames, nullptr}, true);
+}
+
+// The network alone on caller-supplied features or training records (the batched compute_rnn, rnn.cpp:42).
+extern "C" int pnb_compute_rnn_device(pnb_engine *e, int format, const float *d_in, size_t in_stride, int n_frames, float *d_gr,
+                                      size_t gr_stride, void *cuda_stream) {
+  Call c{Call::kNetwork, d_in, in_stride, d_gr, gr_stride, false, n_frames, nullptr};
+  c.format = format;
+  return device_call(e, c, (cudaStream_t)cuda_stream);
+}
+extern "C" int pnb_compute_rnn_host(pnb_engine *e, int format, const float *in, size_t in_stride, int n_frames, float *gr,
+                                    size_t gr_stride) {
+  Call c{Call::kNetwork, in, in_stride, gr, gr_stride, false, n_frames, nullptr};
+  c.format = format;
+  return host_call(e, c, false);
 }
 
 extern "C" int pnb_flush(pnb_engine *e, void *cuda_stream) {

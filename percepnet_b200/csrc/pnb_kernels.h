@@ -85,4 +85,12 @@ int launch_stage_in(float *pcm, size_t pcm_stride, const float *in, const short 
                     const int *hops = nullptr);
 int launch_slide_history(float *pcm, size_t pcm_stride, int n_streams, int n_samples, cudaStream_t st);
 
+// ---- network-only calls (pnb_rnn_io.cu) --------------------------------------------------
+// rows [0, n_streams) of `in` (n_frames hops of width = 70 features or 138 record floats each) -> feat [F][S][70];
+// records are scaled like create_features (x30 on the first 68 values)
+int launch_features_stage(float *feat, const float *in, size_t in_stride, int width, int n_streams, int S, int n_frames,
+                          cudaStream_t st);
+// gr [F][S][68] -> rows [0, n_streams) of `out`, n_frames x 68 floats each
+int launch_gr_store(const float *gr, float *out, size_t out_stride, int n_streams, int S, int n_frames, cudaStream_t st);
+
 }  // namespace pnb

@@ -7,7 +7,8 @@ Exercises the fp32 path, the tensor path (one CTA pair's worth of streams), the 
 the pipelined host entry, the training-data generator, the persistent fp32 GRU chain (both block sizes), submitted
 calls on the chain's anti-diagonal unit order, state export / import, a session-pool schedule (parks, unparks,
 relocations, fresh starts, session export / import / reset), ragged session calls (sessions that stop early, across the
-history slide and the fp32 network's 32-hop chunk) and the pitch-only kernel on tiny batches; prints a checksum per leg."""
+history slide and the fp32 network's 32-hop chunk), network-only calls on features and on records (both network modes)
+and the pitch-only kernel on tiny batches; prints a checksum per leg."""
 import os
 import sys
 
@@ -20,7 +21,7 @@ from percepnet_b200.weights import synth_model  # noqa: E402
 
 
 def main():
-    legs = sys.argv[1:] or ["fp32", "tensor", "train", "fp32chain", "submit", "sessions", "ragged", "pitch"]
+    legs = sys.argv[1:] or ["fp32", "tensor", "train", "fp32chain", "submit", "sessions", "ragged", "rnn", "pitch"]
     m = synth_model(0)
     if "fp32" in legs:
         x = synth_pcm(5, 4, seed=3)
@@ -92,6 +93,19 @@ def main():
                 sums.append(float(np.abs(o).sum()) + float(gr.sum()))
             e.wait()
             print("ragged", flags, sums)
+            e.close()
+    if "rnn" in legs:        # network-only calls on both network modes: features, then records, on an active range
+        for flags in (api.NN_FP32, api.NN_TENSOR):
+            S, F = 130, 3
+            e = api.Engine(S, F, m, flags | api.KEEP_TAPS)
+            e.process(synth_pcm(S, F, seed=17))
+            f = np.ascontiguousarray(e.read_tap("features", F).transpose(1, 0, 2))
+            e.set_active(129)
+            g1 = e.compute_rnn(f[:129])
+            rec = np.zeros((129, F, 138), np.float32)
+            rec[:, :, :68], rec[:, :, 68:70] = f[:129, :, :68] / np.float32(30), f[:129, :, 68:]
+            g2 = e.compute_rnn(rec)
+            print("rnn", flags, float(g1.sum()), float(g2.sum()))
             e.close()
     if "pitch" in legs:
         buf = synth_pcm(40, 4, seed=12)[:, :1728].copy()

@@ -69,8 +69,11 @@ enum {
                             input hundreds to thousands of times louder (the reference's own fp32 arithmetic: 3e-5 there);
                             three terms stay within 2.1e-5 at every scale and cost 8 % of the throughput.  The mode is
                             per engine, never per input, so a stream's result does not depend on its neighbours.          */
-  PNB_TRAIN_DATA = 8     /* training-data generator (pnb_train_records_*): n_streams = 2 x pairs, no network,
+  PNB_TRAIN_DATA = 8,    /* training-data generator (pnb_train_records_*): n_streams = 2 x pairs, no network,
                             no synthesis; model may be NULL; the pnb_process_* entry points are refused      */
+  PNB_TRAIN_AUDIO = 32   /* with PNB_TRAIN_DATA only: the generator also resynthesises every noisy file with its own
+                            labels, as train() writes test_output.pcm (pnb_train_audio_*, which replace
+                            pnb_train_records_* / pnb_submit_train_records on such an engine)                 */
 };
 
 typedef struct pnb_engine pnb_engine;
@@ -147,7 +150,7 @@ int pnb_flush(pnb_engine *e, void *cuda_stream);
  *   Ey_lookahead[34] Ephaty[34] T pitchcorr g[34] r[34]                      (src/denoise.cpp:761-773)
  * are written to records + p*records_stride + t*138 -- a row is what train() writes to its <output> file for that
  * pair of files.  State carries over between calls, so a long pair of files can be fed in chunks of at most
- * max_frames_per_call frames.  The test_input.pcm / test_output.pcm debug audio of train() is not produced. */
+ * max_frames_per_call frames.  Refused on a PNB_TRAIN_AUDIO engine (its audio would have gaps): use pnb_train_audio_*. */
 #define PNB_RECORD_FLOATS 138
 int pnb_train_records_host(pnb_engine *e, const short *speech, size_t speech_stride, const short *noisy,
                            size_t noisy_stride, int n_frames, float *records, size_t records_stride);
@@ -158,6 +161,24 @@ int pnb_submit_train_records(pnb_engine *e, const short *speech, size_t speech_s
 int pnb_train_records_device(pnb_engine *e, const short *d_speech, size_t speech_stride, const short *d_noisy,
                              size_t noisy_stride, int n_frames, float *d_records, size_t records_stride,
                              void *cuda_stream);
+
+/* Training data with its ideal-gain audio (PNB_TRAIN_DATA | PNB_TRAIN_AUDIO engines only).  records receive exactly
+ * what pnb_train_records_* writes.  Row p of audio (audio + p*audio_stride, audio_stride >= n_frames*480) receives
+ * n_frames x 480 int16 samples: what train() writes to test_output.pcm for pair p over these frames
+ * (src/denoise.cpp:742-759): the noisy frame resynthesised with its own labels -- g post-filtered, pitch_filter with r
+ * unless the noisy frame is silent, interp_band_gain(g), frame_synthesis -- and converted by clamping, then truncating:
+ * (short)fmaxf(-32768, fminf(32767, y)) at scale 1 (NaN gives 32767), not the (short)(y*32768) of pnb_process_*_i16.
+ * Every frame is written (nothing is dropped); output frame t carries noisy input frame t - 6.  State carries over
+ * between calls, so the audio does not depend on how frames are grouped into calls; pnb_reset and the state blob
+ * cover the overlap-add memory.  train()'s test_input.pcm is the noisy input itself (its clamp is a no-op on int16).
+ * Refused with PNB_ERR_ARG like pnb_train_records_*, and also on an engine without PNB_TRAIN_AUDIO, a NULL audio
+ * pointer or a short audio_stride.  A call issues one launch more than pnb_train_records_*. */
+int pnb_train_audio_host(pnb_engine *e, const short *speech, size_t speech_stride, const short *noisy,
+                         size_t noisy_stride, int n_frames, float *records, size_t records_stride, short *audio,
+                         size_t audio_stride);
+int pnb_train_audio_device(pnb_engine *e, const short *d_speech, size_t speech_stride, const short *d_noisy,
+                           size_t noisy_stride, int n_frames, float *d_records, size_t records_stride, short *d_audio,
+                           size_t audio_stride, void *cuda_stream);
 
 /* The network alone: the batched compute_rnn (src/rnnoise.h:68, src/rnn.cpp:42) on caller-supplied inputs, to score a
  * model on features or training records exactly as the engine runs it.
@@ -348,7 +369,8 @@ const char *pnb_kernel_class_name(int cls);
 long long pnb_launch_count(const pnb_engine *e);
 /* Kernel launches one pnb_process_* call with n_frames hops issues (one more on the calls that also move the
  * streams' history back to the start of their rows, at most every call, typically every eighth; one more on a ragged
- * session call in which some session runs fewer than n_frames = max(hops) hops). */
+ * session call in which some session runs fewer than n_frames = max(hops) hops).  On a PNB_TRAIN_AUDIO engine it is the
+ * value of a PNB_TRAIN_DATA engine of the same shape plus one: the resynthesis launch. */
 int pnb_launches_per_call(const pnb_engine *e, int n_frames);
 int pnb_n_streams(const pnb_engine *e);
 int pnb_max_frames(const pnb_engine *e);

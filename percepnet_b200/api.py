@@ -18,7 +18,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "libpercepnet_b200.so")
 
 FRAME = 480
-NN_FP32, NN_TENSOR, POSTFILTER, KEEP_TAPS, TRAIN_DATA, CONV_WIDE = 0, 1, 2, 4, 8, 16
+NN_FP32, NN_TENSOR, POSTFILTER, KEEP_TAPS, TRAIN_DATA, CONV_WIDE, TRAIN_AUDIO = 0, 1, 2, 4, 8, 16, 32
 RECORD = 138
 RNN_FEATURES, RNN_RECORDS = 0, 1   # pnb_compute_rnn_* formats: 70 features or 138 record floats per hop
 TAPS = {"features": (0, np.float32, 70), "pitch": (1, np.int32, 4), "pitchf": (2, np.float32, 2),
@@ -49,6 +49,8 @@ def load_library() -> C.CDLL:
     L.pnb_train_records_host.argtypes = [vp, vp, sz, vp, sz, i, vp, sz]
     L.pnb_submit_train_records.argtypes = [vp, vp, sz, vp, sz, i, vp, sz]
     L.pnb_train_records_device.argtypes = [vp, vp, sz, vp, sz, i, vp, sz, vp]
+    L.pnb_train_audio_host.argtypes = [vp, vp, sz, vp, sz, i, vp, sz, vp, sz]
+    L.pnb_train_audio_device.argtypes = [vp, vp, sz, vp, sz, i, vp, sz, vp, sz, vp]
     L.pnb_destroy.argtypes = [vp]
     L.pnb_destroy.restype = None
     L.pnb_reset.argtypes = [vp]
@@ -107,7 +109,7 @@ def load_library() -> C.CDLL:
 
 
 EXPORTS = ("pnb_create", "pnb_destroy", "pnb_reset", "pnb_resolve_device", "pnb_process_host_f32", "pnb_process_host_i16",
-           "pnb_model_load_blob", "pnb_model_load_stream", "pnb_model_free", "pnb_train_records_host", "pnb_train_records_device", "pnb_submit_train_records", "pnb_process_device_f32", "pnb_process_device_i16", "pnb_submit_host_f32", "pnb_submit_host_i16", "pnb_submit_device_f32", "pnb_submit_device_i16", "pnb_flush", "pnb_wait", "pnb_check",
+           "pnb_model_load_blob", "pnb_model_load_stream", "pnb_model_free", "pnb_train_records_host", "pnb_train_records_device", "pnb_submit_train_records", "pnb_train_audio_host", "pnb_train_audio_device", "pnb_process_device_f32", "pnb_process_device_i16", "pnb_submit_host_f32", "pnb_submit_host_i16", "pnb_submit_device_f32", "pnb_submit_device_i16", "pnb_flush", "pnb_wait", "pnb_check",
            "pnb_compute_rnn_device", "pnb_compute_rnn_host",
            "pnb_read_tap", "pnb_state_size", "pnb_get_state", "pnb_set_state",
            "pnb_reset_streams", "pnb_export_states", "pnb_import_states", "pnb_set_active_streams", "pnb_active_streams",
@@ -455,6 +457,28 @@ class Engine:
                              d_records: int, records_stride: int, stream: int = 0):
         self._ck(self.L.pnb_train_records_device(self.h, d_speech, speech_stride, d_noisy, noisy_stride, n_frames,
                                                  d_records, records_stride, stream), "pnb_train_records_device")
+
+    def train_audio(self, speech: np.ndarray, noisy: np.ndarray):
+        """speech, noisy: [n_pairs, F*480] int16 -> (records [n_pairs, F, 138] float32, audio [n_pairs, F*480] int16):
+        the records of train_records and, for each pair, what the reference's train() writes to test_output.pcm over
+        these frames (src/denoise.cpp:742-759: the noisy file resynthesised with its own labels, clamped to int16).
+        Engine must have flags=TRAIN_DATA | TRAIN_AUDIO; state carries over, so call repeatedly with consecutive chunks."""
+        N = self.n_streams // 2
+        assert speech.shape == noisy.shape and speech.shape[0] == N and speech.shape[1] % FRAME == 0
+        assert speech.dtype == np.int16 and noisy.dtype == np.int16
+        F = speech.shape[1] // FRAME
+        speech, noisy = np.ascontiguousarray(speech), np.ascontiguousarray(noisy)
+        rec = np.empty((N, F, RECORD), np.float32)
+        audio = np.empty((N, F * FRAME), np.int16)
+        self._ck(self.L.pnb_train_audio_host(self.h, speech.ctypes.data, speech.shape[1], noisy.ctypes.data, noisy.shape[1],
+                                             F, rec.ctypes.data, F * RECORD, audio.ctypes.data, F * FRAME),
+                 "pnb_train_audio_host")
+        return rec, audio
+
+    def train_audio_device(self, d_speech: int, speech_stride: int, d_noisy: int, noisy_stride: int, n_frames: int,
+                           d_records: int, records_stride: int, d_audio: int, audio_stride: int, stream: int = 0):
+        self._ck(self.L.pnb_train_audio_device(self.h, d_speech, speech_stride, d_noisy, noisy_stride, n_frames, d_records,
+                                               records_stride, d_audio, audio_stride, stream), "pnb_train_audio_device")
 
     def profile(self, on: bool):
         self._ck(self.L.pnb_profile_enable(self.h, 1 if on else 0), "pnb_profile_enable")

@@ -833,7 +833,7 @@ __global__ void __launch_bounds__(kAnaWarps * 32) analysis_kernel(AnalysisArgs A
         return make_float2((1.f / kWin) * v, 0.f);
       });
       ANA_TICK(13);
-      float2 *Pg = A.P ? A.P + fs * kBins : nullptr;
+      float2 *Pg = A.P && s < A.P_rows ? A.P + fs * kBins : nullptr;
       for (int k = lane; k < kBins; k += 32) {
         float2 p = W.fft[fpos(k)], x = Xg[k];
         if (Pg) Pg[k] = p;
@@ -911,6 +911,8 @@ struct SynBlockSmem {
 };
 constexpr int kSynWarps = 4;
 
+// kClamp: the int16 conversion of A.clamp16, one instantiation per mode so that each keeps its own code
+template <bool kClamp>
 __global__ void __launch_bounds__(kSynWarps * 32) synthesis_kernel(SynthesisArgs A) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   SynBlockSmem &B = *reinterpret_cast<SynBlockSmem *>(smem_raw);
@@ -1009,7 +1011,10 @@ __global__ void __launch_bounds__(kSynWarps * 32) synthesis_kernel(SynthesisArgs
       a = a * B.hw[n];
       float o = a + mem[i];
       if (outp) outp[n] = o;
-      if (outs) outs[n] = (short)(int)(o * 32768.f);  // main.cpp:36: truncation toward zero
+      if (outs) {
+        if (kClamp) outs[n] = (short)fmaxf(-32768.f, fminf(32767.f, o));  // denoise.cpp:756-758: NaN -> 32767
+        else outs[n] = (short)(int)(o * 32768.f);                          // main.cpp:36: truncation toward zero
+      }
       int n2 = n + kFrame;
       float c = (float)kWin * W.fft[fpos(kWin - n2)].x;
       mem[i] = c * B.hw[kWin - 1 - n2];
@@ -1098,7 +1103,10 @@ cudaError_t dsp_configure() {
   cudaError_t e = cudaFuncSetAttribute(analysis_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                        (int)analysis_smem_bytes());
   if (e != cudaSuccess) return e;
-  return cudaFuncSetAttribute(synthesis_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+  e = cudaFuncSetAttribute(synthesis_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                           (int)synthesis_smem_bytes());
+  if (e != cudaSuccess) return e;
+  return cudaFuncSetAttribute(synthesis_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                               (int)synthesis_smem_bytes());
 }
 
@@ -1151,6 +1159,7 @@ __global__ void __launch_bounds__(256) train_labels_kernel(LabelArgs A) {
       g *= g_att;
     }
     rec[104 + b] = r;
+    if (A.gr) A.gr[fn * 68 + kBands + b] = r;  // the labels again, for the resynthesis of the noisy row (:742-759)
     sh_g[wib][b] = g;
     // sinf of the reference's libm is correctly rounded in all but rare cases; so is the rounded double sine
     sh_gw[wib][b] = g * (float)sin((double)(float)(M_PI / 2 * (double)g));
@@ -1167,7 +1176,11 @@ __global__ void __launch_bounds__(256) train_labels_kernel(LabelArgs A) {
     rec[69] = A.feat[fn * kFeat + 69];
   }
   G = __shfl_sync(0xffffffffu, G, 0);
-  for (int b = lane; b < kBands; b += 32) rec[70 + b] = G * sh_gw[wib][b];
+  for (int b = lane; b < kBands; b += 32) {
+    const float g = G * sh_gw[wib][b];
+    rec[70 + b] = g;
+    if (A.gr) A.gr[fn * 68 + b] = g;
+  }
 }
 
 #ifdef PNB_ANA_TIMING
@@ -1201,7 +1214,8 @@ int launch_train_labels(const LabelArgs &a, cudaStream_t st) {
 
 int launch_synthesis(const SynthesisArgs &a, cudaStream_t st) {
   dim3 grid((a.n_streams + kSynWarps - 1) / kSynWarps);
-  synthesis_kernel<<<grid, kSynWarps * 32, synthesis_smem_bytes(), st>>>(a);
+  if (a.clamp16) synthesis_kernel<true><<<grid, kSynWarps * 32, synthesis_smem_bytes(), st>>>(a);
+  else synthesis_kernel<false><<<grid, kSynWarps * 32, synthesis_smem_bytes(), st>>>(a);
   return 1;
 }
 int launch_stage_in(float *pcm, size_t pcm_stride, const float *in, const short *in16, size_t in_stride,

@@ -152,7 +152,8 @@ extern "C" int pnb_create(pnb_engine **out, int n_streams, int max_frames, const
   if (n_streams < 1 || max_frames < 1) return fail(PNB_ERR_ARG, "n_streams and max_frames_per_call must be >= 1");
   if ((long long)n_streams * max_frames > (1ll << 24))
     return fail(PNB_ERR_ARG, "n_streams x max_frames_per_call above 2^24 rows per call: split the batch across engines");
-  const bool train_mode = (flags & PNB_TRAIN_DATA) != 0;
+  const bool train_mode = (flags & PNB_TRAIN_DATA) != 0, train_audio = (flags & PNB_TRAIN_AUDIO) != 0;
+  if (train_audio && !train_mode) return fail(PNB_ERR_ARG, "PNB_TRAIN_AUDIO applies to PNB_TRAIN_DATA engines");
   if (train_mode && (n_streams & 1)) return fail(PNB_ERR_ARG, "PNB_TRAIN_DATA needs n_streams = 2 x pairs");
   if ((flags & PNB_CONV_WIDE) && !(flags & PNB_NN_TENSOR)) return fail(PNB_ERR_ARG, "PNB_CONV_WIDE applies to PNB_NN_TENSOR engines");
   if (train_mode && (flags & (PNB_NN_TENSOR | PNB_POSTFILTER)))
@@ -231,10 +232,10 @@ extern "C" int pnb_create(pnb_engine **out, int n_streams, int max_frames, const
   e->ring = (int)F + 5;
   CKD(engine_alloc(e, &e->d_zring, (size_t)e->ring * S * kBins, kStreamState));
   CKD(engine_alloc(e, &e->d_ering, (size_t)e->ring * S * kBands, kStreamState));
-  if (!train_mode) CKD(engine_alloc(e, &e->d_P, F * S * kBins, kScratch));
+  if (!train_mode || train_audio) CKD(engine_alloc(e, &e->d_P, F * S * kBins, kScratch));  // audio: noisy rows only
   CKD(engine_alloc(e, &e->d_Ex, F * S * kBands, kScratch));
   CKD(engine_alloc(e, &e->d_sil, F * S, kScratch));
-  if (!train_mode) CKD(engine_alloc(e, &e->d_gr, F * S * 68, kScratch));
+  if (!train_mode || train_audio) CKD(engine_alloc(e, &e->d_gr, F * S * 68, kScratch));  // audio: the noisy rows' labels
   if (train_mode) CKD(engine_alloc(e, &e->d_raw, F * S * 68, kScratch));
   if (flags & PNB_KEEP_TAPS) {
     CKD(engine_alloc(e, &e->d_tap_pitch, F * S * 4, kScratch));
@@ -392,7 +393,7 @@ static AnalysisArgs analysis_args(pnb_engine *e, int F) {
   a.pcm = e->d_pcm + e->line_off;  // this call's [history | new hops] window of every row
   a.pcm_stride = e->pcm_stride; a.n_streams = e->n_active; a.stride = e->S; a.n_frames = F; a.tab = e->d_tab;
   a.feat = e->d_feat; a.zring = e->d_zring; a.ering = e->d_ering; a.ring = e->ring; a.hop0 = e->hop;
-  a.P = e->d_P; a.Ex = e->d_Ex; a.raw = nullptr; a.silence = e->d_sil;
+  a.P = e->d_P; a.P_rows = e->n_active; a.Ex = e->d_Ex; a.raw = nullptr; a.silence = e->d_sil;
   a.last_period = e->d_last_period; a.last_gain = e->d_last_gain;
   a.tap_pitch = e->d_tap_pitch; a.tap_pitchf = e->d_tap_pitchf;
   a.hops = nullptr;
@@ -408,6 +409,7 @@ static SynthesisArgs synthesis_args(pnb_engine *e, int F, float *d_out, short *d
   s.tap_g = e->d_tap_g;
   s.row = nullptr;
   s.hops = nullptr;
+  s.clamp16 = 0;
   return s;
 }
 
@@ -439,11 +441,17 @@ static int check_call(const pnb_engine *e, bool train, bool buffers, int F, size
   if (stride_b < (size_t)F * width_b) return fail(PNB_ERR_ARG, "row stride smaller than n_frames*%zu", width_b);
   return PNB_OK;
 }
+// A training-data call: records only (audio null) on an engine without PNB_TRAIN_AUDIO, records and audio on one with it.
 static int check_train(const pnb_engine *e, const short *speech, size_t speech_stride, const short *noisy, size_t noisy_stride,
-                       int F, const float *records, size_t records_stride) {
-  const int rc = check_call(e, true, speech && noisy && records, F, speech_stride, noisy_stride);
+                       int F, const float *records, size_t records_stride, bool audio_call = false,
+                       const short *audio = nullptr, size_t audio_stride = 0) {
+  const int rc = check_call(e, true, speech && noisy && records && (audio || !audio_call), F, speech_stride, noisy_stride);
   if (rc) return rc;
+  if (audio_call && !(e->flags & PNB_TRAIN_AUDIO)) return fail(PNB_ERR_ARG, "engine was not created with PNB_TRAIN_AUDIO");
+  if (!audio_call && (e->flags & PNB_TRAIN_AUDIO))
+    return fail(PNB_ERR_ARG, "engine was created with PNB_TRAIN_AUDIO: use pnb_train_audio_*, so that its audio has no gaps");
   if (records_stride < (size_t)F * PNB_RECORD_FLOATS) return fail(PNB_ERR_ARG, "records_stride smaller than n_frames*138");
+  if (audio_call && audio_stride < (size_t)F * kFrame) return fail(PNB_ERR_ARG, "audio_stride smaller than n_frames*480");
   return PNB_OK;
 }
 
@@ -719,11 +727,13 @@ extern "C" int pnb_submit_device_i16(pnb_engine *e, const short *d_in, size_t in
 }
 
 // ------------------------------------------------------------------------------------------
-// training-data generator (row f1): stage both files of every pair, analysis over 2N streams, labels
+// training-data generator (row f1): stage both files of every pair, analysis over 2N streams, labels; on a
+// PNB_TRAIN_AUDIO engine then the resynthesis of the N noisy streams with their labels
 // ------------------------------------------------------------------------------------------
-// One training-record call on st (arguments already checked).
+// One training-record call on st (arguments already checked); d_audio null on an engine without PNB_TRAIN_AUDIO.
 static int enqueue_records(pnb_engine *e, const short *d_speech, size_t speech_stride, const short *d_noisy,
-                           size_t noisy_stride, int F, float *d_records, size_t records_stride, cudaStream_t st) {
+                           size_t noisy_stride, int F, float *d_records, size_t records_stride, short *d_audio,
+                           size_t audio_stride, cudaStream_t st) {
   return enqueue_call(e, F, st, [&]() -> int {
     const int N = e->S / 2;
     float *line = e->d_pcm + e->line_off;
@@ -735,11 +745,20 @@ static int enqueue_records(pnb_engine *e, const short *d_speech, size_t speech_s
     }
     AnalysisArgs a = analysis_args(e, F);  // all S streams: the active range of a training-data engine is always S
     a.raw = e->d_raw;
+    a.P_rows = N;  // an audio engine's P: the noisy rows (the others have none)
     { ProfScope ps(e, PNB_K_ANALYSIS, st); n += launch_analysis(a, st); }
     LabelArgs l;
     l.feat = e->d_feat; l.raw = e->d_raw; l.Ex = e->d_Ex; l.tab = e->d_tab; l.n_pairs = N; l.n_frames = F;
     l.records = d_records; l.pair_stride = records_stride;
+    l.gr = d_audio ? e->d_gr : nullptr;
     { ProfScope ps(e, PNB_K_LABELS, st); n += launch_train_labels(l, st); }
+    if (d_audio) {  // denoise.cpp:742-759 on the noisy rows, their labels post-filtered already (no PNB_POSTFILTER here)
+      SynthesisArgs s = synthesis_args(e, F, nullptr, d_audio, audio_stride);
+      s.n_streams = N;
+      s.clamp16 = 1;
+      ProfScope ps(e, PNB_K_SYNTHESIS, st);
+      n += launch_synthesis(s, st);
+    }
     n += advance_line(e, F, st);
     return n;
   });
@@ -750,7 +769,19 @@ extern "C" int pnb_train_records_device(pnb_engine *e, const short *d_speech, si
                                         size_t records_stride, void *cuda_stream) {
   { int rc = check_train(e, d_speech, speech_stride, d_noisy, noisy_stride, F, d_records, records_stride); if (rc) return rc; }
   CK(cudaSetDevice(e->device));
-  return enqueue_records(e, d_speech, speech_stride, d_noisy, noisy_stride, F, d_records, records_stride, (cudaStream_t)cuda_stream);
+  return enqueue_records(e, d_speech, speech_stride, d_noisy, noisy_stride, F, d_records, records_stride, nullptr, 0,
+                         (cudaStream_t)cuda_stream);
+}
+extern "C" int pnb_train_audio_device(pnb_engine *e, const short *d_speech, size_t speech_stride, const short *d_noisy,
+                                      size_t noisy_stride, int F, float *d_records, size_t records_stride, short *d_audio,
+                                      size_t audio_stride, void *cuda_stream) {
+  {
+    int rc = check_train(e, d_speech, speech_stride, d_noisy, noisy_stride, F, d_records, records_stride, true, d_audio, audio_stride);
+    if (rc) return rc;
+  }
+  CK(cudaSetDevice(e->device));
+  return enqueue_records(e, d_speech, speech_stride, d_noisy, noisy_stride, F, d_records, records_stride, d_audio,
+                         audio_stride, (cudaStream_t)cuda_stream);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -817,26 +848,33 @@ static int round_trip(pnb_engine *e, int k, bool pipelined, H2D h2d, Call call, 
   return PNB_OK;
 }
 
-// pnb_train_records_host (blocking) and pnb_submit_train_records (pipelined)
+// pnb_train_records_host (blocking), pnb_submit_train_records (pipelined) and pnb_train_audio_host (blocking, with audio);
+// the staged audio rows follow the staged records in the slot's output buffer.
 static int records_host(pnb_engine *e, const short *speech, size_t speech_stride, const short *noisy, size_t noisy_stride,
-                        int F, float *records, size_t records_stride, bool pipelined) {
-  { int rc = check_train(e, speech, speech_stride, noisy, noisy_stride, F, records, records_stride); if (rc) return rc; }
+                        int F, float *records, size_t records_stride, bool pipelined, bool audio_call = false,
+                        short *audio = nullptr, size_t audio_stride = 0) {
+  {
+    int rc = check_train(e, speech, speech_stride, noisy, noisy_stride, F, records, records_stride, audio_call, audio, audio_stride);
+    if (rc) return rc;
+  }
   CK(cudaSetDevice(e->device));
   const size_t N = e->S / 2, row = (size_t)e->Fmax * kFrame, rrow = (size_t)e->Fmax * PNB_RECORD_FLOATS;
   const size_t w = (size_t)F * kFrame * sizeof(short);
-  const int k = staging_slot(e, pipelined, 2 * N * row * sizeof(short), N * rrow * sizeof(float));
+  const int k = staging_slot(e, pipelined, 2 * N * row * sizeof(short), N * rrow * sizeof(float) + (audio ? N * row * sizeof(short) : 0));
   if (k < 0) return k;
   short *d_noisy = (short *)e->stage[k].in, *d_speech = d_noisy + N * row;
   float *d_rec = (float *)e->stage[k].out;
+  short *d_audio = audio ? (short *)(d_rec + N * rrow) : nullptr;
   const int rc = round_trip(e, k, pipelined,
       [&](cudaStream_t s) {
         const cudaError_t ce = cudaMemcpy2DAsync(d_noisy, row * 2, noisy, noisy_stride * 2, w, N, cudaMemcpyHostToDevice, s);
         return ce != cudaSuccess ? ce : cudaMemcpy2DAsync(d_speech, row * 2, speech, speech_stride * 2, w, N, cudaMemcpyHostToDevice, s);
       },
-      [&] { return enqueue_records(e, d_speech, row, d_noisy, row, F, d_rec, rrow, e->stream); },
+      [&] { return enqueue_records(e, d_speech, row, d_noisy, row, F, d_rec, rrow, d_audio, row, e->stream); },
       [&](cudaStream_t s) {
-        return cudaMemcpy2DAsync(records, records_stride * 4, d_rec, rrow * 4, (size_t)F * PNB_RECORD_FLOATS * 4, N,
-                                 cudaMemcpyDeviceToHost, s);
+        const cudaError_t ce = cudaMemcpy2DAsync(records, records_stride * 4, d_rec, rrow * 4, (size_t)F * PNB_RECORD_FLOATS * 4, N,
+                                                 cudaMemcpyDeviceToHost, s);
+        return ce != cudaSuccess || !audio ? ce : cudaMemcpy2DAsync(audio, audio_stride * 2, d_audio, row * 2, w, N, cudaMemcpyDeviceToHost, s);
       });
   if (rc || pipelined) return rc;
   CK(cudaStreamSynchronize(e->stream));
@@ -849,6 +887,11 @@ extern "C" int pnb_train_records_host(pnb_engine *e, const short *speech, size_t
 extern "C" int pnb_submit_train_records(pnb_engine *e, const short *speech, size_t speech_stride, const short *noisy,
                                         size_t noisy_stride, int F, float *records, size_t records_stride) {
   return records_host(e, speech, speech_stride, noisy, noisy_stride, F, records, records_stride, true);
+}
+extern "C" int pnb_train_audio_host(pnb_engine *e, const short *speech, size_t speech_stride, const short *noisy,
+                                    size_t noisy_stride, int F, float *records, size_t records_stride, short *audio,
+                                    size_t audio_stride) {
+  return records_host(e, speech, speech_stride, noisy, noisy_stride, F, records, records_stride, false, true, audio, audio_stride);
 }
 
 // after the stream that carried the status copy was synchronised
@@ -1423,8 +1466,10 @@ extern "C" long long pnb_launch_count(const pnb_engine *e) { return e ? e->launc
 extern "C" int pnb_launches_per_call(const pnb_engine *e, int n_frames) {
   if (!e) return 0;
   // stage_in, analysis, the network, synthesis; without the history move of advance_line (at most one more launch per
-  // call), and without the fix-up of a ragged session call in which a session runs fewer hops than the call (one more)
-  return 3 + ((e->flags & PNB_NN_TENSOR) ? tc_network_launches(e, n_frames) : f32_network_launches(e, n_frames));
+  // call), and without the fix-up of a ragged session call in which a session runs fewer hops than the call (one more);
+  // the resynthesis of a PNB_TRAIN_AUDIO engine is one launch more than its records alone
+  return 3 + ((e->flags & PNB_NN_TENSOR) ? tc_network_launches(e, n_frames) : f32_network_launches(e, n_frames)) +
+         ((e->flags & PNB_TRAIN_AUDIO) ? 1 : 0);
 }
 extern "C" int pnb_n_streams(const pnb_engine *e) { return e ? e->S : 0; }
 extern "C" int pnb_max_frames(const pnb_engine *e) { return e ? e->Fmax : 0; }

@@ -16,7 +16,8 @@ struct AnalysisArgs {
   float *ering;            // [ring][S][34] their band energies
   int ring;                // slots (>= n_frames + 5)
   long hop0;               // absolute index of the call's first hop
-  float2 *P;               // [F][S][400] or null (training-data mode has no synthesis)
+  float2 *P;               // [F][S][400] or null (a training-data engine without PNB_TRAIN_AUDIO has no synthesis)
+  int P_rows;              // P is stored for rows [0, P_rows) only (a training-data engine resynthesises the noisy rows)
   float *Ex;               // [F][S][34] or null
   float *raw;              // [F][S][68] or null: look-ahead band energies and pitch coherence before the x30
   unsigned char *silence;  // [F][S]
@@ -47,6 +48,8 @@ struct SynthesisArgs {
   const int *row;          // [n_streams] output row of each slot (session calls), or null: row s
   const int *hops;         // [n_streams] hops of each slot (ragged session calls), or null: n_frames; hops [hops[s],
                            // n_frames) of a slot's output row are written as zeros
+  int clamp16;             // int16 conversion of out16: 0 truncates y*32768 (main.cpp:36), 1 clamps y to [-32768, 32767]
+                           // and truncates (train()'s test_output.pcm, denoise.cpp:756-758)
 };
 
 // training-data records (train(), denoise.cpp:600-787): streams [0,N) are the noisy signals, [N,2N) the clean ones
@@ -58,6 +61,7 @@ struct LabelArgs {
   int n_pairs, n_frames;
   float *records;          // pair p, frame t at records + p*pair_stride + t*138
   size_t pair_stride;
+  float *gr;               // [F][2N][68] or null: the record's g and r of pair p, frame t at row t*2N + p (its noisy row)
 };
 int launch_train_labels(const LabelArgs &a, cudaStream_t st);
 

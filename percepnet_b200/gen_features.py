@@ -3,11 +3,16 @@
 
   python -m percepnet_b200.gen_features <speech.pcm> <noisy.pcm> <count> <output.f32>      # the reference's argv
   python -m percepnet_b200.gen_features --list jobs.txt [--batch 4096] [--chunk 64]         # one job per line
+  ... [--test-audio]                                                                       # plus train()'s TEST audio
 
 Each job reads two raw int16 48 kHz files and writes ``count`` records of 138 float32
 (Ey_lookahead[34] Ephaty[34] T pitchcorr g[34] r[34], denoise.cpp:761-773) -- the file ``rnn_train.py:44-53`` and
 ``utils/bin2h5.py`` consume.  Jobs of a list run as one batch of pairs per GPU call (pnb_train_records_host).
 Like train(), a file shorter than ``count`` frames is re-read from its start (denoise.cpp:676-679, 687-690).
+With ``--test-audio`` each job also writes ``<output>.test_input.pcm`` and ``<output>.test_output.pcm``, ``count`` x 480
+int16 each: what train() writes to test_input.pcm / test_output.pcm in its working directory (denoise.cpp:722-728,
+742-759), the noisy input as read and the noisy input resynthesised with its own labels, named per job so that the
+jobs of a list do not overwrite each other (pnb_train_audio_host).
 There is no CPU path: without the CUDA library / a GPU this exits with an error.
 """
 from __future__ import annotations
@@ -33,8 +38,9 @@ def read_cyclic_frames(path: str, count: int) -> np.ndarray:
     return frames[np.arange(count) % nf].reshape(-1)
 
 
-def run_jobs(jobs, batch: int = 4096, chunk: int = 64, device: int = 0) -> None:
-    """jobs: list of (speech_path, noisy_path, count, output_path)."""
+def run_jobs(jobs, batch: int = 4096, chunk: int = 64, device: int = 0, test_audio: bool = False) -> None:
+    """jobs: list of (speech_path, noisy_path, count, output_path); test_audio: also write each job's
+    <output>.test_input.pcm and <output>.test_output.pcm."""
     from . import api
     jobs = sorted(jobs, key=lambda j: -j[2])                   # similar lengths share a batch
     for b0 in range(0, len(jobs), batch):
@@ -45,15 +51,26 @@ def run_jobs(jobs, batch: int = 4096, chunk: int = 64, device: int = 0) -> None:
         for k, (sp, no, cnt, _) in enumerate(group):
             speech[k, :cnt * FRAME] = read_cyclic_frames(sp, cnt)
             noisy[k, :cnt * FRAME] = read_cyclic_frames(no, cnt)
-        eng = api.Engine(2 * N, min(chunk, Fmax), None, api.TRAIN_DATA, device=device)
-        parts = []
+        flags = api.TRAIN_DATA | (api.TRAIN_AUDIO if test_audio else 0)
+        eng = api.Engine(2 * N, min(chunk, Fmax), None, flags, device=device)
+        parts, audio = [], []
         for t0 in range(0, Fmax, chunk):
             t1 = min(Fmax, t0 + chunk)
-            parts.append(eng.train_records(speech[:, t0 * FRAME:t1 * FRAME], noisy[:, t0 * FRAME:t1 * FRAME]))
+            sp, no = speech[:, t0 * FRAME:t1 * FRAME], noisy[:, t0 * FRAME:t1 * FRAME]
+            if test_audio:
+                r, a = eng.train_audio(sp, no)
+                audio.append(a)
+            else:
+                r = eng.train_records(sp, no)
+            parts.append(r)
         eng.close()
         rec = np.concatenate(parts, axis=1)
+        audio = np.concatenate(audio, axis=1) if test_audio else None
         for k, (_, _, cnt, out) in enumerate(group):
             rec[k, :cnt].astype("<f4").tofile(out)
+            if test_audio:
+                noisy[k, :cnt * FRAME].astype("<i2").tofile(out + ".test_input.pcm")
+                audio[k, :cnt * FRAME].astype("<i2").tofile(out + ".test_output.pcm")
 
 
 def main(argv=None) -> int:
@@ -63,6 +80,8 @@ def main(argv=None) -> int:
     ap.add_argument("--batch", type=int, default=4096, help="pairs per GPU batch")
     ap.add_argument("--chunk", type=int, default=64, help="frames per GPU call")
     ap.add_argument("--device", type=int, default=0)
+    ap.add_argument("--test-audio", action="store_true",
+                    help="also write <output>.test_input.pcm and <output>.test_output.pcm, as train() writes its TEST audio")
     a = ap.parse_args(argv)
     if a.list:
         jobs = []
@@ -75,7 +94,7 @@ def main(argv=None) -> int:
     else:
         sys.stderr.write(f"usage: {sys.argv[0]} <speech> <noisy> <count> <output>\n")   # denoise.cpp:637
         return 1
-    run_jobs(jobs, a.batch, a.chunk, a.device)
+    run_jobs(jobs, a.batch, a.chunk, a.device, a.test_audio)
     return 0
 
 

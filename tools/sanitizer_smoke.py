@@ -4,7 +4,7 @@
     compute-sanitizer --tool racecheck python tools/sanitizer_smoke.py
 
 Exercises the fp32 path, the tensor path (one CTA pair's worth of streams), the post-filter, the int16 entry,
-the pipelined host entry, the training-data generator, the persistent fp32 GRU chain (both block sizes), submitted
+the pipelined host entry, the training-data generator (records alone and with its audio), the persistent fp32 GRU chain (both block sizes), submitted
 calls on the chain's anti-diagonal unit order, state export / import, a session-pool schedule (parks, unparks,
 relocations, fresh starts, session export / import / reset), ragged session calls (sessions that stop early, across the
 history slide and the fp32 network's 32-hop chunk), network-only calls on features and on records (both network modes)
@@ -117,6 +117,13 @@ def main():
         r1 = e.train_records(c[:, :3 * 480], n[:, :3 * 480])
         r2 = e.train_records(c[:, 3 * 480:], n[:, 3 * 480:])
         print("train", float(r1.sum()), float(r2.sum()))
+        e.close()
+        c, n = synth_pairs(6, 10, seed=9)        # output frame t carries input frame t - 6: ten frames, audible audio
+        e = api.Engine(12, 5, None, api.TRAIN_DATA | api.TRAIN_AUDIO)   # with the resynthesis of the noisy rows
+        r3, a3 = e.train_audio(c[:, :5 * 480], n[:, :5 * 480])
+        r4, a4 = e.train_audio(c[:, 5 * 480:], n[:, 5 * 480:])
+        print("train_audio", float(r3.sum()), float(r4.sum()), int(np.abs(a3.astype(np.int64)).sum()),
+              int(np.abs(a4.astype(np.int64)).sum()))
         e.close()
 
 

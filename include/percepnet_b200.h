@@ -106,7 +106,8 @@ int pnb_process_host_f32(pnb_engine *e, const float *in, size_t in_stride, float
                          int n_frames, float *gr);
 
 /* int16 PCM wire format with the CLI's conversions (src/main.cpp:34,36): x = s/32768.f in,
- * (short)(y*32768) out (C truncation).  The first-hop drop of main.cpp:37-38 is the caller's. */
+ * (short)(y*32768) out (C truncation; output past full scale wraps to its low 16 bits, as the CLI built for x86-64
+ * does).  The first-hop drop of main.cpp:37-38 is the caller's. */
 int pnb_process_host_i16(pnb_engine *e, const short *in, size_t in_stride, short *out, size_t out_stride,
                          int n_frames, float *gr);
 

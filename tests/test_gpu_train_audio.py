@@ -3,11 +3,13 @@ file resynthesised with its own labels, as the reference's train() writes test_o
 against the CPU restatement (tests/train_audio_oracle.py, pinned to the reference) and against what the reference itself wrote
 (tests/golden/train_audio.npz).
 
-Bars: records exactly as a PNB_TRAIN_DATA engine writes them; audio within 1 LSB of the oracle and of the reference.
-The device's synthesis transform is not bit-exact, and about 0.6 % of g labels differ by an ulp through the
-post-filter's sinf, so a sample may truncate to the neighbouring integer.  At least 99 % of the samples must be
-identical (measured on an H100 80GB HBM3 at 700 W: 100 % against the oracle and against the reference, every sample
-of these inputs, so the floor leaves room for a 1-LSB truncation difference somewhere else).
+Bars: records exactly as a PNB_TRAIN_DATA engine writes them.  At the synthesis kernel's own inputs -- the labels
+the device wrote and its analysis taps of the noisy rows -- the audio is bit-identical to the restatement
+(tests/synthesis_oracle.py), clamped samples included: the device's synthesis is the reference's operation for
+operation.  Against the oracle's own records and the reference's files the audio is within 1 LSB: about 0.6 % of g
+labels differ by an ulp through the post-filter's sinf (the device rounds a double sine), so a sample may truncate to the
+neighbouring integer.  At least 99 % of the samples must be identical there (measured on an H100 80GB HBM3 at 700 W:
+100 % against the oracle and against the reference, every sample of these inputs).
 """
 import os
 
@@ -15,6 +17,7 @@ import numpy as np
 import pytest
 
 from conftest import GOLDEN
+from synthesis_oracle import FRAME, synthesize, to_short
 from train_audio_oracle import train_audio
 from util import same_bits
 
@@ -87,6 +90,35 @@ def test_audio_matches_oracle_and_records_unchanged(api, oracle):
     plain = api.Engine(2 * N, F, None, api.TRAIN_DATA)
     assert same_bits(rec, plain.train_records(clean, noisy))
     plain.close()
+
+
+def _clamping_pair(n_frames):
+    """A pair loud enough that the resynthesis leaves the int16 range (as tests/test_oracle_train_audio.py builds it)."""
+    t = np.arange(n_frames * FRAME) / 48000.0
+    sq = np.sign(np.sin(2 * np.pi * 150 * t)) + 0.6 * np.sign(np.sin(2 * np.pi * 450 * t + 1))
+    return np.clip(np.rint(sq * 32767), -32768, 32767).astype(np.int16)
+
+
+def test_audio_at_own_inputs_bit_exact(api, oracle):
+    """The audio equals the synthesis composed from each record's g/r and the noisy rows' X, P and silence taps,
+    followed by train()'s clamp, sample for sample, on the pairs above plus one that clamps at both ends."""
+    clean, noisy, F = _pairs()
+    loud = _clamping_pair(F)
+    clean, noisy = np.concatenate([clean, loud[None]]), np.concatenate([noisy, loud[None]])
+    N = clean.shape[0]
+    eng = api.Engine(2 * N, F, None, api.TRAIN_DATA | api.TRAIN_AUDIO | api.KEEP_TAPS)
+    rec, audio = eng.train_audio(clean, noisy)
+    X, P, sil = eng.read_tap("X", F), eng.read_tap("P", F), eng.read_tap("pitch", F)[..., 2]
+    eng.close()
+    hw, _ = oracle.tables()
+    for p in range(N):                                          # the noisy file of pair p is row p
+        mem = np.zeros(FRAME, np.float32)
+        want = np.concatenate([to_short(synthesize(oracle, X[t, p], P[t, p], sil[t, p], rec[p, t, 70:104],
+                                                   rec[p, t, 104:138], mem, hw)) for t in range(F)])
+        d = np.nonzero(audio[p] != want)[0]
+        assert d.size == 0, (p, d.size, d[0], int(audio[p, d[0]]), int(want[d[0]]))
+    assert np.any(audio[N - 1] == 32767) and np.any(audio[N - 1] == -32768)
+    assert np.mean(sil[:, :5]) < 0.25 and np.all(sil[:, 5])        # the comb branch and the silent branch both ran
 
 
 def test_call_grouping_reset_and_device_entry(api):

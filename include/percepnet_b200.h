@@ -71,9 +71,18 @@ enum {
                             per engine, never per input, so a stream's result does not depend on its neighbours.          */
   PNB_TRAIN_DATA = 8,    /* training-data generator (pnb_train_records_*): n_streams = 2 x pairs, no network,
                             no synthesis; model may be NULL; the pnb_process_* entry points are refused      */
-  PNB_TRAIN_AUDIO = 32   /* with PNB_TRAIN_DATA only: the generator also resynthesises every noisy file with its own
+  PNB_TRAIN_AUDIO = 32,  /* with PNB_TRAIN_DATA only: the generator also resynthesises every noisy file with its own
                             labels, as train() writes test_output.pcm (pnb_train_audio_*, which replace
                             pnb_train_records_* / pnb_submit_train_records on such an engine)                 */
+  PNB_NETWORK_ONLY = 64  /* the network alone: an engine for pnb_compute_rnn_* and pnb_score_records_*, without the
+                            signal-path buffers of a PCM engine (history lines, overlap-add and pitch memory, spectrum
+                            rings, per-call spectra; about 14.7 GB at 16 384 streams x 100 hops).  pnb_process_*,
+                            pnb_submit_*, pnb_train_* and pnb_sessions_reserve are refused with PNB_ERR_ARG before
+                            anything is enqueued.  Not with PNB_TRAIN_DATA, PNB_TRAIN_AUDIO or PNB_POSTFILTER; with
+                            PNB_KEEP_TAPS the features, g/r and PNB_TAP_NN_* taps are readable and the other taps are
+                            refused.  State blobs: export writes the network part and zeroes the signal part, import
+                            takes the network part and ignores the signal part, so blobs move both ways between this
+                            engine and a PCM engine of the same network path. */
 };
 
 typedef struct pnb_engine pnb_engine;
@@ -208,6 +217,29 @@ int pnb_compute_rnn_device(pnb_engine *e, int format, const float *d_in, size_t 
                            float *d_gr, size_t gr_stride, void *cuda_stream);
 int pnb_compute_rnn_host(pnb_engine *e, int format, const float *in, size_t in_stride, int n_frames,
                          float *gr, size_t gr_stride);
+
+/* Scoring on the device: pnb_compute_rnn_* on training records (PNB_RNN_RECORDS) with rnn_train.py's CustomLoss
+ * (rnn_train.py:153-176, gamma = 0.5) reduced against the records' own labels, so only four numbers per row leave the
+ * device.  The network input is staged and the network state advanced exactly as a pnb_compute_rnn_* call of the same
+ * records does.
+ *   rec / d_rec  the active rows [0, n) of records, as pnb_compute_rnn_* takes them; rec_stride >= n_frames * 138.
+ *   frames       host array of n ints in [0, n_frames] (reusable when the call returns), or NULL for n_frames each:
+ *                row i's loss counts its first frames[i] hops only (the padding of a shorter file drops out).  Every
+ *                row still advances by n_frames hops.
+ *   sums / d_sums  overwritten with n x 4 float64: {sum dg^2, sum dg^4, sum dr^2, count} per row, over the counted hops
+ *                and the 34 bands, where dg = sqrt(g) - sqrt(g_hat), dr = sqrt(1 - r) - sqrt(1 - r_hat), the labels
+ *                g, r = rec[t][70..103], rec[t][104..137] and count = 34 * frames[i].  CustomLoss's terms are
+ *                sum dg^2 / count, 10 sum dg^4 / count and sum dr^2 / count.  NaN propagates (a label r > 1 makes
+ *                that row's sum dr^2 NaN).  A row's sums depend on its own records only, in a fixed order: they are the
+ *                same bits whatever other rows, n_streams or active range the call has.
+ *   gr / d_gr    NULL, or g/r written as pnb_compute_rnn_* writes them (same bits), gr_stride >= n_frames * 68.
+ * Allowed where pnb_compute_rnn_* is (PCM and PNB_NETWORK_ONLY engines); ordering, blocking, PNB_ERR_DOMAIN and the
+ * refusals are pnb_compute_rnn_*'s, and also NULL sums and frames[i] outside [0, n_frames].  A call without gr issues
+ * as many launches as a pnb_compute_rnn_* call of n_frames hops; with gr, one more. */
+int pnb_score_records_device(pnb_engine *e, const float *d_rec, size_t rec_stride, int n_frames, const int *frames,
+                             double *d_sums, float *d_gr, size_t gr_stride, void *cuda_stream);
+int pnb_score_records_host(pnb_engine *e, const float *rec, size_t rec_stride, int n_frames, const int *frames,
+                           double *sums, float *gr, size_t gr_stride);
 
 /* Per-stream state for migration between engines / GPUs (the live part of the reference's DenoiseState + RNNState,
  * src/denoise.cpp:71-85, src/nnet_data.h:28-38): input history, overlap-add memory, pitch continuity, the spectra the
@@ -371,8 +403,12 @@ long long pnb_launch_count(const pnb_engine *e);
 /* Kernel launches one pnb_process_* call with n_frames hops issues (one more on the calls that also move the
  * streams' history back to the start of their rows, at most every call, typically every eighth; one more on a ragged
  * session call in which some session runs fewer than n_frames = max(hops) hops).  On a PNB_TRAIN_AUDIO engine it is the
- * value of a PNB_TRAIN_DATA engine of the same shape plus one: the resynthesis launch. */
+ * value of a PNB_TRAIN_DATA engine of the same shape plus one: the resynthesis launch.  On a PNB_NETWORK_ONLY engine it
+ * is the launch count of one pnb_compute_rnn_* call of n_frames hops. */
 int pnb_launches_per_call(const pnb_engine *e, int n_frames);
+/* Bytes of the engine's device buffers whose size pnb_create fixes (weights, network buffers, stream state, per-call
+ * scratch); not the staging that host-buffer calls grow on first use, nor a session pool's parking area. */
+size_t pnb_engine_bytes(const pnb_engine *e);
 int pnb_n_streams(const pnb_engine *e);
 int pnb_max_frames(const pnb_engine *e);
 const char *pnb_last_error(void);

@@ -18,7 +18,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "libpercepnet_b200.so")
 
 FRAME = 480
-NN_FP32, NN_TENSOR, POSTFILTER, KEEP_TAPS, TRAIN_DATA, CONV_WIDE, TRAIN_AUDIO = 0, 1, 2, 4, 8, 16, 32
+NN_FP32, NN_TENSOR, POSTFILTER, KEEP_TAPS, TRAIN_DATA, CONV_WIDE, TRAIN_AUDIO, NETWORK_ONLY = 0, 1, 2, 4, 8, 16, 32, 64
 RECORD = 138
 RNN_FEATURES, RNN_RECORDS = 0, 1   # pnb_compute_rnn_* formats: 70 features or 138 record floats per hop
 TAPS = {"features": (0, np.float32, 70), "pitch": (1, np.int32, 4), "pitchf": (2, np.float32, 2),
@@ -65,6 +65,10 @@ def load_library() -> C.CDLL:
     L.pnb_submit_device_i16.argtypes = [vp, vp, sz, vp, sz, i, vp]
     L.pnb_compute_rnn_device.argtypes = [vp, i, vp, sz, i, vp, sz, vp]
     L.pnb_compute_rnn_host.argtypes = [vp, i, vp, sz, i, vp, sz]
+    L.pnb_score_records_device.argtypes = [vp, vp, sz, i, vp, vp, vp, sz, vp]
+    L.pnb_score_records_host.argtypes = [vp, vp, sz, i, vp, vp, vp, sz]
+    L.pnb_engine_bytes.argtypes = [vp]
+    L.pnb_engine_bytes.restype = sz
     L.pnb_flush.argtypes = [vp, vp]
     L.pnb_wait.argtypes = [vp]
     L.pnb_check.argtypes = [vp, vp]
@@ -110,7 +114,8 @@ def load_library() -> C.CDLL:
 
 EXPORTS = ("pnb_create", "pnb_destroy", "pnb_reset", "pnb_resolve_device", "pnb_process_host_f32", "pnb_process_host_i16",
            "pnb_model_load_blob", "pnb_model_load_stream", "pnb_model_free", "pnb_train_records_host", "pnb_train_records_device", "pnb_submit_train_records", "pnb_train_audio_host", "pnb_train_audio_device", "pnb_process_device_f32", "pnb_process_device_i16", "pnb_submit_host_f32", "pnb_submit_host_i16", "pnb_submit_device_f32", "pnb_submit_device_i16", "pnb_flush", "pnb_wait", "pnb_check",
-           "pnb_compute_rnn_device", "pnb_compute_rnn_host",
+           "pnb_compute_rnn_device", "pnb_compute_rnn_host", "pnb_score_records_device", "pnb_score_records_host",
+           "pnb_engine_bytes",
            "pnb_read_tap", "pnb_state_size", "pnb_get_state", "pnb_set_state",
            "pnb_reset_streams", "pnb_export_states", "pnb_import_states", "pnb_set_active_streams", "pnb_active_streams",
            "pnb_sessions_reserve", "pnb_process_sessions_device_f32", "pnb_process_sessions_device_i16",
@@ -268,6 +273,41 @@ class Engine:
         """pnb_compute_rnn_device on raw device pointers (format RNN_FEATURES or RNN_RECORDS; strides in floats)."""
         self._ck(self.L.pnb_compute_rnn_device(self.h, format, d_in or None, in_stride, n_frames, d_gr or None, gr_stride,
                                                stream or None), "pnb_compute_rnn_device")
+
+    def score_records(self, x: np.ndarray, frames=None, want_gr: bool = False):
+        """pnb_score_records_host: compute_rnn on records x ([active, F, 138] float32) with rnn_train.py's CustomLoss
+        reduced on the device against their labels.  frames: None, or one count in [0, F] per row: row i's loss counts
+        its first frames[i] hops (every row still advances F hops).  Returns (sums [active, 4] float64 = {sum dg^2,
+        sum dg^4, sum dr^2, count} per row, as eval_records.loss_sums computes them; g/r [active, F, 68] or None)."""
+        n = self.active
+        if x.dtype != np.float32:
+            raise TypeError("x must be float32")
+        assert x.ndim == 3 and x.shape[0] == n and x.shape[2] == RECORD, "x must be [active, F, 138]"
+        F = x.shape[1]
+        x = np.ascontiguousarray(x)
+        fr = None if frames is None else self._slots(frames)[0]
+        if fr is not None and len(fr) != n:
+            raise PnbError("score_records: frames needs one entry per active row")
+        sums = np.empty((n, 4), np.float64)
+        gr = np.empty((n, F, 68), np.float32) if want_gr else None
+        self._ck(self.L.pnb_score_records_host(self.h, x.ctypes.data, F * RECORD, F, None if fr is None else fr.ctypes.data,
+                                               sums.ctypes.data, gr.ctypes.data if want_gr else None, F * 68),
+                 "pnb_score_records_host")
+        return sums, gr
+
+    def score_records_device(self, d_rec: int, rec_stride: int, n_frames: int, frames, d_sums: int, d_gr: int = 0,
+                             gr_stride: int = 0, stream: int = 0):
+        """pnb_score_records_device on raw device pointers (strides in floats); frames: None or a host sequence of one
+        count per active row; d_sums: [active, 4] float64; d_gr: 0 for no g/r."""
+        fr = None if frames is None else self._slots(frames)[0]
+        self._ck(self.L.pnb_score_records_device(self.h, d_rec or None, rec_stride, n_frames,
+                                                 None if fr is None else fr.ctypes.data, d_sums or None, d_gr or None,
+                                                 gr_stride, stream or None), "pnb_score_records_device")
+
+    @property
+    def device_bytes(self) -> int:
+        """pnb_engine_bytes: the engine's fixed-size device buffers, in bytes."""
+        return int(self.L.pnb_engine_bytes(self.h))
 
     def flush(self, stream: int = 0):
         self._ck(self.L.pnb_flush(self.h, stream or None), "pnb_flush")

@@ -156,8 +156,11 @@ extern "C" int pnb_create(pnb_engine **out, int n_streams, int max_frames, const
   if (train_audio && !train_mode) return fail(PNB_ERR_ARG, "PNB_TRAIN_AUDIO applies to PNB_TRAIN_DATA engines");
   if (train_mode && (n_streams & 1)) return fail(PNB_ERR_ARG, "PNB_TRAIN_DATA needs n_streams = 2 x pairs");
   if ((flags & PNB_CONV_WIDE) && !(flags & PNB_NN_TENSOR)) return fail(PNB_ERR_ARG, "PNB_CONV_WIDE applies to PNB_NN_TENSOR engines");
-  if (train_mode && (flags & (PNB_NN_TENSOR | PNB_POSTFILTER)))
+  if (train_mode && (flags & (PNB_NN_TENSOR | PNB_POSTFILTER | PNB_NETWORK_ONLY)))
     return fail(PNB_ERR_ARG, "PNB_TRAIN_DATA runs no network: combine it only with PNB_KEEP_TAPS");
+  const bool net_only = (flags & PNB_NETWORK_ONLY) != 0;
+  if (net_only && (flags & (PNB_TRAIN_AUDIO | PNB_POSTFILTER)))
+    return fail(PNB_ERR_ARG, "PNB_NETWORK_ONLY runs no signal path: PNB_TRAIN_AUDIO and PNB_POSTFILTER do not apply");
   int rc = train_mode ? 0 : check_model(model);
   if (rc) return rc;
   device = pnb_resolve_device(device);
@@ -205,9 +208,11 @@ extern "C" int pnb_create(pnb_engine **out, int n_streams, int max_frames, const
   // room for several calls' hops behind the history (advance_line): eight calls when calls are short, fewer
   // when one call already carries many hops (the move is then amortised over those hops anyway)
   const size_t line_calls = F >= 128 ? 1 : (128 / F > (size_t)kLineCalls ? (size_t)kLineCalls : 128 / F);
-  e->pcm_stride = kKeep + line_calls * F * kFrame;
-  CKD(engine_alloc(e, &e->d_pcm, S * e->pcm_stride, kStreamState));
-  CKD(engine_alloc(e, &e->d_synth, S * kFrame, kStreamState));
+  if (!net_only) {  // a network-only engine has no signal path: none of its buffers, here and below
+    e->pcm_stride = kKeep + line_calls * F * kFrame;
+    CKD(engine_alloc(e, &e->d_pcm, S * e->pcm_stride, kStreamState));
+    CKD(engine_alloc(e, &e->d_synth, S * kFrame, kStreamState));
+  }
   CKD(engine_alloc(e, &e->d_status, 2, kScratch));  // pnb_reset sets it itself
   CKD(cudaMemset(e->d_status + 1, 0x7F, sizeof(int)));  // kNoRejectedSlot
   CKD(cudaHostAlloc((void **)&e->h_status, 2 * sizeof(int), cudaHostAllocDefault));
@@ -225,19 +230,23 @@ extern "C" int pnb_create(pnb_engine **out, int n_streams, int max_frames, const
   CKD(cudaMalloc((void **)&e->d_ok, S * sizeof(int)));
   e->ok_cap = S;
   CKD(engine_buffer(e, &e->d_blob1, sizeof(StreamState), kScratch, nullptr));
-  CKD(engine_alloc(e, &e->d_last_period, S, kStreamState));
-  CKD(engine_alloc(e, &e->d_last_gain, S, kStreamState));
+  if (!net_only) {
+    CKD(engine_alloc(e, &e->d_last_period, S, kStreamState));
+    CKD(engine_alloc(e, &e->d_last_gain, S, kStreamState));
+  }
   // per-call buffers
   CKD(engine_alloc(e, &e->d_feat, F * S * kFeat, kScratch));
-  e->ring = (int)F + 5;
-  CKD(engine_alloc(e, &e->d_zring, (size_t)e->ring * S * kBins, kStreamState));
-  CKD(engine_alloc(e, &e->d_ering, (size_t)e->ring * S * kBands, kStreamState));
-  if (!train_mode || train_audio) CKD(engine_alloc(e, &e->d_P, F * S * kBins, kScratch));  // audio: noisy rows only
-  CKD(engine_alloc(e, &e->d_Ex, F * S * kBands, kScratch));
-  CKD(engine_alloc(e, &e->d_sil, F * S, kScratch));
+  if (!net_only) {
+    e->ring = (int)F + 5;
+    CKD(engine_alloc(e, &e->d_zring, (size_t)e->ring * S * kBins, kStreamState));
+    CKD(engine_alloc(e, &e->d_ering, (size_t)e->ring * S * kBands, kStreamState));
+    if (!train_mode || train_audio) CKD(engine_alloc(e, &e->d_P, F * S * kBins, kScratch));  // audio: noisy rows only
+    CKD(engine_alloc(e, &e->d_Ex, F * S * kBands, kScratch));
+    CKD(engine_alloc(e, &e->d_sil, F * S, kScratch));
+  }
   if (!train_mode || train_audio) CKD(engine_alloc(e, &e->d_gr, F * S * 68, kScratch));  // audio: the noisy rows' labels
   if (train_mode) CKD(engine_alloc(e, &e->d_raw, F * S * 68, kScratch));
-  if (flags & PNB_KEEP_TAPS) {
+  if ((flags & PNB_KEEP_TAPS) && !net_only) {  // the taps a network-only engine keeps need no buffers of their own
     CKD(engine_alloc(e, &e->d_tap_pitch, F * S * 4, kScratch));
     CKD(engine_alloc(e, &e->d_tap_pitchf, F * S * 2, kScratch));
     if (!train_mode) CKD(engine_alloc(e, &e->d_tap_g, F * S * kBands, kScratch));
@@ -425,12 +434,15 @@ static int mark_call_end(pnb_engine *e, cudaStream_t st) {
   return PNB_OK;
 }
 
-// What every call checks before it allocates or enqueues anything: an engine of the call's family (training records
-// or enhancement) that no failed call has poisoned, 1 <= F <= Fmax, its buffers (`buffers`: none is NULL), and two
-// row strides of at least F hops (of width_a / width_b values each: 480 samples unless a network call says otherwise).
-static int check_call(const pnb_engine *e, bool train, bool buffers, int F, size_t stride_a, size_t stride_b,
+// What every call checks before it allocates or enqueues anything: an engine of the call's family (training records,
+// enhancement or the network alone; a PNB_NETWORK_ONLY engine runs network calls only) that no failed call has
+// poisoned, 1 <= F <= Fmax, its buffers (`buffers`: none is NULL), and two row strides of at least F hops (of width_a /
+// width_b values each: 480 samples unless a network call says otherwise).
+static int check_call(const pnb_engine *e, bool train, bool network, bool buffers, int F, size_t stride_a, size_t stride_b,
                       size_t width_a = kFrame, size_t width_b = kFrame) {
   if (!e) return fail(PNB_ERR_ARG, "engine is NULL");
+  if (!network && (e->flags & PNB_NETWORK_ONLY))
+    return fail(PNB_ERR_ARG, "engine was created with PNB_NETWORK_ONLY: use pnb_compute_rnn_* / pnb_score_records_*");
   if (train && !(e->flags & PNB_TRAIN_DATA)) return fail(PNB_ERR_ARG, "engine was not created with PNB_TRAIN_DATA");
   if (!train && (e->flags & PNB_TRAIN_DATA))
     return fail(PNB_ERR_ARG, "engine was created with PNB_TRAIN_DATA: use pnb_train_records_* / pnb_submit_train_records");
@@ -445,7 +457,7 @@ static int check_call(const pnb_engine *e, bool train, bool buffers, int F, size
 static int check_train(const pnb_engine *e, const short *speech, size_t speech_stride, const short *noisy, size_t noisy_stride,
                        int F, const float *records, size_t records_stride, bool audio_call = false,
                        const short *audio = nullptr, size_t audio_stride = 0) {
-  const int rc = check_call(e, true, speech && noisy && records && (audio || !audio_call), F, speech_stride, noisy_stride);
+  const int rc = check_call(e, true, false, speech && noisy && records && (audio || !audio_call), F, speech_stride, noisy_stride);
   if (rc) return rc;
   if (audio_call && !(e->flags & PNB_TRAIN_AUDIO)) return fail(PNB_ERR_ARG, "engine was not created with PNB_TRAIN_AUDIO");
   if (!audio_call && (e->flags & PNB_TRAIN_AUDIO))
@@ -553,7 +565,8 @@ static int enqueue_plan(pnb_engine *e, const int *ids, int k, const int *hops, i
 
 // One enhancement call as its entry point received it: rows of float samples, or of int16 samples (i16), in and out, in
 // host or device memory by entry point.  A network call (kNetwork, pnb_compute_rnn_*) reads rows of features or
-// training records (format) and writes rows of g/r to out instead.
+// training records (format) and writes rows of g/r to out instead; a score call (pnb_score_records_*) is a network call
+// on records with sums, whose out (g/r) may be null.
 struct Call {
   enum Kind { kSlots, kSessions, kRagged, kNetwork } kind;
   const void *in;
@@ -567,19 +580,25 @@ struct Call {
   int n_ids;
   const int *hops;  // ragged calls: each listed session's hops (host); null once check_enhance finds them all equal to F
   int format;       // network calls: PNB_RNN_FEATURES or PNB_RNN_RECORDS
+  bool score;         // a score call: a network call on records that writes sums, and g/r to out only when out is set
+  double *sums;       // score calls: the loss sums [rows][4] (in the entry point's memory)
+  const int *frames;  // score calls: the hops each row's loss counts (host), or null for F
   // values per hop of an input / output row: 480 samples, or a network call's 70 features / 138 record floats and 68 g/r
+  // (0: a score call that writes no g/r)
   size_t in_width() const { return kind != kNetwork ? kFrame : format == PNB_RNN_RECORDS ? PNB_RECORD_FLOATS : kFeat; }
-  size_t out_width() const { return kind != kNetwork ? kFrame : 68; }
+  size_t out_width() const { return kind != kNetwork ? kFrame : (out || !score) ? 68 : 0; }
 };
 
 // A network call on st (arguments already checked): the caller's rows into the features buffer, the network hook, its
-// g/r out to the caller's rows.  The signal state (history line, overlap-add, pitch memory, spectrum ring, hop
-// counter, line offset) is not touched.
+// g/r out to the caller's rows; a score call reduces the loss from the same g/r and writes g/r only when asked.  The
+// signal state (history line, overlap-add, pitch memory, spectrum ring, hop counter, line offset) is not touched.
 static int enqueue_network(pnb_engine *e, const Call &c, cudaStream_t st) {
   const int F = c.F;
   return enqueue_call(e, F, st, [&]() -> int {
     const int S = e->S, na = e->n_active;
     int n = 0;
+    const int *frames = nullptr;  // a score call's per-row hop counts, staged like a ragged call's hops
+    if (c.frames) { int rc = stage_ints(e, c.frames, (size_t)na, st, &frames); if (rc) return rc; }
     {
       ProfScope ps(e, PNB_K_STAGE_IN, st);
       n += launch_features_stage(e->d_feat, static_cast<const float *>(c.in), c.in_stride, (int)c.in_width(), na, S, F, st);
@@ -590,7 +609,11 @@ static int enqueue_network(pnb_engine *e, const Call &c, cudaStream_t st) {
       if (q < 0) return q;
       n += q;
     }
-    { ProfScope ps(e, PNB_K_STAGE_IN, st); n += launch_gr_store(e->d_gr, static_cast<float *>(c.out), c.out_stride, na, S, F, st); }
+    if (c.score) {
+      ProfScope ps(e, PNB_K_STAGE_IN, st);
+      n += launch_loss_sums(e->d_gr, static_cast<const float *>(c.in), c.in_stride, frames, c.sums, na, S, F, st);
+    }
+    if (c.out) { ProfScope ps(e, PNB_K_STAGE_IN, st); n += launch_gr_store(e->d_gr, static_cast<float *>(c.out), c.out_stride, na, S, F, st); }
     return n;
   }, false);
 }
@@ -693,11 +716,19 @@ static int check_enhance(pnb_engine *e, Call &c) {
     for (int i = 0; i < c.n_ids; i++) uniform = uniform && c.hops[i] == c.F;
     if (uniform) c.hops = nullptr;
   }
-  { int rc = check_call(e, false, c.in && c.out, c.F, c.in_stride, c.out_stride, c.in_width(), c.out_width()); if (rc) return rc; }
+  const bool network = c.kind == Call::kNetwork;
+  {
+    int rc = check_call(e, false, network, c.in && (c.score ? c.sums != nullptr : c.out != nullptr), c.F, c.in_stride,
+                        c.out_stride, c.in_width(), c.out_width());
+    if (rc) return rc;
+  }
   if (c.kind == Call::kSessions) return check_ids(e, c.ids, c.n_ids, e->S);
-  if (c.kind == Call::kNetwork && c.format != PNB_RNN_FEATURES && c.format != PNB_RNN_RECORDS)
+  if (network && c.format != PNB_RNN_FEATURES && c.format != PNB_RNN_RECORDS)
     return fail(PNB_ERR_ARG, "format %d is neither PNB_RNN_FEATURES (0) nor PNB_RNN_RECORDS (1)", c.format);
-  if ((c.kind == Call::kSlots || c.kind == Call::kNetwork) && e->sessions) return refuse_in_session_mode();
+  if ((c.kind == Call::kSlots || network) && e->sessions) return refuse_in_session_mode();
+  if (c.score && c.frames)  // every row's counted hops in [0, F]
+    for (int i = 0; i < e->n_active; i++)
+      if (c.frames[i] < 0 || c.frames[i] > c.F) return fail(PNB_ERR_ARG, "frames[%d] = %d outside [0, %d]", i, c.frames[i], c.F);
   return PNB_OK;
 }
 
@@ -933,14 +964,21 @@ static int host_call(pnb_engine *e, Call c, bool pipelined) {
   if (c.ids && c.gr) { int rc = grow((void **)&e->d_sgr, &e->sgr_bytes, (size_t)e->Fmax * S * 68 * sizeof(float)); if (rc) return rc; }
   Call d = c;  // the call on staging slot k
   d.in = e->stage[k].in;
-  d.out = e->stage[k].out;
+  d.out = c.out ? e->stage[k].out : nullptr;
   d.in_stride = row_in;
   d.out_stride = row_out;
   d.gr = c.ids && c.gr ? e->d_sgr : nullptr;  // session calls gather g/r in list order on the device
+  // a score call's sums follow the g/r rows in the output slot (row_out <= row: the slot has room for both)
+  d.sums = c.score ? reinterpret_cast<double *>(static_cast<char *>(e->stage[k].out) + ((S * row_out * es + 15) & ~(size_t)15)) : nullptr;
   const int rc = round_trip(e, k, pipelined,
       [&](cudaStream_t s) { return cudaMemcpy2DAsync(e->stage[k].in, row_in * es, c.in, c.in_stride * es, w_in, na, cudaMemcpyHostToDevice, s); },
       [&] { return enqueue_enhance(e, d, e->stream); },
-      [&](cudaStream_t s) { return cudaMemcpy2DAsync(c.out, c.out_stride * es, e->stage[k].out, row_out * es, w_out, na, cudaMemcpyDeviceToHost, s); });
+      [&](cudaStream_t s) {
+        const cudaError_t ce = c.out ? cudaMemcpy2DAsync(c.out, c.out_stride * es, e->stage[k].out, row_out * es, w_out, na,
+                                                         cudaMemcpyDeviceToHost, s)
+                                     : cudaSuccess;
+        return ce != cudaSuccess || !c.score ? ce : cudaMemcpyAsync(c.sums, d.sums, na * 4 * sizeof(double), cudaMemcpyDeviceToHost, s);
+      });
   if (rc || pipelined) return rc;
   if (d.gr)
     CK(cudaMemcpyAsync(c.gr, d.gr, (size_t)c.F * na * 68 * sizeof(float), cudaMemcpyDeviceToHost, e->stream));
@@ -983,6 +1021,25 @@ extern "C" int pnb_compute_rnn_host(pnb_engine *e, int format, const float *in, 
   return host_call(e, c, false);
 }
 
+// A network call on records that also reduces rnn_train.py's loss against their labels on the device.
+static Call score_call(const float *rec, size_t rec_stride, int n_frames, const int *frames, double *sums, float *gr,
+                       size_t gr_stride) {
+  Call c{Call::kNetwork, rec, rec_stride, gr, gr_stride, false, n_frames, nullptr};
+  c.format = PNB_RNN_RECORDS;
+  c.score = true;
+  c.sums = sums;
+  c.frames = frames;
+  return c;
+}
+extern "C" int pnb_score_records_device(pnb_engine *e, const float *d_rec, size_t rec_stride, int n_frames, const int *frames,
+                                        double *d_sums, float *d_gr, size_t gr_stride, void *cuda_stream) {
+  return device_call(e, score_call(d_rec, rec_stride, n_frames, frames, d_sums, d_gr, gr_stride), (cudaStream_t)cuda_stream);
+}
+extern "C" int pnb_score_records_host(pnb_engine *e, const float *rec, size_t rec_stride, int n_frames, const int *frames,
+                                      double *sums, float *gr, size_t gr_stride) {
+  return host_call(e, score_call(rec, rec_stride, n_frames, frames, sums, gr, gr_stride), false);
+}
+
 extern "C" int pnb_flush(pnb_engine *e, void *cuda_stream) {
   if (!e) return fail(PNB_ERR_ARG, "engine is NULL");
   CK(cudaSetDevice(e->device));
@@ -1020,6 +1077,7 @@ extern "C" int pnb_read_tap(pnb_engine *e, int what, void *dst, size_t dst_bytes
     case PNB_TAP_PITCH: src = e->d_tap_pitch; bytes = n * 16; break;
     case PNB_TAP_PITCHF: src = e->d_tap_pitchf; bytes = n * 8; break;
     case PNB_TAP_X: {  // gather from the ring: the analysis spectrum of hop c is the slot of hop c-5
+      if (!e->d_zring) return fail(PNB_ERR_ARG, "tap %d: a PNB_NETWORK_ONLY engine has no spectra", what);
       bytes = n * kBins * 8;
       if (dst_bytes < bytes) return fail(PNB_ERR_ARG, "tap %d needs %zu bytes, got %zu", what, bytes, dst_bytes);
       CK(cudaDeviceSynchronize());
@@ -1042,6 +1100,8 @@ extern "C" int pnb_read_tap(pnb_engine *e, int what, void *dst, size_t dst_bytes
     }
     default: return fail(PNB_ERR_ARG, "unknown tap %d", what);
   }
+  if (!src && (e->flags & PNB_NETWORK_ONLY))
+    return fail(PNB_ERR_ARG, "tap %d: a PNB_NETWORK_ONLY engine keeps the features, g/r and network state taps only", what);
   if (!src) return fail(PNB_ERR_ARG, "tap %d needs PNB_KEEP_TAPS at pnb_create", what);
   if (dst_bytes < bytes) return fail(PNB_ERR_ARG, "tap %d needs %zu bytes, got %zu", what, bytes, dst_bytes);
   CK(cudaDeviceSynchronize());
@@ -1194,6 +1254,7 @@ static int grow_ints(pnb_engine *e, size_t n) {
 extern "C" int pnb_sessions_reserve(pnb_engine *e, int n_sessions) {
   if (!e) return fail(PNB_ERR_ARG, "engine is NULL");
   if (e->flags & PNB_TRAIN_DATA) return fail(PNB_ERR_ARG, "PNB_TRAIN_DATA engines have no session pool");
+  if (e->flags & PNB_NETWORK_ONLY) return fail(PNB_ERR_ARG, "PNB_NETWORK_ONLY engines have no session pool");
   if (e->poisoned) return fail(PNB_ERR_ARG, "an earlier call failed while enqueuing work; the streams' state is undefined until pnb_reset");
   if (n_sessions < 1) return fail(PNB_ERR_ARG, "n_sessions = %d, need >= 1", n_sessions);
   if (e->sessions && n_sessions <= e->pool.capacity()) return PNB_OK;  // the pool never shrinks
@@ -1467,9 +1528,17 @@ extern "C" int pnb_launches_per_call(const pnb_engine *e, int n_frames) {
   if (!e) return 0;
   // stage_in, analysis, the network, synthesis; without the history move of advance_line (at most one more launch per
   // call), and without the fix-up of a ragged session call in which a session runs fewer hops than the call (one more);
-  // the resynthesis of a PNB_TRAIN_AUDIO engine is one launch more than its records alone
-  return 3 + ((e->flags & PNB_NN_TENSOR) ? tc_network_launches(e, n_frames) : f32_network_launches(e, n_frames)) +
-         ((e->flags & PNB_TRAIN_AUDIO) ? 1 : 0);
+  // the resynthesis of a PNB_TRAIN_AUDIO engine is one launch more than its records alone; a PNB_NETWORK_ONLY engine's
+  // call is pnb_compute_rnn_*: features_stage, the network, gr_store
+  const int net = (e->flags & PNB_NN_TENSOR) ? tc_network_launches(e, n_frames) : f32_network_launches(e, n_frames);
+  if (e->flags & PNB_NETWORK_ONLY) return 2 + net;
+  return 3 + net + ((e->flags & PNB_TRAIN_AUDIO) ? 1 : 0);
+}
+extern "C" size_t pnb_engine_bytes(const pnb_engine *e) {
+  size_t n = 0;
+  if (e)
+    for (const auto &b : e->buffers) n += b.bytes;
+  return n;
 }
 extern "C" int pnb_n_streams(const pnb_engine *e) { return e ? e->S : 0; }
 extern "C" int pnb_max_frames(const pnb_engine *e) { return e ? e->Fmax : 0; }

@@ -96,5 +96,9 @@ int launch_features_stage(float *feat, const float *in, size_t in_stride, int wi
                           cudaStream_t st);
 // gr [F][S][68] -> rows [0, n_streams) of `out`, n_frames x 68 floats each
 int launch_gr_store(const float *gr, float *out, size_t out_stride, int n_streams, int S, int n_frames, cudaStream_t st);
+// rnn_train.py's CustomLoss sums of rows [0, n_streams): gr [F][S][68] against the labels rec[t][70..137] of row i's
+// first frames[i] hops (frames null: all n_frames) -> sums[i] = {sum dg^2, sum dg^4, sum dr^2, count} in float64
+int launch_loss_sums(const float *gr, const float *rec, size_t rec_stride, const int *frames, double *sums, int n_streams,
+                     int S, int n_frames, cudaStream_t st);
 
 }  // namespace pnb

@@ -1,6 +1,8 @@
-// pnb_rnn_io.cu -- the two copies of a network-only call (pnb_compute_rnn_*): the caller's stream-major rows of
+// pnb_rnn_io.cu -- the two copies of a network call (pnb_compute_rnn_*): the caller's stream-major rows of
 // features or training records into the per-call buffer [F][S][70] the network hooks read, and the hooks' g/r
-// [F][S][68] back out to stream-major rows.
+// [F][S][68] back out to stream-major rows; and the loss of a score call (pnb_score_records_*), reduced from the same
+// g/r and the records' labels.
+#include "../../include/percepnet_b200.h"
 #include "pnb_kernels.h"
 
 namespace pnb {
@@ -34,6 +36,51 @@ __global__ void gr_store_kernel(const float *__restrict__ gr, float *__restrict_
   }
 }
 
+// The loss rnn_train.py trains on (CustomLoss, rnn_train.py:153-176, gamma = 0.5), before its means and its C4 factor:
+// for row i, over its first frames[i] hops t and the 34 bands b, with y the label rec[t][70..137] and p the prediction
+// gr[t][i] (both widened to float64),
+//   dg = sqrt(y_g) - sqrt(p_g)    dr = sqrt(1 - y_r) - sqrt(1 - p_r)
+//   sums[i] = {sum dg^2, sum dg^4, sum dr^2, 34 frames[i]}
+// One warp per row walks its hops in order; lane l keeps the partials of bands l and l + 32 (lanes 0 and 1), and a
+// fixed shuffle tree adds the lanes.  No atomics: a row's sums depend on its own predictions and labels only, in a fixed
+// order, so they are the same bits whatever else the call holds.  Every product and sum is rounded on its own (no
+// contraction), as numpy's `** 0.5` (sqrt), `** 2` and the sums of eval_records.loss_sums round them; NaN (a label
+// r > 1, say) propagates the same way.
+__global__ void __launch_bounds__(256) loss_sums_kernel(const float *__restrict__ gr, const float *__restrict__ rec,
+                                                        size_t rec_stride, const int *__restrict__ frames,
+                                                        double *__restrict__ sums, int n, int S, int F) {
+  const int i = (int)(((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5), lane = threadIdx.x & 31;
+  if (i >= n) return;
+  const int T = frames ? frames[i] : F;
+  double g2 = 0.0, g4 = 0.0, r2 = 0.0;
+  const float *y = rec + (size_t)i * rec_stride + 70;
+  const float *p = gr + (size_t)i * 68;
+  auto band = [&](int t, int b) {
+    const double yg = y[(size_t)t * PNB_RECORD_FLOATS + b], yr = y[(size_t)t * PNB_RECORD_FLOATS + kBands + b];
+    const double pg = p[(size_t)t * S * 68 + b], pr = p[(size_t)t * S * 68 + kBands + b];
+    const double dg = __dsub_rn(sqrt(yg), sqrt(pg));
+    const double dr = __dsub_rn(sqrt(__dsub_rn(1.0, yr)), sqrt(__dsub_rn(1.0, pr)));
+    const double dg2 = __dmul_rn(dg, dg);
+    g2 = __dadd_rn(g2, dg2);
+    g4 = __dadd_rn(g4, __dmul_rn(dg2, dg2));
+    r2 = __dadd_rn(r2, __dmul_rn(dr, dr));
+  };
+#pragma unroll 4
+  for (int t = 0; t < T; t++) {
+    band(t, lane);
+    if (lane < kBands - 32) band(t, lane + 32);
+  }
+  for (int o = 16; o > 0; o >>= 1) {
+    g2 = __dadd_rn(g2, __shfl_down_sync(0xffffffffu, g2, o));
+    g4 = __dadd_rn(g4, __shfl_down_sync(0xffffffffu, g4, o));
+    r2 = __dadd_rn(r2, __shfl_down_sync(0xffffffffu, r2, o));
+  }
+  if (lane == 0) {
+    double *s = sums + (size_t)i * 4;
+    s[0] = g2; s[1] = g4; s[2] = r2; s[3] = (double)T * kBands;
+  }
+}
+
 static unsigned copy_blocks(long long total) {
   const long long b = (total + 255) / 256;
   return (unsigned)(b < 8192 ? b : 8192);
@@ -49,6 +96,13 @@ int launch_features_stage(float *feat, const float *in, size_t in_stride, int wi
 int launch_gr_store(const float *gr, float *out, size_t out_stride, int n_streams, int S, int n_frames, cudaStream_t st) {
   gr_store_kernel<<<copy_blocks((long long)n_frames * n_streams * 68), 256, 0, st>>>(gr, out, out_stride, n_streams, S,
                                                                                     n_frames);
+  return 1;
+}
+
+int launch_loss_sums(const float *gr, const float *rec, size_t rec_stride, const int *frames, double *sums, int n_streams,
+                     int S, int n_frames, cudaStream_t st) {
+  loss_sums_kernel<<<(unsigned)(((long long)n_streams * 32 + 255) / 256), 256, 0, st>>>(gr, rec, rec_stride, frames, sums,
+                                                                                      n_streams, S, n_frames);
   return 1;
 }
 

@@ -328,16 +328,21 @@ __global__ void state_clear_reject_kernel(int *status) {
 int state_segs(const pnb_engine *e, StateSeg *seg) {
   int ns = 0;
   const size_t S = e->S;
-  // signal state: the history line at line_off, overlap-add memory, pitch continuity, the five live spectrum slots
-  add_words(seg, ns, kSegCopy, e->d_pcm + e->line_off, e->pcm_stride * 4, offsetof(StreamState, pcm), kKeep);
-  add_words(seg, ns, kSegCopy, e->d_synth, kFrame * 4, offsetof(StreamState, synth), kFrame);
-  add_words(seg, ns, kSegCopy, e->d_last_period, 4, offsetof(StreamState, last_period), 1);
-  add_words(seg, ns, kSegCopy, e->d_last_gain, 4, offsetof(StreamState, last_gain), 1);
-  for (int k = 0; k < 5; k++) {
-    const long c = e->hop - 5 + k;
-    const size_t slot = (size_t)((c % e->ring + e->ring) % e->ring);
-    add_words(seg, ns, kSegCopy, e->d_zring + slot * S * kBins, kBins * 8, offsetof(StreamState, spec) + (size_t)k * kBins * 8, 2 * kBins);
-    add_words(seg, ns, kSegCopy, e->d_ering + slot * S * kBands, kBands * 4, offsetof(StreamState, eband) + (size_t)k * kBands * 4, kBands);
+  if (e->flags & PNB_NETWORK_ONLY) {  // no signal path: its part of the blob is zero on export and ignored on import
+    add_words(seg, ns, kSegBlobZero, nullptr, 0, offsetof(StreamState, pcm),
+              (offsetof(StreamState, fc_hist) - offsetof(StreamState, pcm)) / 4);
+  } else {
+    // signal state: the history line at line_off, overlap-add memory, pitch continuity, the five live spectrum slots
+    add_words(seg, ns, kSegCopy, e->d_pcm + e->line_off, e->pcm_stride * 4, offsetof(StreamState, pcm), kKeep);
+    add_words(seg, ns, kSegCopy, e->d_synth, kFrame * 4, offsetof(StreamState, synth), kFrame);
+    add_words(seg, ns, kSegCopy, e->d_last_period, 4, offsetof(StreamState, last_period), 1);
+    add_words(seg, ns, kSegCopy, e->d_last_gain, 4, offsetof(StreamState, last_gain), 1);
+    for (int k = 0; k < 5; k++) {
+      const long c = e->hop - 5 + k;
+      const size_t slot = (size_t)((c % e->ring + e->ring) % e->ring);
+      add_words(seg, ns, kSegCopy, e->d_zring + slot * S * kBins, kBins * 8, offsetof(StreamState, spec) + (size_t)k * kBins * 8, 2 * kBins);
+      add_words(seg, ns, kSegCopy, e->d_ering + slot * S * kBands, kBands * 4, offsetof(StreamState, eband) + (size_t)k * kBands * 4, kBands);
+    }
   }
   if (e->flags & PNB_TRAIN_DATA) {  // no network: its part of the blob is zero
     add_words(seg, ns, kSegBlobZero, nullptr, 0, offsetof(StreamState, fc_hist),

@@ -3,14 +3,18 @@
 
   python -m percepnet_b200.eval_records --model model.pnbw rec1.f32 rec2.f32 ...
   python -m percepnet_b200.eval_records --model model.pnbw --list files.txt [--tensor [--conv-wide]] [--batch 4096]
-                                        [--chunk 100] [--pred-dir DIR]
+                                        [--chunk 100] [--window N] [--pred-dir DIR]
 
 Each record file (138 float32 per frame: Ey_lookahead[34] Ephaty[34] T pitchcorr g[34] r[34], denoise.cpp:761-773)
-is one stream that starts from a fresh network state, which is how ``rnn_train.py`` sees a sequence.  Files are batched
-like ``gen_features.run_jobs``: sorted by length, ``--batch`` files per engine, the shorter ones zero-padded to the
-longest.  The padding is exact: the network is causal and the streams are independent, so frames after a file's end
-cannot change its earlier outputs; the outputs of padded frames are dropped.  A batch is fed in calls of ``--chunk``
-frames with the state carried between calls (pnb_compute_rnn_host, records format).
+is one stream that starts from a fresh network state.  With ``--window N`` each file is instead cut into consecutive
+N-frame windows (the last one may be shorter), and every window is a stream of its own that starts fresh: that is how
+``rnn_train.py`` sees its data (``CppRawListDataset`` reshapes every file to 500-frame sequences, ``h5Dataset`` cuts
+windows of 500), so ``--window 500`` on 500-frame files gives the loss a training run logs.  A file's sums are the sums
+of its windows.  Streams are batched like ``gen_features.run_jobs``: sorted by length, ``--batch`` streams per engine,
+the shorter ones zero-padded to the longest.  The padding is exact: the network is causal and the streams are
+independent, so frames after a stream's end cannot change its earlier outputs, and they are left out of its loss.  A
+batch is fed in calls of ``--chunk`` frames with the state carried between calls, on a network-only engine
+(PNB_NETWORK_ONLY, which holds none of the signal path's buffers).
 
 The network input is {30 * rec[0..67], rec[68], rec[69]}: the device scales the records exactly as ``create_features``
 (denoise.cpp:487-496) and ``rnn_train.py``'s ``CppRawListDataset`` (rnn_train.py:44-48) do, so the model sees what the
@@ -18,13 +22,15 @@ deployed network sees.  ``utils/bin2h5.py`` -> ``h5Dataset`` does NOT apply the 
 saw unscaled band energies, and the reference is inconsistent with itself there.  This tool follows the deployed one.
 
 For every file and over all files it prints the three terms of ``rnn_train.py``'s ``CustomLoss`` (rnn_train.py:153-176,
-gamma = 0.5, C4 = 10; means over frames and bands) and their total, computed in float64 on the host from the
-predictions and the labels rec[70..137]:
+gamma = 0.5, C4 = 10; means over frames and bands) and their total:
 
   g2 = mean((g^0.5 - g_hat^0.5)^2)   g4 = C4 * mean((g^0.5 - g_hat^0.5)^4)   r2 = mean(((1-r)^0.5 - (1-r_hat)^0.5)^2)
 
-"overall" takes the same means over every frame of every file.  With ``--pred-dir`` the predictions of each file
-(frames x 68 float32: 34 g then 34 r) go to DIR/<file name>.pred.f32.  There is no CPU path.
+The sums behind the means are reduced in float64 on the device from the predictions and the labels rec[70..137]
+(pnb_score_records_host), so only four numbers per stream and call come back; the host adds them per file in float64,
+in chunk order.  ``loss_sums`` is the same reduction in numpy, kept as the reference it is checked against.  "overall"
+takes the same means over every frame of every file.  With ``--pred-dir`` the predictions of each file (frames x 68
+float32: 34 g then 34 r) are fetched too and go to DIR/<file name>.pred.f32.  There is no CPU path.
 """
 from __future__ import annotations
 
@@ -79,22 +85,45 @@ def loss_terms(sums: np.ndarray) -> dict:
     return t
 
 
-def predict(recs, model, flags: int, batch: int, chunk: int, device: int = 0):
-    """g/r [frames, 68] float32 of every record array in `recs`, each from a fresh stream."""
+def window_plan(lengths, window: int):
+    """The streams of files of `lengths` frames: (file index, first frame, frames) in file order, then frame order.
+    window 0: one stream per file; else consecutive `window`-frame pieces, the last one possibly shorter."""
+    plan = []
+    for k, n in enumerate(lengths):
+        step = window if window > 0 else n
+        plan += [(k, t0, min(step, n - t0)) for t0 in range(0, n, step)]
+    return plan
+
+
+def chunk_frames(lengths, t0: int, chunk: int) -> np.ndarray:
+    """The frames of the call that starts at frame t0 which belong to each stream of `lengths` frames (int32)."""
+    return np.clip(np.asarray(lengths, np.int64) - t0, 0, chunk).astype(np.int32)
+
+
+def score(recs, model, flags: int, batch: int, chunk: int, device: int = 0, want_pred: bool = False):
+    """Loss sums [len(recs), 4] float64 of every record array in `recs`, each from a fresh stream, and its g/r
+    [frames, 68] float32 (None unless want_pred)."""
     from . import api
+    sums = np.zeros((len(recs), 4), np.float64)
     preds = [None] * len(recs)
     for group in plan_batches([r.shape[0] for r in recs], batch):
         x = pad_batch([recs[k] for k in group])
+        lengths = [recs[k].shape[0] for k in group]
         N, F = x.shape[0], x.shape[1]
-        eng = api.Engine(N, min(chunk, F), model, flags, device=device)
+        eng = api.Engine(N, min(chunk, F), model, flags | api.NETWORK_ONLY, device=device)
+        parts = []
         try:
-            parts = [eng.compute_rnn(x[:, t0:min(F, t0 + chunk)]) for t0 in range(0, F, chunk)]
+            for t0 in range(0, F, chunk):
+                s, gr = eng.score_records(x[:, t0:min(F, t0 + chunk)], chunk_frames(lengths, t0, chunk), want_pred)
+                sums[group] += s
+                parts.append(gr)
         finally:
             eng.close()
-        gr = np.concatenate(parts, axis=1)
-        for i, k in enumerate(group):
-            preds[k] = gr[i, :recs[k].shape[0]]
-    return preds
+        if want_pred:
+            gr = np.concatenate(parts, axis=1)
+            for i, k in enumerate(group):
+                preds[k] = gr[i, :recs[k].shape[0]]
+    return sums, preds
 
 
 def parse_args(argv=None):
@@ -106,6 +135,8 @@ def parse_args(argv=None):
     ap.add_argument("--conv-wide", action="store_true", help="with --tensor: three bf16 terms in conv1 / conv2 (PNB_CONV_WIDE)")
     ap.add_argument("--batch", type=int, default=4096, help="files (streams) per engine")
     ap.add_argument("--chunk", type=int, default=100, help="frames per GPU call")
+    ap.add_argument("--window", type=int, default=0,
+                    help="cut each file into N-frame windows, each a fresh stream (0: whole files)")
     ap.add_argument("--pred-dir", help="write each file's predictions to DIR/<file name>.pred.f32")
     ap.add_argument("--device", type=int, default=0)
     a = ap.parse_args(argv)
@@ -116,6 +147,8 @@ def parse_args(argv=None):
         ap.error("no record files given")
     if a.batch < 1 or a.chunk < 1:
         ap.error("--batch and --chunk must be >= 1")
+    if a.window < 0:
+        ap.error("--window must be >= 0")
     if a.conv_wide and not a.tensor:
         ap.error("--conv-wide applies to --tensor")
     return a
@@ -130,25 +163,30 @@ def main(argv=None) -> int:
     a = parse_args(argv)
     from . import api
     recs = [read_records(p) for p in a.files]
+    plan = window_plan([r.shape[0] for r in recs], a.window)
     model = api.BlobModel(a.model)
     try:
-        preds = predict(recs, model, engine_flags(a), a.batch, a.chunk, a.device)
+        sums, preds = score([recs[k][t0:t0 + n] for k, t0, n in plan], model, engine_flags(a), a.batch, a.chunk,
+                            a.device, bool(a.pred_dir))
     except api.PnbError as ex:
         sys.stderr.write(f"{ex}\n")
         return 2
     finally:
         model.free()
+    file_sums = np.zeros((len(recs), 4), np.float64)
+    for (k, _, _), s in zip(plan, sums):          # in window order
+        file_sums[k] += s
     if a.pred_dir:
         os.makedirs(a.pred_dir, exist_ok=True)
+        for k, path in enumerate(a.files):
+            pred = np.concatenate([p for (j, _, _), p in zip(plan, preds) if j == k])
+            pred.astype("<f4").tofile(os.path.join(a.pred_dir, os.path.basename(path) + ".pred.f32"))
     total = np.zeros(4, np.float64)
     print(f"{'file':<40} {'frames':>7} {'g2':>12} {'g4':>12} {'r2':>12} {'total':>12}")
-    for path, rec, pred in zip(a.files, recs, preds):
-        s = loss_sums(pred, rec)
+    for path, rec, s in zip(a.files, recs, file_sums):
         total += s
         t = loss_terms(s)
         print(f"{path:<40} {rec.shape[0]:>7} {t['g2']:12.6e} {t['g4']:12.6e} {t['r2']:12.6e} {t['total']:12.6e}")
-        if a.pred_dir:
-            pred.astype("<f4").tofile(os.path.join(a.pred_dir, os.path.basename(path) + ".pred.f32"))
     t = loss_terms(total)
     print(f"{'overall':<40} {sum(r.shape[0] for r in recs):>7} {t['g2']:12.6e} {t['g4']:12.6e} {t['r2']:12.6e} "
           f"{t['total']:12.6e}")

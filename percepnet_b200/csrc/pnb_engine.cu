@@ -434,39 +434,6 @@ static int mark_call_end(pnb_engine *e, cudaStream_t st) {
   return PNB_OK;
 }
 
-// What every call checks before it allocates or enqueues anything: an engine of the call's family (training records,
-// enhancement or the network alone; a PNB_NETWORK_ONLY engine runs network calls only) that no failed call has
-// poisoned, 1 <= F <= Fmax, its buffers (`buffers`: none is NULL), and two row strides of at least F hops (of width_a /
-// width_b values each: 480 samples unless a network call says otherwise).
-static int check_call(const pnb_engine *e, bool train, bool network, bool buffers, int F, size_t stride_a, size_t stride_b,
-                      size_t width_a = kFrame, size_t width_b = kFrame) {
-  if (!e) return fail(PNB_ERR_ARG, "engine is NULL");
-  if (!network && (e->flags & PNB_NETWORK_ONLY))
-    return fail(PNB_ERR_ARG, "engine was created with PNB_NETWORK_ONLY: use pnb_compute_rnn_* / pnb_score_records_*");
-  if (train && !(e->flags & PNB_TRAIN_DATA)) return fail(PNB_ERR_ARG, "engine was not created with PNB_TRAIN_DATA");
-  if (!train && (e->flags & PNB_TRAIN_DATA))
-    return fail(PNB_ERR_ARG, "engine was created with PNB_TRAIN_DATA: use pnb_train_records_* / pnb_submit_train_records");
-  if (e->poisoned) return fail(PNB_ERR_CUDA, "an earlier call failed while enqueuing work; the streams' state is undefined until pnb_reset");
-  if (F < 1 || F > e->Fmax) return fail(PNB_ERR_ARG, "n_frames %d outside [1, %d]", F, e->Fmax);
-  if (!buffers) return fail(PNB_ERR_ARG, train ? "speech/noisy/records pointer is NULL" : "input/output pointer is NULL");
-  if (stride_a < (size_t)F * width_a) return fail(PNB_ERR_ARG, "row stride smaller than n_frames*%zu", width_a);
-  if (stride_b < (size_t)F * width_b) return fail(PNB_ERR_ARG, "row stride smaller than n_frames*%zu", width_b);
-  return PNB_OK;
-}
-// A training-data call: records only (audio null) on an engine without PNB_TRAIN_AUDIO, records and audio on one with it.
-static int check_train(const pnb_engine *e, const short *speech, size_t speech_stride, const short *noisy, size_t noisy_stride,
-                       int F, const float *records, size_t records_stride, bool audio_call = false,
-                       const short *audio = nullptr, size_t audio_stride = 0) {
-  const int rc = check_call(e, true, false, speech && noisy && records && (audio || !audio_call), F, speech_stride, noisy_stride);
-  if (rc) return rc;
-  if (audio_call && !(e->flags & PNB_TRAIN_AUDIO)) return fail(PNB_ERR_ARG, "engine was not created with PNB_TRAIN_AUDIO");
-  if (!audio_call && (e->flags & PNB_TRAIN_AUDIO))
-    return fail(PNB_ERR_ARG, "engine was created with PNB_TRAIN_AUDIO: use pnb_train_audio_*, so that its audio has no gaps");
-  if (records_stride < (size_t)F * PNB_RECORD_FLOATS) return fail(PNB_ERR_ARG, "records_stride smaller than n_frames*138");
-  if (audio_call && audio_stride < (size_t)F * kFrame) return fail(PNB_ERR_ARG, "audio_stride smaller than n_frames*480");
-  return PNB_OK;
-}
-
 // The call's own launches, in ev_call's order; returns their count or a negative error.
 template <typename Launches>
 static int enqueue_ordered(pnb_engine *e, cudaStream_t st, Launches launches) {
@@ -563,30 +530,36 @@ static int enqueue_plan(pnb_engine *e, const int *ids, int k, const int *hops, i
   return launch_session_move(a, st);
 }
 
-// One enhancement call as its entry point received it: rows of float samples, or of int16 samples (i16), in and out, in
-// host or device memory by entry point.  A network call (kNetwork, pnb_compute_rnn_*) reads rows of features or
-// training records (format) and writes rows of g/r to out instead; a score call (pnb_score_records_*) is a network call
-// on records with sums, whose out (g/r) may be null.
+// One array of a call's rows, in host or device memory by entry point: row r at p + r * stride values of `bytes` bytes
+// each, `width` values per hop, or `width` values whatever the hops (per_row: a score call's sums).  `name` is the
+// stride's name in its refusal.  width 0: the call has no such array.
+struct Rows {
+  void *p;
+  size_t stride, width, bytes;
+  const char *name;
+  bool per_row;
+  size_t values(int F) const { return per_row ? width : (size_t)F * width; }  // the values of a row of an F-hop call
+};
+static Rows rows(const void *p, size_t stride, size_t width, size_t bytes, const char *name = "row stride", bool per_row = false) {
+  return {const_cast<void *>(p), stride, width, bytes, name, per_row};
+}
+template <typename T>
+static Rows pcm(const T *p, size_t stride) { return rows(p, stride, kFrame, sizeof(T)); }
+
+// One call as its entry point received it, its buffers as row arrays.  In / out: PCM / PCM of a slot, session or ragged
+// call; speech, noisy / records and (pnb_train_audio_*) audio of a training-record call; features or records / g/r of a
+// network call; records / g/r (when asked for) and the loss sums of a score call.
 struct Call {
-  enum Kind { kSlots, kSessions, kRagged, kNetwork } kind;
-  const void *in;
-  size_t in_stride;
-  void *out;
-  size_t out_stride;
-  bool i16;
-  int F;           // hops; a ragged call's is max(hops), set by check_enhance
-  float *gr;       // g/r destination [F][rows][68], or null
+  enum Kind { kSlots, kSessions, kRagged, kNetwork, kRecords } kind;
+  Rows in[2], out[2];
+  int F;           // hops; a ragged call's is max(hops), set by check_call
+  float *gr;       // enhancement calls: g/r destination [F][rows][68], or null
   const int *ids;  // session and ragged calls: the session list (host), n_ids long
   int n_ids;
-  const int *hops;  // ragged calls: each listed session's hops (host); null once check_enhance finds them all equal to F
-  int format;       // network calls: PNB_RNN_FEATURES or PNB_RNN_RECORDS
-  bool score;         // a score call: a network call on records that writes sums, and g/r to out only when out is set
-  double *sums;       // score calls: the loss sums [rows][4] (in the entry point's memory)
+  const int *hops;    // ragged calls: each listed session's hops (host); null once check_call finds them all equal to F
+  int format;         // network calls: PNB_RNN_FEATURES or PNB_RNN_RECORDS
   const int *frames;  // score calls: the hops each row's loss counts (host), or null for F
-  // values per hop of an input / output row: 480 samples, or a network call's 70 features / 138 record floats and 68 g/r
-  // (0: a score call that writes no g/r)
-  size_t in_width() const { return kind != kNetwork ? kFrame : format == PNB_RNN_RECORDS ? PNB_RECORD_FLOATS : kFeat; }
-  size_t out_width() const { return kind != kNetwork ? kFrame : (out || !score) ? 68 : 0; }
+  bool status = true;  // a blocking host call reads back and reports the status word (rejected imports, PNB_ERR_DOMAIN)
 };
 
 // A network call on st (arguments already checked): the caller's rows into the features buffer, the network hook, its
@@ -594,6 +567,7 @@ struct Call {
 // signal state (history line, overlap-add, pitch memory, spectrum ring, hop counter, line offset) is not touched.
 static int enqueue_network(pnb_engine *e, const Call &c, cudaStream_t st) {
   const int F = c.F;
+  const Rows &in = c.in[0], &gr = c.out[0], &sums = c.out[1];
   return enqueue_call(e, F, st, [&]() -> int {
     const int S = e->S, na = e->n_active;
     int n = 0;
@@ -601,7 +575,7 @@ static int enqueue_network(pnb_engine *e, const Call &c, cudaStream_t st) {
     if (c.frames) { int rc = stage_ints(e, c.frames, (size_t)na, st, &frames); if (rc) return rc; }
     {
       ProfScope ps(e, PNB_K_STAGE_IN, st);
-      n += launch_features_stage(e->d_feat, static_cast<const float *>(c.in), c.in_stride, (int)c.in_width(), na, S, F, st);
+      n += launch_features_stage(e->d_feat, static_cast<const float *>(in.p), in.stride, (int)in.width, na, S, F, st);
     }
     CK(cudaGetLastError());
     {
@@ -609,13 +583,50 @@ static int enqueue_network(pnb_engine *e, const Call &c, cudaStream_t st) {
       if (q < 0) return q;
       n += q;
     }
-    if (c.score) {
+    if (sums.p) {
       ProfScope ps(e, PNB_K_STAGE_IN, st);
-      n += launch_loss_sums(e->d_gr, static_cast<const float *>(c.in), c.in_stride, frames, c.sums, na, S, F, st);
+      n += launch_loss_sums(e->d_gr, static_cast<const float *>(in.p), in.stride, frames, static_cast<double *>(sums.p), na, S, F, st);
     }
-    if (c.out) { ProfScope ps(e, PNB_K_STAGE_IN, st); n += launch_gr_store(e->d_gr, static_cast<float *>(c.out), c.out_stride, na, S, F, st); }
+    if (gr.p) { ProfScope ps(e, PNB_K_STAGE_IN, st); n += launch_gr_store(e->d_gr, static_cast<float *>(gr.p), gr.stride, na, S, F, st); }
     return n;
   }, false);
+}
+
+// One training-record call on st (arguments already checked), the training-data generator (row f1): stage both files of
+// every pair, analysis over 2N streams, labels; with audio (a PNB_TRAIN_AUDIO engine) then the resynthesis of the N
+// noisy streams with their labels.
+static int enqueue_records(pnb_engine *e, const Call &c, cudaStream_t st) {
+  const int F = c.F;
+  const Rows &speech = c.in[0], &noisy = c.in[1], &records = c.out[0], &audio = c.out[1];
+  return enqueue_call(e, F, st, [&]() -> int {
+    const int N = e->S / 2;
+    float *line = e->d_pcm + e->line_off;
+    int n = 0;
+    {
+      ProfScope ps(e, PNB_K_STAGE_IN, st);
+      n += launch_stage_in(line, e->pcm_stride, nullptr, static_cast<const short *>(noisy.p), noisy.stride, N, F * kFrame, st, 1.f);
+      n += launch_stage_in(line + (size_t)N * e->pcm_stride, e->pcm_stride, nullptr, static_cast<const short *>(speech.p),
+                           speech.stride, N, F * kFrame, st, 1.f);
+    }
+    AnalysisArgs a = analysis_args(e, F);  // all S streams: the active range of a training-data engine is always S
+    a.raw = e->d_raw;
+    a.P_rows = N;  // an audio engine's P: the noisy rows (the others have none)
+    { ProfScope ps(e, PNB_K_ANALYSIS, st); n += launch_analysis(a, st); }
+    LabelArgs l;
+    l.feat = e->d_feat; l.raw = e->d_raw; l.Ex = e->d_Ex; l.tab = e->d_tab; l.n_pairs = N; l.n_frames = F;
+    l.records = static_cast<float *>(records.p); l.pair_stride = records.stride;
+    l.gr = audio.p ? e->d_gr : nullptr;
+    { ProfScope ps(e, PNB_K_LABELS, st); n += launch_train_labels(l, st); }
+    if (audio.p) {  // denoise.cpp:742-759 on the noisy rows, their labels post-filtered already (no PNB_POSTFILTER here)
+      SynthesisArgs s = synthesis_args(e, F, nullptr, static_cast<short *>(audio.p), audio.stride);
+      s.n_streams = N;
+      s.clamp16 = 1;
+      ProfScope ps(e, PNB_K_SYNTHESIS, st);
+      n += launch_synthesis(s, st);
+    }
+    n += advance_line(e, F, st);
+    return n;
+  });
 }
 
 // One enhancement call on st, its buffers on the device (arguments already checked).  A session call first applies its
@@ -623,8 +634,8 @@ static int enqueue_network(pnb_engine *e, const Call &c, cudaStream_t st) {
 // slot p runs the hops of its list row, and the slots that stop early are moved to the counters of hop F after
 // synthesis.
 static int enqueue_enhance(pnb_engine *e, const Call &c, cudaStream_t st) {
-  if (c.kind == Call::kNetwork) return enqueue_network(e, c, st);
   const int F = c.F;
+  const bool i16 = c.in[0].bytes == sizeof(short);
   return enqueue_call(e, F, st, [&]() -> int {
     int n = 0;
     const int *row = nullptr;
@@ -634,9 +645,9 @@ static int enqueue_enhance(pnb_engine *e, const Call &c, cudaStream_t st) {
       if (n < 0) return n;
     }
     const int S = e->S, na = e->n_active;  // the call advances streams [0, na); per-call buffers keep the stride S
-    const float *in = c.i16 ? nullptr : static_cast<const float *>(c.in);
-    const short *in16 = c.i16 ? static_cast<const short *>(c.in) : nullptr;
-    { ProfScope ps(e, PNB_K_STAGE_IN, st); n += launch_stage_in(e->d_pcm + e->line_off, e->pcm_stride, in, in16, c.in_stride, na, F * kFrame, st, 32768.f, row, rg.hops); }
+    const float *in = i16 ? nullptr : static_cast<const float *>(c.in[0].p);
+    const short *in16 = i16 ? static_cast<const short *>(c.in[0].p) : nullptr;
+    { ProfScope ps(e, PNB_K_STAGE_IN, st); n += launch_stage_in(e->d_pcm + e->line_off, e->pcm_stride, in, in16, c.in[0].stride, na, F * kFrame, st, 32768.f, row, rg.hops); }
     {
       AnalysisArgs aa = analysis_args(e, F);
       aa.hops = rg.hops;
@@ -650,8 +661,8 @@ static int enqueue_enhance(pnb_engine *e, const Call &c, cudaStream_t st) {
       n += q;
     }
     {
-      SynthesisArgs sa = synthesis_args(e, F, c.i16 ? nullptr : static_cast<float *>(c.out),
-                                        c.i16 ? static_cast<short *>(c.out) : nullptr, c.out_stride);
+      SynthesisArgs sa = synthesis_args(e, F, i16 ? nullptr : static_cast<float *>(c.out[0].p),
+                                        i16 ? static_cast<short *>(c.out[0].p) : nullptr, c.out[0].stride);
       sa.row = row;
       sa.hops = rg.hops;
       ProfScope ps(e, PNB_K_SYNTHESIS, st);
@@ -669,6 +680,11 @@ static int enqueue_enhance(pnb_engine *e, const Call &c, cudaStream_t st) {
                            cudaMemcpyDeviceToDevice, st));
     return n;
   });
+}
+
+// The call's enqueue body (arguments already checked).
+static int enqueue(pnb_engine *e, const Call &c, cudaStream_t st) {
+  return c.kind == Call::kNetwork ? enqueue_network(e, c, st) : c.kind == Call::kRecords ? enqueue_records(e, c, st) : enqueue_enhance(e, c, st);
 }
 
 // The slot-level entry points of an engine in session mode: refused before anything is enqueued.
@@ -698,11 +714,21 @@ static int check_ids(pnb_engine *e, const int *ids, int n, int n_max) {
   return check_list(e, ids, n, e->pool.capacity(), e->pool.capacity(), "ids");
 }
 
-// Every refusal of an enhancement call, before anything changes.  A slot call: check_call, then session mode.  A network
-// call: check_call with its row widths, then its format, then session mode.  A session call: check_call, then the list.
-// A ragged call checks the list and its hop counts first, because their largest is the call's length F; when every
-// session runs F hops, hops becomes null and the call is the plain session call.
-static int check_enhance(pnb_engine *e, Call &c) {
+// The stride refusal of each of the arrays: a row of F hops fits in its stride.
+static int check_strides(const Rows (&a)[2], int F) {
+  for (const Rows &r : a)
+    if (r.width && r.stride < r.values(F)) return fail(PNB_ERR_ARG, "%s smaller than n_frames*%zu", r.name, r.width);
+  return PNB_OK;
+}
+
+// Every refusal of a call, before anything changes.  Every call checks an engine of its family (training records,
+// enhancement or the network alone; a PNB_NETWORK_ONLY engine runs network calls only) that no failed call has
+// poisoned, 1 <= F <= Fmax, none of its arrays NULL, the input strides; a training-record call then that its engine
+// has audio exactly when the call does; every call then the output strides.  After that a slot call checks session
+// mode, a session call its list, a network call its format, then session mode, and a score call its frames.  A ragged
+// call checks the list and its hop counts first, because their largest is the call's length F; when every session runs
+// F hops, hops becomes null and the call is the plain session call.
+static int check_call(pnb_engine *e, Call &c) {
   if (c.kind == Call::kRagged) {
     if (!e) return fail(PNB_ERR_ARG, "engine is NULL");
     { int rc = check_ids(e, c.ids, c.n_ids, e->S); if (rc) return rc; }
@@ -716,103 +742,83 @@ static int check_enhance(pnb_engine *e, Call &c) {
     for (int i = 0; i < c.n_ids; i++) uniform = uniform && c.hops[i] == c.F;
     if (uniform) c.hops = nullptr;
   }
-  const bool network = c.kind == Call::kNetwork;
-  {
-    int rc = check_call(e, false, network, c.in && (c.score ? c.sums != nullptr : c.out != nullptr), c.F, c.in_stride,
-                        c.out_stride, c.in_width(), c.out_width());
-    if (rc) return rc;
-  }
+  const bool train = c.kind == Call::kRecords, network = c.kind == Call::kNetwork;
+  if (!e) return fail(PNB_ERR_ARG, "engine is NULL");
+  if (!network && (e->flags & PNB_NETWORK_ONLY))
+    return fail(PNB_ERR_ARG, "engine was created with PNB_NETWORK_ONLY: use pnb_compute_rnn_* / pnb_score_records_*");
+  if (train && !(e->flags & PNB_TRAIN_DATA)) return fail(PNB_ERR_ARG, "engine was not created with PNB_TRAIN_DATA");
+  if (!train && (e->flags & PNB_TRAIN_DATA))
+    return fail(PNB_ERR_ARG, "engine was created with PNB_TRAIN_DATA: use pnb_train_records_* / pnb_submit_train_records");
+  if (e->poisoned) return fail(PNB_ERR_CUDA, "an earlier call failed while enqueuing work; the streams' state is undefined until pnb_reset");
+  if (c.F < 1 || c.F > e->Fmax) return fail(PNB_ERR_ARG, "n_frames %d outside [1, %d]", c.F, e->Fmax);
+  for (int i = 0; i < 2; i++)
+    if ((c.in[i].width && !c.in[i].p) || (c.out[i].width && !c.out[i].p))
+      return fail(PNB_ERR_ARG, train ? "speech/noisy/records pointer is NULL" : "input/output pointer is NULL");
+  { int rc = check_strides(c.in, c.F); if (rc) return rc; }
+  const bool audio = c.out[1].width != 0;
+  if (train && audio && !(e->flags & PNB_TRAIN_AUDIO)) return fail(PNB_ERR_ARG, "engine was not created with PNB_TRAIN_AUDIO");
+  if (train && !audio && (e->flags & PNB_TRAIN_AUDIO))
+    return fail(PNB_ERR_ARG, "engine was created with PNB_TRAIN_AUDIO: use pnb_train_audio_*, so that its audio has no gaps");
+  { int rc = check_strides(c.out, c.F); if (rc) return rc; }
   if (c.kind == Call::kSessions) return check_ids(e, c.ids, c.n_ids, e->S);
   if (network && c.format != PNB_RNN_FEATURES && c.format != PNB_RNN_RECORDS)
     return fail(PNB_ERR_ARG, "format %d is neither PNB_RNN_FEATURES (0) nor PNB_RNN_RECORDS (1)", c.format);
   if ((c.kind == Call::kSlots || network) && e->sessions) return refuse_in_session_mode();
-  if (c.score && c.frames)  // every row's counted hops in [0, F]
+  if (c.frames)  // every row's counted hops in [0, F]
     for (int i = 0; i < e->n_active; i++)
       if (c.frames[i] < 0 || c.frames[i] > c.F) return fail(PNB_ERR_ARG, "frames[%d] = %d outside [0, %d]", i, c.frames[i], c.F);
   return PNB_OK;
 }
 
-// pnb_process_device_*, pnb_submit_device_* and the device forms of the session calls.
+// Every device-buffer call entry point.
 static int device_call(pnb_engine *e, Call c, cudaStream_t st) {
-  { int rc = check_enhance(e, c); if (rc) return rc; }
+  { int rc = check_call(e, c); if (rc) return rc; }
   CK(cudaSetDevice(e->device));
-  return enqueue_enhance(e, c, st);
+  return enqueue(e, c, st);
 }
 
 extern "C" int pnb_process_device_f32(pnb_engine *e, const float *d_in, size_t in_stride, float *d_out,
                                       size_t out_stride, int n_frames, float *d_gr, void *cuda_stream) {
-  return device_call(e, {Call::kSlots, d_in, in_stride, d_out, out_stride, false, n_frames, d_gr}, (cudaStream_t)cuda_stream);
+  return device_call(e, {Call::kSlots, {pcm(d_in, in_stride)}, {pcm(d_out, out_stride)}, n_frames, d_gr}, (cudaStream_t)cuda_stream);
 }
 extern "C" int pnb_process_device_i16(pnb_engine *e, const short *d_in, size_t in_stride, short *d_out,
                                       size_t out_stride, int n_frames, float *d_gr, void *cuda_stream) {
-  return device_call(e, {Call::kSlots, d_in, in_stride, d_out, out_stride, true, n_frames, d_gr}, (cudaStream_t)cuda_stream);
+  return device_call(e, {Call::kSlots, {pcm(d_in, in_stride)}, {pcm(d_out, out_stride)}, n_frames, d_gr}, (cudaStream_t)cuda_stream);
 }
 // pnb_process_device_* without g/r; both names are part of the ABI.
 extern "C" int pnb_submit_device_f32(pnb_engine *e, const float *d_in, size_t in_stride, float *d_out, size_t out_stride,
                                      int n_frames, void *cuda_stream) {
-  return device_call(e, {Call::kSlots, d_in, in_stride, d_out, out_stride, false, n_frames, nullptr}, (cudaStream_t)cuda_stream);
+  return device_call(e, {Call::kSlots, {pcm(d_in, in_stride)}, {pcm(d_out, out_stride)}, n_frames}, (cudaStream_t)cuda_stream);
 }
 extern "C" int pnb_submit_device_i16(pnb_engine *e, const short *d_in, size_t in_stride, short *d_out, size_t out_stride,
                                      int n_frames, void *cuda_stream) {
-  return device_call(e, {Call::kSlots, d_in, in_stride, d_out, out_stride, true, n_frames, nullptr}, (cudaStream_t)cuda_stream);
+  return device_call(e, {Call::kSlots, {pcm(d_in, in_stride)}, {pcm(d_out, out_stride)}, n_frames}, (cudaStream_t)cuda_stream);
 }
 
-// ------------------------------------------------------------------------------------------
-// training-data generator (row f1): stage both files of every pair, analysis over 2N streams, labels; on a
-// PNB_TRAIN_AUDIO engine then the resynthesis of the N noisy streams with their labels
-// ------------------------------------------------------------------------------------------
-// One training-record call on st (arguments already checked); d_audio null on an engine without PNB_TRAIN_AUDIO.
-static int enqueue_records(pnb_engine *e, const short *d_speech, size_t speech_stride, const short *d_noisy,
-                           size_t noisy_stride, int F, float *d_records, size_t records_stride, short *d_audio,
-                           size_t audio_stride, cudaStream_t st) {
-  return enqueue_call(e, F, st, [&]() -> int {
-    const int N = e->S / 2;
-    float *line = e->d_pcm + e->line_off;
-    int n = 0;
-    {
-      ProfScope ps(e, PNB_K_STAGE_IN, st);
-      n += launch_stage_in(line, e->pcm_stride, nullptr, d_noisy, noisy_stride, N, F * kFrame, st, 1.f);
-      n += launch_stage_in(line + (size_t)N * e->pcm_stride, e->pcm_stride, nullptr, d_speech, speech_stride, N, F * kFrame, st, 1.f);
-    }
-    AnalysisArgs a = analysis_args(e, F);  // all S streams: the active range of a training-data engine is always S
-    a.raw = e->d_raw;
-    a.P_rows = N;  // an audio engine's P: the noisy rows (the others have none)
-    { ProfScope ps(e, PNB_K_ANALYSIS, st); n += launch_analysis(a, st); }
-    LabelArgs l;
-    l.feat = e->d_feat; l.raw = e->d_raw; l.Ex = e->d_Ex; l.tab = e->d_tab; l.n_pairs = N; l.n_frames = F;
-    l.records = d_records; l.pair_stride = records_stride;
-    l.gr = d_audio ? e->d_gr : nullptr;
-    { ProfScope ps(e, PNB_K_LABELS, st); n += launch_train_labels(l, st); }
-    if (d_audio) {  // denoise.cpp:742-759 on the noisy rows, their labels post-filtered already (no PNB_POSTFILTER here)
-      SynthesisArgs s = synthesis_args(e, F, nullptr, d_audio, audio_stride);
-      s.n_streams = N;
-      s.clamp16 = 1;
-      ProfScope ps(e, PNB_K_SYNTHESIS, st);
-      n += launch_synthesis(s, st);
-    }
-    n += advance_line(e, F, st);
-    return n;
-  });
+// A training-record call: int16 speech and noisy rows in, records and, for pnb_train_audio_* (with_audio), audio out.  A
+// blocking host call does not read the status word: a training-data engine reports a rejected pnb_import_states through
+// pnb_wait / pnb_check only.
+static Call records_call(const short *speech, size_t speech_stride, const short *noisy, size_t noisy_stride, int F,
+                         float *records, size_t records_stride, bool with_audio = false, short *audio = nullptr,
+                         size_t audio_stride = 0) {
+  Call c{Call::kRecords, {pcm(speech, speech_stride), pcm(noisy, noisy_stride)},
+         {rows(records, records_stride, PNB_RECORD_FLOATS, sizeof(float), "records_stride")}, F};
+  if (with_audio) c.out[1] = rows(audio, audio_stride, kFrame, sizeof(short), "audio_stride");
+  c.status = false;
+  return c;
 }
 
 extern "C" int pnb_train_records_device(pnb_engine *e, const short *d_speech, size_t speech_stride,
                                         const short *d_noisy, size_t noisy_stride, int F, float *d_records,
                                         size_t records_stride, void *cuda_stream) {
-  { int rc = check_train(e, d_speech, speech_stride, d_noisy, noisy_stride, F, d_records, records_stride); if (rc) return rc; }
-  CK(cudaSetDevice(e->device));
-  return enqueue_records(e, d_speech, speech_stride, d_noisy, noisy_stride, F, d_records, records_stride, nullptr, 0,
-                         (cudaStream_t)cuda_stream);
+  return device_call(e, records_call(d_speech, speech_stride, d_noisy, noisy_stride, F, d_records, records_stride),
+                     (cudaStream_t)cuda_stream);
 }
 extern "C" int pnb_train_audio_device(pnb_engine *e, const short *d_speech, size_t speech_stride, const short *d_noisy,
                                       size_t noisy_stride, int F, float *d_records, size_t records_stride, short *d_audio,
                                       size_t audio_stride, void *cuda_stream) {
-  {
-    int rc = check_train(e, d_speech, speech_stride, d_noisy, noisy_stride, F, d_records, records_stride, true, d_audio, audio_stride);
-    if (rc) return rc;
-  }
-  CK(cudaSetDevice(e->device));
-  return enqueue_records(e, d_speech, speech_stride, d_noisy, noisy_stride, F, d_records, records_stride, d_audio,
-                         audio_stride, (cudaStream_t)cuda_stream);
+  return device_call(e, records_call(d_speech, speech_stride, d_noisy, noisy_stride, F, d_records, records_stride, true,
+                                     d_audio, audio_stride), (cudaStream_t)cuda_stream);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -879,52 +885,6 @@ static int round_trip(pnb_engine *e, int k, bool pipelined, H2D h2d, Call call, 
   return PNB_OK;
 }
 
-// pnb_train_records_host (blocking), pnb_submit_train_records (pipelined) and pnb_train_audio_host (blocking, with audio);
-// the staged audio rows follow the staged records in the slot's output buffer.
-static int records_host(pnb_engine *e, const short *speech, size_t speech_stride, const short *noisy, size_t noisy_stride,
-                        int F, float *records, size_t records_stride, bool pipelined, bool audio_call = false,
-                        short *audio = nullptr, size_t audio_stride = 0) {
-  {
-    int rc = check_train(e, speech, speech_stride, noisy, noisy_stride, F, records, records_stride, audio_call, audio, audio_stride);
-    if (rc) return rc;
-  }
-  CK(cudaSetDevice(e->device));
-  const size_t N = e->S / 2, row = (size_t)e->Fmax * kFrame, rrow = (size_t)e->Fmax * PNB_RECORD_FLOATS;
-  const size_t w = (size_t)F * kFrame * sizeof(short);
-  const int k = staging_slot(e, pipelined, 2 * N * row * sizeof(short), N * rrow * sizeof(float) + (audio ? N * row * sizeof(short) : 0));
-  if (k < 0) return k;
-  short *d_noisy = (short *)e->stage[k].in, *d_speech = d_noisy + N * row;
-  float *d_rec = (float *)e->stage[k].out;
-  short *d_audio = audio ? (short *)(d_rec + N * rrow) : nullptr;
-  const int rc = round_trip(e, k, pipelined,
-      [&](cudaStream_t s) {
-        const cudaError_t ce = cudaMemcpy2DAsync(d_noisy, row * 2, noisy, noisy_stride * 2, w, N, cudaMemcpyHostToDevice, s);
-        return ce != cudaSuccess ? ce : cudaMemcpy2DAsync(d_speech, row * 2, speech, speech_stride * 2, w, N, cudaMemcpyHostToDevice, s);
-      },
-      [&] { return enqueue_records(e, d_speech, row, d_noisy, row, F, d_rec, rrow, d_audio, row, e->stream); },
-      [&](cudaStream_t s) {
-        const cudaError_t ce = cudaMemcpy2DAsync(records, records_stride * 4, d_rec, rrow * 4, (size_t)F * PNB_RECORD_FLOATS * 4, N,
-                                                 cudaMemcpyDeviceToHost, s);
-        return ce != cudaSuccess || !audio ? ce : cudaMemcpy2DAsync(audio, audio_stride * 2, d_audio, row * 2, w, N, cudaMemcpyDeviceToHost, s);
-      });
-  if (rc || pipelined) return rc;
-  CK(cudaStreamSynchronize(e->stream));
-  return PNB_OK;
-}
-extern "C" int pnb_train_records_host(pnb_engine *e, const short *speech, size_t speech_stride, const short *noisy,
-                                      size_t noisy_stride, int F, float *records, size_t records_stride) {
-  return records_host(e, speech, speech_stride, noisy, noisy_stride, F, records, records_stride, false);
-}
-extern "C" int pnb_submit_train_records(pnb_engine *e, const short *speech, size_t speech_stride, const short *noisy,
-                                        size_t noisy_stride, int F, float *records, size_t records_stride) {
-  return records_host(e, speech, speech_stride, noisy, noisy_stride, F, records, records_stride, true);
-}
-extern "C" int pnb_train_audio_host(pnb_engine *e, const short *speech, size_t speech_stride, const short *noisy,
-                                    size_t noisy_stride, int F, float *records, size_t records_stride, short *audio,
-                                    size_t audio_stride) {
-  return records_host(e, speech, speech_stride, noisy, noisy_stride, F, records, records_stride, false, true, audio, audio_stride);
-}
-
 // after the stream that carried the status copy was synchronised
 static int report_status(pnb_engine *e) {
   if (e->h_status[0] & kStatusRejected) {  // reported once: no other stream was affected
@@ -947,87 +907,122 @@ static int report_status(pnb_engine *e) {
   return PNB_OK;
 }
 
-// pnb_process_host_*, pnb_process_sessions_host_*, pnb_process_sessions_ragged_host_*, pnb_compute_rnn_host (blocking)
-// and pnb_submit_host_* (pipelined).  The blocking form then copies g/r and the status word back on the engine's stream
-// too, and synchronises it once.  Rows travel F hops wide: a ragged call's input beyond a row's hops is copied but not
-// read.  A network call's rows (in_width / out_width floats per hop) fit the slot sized for float PCM.
+// Lays a call's arrays out in a staging buffer, n_rows rows each at a stride of Fmax hops: sets their strides and byte
+// offsets at[i] (16-byte aligned), and returns the bytes they take.
+static size_t staged_layout(Rows (&a)[2], size_t n_rows, int Fmax, size_t at[2]) {
+  size_t bytes = 0;
+  for (int i = 0; i < 2; i++) {
+    at[i] = bytes;
+    a[i].stride = a[i].values(Fmax);
+    bytes += (n_rows * a[i].stride * a[i].bytes + 15) & ~(size_t)15;
+  }
+  return bytes;
+}
+
+// F hops of n_rows rows of each array of src into the same array of dst (absent arrays: nothing).
+static cudaError_t copy_rows(const Rows (&dst)[2], const Rows (&src)[2], int F, size_t n_rows, cudaMemcpyKind kind, cudaStream_t s) {
+  for (int i = 0; i < 2; i++) {
+    if (!src[i].p) continue;
+    const size_t b = src[i].bytes;
+    const cudaError_t ce = cudaMemcpy2DAsync(dst[i].p, dst[i].stride * b, src[i].p, src[i].stride * b, src[i].values(F) * b,
+                                             n_rows, kind, s);
+    if (ce != cudaSuccess) return ce;
+  }
+  return cudaSuccess;
+}
+
+// Every host-buffer call entry point: pnb_submit_host_* and pnb_submit_train_records pipelined, the others blocking.
+// Each array is staged at its place in the slot's input or output buffer, laid out for the engine's most rows (its
+// pairs on a training-data engine, else its slots) at Fmax hops, so a slot grows at most once per kind of call.  The
+// blocking form then copies an enhancement call's g/r and (when the call reports it) the status word back on the
+// engine's stream too, and synchronises it once.  Rows travel F hops wide: a ragged call's input beyond a row's hops is
+// copied but not read.
 static int host_call(pnb_engine *e, Call c, bool pipelined) {
-  { int rc = check_enhance(e, c); if (rc) return rc; }
+  { int rc = check_call(e, c); if (rc) return rc; }
   CK(cudaSetDevice(e->device));
-  const size_t es = c.i16 ? sizeof(short) : sizeof(float);
-  const size_t S = e->S, row = (size_t)e->Fmax * kFrame;
-  const size_t row_in = (size_t)e->Fmax * c.in_width(), row_out = (size_t)e->Fmax * c.out_width();  // staged row strides
-  const size_t w_in = (size_t)c.F * c.in_width() * es, w_out = (size_t)c.F * c.out_width() * es;
-  const size_t na = c.ids ? c.n_ids : e->n_active;  // the rows of in / out / gr
-  const int k = staging_slot(e, pipelined, S * row * es, S * row * es);
+  const size_t S = e->S, per = (e->flags & PNB_TRAIN_DATA) ? 2 : 1;  // a training-data engine's rows are its pairs
+  const size_t na = (c.ids ? c.n_ids : e->n_active) / per;       // the rows of the arrays and of gr
+  Call d = c;  // the call on staging slot k
+  size_t at_in[2], at_out[2];
+  const int k = staging_slot(e, pipelined, staged_layout(d.in, S / per, e->Fmax, at_in), staged_layout(d.out, S / per, e->Fmax, at_out));
   if (k < 0) return k;
   if (c.ids && c.gr) { int rc = grow((void **)&e->d_sgr, &e->sgr_bytes, (size_t)e->Fmax * S * 68 * sizeof(float)); if (rc) return rc; }
-  Call d = c;  // the call on staging slot k
-  d.in = e->stage[k].in;
-  d.out = c.out ? e->stage[k].out : nullptr;
-  d.in_stride = row_in;
-  d.out_stride = row_out;
+  for (int i = 0; i < 2; i++) {
+    if (c.in[i].p) d.in[i].p = static_cast<char *>(e->stage[k].in) + at_in[i];
+    if (c.out[i].p) d.out[i].p = static_cast<char *>(e->stage[k].out) + at_out[i];
+  }
   d.gr = c.ids && c.gr ? e->d_sgr : nullptr;  // session calls gather g/r in list order on the device
-  // a score call's sums follow the g/r rows in the output slot (row_out <= row: the slot has room for both)
-  d.sums = c.score ? reinterpret_cast<double *>(static_cast<char *>(e->stage[k].out) + ((S * row_out * es + 15) & ~(size_t)15)) : nullptr;
   const int rc = round_trip(e, k, pipelined,
-      [&](cudaStream_t s) { return cudaMemcpy2DAsync(e->stage[k].in, row_in * es, c.in, c.in_stride * es, w_in, na, cudaMemcpyHostToDevice, s); },
-      [&] { return enqueue_enhance(e, d, e->stream); },
-      [&](cudaStream_t s) {
-        const cudaError_t ce = c.out ? cudaMemcpy2DAsync(c.out, c.out_stride * es, e->stage[k].out, row_out * es, w_out, na,
-                                                         cudaMemcpyDeviceToHost, s)
-                                     : cudaSuccess;
-        return ce != cudaSuccess || !c.score ? ce : cudaMemcpyAsync(c.sums, d.sums, na * 4 * sizeof(double), cudaMemcpyDeviceToHost, s);
-      });
+      [&](cudaStream_t s) { return copy_rows(d.in, c.in, c.F, na, cudaMemcpyHostToDevice, s); },
+      [&] { return enqueue(e, d, e->stream); },
+      [&](cudaStream_t s) { return copy_rows(c.out, d.out, c.F, na, cudaMemcpyDeviceToHost, s); });
   if (rc || pipelined) return rc;
   if (d.gr)
     CK(cudaMemcpyAsync(c.gr, d.gr, (size_t)c.F * na * 68 * sizeof(float), cudaMemcpyDeviceToHost, e->stream));
   else if (c.gr)
     CK(cudaMemcpy2DAsync(c.gr, na * 68 * sizeof(float), e->d_gr, S * 68 * sizeof(float), na * 68 * sizeof(float), c.F, cudaMemcpyDeviceToHost,
                          e->stream));
-  CK(cudaMemcpyAsync(e->h_status, e->d_status, 2 * sizeof(int), cudaMemcpyDeviceToHost, e->stream));
+  if (c.status) CK(cudaMemcpyAsync(e->h_status, e->d_status, 2 * sizeof(int), cudaMemcpyDeviceToHost, e->stream));
   CK(cudaStreamSynchronize(e->stream));
-  return report_status(e);
+  return c.status ? report_status(e) : PNB_OK;
 }
 
 extern "C" int pnb_process_host_f32(pnb_engine *e, const float *in, size_t in_stride, float *out, size_t out_stride,
                                     int n_frames, float *gr) {
-  return host_call(e, {Call::kSlots, in, in_stride, out, out_stride, false, n_frames, gr}, false);
+  return host_call(e, {Call::kSlots, {pcm(in, in_stride)}, {pcm(out, out_stride)}, n_frames, gr}, false);
 }
 extern "C" int pnb_process_host_i16(pnb_engine *e, const short *in, size_t in_stride, short *out, size_t out_stride,
                                     int n_frames, float *gr) {
-  return host_call(e, {Call::kSlots, in, in_stride, out, out_stride, true, n_frames, gr}, false);
+  return host_call(e, {Call::kSlots, {pcm(in, in_stride)}, {pcm(out, out_stride)}, n_frames, gr}, false);
 }
 extern "C" int pnb_submit_host_f32(pnb_engine *e, const float *in, size_t in_stride, float *out, size_t out_stride,
                                    int n_frames) {
-  return host_call(e, {Call::kSlots, in, in_stride, out, out_stride, false, n_frames, nullptr}, true);
+  return host_call(e, {Call::kSlots, {pcm(in, in_stride)}, {pcm(out, out_stride)}, n_frames}, true);
 }
 extern "C" int pnb_submit_host_i16(pnb_engine *e, const short *in, size_t in_stride, short *out, size_t out_stride,
                                    int n_frames) {
-  return host_call(e, {Call::kSlots, in, in_stride, out, out_stride, true, n_frames, nullptr}, true);
+  return host_call(e, {Call::kSlots, {pcm(in, in_stride)}, {pcm(out, out_stride)}, n_frames}, true);
 }
 
-// The network alone on caller-supplied features or training records (the batched compute_rnn, rnn.cpp:42).
+extern "C" int pnb_train_records_host(pnb_engine *e, const short *speech, size_t speech_stride, const short *noisy,
+                                      size_t noisy_stride, int F, float *records, size_t records_stride) {
+  return host_call(e, records_call(speech, speech_stride, noisy, noisy_stride, F, records, records_stride), false);
+}
+extern "C" int pnb_submit_train_records(pnb_engine *e, const short *speech, size_t speech_stride, const short *noisy,
+                                        size_t noisy_stride, int F, float *records, size_t records_stride) {
+  return host_call(e, records_call(speech, speech_stride, noisy, noisy_stride, F, records, records_stride), true);
+}
+extern "C" int pnb_train_audio_host(pnb_engine *e, const short *speech, size_t speech_stride, const short *noisy,
+                                    size_t noisy_stride, int F, float *records, size_t records_stride, short *audio,
+                                    size_t audio_stride) {
+  return host_call(e, records_call(speech, speech_stride, noisy, noisy_stride, F, records, records_stride, true, audio,
+                                   audio_stride), false);
+}
+
+// The network alone on caller-supplied features or training records (the batched compute_rnn, rnn.cpp:42): rows of 70
+// features (any format but PNB_RNN_RECORDS, which check_call then refuses) or 138 record floats in, rows of g/r out.
+static Call network_call(int format, const float *in, size_t in_stride, int n_frames, float *gr, size_t gr_stride) {
+  Call c{Call::kNetwork, {rows(in, in_stride, format == PNB_RNN_RECORDS ? PNB_RECORD_FLOATS : kFeat, sizeof(float))},
+         {rows(gr, gr_stride, 68, sizeof(float))}, n_frames};
+  c.format = format;
+  return c;
+}
 extern "C" int pnb_compute_rnn_device(pnb_engine *e, int format, const float *d_in, size_t in_stride, int n_frames, float *d_gr,
                                       size_t gr_stride, void *cuda_stream) {
-  Call c{Call::kNetwork, d_in, in_stride, d_gr, gr_stride, false, n_frames, nullptr};
-  c.format = format;
-  return device_call(e, c, (cudaStream_t)cuda_stream);
+  return device_call(e, network_call(format, d_in, in_stride, n_frames, d_gr, gr_stride), (cudaStream_t)cuda_stream);
 }
 extern "C" int pnb_compute_rnn_host(pnb_engine *e, int format, const float *in, size_t in_stride, int n_frames, float *gr,
                                     size_t gr_stride) {
-  Call c{Call::kNetwork, in, in_stride, gr, gr_stride, false, n_frames, nullptr};
-  c.format = format;
-  return host_call(e, c, false);
+  return host_call(e, network_call(format, in, in_stride, n_frames, gr, gr_stride), false);
 }
 
-// A network call on records that also reduces rnn_train.py's loss against their labels on the device.
+// A network call on records that also reduces rnn_train.py's loss against their labels on the device: the sums, four
+// doubles per row, are its second output; g/r its first only when asked for.
 static Call score_call(const float *rec, size_t rec_stride, int n_frames, const int *frames, double *sums, float *gr,
                        size_t gr_stride) {
-  Call c{Call::kNetwork, rec, rec_stride, gr, gr_stride, false, n_frames, nullptr};
-  c.format = PNB_RNN_RECORDS;
-  c.score = true;
-  c.sums = sums;
+  Call c = network_call(PNB_RNN_RECORDS, rec, rec_stride, n_frames, gr, gr_stride);
+  if (!gr) c.out[0] = {};
+  c.out[1] = rows(sums, 4, 4, sizeof(double), "row stride", true);
   c.frames = frames;
   return c;
 }
@@ -1301,39 +1296,39 @@ extern "C" int pnb_session_stats(const pnb_engine *e, long long *out) {
 
 extern "C" int pnb_process_sessions_device_f32(pnb_engine *e, const int *ids, int n, const float *d_in, size_t in_stride,
                                                float *d_out, size_t out_stride, int n_frames, float *d_gr, void *cuda_stream) {
-  return device_call(e, {Call::kSessions, d_in, in_stride, d_out, out_stride, false, n_frames, d_gr, ids, n}, (cudaStream_t)cuda_stream);
+  return device_call(e, {Call::kSessions, {pcm(d_in, in_stride)}, {pcm(d_out, out_stride)}, n_frames, d_gr, ids, n}, (cudaStream_t)cuda_stream);
 }
 extern "C" int pnb_process_sessions_device_i16(pnb_engine *e, const int *ids, int n, const short *d_in, size_t in_stride,
                                                short *d_out, size_t out_stride, int n_frames, float *d_gr, void *cuda_stream) {
-  return device_call(e, {Call::kSessions, d_in, in_stride, d_out, out_stride, true, n_frames, d_gr, ids, n}, (cudaStream_t)cuda_stream);
+  return device_call(e, {Call::kSessions, {pcm(d_in, in_stride)}, {pcm(d_out, out_stride)}, n_frames, d_gr, ids, n}, (cudaStream_t)cuda_stream);
 }
 extern "C" int pnb_process_sessions_host_f32(pnb_engine *e, const int *ids, int n, const float *in, size_t in_stride, float *out,
                                              size_t out_stride, int n_frames, float *gr) {
-  return host_call(e, {Call::kSessions, in, in_stride, out, out_stride, false, n_frames, gr, ids, n}, false);
+  return host_call(e, {Call::kSessions, {pcm(in, in_stride)}, {pcm(out, out_stride)}, n_frames, gr, ids, n}, false);
 }
 extern "C" int pnb_process_sessions_host_i16(pnb_engine *e, const int *ids, int n, const short *in, size_t in_stride, short *out,
                                              size_t out_stride, int n_frames, float *gr) {
-  return host_call(e, {Call::kSessions, in, in_stride, out, out_stride, true, n_frames, gr, ids, n}, false);
+  return host_call(e, {Call::kSessions, {pcm(in, in_stride)}, {pcm(out, out_stride)}, n_frames, gr, ids, n}, false);
 }
 
-// Ragged session calls: session ids[i] advances by hops[i]; the call is max(hops) hops long (check_enhance).
+// Ragged session calls: session ids[i] advances by hops[i]; the call is max(hops) hops long (check_call).
 extern "C" int pnb_process_sessions_ragged_device_f32(pnb_engine *e, const int *ids, const int *hops, int n, const float *d_in,
                                                       size_t in_stride, float *d_out, size_t out_stride, float *d_gr,
                                                       void *cuda_stream) {
-  return device_call(e, {Call::kRagged, d_in, in_stride, d_out, out_stride, false, 0, d_gr, ids, n, hops}, (cudaStream_t)cuda_stream);
+  return device_call(e, {Call::kRagged, {pcm(d_in, in_stride)}, {pcm(d_out, out_stride)}, 0, d_gr, ids, n, hops}, (cudaStream_t)cuda_stream);
 }
 extern "C" int pnb_process_sessions_ragged_device_i16(pnb_engine *e, const int *ids, const int *hops, int n, const short *d_in,
                                                       size_t in_stride, short *d_out, size_t out_stride, float *d_gr,
                                                       void *cuda_stream) {
-  return device_call(e, {Call::kRagged, d_in, in_stride, d_out, out_stride, true, 0, d_gr, ids, n, hops}, (cudaStream_t)cuda_stream);
+  return device_call(e, {Call::kRagged, {pcm(d_in, in_stride)}, {pcm(d_out, out_stride)}, 0, d_gr, ids, n, hops}, (cudaStream_t)cuda_stream);
 }
 extern "C" int pnb_process_sessions_ragged_host_f32(pnb_engine *e, const int *ids, const int *hops, int n, const float *in,
                                                     size_t in_stride, float *out, size_t out_stride, float *gr) {
-  return host_call(e, {Call::kRagged, in, in_stride, out, out_stride, false, 0, gr, ids, n, hops}, false);
+  return host_call(e, {Call::kRagged, {pcm(in, in_stride)}, {pcm(out, out_stride)}, 0, gr, ids, n, hops}, false);
 }
 extern "C" int pnb_process_sessions_ragged_host_i16(pnb_engine *e, const int *ids, const int *hops, int n, const short *in,
                                                     size_t in_stride, short *out, size_t out_stride, float *gr) {
-  return host_call(e, {Call::kRagged, in, in_stride, out, out_stride, true, 0, gr, ids, n, hops}, false);
+  return host_call(e, {Call::kRagged, {pcm(in, in_stride)}, {pcm(out, out_stride)}, 0, gr, ids, n, hops}, false);
 }
 
 // pnb_reset_sessions / pnb_export_sessions / pnb_import_sessions.  A reset or an import takes the listed sessions out

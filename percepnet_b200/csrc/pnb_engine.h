@@ -60,8 +60,8 @@ struct pnb_engine {
   float *h[5] = {};
   long hop = 0;  // hops processed since reset
 
-  // Device staging of the host-buffer calls (pnb_process_host_*, pnb_submit_host_*, pnb_train_records_host,
-  // pnb_submit_train_records): two slots, each an input and an output buffer, allocated on first use and only ever
+  // Device staging of the host-buffer calls (every *_host entry point, pnb_submit_host_* and pnb_submit_train_records):
+  // two slots, each an input and an output buffer, allocated on first use and only ever
   // grown.  Pipelined calls take slot submitted & 1 and copy on s_in / s_out (created for the first of them), ordered
   // with the call on `stream` by the slot's events; blocking calls borrow the slot the next pipelined call will take and
   // run on `stream` alone.

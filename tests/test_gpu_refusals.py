@@ -1,7 +1,8 @@
 """Every refusal of the engine's entry points.  Each bad argument, alone and together with others where the order of the
 checks decides which one is reported, gives a fixed return code and pnb_last_error() text, and every entry point of a
 family refuses alike.  A refused call enqueues nothing and changes nothing: each engine's launch count stays, and its
-next valid slot, session, ragged and training-record call gives the bits of a twin engine that saw no refusal."""
+next valid slot, session, ragged, training-record, training-audio and network call gives the bits of a twin engine that
+saw no refusal."""
 import ctypes
 
 import numpy as np
@@ -28,12 +29,16 @@ SESSION = ["pnb_process_sessions_host_f32", "pnb_process_sessions_host_i16", "pn
 RAGGED = ["pnb_process_sessions_ragged_host_f32", "pnb_process_sessions_ragged_host_i16",
           "pnb_process_sessions_ragged_device_f32", "pnb_process_sessions_ragged_device_i16"]
 TRAIN = ["pnb_train_records_host", "pnb_submit_train_records", "pnb_train_records_device"]
+AUDIO = ["pnb_train_audio_host", "pnb_train_audio_device"]
+NETWORK = ["pnb_compute_rnn_host", "pnb_compute_rnn_device"]
+SCORE = ["pnb_score_records_host", "pnb_score_records_device"]
 STATES = ["pnb_reset_streams", "pnb_export_states", "pnb_import_states"]
 ONE_STATE = ["pnb_get_state", "pnb_set_state"]
 SESSION_STATES = ["pnb_reset_sessions", "pnb_export_sessions", "pnb_import_sessions"]
 
 # family: (entry points, engine, valid arguments, {case: the arguments it changes}).  "e" names the engine: slot (an
-# enhancement engine with active range ACTIVE), ses (one in session mode), trn (PNB_TRAIN_DATA), or None for NULL.
+# enhancement engine with active range ACTIVE), ses (one in session mode), trn (PNB_TRAIN_DATA), aud (PNB_TRAIN_DATA |
+# PNB_TRAIN_AUDIO), net (PNB_NETWORK_ONLY), or None for NULL.
 FAMILIES = {
     "slot": (SLOT, "slot", {"F": FMAX}, {
         "engine NULL": {"e": None},
@@ -45,6 +50,7 @@ FAMILIES = {
         "in_stride short": {"in_stride": ROW - 1},
         "out_stride short": {"out_stride": ROW - 1},
         "session mode": {"e": "ses"},
+        "network-only engine": {"e": "net"},
         "training engine, F 0": {"e": "trn", "F": 0},
         "F 0, in NULL": {"F": 0, "in": None},
         "out NULL, in_stride short": {"out": None, "in_stride": ROW - 1},
@@ -107,6 +113,8 @@ FAMILIES = {
         "engine NULL": {"e": None},
         "enhancement engine": {"e": "slot"},
         "session engine": {"e": "ses"},
+        "audio engine": {"e": "aud"},
+        "network-only engine": {"e": "net"},
         "F 0": {"F": 0},
         "F max+1": {"F": FMAX + 1},
         "speech NULL": {"speech": None},
@@ -119,6 +127,48 @@ FAMILIES = {
         "F 0, speech NULL": {"F": 0, "speech": None},
         "records NULL, speech_stride short": {"records": None, "speech_stride": ROW - 1},
         "records_stride short, noisy_stride short": {"records_stride": FMAX * 138 - 1, "noisy_stride": ROW - 1},
+        "audio engine, F 0": {"e": "aud", "F": 0},
+    }),
+    "audio": (AUDIO, "aud", {"F": FMAX}, {
+        "engine NULL": {"e": None},
+        "enhancement engine": {"e": "slot"},
+        "records engine": {"e": "trn"},
+        "F 0": {"F": 0},
+        "F max+1": {"F": FMAX + 1},
+        "speech NULL": {"speech": None},
+        "noisy NULL": {"noisy": None},
+        "records NULL": {"records": None},
+        "audio NULL": {"audio": None},
+        "speech_stride short": {"speech_stride": ROW - 1},
+        "noisy_stride short": {"noisy_stride": ROW - 1},
+        "records_stride short": {"records_stride": FMAX * 138 - 1},
+        "audio_stride short": {"audio_stride": ROW - 1},
+        "records engine, F 0": {"e": "trn", "F": 0},
+        "records engine, records_stride short": {"e": "trn", "records_stride": FMAX * 138 - 1},
+        "records_stride short, audio_stride short": {"records_stride": FMAX * 138 - 1, "audio_stride": ROW - 1},
+    }),
+    "network": (NETWORK, "net", {"F": FMAX, "in_stride": FMAX * 70}, {
+        "training engine": {"e": "trn"},
+        "F 0": {"F": 0},
+        "in NULL": {"in": None},
+        "gr NULL": {"gr": None},
+        "in_stride short": {"in_stride": FMAX * 70 - 1},
+        "in_stride short, records": {"format": 1, "in_stride": FMAX * 138 - 1},
+        "gr_stride short": {"gr_stride": FMAX * 68 - 1},
+        "format 2": {"format": 2},
+        "session mode": {"e": "ses"},
+        "format 2, in_stride short": {"format": 2, "in_stride": FMAX * 70 - 1},
+        "session mode, format 2": {"e": "ses", "format": 2},
+    }),
+    "score": (SCORE, "net", {"F": FMAX}, {
+        "sums NULL": {"sums": None},
+        "rec_stride short": {"records_stride": FMAX * 138 - 1},
+        "gr_stride short": {"gr_stride": FMAX * 68 - 1},
+        "frames[i] -1": {"frames": [FMAX] * 5 + [-1] + [FMAX] * (S - 6)},
+        "frames[i] F+1": {"frames": [FMAX] * 2 + [FMAX + 1] + [FMAX] * (S - 3)},
+        "training engine": {"e": "trn"},
+        "session mode": {"e": "ses"},
+        "session mode, frames[i] -1": {"e": "ses", "frames": [FMAX] * 5 + [-1] + [FMAX] * (S - 6)},
     }),
     "states": (STATES, "slot", {"ids": SLOTS}, {
         "engine NULL": {"e": None},
@@ -194,6 +244,9 @@ BLOB_CASE_KEYS = ("blobs", "stride")   # arguments pnb_reset_streams / pnb_reset
 SESSION_MODE = "engine is in session mode (pnb_sessions_reserve): slots are the pool's; use the *_sessions entry points"
 TRAINING_ENGINE = "engine was created with PNB_TRAIN_DATA: use pnb_train_records_* / pnb_submit_train_records"
 NO_POOL = "no session pool: call pnb_sessions_reserve first"
+NETWORK_ENGINE = "engine was created with PNB_NETWORK_ONLY: use pnb_compute_rnn_* / pnb_score_records_*"
+AUDIO_ENGINE = "engine was created with PNB_TRAIN_AUDIO: use pnb_train_audio_*, so that its audio has no gaps"
+NOT_AUDIO = "engine was not created with PNB_TRAIN_AUDIO"
 STRIDE = "row stride smaller than n_frames*480"
 # (family, case): (return code, pnb_last_error()); -1 is PNB_ERR_ARG.
 EXPECTED = {
@@ -206,6 +259,7 @@ EXPECTED = {
     ("slot", "in_stride short"): (-1, STRIDE),
     ("slot", "out_stride short"): (-1, STRIDE),
     ("slot", "session mode"): (-1, SESSION_MODE),
+    ("slot", "network-only engine"): (-1, NETWORK_ENGINE),
     ("slot", "training engine, F 0"): (-1, TRAINING_ENGINE),
     ("slot", "F 0, in NULL"): (-1, "n_frames 0 outside [1, 4]"),
     ("slot", "out NULL, in_stride short"): (-1, "input/output pointer is NULL"),
@@ -262,6 +316,8 @@ EXPECTED = {
     ("train", "engine NULL"): (-1, "engine is NULL"),
     ("train", "enhancement engine"): (-1, "engine was not created with PNB_TRAIN_DATA"),
     ("train", "session engine"): (-1, "engine was not created with PNB_TRAIN_DATA"),
+    ("train", "audio engine"): (-1, AUDIO_ENGINE),
+    ("train", "network-only engine"): (-1, NETWORK_ENGINE),
     ("train", "F 0"): (-1, "n_frames 0 outside [1, 4]"),
     ("train", "F max+1"): (-1, "n_frames 5 outside [1, 4]"),
     ("train", "speech NULL"): (-1, "speech/noisy/records pointer is NULL"),
@@ -274,6 +330,42 @@ EXPECTED = {
     ("train", "F 0, speech NULL"): (-1, "n_frames 0 outside [1, 4]"),
     ("train", "records NULL, speech_stride short"): (-1, "speech/noisy/records pointer is NULL"),
     ("train", "records_stride short, noisy_stride short"): (-1, STRIDE),
+    ("train", "audio engine, F 0"): (-1, "n_frames 0 outside [1, 4]"),
+    ("audio", "engine NULL"): (-1, "engine is NULL"),
+    ("audio", "enhancement engine"): (-1, "engine was not created with PNB_TRAIN_DATA"),
+    ("audio", "records engine"): (-1, NOT_AUDIO),
+    ("audio", "F 0"): (-1, "n_frames 0 outside [1, 4]"),
+    ("audio", "F max+1"): (-1, "n_frames 5 outside [1, 4]"),
+    ("audio", "speech NULL"): (-1, "speech/noisy/records pointer is NULL"),
+    ("audio", "noisy NULL"): (-1, "speech/noisy/records pointer is NULL"),
+    ("audio", "records NULL"): (-1, "speech/noisy/records pointer is NULL"),
+    ("audio", "audio NULL"): (-1, "speech/noisy/records pointer is NULL"),
+    ("audio", "speech_stride short"): (-1, STRIDE),
+    ("audio", "noisy_stride short"): (-1, STRIDE),
+    ("audio", "records_stride short"): (-1, "records_stride smaller than n_frames*138"),
+    ("audio", "audio_stride short"): (-1, "audio_stride smaller than n_frames*480"),
+    ("audio", "records engine, F 0"): (-1, "n_frames 0 outside [1, 4]"),
+    ("audio", "records engine, records_stride short"): (-1, NOT_AUDIO),
+    ("audio", "records_stride short, audio_stride short"): (-1, "records_stride smaller than n_frames*138"),
+    ("network", "training engine"): (-1, TRAINING_ENGINE),
+    ("network", "F 0"): (-1, "n_frames 0 outside [1, 4]"),
+    ("network", "in NULL"): (-1, "input/output pointer is NULL"),
+    ("network", "gr NULL"): (-1, "input/output pointer is NULL"),
+    ("network", "in_stride short"): (-1, "row stride smaller than n_frames*70"),
+    ("network", "in_stride short, records"): (-1, "row stride smaller than n_frames*138"),
+    ("network", "gr_stride short"): (-1, "row stride smaller than n_frames*68"),
+    ("network", "format 2"): (-1, "format 2 is neither PNB_RNN_FEATURES (0) nor PNB_RNN_RECORDS (1)"),
+    ("network", "session mode"): (-1, SESSION_MODE),
+    ("network", "format 2, in_stride short"): (-1, "row stride smaller than n_frames*70"),
+    ("network", "session mode, format 2"): (-1, "format 2 is neither PNB_RNN_FEATURES (0) nor PNB_RNN_RECORDS (1)"),
+    ("score", "sums NULL"): (-1, "input/output pointer is NULL"),
+    ("score", "rec_stride short"): (-1, "row stride smaller than n_frames*138"),
+    ("score", "gr_stride short"): (-1, "row stride smaller than n_frames*68"),
+    ("score", "frames[i] -1"): (-1, "frames[5] = -1 outside [0, 4]"),
+    ("score", "frames[i] F+1"): (-1, "frames[2] = 5 outside [0, 4]"),
+    ("score", "training engine"): (-1, TRAINING_ENGINE),
+    ("score", "session mode"): (-1, SESSION_MODE),
+    ("score", "session mode, frames[i] -1"): (-1, SESSION_MODE),
     ("states", "engine NULL"): (-1, "engine is NULL"),
     ("states", "session mode"): (-1, SESSION_MODE),
     ("states", "n -1"): (-1, "n = -1 is negative"),
@@ -360,10 +452,17 @@ def _call(L, name, a, keep):
         args += [] if name.startswith("pnb_submit") else [None]
         args += [a["stream"]] if "device" in name else []
         return f(*args)
-    if name in TRAIN:
+    tail = [a["stream"]] if name.endswith("device") else []
+    if name in TRAIN + AUDIO:
         args = [a["e"], a["speech"], a["speech_stride"], a["noisy"], a["noisy_stride"], a["F"], a["records"],
                 a["records_stride"]]
-        return f(*args, *([a["stream"]] if name.endswith("device") else []))
+        args += [a["audio"], a["audio_stride"]] if name in AUDIO else []
+        return f(*args, *tail)
+    if name in NETWORK:
+        return f(a["e"], a["format"], a["in"], a["in_stride"], a["F"], a["gr"], a["gr_stride"], *tail)
+    if name in SCORE:
+        return f(a["e"], a["records"], a["records_stride"], a["F"], _ints(a.get("frames"), keep), a["sums"], a["gr"],
+                 a["gr_stride"], *tail)
     if name in STATES + SESSION_STATES:
         if "reset" in name:
             return f(a["e"], ids, n, a["stream"])
@@ -383,9 +482,10 @@ class _Buffers:
         self.h32, self.h16 = np.zeros((S, ROW), np.float32), np.zeros((S, ROW), np.int16)
         self.d32 = torch.zeros((2, S, ROW), dtype=torch.float32, device="cuda")
         self.d16 = torch.zeros((2, S, ROW), dtype=torch.int16, device="cuda")
-        self.hsp, self.hrec = np.zeros((S // 2, ROW), np.int16), np.zeros((S // 2, FMAX * 138), np.float32)
-        self.dsp = torch.zeros((2, S // 2, ROW), dtype=torch.int16, device="cuda")
-        self.drec = torch.zeros((S // 2, FMAX * 138), device="cuda")
+        self.hsp, self.hrec = np.zeros((S // 2, ROW), np.int16), np.zeros((S, FMAX * 138), np.float32)
+        self.dsp = torch.zeros((3, S // 2, ROW), dtype=torch.int16, device="cuda")
+        self.drec = torch.zeros((S, FMAX * 138), device="cuda")
+        self.hsums, self.dsums = np.zeros((S, 4)), torch.zeros((S, 4), dtype=torch.float64, device="cuda")
         self.blobs = torch.zeros(((CAP + 1) * (SZ + 4),), dtype=torch.uint8, device="cuda")
         self.state = ctypes.create_string_buffer(SZ)   # zeros: not a pnb_get_state blob
         self.stream = torch.cuda.current_stream().cuda_stream
@@ -395,14 +495,16 @@ class _Buffers:
         a = {"stream": self.stream, "blobs": self.blobs.data_ptr(), "stride": SZ, "buf": self.state, "bytes": SZ}
         if "host" in name or "submit_host" in name or name == "pnb_submit_train_records":
             h = self.h16 if name.endswith("i16") else self.h32
-            a.update({"in": h.ctypes.data, "out": h.ctypes.data, "speech": self.hsp.ctypes.data,
-                      "noisy": self.hsp.ctypes.data, "records": self.hrec.ctypes.data})
+            a.update({"in": h.ctypes.data, "out": h.ctypes.data, "gr": h.ctypes.data, "speech": self.hsp.ctypes.data,
+                      "noisy": self.hsp.ctypes.data, "records": self.hrec.ctypes.data, "audio": self.hsp.ctypes.data,
+                      "sums": self.hsums.ctypes.data})
         else:
             d = self.d16 if name.endswith("i16") else self.d32
-            a.update({"in": d[0].data_ptr(), "out": d[1].data_ptr(), "speech": self.dsp[0].data_ptr(),
-                      "noisy": self.dsp[1].data_ptr(), "records": self.drec.data_ptr()})
+            a.update({"in": d[0].data_ptr(), "out": d[1].data_ptr(), "gr": d[1].data_ptr(),
+                      "speech": self.dsp[0].data_ptr(), "noisy": self.dsp[1].data_ptr(), "records": self.drec.data_ptr(),
+                      "audio": self.dsp[2].data_ptr(), "sums": self.dsums.data_ptr()})
         a.update({"in_stride": ROW, "out_stride": ROW, "speech_stride": ROW, "noisy_stride": ROW,
-                  "records_stride": FMAX * 138})
+                  "records_stride": FMAX * 138, "audio_stride": ROW, "gr_stride": FMAX * 68, "format": 0})
         return a
 
 
@@ -436,7 +538,9 @@ def _engines(api, model, mode):
     slot, ses = api.Engine(S, FMAX, model, flags), api.Engine(S, FMAX, model, flags)
     slot.set_active(ACTIVE)
     ses.reserve_sessions(CAP)
-    return {"slot": slot, "ses": ses, "trn": api.Engine(S, FMAX, None, api.TRAIN_DATA)}
+    return {"slot": slot, "ses": ses, "trn": api.Engine(S, FMAX, None, api.TRAIN_DATA),
+            "aud": api.Engine(S, FMAX, None, api.TRAIN_DATA | api.TRAIN_AUDIO),
+            "net": api.Engine(S, FMAX, model, flags | api.NETWORK_ONLY)}
 
 
 @pytest.mark.parametrize("mode", MODES)
@@ -446,11 +550,14 @@ def test_refusals(api, model0, mode):
     import torch
     x = _signal(S, 2, 43)
     speech, noisy = _pairs(S // 2, 2 * FMAX, 7)
+    rec = np.random.RandomState(44).rand(S, 2 * FMAX, 138).astype(np.float32)   # labels in [0, 1)
     engines, twins = _engines(api, model0, mode), _engines(api, model0, mode)
     for es in (engines, twins):   # one valid call of each kind before the refusals
         es["slot"].process(np.ascontiguousarray(x[:ACTIVE, :ROW]))
         es["ses"].process_sessions(IDS, np.ascontiguousarray(x[:len(IDS), :ROW]))
         es["trn"].train_records(np.ascontiguousarray(speech[:, :ROW]), np.ascontiguousarray(noisy[:, :ROW]))
+        es["aud"].train_audio(np.ascontiguousarray(speech[:, :ROW]), np.ascontiguousarray(noisy[:, :ROW]))
+        es["net"].compute_rnn(np.ascontiguousarray(rec[:, :FMAX, :70]))
     bufs = _Buffers()
     torch.cuda.synchronize()
     launches = {k: e.launches for k, e in engines.items()}
@@ -474,6 +581,10 @@ def test_refusals(api, model0, mode):
     s, y = np.ascontiguousarray(speech[:, ROW:]), np.ascontiguousarray(noisy[:, ROW:])
     ra, rb = (es["trn"].train_records(s, y) for es in (engines, twins))
     assert np.array_equal(ra.view(np.int32), rb.view(np.int32))
+    (ra, aa), (rb, ab) = (es["aud"].train_audio(s, y) for es in (engines, twins))
+    assert np.array_equal(ra.view(np.int32), rb.view(np.int32)) and np.array_equal(aa, ab) and np.abs(aa).max() > 0
+    (sa, ga), (sb, gb) = (es["net"].score_records(rec[:, FMAX:], want_gr=True) for es in (engines, twins))
+    assert np.array_equal(sa, sb) and np.array_equal(ga, gb) and np.abs(ga).max() > 0
     for es in (engines, twins):
         for e in es.values():
             e.check()

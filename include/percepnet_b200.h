@@ -74,7 +74,7 @@ enum {
   PNB_TRAIN_AUDIO = 32,  /* with PNB_TRAIN_DATA only: the generator also resynthesises every noisy file with its own
                             labels, as train() writes test_output.pcm (pnb_train_audio_*, which replace
                             pnb_train_records_* / pnb_submit_train_records on such an engine)                 */
-  PNB_NETWORK_ONLY = 64  /* the network alone: an engine for pnb_compute_rnn_* and pnb_score_records_*, without the
+  PNB_NETWORK_ONLY = 64, /* the network alone: an engine for pnb_compute_rnn_* and pnb_score_records_*, without the
                             signal-path buffers of a PCM engine (history lines, overlap-add and pitch memory, spectrum
                             rings, per-call spectra; about 14.7 GB at 16 384 streams x 100 hops).  pnb_process_*,
                             pnb_submit_*, pnb_train_* and pnb_sessions_reserve are refused with PNB_ERR_ARG before
@@ -83,6 +83,14 @@ enum {
                             refused.  State blobs: export writes the network part and zeroes the signal part, import
                             takes the network part and ignores the signal part, so blobs move both ways between this
                             engine and a PCM engine of the same network path. */
+  PNB_SIGNAL_ONLY = 128  /* the signal path alone: an engine for pnb_analyze_* / pnb_synthesize_*, with g/r from the caller.
+                            model may be NULL and is ignored; no fc weights, network state or network buffers are
+                            allocated.  Every other call, pnb_train_* and pnb_sessions_reserve are refused with PNB_ERR_ARG
+                            before anything is enqueued.  Not with PNB_NN_TENSOR, PNB_CONV_WIDE, PNB_TRAIN_DATA,
+                            PNB_TRAIN_AUDIO or PNB_NETWORK_ONLY; with PNB_POSTFILTER and PNB_KEEP_TAPS (the PNB_TAP_NN_*
+                            taps are refused).  State blobs: export writes the signal part and zeroes the network part,
+                            import takes the signal part and ignores the network part, so blobs move both ways between
+                            this engine and a PCM engine. */
 };
 
 typedef struct pnb_engine pnb_engine;
@@ -241,12 +249,54 @@ int pnb_score_records_device(pnb_engine *e, const float *d_rec, size_t rec_strid
 int pnb_score_records_host(pnb_engine *e, const float *rec, size_t rec_stride, int n_frames, const int *frames,
                            double *sums, float *gr, size_t gr_stride);
 
+/* The signal path without the network: pnb_process_* cut where the network sits, so the g/r between analysis and
+ * synthesis come from the caller -- another engine's pnb_compute_rnn_*, a torch model, a records file's ideal gains,
+ * the reference's feature_test.raw.  Both halves work on the active rows [0, n), stream-major:
+ *   in / d_in     PCM rows as pnb_process_*_* takes them (int16: s/32768.f)
+ *   feat / d_feat row i receives n_frames x 70 floats, feat_stride >= n_frames*70: hop t is bit for bit
+ *                 PNB_TAP_FEATURES[t][i] of a pnb_process_* call on the same input
+ *   gr / d_gr     row i holds n_frames x 68 floats (34 g then 34 r per hop), gr_stride >= n_frames*68
+ *   out / d_out   PCM rows as pnb_process_*_* writes them (int16: C truncation of y*32768, wrapping)
+ * These are the layouts of pnb_compute_rnn_* (PNB_RNN_FEATURES in, g/r out), so the three calls chain on device
+ * pointers with no reshaping; f32 and int16 forms of the two halves mix freely.
+ * pnb_analyze_* advances the active slots' signal input by n_frames hops (stage-in, analysis, history bookkeeping) and
+ * leaves a pending synthesis on the engine.  The next pnb_synthesize_*, with the same n_frames, completes those hops
+ * with the caller's g/r in place of the network's (post-filtered on a PNB_POSTFILTER engine), writes the PCM and commits
+ * the hops.  A pnb_process_* call on the same input with the same g/r produces the same output and leaves the engine in
+ * the same state.  g/r are used as given: for finite values the output is the reference's synthesis arithmetic on them
+ * (pitch_filter and interp_band_gain are linear in r and g; nothing is clamped); for non-finite values the affected
+ * rows' output is unspecified, the call still completes and the other rows are unaffected.
+ * While a synthesis is pending, only pnb_synthesize_*, pnb_compute_rnn_* / pnb_score_records_* (they touch no signal
+ * state), pnb_wait, pnb_check, pnb_flush, pnb_read_tap, the profile readers and pnb_reset (which cancels it) are
+ * accepted.  Every other call and state operation -- another pnb_analyze_*, pnb_process_* / pnb_submit_*,
+ * pnb_set_active_streams, pnb_reset_streams / pnb_export_states / pnb_import_states, pnb_get_state / pnb_set_state,
+ * pnb_sessions_reserve -- returns PNB_ERR_ARG before anything is enqueued: between the halves a stream is mid-hop (its
+ * overlap-add memory lags its history), a state no blob may capture.
+ * Also refused with PNB_ERR_ARG before anything is enqueued: pnb_synthesize_* with nothing pending or another n_frames,
+ * an engine in session mode, PNB_TRAIN_DATA and PNB_NETWORK_ONLY engines, NULL pointers, short strides, n_frames outside
+ * [1, max_frames]; a poisoned engine returns PNB_ERR_CUDA.  Ordering, blocking and poisoning are those of
+ * pnb_process_device_* / pnb_process_host_*.
+ * Launches: pnb_analyze_* issues three (stage-in, analysis, feature store), plus the history move on the calls where
+ * pnb_process_* would issue it; pnb_synthesize_* issues two (g/r stage-in, synthesis). */
+int pnb_analyze_host_f32(pnb_engine *e, const float *in, size_t in_stride, int n_frames, float *feat, size_t feat_stride);
+int pnb_analyze_host_i16(pnb_engine *e, const short *in, size_t in_stride, int n_frames, float *feat, size_t feat_stride);
+int pnb_analyze_device_f32(pnb_engine *e, const float *d_in, size_t in_stride, int n_frames, float *d_feat,
+                           size_t feat_stride, void *cuda_stream);
+int pnb_analyze_device_i16(pnb_engine *e, const short *d_in, size_t in_stride, int n_frames, float *d_feat,
+                           size_t feat_stride, void *cuda_stream);
+int pnb_synthesize_host_f32(pnb_engine *e, const float *gr, size_t gr_stride, int n_frames, float *out, size_t out_stride);
+int pnb_synthesize_host_i16(pnb_engine *e, const float *gr, size_t gr_stride, int n_frames, short *out, size_t out_stride);
+int pnb_synthesize_device_f32(pnb_engine *e, const float *d_gr, size_t gr_stride, int n_frames, float *d_out,
+                              size_t out_stride, void *cuda_stream);
+int pnb_synthesize_device_i16(pnb_engine *e, const float *d_gr, size_t gr_stride, int n_frames, short *d_out,
+                              size_t out_stride, void *cuda_stream);
+
 /* Per-stream state for migration between engines / GPUs (the live part of the reference's DenoiseState + RNNState,
  * src/denoise.cpp:71-85, src/nnet_data.h:28-38): input history, overlap-add memory, pitch continuity, the spectra the
  * next five hops will analyse, conv histories and GRU states -- pnb_state_size() bytes, a flat host blob.
  * Both calls wait for the engine to be idle.  A state taken from stream a of one engine and set on stream b of another
  * (any batch size, either network mode, same model) continues the stream exactly where it left off: bit for bit between
- * engines of the same mode.  PNB_TRAIN_DATA engines carry the signal part only. */
+ * engines of the same mode.  PNB_TRAIN_DATA and PNB_SIGNAL_ONLY engines carry the signal part only. */
 size_t pnb_state_size(void);
 int pnb_get_state(pnb_engine *e, int stream, void *dst, size_t dst_bytes);
 int pnb_set_state(pnb_engine *e, int stream, const void *src, size_t src_bytes);
@@ -404,7 +454,8 @@ long long pnb_launch_count(const pnb_engine *e);
  * streams' history back to the start of their rows, at most every call, typically every eighth; one more on a ragged
  * session call in which some session runs fewer than n_frames = max(hops) hops).  On a PNB_TRAIN_AUDIO engine it is the
  * value of a PNB_TRAIN_DATA engine of the same shape plus one: the resynthesis launch.  On a PNB_NETWORK_ONLY engine it
- * is the launch count of one pnb_compute_rnn_* call of n_frames hops. */
+ * is the launch count of one pnb_compute_rnn_* call of n_frames hops; on a PNB_SIGNAL_ONLY engine that of one
+ * pnb_analyze_* and one pnb_synthesize_* call of n_frames hops (five, without the history move). */
 int pnb_launches_per_call(const pnb_engine *e, int n_frames);
 /* Bytes of the engine's device buffers whose size pnb_create fixes (weights, network buffers, stream state, per-call
  * scratch); not the staging that host-buffer calls grow on first use, nor a session pool's parking area. */

@@ -19,6 +19,7 @@ LIB_PATH = os.path.join(HERE, "libpercepnet_b200.so")
 
 FRAME = 480
 NN_FP32, NN_TENSOR, POSTFILTER, KEEP_TAPS, TRAIN_DATA, CONV_WIDE, TRAIN_AUDIO, NETWORK_ONLY = 0, 1, 2, 4, 8, 16, 32, 64
+SIGNAL_ONLY = 128
 RECORD = 138
 RNN_FEATURES, RNN_RECORDS = 0, 1   # pnb_compute_rnn_* formats: 70 features or 138 record floats per hop
 TAPS = {"features": (0, np.float32, 70), "pitch": (1, np.int32, 4), "pitchf": (2, np.float32, 2),
@@ -67,6 +68,10 @@ def load_library() -> C.CDLL:
     L.pnb_compute_rnn_host.argtypes = [vp, i, vp, sz, i, vp, sz]
     L.pnb_score_records_device.argtypes = [vp, vp, sz, i, vp, vp, vp, sz, vp]
     L.pnb_score_records_host.argtypes = [vp, vp, sz, i, vp, vp, vp, sz]
+    for name in ("pnb_analyze_host_f32", "pnb_analyze_host_i16", "pnb_synthesize_host_f32", "pnb_synthesize_host_i16"):
+        getattr(L, name).argtypes = [vp, vp, sz, i, vp, sz]
+    for name in ("pnb_analyze_device_f32", "pnb_analyze_device_i16", "pnb_synthesize_device_f32", "pnb_synthesize_device_i16"):
+        getattr(L, name).argtypes = [vp, vp, sz, i, vp, sz, vp]
     L.pnb_engine_bytes.argtypes = [vp]
     L.pnb_engine_bytes.restype = sz
     L.pnb_flush.argtypes = [vp, vp]
@@ -115,6 +120,8 @@ def load_library() -> C.CDLL:
 EXPORTS = ("pnb_create", "pnb_destroy", "pnb_reset", "pnb_resolve_device", "pnb_process_host_f32", "pnb_process_host_i16",
            "pnb_model_load_blob", "pnb_model_load_stream", "pnb_model_free", "pnb_train_records_host", "pnb_train_records_device", "pnb_submit_train_records", "pnb_train_audio_host", "pnb_train_audio_device", "pnb_process_device_f32", "pnb_process_device_i16", "pnb_submit_host_f32", "pnb_submit_host_i16", "pnb_submit_device_f32", "pnb_submit_device_i16", "pnb_flush", "pnb_wait", "pnb_check",
            "pnb_compute_rnn_device", "pnb_compute_rnn_host", "pnb_score_records_device", "pnb_score_records_host",
+           "pnb_analyze_host_f32", "pnb_analyze_host_i16", "pnb_analyze_device_f32", "pnb_analyze_device_i16",
+           "pnb_synthesize_host_f32", "pnb_synthesize_host_i16", "pnb_synthesize_device_f32", "pnb_synthesize_device_i16",
            "pnb_engine_bytes",
            "pnb_read_tap", "pnb_state_size", "pnb_get_state", "pnb_set_state",
            "pnb_reset_streams", "pnb_export_states", "pnb_import_states", "pnb_set_active_streams", "pnb_active_streams",
@@ -303,6 +310,53 @@ class Engine:
         self._ck(self.L.pnb_score_records_device(self.h, d_rec or None, rec_stride, n_frames,
                                                  None if fr is None else fr.ctypes.data, d_sums or None, d_gr or None,
                                                  gr_stride, stream or None), "pnb_score_records_device")
+
+    def analyze(self, x: np.ndarray) -> np.ndarray:
+        """pnb_analyze_host_*: the analysis half of process.  x: [active, F*480] float32 (C-API scale) or int16 (CLI wire
+        format).  Returns the network input [active, F, 70] float32 (the features tap of a process call on x) and leaves
+        a synthesis of F hops pending: the next call must be synthesize (or compute_rnn, or reset)."""
+        n = self.active
+        assert x.ndim == 2 and x.shape[0] == n and x.shape[1] % FRAME == 0
+        F = x.shape[1] // FRAME
+        x = np.ascontiguousarray(x)
+        feat = np.empty((n, F, 70), np.float32)
+        if x.dtype == np.float32:
+            f = self.L.pnb_analyze_host_f32
+        elif x.dtype == np.int16:
+            f = self.L.pnb_analyze_host_i16
+        else:
+            raise TypeError("x must be float32 or int16")
+        self._ck(f(self.h, x.ctypes.data, x.shape[1], F, feat.ctypes.data, F * 70), "pnb_analyze_host")
+        return feat
+
+    def synthesize(self, gr: np.ndarray, int16: bool = False) -> np.ndarray:
+        """pnb_synthesize_host_*: the synthesis half of process, with the caller's gains.  gr: [active, F, 68] float32
+        (34 g then 34 r per hop), F the hops of the pending analysis.  Returns [active, F*480] float32, or int16 with
+        the CLI's conversion."""
+        n = self.active
+        if gr.dtype != np.float32:
+            raise TypeError("gr must be float32")
+        assert gr.ndim == 3 and gr.shape[0] == n and gr.shape[2] == 68, "gr must be [active, F, 68]"
+        F = gr.shape[1]
+        gr = np.ascontiguousarray(gr)
+        out = np.empty((n, F * FRAME), np.int16 if int16 else np.float32)
+        f = self.L.pnb_synthesize_host_i16 if int16 else self.L.pnb_synthesize_host_f32
+        self._ck(f(self.h, gr.ctypes.data, F * 68, F, out.ctypes.data, F * FRAME), "pnb_synthesize_host")
+        return out
+
+    def analyze_device(self, d_in: int, in_stride: int, n_frames: int, d_feat: int, feat_stride: int, stream: int = 0,
+                       int16: bool = False):
+        """pnb_analyze_device_* on raw device pointers (strides in elements)."""
+        f = self.L.pnb_analyze_device_i16 if int16 else self.L.pnb_analyze_device_f32
+        self._ck(f(self.h, d_in or None, in_stride, n_frames, d_feat or None, feat_stride, stream or None),
+                 "pnb_analyze_device")
+
+    def synthesize_device(self, d_gr: int, gr_stride: int, n_frames: int, d_out: int, out_stride: int, stream: int = 0,
+                          int16: bool = False):
+        """pnb_synthesize_device_* on raw device pointers (strides in elements)."""
+        f = self.L.pnb_synthesize_device_i16 if int16 else self.L.pnb_synthesize_device_f32
+        self._ck(f(self.h, d_gr or None, gr_stride, n_frames, d_out or None, out_stride, stream or None),
+                 "pnb_synthesize_device")
 
     @property
     def device_bytes(self) -> int:

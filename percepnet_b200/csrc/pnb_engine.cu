@@ -5,8 +5,10 @@
 //   stage_in -> analysis (all F hops; one warp per stream) -> F x network step -> synthesis -> slide history
 // The network step is the only part that is sequential in time across the batch; analysis and synthesis
 // need no network state, so hops are processed F at a time.  A network-only call (pnb_compute_rnn_*) is
-//   features_stage -> F x network step -> gr_store
-// on caller-supplied features or training records.
+//   rows_stage (features) -> F x network step -> rows_store (g/r)
+// on caller-supplied features or training records.  The split call cuts the PCM call where the network sits:
+//   pnb_analyze_*:    stage_in -> analysis -> rows_store (features) [-> slide history]
+//   pnb_synthesize_*: rows_stage (caller g/r) -> synthesis
 #include <math.h>
 #include <stdarg.h>
 #include <stdio.h>
@@ -161,7 +163,11 @@ extern "C" int pnb_create(pnb_engine **out, int n_streams, int max_frames, const
   const bool net_only = (flags & PNB_NETWORK_ONLY) != 0;
   if (net_only && (flags & (PNB_TRAIN_AUDIO | PNB_POSTFILTER)))
     return fail(PNB_ERR_ARG, "PNB_NETWORK_ONLY runs no signal path: PNB_TRAIN_AUDIO and PNB_POSTFILTER do not apply");
-  int rc = train_mode ? 0 : check_model(model);
+  const bool sig_only = (flags & PNB_SIGNAL_ONLY) != 0;
+  if (sig_only && (flags & (PNB_NN_TENSOR | PNB_CONV_WIDE | PNB_TRAIN_DATA | PNB_TRAIN_AUDIO | PNB_NETWORK_ONLY)))
+    return fail(PNB_ERR_ARG, "PNB_SIGNAL_ONLY runs no network: combine it only with PNB_POSTFILTER and PNB_KEEP_TAPS");
+  const bool has_net = !train_mode && !sig_only;
+  int rc = has_net ? check_model(model) : 0;
   if (rc) return rc;
   device = pnb_resolve_device(device);
   if (device < 0) return device;
@@ -199,7 +205,7 @@ extern "C" int pnb_create(pnb_engine **out, int n_streams, int max_frames, const
     delete t;
     CKD(r);
   }
-  if (!train_mode) {  // both paths run fc from the reference's layout (SURVEY.md App. B)
+  if (has_net) {  // both paths run fc from the reference's layout (SURVEY.md App. B)
     CKD(engine_upload(e, &e->fc.W, model->fc->input_weights, 70 * 128));
     CKD(engine_upload(e, &e->fc.b, model->fc->bias, 128));
   }
@@ -251,7 +257,7 @@ extern "C" int pnb_create(pnb_engine **out, int n_streams, int max_frames, const
     CKD(engine_alloc(e, &e->d_tap_pitchf, F * S * 2, kScratch));
     if (!train_mode) CKD(engine_alloc(e, &e->d_tap_g, F * S * kBands, kScratch));
   }
-  if (!train_mode) {
+  if (has_net) {  // a signal-only engine has no network: no weights, network state or network buffers
     CKD(engine_alloc(e, &e->c2, S * 512, kStreamState));
     const int rc = (flags & PNB_NN_TENSOR) ? tc_prepare(e, model) : f32_prepare(e, model);
     if (rc) { pnb_destroy(e); return rc; }
@@ -304,6 +310,7 @@ extern "C" int pnb_reset(pnb_engine *e) {
   e->h_status[0] = 0;
   e->h_status[1] = kNoRejectedSlot;
   e->hop = 0;
+  e->pending = 0;
   e->n_active = e->S;
   e->poisoned = false;
   if (e->sessions) {  // every session fresh: all parked, every blob marked fresh
@@ -444,18 +451,19 @@ static int enqueue_ordered(pnb_engine *e, cudaStream_t st, Launches launches) {
   CK(cudaGetLastError());
   return n;
 }
-// Enqueues one call of F hops on st (arguments already checked) and commits the hop counter (unless the call leaves the
-// signal state alone: `signal` false, a network call), last_frames and the launch count when all of it was accepted.
+// Enqueues one call of F hops on st (arguments already checked) and commits the hop counter (unless commit_hop is false:
+// a network call, which leaves the signal state alone, or an analysis, whose synthesis commits it), last_frames and the
+// launch count when all of it was accepted.
 // The enqueue itself moves host-side stream state (advance_line the line offset), so a failure after it started leaves
 // the streams' state undefined: the engine is poisoned, and refuses calls until pnb_reset.
 template <typename Launches>
-static int enqueue_call(pnb_engine *e, int F, cudaStream_t st, Launches launches, bool signal = true) {
+static int enqueue_call(pnb_engine *e, int F, cudaStream_t st, Launches launches, bool commit_hop = true) {
   const int n = enqueue_ordered(e, st, launches);
   if (n < 0) {
     e->poisoned = true;
     return n;
   }
-  if (signal) e->hop += F;
+  if (commit_hop) e->hop += F;
   e->last_frames = F;
   e->launches += n;
   return PNB_OK;
@@ -548,9 +556,10 @@ static Rows pcm(const T *p, size_t stride) { return rows(p, stride, kFrame, size
 
 // One call as its entry point received it, its buffers as row arrays.  In / out: PCM / PCM of a slot, session or ragged
 // call; speech, noisy / records and (pnb_train_audio_*) audio of a training-record call; features or records / g/r of a
-// network call; records / g/r (when asked for) and the loss sums of a score call.
+// network call; records / g/r (when asked for) and the loss sums of a score call; PCM / features of an analysis; g/r /
+// PCM of a synthesis.
 struct Call {
-  enum Kind { kSlots, kSessions, kRagged, kNetwork, kRecords } kind;
+  enum Kind { kSlots, kSessions, kRagged, kNetwork, kRecords, kAnalyze, kSynthesize } kind;
   Rows in[2], out[2];
   int F;           // hops; a ragged call's is max(hops), set by check_call
   float *gr;       // enhancement calls: g/r destination [F][rows][68], or null
@@ -575,7 +584,8 @@ static int enqueue_network(pnb_engine *e, const Call &c, cudaStream_t st) {
     if (c.frames) { int rc = stage_ints(e, c.frames, (size_t)na, st, &frames); if (rc) return rc; }
     {
       ProfScope ps(e, PNB_K_STAGE_IN, st);
-      n += launch_features_stage(e->d_feat, static_cast<const float *>(in.p), in.stride, (int)in.width, na, S, F, st);
+      n += launch_rows_stage(e->d_feat, kFeat, static_cast<const float *>(in.p), in.stride, (int)in.width,
+                             c.format == PNB_RNN_RECORDS ? 68 : 0, na, S, F, st);
     }
     CK(cudaGetLastError());
     {
@@ -587,7 +597,7 @@ static int enqueue_network(pnb_engine *e, const Call &c, cudaStream_t st) {
       ProfScope ps(e, PNB_K_STAGE_IN, st);
       n += launch_loss_sums(e->d_gr, static_cast<const float *>(in.p), in.stride, frames, static_cast<double *>(sums.p), na, S, F, st);
     }
-    if (gr.p) { ProfScope ps(e, PNB_K_STAGE_IN, st); n += launch_gr_store(e->d_gr, static_cast<float *>(gr.p), gr.stride, na, S, F, st); }
+    if (gr.p) { ProfScope ps(e, PNB_K_STAGE_IN, st); n += launch_rows_store(e->d_gr, 68, static_cast<float *>(gr.p), gr.stride, na, S, F, st); }
     return n;
   }, false);
 }
@@ -682,9 +692,69 @@ static int enqueue_enhance(pnb_engine *e, const Call &c, cudaStream_t st) {
   });
 }
 
+// The analysis half of a slot call on st (arguments already checked): stage-in, analysis and, when it falls due, the
+// history slide, exactly as enqueue_enhance runs them, and the features out to the caller's rows.  The hop counter stays
+// where it is (the analysis and synthesis kernels both take hop0 = e->hop); the synthesis that completes these hops
+// commits it.  The slide may run before the synthesis: synthesis reads the spectra, not the history line.
+static int enqueue_analyze(pnb_engine *e, const Call &c, cudaStream_t st) {
+  const int F = c.F;
+  const Rows &in = c.in[0], &feat = c.out[0];
+  const bool i16 = in.bytes == sizeof(short);
+  const int rc = enqueue_call(e, F, st, [&]() -> int {
+    const int S = e->S, na = e->n_active;
+    int n = 0;
+    {
+      ProfScope ps(e, PNB_K_STAGE_IN, st);
+      n += launch_stage_in(e->d_pcm + e->line_off, e->pcm_stride, i16 ? nullptr : static_cast<const float *>(in.p),
+                           i16 ? static_cast<const short *>(in.p) : nullptr, in.stride, na, F * kFrame, st, 32768.f);
+    }
+    { ProfScope ps(e, PNB_K_ANALYSIS, st); n += launch_analysis(analysis_args(e, F), st); }
+    { ProfScope ps(e, PNB_K_STAGE_IN, st); n += launch_rows_store(e->d_feat, kFeat, static_cast<float *>(feat.p), feat.stride, na, S, F, st); }
+    n += advance_line(e, F, st);
+    return n;
+  }, false);
+  if (rc == PNB_OK) e->pending = F;
+  return rc;
+}
+
+// The synthesis half (arguments already checked, an analysis of F hops pending): the caller's g/r rows into d_gr where
+// the network hook would have left them, then the synthesis of enqueue_enhance, which commits the hop counter.
+static int enqueue_synthesize(pnb_engine *e, const Call &c, cudaStream_t st) {
+  const int F = c.F;
+  const Rows &gr = c.in[0], &out = c.out[0];
+  const bool i16 = out.bytes == sizeof(short);
+  const int rc = enqueue_call(e, F, st, [&]() -> int {
+    int n = 0;
+    {
+      ProfScope ps(e, PNB_K_STAGE_IN, st);
+      n += launch_rows_stage(e->d_gr, 68, static_cast<const float *>(gr.p), gr.stride, 68, 0, e->n_active, e->S, F, st);
+    }
+    SynthesisArgs sa = synthesis_args(e, F, i16 ? nullptr : static_cast<float *>(out.p),
+                                      i16 ? static_cast<short *>(out.p) : nullptr, out.stride);
+    ProfScope ps(e, PNB_K_SYNTHESIS, st);
+    n += launch_synthesis(sa, st);
+    return n;
+  });
+  if (rc == PNB_OK) e->pending = 0;
+  return rc;
+}
+
 // The call's enqueue body (arguments already checked).
 static int enqueue(pnb_engine *e, const Call &c, cudaStream_t st) {
-  return c.kind == Call::kNetwork ? enqueue_network(e, c, st) : c.kind == Call::kRecords ? enqueue_records(e, c, st) : enqueue_enhance(e, c, st);
+  switch (c.kind) {
+    case Call::kNetwork: return enqueue_network(e, c, st);
+    case Call::kRecords: return enqueue_records(e, c, st);
+    case Call::kAnalyze: return enqueue_analyze(e, c, st);
+    case Call::kSynthesize: return enqueue_synthesize(e, c, st);
+    default: return enqueue_enhance(e, c, st);
+  }
+}
+
+// Every call and state operation but pnb_synthesize_* and the network calls, while an analysis waits for its synthesis:
+// a stream's state between the halves is mid-hop (its overlap-add memory lags its history), and no blob may capture it.
+static int refuse_pending(const pnb_engine *e) {
+  return fail(PNB_ERR_ARG, "a synthesis is pending (pnb_analyze_* of %d hops): call pnb_synthesize_* with the same n_frames, or pnb_reset",
+              e->pending);
 }
 
 // The slot-level entry points of an engine in session mode: refused before anything is enqueued.
@@ -722,10 +792,12 @@ static int check_strides(const Rows (&a)[2], int F) {
 }
 
 // Every refusal of a call, before anything changes.  Every call checks an engine of its family (training records,
-// enhancement or the network alone; a PNB_NETWORK_ONLY engine runs network calls only) that no failed call has
-// poisoned, 1 <= F <= Fmax, none of its arrays NULL, the input strides; a training-record call then that its engine
-// has audio exactly when the call does; every call then the output strides.  After that a slot call checks session
-// mode, a session call its list, a network call its format, then session mode, and a score call its frames.  A ragged
+// enhancement or the network alone; a PNB_NETWORK_ONLY engine runs network calls only, a PNB_SIGNAL_ONLY engine split
+// calls only) that no failed call has poisoned, 1 <= F <= Fmax, none of its arrays NULL, the input strides; a
+// training-record call then that its engine has audio exactly when the call does; every call then the output strides,
+// and the pending synthesis: a synthesis needs one of F hops, every other call but a network call needs none.  After
+// that a slot or split call checks session mode, a session call its list, a network call its format, then session mode,
+// and a score call its frames.  A ragged
 // call checks the list and its hop counts first, because their largest is the call's length F; when every session runs
 // F hops, hops becomes null and the call is the plain session call.
 static int check_call(pnb_engine *e, Call &c) {
@@ -743,9 +815,12 @@ static int check_call(pnb_engine *e, Call &c) {
     if (uniform) c.hops = nullptr;
   }
   const bool train = c.kind == Call::kRecords, network = c.kind == Call::kNetwork;
+  const bool split = c.kind == Call::kAnalyze || c.kind == Call::kSynthesize;
   if (!e) return fail(PNB_ERR_ARG, "engine is NULL");
   if (!network && (e->flags & PNB_NETWORK_ONLY))
     return fail(PNB_ERR_ARG, "engine was created with PNB_NETWORK_ONLY: use pnb_compute_rnn_* / pnb_score_records_*");
+  if (!split && (e->flags & PNB_SIGNAL_ONLY))
+    return fail(PNB_ERR_ARG, "engine was created with PNB_SIGNAL_ONLY: use pnb_analyze_* / pnb_synthesize_*");
   if (train && !(e->flags & PNB_TRAIN_DATA)) return fail(PNB_ERR_ARG, "engine was not created with PNB_TRAIN_DATA");
   if (!train && (e->flags & PNB_TRAIN_DATA))
     return fail(PNB_ERR_ARG, "engine was created with PNB_TRAIN_DATA: use pnb_train_records_* / pnb_submit_train_records");
@@ -760,10 +835,16 @@ static int check_call(pnb_engine *e, Call &c) {
   if (train && !audio && (e->flags & PNB_TRAIN_AUDIO))
     return fail(PNB_ERR_ARG, "engine was created with PNB_TRAIN_AUDIO: use pnb_train_audio_*, so that its audio has no gaps");
   { int rc = check_strides(c.out, c.F); if (rc) return rc; }
+  if (c.kind == Call::kSynthesize) {
+    if (!e->pending) return fail(PNB_ERR_ARG, "no analysis awaits its synthesis: call pnb_analyze_* first");
+    if (c.F != e->pending) return fail(PNB_ERR_ARG, "n_frames %d, but the pending analysis has %d hops", c.F, e->pending);
+  } else if (e->pending && !network) {
+    return refuse_pending(e);
+  }
   if (c.kind == Call::kSessions) return check_ids(e, c.ids, c.n_ids, e->S);
   if (network && c.format != PNB_RNN_FEATURES && c.format != PNB_RNN_RECORDS)
     return fail(PNB_ERR_ARG, "format %d is neither PNB_RNN_FEATURES (0) nor PNB_RNN_RECORDS (1)", c.format);
-  if ((c.kind == Call::kSlots || network) && e->sessions) return refuse_in_session_mode();
+  if ((c.kind == Call::kSlots || network || split) && e->sessions) return refuse_in_session_mode();
   if (c.frames)  // every row's counted hops in [0, F]
     for (int i = 0; i < e->n_active; i++)
       if (c.frames[i] < 0 || c.frames[i] > c.F) return fail(PNB_ERR_ARG, "frames[%d] = %d outside [0, %d]", i, c.frames[i], c.F);
@@ -1035,6 +1116,43 @@ extern "C" int pnb_score_records_host(pnb_engine *e, const float *rec, size_t re
   return host_call(e, score_call(rec, rec_stride, n_frames, frames, sums, gr, gr_stride), false);
 }
 
+// The split call: the analysis half of a slot call (PCM rows in, the network input out) and its synthesis half (the
+// caller's g/r in, PCM rows out); f32 and int16 forms of either half mix freely.
+static Call analyze_call(const void *in, size_t in_bytes, size_t in_stride, int n_frames, float *feat, size_t feat_stride) {
+  return {Call::kAnalyze, {rows(in, in_stride, kFrame, in_bytes)}, {rows(feat, feat_stride, kFeat, sizeof(float), "feat_stride")}, n_frames};
+}
+static Call synthesize_call(const float *gr, size_t gr_stride, int n_frames, void *out, size_t out_bytes, size_t out_stride) {
+  return {Call::kSynthesize, {rows(gr, gr_stride, 68, sizeof(float), "gr_stride")}, {rows(out, out_stride, kFrame, out_bytes)}, n_frames};
+}
+extern "C" int pnb_analyze_host_f32(pnb_engine *e, const float *in, size_t in_stride, int n_frames, float *feat, size_t feat_stride) {
+  return host_call(e, analyze_call(in, sizeof(float), in_stride, n_frames, feat, feat_stride), false);
+}
+extern "C" int pnb_analyze_host_i16(pnb_engine *e, const short *in, size_t in_stride, int n_frames, float *feat, size_t feat_stride) {
+  return host_call(e, analyze_call(in, sizeof(short), in_stride, n_frames, feat, feat_stride), false);
+}
+extern "C" int pnb_analyze_device_f32(pnb_engine *e, const float *d_in, size_t in_stride, int n_frames, float *d_feat,
+                                      size_t feat_stride, void *cuda_stream) {
+  return device_call(e, analyze_call(d_in, sizeof(float), in_stride, n_frames, d_feat, feat_stride), (cudaStream_t)cuda_stream);
+}
+extern "C" int pnb_analyze_device_i16(pnb_engine *e, const short *d_in, size_t in_stride, int n_frames, float *d_feat,
+                                      size_t feat_stride, void *cuda_stream) {
+  return device_call(e, analyze_call(d_in, sizeof(short), in_stride, n_frames, d_feat, feat_stride), (cudaStream_t)cuda_stream);
+}
+extern "C" int pnb_synthesize_host_f32(pnb_engine *e, const float *gr, size_t gr_stride, int n_frames, float *out, size_t out_stride) {
+  return host_call(e, synthesize_call(gr, gr_stride, n_frames, out, sizeof(float), out_stride), false);
+}
+extern "C" int pnb_synthesize_host_i16(pnb_engine *e, const float *gr, size_t gr_stride, int n_frames, short *out, size_t out_stride) {
+  return host_call(e, synthesize_call(gr, gr_stride, n_frames, out, sizeof(short), out_stride), false);
+}
+extern "C" int pnb_synthesize_device_f32(pnb_engine *e, const float *d_gr, size_t gr_stride, int n_frames, float *d_out,
+                                         size_t out_stride, void *cuda_stream) {
+  return device_call(e, synthesize_call(d_gr, gr_stride, n_frames, d_out, sizeof(float), out_stride), (cudaStream_t)cuda_stream);
+}
+extern "C" int pnb_synthesize_device_i16(pnb_engine *e, const float *d_gr, size_t gr_stride, int n_frames, short *d_out,
+                                         size_t out_stride, void *cuda_stream) {
+  return device_call(e, synthesize_call(d_gr, gr_stride, n_frames, d_out, sizeof(short), out_stride), (cudaStream_t)cuda_stream);
+}
+
 extern "C" int pnb_flush(pnb_engine *e, void *cuda_stream) {
   if (!e) return fail(PNB_ERR_ARG, "engine is NULL");
   CK(cudaSetDevice(e->device));
@@ -1095,6 +1213,8 @@ extern "C" int pnb_read_tap(pnb_engine *e, int what, void *dst, size_t dst_bytes
     }
     default: return fail(PNB_ERR_ARG, "unknown tap %d", what);
   }
+  if (!src && (e->flags & PNB_SIGNAL_ONLY) && what >= PNB_TAP_NN_C2 && what < PNB_TAP_G_USED)
+    return fail(PNB_ERR_ARG, "tap %d: a PNB_SIGNAL_ONLY engine has no network state", what);
   if (!src && (e->flags & PNB_NETWORK_ONLY))
     return fail(PNB_ERR_ARG, "tap %d: a PNB_NETWORK_ONLY engine keeps the features, g/r and network state taps only", what);
   if (!src) return fail(PNB_ERR_ARG, "tap %d needs PNB_KEEP_TAPS at pnb_create", what);
@@ -1144,6 +1264,7 @@ static int check_blobs(const void *d_blobs, size_t blob_stride) {
 static int state_batch(pnb_engine *e, int mode, const int *streams, int n, void *d_blobs, size_t blob_stride, void *cuda_stream) {
   if (!e) return fail(PNB_ERR_ARG, "engine is NULL");
   if (e->sessions) return refuse_in_session_mode();
+  if (e->pending) return refuse_pending(e);
   if (n < 0) return fail(PNB_ERR_ARG, "n = %d is negative", n);
   if (n == 0) return PNB_OK;
   if (!streams) return fail(PNB_ERR_ARG, "streams is NULL");
@@ -1173,6 +1294,7 @@ extern "C" int pnb_set_active_streams(pnb_engine *e, int n, void *cuda_stream) {
   if (!e) return fail(PNB_ERR_ARG, "engine is NULL");
   if (e->flags & PNB_TRAIN_DATA) return fail(PNB_ERR_ARG, "PNB_TRAIN_DATA engines always advance all their streams");
   if (e->sessions) return refuse_in_session_mode();
+  if (e->pending) return refuse_pending(e);
   if (n < 1 || n > e->S) return fail(PNB_ERR_ARG, "active streams %d outside [1, %d]", n, e->S);
   if (e->poisoned) return fail(PNB_ERR_ARG, "an earlier call failed while enqueuing work; the streams' state is undefined until pnb_reset");
   if (n > e->n_active) {
@@ -1190,6 +1312,7 @@ extern "C" int pnb_active_streams(const pnb_engine *e) { return e ? e->n_active 
 static int state_args(pnb_engine *e, int stream, const void *buf, size_t bytes) {
   if (!e || !buf) return fail(PNB_ERR_ARG, "NULL argument");
   if (e->sessions) return refuse_in_session_mode();
+  if (e->pending) return refuse_pending(e);
   { int rc = check_list(e, &stream, 1, e->S, e->n_active, "stream"); if (rc) return rc; }
   if (bytes < sizeof(StreamState)) return fail(PNB_ERR_ARG, "state buffer of %zu bytes, need pnb_state_size() = %zu", bytes, sizeof(StreamState));
   if (e->poisoned) return fail(PNB_ERR_CUDA, "engine state is undefined after a failed call; pnb_reset it");
@@ -1250,6 +1373,8 @@ extern "C" int pnb_sessions_reserve(pnb_engine *e, int n_sessions) {
   if (!e) return fail(PNB_ERR_ARG, "engine is NULL");
   if (e->flags & PNB_TRAIN_DATA) return fail(PNB_ERR_ARG, "PNB_TRAIN_DATA engines have no session pool");
   if (e->flags & PNB_NETWORK_ONLY) return fail(PNB_ERR_ARG, "PNB_NETWORK_ONLY engines have no session pool");
+  if (e->flags & PNB_SIGNAL_ONLY) return fail(PNB_ERR_ARG, "PNB_SIGNAL_ONLY engines have no session pool");
+  if (e->pending) return refuse_pending(e);
   if (e->poisoned) return fail(PNB_ERR_ARG, "an earlier call failed while enqueuing work; the streams' state is undefined until pnb_reset");
   if (n_sessions < 1) return fail(PNB_ERR_ARG, "n_sessions = %d, need >= 1", n_sessions);
   if (e->sessions && n_sessions <= e->pool.capacity()) return PNB_OK;  // the pool never shrinks
@@ -1524,7 +1649,9 @@ extern "C" int pnb_launches_per_call(const pnb_engine *e, int n_frames) {
   // stage_in, analysis, the network, synthesis; without the history move of advance_line (at most one more launch per
   // call), and without the fix-up of a ragged session call in which a session runs fewer hops than the call (one more);
   // the resynthesis of a PNB_TRAIN_AUDIO engine is one launch more than its records alone; a PNB_NETWORK_ONLY engine's
-  // call is pnb_compute_rnn_*: features_stage, the network, gr_store
+  // call is pnb_compute_rnn_*: rows_stage, the network, rows_store; a PNB_SIGNAL_ONLY engine's is one pnb_analyze_*
+  // (stage_in, analysis, rows_store) and one pnb_synthesize_* (rows_stage, synthesis)
+  if (e->flags & PNB_SIGNAL_ONLY) return 5;
   const int net = (e->flags & PNB_NN_TENSOR) ? tc_network_launches(e, n_frames) : f32_network_launches(e, n_frames);
   if (e->flags & PNB_NETWORK_ONLY) return 2 + net;
   return 3 + net + ((e->flags & PNB_TRAIN_AUDIO) ? 1 : 0);

@@ -76,6 +76,9 @@ struct pnb_engine {
   std::shared_ptr<pnb_tc_state> tc;
   std::shared_ptr<pnb_f32_state> f32;
   int last_frames = 0;
+  // hops of an analysis (pnb_analyze_*) whose synthesis (pnb_synthesize_*) is still due, or 0.  Between the two halves
+  // the analysed streams are mid-hop, so every call and state operation but the synthesis and network calls is refused.
+  int pending = 0;
   long long launches = 0;
   // status word on the device: bit 0 = an activation left the domain in which the reference's tansig_approx is
   // defined (tensor path only; reported as PNB_ERR_DOMAIN by the synchronising entry points, cleared by pnb_reset);

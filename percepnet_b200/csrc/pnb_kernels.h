@@ -89,13 +89,14 @@ int launch_stage_in(float *pcm, size_t pcm_stride, const float *in, const short 
                     const int *hops = nullptr);
 int launch_slide_history(float *pcm, size_t pcm_stride, int n_streams, int n_samples, cudaStream_t st);
 
-// ---- network-only calls (pnb_rnn_io.cu) --------------------------------------------------
-// rows [0, n_streams) of `in` (n_frames hops of width = 70 features or 138 record floats each) -> feat [F][S][70];
-// records are scaled like create_features (x30 on the first 68 values)
-int launch_features_stage(float *feat, const float *in, size_t in_stride, int width, int n_streams, int S, int n_frames,
-                          cudaStream_t st);
-// gr [F][S][68] -> rows [0, n_streams) of `out`, n_frames x 68 floats each
-int launch_gr_store(const float *gr, float *out, size_t out_stride, int n_streams, int S, int n_frames, cudaStream_t st);
+// ---- layout moves of the network and split calls (pnb_rnn_io.cu) ---------------------------
+// rows [0, n_streams) of `in` (n_frames hops of in_width floats each) -> dst [F][S][w], w = 70 (features, or records
+// with in_width 138) or 68 (g/r); the first n_scaled values of each hop are multiplied by 30 (records: 68, else 0)
+int launch_rows_stage(float *dst, int w, const float *in, size_t in_stride, int in_width, int n_scaled, int n_streams,
+                      int S, int n_frames, cudaStream_t st);
+// src [F][S][w] -> rows [0, n_streams) of `out`, n_frames x w floats each; w = 68 (g/r) or 70 (features)
+int launch_rows_store(const float *src, int w, float *out, size_t out_stride, int n_streams, int S, int n_frames,
+                      cudaStream_t st);
 // rnn_train.py's CustomLoss sums of rows [0, n_streams): gr [F][S][68] against the labels rec[t][70..137] of row i's
 // first frames[i] hops (frames null: all n_frames) -> sums[i] = {sum dg^2, sum dg^4, sum dr^2, count} in float64
 int launch_loss_sums(const float *gr, const float *rec, size_t rec_stride, const int *frames, double *sums, int n_streams,

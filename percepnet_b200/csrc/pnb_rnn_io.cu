@@ -1,38 +1,42 @@
-// pnb_rnn_io.cu -- the two copies of a network call (pnb_compute_rnn_*): the caller's stream-major rows of
-// features or training records into the per-call buffer [F][S][70] the network hooks read, and the hooks' g/r
-// [F][S][68] back out to stream-major rows; and the loss of a score call (pnb_score_records_*), reduced from the same
-// g/r and the records' labels.
+// pnb_rnn_io.cu -- the layout moves between a caller's stream-major rows and the per-call buffers [F][S][w] of the
+// engine: the network call's features or training records into d_feat and its g/r out of d_gr (pnb_compute_rnn_*), the
+// analysis half's features out of d_feat (pnb_analyze_*) and the synthesis half's caller g/r into d_gr
+// (pnb_synthesize_*); and the loss of a score call (pnb_score_records_*), reduced from the same g/r and the records'
+// labels.
 #include "../../include/percepnet_b200.h"
 #include "pnb_kernels.h"
 
 namespace pnb {
 
-// feat[(t*S + s)*70 + j] = in[s*in_stride + t*width + j] for the rows [0, n) of every hop t.  width = 138 (records):
-// the first 68 values are scaled by 30 (create_features, denoise.cpp:487-496; rnn_train.py:44-48), T and pitchcorr
-// are taken as they are, the labels rec[70..137] are never read.  Threads walk the output in order: the writes are
-// contiguous, the reads contiguous runs of 70 floats.
-__global__ void features_stage_kernel(float *__restrict__ feat, const float *__restrict__ in, size_t in_stride, int width,
-                                      int n, int S, int F) {
-  const long long total = (long long)F * n * kFeat;
+// dst[(t*S + s)*W + j] = in[s*in_stride + t*in_width + j] for the rows [0, n) of every hop t and j < W; the first
+// n_scaled values of a hop are multiplied by 30, the others copied as they are.  Features: W = 70, in_width 70, none
+// scaled.  Records: W = 70, in_width 138, the first 68 scaled (create_features, denoise.cpp:487-496; rnn_train.py:44-48),
+// T and pitchcorr as they are, the labels rec[70..137] never read.  g/r: W = 68, in_width 68, none scaled.  Threads walk
+// the output in order: the writes are contiguous, the reads contiguous runs of W floats.
+template <int W>
+__global__ void rows_stage_kernel(float *__restrict__ dst, const float *__restrict__ in, size_t in_stride, int in_width,
+                                  int n_scaled, int n, int S, int F) {
+  const long long total = (long long)F * n * W;
   for (long long x = (long long)blockIdx.x * blockDim.x + threadIdx.x; x < total; x += (long long)gridDim.x * blockDim.x) {
-    const int j = (int)(x % kFeat);
-    const long long ts = x / kFeat;
+    const int j = (int)(x % W);
+    const long long ts = x / W;
     const int s = (int)(ts % n), t = (int)(ts / n);
-    const float v = in[(size_t)s * in_stride + (size_t)t * width + j];
-    feat[((size_t)t * S + s) * kFeat + j] = (width != kFeat && j < 68) ? v * 30.f : v;
+    const float v = in[(size_t)s * in_stride + (size_t)t * in_width + j];
+    dst[((size_t)t * S + s) * W + j] = j < n_scaled ? v * 30.f : v;
   }
 }
 
-// out[s*out_stride + t*68 + c] = gr[(t*S + s)*68 + c] for the rows [0, n).  Threads walk the output in order: the
-// writes are contiguous, the reads contiguous runs of 68 floats.
-__global__ void gr_store_kernel(const float *__restrict__ gr, float *__restrict__ out, size_t out_stride, int n, int S,
-                                int F) {
-  const long long total = (long long)n * F * 68;
+// out[s*out_stride + t*W + c] = src[(t*S + s)*W + c] for the rows [0, n): g/r (W = 68) and features (W = 70).  Threads
+// walk the output in order: the writes are contiguous, the reads contiguous runs of W floats.
+template <int W>
+__global__ void rows_store_kernel(const float *__restrict__ src, float *__restrict__ out, size_t out_stride, int n, int S,
+                                  int F) {
+  const long long total = (long long)n * F * W;
   for (long long x = (long long)blockIdx.x * blockDim.x + threadIdx.x; x < total; x += (long long)gridDim.x * blockDim.x) {
-    const int c = (int)(x % 68);
-    const long long st = x / 68;
+    const int c = (int)(x % W);
+    const long long st = x / W;
     const int t = (int)(st % F), s = (int)(st / F);
-    out[(size_t)s * out_stride + (size_t)t * 68 + c] = gr[((size_t)t * S + s) * 68 + c];
+    out[(size_t)s * out_stride + (size_t)t * W + c] = src[((size_t)t * S + s) * W + c];
   }
 }
 
@@ -86,16 +90,19 @@ static unsigned copy_blocks(long long total) {
   return (unsigned)(b < 8192 ? b : 8192);
 }
 
-int launch_features_stage(float *feat, const float *in, size_t in_stride, int width, int n_streams, int S, int n_frames,
-                          cudaStream_t st) {
-  features_stage_kernel<<<copy_blocks((long long)n_frames * n_streams * kFeat), 256, 0, st>>>(feat, in, in_stride, width,
-                                                                                             n_streams, S, n_frames);
+int launch_rows_stage(float *dst, int w, const float *in, size_t in_stride, int in_width, int n_scaled, int n_streams,
+                      int S, int n_frames, cudaStream_t st) {
+  const unsigned blocks = copy_blocks((long long)n_frames * n_streams * w);
+  if (w == kFeat) rows_stage_kernel<kFeat><<<blocks, 256, 0, st>>>(dst, in, in_stride, in_width, n_scaled, n_streams, S, n_frames);
+  else rows_stage_kernel<68><<<blocks, 256, 0, st>>>(dst, in, in_stride, in_width, n_scaled, n_streams, S, n_frames);
   return 1;
 }
 
-int launch_gr_store(const float *gr, float *out, size_t out_stride, int n_streams, int S, int n_frames, cudaStream_t st) {
-  gr_store_kernel<<<copy_blocks((long long)n_frames * n_streams * 68), 256, 0, st>>>(gr, out, out_stride, n_streams, S,
-                                                                                    n_frames);
+int launch_rows_store(const float *src, int w, float *out, size_t out_stride, int n_streams, int S, int n_frames,
+                      cudaStream_t st) {
+  const unsigned blocks = copy_blocks((long long)n_frames * n_streams * w);
+  if (w == kFeat) rows_store_kernel<kFeat><<<blocks, 256, 0, st>>>(src, out, out_stride, n_streams, S, n_frames);
+  else rows_store_kernel<68><<<blocks, 256, 0, st>>>(src, out, out_stride, n_streams, S, n_frames);
   return 1;
 }
 

@@ -344,7 +344,7 @@ int state_segs(const pnb_engine *e, StateSeg *seg) {
       add_words(seg, ns, kSegCopy, e->d_ering + slot * S * kBands, kBands * 4, offsetof(StreamState, eband) + (size_t)k * kBands * 4, kBands);
     }
   }
-  if (e->flags & PNB_TRAIN_DATA) {  // no network: its part of the blob is zero
+  if (e->flags & (PNB_TRAIN_DATA | PNB_SIGNAL_ONLY)) {  // no network: its part of the blob is zero on export, ignored on import
     add_words(seg, ns, kSegBlobZero, nullptr, 0, offsetof(StreamState, fc_hist),
               (offsetof(StreamState, has_terms) - offsetof(StreamState, fc_hist)) / 4);
     add_words(seg, ns, kSegBlobZero, nullptr, 0, offsetof(StreamState, fc_terms), (sizeof(StreamState) - offsetof(StreamState, fc_terms)) / 4);

@@ -430,42 +430,40 @@ static SynthesisArgs synthesis_args(pnb_engine *e, int F, float *d_out, short *d
 }
 
 // Ordering of an engine's work (see pnb_engine.h): every call and state operation makes its stream wait for the last
-// one before its first launch, and marks its own end behind its last launch.
+// one before its first launch, and marks its own end behind its last launch once all of them were accepted.
 static int wait_last_call(pnb_engine *e, cudaStream_t st) {
   if (e->call_recorded) CK(cudaStreamWaitEvent(st, e->ev_call, 0));
   return PNB_OK;
 }
 static int mark_call_end(pnb_engine *e, cudaStream_t st) {
+  CK(cudaGetLastError());
   CK(cudaEventRecord(e->ev_call, st));
   e->call_recorded = true;
   return PNB_OK;
 }
 
-// The call's own launches, in ev_call's order; returns their count or a negative error.
+// The launches of one call or state operation, in ev_call's order, added to the launch count; returns their count or a
+// negative error.  The enqueue itself may move host-side stream state (advance_line the line offset, a session
+// operation the residency plan) and part of the work may already be enqueued, so a failure after it started leaves the
+// streams' state undefined: the engine is poisoned, and refuses calls and state operations until pnb_reset.
 template <typename Launches>
 static int enqueue_ordered(pnb_engine *e, cudaStream_t st, Launches launches) {
-  { int rc = wait_last_call(e, st); if (rc) return rc; }
-  const int n = launches();
-  if (n < 0) return n;
-  { int rc = mark_call_end(e, st); if (rc) return rc; }
-  CK(cudaGetLastError());
+  int n = wait_last_call(e, st);
+  if (n == PNB_OK) n = launches();
+  if (n >= 0) { const int rc = mark_call_end(e, st); if (rc) n = rc; }
+  if (n < 0) e->poisoned = true;
+  else e->launches += n;
   return n;
 }
 // Enqueues one call of F hops on st (arguments already checked) and commits the hop counter (unless commit_hop is false:
-// a network call, which leaves the signal state alone, or an analysis, whose synthesis commits it), last_frames and the
-// launch count when all of it was accepted.
-// The enqueue itself moves host-side stream state (advance_line the line offset), so a failure after it started leaves
-// the streams' state undefined: the engine is poisoned, and refuses calls until pnb_reset.
+// a network call, which leaves the signal state alone, or an analysis, whose synthesis commits it) and last_frames when
+// all of it was accepted.
 template <typename Launches>
 static int enqueue_call(pnb_engine *e, int F, cudaStream_t st, Launches launches, bool commit_hop = true) {
   const int n = enqueue_ordered(e, st, launches);
-  if (n < 0) {
-    e->poisoned = true;
-    return n;
-  }
+  if (n < 0) return n;
   if (commit_hop) e->hop += F;
   e->last_frames = F;
-  e->launches += n;
   return PNB_OK;
 }
 
@@ -482,8 +480,9 @@ static int stage_ints(pnb_engine *e, const int *src, size_t n, cudaStream_t st, 
   return PNB_OK;
 }
 
-// The state-operation arguments of a session pool: the pieces of a slot at the counters committed by the last call.
-static StateArgs session_args(pnb_engine *e) {
+// What the state kernels of every slot and session operation share: the pieces of a slot at the counters committed by
+// the last call, the import verdicts and status word, and the parking area of a session pool (null without one).
+static StateArgs state_args(pnb_engine *e) {
   StateArgs a;
   memset(&a, 0, sizeof a);
   a.n_seg = state_segs(e, a.seg);
@@ -509,7 +508,7 @@ struct RaggedSlots {
 // active range to the list; *d_row: the row map on the device.  Returns the number of launches or a negative error.
 static int enqueue_plan(pnb_engine *e, const int *ids, int k, const int *hops, int F, cudaStream_t st, const int **d_row,
                         RaggedSlots *rg) {
-  StateArgs a = session_args(e);  // before the plan: parking reads the pieces where the last call left them
+  StateArgs a = state_args(e);  // before the plan: parking reads the pieces where the last call left them
   e->pool.plan(ids, k, e->plan_row, e->plan_moves);
   e->n_active = k;
   const size_t k4 = ((size_t)k + 3) & ~(size_t)3;  // the moves start 16-byte aligned
@@ -536,6 +535,60 @@ static int enqueue_plan(pnb_engine *e, const int *ids, int k, const int *hops, i
   a.n = (int)e->plan_moves.size();
   a.moves = d + k4;
   return launch_session_move(a, st);
+}
+
+// A session export into the caller's blobs (a: their address and stride): resident sessions from their slots
+// (session_move_kernel), parked ones from their parking blobs (session_blob_kernel); nothing moves.  Its upload is
+// [moves of the resident ones][ids of the parked ones][their rows].  Returns the number of launches or a negative error.
+static int enqueue_session_export(pnb_engine *e, const int *ids, int n, StateArgs a, cudaStream_t st) {
+  std::vector<int> &up = e->plan_up;
+  up.clear();
+  std::vector<int> parked, rows;
+  for (int i = 0; i < n; i++) {
+    const int s = e->pool.where[ids[i]];
+    if (s >= 0) up.insert(up.end(), {s, i, kFillNone, -1});
+    else { parked.push_back(ids[i]); rows.push_back(i); }
+  }
+  const int r = (int)up.size() / 4, p = (int)parked.size();
+  up.insert(up.end(), parked.begin(), parked.end());
+  up.insert(up.end(), rows.begin(), rows.end());
+  const int *d = nullptr;
+  { int rc = stage_ints(e, up.data(), up.size(), st, &d); if (rc) return rc; }
+  int n_launches = 0;
+  if (r) { a.n = r; a.moves = d; n_launches += launch_session_move(a, st); }
+  if (p) { a.n = p; a.streams = d + 4 * r; a.rows = d + 4 * r + p; n_launches += launch_session_blob(a, st); }
+  return n_launches;
+}
+
+// One stream-state operation (reset, export or import: mode) as its entry point received it.
+struct StateOp {
+  int mode;
+  const int *list;     // n slots, or session ids when sessions (host)
+  int n;
+  void *blobs;         // blob i at blobs + i * blob_stride; a reset has none
+  size_t blob_stride;
+  bool sessions;
+};
+
+// Enqueues one state operation on st (arguments already checked), after every call and state operation issued earlier
+// on the engine and before every one issued later.  Slots: the list through the index staging, the blob check of an
+// import, the move.  Sessions: an export as enqueue_session_export; a reset or an import takes the sessions out of
+// their slots on the host, then stages the ids, checks the blobs of an import and rewrites their parking blobs.
+static int enqueue_state(pnb_engine *e, const StateOp &op, cudaStream_t st) {
+  const int n = enqueue_ordered(e, st, [&]() -> int {
+    StateArgs a = state_args(e);
+    a.mode = op.mode;
+    a.blobs = static_cast<char *>(op.blobs);
+    a.blob_stride = op.blob_stride;
+    if (op.sessions && op.mode == kStateExport) return enqueue_session_export(e, op.list, op.n, a, st);
+    if (op.sessions)
+      for (int i = 0; i < op.n; i++) e->pool.evict(op.list[i]);
+    { int rc = stage_ints(e, op.list, (size_t)op.n, st, &a.streams); if (rc) return rc; }
+    a.n = op.n;
+    const int check = op.mode == kStateImport ? launch_state_check(a, st) : 0;  // a session import reports session ids
+    return check + (op.sessions ? launch_session_blob(a, st) : launch_state_move(a, st));
+  });
+  return n < 0 ? n : PNB_OK;
 }
 
 // One array of a call's rows, in host or device memory by entry point: row r at p + r * stride values of `bytes` bytes
@@ -762,6 +815,11 @@ static int refuse_in_session_mode() {
   return fail(PNB_ERR_ARG, "engine is in session mode (pnb_sessions_reserve): slots are the pool's; use the *_sessions entry points");
 }
 
+// Every call and state operation of a poisoned engine (enqueue_ordered), with the code its entry point documents.
+static int refuse_poisoned(int code) {
+  return fail(code, "an earlier call failed while enqueuing work; the streams' state is undefined until pnb_reset");
+}
+
 // The entries of a slot or session list, the argument `name`: each in [0, end) and in the active range [0, active) (a
 // session list passes active = end), none listed twice.  Repeats are found with the session pool's scratch, which is -1
 // everywhere between calls; a slot list of an engine without a pool grows it to the number of slots.
@@ -824,7 +882,7 @@ static int check_call(pnb_engine *e, Call &c) {
   if (train && !(e->flags & PNB_TRAIN_DATA)) return fail(PNB_ERR_ARG, "engine was not created with PNB_TRAIN_DATA");
   if (!train && (e->flags & PNB_TRAIN_DATA))
     return fail(PNB_ERR_ARG, "engine was created with PNB_TRAIN_DATA: use pnb_train_records_* / pnb_submit_train_records");
-  if (e->poisoned) return fail(PNB_ERR_CUDA, "an earlier call failed while enqueuing work; the streams' state is undefined until pnb_reset");
+  if (e->poisoned) return refuse_poisoned(PNB_ERR_CUDA);
   if (c.F < 1 || c.F > e->Fmax) return fail(PNB_ERR_ARG, "n_frames %d outside [1, %d]", c.F, e->Fmax);
   for (int i = 0; i < 2; i++)
     if ((c.in[i].width && !c.in[i].p) || (c.out[i].width && !c.out[i].p))
@@ -1230,28 +1288,6 @@ extern "C" int pnb_read_tap(pnb_engine *e, int what, void *dst, size_t dst_bytes
 // ------------------------------------------------------------------------------------------
 extern "C" size_t pnb_state_size(void) { return sizeof(StreamState); }
 
-// Enqueues one batched state operation on st (arguments already checked): after every call and state operation issued
-// earlier on the engine, before every one issued later (ev_call, see pnb_engine.h).
-static int state_enqueue(pnb_engine *e, int mode, const int *streams, int n, void *d_blobs, size_t blob_stride, cudaStream_t st) {
-  StateArgs a;
-  memset(&a, 0, sizeof a);
-  a.n_seg = state_segs(e, a.seg);
-  { int rc = wait_last_call(e, st); if (rc) return rc; }
-  // the slot indices travel through pinned staging: the caller's array is free again when this returns
-  { int rc = stage_ints(e, streams, (size_t)n, st, &a.streams); if (rc) return rc; }
-  a.n = n; a.blobs = static_cast<char *>(d_blobs); a.blob_stride = blob_stride;
-  a.ok = e->d_ok; a.mode = mode; a.status = e->d_status;
-  a.has_terms = (e->flags & PNB_NN_TENSOR) ? 1u : 0u;
-  a.check_gru = (e->flags & PNB_NN_TENSOR) ? 1 : 0;
-  long long nl = 0;
-  if (mode == kStateImport) nl += launch_state_check(a, st);
-  nl += launch_state_move(a, st);
-  CK(cudaGetLastError());
-  { int rc = mark_call_end(e, st); if (rc) return rc; }
-  e->launches += nl;
-  return PNB_OK;
-}
-
 // The blobs of a batched state operation: not NULL, blob_stride at least pnb_state_size(), both 4-byte aligned.
 static int check_blobs(const void *d_blobs, size_t blob_stride) {
   if (!d_blobs) return fail(PNB_ERR_ARG, "d_blobs is NULL");
@@ -1269,13 +1305,11 @@ static int state_batch(pnb_engine *e, int mode, const int *streams, int n, void 
   if (n == 0) return PNB_OK;
   if (!streams) return fail(PNB_ERR_ARG, "streams is NULL");
   if (mode != kStateReset) { int rc = check_blobs(d_blobs, blob_stride); if (rc) return rc; }
-  if (e->poisoned) return fail(PNB_ERR_ARG, "an earlier call failed while enqueuing work; the streams' state is undefined until pnb_reset");
+  if (e->poisoned) return refuse_poisoned(PNB_ERR_ARG);
   if (n > e->S) return fail(PNB_ERR_ARG, "n = %d streams, the engine has %d", n, e->S);
   { int rc = check_list(e, streams, n, e->S, e->n_active, "streams"); if (rc) return rc; }
   CK(cudaSetDevice(e->device));
-  const int rc = state_enqueue(e, mode, streams, n, d_blobs, blob_stride, (cudaStream_t)cuda_stream);
-  if (rc) e->poisoned = true;  // part of the operation may have been enqueued
-  return rc;
+  return enqueue_state(e, {mode, streams, n, d_blobs, blob_stride, false}, (cudaStream_t)cuda_stream);
 }
 
 extern "C" int pnb_reset_streams(pnb_engine *e, const int *streams, int n, void *cuda_stream) {
@@ -1296,44 +1330,44 @@ extern "C" int pnb_set_active_streams(pnb_engine *e, int n, void *cuda_stream) {
   if (e->sessions) return refuse_in_session_mode();
   if (e->pending) return refuse_pending(e);
   if (n < 1 || n > e->S) return fail(PNB_ERR_ARG, "active streams %d outside [1, %d]", n, e->S);
-  if (e->poisoned) return fail(PNB_ERR_ARG, "an earlier call failed while enqueuing work; the streams' state is undefined until pnb_reset");
+  if (e->poisoned) return refuse_poisoned(PNB_ERR_ARG);
   if (n > e->n_active) {
     std::vector<int> entering(n - e->n_active);
     for (int i = 0; i < n - e->n_active; i++) entering[i] = e->n_active + i;
     CK(cudaSetDevice(e->device));
-    const int rc = state_enqueue(e, kStateReset, entering.data(), (int)entering.size(), nullptr, 0, (cudaStream_t)cuda_stream);
-    if (rc) { e->poisoned = true; return rc; }
+    const int rc = enqueue_state(e, {kStateReset, entering.data(), (int)entering.size(), nullptr, 0, false}, (cudaStream_t)cuda_stream);
+    if (rc) return rc;
   }
   e->n_active = n;
   return PNB_OK;
 }
 extern "C" int pnb_active_streams(const pnb_engine *e) { return e ? e->n_active : 0; }
 
-static int state_args(pnb_engine *e, int stream, const void *buf, size_t bytes) {
+static int check_one_state(pnb_engine *e, int stream, const void *buf, size_t bytes) {
   if (!e || !buf) return fail(PNB_ERR_ARG, "NULL argument");
   if (e->sessions) return refuse_in_session_mode();
   if (e->pending) return refuse_pending(e);
   { int rc = check_list(e, &stream, 1, e->S, e->n_active, "stream"); if (rc) return rc; }
   if (bytes < sizeof(StreamState)) return fail(PNB_ERR_ARG, "state buffer of %zu bytes, need pnb_state_size() = %zu", bytes, sizeof(StreamState));
-  if (e->poisoned) return fail(PNB_ERR_CUDA, "engine state is undefined after a failed call; pnb_reset it");
+  if (e->poisoned) return refuse_poisoned(PNB_ERR_CUDA);
   return PNB_OK;
 }
 
 // The single-stream host forms: the batched kernels through one blob of device scratch, with the engine idle before
 // and after.
 extern "C" int pnb_get_state(pnb_engine *e, int stream, void *dst, size_t bytes) {
-  int rc = state_args(e, stream, dst, bytes);
+  int rc = check_one_state(e, stream, dst, bytes);
   if (rc) return rc;
   CK(cudaSetDevice(e->device));
   CK(cudaDeviceSynchronize());
-  if ((rc = state_enqueue(e, kStateExport, &stream, 1, e->d_blob1, sizeof(StreamState), e->stream))) return rc;
+  if ((rc = enqueue_state(e, {kStateExport, &stream, 1, e->d_blob1, sizeof(StreamState), false}, e->stream))) return rc;
   CK(cudaMemcpyAsync(dst, e->d_blob1, sizeof(StreamState), cudaMemcpyDeviceToHost, e->stream));
   CK(cudaStreamSynchronize(e->stream));
   return PNB_OK;
 }
 
 extern "C" int pnb_set_state(pnb_engine *e, int stream, const void *src, size_t bytes) {
-  int rc = state_args(e, stream, src, bytes);
+  int rc = check_one_state(e, stream, src, bytes);
   if (rc) return rc;
   const StreamState *st = static_cast<const StreamState *>(src);
   if (st->magic != kStateMagic || st->version != kStateVersion) return fail(PNB_ERR_ARG, "not a pnb_get_state blob (magic/version)");
@@ -1344,7 +1378,7 @@ extern "C" int pnb_set_state(pnb_engine *e, int stream, const void *src, size_t 
   CK(cudaSetDevice(e->device));
   CK(cudaDeviceSynchronize());
   CK(cudaMemcpyAsync(e->d_blob1, src, sizeof(StreamState), cudaMemcpyHostToDevice, e->stream));
-  if ((rc = state_enqueue(e, kStateImport, &stream, 1, e->d_blob1, sizeof(StreamState), e->stream))) return rc;
+  if ((rc = enqueue_state(e, {kStateImport, &stream, 1, e->d_blob1, sizeof(StreamState), false}, e->stream))) return rc;
   CK(cudaStreamSynchronize(e->stream));
   return PNB_OK;
 }
@@ -1375,7 +1409,7 @@ extern "C" int pnb_sessions_reserve(pnb_engine *e, int n_sessions) {
   if (e->flags & PNB_NETWORK_ONLY) return fail(PNB_ERR_ARG, "PNB_NETWORK_ONLY engines have no session pool");
   if (e->flags & PNB_SIGNAL_ONLY) return fail(PNB_ERR_ARG, "PNB_SIGNAL_ONLY engines have no session pool");
   if (e->pending) return refuse_pending(e);
-  if (e->poisoned) return fail(PNB_ERR_ARG, "an earlier call failed while enqueuing work; the streams' state is undefined until pnb_reset");
+  if (e->poisoned) return refuse_poisoned(PNB_ERR_ARG);
   if (n_sessions < 1) return fail(PNB_ERR_ARG, "n_sessions = %d, need >= 1", n_sessions);
   if (e->sessions && n_sessions <= e->pool.capacity()) return PNB_OK;  // the pool never shrinks
   CK(cudaSetDevice(e->device));
@@ -1458,54 +1492,15 @@ extern "C" int pnb_process_sessions_ragged_host_i16(pnb_engine *e, const int *id
 
 // pnb_reset_sessions / pnb_export_sessions / pnb_import_sessions.  A reset or an import takes the listed sessions out
 // of their slots (the slot's content is abandoned) and rewrites their parking blobs; the next call that lists them
-// unparks them.  An export writes resident sessions from their slots (session_move_kernel) and parked ones from their
-// parking blobs (session_blob_kernel); nothing moves.
+// unparks them.  An export writes each session from where it is; nothing moves.
 static int session_batch(pnb_engine *e, int mode, const int *ids, int n, void *d_blobs, size_t blob_stride, void *cuda_stream) {
   if (!e) return fail(PNB_ERR_ARG, "engine is NULL");
-  if (e->poisoned) return fail(PNB_ERR_ARG, "an earlier call failed while enqueuing work; the streams' state is undefined until pnb_reset");
+  if (e->poisoned) return refuse_poisoned(PNB_ERR_ARG);
   if (n == 0 && e->sessions) return PNB_OK;
   if (mode != kStateReset) { int rc = check_blobs(d_blobs, blob_stride); if (rc) return rc; }
   { int rc = check_ids(e, ids, n, e->pool.capacity()); if (rc) return rc; }
   CK(cudaSetDevice(e->device));
-  const cudaStream_t st = (cudaStream_t)cuda_stream;
-  const int rc = [&]() -> int {
-    { int rc = wait_last_call(e, st); if (rc) return rc; }
-    StateArgs a = session_args(e);
-    a.blobs = static_cast<char *>(d_blobs);
-    a.blob_stride = blob_stride;
-    a.mode = mode;
-    long long nl = 0;
-    std::vector<int> &up = e->plan_up;
-    up.clear();
-    if (mode == kStateExport) {  // [moves of the resident ones][ids of the parked ones][their rows]
-      std::vector<int> parked, rows;
-      for (int i = 0; i < n; i++) {
-        const int s = e->pool.where[ids[i]];
-        if (s >= 0) up.insert(up.end(), {s, i, kFillNone, -1});
-        else { parked.push_back(ids[i]); rows.push_back(i); }
-      }
-      const int r = (int)up.size() / 4, p = (int)parked.size();
-      up.insert(up.end(), parked.begin(), parked.end());
-      up.insert(up.end(), rows.begin(), rows.end());
-      const int *d = nullptr;
-      { int rc = stage_ints(e, up.data(), up.size(), st, &d); if (rc) return rc; }
-      if (r) { a.n = r; a.moves = d; nl += launch_session_move(a, st); }
-      if (p) { a.n = p; a.streams = d + 4 * r; a.rows = d + 4 * r + p; a.blobs = static_cast<char *>(d_blobs); nl += launch_session_blob(a, st); }
-    } else {
-      for (int i = 0; i < n; i++) e->pool.evict(ids[i]);
-      const int *d = nullptr;
-      { int rc = stage_ints(e, ids, (size_t)n, st, &d); if (rc) return rc; }
-      a.n = n; a.streams = d;
-      if (mode == kStateImport) nl += launch_state_check(a, st);  // reports session ids: a.streams are the ids
-      nl += launch_session_blob(a, st);
-    }
-    CK(cudaGetLastError());
-    { int rc = mark_call_end(e, st); if (rc) return rc; }
-    e->launches += nl;
-    return PNB_OK;
-  }();
-  if (rc) e->poisoned = true;  // part of the operation may have been enqueued
-  return rc;
+  return enqueue_state(e, {mode, ids, n, d_blobs, blob_stride, true}, (cudaStream_t)cuda_stream);
 }
 extern "C" int pnb_reset_sessions(pnb_engine *e, const int *ids, int n, void *cuda_stream) {
   return session_batch(e, kStateReset, ids, n, nullptr, 0, cuda_stream);

@@ -87,10 +87,11 @@ struct pnb_engine {
   int *d_status = nullptr;  // [2]
   int *h_status = nullptr;  // [2] pinned host copy, refreshed by the synchronising entry points
 
-  // Ordering: every call (process, submit, train records) and every state operation (pnb_reset_streams /
-  // pnb_export_states / pnb_import_states) makes the stream it is issued on wait for ev_call before its first launch and
-  // records ev_call there after its last.  Each waits for the one before, so ev_call stands for everything issued
-  // earlier on the engine, whichever stream it went to; pnb_flush and pnb_wait wait for it too.
+  // Ordering: every call and every state operation (of slots or sessions, pnb_get_state / pnb_set_state and a grown
+  // active range included) is enqueued through one ordered enqueue (enqueue_ordered), which makes the stream it is
+  // issued on wait for ev_call before its first launch and records ev_call there after its last.  Each waits for the one
+  // before, so ev_call stands for everything issued earlier on the engine, whichever stream it went to; pnb_flush and
+  // pnb_wait wait for it too.  A failure after that enqueue started sets `poisoned`, for every one of them.
   cudaEvent_t ev_call = nullptr;
   bool call_recorded = false;    // ev_call has been recorded at least once
   // batched stream-state operations: staging of the slot indices, import verdicts, one blob of scratch

@@ -312,3 +312,33 @@ def test_bad_arguments_are_refused(api, model0, cfg):
     e.check()
     e.close()
     ref.close()
+
+
+# ---------------------------------------------------------------------------------------------- 7
+@pytest.mark.parametrize("mode", ["fp32", "tensor"])
+def test_state_operation_launches(api, model0, mode):
+    """pnb_launch_count grows by each state operation's own launches: one move for a reset, an export, pnb_get_state and
+    a grown active range; a blob check and a move for an import and pnb_set_state; none for n = 0 or a shrunk range."""
+    import torch
+    S = 16
+    e = _engine(api, model0, S, mode)
+    e.process(_call(_signal(S, 1, 9), 0))
+    blobs = e.export_states([1, 2], None)
+    blob = e.get_state(3)
+    ops = [("reset", lambda: e.reset_streams([0, 5]), 1),
+           ("export", lambda: e.export_states([4, 6], blobs.data_ptr()), 1),
+           ("import", lambda: e.import_states([7, 8], blobs), 2),
+           ("get_state", lambda: e.get_state(9), 1),
+           ("set_state", lambda: e.set_state(10, blob), 2),
+           ("shrink", lambda: e.set_active(12), 0),
+           ("grow", lambda: e.set_active(S), 1),
+           ("reset n 0", lambda: e.reset_streams([]), 0),
+           ("export n 0", lambda: e.export_states([], blobs.data_ptr()), 0),
+           ("import n 0", lambda: e.import_states([], 0), 0)]
+    for name, op, want in ops:
+        n = e.launches
+        op()
+        assert e.launches - n == want, name
+    torch.cuda.synchronize()
+    e.check()
+    e.close()

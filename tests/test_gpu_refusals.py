@@ -2,7 +2,7 @@
 checks decides which one is reported, gives a fixed return code and pnb_last_error() text, and every entry point of a
 family refuses alike.  A refused call enqueues nothing and changes nothing: each engine's launch count stays, and its
 next valid slot, session, ragged, training-record, training-audio and network call gives the bits of a twin engine that
-saw no refusal."""
+saw no refusal.  So do the synthesis of an engine whose analysis was pending during the refusals and the call after it."""
 import ctypes
 
 import numpy as np
@@ -21,6 +21,7 @@ SZ = 63804                             # pnb_state_size()
 IDS = [3, 20, 0, 7, 11, 5]             # a valid session list (ids >= S: more sessions than slots)
 HOPS = [4, 2, 4, 1, 3, 4]
 SLOTS = [2, 0, 11]                     # a valid slot list, inside the active range
+PEND = 3                               # hops of the analysis the pending engine waits to synthesise
 
 SLOT = ["pnb_process_host_f32", "pnb_process_host_i16", "pnb_submit_host_f32", "pnb_submit_host_i16",
         "pnb_process_device_f32", "pnb_process_device_i16", "pnb_submit_device_f32", "pnb_submit_device_i16"]
@@ -37,8 +38,8 @@ ONE_STATE = ["pnb_get_state", "pnb_set_state"]
 SESSION_STATES = ["pnb_reset_sessions", "pnb_export_sessions", "pnb_import_sessions"]
 
 # family: (entry points, engine, valid arguments, {case: the arguments it changes}).  "e" names the engine: slot (an
-# enhancement engine with active range ACTIVE), ses (one in session mode), trn (PNB_TRAIN_DATA), aud (PNB_TRAIN_DATA |
-# PNB_TRAIN_AUDIO), net (PNB_NETWORK_ONLY), or None for NULL.
+# enhancement engine with active range ACTIVE), pend (one like it, with a synthesis pending), ses (one in session mode),
+# trn (PNB_TRAIN_DATA), aud (PNB_TRAIN_DATA | PNB_TRAIN_AUDIO), net (PNB_NETWORK_ONLY), or None for NULL.
 FAMILIES = {
     "slot": (SLOT, "slot", {"F": FMAX}, {
         "engine NULL": {"e": None},
@@ -191,6 +192,11 @@ FAMILIES = {
         "blobs NULL, streams listed twice": {"blobs": None, "ids": [2, 2]},
         "blob_stride short, n slots+1": {"stride": SZ - 4, "ids": list(range(S + 1))},
         "streams[i] inactive, then slots": {"ids": [2, ACTIVE, S]},
+        "pending": {"e": "pend"},
+        "pending, n -1": {"e": "pend", "n": -1},
+        "pending, streams NULL": {"e": "pend", "ids": None, "n": len(SLOTS)},
+        "pending, blobs NULL": {"e": "pend", "blobs": None},
+        "pending, stream slots": {"e": "pend", "ids": [2, S]},
     }),
     "one state": (ONE_STATE, "slot", {"slot": 2}, {
         "engine NULL": {"e": None},
@@ -203,6 +209,10 @@ FAMILIES = {
         "session mode, buffer NULL": {"e": "ses", "buf": None},
         "session mode, stream slots": {"e": "ses", "slot": S},
         "stream slots, bytes short": {"slot": S, "bytes": SZ - 1},
+        "pending": {"e": "pend"},
+        "pending, buffer NULL": {"e": "pend", "buf": None},
+        "pending, stream slots": {"e": "pend", "slot": S},
+        "pending, bytes short": {"e": "pend", "bytes": SZ - 1},
     }),
     "active": (["pnb_set_active_streams"], "slot", {"n": ACTIVE}, {
         "engine NULL": {"e": None},
@@ -212,12 +222,17 @@ FAMILIES = {
         "n slots+1": {"n": S + 1},
         "training engine, n 0": {"e": "trn", "n": 0},
         "session mode, n 0": {"e": "ses", "n": 0},
+        "pending": {"e": "pend"},
+        "pending, n 0": {"e": "pend", "n": 0},
+        "pending, n slots+1": {"e": "pend", "n": S + 1},
     }),
     "reserve": (["pnb_sessions_reserve"], "slot", {"n": CAP}, {
         "engine NULL": {"e": None},
         "training engine": {"e": "trn"},
         "n 0": {"n": 0},
         "training engine, n 0": {"e": "trn", "n": 0},
+        "pending": {"e": "pend"},
+        "pending, n 0": {"e": "pend", "n": 0},
     }),
     "session states": (SESSION_STATES, "ses", {"ids": IDS}, {
         "engine NULL": {"e": None},
@@ -248,6 +263,8 @@ NETWORK_ENGINE = "engine was created with PNB_NETWORK_ONLY: use pnb_compute_rnn_
 AUDIO_ENGINE = "engine was created with PNB_TRAIN_AUDIO: use pnb_train_audio_*, so that its audio has no gaps"
 NOT_AUDIO = "engine was not created with PNB_TRAIN_AUDIO"
 STRIDE = "row stride smaller than n_frames*480"
+PENDING = (f"a synthesis is pending (pnb_analyze_* of {PEND} hops): call pnb_synthesize_* with the same n_frames, "
+           "or pnb_reset")
 # (family, case): (return code, pnb_last_error()); -1 is PNB_ERR_ARG.
 EXPECTED = {
     ("slot", "engine NULL"): (-1, "engine is NULL"),
@@ -386,6 +403,11 @@ EXPECTED = {
     ("states", "blobs NULL, streams listed twice"): (-1, "d_blobs is NULL"),
     ("states", "blob_stride short, n slots+1"): (-1, "blob_stride 63800 below pnb_state_size() = 63804"),
     ("states", "streams[i] inactive, then slots"): (-1, "streams[1] = 12 outside the active range [0, 12)"),
+    ("states", "pending"): (-1, PENDING),
+    ("states", "pending, n -1"): (-1, PENDING),
+    ("states", "pending, streams NULL"): (-1, PENDING),
+    ("states", "pending, blobs NULL"): (-1, PENDING),
+    ("states", "pending, stream slots"): (-1, PENDING),
     ("one state", "engine NULL"): (-1, "NULL argument"),
     ("one state", "buffer NULL"): (-1, "NULL argument"),
     ("one state", "session mode"): (-1, SESSION_MODE),
@@ -396,6 +418,10 @@ EXPECTED = {
     ("one state", "session mode, buffer NULL"): (-1, "NULL argument"),
     ("one state", "session mode, stream slots"): (-1, SESSION_MODE),
     ("one state", "stream slots, bytes short"): (-1, "stream[0] = 16 outside [0, 16)"),
+    ("one state", "pending"): (-1, PENDING),
+    ("one state", "pending, buffer NULL"): (-1, "NULL argument"),
+    ("one state", "pending, stream slots"): (-1, PENDING),
+    ("one state", "pending, bytes short"): (-1, PENDING),
     ("active", "engine NULL"): (-1, "engine is NULL"),
     ("active", "training engine"): (-1, "PNB_TRAIN_DATA engines always advance all their streams"),
     ("active", "session mode"): (-1, SESSION_MODE),
@@ -403,10 +429,15 @@ EXPECTED = {
     ("active", "n slots+1"): (-1, "active streams 17 outside [1, 16]"),
     ("active", "training engine, n 0"): (-1, "PNB_TRAIN_DATA engines always advance all their streams"),
     ("active", "session mode, n 0"): (-1, SESSION_MODE),
+    ("active", "pending"): (-1, PENDING),
+    ("active", "pending, n 0"): (-1, PENDING),
+    ("active", "pending, n slots+1"): (-1, PENDING),
     ("reserve", "engine NULL"): (-1, "engine is NULL"),
     ("reserve", "training engine"): (-1, "PNB_TRAIN_DATA engines have no session pool"),
     ("reserve", "n 0"): (-1, "n_sessions = 0, need >= 1"),
     ("reserve", "training engine, n 0"): (-1, "PNB_TRAIN_DATA engines have no session pool"),
+    ("reserve", "pending"): (-1, PENDING),
+    ("reserve", "pending, n 0"): (-1, PENDING),
     ("session states", "engine NULL"): (-1, "engine is NULL"),
     ("session states", "no pool"): (-1, NO_POOL),
     ("session states", "no pool, n 0"): (-1, NO_POOL),
@@ -535,10 +566,11 @@ def _refusals(L, engines, bufs):
 
 def _engines(api, model, mode):
     flags = api.NN_FP32 if mode == "fp32" else api.NN_TENSOR
-    slot, ses = api.Engine(S, FMAX, model, flags), api.Engine(S, FMAX, model, flags)
+    slot, pend, ses = (api.Engine(S, FMAX, model, flags) for _ in range(3))
     slot.set_active(ACTIVE)
+    pend.set_active(ACTIVE)
     ses.reserve_sessions(CAP)
-    return {"slot": slot, "ses": ses, "trn": api.Engine(S, FMAX, None, api.TRAIN_DATA),
+    return {"slot": slot, "pend": pend, "ses": ses, "trn": api.Engine(S, FMAX, None, api.TRAIN_DATA),
             "aud": api.Engine(S, FMAX, None, api.TRAIN_DATA | api.TRAIN_AUDIO),
             "net": api.Engine(S, FMAX, model, flags | api.NETWORK_ONLY)}
 
@@ -554,6 +586,8 @@ def test_refusals(api, model0, mode):
     engines, twins = _engines(api, model0, mode), _engines(api, model0, mode)
     for es in (engines, twins):   # one valid call of each kind before the refusals
         es["slot"].process(np.ascontiguousarray(x[:ACTIVE, :ROW]))
+        es["pend"].process(np.ascontiguousarray(x[:ACTIVE, :ROW]))
+        es["pend"].analyze(np.ascontiguousarray(x[:ACTIVE, ROW:ROW + PEND * HOP]))
         es["ses"].process_sessions(IDS, np.ascontiguousarray(x[:len(IDS), :ROW]))
         es["trn"].train_records(np.ascontiguousarray(speech[:, :ROW]), np.ascontiguousarray(noisy[:, :ROW]))
         es["aud"].train_audio(np.ascontiguousarray(speech[:, :ROW]), np.ascontiguousarray(noisy[:, :ROW]))
@@ -571,6 +605,12 @@ def test_refusals(api, model0, mode):
 
     nxt = np.ascontiguousarray(x[:, ROW:2 * ROW])
     (a, ga), (b, gb) = (es["slot"].process(nxt[:ACTIVE], want_gr=True) for es in (engines, twins))
+    assert np.array_equal(a, b) and np.array_equal(ga, gb) and np.abs(a).max() > 0
+    gr = np.random.RandomState(45).rand(ACTIVE, PEND, 68).astype(np.float32)
+    a, b = (es["pend"].synthesize(gr) for es in (engines, twins))
+    assert np.array_equal(a, b) and np.abs(a).max() > 0
+    after = np.ascontiguousarray(x[:ACTIVE, ROW + PEND * HOP:2 * ROW + PEND * HOP])
+    (a, ga), (b, gb) = (es["pend"].process(after, want_gr=True) for es in (engines, twins))
     assert np.array_equal(a, b) and np.array_equal(ga, gb) and np.abs(a).max() > 0
     ids = [5, 20, 9, 3]                 # three resident, one fresh
     (a, ga), (b, gb) = (es["ses"].process_sessions(ids, nxt[:4, :2 * HOP], want_gr=True) for es in (engines, twins))

@@ -286,3 +286,31 @@ def test_reset_and_refusals(api, model0, mode):
     t = api.Engine(270, 4, None, api.TRAIN_DATA)
     assert t.L.pnb_sessions_reserve(t.h, 10) == -1
     t.close()
+
+
+@pytest.mark.parametrize("mode", ["fp32", "tensor"])
+def test_session_state_launches(api, model0, mode):
+    """pnb_launch_count grows by each session operation's own launches: one for a reset, a blob check and the blob
+    rewrite for an import, and for an export one per kind of session listed (resident ones from their slots, parked
+    ones from their parking blobs); none for n = 0."""
+    import torch
+    e = _engine(api, model0, 16, mode, Fm=4)
+    e.reserve_sessions(64)
+    x = _signal(16, 1, 9)
+    e.process_sessions(np.arange(8, dtype=np.int32), np.ascontiguousarray(x[:8, :4 * HOP]))   # 0..7 resident
+    blobs = e.export_sessions([0, 1], None)
+    ops = [("export resident", lambda: e.export_sessions([2, 5, 3], None), 1),
+           ("export parked", lambda: e.export_sessions([40, 20], None), 1),
+           ("export mixed", lambda: e.export_sessions([41, 4, 21], None), 2),
+           ("reset", lambda: e.reset_sessions([6, 30]), 1),
+           ("import", lambda: e.import_sessions([7, 31], blobs), 2),
+           ("reset n 0", lambda: e.reset_sessions([]), 0),
+           ("export n 0", lambda: e.export_sessions([], None), 0),
+           ("import n 0", lambda: e.import_sessions([], 0), 0)]
+    for name, op, want in ops:
+        n = e.launches
+        op()
+        assert e.launches - n == want, name
+    torch.cuda.synchronize()
+    e.check()
+    e.close()

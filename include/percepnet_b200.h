@@ -83,7 +83,7 @@ enum {
                             refused.  State blobs: export writes the network part and zeroes the signal part, import
                             takes the network part and ignores the signal part, so blobs move both ways between this
                             engine and a PCM engine of the same network path. */
-  PNB_SIGNAL_ONLY = 128  /* the signal path alone: an engine for pnb_analyze_* / pnb_synthesize_*, with g/r from the caller.
+  PNB_SIGNAL_ONLY = 128, /* the signal path alone: an engine for pnb_analyze_* / pnb_synthesize_*, with g/r from the caller.
                             model may be NULL and is ignored; no fc weights, network state or network buffers are
                             allocated.  Every other call, pnb_train_* and pnb_sessions_reserve are refused with PNB_ERR_ARG
                             before anything is enqueued.  Not with PNB_NN_TENSOR, PNB_CONV_WIDE, PNB_TRAIN_DATA,
@@ -91,6 +91,14 @@ enum {
                             taps are refused).  State blobs: export writes the signal part and zeroes the network part,
                             import takes the signal part and ignores the network part, so blobs move both ways between
                             this engine and a PCM engine. */
+  PNB_TRAIN_NETWORK = 256 /* a PNB_NETWORK_ONLY engine that also trains its fp32 network (pnb_train_*): n_streams windows per
+                            step, max_frames_per_call the window length T.  Its parameters are the fp32 path's weight
+                            buffers, so pnb_compute_rnn_* / pnb_score_records_* on it run the weights of the last Adam step
+                            in the deployed tansig arithmetic.  PNB_NN_FP32 only: not with PNB_NN_TENSOR, PNB_CONV_WIDE,
+                            PNB_TRAIN_DATA, PNB_TRAIN_AUDIO, PNB_POSTFILTER or PNB_SIGNAL_ONLY.  Besides what a network-only
+                            engine holds it keeps the gradient and Adam's two moments (3 x 31.9 MB) and the activations one
+                            gradient call saves for its backward pass, about 72 KB per frame of n_streams x T (128 windows
+                            x 2000 hops: 18.5 GB); n_streams x T at most 65535 x 64. */
 };
 
 typedef struct pnb_engine pnb_engine;
@@ -248,6 +256,46 @@ int pnb_score_records_device(pnb_engine *e, const float *d_rec, size_t rec_strid
                              double *d_sums, float *d_gr, size_t gr_stride, void *cuda_stream);
 int pnb_score_records_host(pnb_engine *e, const float *rec, size_t rec_stride, int n_frames, const int *frames,
                            double *sums, float *gr, size_t gr_stride);
+
+/* Training (PNB_TRAIN_NETWORK engines): rnn_train.py's step -- CustomLoss (gamma = 0.5, C4 = 10) of its PercepNet on a
+ * batch of windows, the gradient of every parameter, and a torch.optim.Adam step (defaults: betas 0.9 / 0.999, eps 1e-8,
+ * no weight decay, no amsgrad) -- on the device, in fp32 FMA.  The model is PercepNet.forward (rnn_train.py:105-145) with
+ * exact tanh and sigmoid (not the tansig table of inference), torch's GRU gate formula, and every window starting from
+ * zero GRU state and zero conv history.  Nothing carries between calls; the slots' network state is not touched.
+ *   pnb_train_grad_*  rec / d_rec hold the active rows [0, n) of records as pnb_score_records_* takes them (network input
+ *                     {30 rec[0..67], rec[68], rec[69]}), one window per row, rec_stride >= n_frames * 138.  frames: host
+ *                     array of n ints in [1, n_frames] (window i ends after frames[i] hops), or NULL for n_frames each;
+ *                     the hops past a window's end contribute nothing to the loss or the gradient, whatever they hold
+ *                     (NaN included).  sums / d_sums: n x 4 float64 as pnb_score_records_* writes them, for the trainer's
+ *                     exact-activation predictions.  The gradient of the loss -- the mean over the counted hops x 34 bands
+ *                     of all windows -- overwrites the engine's gradient buffer.  It is computed at the output
+ *                     pre-activations in closed form, g: -dg (1 + 2 C4 dg^2) sqrt(p) (1 - p), r: dr p sqrt(1 - p); this
+ *                     equals torch's autograd wherever that is finite, and is its finite limit where a sigmoid output
+ *                     rounds to exactly 0 or 1 in fp32, where torch's autograd returns NaN (rnn_train.py:198's "CustomLoss
+ *                     cause Nan error").  That is the one deliberate difference from torch.  A gradient with a non-finite
+ *                     value (from non-finite records inside a window or non-finite weights) raises the domain bit: the next
+ *                     synchronising entry point returns PNB_ERR_DOMAIN, sticky until pnb_reset.  No floating-point atomics:
+ *                     the loss and the gradient of a call are the same bits from run to run, on any stream, host or device
+ *                     entry.  Ordering, blocking and the refusals are those of pnb_score_records_* (frames in [1, n_frames]);
+ *                     also refused on any engine without PNB_TRAIN_NETWORK.  A call issues pnb_launches_per_call(e, .)
+ *                     launches, whatever n_frames.
+ *   pnb_train_adam    one Adam step with the held gradient, lr >= 0 and finite, step >= 1 the step number (torch's
+ *                     state['step'], for the bias corrections), asynchronous on cuda_stream and ordered like a call.  When
+ *                     the last gradient call flagged a non-finite value the step is skipped on the device: weights and
+ *                     moments stay as they are, with no host synchronisation.  The arithmetic is torch's single-tensor
+ *                     CPU step: m = lerp(m, g, 0.1) (fused), v = fma(0.001 g, g, 0.999 v), p += (-lr / bc1) m / (sqrt(v) /
+ *                     sqrt(bc2) + eps).  pnb_reset touches neither weights nor moments.
+ *   pnb_train_export / pnb_train_import  one array as a flat float32 vector in PNBW blob order (the ten layers in
+ *                     RNNModel order, each layer's weights, recurrent weights, bias; 7 962 564 floats): the weights, the
+ *                     gradient (export only) or Adam's m or v.  Both wait for the engine's earlier work and return when
+ *                     the copy is complete; export needs bytes >= the vector, import exactly the vector. */
+enum { PNB_TRAIN_WEIGHTS = 0, PNB_TRAIN_GRADIENT = 1, PNB_TRAIN_ADAM_M = 2, PNB_TRAIN_ADAM_V = 3 };
+int pnb_train_grad_host(pnb_engine *e, const float *rec, size_t rec_stride, int n_frames, const int *frames, double *sums);
+int pnb_train_grad_device(pnb_engine *e, const float *d_rec, size_t rec_stride, int n_frames, const int *frames,
+                          double *d_sums, void *cuda_stream);
+int pnb_train_adam(pnb_engine *e, double lr, long long step, void *cuda_stream);
+int pnb_train_export(pnb_engine *e, int what, void *dst, size_t bytes);
+int pnb_train_import(pnb_engine *e, int what, const void *src, size_t bytes);
 
 /* The signal path without the network: pnb_process_* cut where the network sits, so the g/r between analysis and
  * synthesis come from the caller -- another engine's pnb_compute_rnn_*, a torch model, a records file's ideal gains,
@@ -454,7 +502,8 @@ long long pnb_launch_count(const pnb_engine *e);
  * streams' history back to the start of their rows, at most every call, typically every eighth; one more on a ragged
  * session call in which some session runs fewer than n_frames = max(hops) hops).  On a PNB_TRAIN_AUDIO engine it is the
  * value of a PNB_TRAIN_DATA engine of the same shape plus one: the resynthesis launch.  On a PNB_NETWORK_ONLY engine it
- * is the launch count of one pnb_compute_rnn_* call of n_frames hops; on a PNB_SIGNAL_ONLY engine that of one
+ * is the launch count of one pnb_compute_rnn_* call of n_frames hops (PNB_TRAIN_NETWORK: of one pnb_train_grad_* call,
+ * the same for every n_frames); on a PNB_SIGNAL_ONLY engine that of one
  * pnb_analyze_* and one pnb_synthesize_* call of n_frames hops (five, without the history move). */
 int pnb_launches_per_call(const pnb_engine *e, int n_frames);
 /* Bytes of the engine's device buffers whose size pnb_create fixes (weights, network buffers, stream state, per-call

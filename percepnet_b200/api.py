@@ -20,6 +20,8 @@ LIB_PATH = os.path.join(HERE, "libpercepnet_b200.so")
 FRAME = 480
 NN_FP32, NN_TENSOR, POSTFILTER, KEEP_TAPS, TRAIN_DATA, CONV_WIDE, TRAIN_AUDIO, NETWORK_ONLY = 0, 1, 2, 4, 8, 16, 32, 64
 SIGNAL_ONLY = 128
+TRAIN_NETWORK = 256
+TRAIN_ARRAYS = {"weights": 0, "gradient": 1, "m": 2, "v": 3}   # pnb_train_export / pnb_train_import
 RECORD = 138
 RNN_FEATURES, RNN_RECORDS = 0, 1   # pnb_compute_rnn_* formats: 70 features or 138 record floats per hop
 TAPS = {"features": (0, np.float32, 70), "pitch": (1, np.int32, 4), "pitchf": (2, np.float32, 2),
@@ -72,6 +74,11 @@ def load_library() -> C.CDLL:
         getattr(L, name).argtypes = [vp, vp, sz, i, vp, sz]
     for name in ("pnb_analyze_device_f32", "pnb_analyze_device_i16", "pnb_synthesize_device_f32", "pnb_synthesize_device_i16"):
         getattr(L, name).argtypes = [vp, vp, sz, i, vp, sz, vp]
+    L.pnb_train_grad_host.argtypes = [vp, vp, sz, i, vp, vp]
+    L.pnb_train_grad_device.argtypes = [vp, vp, sz, i, vp, vp, vp]
+    L.pnb_train_adam.argtypes = [vp, C.c_double, C.c_longlong, vp]
+    L.pnb_train_export.argtypes = [vp, i, vp, sz]
+    L.pnb_train_import.argtypes = [vp, i, vp, sz]
     L.pnb_engine_bytes.argtypes = [vp]
     L.pnb_engine_bytes.restype = sz
     L.pnb_flush.argtypes = [vp, vp]
@@ -122,6 +129,7 @@ EXPORTS = ("pnb_create", "pnb_destroy", "pnb_reset", "pnb_resolve_device", "pnb_
            "pnb_compute_rnn_device", "pnb_compute_rnn_host", "pnb_score_records_device", "pnb_score_records_host",
            "pnb_analyze_host_f32", "pnb_analyze_host_i16", "pnb_analyze_device_f32", "pnb_analyze_device_i16",
            "pnb_synthesize_host_f32", "pnb_synthesize_host_i16", "pnb_synthesize_device_f32", "pnb_synthesize_device_i16",
+           "pnb_train_grad_host", "pnb_train_grad_device", "pnb_train_adam", "pnb_train_export", "pnb_train_import",
            "pnb_engine_bytes",
            "pnb_read_tap", "pnb_state_size", "pnb_get_state", "pnb_set_state",
            "pnb_reset_streams", "pnb_export_states", "pnb_import_states", "pnb_set_active_streams", "pnb_active_streams",
@@ -310,6 +318,52 @@ class Engine:
         self._ck(self.L.pnb_score_records_device(self.h, d_rec or None, rec_stride, n_frames,
                                                  None if fr is None else fr.ctypes.data, d_sums or None, d_gr or None,
                                                  gr_stride, stream or None), "pnb_score_records_device")
+
+    # ---- training (TRAIN_NETWORK engines; see pnb_train_grad_host in the header) -----------------------------------
+    def train_grad(self, rec: np.ndarray, frames=None) -> np.ndarray:
+        """pnb_train_grad_host: rnn_train.py's CustomLoss on the windows rec ([active, F, 138] float32 records, one window
+        per row) and its gradient with respect to every parameter, kept on the engine for train_adam.  frames: None, or
+        one count in [1, F] per window (its hops after that are ignored).  Returns the loss sums [active, 4] float64 as
+        score_records returns them (eval_records.loss_terms of their sum gives the loss)."""
+        n = self.active
+        if rec.dtype != np.float32:
+            raise TypeError("rec must be float32")
+        assert rec.ndim == 3 and rec.shape[0] == n and rec.shape[2] == RECORD, "rec must be [active, F, 138]"
+        F = rec.shape[1]
+        rec = np.ascontiguousarray(rec)
+        fr = None if frames is None else self._slots(frames)[0]
+        if fr is not None and len(fr) != n:
+            raise PnbError("train_grad: frames needs one entry per active row")
+        sums = np.empty((n, 4), np.float64)
+        self._ck(self.L.pnb_train_grad_host(self.h, rec.ctypes.data, F * RECORD, F, None if fr is None else fr.ctypes.data,
+                                            sums.ctypes.data), "pnb_train_grad_host")
+        return sums
+
+    def train_grad_device(self, d_rec: int, rec_stride: int, n_frames: int, frames, d_sums: int, stream: int = 0):
+        """pnb_train_grad_device on raw device pointers (rec_stride in floats); frames: None or a host sequence of one
+        count per active row; d_sums: [active, 4] float64."""
+        fr = None if frames is None else self._slots(frames)[0]
+        self._ck(self.L.pnb_train_grad_device(self.h, d_rec or None, rec_stride, n_frames,
+                                              None if fr is None else fr.ctypes.data, d_sums or None, stream or None),
+                 "pnb_train_grad_device")
+
+    def train_adam(self, lr: float, step: int, stream: int = 0):
+        """pnb_train_adam: one torch.optim.Adam step (defaults) with the gradient of the last train_grad; step counts
+        from 1.  Skipped on the device when that gradient was not finite."""
+        self._ck(self.L.pnb_train_adam(self.h, float(lr), int(step), stream or None), "pnb_train_adam")
+
+    def train_export(self, what: str) -> np.ndarray:
+        """pnb_train_export: 'weights', 'gradient', 'm' or 'v' as one float32 vector in PNBW blob order
+        (weights.PackedModel.from_flat turns it into a model)."""
+        from .weights import N_PARAMS
+        a = np.empty(N_PARAMS, np.float32)
+        self._ck(self.L.pnb_train_export(self.h, TRAIN_ARRAYS[what], a.ctypes.data, a.nbytes), "pnb_train_export")
+        return a
+
+    def train_import(self, what: str, a: np.ndarray):
+        """pnb_train_import: 'weights', 'm' or 'v' from a flat float32 vector in PNBW blob order (resuming a run)."""
+        a = np.ascontiguousarray(a, np.float32)
+        self._ck(self.L.pnb_train_import(self.h, TRAIN_ARRAYS[what], a.ctypes.data, a.nbytes), "pnb_train_import")
 
     def analyze(self, x: np.ndarray) -> np.ndarray:
         """pnb_analyze_host_*: the analysis half of process.  x: [active, F*480] float32 (C-API scale) or int16 (CLI wire

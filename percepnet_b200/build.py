@@ -26,6 +26,7 @@ SOURCES = {
     "pnb_engine.cu": [],
     "pnb_state.cu": [],
     "pnb_rnn_io.cu": [],
+    "pnb_train.cu": [],
 }
 
 

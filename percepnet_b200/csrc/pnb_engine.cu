@@ -154,6 +154,10 @@ extern "C" int pnb_create(pnb_engine **out, int n_streams, int max_frames, const
   if (n_streams < 1 || max_frames < 1) return fail(PNB_ERR_ARG, "n_streams and max_frames_per_call must be >= 1");
   if ((long long)n_streams * max_frames > (1ll << 24))
     return fail(PNB_ERR_ARG, "n_streams x max_frames_per_call above 2^24 rows per call: split the batch across engines");
+  if ((flags & PNB_TRAIN_NETWORK) &&
+      (flags & (PNB_NN_TENSOR | PNB_CONV_WIDE | PNB_TRAIN_DATA | PNB_TRAIN_AUDIO | PNB_POSTFILTER | PNB_SIGNAL_ONLY)))
+    return fail(PNB_ERR_ARG, "PNB_TRAIN_NETWORK trains the fp32 network alone: combine it only with PNB_NETWORK_ONLY and PNB_KEEP_TAPS");
+  if (flags & PNB_TRAIN_NETWORK) flags |= PNB_NETWORK_ONLY;  // a training engine is a network-only engine that also trains
   const bool train_mode = (flags & PNB_TRAIN_DATA) != 0, train_audio = (flags & PNB_TRAIN_AUDIO) != 0;
   if (train_audio && !train_mode) return fail(PNB_ERR_ARG, "PNB_TRAIN_AUDIO applies to PNB_TRAIN_DATA engines");
   if (train_mode && (n_streams & 1)) return fail(PNB_ERR_ARG, "PNB_TRAIN_DATA needs n_streams = 2 x pairs");
@@ -259,7 +263,8 @@ extern "C" int pnb_create(pnb_engine **out, int n_streams, int max_frames, const
   }
   if (has_net) {  // a signal-only engine has no network: no weights, network state or network buffers
     CKD(engine_alloc(e, &e->c2, S * 512, kStreamState));
-    const int rc = (flags & PNB_NN_TENSOR) ? tc_prepare(e, model) : f32_prepare(e, model);
+    int rc = (flags & PNB_NN_TENSOR) ? tc_prepare(e, model) : f32_prepare(e, model);
+    if (!rc && (flags & PNB_TRAIN_NETWORK)) rc = train_prepare(e);
     if (rc) { pnb_destroy(e); return rc; }
   }
   CKD(cudaDeviceSynchronize());
@@ -612,7 +617,7 @@ static Rows pcm(const T *p, size_t stride) { return rows(p, stride, kFrame, size
 // network call; records / g/r (when asked for) and the loss sums of a score call; PCM / features of an analysis; g/r /
 // PCM of a synthesis.
 struct Call {
-  enum Kind { kSlots, kSessions, kRagged, kNetwork, kRecords, kAnalyze, kSynthesize } kind;
+  enum Kind { kSlots, kSessions, kRagged, kNetwork, kRecords, kAnalyze, kSynthesize, kTrain } kind;
   Rows in[2], out[2];
   int F;           // hops; a ragged call's is max(hops), set by check_call
   float *gr;       // enhancement calls: g/r destination [F][rows][68], or null
@@ -620,7 +625,7 @@ struct Call {
   int n_ids;
   const int *hops;    // ragged calls: each listed session's hops (host); null once check_call finds them all equal to F
   int format;         // network calls: PNB_RNN_FEATURES or PNB_RNN_RECORDS
-  const int *frames;  // score calls: the hops each row's loss counts (host), or null for F
+  const int *frames;  // score and gradient calls: the hops each row's loss counts (host), or null for F
   bool status = true;  // a blocking host call reads back and reports the status word (rejected imports, PNB_ERR_DOMAIN)
 };
 
@@ -792,6 +797,18 @@ static int enqueue_synthesize(pnb_engine *e, const Call &c, cudaStream_t st) {
   return rc;
 }
 
+// A gradient call on st (arguments already checked): the trainer's forward, loss and backward on the records of windows
+// [0, n_active), each from zero state; the loss sums to the caller, the gradient into the engine's buffer.  Neither the
+// network state of the slots nor the signal state is touched.
+static int enqueue_train(pnb_engine *e, const Call &c, cudaStream_t st) {
+  return enqueue_call(e, c.F, st, [&]() -> int {
+    const int *frames = nullptr;
+    if (c.frames) { int rc = stage_ints(e, c.frames, (size_t)e->n_active, st, &frames); if (rc) return rc; }
+    return train_grad(e, static_cast<const float *>(c.in[0].p), c.in[0].stride, frames, c.frames,
+                      static_cast<double *>(c.out[1].p), c.F, st);
+  }, false);
+}
+
 // The call's enqueue body (arguments already checked).
 static int enqueue(pnb_engine *e, const Call &c, cudaStream_t st) {
   switch (c.kind) {
@@ -799,6 +816,7 @@ static int enqueue(pnb_engine *e, const Call &c, cudaStream_t st) {
     case Call::kRecords: return enqueue_records(e, c, st);
     case Call::kAnalyze: return enqueue_analyze(e, c, st);
     case Call::kSynthesize: return enqueue_synthesize(e, c, st);
+    case Call::kTrain: return enqueue_train(e, c, st);
     default: return enqueue_enhance(e, c, st);
   }
 }
@@ -872,13 +890,14 @@ static int check_call(pnb_engine *e, Call &c) {
     for (int i = 0; i < c.n_ids; i++) uniform = uniform && c.hops[i] == c.F;
     if (uniform) c.hops = nullptr;
   }
-  const bool train = c.kind == Call::kRecords, network = c.kind == Call::kNetwork;
+  const bool train = c.kind == Call::kRecords, network = c.kind == Call::kNetwork || c.kind == Call::kTrain;
   const bool split = c.kind == Call::kAnalyze || c.kind == Call::kSynthesize;
   if (!e) return fail(PNB_ERR_ARG, "engine is NULL");
   if (!network && (e->flags & PNB_NETWORK_ONLY))
     return fail(PNB_ERR_ARG, "engine was created with PNB_NETWORK_ONLY: use pnb_compute_rnn_* / pnb_score_records_*");
   if (!split && (e->flags & PNB_SIGNAL_ONLY))
     return fail(PNB_ERR_ARG, "engine was created with PNB_SIGNAL_ONLY: use pnb_analyze_* / pnb_synthesize_*");
+  if (c.kind == Call::kTrain && !(e->flags & PNB_TRAIN_NETWORK)) return fail(PNB_ERR_ARG, "engine was not created with PNB_TRAIN_NETWORK");
   if (train && !(e->flags & PNB_TRAIN_DATA)) return fail(PNB_ERR_ARG, "engine was not created with PNB_TRAIN_DATA");
   if (!train && (e->flags & PNB_TRAIN_DATA))
     return fail(PNB_ERR_ARG, "engine was created with PNB_TRAIN_DATA: use pnb_train_records_* / pnb_submit_train_records");
@@ -900,12 +919,14 @@ static int check_call(pnb_engine *e, Call &c) {
     return refuse_pending(e);
   }
   if (c.kind == Call::kSessions) return check_ids(e, c.ids, c.n_ids, e->S);
-  if (network && c.format != PNB_RNN_FEATURES && c.format != PNB_RNN_RECORDS)
+  if (c.kind == Call::kNetwork && c.format != PNB_RNN_FEATURES && c.format != PNB_RNN_RECORDS)
     return fail(PNB_ERR_ARG, "format %d is neither PNB_RNN_FEATURES (0) nor PNB_RNN_RECORDS (1)", c.format);
   if ((c.kind == Call::kSlots || network || split) && e->sessions) return refuse_in_session_mode();
-  if (c.frames)  // every row's counted hops in [0, F]
+  const int fr_lo = c.kind == Call::kTrain ? 1 : 0;  // a window of a gradient call has at least one hop
+  if (c.frames)  // every row's counted hops in [fr_lo, F]
     for (int i = 0; i < e->n_active; i++)
-      if (c.frames[i] < 0 || c.frames[i] > c.F) return fail(PNB_ERR_ARG, "frames[%d] = %d outside [0, %d]", i, c.frames[i], c.F);
+      if (c.frames[i] < fr_lo || c.frames[i] > c.F)
+        return fail(PNB_ERR_ARG, "frames[%d] = %d outside [%d, %d]", i, c.frames[i], fr_lo, c.F);
   return PNB_OK;
 }
 
@@ -1039,6 +1060,9 @@ static int report_status(pnb_engine *e) {
     return fail(PNB_ERR_ARG, "pnb_import_states rejected a blob (bad magic / version, or a GRU state outside [-1, 1] for a "
                              "tensor-mode engine); lowest rejected stream %d, left reset like every rejected one", slot);
   }
+  if ((e->h_status[0] & 1) && (e->flags & PNB_TRAIN_NETWORK))
+    return fail(PNB_ERR_DOMAIN, "a pnb_train_grad_* call met a non-finite gradient (non-finite records inside a window, or "
+                                "non-finite weights); the Adam step after it was skipped.  Sticky until pnb_reset");
   if (e->h_status[0] & 1)
     return fail(PNB_ERR_DOMAIN, "tensor path: a pre-activation left the domain of the reference's tansig_approx (|x| >= 8.5e7, "
                                 "src/vec.h:63 is undefined there); results since the last pnb_reset are not the reference's -- "
@@ -1172,6 +1196,63 @@ extern "C" int pnb_score_records_device(pnb_engine *e, const float *d_rec, size_
 extern "C" int pnb_score_records_host(pnb_engine *e, const float *rec, size_t rec_stride, int n_frames, const int *frames,
                                       double *sums, float *gr, size_t gr_stride) {
   return host_call(e, score_call(rec, rec_stride, n_frames, frames, sums, gr, gr_stride), false);
+}
+
+// A gradient call (PNB_TRAIN_NETWORK): records in, the loss sums out, the gradient kept on the engine.
+static Call train_call(const float *rec, size_t rec_stride, int n_frames, const int *frames, double *sums) {
+  Call c{Call::kTrain, {rows(rec, rec_stride, PNB_RECORD_FLOATS, sizeof(float))}, {}, n_frames};
+  c.out[1] = rows(sums, 4, 4, sizeof(double), "row stride", true);
+  c.frames = frames;
+  return c;
+}
+extern "C" int pnb_train_grad_device(pnb_engine *e, const float *d_rec, size_t rec_stride, int n_frames, const int *frames,
+                                     double *d_sums, void *cuda_stream) {
+  return device_call(e, train_call(d_rec, rec_stride, n_frames, frames, d_sums), (cudaStream_t)cuda_stream);
+}
+extern "C" int pnb_train_grad_host(pnb_engine *e, const float *rec, size_t rec_stride, int n_frames, const int *frames,
+                                   double *sums) {
+  return host_call(e, train_call(rec, rec_stride, n_frames, frames, sums), false);
+}
+
+// The refusals every training entry point shares: an engine of its kind that no failed call has poisoned.
+static int check_trainer(pnb_engine *e) {
+  if (!e) return fail(PNB_ERR_ARG, "engine is NULL");
+  if (!(e->flags & PNB_TRAIN_NETWORK)) return fail(PNB_ERR_ARG, "engine was not created with PNB_TRAIN_NETWORK");
+  if (e->poisoned) return refuse_poisoned(PNB_ERR_CUDA);
+  return PNB_OK;
+}
+
+extern "C" int pnb_train_adam(pnb_engine *e, double lr, long long step, void *cuda_stream) {
+  { int rc = check_trainer(e); if (rc) return rc; }
+  if (!(lr >= 0.0) || !isfinite(lr)) return fail(PNB_ERR_ARG, "lr = %g is not a finite number >= 0", lr);
+  if (step < 1) return fail(PNB_ERR_ARG, "step = %lld, Adam counts steps from 1", step);
+  CK(cudaSetDevice(e->device));
+  const int n = enqueue_ordered(e, (cudaStream_t)cuda_stream, [&] { return train_adam(e, lr, step, (cudaStream_t)cuda_stream); });
+  return n < 0 ? n : PNB_OK;
+}
+
+// Export / import of the trainer's arrays as one flat float32 vector in PNBW blob order; both wait for the engine's
+// earlier work and finish before they return.
+static int train_transfer(pnb_engine *e, int what, void *host, size_t bytes, bool to_host) {
+  { int rc = check_trainer(e); if (rc) return rc; }
+  if (!host) return fail(PNB_ERR_ARG, "%s is NULL", to_host ? "dst" : "src");
+  if (what < PNB_TRAIN_WEIGHTS || what > PNB_TRAIN_ADAM_V) return fail(PNB_ERR_ARG, "what = %d is not a PNB_TRAIN_* array", what);
+  if (!to_host && what == PNB_TRAIN_GRADIENT) return fail(PNB_ERR_ARG, "the gradient is computed, not imported");
+  const size_t need = train_params(e) * sizeof(float);
+  if (to_host ? bytes < need : bytes != need)
+    return fail(PNB_ERR_ARG, "%zu bytes, the model has %zu parameters (%zu bytes)", bytes, train_params(e), need);
+  CK(cudaSetDevice(e->device));
+  const int n = enqueue_ordered(e, e->stream, [&] {
+    const int rc = train_copy(e, what, host, to_host, e->stream);
+    return rc ? rc : 0;
+  });
+  if (n < 0) return n;
+  CK(cudaStreamSynchronize(e->stream));
+  return PNB_OK;
+}
+extern "C" int pnb_train_export(pnb_engine *e, int what, void *dst, size_t bytes) { return train_transfer(e, what, dst, bytes, true); }
+extern "C" int pnb_train_import(pnb_engine *e, int what, const void *src, size_t bytes) {
+  return train_transfer(e, what, const_cast<void *>(src), bytes, false);
 }
 
 // The split call: the analysis half of a slot call (PCM rows in, the network input out) and its synthesis half (the
@@ -1647,6 +1728,7 @@ extern "C" int pnb_launches_per_call(const pnb_engine *e, int n_frames) {
   // call is pnb_compute_rnn_*: rows_stage, the network, rows_store; a PNB_SIGNAL_ONLY engine's is one pnb_analyze_*
   // (stage_in, analysis, rows_store) and one pnb_synthesize_* (rows_stage, synthesis)
   if (e->flags & PNB_SIGNAL_ONLY) return 5;
+  if (e->flags & PNB_TRAIN_NETWORK) return train_grad_launches(e);  // one pnb_train_grad_* call, whatever n_frames
   const int net = (e->flags & PNB_NN_TENSOR) ? tc_network_launches(e, n_frames) : f32_network_launches(e, n_frames);
   if (e->flags & PNB_NETWORK_ONLY) return 2 + net;
   return 3 + net + ((e->flags & PNB_TRAIN_AUDIO) ? 1 : 0);

@@ -11,6 +11,7 @@
 
 struct pnb_tc_state;   // tensor-core path (pnb_nn_tc.cu)
 struct pnb_f32_state;  // fp32 FMA path (pnb_nn_f32.cu)
+struct pnb_train_state;  // PNB_TRAIN_NETWORK: gradients, Adam's moments, saved activations (pnb_train.cu)
 
 constexpr int kGruH[5] = {512, 512, 512, 512, 128};  // hidden sizes of gru1..3, gru_gb, gru_rb (check_model)
 
@@ -75,6 +76,7 @@ struct pnb_engine {
   // where the type is complete
   std::shared_ptr<pnb_tc_state> tc;
   std::shared_ptr<pnb_f32_state> f32;
+  std::shared_ptr<pnb_train_state> train;
   int last_frames = 0;
   // hops of an analysis (pnb_analyze_*) whose synthesis (pnb_synthesize_*) is still due, or 0.  Between the two halves
   // the analysed streams are mid-hop, so every call and state operation but the synthesis and network calls is refused.
@@ -159,6 +161,19 @@ int f32_network_launches(const pnb_engine *e, int F);
 // the path's pieces of a stream's state (state_segs, pnb_state.cu): appended to seg[ns..]; returns the new count
 int tc_state_segs(const pnb_engine *e, pnb::StateSeg *seg, int ns);
 int f32_state_segs(const pnb_engine *e, pnb::StateSeg *seg, int ns);
+
+// PNB_TRAIN_NETWORK (pnb_train.cu).  prepare: after f32_prepare, the trainer's buffers.  grad: the loss sums and the
+// gradient of a call of F hops on windows [0, n_active) (records on the device; frames: device / host copies of the
+// hops per window, or null), returns its launch count.  adam: one step with the held gradient.  copy: what = 0 weights,
+// 1 gradient, 2 m, 3 v between the device and train_params(e) floats of host memory, on st.
+int f32_params(const pnb_engine *e, float **p, size_t *count);
+int train_prepare(pnb_engine *e);
+int train_grad(pnb_engine *e, const float *rec, size_t rec_stride, const int *frames, const int *h_frames, double *sums,
+               int F, cudaStream_t st);
+int train_grad_launches(const pnb_engine *e);
+int train_adam(pnb_engine *e, double lr, long long step, cudaStream_t st);
+int train_copy(pnb_engine *e, int what, void *host, bool to_host, cudaStream_t st);
+size_t train_params(const pnb_engine *e);
 
 // RAII marker used by the launch schedule: records an event pair around a launch when profiling
 struct ProfScope {

@@ -603,3 +603,21 @@ int f32_state_segs(const pnb_engine *e, StateSeg *seg, int ns) {
   add_words(seg, ns, kSegBlobZero, nullptr, 0, offsetof(StreamState, fc_terms), (sizeof(StreamState) - offsetof(StreamState, fc_terms)) / 4);
   return ns;
 }
+
+// The path's weights as the PNBW blob orders them (RNNModel layer order; per layer weights, recurrent weights, bias):
+// the 25 device arrays and their float counts.  A PNB_TRAIN_NETWORK engine trains these in place.
+int f32_params(const pnb_engine *e, float **p, size_t *count) {
+  const pnb_f32_state &f = *e->f32;
+  int k = 0;
+  auto put = [&](float *a, size_t n) { p[k] = a; count[k] = n; k++; };
+  put(e->fc.W, 70 * 128); put(e->fc.b, 128);
+  put(f.conv1.W, 5 * 128 * 512); put(f.conv1.b, 512);
+  put(f.conv2.W, 3 * 512 * 512); put(f.conv2.b, 512);
+  for (int i = 0; i < 5; i++) {
+    const size_t H = kGruH[i], M = i == 4 ? 1024 : 512;
+    put(f.gru[i].W, M * 3 * H); put(f.gru[i].U, H * 3 * H); put(f.gru[i].b, 6 * H);
+  }
+  put(f.fc_gb.W, 2560 * 34); put(f.fc_gb.b, 34);
+  put(f.fc_rb.W, 128 * 34); put(f.fc_rb.b, 34);
+  return PNB_OK;
+}

@@ -196,6 +196,41 @@ class PackedModel:
     def n_params(self) -> int:
         return int(sum(v.size for v in self.arrays.values()))
 
+    @staticmethod
+    def blob_keys() -> list[str]:
+        """The array names in PNBW blob order: layers in RNNModel order, each weights, recurrent weights, bias."""
+        keys = []
+        for spec in LAYERS:
+            name = spec[0]
+            keys += [name + "_weights"] + ([name + "_recurrent_weights"] if spec[1] == "gru" else []) + [name + "_bias"]
+        return keys
+
+    def flat(self) -> np.ndarray:
+        """All arrays as one float32 vector in blob order (what pnb_train_export / pnb_train_import move)."""
+        return np.concatenate([np.asarray(self.arrays[k], np.float32).reshape(-1) for k in self.blob_keys()])
+
+    @classmethod
+    def from_flat(cls, v: np.ndarray) -> "PackedModel":
+        """The inverse of flat(): a model from a blob-order vector of N_PARAMS floats."""
+        v = np.asarray(v, np.float32).reshape(-1)
+        if v.size != N_PARAMS:
+            raise ValueError(f"{v.size} floats, a PercepNet model has {N_PARAMS}")
+        out, at = {}, 0
+        for spec in LAYERS:
+            name, kind = spec[0], spec[1]
+            if kind == "dense":
+                shapes = [(spec[2], spec[3]), (spec[3],)]
+            elif kind == "conv":
+                shapes = [(spec[3], spec[2], spec[4]), (spec[4],)]
+            else:
+                shapes = [(spec[2], 3 * spec[3]), (spec[3], 3 * spec[3]), (6 * spec[3],)]
+            keys = [name + "_weights"] + ([name + "_recurrent_weights"] if kind == "gru" else []) + [name + "_bias"]
+            for k, shp in zip(keys, shapes):
+                n = int(np.prod(shp))
+                out[k] = v[at:at + n].reshape(shp).copy()
+                at += n
+        return cls(out)
+
 
 def pack_state_dict(sd: dict[str, np.ndarray]) -> PackedModel:
     out: dict[str, np.ndarray] = {}
@@ -214,6 +249,34 @@ def pack_state_dict(sd: dict[str, np.ndarray]) -> PackedModel:
             out[name + "_bias"] = _gru_bias(np.asarray(sd[f"{name}.bias_ih_l0"], np.float32),
                                             np.asarray(sd[f"{name}.bias_hh_l0"], np.float32))
     return PackedModel(out)
+
+
+def _gru_unkernel(w: np.ndarray) -> np.ndarray:
+    """The inverse of _gru_kernel: [M, 3H] with gate columns (z, r, n) -> torch [3H, M] with gate rows (r, z, n)."""
+    z, r, n = np.hsplit(np.asarray(w, np.float32), 3)
+    return np.ascontiguousarray(np.vstack([r.T, z.T, n.T]), dtype=np.float32)
+
+
+def unpack_state_dict(pm: PackedModel) -> dict[str, np.ndarray]:
+    """The inverse of pack_state_dict: nnet_data.cpp layout back to rnn_train.PercepNet's state_dict names and shapes
+    (float32 numpy arrays; torch.from_numpy of each is what dump_percepnet.py reads).  Every transform is a permutation,
+    so unpack_state_dict(pack_state_dict(sd)) equals sd bit for bit."""
+    a, sd = pm.arrays, {}
+    for spec in LAYERS:
+        name, kind = spec[0], spec[1]
+        if kind == "dense":
+            sd[f"{name}.0.weight"] = np.ascontiguousarray(np.asarray(a[name + "_weights"], np.float32).T)
+            sd[f"{name}.0.bias"] = np.ascontiguousarray(a[name + "_bias"], dtype=np.float32)
+        elif kind == "conv":
+            sd[f"{name}.0.weight"] = np.ascontiguousarray(np.transpose(np.asarray(a[name + "_weights"], np.float32), (2, 1, 0)))
+            sd[f"{name}.0.bias"] = np.ascontiguousarray(a[name + "_bias"], dtype=np.float32)
+        else:
+            sd[f"{name}.weight_ih_l0"] = _gru_unkernel(a[name + "_weights"])
+            sd[f"{name}.weight_hh_l0"] = _gru_unkernel(a[name + "_recurrent_weights"])
+            b = np.asarray(a[name + "_bias"], np.float32).reshape(2, 3, -1)[:, [1, 0, 2], :]
+            sd[f"{name}.bias_ih_l0"] = np.ascontiguousarray(b[0].reshape(-1))
+            sd[f"{name}.bias_hh_l0"] = np.ascontiguousarray(b[1].reshape(-1))
+    return sd
 
 
 def synth_model(seed: int = 0, gain: float = 1.0) -> PackedModel:

@@ -449,6 +449,64 @@ int pnb_export_sessions(pnb_engine *e, const int *ids, int n, void *d_blobs, siz
 int pnb_import_sessions(pnb_engine *e, const int *ids, int n, const void *d_blobs, size_t blob_stride, void *cuda_stream);
 int pnb_session_stats(const pnb_engine *e, long long *out);
 
+/* Split and network calls on a session pool: pnb_analyze_* / pnb_synthesize_* and pnb_compute_rnn_* on a list of
+ * sessions, so a host can put its own g/r (a torch model, a second engine, a per-session policy) between the halves of
+ * a pooled engine, with parked sessions and ragged hop counts as pnb_process_sessions_* / _ragged_* have them.
+ *   ids          host array of n distinct session ids, 1 <= n <= n_streams; row i of every array belongs to ids[i]
+ *   hops         NULL: every listed session runs n_frames hops.  Else the call is ragged: 1 <= hops[i] <= max_frames,
+ *                n_frames must equal max(hops) (strides are checked against it), and each session ends in the state of
+ *                its own hops[i] hops, as in pnb_process_sessions_ragged_*
+ *   in / d_in    PCM rows as pnb_process_sessions_* takes them; row i is read for its first hops[i]*480 samples only
+ *   feat / d_feat row i: n_frames x 70 floats; hop t is bit for bit PNB_TAP_FEATURES[t] of the session's slot in the
+ *                pnb_process_sessions_* call on the same input, for t < hops[i], and zero after
+ *   gr / d_gr    row i: n_frames x 68 floats (34 g then 34 r per hop); the synthesis reads t < hops[i] only, the network
+ *                call writes zeros for t >= hops[i]
+ *   out / d_out  PCM rows as a ragged call writes them: hops[i] hops of output, then zeros up to n_frames*480
+ * pnb_analyze_sessions_* applies the residency plan exactly as a session call does (the same parks, unparks and
+ *   relocations, counted by pnb_session_stats), analyses the listed sessions and leaves a synthesis pending that records
+ *   the list, the hops and n_frames.
+ * pnb_synthesize_sessions_* must pass the pending list: the same n, the same ids in the same order, the same n_frames
+ *   (the hops are the analysis's).  It completes the hops with the caller's g/r (post-filtered on a PNB_POSTFILTER
+ *   engine), moves the state of sessions that ran fewer hops to the call's end and commits the hops.  With the
+ *   network's g/r in between, the pair is pnb_process_sessions_* (or _ragged_*) bit for bit: output, state and blobs.
+ * pnb_compute_rnn_sessions_*: pnb_compute_rnn_* on the listed sessions (format PNB_RNN_FEATURES or PNB_RNN_RECORDS).
+ *   With no split pending it plans residency like any session call and advances the sessions' network state only: the
+ *   signal state and the hop counter stay where they are.  With a session split pending it must pass the pending list,
+ *   hops and n_frames, and nothing moves.
+ * The three run on PCM engines in session mode (fp32 or tensor, PNB_CONV_WIDE and PNB_POSTFILTER included).  While a
+ * session split is pending, pnb_process_sessions_* (plain and ragged), another pnb_analyze_sessions_*,
+ * pnb_reset_sessions, pnb_export_sessions, pnb_import_sessions, pnb_sessions_reserve and a pnb_compute_rnn_sessions_*
+ * with another list, hops or n_frames return PNB_ERR_ARG before anything is enqueued; pnb_reset cancels the pending
+ * synthesis and keeps session mode.  Also refused with PNB_ERR_ARG before anything changes: an engine not in session
+ * mode, a synthesis with nothing pending, NULL pointers, ids out of range or listed twice, hops out of range,
+ * n_frames != max(hops), short strides.  Ordering, blocking, poisoning and PNB_ERR_DOMAIN are those of the slot forms;
+ * the slot forms stay refused in session mode.  Host forms block and take no stream.
+ * Launches:  pnb_analyze_sessions_*     [move] + stage-in + analysis + feature store
+ *            pnb_synthesize_sessions_*  g/r stage + synthesis + [fix-up] + [history move]
+ *            pnb_compute_rnn_sessions_* [move] + stage + the network's launches + g/r store
+ * with the move when a session changes membership, the fix-up when a session runs fewer than n_frames hops and the
+ * history move on the synthesis where pnb_process_sessions_* would issue it. */
+int pnb_analyze_sessions_device_f32(pnb_engine *e, const int *ids, const int *hops, int n, const float *d_in, size_t in_stride,
+                                    int n_frames, float *d_feat, size_t feat_stride, void *cuda_stream);
+int pnb_analyze_sessions_device_i16(pnb_engine *e, const int *ids, const int *hops, int n, const short *d_in, size_t in_stride,
+                                    int n_frames, float *d_feat, size_t feat_stride, void *cuda_stream);
+int pnb_analyze_sessions_host_f32(pnb_engine *e, const int *ids, const int *hops, int n, const float *in, size_t in_stride,
+                                  int n_frames, float *feat, size_t feat_stride);
+int pnb_analyze_sessions_host_i16(pnb_engine *e, const int *ids, const int *hops, int n, const short *in, size_t in_stride,
+                                  int n_frames, float *feat, size_t feat_stride);
+int pnb_synthesize_sessions_device_f32(pnb_engine *e, const int *ids, int n, const float *d_gr, size_t gr_stride,
+                                       int n_frames, float *d_out, size_t out_stride, void *cuda_stream);
+int pnb_synthesize_sessions_device_i16(pnb_engine *e, const int *ids, int n, const float *d_gr, size_t gr_stride,
+                                       int n_frames, short *d_out, size_t out_stride, void *cuda_stream);
+int pnb_synthesize_sessions_host_f32(pnb_engine *e, const int *ids, int n, const float *gr, size_t gr_stride, int n_frames,
+                                     float *out, size_t out_stride);
+int pnb_synthesize_sessions_host_i16(pnb_engine *e, const int *ids, int n, const float *gr, size_t gr_stride, int n_frames,
+                                     short *out, size_t out_stride);
+int pnb_compute_rnn_sessions_device(pnb_engine *e, const int *ids, const int *hops, int n, int format, const float *d_in,
+                                    size_t in_stride, int n_frames, float *d_gr, size_t gr_stride, void *cuda_stream);
+int pnb_compute_rnn_sessions_host(pnb_engine *e, const int *ids, const int *hops, int n, int format, const float *in,
+                                  size_t in_stride, int n_frames, float *gr, size_t gr_stride);
+
 /* The pitch analysis alone (BASELINE.json config 5; needs no engine): for each of n_units pitch buffers of 1728
  * float samples (unit u at d_pitch_buf + u*stride; the reference's st->pitch_buf, src/denoise.cpp:80,405-411) runs
  * pitch_downsample, pitch_search and remove_doubling (src/pitch.cpp:148-216, 283-386, 423-527) exactly as the hot path

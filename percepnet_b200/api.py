@@ -106,6 +106,16 @@ def load_library() -> C.CDLL:
     L.pnb_export_sessions.argtypes = [vp, vp, i, vp, sz, vp]
     L.pnb_import_sessions.argtypes = [vp, vp, i, vp, sz, vp]
     L.pnb_session_stats.argtypes = [vp, vp]
+    for name in ("pnb_analyze_sessions_device_f32", "pnb_analyze_sessions_device_i16"):
+        getattr(L, name).argtypes = [vp, vp, vp, i, vp, sz, i, vp, sz, vp]
+    for name in ("pnb_analyze_sessions_host_f32", "pnb_analyze_sessions_host_i16"):
+        getattr(L, name).argtypes = [vp, vp, vp, i, vp, sz, i, vp, sz]
+    for name in ("pnb_synthesize_sessions_device_f32", "pnb_synthesize_sessions_device_i16"):
+        getattr(L, name).argtypes = [vp, vp, i, vp, sz, i, vp, sz, vp]
+    for name in ("pnb_synthesize_sessions_host_f32", "pnb_synthesize_sessions_host_i16"):
+        getattr(L, name).argtypes = [vp, vp, i, vp, sz, i, vp, sz]
+    L.pnb_compute_rnn_sessions_device.argtypes = [vp, vp, vp, i, i, vp, sz, i, vp, sz, vp]
+    L.pnb_compute_rnn_sessions_host.argtypes = [vp, vp, vp, i, i, vp, sz, i, vp, sz]
     L.pnb_pitch_only_device.argtypes = [vp, sz, C.c_longlong, vp, vp, vp, vp, vp, vp, vp]
     L.pnb_pitch_only_host.argtypes = [vp, sz, C.c_longlong, vp, vp, vp, vp, vp, vp]
     L.pnb_launch_count.argtypes = [vp]
@@ -137,7 +147,10 @@ EXPORTS = ("pnb_create", "pnb_destroy", "pnb_reset", "pnb_resolve_device", "pnb_
            "pnb_process_sessions_host_f32", "pnb_process_sessions_host_i16", "pnb_process_sessions_ragged_device_f32",
            "pnb_process_sessions_ragged_device_i16", "pnb_process_sessions_ragged_host_f32",
            "pnb_process_sessions_ragged_host_i16", "pnb_reset_sessions", "pnb_export_sessions",
-           "pnb_import_sessions", "pnb_session_stats", "pnb_pitch_only_device", "pnb_pitch_only_host", "pnb_launch_count",
+           "pnb_import_sessions", "pnb_session_stats", "pnb_analyze_sessions_device_f32", "pnb_analyze_sessions_device_i16",
+           "pnb_analyze_sessions_host_f32", "pnb_analyze_sessions_host_i16", "pnb_synthesize_sessions_device_f32",
+           "pnb_synthesize_sessions_device_i16", "pnb_synthesize_sessions_host_f32", "pnb_synthesize_sessions_host_i16",
+           "pnb_compute_rnn_sessions_device", "pnb_compute_rnn_sessions_host", "pnb_pitch_only_device", "pnb_pitch_only_host", "pnb_launch_count",
            "pnb_launches_per_call", "pnb_profile_enable", "pnb_profile_read", "pnb_profile_timeline", "pnb_kernel_class_name", "pnb_n_streams", "pnb_max_frames", "pnb_last_error", "pnb_version")
 
 
@@ -576,6 +589,95 @@ class Engine:
         c = (C.c_longlong * 3)()
         self._ck(self.L.pnb_session_stats(self.h, c), "pnb_session_stats")
         return {"parks": int(c[0]), "unparks": int(c[1]), "relocations": int(c[2])}
+
+    # ---- split and network calls on a session list (see pnb_analyze_sessions_device_f32 in the header) ---------------
+    def _session_hops(self, ids, hops, F, what):
+        """(ids int32, n, hops int32 or None) with hops checked against the list and the call's F hops."""
+        a, n = self._slots(ids)
+        if hops is None:
+            return a, n, None
+        hp, nh = self._slots(hops)
+        if nh != n or int(hp.max(initial=0)) != F:
+            raise PnbError(f"{what}: hops needs one entry per session, and the call must be max(hops) hops long")
+        return a, n, hp
+
+    def analyze_sessions(self, ids, x: np.ndarray, hops=None) -> np.ndarray:
+        """pnb_analyze_sessions_host_*: the analysis half of process_sessions.  x: [len(ids), F*480] float32 or int16, row
+        i for ids[i]; hops: None or one count per session (ragged, F = max(hops)).  Returns the features [len(ids), F, 70]
+        (zero after a session's own hops) and leaves a synthesis pending: synthesize_sessions with the same ids next (or
+        compute_rnn_sessions on them, or reset)."""
+        assert x.ndim == 2 and x.shape[1] % FRAME == 0
+        F = x.shape[1] // FRAME
+        a, n, hp = self._session_hops(ids, hops, F, "analyze_sessions")
+        assert x.shape[0] == n
+        x = np.ascontiguousarray(x)
+        feat = np.empty((n, F, 70), np.float32)
+        if x.dtype not in (np.float32, np.int16):
+            raise TypeError("x must be float32 or int16")
+        f = self.L.pnb_analyze_sessions_host_i16 if x.dtype == np.int16 else self.L.pnb_analyze_sessions_host_f32
+        self._ck(f(self.h, a.ctypes.data, None if hp is None else hp.ctypes.data, n, x.ctypes.data, x.shape[1], F,
+                   feat.ctypes.data, F * 70), "pnb_analyze_sessions_host")
+        return feat
+
+    def synthesize_sessions(self, ids, gr: np.ndarray, int16: bool = False) -> np.ndarray:
+        """pnb_synthesize_sessions_host_*: the synthesis half, on the pending list (same ids, same order).  gr:
+        [len(ids), F, 68] float32, read for each session's own hops.  Returns [len(ids), F*480] float32 (or int16): a
+        session's hops of output, then zeros."""
+        a, n = self._slots(ids)
+        if gr.dtype != np.float32:
+            raise TypeError("gr must be float32")
+        assert gr.ndim == 3 and gr.shape[0] == n and gr.shape[2] == 68, "gr must be [len(ids), F, 68]"
+        F = gr.shape[1]
+        gr = np.ascontiguousarray(gr)
+        out = np.empty((n, F * FRAME), np.int16 if int16 else np.float32)
+        f = self.L.pnb_synthesize_sessions_host_i16 if int16 else self.L.pnb_synthesize_sessions_host_f32
+        self._ck(f(self.h, a.ctypes.data, n, gr.ctypes.data, F * 68, F, out.ctypes.data, F * FRAME),
+                 "pnb_synthesize_sessions_host")
+        return out
+
+    def compute_rnn_sessions(self, ids, x: np.ndarray, hops=None) -> np.ndarray:
+        """pnb_compute_rnn_sessions_host: compute_rnn on the listed sessions.  x: [len(ids), F, 70 | 138] float32 (the
+        last dimension selects the format); hops: None or one count per session (F = max(hops)).  Returns g/r
+        [len(ids), F, 68], zero after a session's own hops.  Between the halves of a session split it must list the
+        pending sessions, hops and F."""
+        if x.dtype != np.float32:
+            raise TypeError("x must be float32")
+        assert x.ndim == 3 and x.shape[2] in (70, RECORD), "x must be [len(ids), F, 70 | 138]"
+        F, W = x.shape[1], x.shape[2]
+        a, n, hp = self._session_hops(ids, hops, F, "compute_rnn_sessions")
+        assert x.shape[0] == n
+        x = np.ascontiguousarray(x)
+        gr = np.empty((n, F, 68), np.float32)
+        fmt = RNN_FEATURES if W == 70 else RNN_RECORDS
+        self._ck(self.L.pnb_compute_rnn_sessions_host(self.h, a.ctypes.data, None if hp is None else hp.ctypes.data, n, fmt,
+                                                      x.ctypes.data, F * W, F, gr.ctypes.data, F * 68),
+                 "pnb_compute_rnn_sessions_host")
+        return gr
+
+    def analyze_sessions_device(self, ids, d_in: int, in_stride: int, n_frames: int, d_feat: int, feat_stride: int,
+                                stream: int = 0, int16: bool = False, hops=None):
+        """pnb_analyze_sessions_device_* on raw device pointers (strides in elements); hops: None or one count per
+        session, with n_frames = max(hops)."""
+        a, n, hp = self._session_hops(ids, hops, n_frames, "analyze_sessions_device")
+        f = self.L.pnb_analyze_sessions_device_i16 if int16 else self.L.pnb_analyze_sessions_device_f32
+        self._ck(f(self.h, a.ctypes.data, None if hp is None else hp.ctypes.data, n, d_in or None, in_stride, n_frames,
+                   d_feat or None, feat_stride, stream or None), "pnb_analyze_sessions_device")
+
+    def synthesize_sessions_device(self, ids, d_gr: int, gr_stride: int, n_frames: int, d_out: int, out_stride: int,
+                                   stream: int = 0, int16: bool = False):
+        """pnb_synthesize_sessions_device_* on raw device pointers (strides in elements)."""
+        a, n = self._slots(ids)
+        f = self.L.pnb_synthesize_sessions_device_i16 if int16 else self.L.pnb_synthesize_sessions_device_f32
+        self._ck(f(self.h, a.ctypes.data, n, d_gr or None, gr_stride, n_frames, d_out or None, out_stride, stream or None),
+                 "pnb_synthesize_sessions_device")
+
+    def compute_rnn_sessions_device(self, ids, format: int, d_in: int, in_stride: int, n_frames: int, d_gr: int,
+                                    gr_stride: int, stream: int = 0, hops=None):
+        """pnb_compute_rnn_sessions_device on raw device pointers (format RNN_FEATURES or RNN_RECORDS; strides in floats)."""
+        a, n, hp = self._session_hops(ids, hops, n_frames, "compute_rnn_sessions_device")
+        self._ck(self.L.pnb_compute_rnn_sessions_device(self.h, a.ctypes.data, None if hp is None else hp.ctypes.data, n,
+                                                        format, d_in or None, in_stride, n_frames, d_gr or None, gr_stride,
+                                                        stream or None), "pnb_compute_rnn_sessions_device")
 
     def read_nn_state(self) -> dict:
         """fp32 network state after the last hop: conv2 output and the five GRU states, [S, width]."""

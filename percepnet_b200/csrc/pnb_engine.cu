@@ -9,6 +9,10 @@
 // on caller-supplied features or training records.  The split call cuts the PCM call where the network sits:
 //   pnb_analyze_*:    stage_in -> analysis -> rows_store (features) [-> slide history]
 //   pnb_synthesize_*: rows_stage (caller g/r) -> synthesis
+// and on a session list (pnb_*_sessions_*), where the ragged fix-up and the slide follow the synthesis as in the fused
+// session call:
+//   pnb_analyze_sessions_*:    [session move] -> stage_in -> analysis -> rows_store (features)
+//   pnb_synthesize_sessions_*: rows_stage (caller g/r) -> synthesis [-> ragged fix-up] [-> slide history]
 #include <math.h>
 #include <stdarg.h>
 #include <stdio.h>
@@ -17,6 +21,7 @@
 
 #include <stddef.h>
 #include <stdint.h>
+#include <algorithm>
 #include <string>
 #include <vector>
 
@@ -316,6 +321,9 @@ extern "C" int pnb_reset(pnb_engine *e) {
   e->h_status[1] = kNoRejectedSlot;
   e->hop = 0;
   e->pending = 0;
+  e->pend_ids.clear();
+  e->pend_hops.clear();
+  e->pend_up.clear();
   e->n_active = e->S;
   e->poisoned = false;
   if (e->sessions) {  // every session fresh: all parked, every blob marked fresh
@@ -508,38 +516,66 @@ struct RaggedSlots {
   int n_short = 0;
 };
 
-// A session call's residency plan, applied (pnb_session_plan.h), its upload (row map, then the moves, then for a ragged
-// call the hops of every slot and the slots with fewer than F), and its state launch when membership changed.  Sets the
-// active range to the list; *d_row: the row map on the device.  Returns the number of launches or a negative error.
-static int enqueue_plan(pnb_engine *e, const int *ids, int k, const int *hops, int F, cudaStream_t st, const int **d_row,
-                        RaggedSlots *rg) {
+// The rows of a session call on the device, one upload: the row map (list row of slot p), for a split or network call
+// the slot map (slot of list row i: their layout kernels walk the caller's rows), and for a ragged call the hops of
+// every slot and the slots with fewer than F.  n_up: the ints of that upload, [row][slot][hops][short slots].
+struct SessionRows {
+  const int *row = nullptr;
+  const int *slot = nullptr;
+  RaggedSlots rg;
+  size_t n_up = 0;
+};
+static void point_rows(const int *d, int k, bool with_slot, bool ragged, size_t n_up, SessionRows *r) {
+  size_t at = (size_t)k;
+  r->row = d;
+  if (with_slot) { r->slot = d + at; at += k; }
+  if (ragged) {
+    r->rg.hops = d + at;
+    r->rg.slots = d + at + k;
+    r->rg.n_short = (int)(n_up - at - k);
+  }
+  r->n_up = n_up;
+}
+
+// A session call's residency plan, applied (pnb_session_plan.h), its upload (the rows of SessionRows, then the moves
+// 16-byte aligned), and its state launch when membership changed.  Sets the active range to the list; *r: the rows on
+// the device.  Returns the number of launches or a negative error.
+static int enqueue_plan(pnb_engine *e, const int *ids, int k, const int *hops, int F, bool with_slot, cudaStream_t st,
+                        SessionRows *r) {
   StateArgs a = state_args(e);  // before the plan: parking reads the pieces where the last call left them
   e->pool.plan(ids, k, e->plan_row, e->plan_moves);
   e->n_active = k;
-  const size_t k4 = ((size_t)k + 3) & ~(size_t)3;  // the moves start 16-byte aligned
   std::vector<int> &up = e->plan_up;
   up.assign(e->plan_row.begin(), e->plan_row.end());
-  up.resize(k4, 0);
-  const int *mv = reinterpret_cast<const int *>(e->plan_moves.data());
-  up.insert(up.end(), mv, mv + 4 * e->plan_moves.size());
-  const size_t at_hops = up.size();
+  if (with_slot) {
+    up.resize(2 * (size_t)k);
+    for (int p = 0; p < k; p++) up[k + e->plan_row[p]] = p;
+  }
   if (hops) {  // slot p runs the hops of its list row; then the slots that stop early
     for (int p = 0; p < k; p++) up.push_back(hops[e->plan_row[p]]);
     for (int p = 0; p < k; p++)
       if (hops[e->plan_row[p]] < F) up.push_back(p);
   }
+  const size_t n_up = up.size();
+  up.resize((n_up + 3) & ~(size_t)3, 0);  // the moves start 16-byte aligned
+  const size_t at_moves = up.size();
+  const int *mv = reinterpret_cast<const int *>(e->plan_moves.data());
+  up.insert(up.end(), mv, mv + 4 * e->plan_moves.size());
   const int *d = nullptr;
   { int rc = stage_ints(e, up.data(), up.size(), st, &d); if (rc) return rc; }
-  *d_row = d;
-  if (hops) {
-    rg->hops = d + at_hops;
-    rg->slots = d + at_hops + k;
-    rg->n_short = (int)(up.size() - at_hops - k);
-  }
+  point_rows(d, k, with_slot, hops != nullptr, n_up, r);
   if (e->plan_moves.empty()) return 0;
   a.n = (int)e->plan_moves.size();
-  a.moves = d + k4;
+  a.moves = d + at_moves;
   return launch_session_move(a, st);
+}
+
+// The rows of the pending session split, from its host copy (pnb_engine::pend_up): nothing is planned again.
+static int stage_pending_rows(pnb_engine *e, cudaStream_t st, SessionRows *r) {
+  const int *d = nullptr;
+  { int rc = stage_ints(e, e->pend_up.data(), e->pend_up.size(), st, &d); if (rc) return rc; }
+  point_rows(d, (int)e->pend_ids.size(), true, !e->pend_hops.empty(), e->pend_up.size(), r);
+  return PNB_OK;
 }
 
 // A session export into the caller's blobs (a: their address and stride): resident sessions from their slots
@@ -615,39 +651,53 @@ static Rows pcm(const T *p, size_t stride) { return rows(p, stride, kFrame, size
 // One call as its entry point received it, its buffers as row arrays.  In / out: PCM / PCM of a slot, session or ragged
 // call; speech, noisy / records and (pnb_train_audio_*) audio of a training-record call; features or records / g/r of a
 // network call; records / g/r (when asked for) and the loss sums of a score call; PCM / features of an analysis; g/r /
-// PCM of a synthesis.
+// PCM of a synthesis.  An analysis, synthesis or network call on a session list (pool) has ids too; its analysis and
+// network forms may have hops.
 struct Call {
   enum Kind { kSlots, kSessions, kRagged, kNetwork, kRecords, kAnalyze, kSynthesize, kTrain } kind;
   Rows in[2], out[2];
   int F;           // hops; a ragged call's is max(hops), set by check_call
   float *gr;       // enhancement calls: g/r destination [F][rows][68], or null
-  const int *ids;  // session and ragged calls: the session list (host), n_ids long
+  const int *ids;  // session, ragged and pool calls: the session list (host), n_ids long
   int n_ids;
-  const int *hops;    // ragged calls: each listed session's hops (host); null once check_call finds them all equal to F
+  const int *hops;    // ragged and pool calls: each listed session's hops (host), or null; null once check_call finds
+                      // them all equal to F
   int format;         // network calls: PNB_RNN_FEATURES or PNB_RNN_RECORDS
   const int *frames;  // score and gradient calls: the hops each row's loss counts (host), or null for F
   bool status = true;  // a blocking host call reads back and reports the status word (rejected imports, PNB_ERR_DOMAIN)
+  bool pool = false;   // an analysis, synthesis or network call on a session list (pnb_*_sessions_*)
 };
 
 // A network call on st (arguments already checked): the caller's rows into the features buffer, the network hook, its
 // g/r out to the caller's rows; a score call reduces the loss from the same g/r and writes g/r only when asked.  The
-// signal state (history line, overlap-add, pitch memory, spectrum ring, hop counter, line offset) is not touched.
+// signal state (history line, overlap-add, pitch memory, spectrum ring, hop counter, line offset) is not touched.  On a
+// session list the call first applies its residency plan like any session call, or, between the halves of a session
+// split, stages the pending split's rows again (the same list: nothing moves mid-hop); row i of the caller's arrays is
+// then ids[i]'s, and a ragged call's frozen hops stage and store zeros.
 static int enqueue_network(pnb_engine *e, const Call &c, cudaStream_t st) {
   const int F = c.F;
   const Rows &in = c.in[0], &gr = c.out[0], &sums = c.out[1];
   return enqueue_call(e, F, st, [&]() -> int {
-    const int S = e->S, na = e->n_active;
     int n = 0;
+    SessionRows r;
+    if (c.pool && e->pending) {
+      const int rc = stage_pending_rows(e, st, &r);
+      if (rc) return rc;
+    } else if (c.pool) {
+      n = enqueue_plan(e, c.ids, c.n_ids, c.hops, F, true, st, &r);
+      if (n < 0) return n;
+    }
+    const int S = e->S, na = e->n_active;
     const int *frames = nullptr;  // a score call's per-row hop counts, staged like a ragged call's hops
     if (c.frames) { int rc = stage_ints(e, c.frames, (size_t)na, st, &frames); if (rc) return rc; }
     {
       ProfScope ps(e, PNB_K_STAGE_IN, st);
       n += launch_rows_stage(e->d_feat, kFeat, static_cast<const float *>(in.p), in.stride, (int)in.width,
-                             c.format == PNB_RNN_RECORDS ? 68 : 0, na, S, F, st);
+                             c.format == PNB_RNN_RECORDS ? 68 : 0, na, S, F, st, r.row, r.rg.hops);
     }
     CK(cudaGetLastError());
     {
-      const int q = (e->flags & PNB_NN_TENSOR) ? tc_network(e, F, nullptr, st) : f32_network(e, F, nullptr, st);
+      const int q = (e->flags & PNB_NN_TENSOR) ? tc_network(e, F, r.rg.hops, st) : f32_network(e, F, r.rg.hops, st);
       if (q < 0) return q;
       n += q;
     }
@@ -655,7 +705,10 @@ static int enqueue_network(pnb_engine *e, const Call &c, cudaStream_t st) {
       ProfScope ps(e, PNB_K_STAGE_IN, st);
       n += launch_loss_sums(e->d_gr, static_cast<const float *>(in.p), in.stride, frames, static_cast<double *>(sums.p), na, S, F, st);
     }
-    if (gr.p) { ProfScope ps(e, PNB_K_STAGE_IN, st); n += launch_rows_store(e->d_gr, 68, static_cast<float *>(gr.p), gr.stride, na, S, F, st); }
+    if (gr.p) {
+      ProfScope ps(e, PNB_K_STAGE_IN, st);
+      n += launch_rows_store(e->d_gr, 68, static_cast<float *>(gr.p), gr.stride, na, S, F, st, r.slot, r.rg.hops);
+    }
     return n;
   }, false);
 }
@@ -706,12 +759,13 @@ static int enqueue_enhance(pnb_engine *e, const Call &c, cudaStream_t st) {
   const bool i16 = c.in[0].bytes == sizeof(short);
   return enqueue_call(e, F, st, [&]() -> int {
     int n = 0;
-    const int *row = nullptr;
-    RaggedSlots rg;
+    SessionRows r;
     if (c.ids) {
-      n = enqueue_plan(e, c.ids, c.n_ids, c.hops, F, st, &row, &rg);
+      n = enqueue_plan(e, c.ids, c.n_ids, c.hops, F, false, st, &r);
       if (n < 0) return n;
     }
+    const int *row = r.row;
+    const RaggedSlots &rg = r.rg;
     const int S = e->S, na = e->n_active;  // the call advances streams [0, na); per-call buffers keep the stride S
     const float *in = i16 ? nullptr : static_cast<const float *>(c.in[0].p);
     const short *in16 = i16 ? static_cast<const short *>(c.in[0].p) : nullptr;
@@ -754,46 +808,91 @@ static int enqueue_enhance(pnb_engine *e, const Call &c, cudaStream_t st) {
 // history slide, exactly as enqueue_enhance runs them, and the features out to the caller's rows.  The hop counter stays
 // where it is (the analysis and synthesis kernels both take hop0 = e->hop); the synthesis that completes these hops
 // commits it.  The slide may run before the synthesis: synthesis reads the spectra, not the history line.
+// On a session list the call first applies its residency plan as enqueue_enhance does, stages and analyses through the
+// row map and per-slot hops, and leaves the slide to the synthesis half: there a ragged call's fix-up runs after the
+// synthesis and before the slide, the fused call's order, so this half moves nothing bound to the counters.  The pending
+// split keeps the list, the hops and the rows of its upload.
 static int enqueue_analyze(pnb_engine *e, const Call &c, cudaStream_t st) {
   const int F = c.F;
   const Rows &in = c.in[0], &feat = c.out[0];
   const bool i16 = in.bytes == sizeof(short);
+  SessionRows r;
   const int rc = enqueue_call(e, F, st, [&]() -> int {
-    const int S = e->S, na = e->n_active;
     int n = 0;
+    if (c.pool) {
+      n = enqueue_plan(e, c.ids, c.n_ids, c.hops, F, true, st, &r);
+      if (n < 0) return n;
+    }
+    const int S = e->S, na = e->n_active;
     {
       ProfScope ps(e, PNB_K_STAGE_IN, st);
       n += launch_stage_in(e->d_pcm + e->line_off, e->pcm_stride, i16 ? nullptr : static_cast<const float *>(in.p),
-                           i16 ? static_cast<const short *>(in.p) : nullptr, in.stride, na, F * kFrame, st, 32768.f);
+                           i16 ? static_cast<const short *>(in.p) : nullptr, in.stride, na, F * kFrame, st, 32768.f, r.row,
+                           r.rg.hops);
     }
-    { ProfScope ps(e, PNB_K_ANALYSIS, st); n += launch_analysis(analysis_args(e, F), st); }
-    { ProfScope ps(e, PNB_K_STAGE_IN, st); n += launch_rows_store(e->d_feat, kFeat, static_cast<float *>(feat.p), feat.stride, na, S, F, st); }
-    n += advance_line(e, F, st);
+    {
+      AnalysisArgs aa = analysis_args(e, F);
+      aa.hops = r.rg.hops;
+      ProfScope ps(e, PNB_K_ANALYSIS, st);
+      n += launch_analysis(aa, st);
+    }
+    {
+      ProfScope ps(e, PNB_K_STAGE_IN, st);
+      n += launch_rows_store(e->d_feat, kFeat, static_cast<float *>(feat.p), feat.stride, na, S, F, st, r.slot, r.rg.hops);
+    }
+    if (!c.pool) n += advance_line(e, F, st);
     return n;
   }, false);
-  if (rc == PNB_OK) e->pending = F;
+  if (rc == PNB_OK) {
+    e->pending = F;
+    if (c.pool) {
+      e->pend_ids.assign(c.ids, c.ids + c.n_ids);
+      if (c.hops) e->pend_hops.assign(c.hops, c.hops + c.n_ids);
+      else e->pend_hops.clear();
+      e->pend_up.assign(e->plan_up.begin(), e->plan_up.begin() + r.n_up);
+    }
+  }
   return rc;
 }
 
 // The synthesis half (arguments already checked, an analysis of F hops pending): the caller's g/r rows into d_gr where
-// the network hook would have left them, then the synthesis of enqueue_enhance, which commits the hop counter.
+// the network hook would have left them, then the synthesis of enqueue_enhance, which commits the hop counter.  For a
+// session split the pending rows are staged again, and the ragged fix-up and the history slide follow the synthesis,
+// in enqueue_enhance's order.
 static int enqueue_synthesize(pnb_engine *e, const Call &c, cudaStream_t st) {
   const int F = c.F;
   const Rows &gr = c.in[0], &out = c.out[0];
   const bool i16 = out.bytes == sizeof(short);
   const int rc = enqueue_call(e, F, st, [&]() -> int {
     int n = 0;
+    SessionRows r;
+    if (c.pool) { int q = stage_pending_rows(e, st, &r); if (q) return q; }
     {
       ProfScope ps(e, PNB_K_STAGE_IN, st);
-      n += launch_rows_stage(e->d_gr, 68, static_cast<const float *>(gr.p), gr.stride, 68, 0, e->n_active, e->S, F, st);
+      n += launch_rows_stage(e->d_gr, 68, static_cast<const float *>(gr.p), gr.stride, 68, 0, e->n_active, e->S, F, st,
+                             r.row, r.rg.hops);
     }
-    SynthesisArgs sa = synthesis_args(e, F, i16 ? nullptr : static_cast<float *>(out.p),
-                                      i16 ? static_cast<short *>(out.p) : nullptr, out.stride);
-    ProfScope ps(e, PNB_K_SYNTHESIS, st);
-    n += launch_synthesis(sa, st);
+    {
+      SynthesisArgs sa = synthesis_args(e, F, i16 ? nullptr : static_cast<float *>(out.p),
+                                        i16 ? static_cast<short *>(out.p) : nullptr, out.stride);
+      sa.row = r.row;
+      sa.hops = r.rg.hops;
+      ProfScope ps(e, PNB_K_SYNTHESIS, st);
+      n += launch_synthesis(sa, st);
+    }
+    if (r.rg.n_short) {  // before the slide: it moves the window the counters of hop F point at
+      ProfScope ps(e, PNB_K_SLIDE, st);
+      n += launch_ragged_carry(e, F, r.rg.hops, r.rg.slots, r.rg.n_short, st);
+    }
+    if (c.pool) n += advance_line(e, F, st);
     return n;
   });
-  if (rc == PNB_OK) e->pending = 0;
+  if (rc == PNB_OK) {
+    e->pending = 0;
+    e->pend_ids.clear();
+    e->pend_hops.clear();
+    e->pend_up.clear();
+  }
   return rc;
 }
 
@@ -867,25 +966,43 @@ static int check_strides(const Rows (&a)[2], int F) {
   return PNB_OK;
 }
 
+// A call on a session list while a session split is pending: the pending list in its order and n_frames, and for a
+// network call (which passes hops) the pending hops.
+static int check_pending_list(const pnb_engine *e, const Call &c) {
+  const std::vector<int> &ids = e->pend_ids, &hops = e->pend_hops;
+  bool same = c.n_ids == (int)ids.size() && c.F == e->pending && std::equal(ids.begin(), ids.end(), c.ids);
+  if (same && c.kind == Call::kNetwork)
+    same = c.hops ? !hops.empty() && std::equal(hops.begin(), hops.end(), c.hops) : hops.empty();
+  if (!same)
+    return fail(PNB_ERR_ARG, "a session split of %d sessions and %d hops is pending: pass its list in the same order, its n_frames%s",
+                (int)ids.size(), e->pending, c.kind == Call::kNetwork ? " and its hops" : "");
+  return PNB_OK;
+}
+
 // Every refusal of a call, before anything changes.  Every call checks an engine of its family (training records,
 // enhancement or the network alone; a PNB_NETWORK_ONLY engine runs network calls only, a PNB_SIGNAL_ONLY engine split
 // calls only) that no failed call has poisoned, 1 <= F <= Fmax, none of its arrays NULL, the input strides; a
 // training-record call then that its engine has audio exactly when the call does; every call then the output strides,
-// and the pending synthesis: a synthesis needs one of F hops, every other call but a network call needs none.  After
-// that a slot or split call checks session mode, a session call its list, a network call its format, then session mode,
-// and a score call its frames.  A ragged
-// call checks the list and its hop counts first, because their largest is the call's length F; when every session runs
-// F hops, hops becomes null and the call is the plain session call.
+// and the pending synthesis: a synthesis needs one of F hops (on a session list: the pending list), a network call on a
+// session list while one is pending the pending list and hops, every other call but a network call none.  After that a
+// slot or split call checks session mode, a session call its list, a network call its format, then session mode, and a
+// score call its frames.  A ragged call, and a split or network call on a session list, checks the list first (so
+// session mode) and then the hop counts, because their largest is a ragged call's length F and must be a pool call's
+// n_frames; when every session runs F hops, hops becomes null and the call is the call without hops.
 static int check_call(pnb_engine *e, Call &c) {
-  if (c.kind == Call::kRagged) {
+  if (c.kind == Call::kRagged || c.pool) {
     if (!e) return fail(PNB_ERR_ARG, "engine is NULL");
     { int rc = check_ids(e, c.ids, c.n_ids, e->S); if (rc) return rc; }
-    if (!c.hops) return fail(PNB_ERR_ARG, "hops is NULL");
-    c.F = 0;
+    if (c.kind == Call::kRagged && !c.hops) return fail(PNB_ERR_ARG, "hops is NULL");
+  }
+  if (c.hops) {
+    int F = 0;
     for (int i = 0; i < c.n_ids; i++) {
       if (c.hops[i] < 1 || c.hops[i] > e->Fmax) return fail(PNB_ERR_ARG, "hops[%d] = %d outside [1, %d]", i, c.hops[i], e->Fmax);
-      c.F = c.hops[i] > c.F ? c.hops[i] : c.F;
+      F = c.hops[i] > F ? c.hops[i] : F;
     }
+    if (c.kind == Call::kRagged) c.F = F;
+    else if (c.F != F) return fail(PNB_ERR_ARG, "n_frames %d, but max(hops) = %d", c.F, F);
     bool uniform = true;
     for (int i = 0; i < c.n_ids; i++) uniform = uniform && c.hops[i] == c.F;
     if (uniform) c.hops = nullptr;
@@ -915,13 +1032,17 @@ static int check_call(pnb_engine *e, Call &c) {
   if (c.kind == Call::kSynthesize) {
     if (!e->pending) return fail(PNB_ERR_ARG, "no analysis awaits its synthesis: call pnb_analyze_* first");
     if (c.F != e->pending) return fail(PNB_ERR_ARG, "n_frames %d, but the pending analysis has %d hops", c.F, e->pending);
+    if (c.pool) { int rc = check_pending_list(e, c); if (rc) return rc; }
   } else if (e->pending && !network) {
     return refuse_pending(e);
+  } else if (e->pending && c.pool) {
+    int rc = check_pending_list(e, c);
+    if (rc) return rc;
   }
   if (c.kind == Call::kSessions) return check_ids(e, c.ids, c.n_ids, e->S);
   if (c.kind == Call::kNetwork && c.format != PNB_RNN_FEATURES && c.format != PNB_RNN_RECORDS)
     return fail(PNB_ERR_ARG, "format %d is neither PNB_RNN_FEATURES (0) nor PNB_RNN_RECORDS (1)", c.format);
-  if ((c.kind == Call::kSlots || network || split) && e->sessions) return refuse_in_session_mode();
+  if ((c.kind == Call::kSlots || network || split) && !c.pool && e->sessions) return refuse_in_session_mode();
   const int fr_lo = c.kind == Call::kTrain ? 1 : 0;  // a window of a gradient call has at least one hop
   if (c.frames)  // every row's counted hops in [fr_lo, F]
     for (int i = 0; i < e->n_active; i++)
@@ -1292,6 +1413,61 @@ extern "C" int pnb_synthesize_device_i16(pnb_engine *e, const float *d_gr, size_
   return device_call(e, synthesize_call(d_gr, gr_stride, n_frames, d_out, sizeof(short), out_stride), (cudaStream_t)cuda_stream);
 }
 
+// The split and network calls on a session list: row i of every array belongs to ids[i]; hops NULL, or each listed
+// session's own hops (ragged, n_frames = max(hops)).  The synthesis takes the list, hops and rows of the pending analysis.
+static Call on_sessions(Call c, const int *ids, const int *hops, int n) {
+  c.ids = ids;
+  c.n_ids = n;
+  c.hops = hops;
+  c.pool = true;
+  return c;
+}
+extern "C" int pnb_analyze_sessions_device_f32(pnb_engine *e, const int *ids, const int *hops, int n, const float *d_in,
+                                               size_t in_stride, int n_frames, float *d_feat, size_t feat_stride, void *cuda_stream) {
+  return device_call(e, on_sessions(analyze_call(d_in, sizeof(float), in_stride, n_frames, d_feat, feat_stride), ids, hops, n),
+                     (cudaStream_t)cuda_stream);
+}
+extern "C" int pnb_analyze_sessions_device_i16(pnb_engine *e, const int *ids, const int *hops, int n, const short *d_in,
+                                               size_t in_stride, int n_frames, float *d_feat, size_t feat_stride, void *cuda_stream) {
+  return device_call(e, on_sessions(analyze_call(d_in, sizeof(short), in_stride, n_frames, d_feat, feat_stride), ids, hops, n),
+                     (cudaStream_t)cuda_stream);
+}
+extern "C" int pnb_analyze_sessions_host_f32(pnb_engine *e, const int *ids, const int *hops, int n, const float *in,
+                                             size_t in_stride, int n_frames, float *feat, size_t feat_stride) {
+  return host_call(e, on_sessions(analyze_call(in, sizeof(float), in_stride, n_frames, feat, feat_stride), ids, hops, n), false);
+}
+extern "C" int pnb_analyze_sessions_host_i16(pnb_engine *e, const int *ids, const int *hops, int n, const short *in,
+                                             size_t in_stride, int n_frames, float *feat, size_t feat_stride) {
+  return host_call(e, on_sessions(analyze_call(in, sizeof(short), in_stride, n_frames, feat, feat_stride), ids, hops, n), false);
+}
+extern "C" int pnb_synthesize_sessions_device_f32(pnb_engine *e, const int *ids, int n, const float *d_gr, size_t gr_stride,
+                                                  int n_frames, float *d_out, size_t out_stride, void *cuda_stream) {
+  return device_call(e, on_sessions(synthesize_call(d_gr, gr_stride, n_frames, d_out, sizeof(float), out_stride), ids, nullptr, n),
+                     (cudaStream_t)cuda_stream);
+}
+extern "C" int pnb_synthesize_sessions_device_i16(pnb_engine *e, const int *ids, int n, const float *d_gr, size_t gr_stride,
+                                                  int n_frames, short *d_out, size_t out_stride, void *cuda_stream) {
+  return device_call(e, on_sessions(synthesize_call(d_gr, gr_stride, n_frames, d_out, sizeof(short), out_stride), ids, nullptr, n),
+                     (cudaStream_t)cuda_stream);
+}
+extern "C" int pnb_synthesize_sessions_host_f32(pnb_engine *e, const int *ids, int n, const float *gr, size_t gr_stride,
+                                                int n_frames, float *out, size_t out_stride) {
+  return host_call(e, on_sessions(synthesize_call(gr, gr_stride, n_frames, out, sizeof(float), out_stride), ids, nullptr, n), false);
+}
+extern "C" int pnb_synthesize_sessions_host_i16(pnb_engine *e, const int *ids, int n, const float *gr, size_t gr_stride,
+                                                int n_frames, short *out, size_t out_stride) {
+  return host_call(e, on_sessions(synthesize_call(gr, gr_stride, n_frames, out, sizeof(short), out_stride), ids, nullptr, n), false);
+}
+extern "C" int pnb_compute_rnn_sessions_device(pnb_engine *e, const int *ids, const int *hops, int n, int format, const float *d_in,
+                                               size_t in_stride, int n_frames, float *d_gr, size_t gr_stride, void *cuda_stream) {
+  return device_call(e, on_sessions(network_call(format, d_in, in_stride, n_frames, d_gr, gr_stride), ids, hops, n),
+                     (cudaStream_t)cuda_stream);
+}
+extern "C" int pnb_compute_rnn_sessions_host(pnb_engine *e, const int *ids, const int *hops, int n, int format, const float *in,
+                                             size_t in_stride, int n_frames, float *gr, size_t gr_stride) {
+  return host_call(e, on_sessions(network_call(format, in, in_stride, n_frames, gr, gr_stride), ids, hops, n), false);
+}
+
 extern "C" int pnb_flush(pnb_engine *e, void *cuda_stream) {
   if (!e) return fail(PNB_ERR_ARG, "engine is NULL");
   CK(cudaSetDevice(e->device));
@@ -1496,9 +1672,9 @@ extern "C" int pnb_sessions_reserve(pnb_engine *e, int n_sessions) {
   CK(cudaSetDevice(e->device));
   CK(cudaDeviceSynchronize());
   const size_t cap = (size_t)n_sessions, wide = cap > (size_t)e->S ? cap : (size_t)e->S;
-  // staging: a call's row map, moves, and for a ragged call slot hops and short slots (<= 7 S + 3 ints), an export's
-  // moves, ids and rows (<= 6 n)
-  { int rc = grow_ints(e, 7 * wide + 4); if (rc) return rc; }
+  // staging: a call's row and slot maps, for a ragged call slot hops and short slots, then the moves (<= 8 S + 3 ints),
+  // an export's moves, ids and rows (<= 6 n)
+  { int rc = grow_ints(e, 8 * wide + 4); if (rc) return rc; }
   if (wide > e->ok_cap) {
     int *ok = nullptr;
     CK(cudaMalloc((void **)&ok, wide * sizeof(int)));
@@ -1577,6 +1753,7 @@ extern "C" int pnb_process_sessions_ragged_host_i16(pnb_engine *e, const int *id
 static int session_batch(pnb_engine *e, int mode, const int *ids, int n, void *d_blobs, size_t blob_stride, void *cuda_stream) {
   if (!e) return fail(PNB_ERR_ARG, "engine is NULL");
   if (e->poisoned) return refuse_poisoned(PNB_ERR_ARG);
+  if (e->pending) return refuse_pending(e);
   if (n == 0 && e->sessions) return PNB_OK;
   if (mode != kStateReset) { int rc = check_blobs(d_blobs, blob_stride); if (rc) return rc; }
   { int rc = check_ids(e, ids, n, e->pool.capacity()); if (rc) return rc; }

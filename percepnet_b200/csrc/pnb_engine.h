@@ -81,6 +81,12 @@ struct pnb_engine {
   // hops of an analysis (pnb_analyze_*) whose synthesis (pnb_synthesize_*) is still due, or 0.  Between the two halves
   // the analysed streams are mid-hop, so every call and state operation but the synthesis and network calls is refused.
   int pending = 0;
+  // A session split (pnb_analyze_sessions_*) pending: its list, its hops in list order (empty when every session runs
+  // `pending` hops) and the host copy of its row upload (row map, slot map, and for a ragged call the hops of every slot
+  // and the slots that stop early).  The index staging that upload went through is reused by the next call, and the
+  // plan is already applied to the pool, so the synthesis and a network call between the halves stage this copy again.
+  // All empty for a slot split.
+  std::vector<int> pend_ids, pend_hops, pend_up;
   long long launches = 0;
   // status word on the device: bit 0 = an activation left the domain in which the reference's tansig_approx is
   // defined (tensor path only; reported as PNB_ERR_DOMAIN by the synchronising entry points, cleared by pnb_reset);
@@ -115,7 +121,7 @@ struct pnb_engine {
   char *d_park = nullptr;        // [capacity][kParkStride] parking blobs; magic 0 = a fresh (or rejected) session
   float *d_sgr = nullptr;        // pnb_process_sessions_host_*: g/r of the call in list order, grown on first use
   size_t sgr_bytes = 0;
-  std::vector<int> plan_row, plan_up;       // scratch of a session call: row map, and what is uploaded
+  std::vector<int> plan_row, plan_up;       // scratch of a session call: row map, and what is uploaded (session_rows)
   std::vector<pnb::SessionMove> plan_moves;
 
   // optional per-kernel-class timing (pnb_profile_enable): CUDA events around every launch

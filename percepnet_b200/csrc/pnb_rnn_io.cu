@@ -1,42 +1,53 @@
 // pnb_rnn_io.cu -- the layout moves between a caller's stream-major rows and the per-call buffers [F][S][w] of the
 // engine: the network call's features or training records into d_feat and its g/r out of d_gr (pnb_compute_rnn_*), the
 // analysis half's features out of d_feat (pnb_analyze_*) and the synthesis half's caller g/r into d_gr
-// (pnb_synthesize_*); and the loss of a score call (pnb_score_records_*), reduced from the same g/r and the records'
+// (pnb_synthesize_*), and the same on a session list (row-mapped, with per-slot hops); and the loss of a score call (pnb_score_records_*), reduced from the same g/r and the records'
 // labels.
 #include "../../include/percepnet_b200.h"
 #include "pnb_kernels.h"
 
 namespace pnb {
 
-// dst[(t*S + s)*W + j] = in[s*in_stride + t*in_width + j] for the rows [0, n) of every hop t and j < W; the first
-// n_scaled values of a hop are multiplied by 30, the others copied as they are.  Features: W = 70, in_width 70, none
-// scaled.  Records: W = 70, in_width 138, the first 68 scaled (create_features, denoise.cpp:487-496; rnn_train.py:44-48),
-// T and pitchcorr as they are, the labels rec[70..137] never read.  g/r: W = 68, in_width 68, none scaled.  Threads walk
-// the output in order: the writes are contiguous, the reads contiguous runs of W floats.
-template <int W>
+// dst[(t*S + s)*W + j] = in[r*in_stride + t*in_width + j] for the rows [0, n) of every hop t and j < W, r = s (kMapped
+// false) or row[s]: the list row of slot s in a session call; the first n_scaled values of a hop are multiplied by 30,
+// the others copied as they are.  With hops (kMapped only) slot s gets zeros for its hops t >= hops[s], and the caller's
+// row is not read there.  Features: W = 70, in_width 70, none scaled.  Records: W = 70, in_width 138, the first 68
+// scaled (create_features, denoise.cpp:487-496; rnn_train.py:44-48), T and pitchcorr as they are, the labels
+// rec[70..137] never read.  g/r: W = 68, in_width 68, none scaled.  Threads walk the output in order: the writes are
+// contiguous, the reads contiguous runs of W floats.
+template <int W, bool kMapped>
 __global__ void rows_stage_kernel(float *__restrict__ dst, const float *__restrict__ in, size_t in_stride, int in_width,
-                                  int n_scaled, int n, int S, int F) {
+                                  int n_scaled, int n, int S, int F, const int *__restrict__ row,
+                                  const int *__restrict__ hops) {
   const long long total = (long long)F * n * W;
   for (long long x = (long long)blockIdx.x * blockDim.x + threadIdx.x; x < total; x += (long long)gridDim.x * blockDim.x) {
     const int j = (int)(x % W);
     const long long ts = x / W;
     const int s = (int)(ts % n), t = (int)(ts / n);
-    const float v = in[(size_t)s * in_stride + (size_t)t * in_width + j];
-    dst[((size_t)t * S + s) * W + j] = j < n_scaled ? v * 30.f : v;
+    float *d = dst + ((size_t)t * S + s) * W + j;
+    if (kMapped && hops && t >= hops[s]) {
+      *d = 0.f;
+      continue;
+    }
+    const float v = in[(size_t)(kMapped ? row[s] : s) * in_stride + (size_t)t * in_width + j];
+    *d = j < n_scaled ? v * 30.f : v;
   }
 }
 
-// out[s*out_stride + t*W + c] = src[(t*S + s)*W + c] for the rows [0, n): g/r (W = 68) and features (W = 70).  Threads
-// walk the output in order: the writes are contiguous, the reads contiguous runs of W floats.
-template <int W>
+// out[r*out_stride + t*W + c] = src[(t*S + s)*W + c] for the rows r of [0, n), s = r (kMapped false) or slot[r]: the
+// slot of list row r in a session call; with hops (kMapped only) zeros for the hops t >= hops[s] the slot did not run.
+// g/r (W = 68) and features (W = 70).  Threads walk the output in order: the writes are contiguous, the reads
+// contiguous runs of W floats.
+template <int W, bool kMapped>
 __global__ void rows_store_kernel(const float *__restrict__ src, float *__restrict__ out, size_t out_stride, int n, int S,
-                                  int F) {
+                                  int F, const int *__restrict__ slot, const int *__restrict__ hops) {
   const long long total = (long long)n * F * W;
   for (long long x = (long long)blockIdx.x * blockDim.x + threadIdx.x; x < total; x += (long long)gridDim.x * blockDim.x) {
     const int c = (int)(x % W);
-    const long long st = x / W;
-    const int t = (int)(st % F), s = (int)(st / F);
-    out[(size_t)s * out_stride + (size_t)t * W + c] = src[((size_t)t * S + s) * W + c];
+    const long long rt = x / W;
+    const int t = (int)(rt % F), r = (int)(rt / F);
+    const int s = kMapped ? slot[r] : r;
+    out[(size_t)r * out_stride + (size_t)t * W + c] = (kMapped && hops && t >= hops[s]) ? 0.f : src[((size_t)t * S + s) * W + c];
   }
 }
 
@@ -90,19 +101,31 @@ static unsigned copy_blocks(long long total) {
   return (unsigned)(b < 8192 ? b : 8192);
 }
 
+template <int W>
+static void rows_stage(unsigned blocks, float *dst, const float *in, size_t in_stride, int in_width, int n_scaled, int n,
+                       int S, int F, const int *row, const int *hops, cudaStream_t st) {
+  if (row) rows_stage_kernel<W, true><<<blocks, 256, 0, st>>>(dst, in, in_stride, in_width, n_scaled, n, S, F, row, hops);
+  else rows_stage_kernel<W, false><<<blocks, 256, 0, st>>>(dst, in, in_stride, in_width, n_scaled, n, S, F, nullptr, nullptr);
+}
 int launch_rows_stage(float *dst, int w, const float *in, size_t in_stride, int in_width, int n_scaled, int n_streams,
-                      int S, int n_frames, cudaStream_t st) {
+                      int S, int n_frames, cudaStream_t st, const int *row, const int *hops) {
   const unsigned blocks = copy_blocks((long long)n_frames * n_streams * w);
-  if (w == kFeat) rows_stage_kernel<kFeat><<<blocks, 256, 0, st>>>(dst, in, in_stride, in_width, n_scaled, n_streams, S, n_frames);
-  else rows_stage_kernel<68><<<blocks, 256, 0, st>>>(dst, in, in_stride, in_width, n_scaled, n_streams, S, n_frames);
+  if (w == kFeat) rows_stage<kFeat>(blocks, dst, in, in_stride, in_width, n_scaled, n_streams, S, n_frames, row, hops, st);
+  else rows_stage<68>(blocks, dst, in, in_stride, in_width, n_scaled, n_streams, S, n_frames, row, hops, st);
   return 1;
 }
 
+template <int W>
+static void rows_store(unsigned blocks, const float *src, float *out, size_t out_stride, int n, int S, int F, const int *slot,
+                       const int *hops, cudaStream_t st) {
+  if (slot) rows_store_kernel<W, true><<<blocks, 256, 0, st>>>(src, out, out_stride, n, S, F, slot, hops);
+  else rows_store_kernel<W, false><<<blocks, 256, 0, st>>>(src, out, out_stride, n, S, F, nullptr, nullptr);
+}
 int launch_rows_store(const float *src, int w, float *out, size_t out_stride, int n_streams, int S, int n_frames,
-                      cudaStream_t st) {
+                      cudaStream_t st, const int *slot, const int *hops) {
   const unsigned blocks = copy_blocks((long long)n_frames * n_streams * w);
-  if (w == kFeat) rows_store_kernel<kFeat><<<blocks, 256, 0, st>>>(src, out, out_stride, n_streams, S, n_frames);
-  else rows_store_kernel<68><<<blocks, 256, 0, st>>>(src, out, out_stride, n_streams, S, n_frames);
+  if (w == kFeat) rows_store<kFeat>(blocks, src, out, out_stride, n_streams, S, n_frames, slot, hops, st);
+  else rows_store<68>(blocks, src, out, out_stride, n_streams, S, n_frames, slot, hops, st);
   return 1;
 }
 

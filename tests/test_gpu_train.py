@@ -1,8 +1,10 @@
 """The trainer on the GPU (PNB_TRAIN_NETWORK): gradients against float64 autograd of the torch restatement
-(train_oracle), saturated outputs, padding, determinism, the launch count, Adam against torch.optim.Adam, non-finite
-gradients, a closed training loop, and the refusals."""
+(train_oracle), at small shapes and at the shapes training runs at, saturated outputs, padding, determinism, the bits
+of a call against the engine's shape, active range, stride and earlier calls, the launch count, Adam against
+torch.optim.Adam, non-finite gradients, a closed training loop, and the refusals."""
 import ctypes as C
 import os
+import time
 
 import numpy as np
 import pytest
@@ -59,29 +61,62 @@ def moderate_records(B, T, seed):
     return rec
 
 
-def check_against_float64(sd, rec, frames, label, lower=True):
+def ragged_frames(B, T, seed):
+    """One count in [1, T] per window, with window 0 ending mid-way, window 1 after one hop and window B - 1 at the end;
+    from B = 10 on, window 8 (the second row of recurrence warp 0) ends after one hop and window 9 (warp 1's second row)
+    at the end, so rows that share a warp end at different hops."""
+    fr = np.random.RandomState(seed).randint(1, T + 1, size=B)
+    fr[0], fr[1], fr[-1] = T // 2, 1, T
+    if B >= 10:
+        fr[8], fr[9] = 1, T
+    return [int(f) for f in fr]
+
+
+def conv2_saturation(sd, rec, chunk=16):
+    """The share of conv2's float32 outputs at exactly +-1 (on the GPU, TF32 off, `chunk` windows at a time)."""
+    m = O.model(sd, torch.float32, "cuda")
+    sat = 0.0
+    with torch.no_grad(), torch.backends.cudnn.flags(enabled=True, allow_tf32=False):
+        for c0 in range(0, rec.shape[0], chunk):
+            x = torch.from_numpy(O.features(rec[c0:c0 + chunk])).cuda()
+            y = m.fc(x).permute(0, 2, 1)
+            pre = m.conv2[0](m.conv1(y)[:, :, :-4])[:, :, :-2]
+            sat += float((torch.tanh(pre).abs() == 1).double().sum())
+    return sat / (rec.shape[0] * rec.shape[1] * 512)
+
+
+def check_against_float64(sd, rec, frames, label, lower=True, chunk=16):
     """Every one of the 30 parameter tensors (lower=False: all but fc, conv1 and conv2, whose errors are printed) within
-    |g - g64| / |g64| <= 1e-4 and max|g - g64| <= 1e-3 max|g64|, and the loss within 1e-6 of float64."""
+    |g - g64| / |g64| <= 1e-4 and max|g - g64| <= 1e-3 max|g64|, and the loss within 1e-6 of float64.  The float64
+    reference runs `chunk` windows per autograd pass, so that its memory stays bounded at 128 x 2000."""
     B, T = rec.shape[:2]
     eng = trainer(sd, B, T)
+    t0 = time.perf_counter()
     sums = eng.train_grad(rec, frames)
+    t_gpu = time.perf_counter() - t0
     g = grads_of(eng)
     eng.close()
-    L64, g64 = O.grads(sd, rec, frames, torch.float64, "cuda")
+    torch.cuda.reset_peak_memory_stats()
+    t0 = time.perf_counter()
+    L64, g64 = O.grads(sd, rec, frames, torch.float64, "cuda", chunk=chunk)
+    torch.cuda.synchronize()
+    t64 = time.perf_counter() - t0
     loss = loss_terms(sums.sum(0))["total"]
-    print(f"\n{label}: loss {loss:.9e} float64 {L64:.9e} rel {abs(loss - L64) / L64:.2e}")
+    print(f"\n{label}: loss {loss:.9e} float64 {L64:.9e} rel {abs(loss - L64) / L64:.2e}; trainer call {t_gpu:.3f} s, "
+          f"float64 autograd {t64:.1f} s ({chunk} windows per pass, peak {torch.cuda.max_memory_allocated() / 2**30:.1f} GiB)")
     assert abs(loss - L64) <= 1e-6 * abs(L64)
     err = {}
     for k, w in g64.items():
         assert np.all(np.isfinite(g[k])), k
         d = np.asarray(g[k], np.float64) - w
         err[k] = (np.linalg.norm(d) / max(np.linalg.norm(w), 1e-300), np.abs(d).max() / max(np.abs(w).max(), 1e-300))
-    for k in sorted(err, key=lambda k: -err[k][0])[:3]:
+    held = [k for k in err if lower or not k.startswith(LOWER)]
+    for k in sorted(held, key=lambda k: -err[k][0])[:3]:
         print(f"  {k}: |g - g64| / |g64| = {err[k][0]:.2e}, max|g - g64| / max|g64| = {err[k][1]:.2e}")
     for k in sorted(err):
         if k.startswith(LOWER) and not lower:
             print(f"  {k}: |g - g64| / |g64| = {err[k][0]:.2e} (|g64| = {np.linalg.norm(g64[k]):.2e})")
-    bad = {k: e for k, e in err.items() if not (e[0] <= 1e-4 and e[1] <= 1e-3) and (lower or not k.startswith(LOWER))}
+    bad = {k: err[k] for k in held if not (err[k][0] <= 1e-4 and err[k][1] <= 1e-3)}
     assert not bad, sorted((k, f"{e[0]:.1e}", f"{e[1]:.1e}") for k, e in bad.items())
     return g, g64
 
@@ -105,14 +140,90 @@ def test_gradients_against_float64_unsaturated(B, T, frames):
     """Records of moderate scale: conv2 stays out of saturation, and all 30 tensors are held to the bar."""
     rec = moderate_records(B, T, 110 + B)
     sd = synth_state_dict(1)
-    m = O.model(sd)
-    with torch.no_grad():
-        y = m.fc(torch.from_numpy(O.features(rec))).permute(0, 2, 1)
-        pre = m.conv2[0](m.conv1(y)[:, :, :-4])[:, :, :-2]
-    sat = float((torch.tanh(pre).abs() == 1).float().mean())
+    sat = conv2_saturation(sd, rec)
     print(f"\nconv2 outputs at +-1 in fp32: {sat:.2%}")
     assert sat < 0.01
     check_against_float64(sd, rec, frames, f"{B}x{T} quiet")
+
+
+# The shapes training runs at: the CLI's default batch (10 x 500) and tools/bench_train.py's 32 x 500 and 128 x 2000.
+# From 9 windows on, a warp of the recurrence kernels holds several rows (b = warp, warp + 8, ...), each with its own
+# carry and end hop; and the weight-gradient contractions cut their R = B x F rows into more parts (up to 64), the
+# 512 x 1536 GRU products into 2 slices of 128 000 rows at 128 x 2000.
+TRAINING_SHAPES = [(10, 500), (32, 500), (128, 2000)]
+
+
+@pytest.mark.parametrize("B,T", TRAINING_SHAPES, ids=["10x500", "32x500", "128x2000"])
+def test_gradients_against_float64_at_training_shapes(B, T):
+    """Moderate records (all 30 tensors held to the bar), ragged windows at 500 frames, full windows at 128 x 2000
+    (the longest contractions)."""
+    rec = moderate_records(B, T, 120 + B)
+    sd = synth_state_dict(1)
+    sat = conv2_saturation(sd, rec)
+    frames = ragged_frames(B, T, 130 + B) if T == 500 else None
+    print(f"\n{B}x{T}: conv2 outputs at +-1 in fp32: {sat:.2%}; frames {frames}")
+    assert sat < 0.01
+    check_against_float64(sd, rec, frames, f"{B}x{T} quiet")
+
+
+@pytest.mark.parametrize("B,T", [(10, 500), (128, 2000)], ids=["10x500", "128x2000"])
+def test_gradients_against_float64_at_training_shapes_generator_scale(B, T):
+    """Generator records at int16 scale, as test_gradients_against_float64: 24 tensors held, fc, conv1 and conv2
+    printed."""
+    rec = windows(B, T, 140 + B)
+    frames = ragged_frames(B, T, 150 + B) if T == 500 else None
+    check_against_float64(synth_state_dict(0), rec, frames, f"{B}x{T} generator scale", lower=False)
+
+
+def test_gradient_bits_depend_on_the_call_alone():
+    """A gradient call's loss sums and gradient are the same bits whatever the engine's n_streams and
+    max_frames_per_call, the record stride, the entry point and the calls before it: a 10 x 40 ragged call on the
+    active rows of a 16-stream, 48-frame engine (after 16 x 48 and 10 x 48 calls, whose rows reach past this call's)
+    equals the call on a fresh 10-stream, 40-frame engine, and so does the call at a padded stride (padding NaN and
+    1e30) through the device and the host entries."""
+    sd = synth_state_dict(1)
+    rec = moderate_records(10, 40, 160)
+    frames = ragged_frames(10, 40, 161)
+    ref = trainer(sd, 10, 40)
+    want_s = ref.train_grad(rec, frames)
+    want_g = ref.train_export("gradient")
+    ref.close()
+    assert np.all(np.isfinite(want_g)) and np.any(want_g != 0)
+
+    def same(sums, label):
+        g = eng.train_export("gradient")
+        ok_s = np.array_equal(np.asarray(sums).view(np.int64), want_s.view(np.int64))
+        ok_g = np.array_equal(g.view(np.int32), want_g.view(np.int32))
+        print(f"  {label}: loss sums {'identical' if ok_s else 'DIFFER'}, gradient "
+              f"{'identical' if ok_g else f'differs at {np.count_nonzero(g != want_g)} of {g.size}'}")
+        assert ok_s and ok_g, label
+
+    print()
+    eng = trainer(sd, 16, 48)
+    eng.train_grad(moderate_records(16, 48, 162), ragged_frames(16, 48, 163))
+    eng.set_active(10)
+    same(eng.train_grad(rec, frames), "16 x 48 engine, active 10, after a 16 x 48 call")
+    eng.train_grad(moderate_records(10, 48, 164))
+    same(eng.train_grad(rec, frames), "after a 10 x 48 call")
+    eng.set_active(16)
+    eng.train_grad(moderate_records(16, 48, 165))
+    eng.set_active(10)
+    same(eng.train_grad(rec, frames), "after another 16 x 48 call")
+    stride = 40 * 138 + 7
+    padded = np.empty((10, stride), np.float32)
+    padded[:, 40 * 138::2], padded[:, 40 * 138 + 1::2] = np.nan, 1e30
+    padded[:, :40 * 138] = rec.reshape(10, -1)
+    d_rec = torch.from_numpy(padded).cuda()
+    d_sums = torch.empty((10, 4), dtype=torch.float64, device="cuda")
+    s = torch.cuda.Stream()
+    eng.train_grad_device(d_rec.data_ptr(), stride, 40, frames, d_sums.data_ptr(), s.cuda_stream)
+    eng.check(s.cuda_stream)
+    same(d_sums.cpu().numpy(), f"device entry, stride {stride}")
+    fr = np.asarray(frames, np.int32)
+    sums = np.empty((10, 4), np.float64)
+    assert eng.L.pnb_train_grad_host(eng.h, padded.ctypes.data, stride, 40, fr.ctypes.data, sums.ctypes.data) == 0
+    same(sums, f"host entry, stride {stride}")
+    eng.close()
 
 
 def test_saturated_outputs_are_finite():

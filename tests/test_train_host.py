@@ -124,3 +124,72 @@ def test_adam_restatement_is_torch():
         assert not np.any((t.detach().numpy() != p) & rounded), step
         assert bits_equal(st["exp_avg"].numpy(), m) and bits_equal(st["exp_avg_sq"].numpy(), v), step
         p = t.detach().numpy().copy()
+
+
+# ---- the training CLI's host side (percepnet_b200.train)
+
+def write_records(path, frames, seed):
+    rec = records(1, frames, seed)[0]
+    rec.astype("<f4").tofile(path)
+    return rec
+
+
+def test_windows_of_cuts_files_into_windows(tmp_path):
+    """Each file is cut into --window-frame windows in file order; a file's last window is shorter, zero-padded, and
+    counts only its own frames."""
+    from percepnet_b200.train import windows_of
+    a = write_records(tmp_path / "a.f32", 7, 20)
+    b = write_records(tmp_path / "b.f32", 3, 21)
+    c = write_records(tmp_path / "c.f32", 6, 22)
+    x, frames = windows_of([str(tmp_path / n) for n in ("a.f32", "b.f32", "c.f32")], 3)
+    assert x.shape == (6, 3, 138) and x.dtype == np.float32
+    assert frames.dtype == np.int32 and frames.tolist() == [3, 3, 1, 3, 3, 3]
+    for i, w in enumerate([a[0:3], a[3:6], a[6:7], b[0:3], c[0:3], c[3:6]]):
+        assert bits_equal(x[i, :len(w)], w), i
+    assert not np.any(x[2, 1:])
+
+
+def test_batches_are_seeded_full_and_reshuffled():
+    """Full batches only (the remainder of an epoch is dropped), each epoch a permutation of its own, the same for the
+    same seed."""
+    from percepnet_b200.train import batches
+    it = batches(11, 3, 5)
+    first = [next(it) for _ in range(9)]
+    assert [e for e, _ in first] == [0, 0, 0, 1, 1, 1, 2, 2, 2]
+    for e in range(3):
+        got = np.concatenate([idx for ep, idx in first if ep == e])
+        assert all(len(idx) == 3 for ep, idx in first if ep == e)
+        assert len(set(got.tolist())) == 9 and got.min() >= 0 and got.max() < 11
+        assert got.tolist() == np.random.default_rng([5, e]).permutation(11)[:9].tolist()
+    assert first[0][1].tolist() != first[3][1].tolist() or first[1][1].tolist() != first[4][1].tolist()
+    again = batches(11, 3, 5)
+    assert all(np.array_equal(next(again)[1], idx) for _, idx in first)
+    other = batches(11, 3, 6)
+    assert any(not np.array_equal(next(other)[1], idx) for _, idx in first)
+
+
+@pytest.mark.parametrize("extra", [["--window", "0"], ["--batch", "0"], ["--steps", "-1"], ["--lr", "nan"],
+                                   ["--lr", "-1e-4"], ["--lr", "inf"], ["--dev-list", "dev.txt"]],
+                         ids=["window0", "batch0", "steps-1", "lr_nan", "lr_negative", "lr_inf", "dev_without_every"])
+def test_parse_args_refusals(extra, capsys):
+    from percepnet_b200.train import parse_args
+    base = ["--list", "l.txt", "--steps", "1", "--out", "o.pnbw"]
+    a = parse_args(base)
+    assert (a.window, a.batch, a.lr, a.seed) == (500, 10, 1e-4, 0)
+    with pytest.raises(SystemExit) as ex:
+        parse_args(base + extra)
+    assert ex.value.code == 2
+    assert "error" in capsys.readouterr().err
+
+
+def test_fewer_windows_than_the_batch(tmp_path, capsys):
+    """Two files of 5 and 3 frames at --window 4 are three windows: --batch 4 returns 2 before any engine exists."""
+    from percepnet_b200 import train
+    for name, n in (("a.f32", 5), ("b.f32", 3)):
+        write_records(tmp_path / name, n, 23)
+    lst = tmp_path / "list.txt"
+    lst.write_text(f"{tmp_path / 'a.f32'}\n\n{tmp_path / 'b.f32'}\n")
+    out = tmp_path / "o.pnbw"
+    assert train.main(["--list", str(lst), "--window", "4", "--batch", "4", "--steps", "1", "--out", str(out)]) == 2
+    assert "3 windows, fewer than --batch 4" in capsys.readouterr().err
+    assert not out.exists()

@@ -72,18 +72,32 @@ def loss(out, y, frames=None):
     return (dg * w).sum() / n + C4 * (dg4 * w).sum() / n + (dr * w).sum() / n
 
 
-def grads(sd: dict, rec: np.ndarray, frames=None, dtype=torch.float64, device="cpu"):
-    """(loss, {state_dict name: gradient as numpy}) of the records' windows, by autograd in `dtype`."""
+def grads(sd: dict, rec: np.ndarray, frames=None, dtype=torch.float64, device="cpu", chunk=None):
+    """(loss, {state_dict name: gradient as numpy}) of the records' windows, by autograd in `dtype`.  chunk: windows
+    per autograd pass (None: all in one).  The loss is a mean over every counted hop x 34 bands of the whole batch, so
+    chunk c's loss is its own mean times count_c / count_total; the passes' gradients add up in .grad."""
     m = model(sd, dtype, device)
-    x = features(rec)
-    if frames is not None:
-        for b, f in enumerate(frames):
-            x[b, f:] = 0
-    xt = torch.from_numpy(x).to(device=device, dtype=dtype)
-    y = torch.from_numpy(np.ascontiguousarray(rec[..., 70:])).to(device=device, dtype=dtype)
-    L = loss(m(xt), y, frames)
-    L.backward()
-    return float(L), {k: p.grad.detach().cpu().numpy() for k, p in m.named_parameters()}
+    B, T = rec.shape[:2]
+    chunk = chunk or B
+    counts = np.full(B, T, np.int64) if frames is None else np.asarray(frames, np.int64)
+    total = float(counts.sum())
+    L = 0.0
+    for c0 in range(0, B, chunk):
+        part = slice(c0, min(B, c0 + chunk))
+        fr = None if frames is None else [int(f) for f in counts[part]]
+        x = features(rec[part])
+        if fr is not None:
+            for b, f in enumerate(fr):
+                x[b, f:] = 0
+        xt = torch.from_numpy(x).to(device=device, dtype=dtype)
+        y = torch.from_numpy(np.ascontiguousarray(rec[part, :, 70:])).to(device=device, dtype=dtype)
+        Lc = loss(m(xt), y, fr)
+        if chunk < B:
+            Lc = Lc * (float(counts[part].sum()) / total)
+        Lc.backward()
+        L += float(Lc.detach())
+        del xt, y, Lc
+    return L, {k: p.grad.detach().cpu().numpy() for k, p in m.named_parameters()}
 
 
 def dloss_dpre(p: np.ndarray, y: np.ndarray, count: int) -> np.ndarray:

@@ -7,8 +7,10 @@ Exercises the fp32 path, the tensor path (one CTA pair's worth of streams), the 
 the pipelined host entry, the training-data generator (records alone and with its audio), the persistent fp32 GRU chain (both block sizes), submitted
 calls on the chain's anti-diagonal unit order, state export / import, a session-pool schedule (parks, unparks,
 relocations, fresh starts, session export / import / reset), ragged session calls (sessions that stop early, across the
-history slide and the fp32 network's 32-hop chunk), network-only calls on features and on records (both network modes)
-and the pitch-only kernel on tiny batches; prints a checksum per leg."""
+history slide and the fp32 network's 32-hop chunk), network-only calls on features and on records (both network modes),
+the pitch-only kernel on tiny batches and the network trainer (ten windows, more than a recurrence CTA's eight warps,
+on an active range, a call shorter than max_frames_per_call, ragged frames, then one Adam step); prints a checksum per
+leg."""
 import os
 import sys
 
@@ -17,11 +19,11 @@ import numpy as np
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from percepnet_b200 import api  # noqa: E402
 from percepnet_b200.synth import synth_pairs, synth_pcm, to_int16  # noqa: E402
-from percepnet_b200.weights import synth_model  # noqa: E402
+from percepnet_b200.weights import pack_state_dict, synth_model, synth_state_dict  # noqa: E402
 
 
 def main():
-    legs = sys.argv[1:] or ["fp32", "tensor", "train", "fp32chain", "submit", "sessions", "ragged", "rnn", "pitch"]
+    legs = sys.argv[1:] or ["fp32", "tensor", "train", "fp32chain", "submit", "sessions", "ragged", "rnn", "pitch", "trainnet"]
     m = synth_model(0)
     if "fp32" in legs:
         x = synth_pcm(5, 4, seed=3)
@@ -124,6 +126,18 @@ def main():
         r4, a4 = e.train_audio(c[:, 5 * 480:], n[:, 5 * 480:])
         print("train_audio", float(r3.sum()), float(r4.sum()), int(np.abs(a3.astype(np.int64)).sum()),
               int(np.abs(a4.astype(np.int64)).sum()))
+        e.close()
+    if "trainnet" in legs:   # 12 slots, 10 active, F = 6 of Fmax 8, windows ending after 1 to 6 hops
+        rng = np.random.RandomState(18)
+        rec = rng.rand(10, 6, 138).astype(np.float32)
+        rec[..., :68] *= np.float32(0.05)
+        e = api.Engine(12, 8, pack_state_dict(synth_state_dict(0)), api.TRAIN_NETWORK)
+        e.set_active(10)
+        sums = e.train_grad(rec, [3, 6, 1, 6, 2, 5, 4, 6, 1, 6])
+        e.train_adam(1e-3, 1)
+        e.wait()
+        print("trainnet", float(sums.sum()), float(np.abs(e.train_export("gradient").astype(np.float64)).sum()),
+              float(e.train_export("weights").astype(np.float64).sum()))
         e.close()
 
 

@@ -288,12 +288,35 @@ int pnb_score_records_host(pnb_engine *e, const float *rec, size_t rec_stride, i
  *   pnb_train_export / pnb_train_import  one array as a flat float32 vector in PNBW blob order (the ten layers in
  *                     RNNModel order, each layer's weights, recurrent weights, bias; 7 962 564 floats): the weights, the
  *                     gradient (export only) or Adam's m or v.  Both wait for the engine's earlier work and return when
- *                     the copy is complete; export needs bytes >= the vector, import exactly the vector. */
-enum { PNB_TRAIN_WEIGHTS = 0, PNB_TRAIN_GRADIENT = 1, PNB_TRAIN_ADAM_M = 2, PNB_TRAIN_ADAM_V = 3 };
+ *                     the copy is complete; export needs bytes >= the vector, import exactly the vector.
+ *
+ * Accumulation (micro-batches on one engine, and data-parallel ranks): one Adam step on the gradient of a batch larger
+ * than one call.  A gradient call's gradient g_k is the mean over its own c_k counted hops (c_k = the sum of its
+ * frames), so the batch's is g = sum_k c_k g_k / sum_k c_k: the weight is the hops, not the windows.
+ *   pnb_train_accumulate  A += (double)g_k * c_k and C += c_k, into an accumulator of N + 1 float64 values (N = 7 962 564
+ *                     parameters, C last), asynchronous on cuda_stream and ordered like a call.  The accumulator (64 MB)
+ *                     is allocated on its first use and counted by pnb_engine_bytes.
+ *   pnb_train_finish  the held gradient becomes (float)(A / C), the accumulator is zeroed, and the gradient is checked
+ *                     as a gradient call's is: a non-finite value (a NaN from any part of the batch reaches A) skips the
+ *                     next Adam step on the device and raises PNB_ERR_DOMAIN.  Asynchronous, ordered like a call.
+ *   PNB_TRAIN_ACCUM   pnb_train_export / pnb_train_import of the accumulator: N + 1 float64 values, in host memory or in
+ *                     device memory of the engine's device (copied with cudaMemcpyDefault), so that ranks can sum it
+ *                     with an all-reduce (NCCL on a device buffer, or any host collective) and import the sum; export
+ *                     needs bytes >= (N + 1) x 8, import exactly that.  An import counts as accumulated.
+ * Exactness: g_k c_k is exact in float64 (a 24-bit mantissa times c_k < 2^29), so one call accumulated and finished is
+ * its own gradient bit for bit, and two contributions sum to the same bits in either order: two ranks of one call each
+ * equal one engine accumulating both calls.  Refused with PNB_ERR_ARG, before anything is enqueued and with weights,
+ * moments and accumulator as they were: pnb_train_accumulate with no gradient call since the last accumulate or
+ * finish (it would count a gradient twice); pnb_train_finish with nothing accumulated or imported since the last
+ * finish; pnb_train_adam while accumulated gradients are not finished (it would step on part of the batch); all of
+ * them on engines without PNB_TRAIN_NETWORK.  pnb_reset empties the accumulator and keeps the held gradient. */
+enum { PNB_TRAIN_WEIGHTS = 0, PNB_TRAIN_GRADIENT = 1, PNB_TRAIN_ADAM_M = 2, PNB_TRAIN_ADAM_V = 3, PNB_TRAIN_ACCUM = 4 };
 int pnb_train_grad_host(pnb_engine *e, const float *rec, size_t rec_stride, int n_frames, const int *frames, double *sums);
 int pnb_train_grad_device(pnb_engine *e, const float *d_rec, size_t rec_stride, int n_frames, const int *frames,
                           double *d_sums, void *cuda_stream);
 int pnb_train_adam(pnb_engine *e, double lr, long long step, void *cuda_stream);
+int pnb_train_accumulate(pnb_engine *e, void *cuda_stream);
+int pnb_train_finish(pnb_engine *e, void *cuda_stream);
 int pnb_train_export(pnb_engine *e, int what, void *dst, size_t bytes);
 int pnb_train_import(pnb_engine *e, int what, const void *src, size_t bytes);
 

@@ -21,7 +21,7 @@ FRAME = 480
 NN_FP32, NN_TENSOR, POSTFILTER, KEEP_TAPS, TRAIN_DATA, CONV_WIDE, TRAIN_AUDIO, NETWORK_ONLY = 0, 1, 2, 4, 8, 16, 32, 64
 SIGNAL_ONLY = 128
 TRAIN_NETWORK = 256
-TRAIN_ARRAYS = {"weights": 0, "gradient": 1, "m": 2, "v": 3}   # pnb_train_export / pnb_train_import
+TRAIN_ARRAYS = {"weights": 0, "gradient": 1, "m": 2, "v": 3, "accum": 4}   # pnb_train_export / pnb_train_import
 RECORD = 138
 RNN_FEATURES, RNN_RECORDS = 0, 1   # pnb_compute_rnn_* formats: 70 features or 138 record floats per hop
 TAPS = {"features": (0, np.float32, 70), "pitch": (1, np.int32, 4), "pitchf": (2, np.float32, 2),
@@ -77,6 +77,8 @@ def load_library() -> C.CDLL:
     L.pnb_train_grad_host.argtypes = [vp, vp, sz, i, vp, vp]
     L.pnb_train_grad_device.argtypes = [vp, vp, sz, i, vp, vp, vp]
     L.pnb_train_adam.argtypes = [vp, C.c_double, C.c_longlong, vp]
+    L.pnb_train_accumulate.argtypes = [vp, vp]
+    L.pnb_train_finish.argtypes = [vp, vp]
     L.pnb_train_export.argtypes = [vp, i, vp, sz]
     L.pnb_train_import.argtypes = [vp, i, vp, sz]
     L.pnb_engine_bytes.argtypes = [vp]
@@ -139,7 +141,8 @@ EXPORTS = ("pnb_create", "pnb_destroy", "pnb_reset", "pnb_resolve_device", "pnb_
            "pnb_compute_rnn_device", "pnb_compute_rnn_host", "pnb_score_records_device", "pnb_score_records_host",
            "pnb_analyze_host_f32", "pnb_analyze_host_i16", "pnb_analyze_device_f32", "pnb_analyze_device_i16",
            "pnb_synthesize_host_f32", "pnb_synthesize_host_i16", "pnb_synthesize_device_f32", "pnb_synthesize_device_i16",
-           "pnb_train_grad_host", "pnb_train_grad_device", "pnb_train_adam", "pnb_train_export", "pnb_train_import",
+           "pnb_train_grad_host", "pnb_train_grad_device", "pnb_train_adam", "pnb_train_accumulate", "pnb_train_finish",
+           "pnb_train_export", "pnb_train_import",
            "pnb_engine_bytes",
            "pnb_read_tap", "pnb_state_size", "pnb_get_state", "pnb_set_state",
            "pnb_reset_streams", "pnb_export_states", "pnb_import_states", "pnb_set_active_streams", "pnb_active_streams",
@@ -365,18 +368,38 @@ class Engine:
         from 1.  Skipped on the device when that gradient was not finite."""
         self._ck(self.L.pnb_train_adam(self.h, float(lr), int(step), stream or None), "pnb_train_adam")
 
+    def train_accumulate(self, stream: int = 0):
+        """pnb_train_accumulate: the gradient of the last train_grad, weighted by the hops it counted, into the engine's
+        float64 accumulator (micro-batches and ranks summed before one train_adam)."""
+        self._ck(self.L.pnb_train_accumulate(self.h, stream or None), "pnb_train_accumulate")
+
+    def train_finish(self, stream: int = 0):
+        """pnb_train_finish: the accumulated batch's gradient (sum c_k g_k / sum c_k) becomes the held gradient for
+        train_adam, and the accumulator is emptied."""
+        self._ck(self.L.pnb_train_finish(self.h, stream or None), "pnb_train_finish")
+
     def train_export(self, what: str) -> np.ndarray:
         """pnb_train_export: 'weights', 'gradient', 'm' or 'v' as one float32 vector in PNBW blob order
-        (weights.PackedModel.from_flat turns it into a model)."""
+        (weights.PackedModel.from_flat turns it into a model), or 'accum', the accumulator's N + 1 float64 values."""
         from .weights import N_PARAMS
-        a = np.empty(N_PARAMS, np.float32)
+        a = np.empty(N_PARAMS + 1, np.float64) if what == "accum" else np.empty(N_PARAMS, np.float32)
         self._ck(self.L.pnb_train_export(self.h, TRAIN_ARRAYS[what], a.ctypes.data, a.nbytes), "pnb_train_export")
         return a
 
     def train_import(self, what: str, a: np.ndarray):
-        """pnb_train_import: 'weights', 'm' or 'v' from a flat float32 vector in PNBW blob order (resuming a run)."""
-        a = np.ascontiguousarray(a, np.float32)
+        """pnb_train_import: 'weights', 'm' or 'v' from a flat float32 vector in PNBW blob order (resuming a run), or
+        'accum' from N + 1 float64 values (a sum of several engines' accumulators)."""
+        a = np.ascontiguousarray(a, np.float64 if what == "accum" else np.float32)
         self._ck(self.L.pnb_train_import(self.h, TRAIN_ARRAYS[what], a.ctypes.data, a.nbytes), "pnb_train_import")
+
+    def train_export_ptr(self, what: str, ptr: int, nbytes: int):
+        """pnb_train_export into raw memory: 'accum' may be device memory of the engine's device (a torch CUDA tensor's
+        data_ptr(), N + 1 float64), the other arrays host memory.  Returns when the copy is complete."""
+        self._ck(self.L.pnb_train_export(self.h, TRAIN_ARRAYS[what], ptr or None, nbytes), "pnb_train_export")
+
+    def train_import_ptr(self, what: str, ptr: int, nbytes: int):
+        """pnb_train_import from raw memory, as train_export_ptr."""
+        self._ck(self.L.pnb_train_import(self.h, TRAIN_ARRAYS[what], ptr or None, nbytes), "pnb_train_import")
 
     def analyze(self, x: np.ndarray) -> np.ndarray:
         """pnb_analyze_host_*: the analysis half of process.  x: [active, F*480] float32 (C-API scale) or int16 (CLI wire

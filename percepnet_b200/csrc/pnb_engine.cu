@@ -326,6 +326,7 @@ extern "C" int pnb_reset(pnb_engine *e) {
   e->pend_up.clear();
   e->n_active = e->S;
   e->poisoned = false;
+  e->train_open = false;  // the accumulator (stream state) was zeroed above; the held gradient stays, and stays due
   if (e->sessions) {  // every session fresh: all parked, every blob marked fresh
     CK(cudaMemset(e->d_park, 0, (size_t)e->pool.capacity() * kParkStride));
     e->pool.init(e->S, e->pool.capacity());
@@ -1182,8 +1183,9 @@ static int report_status(pnb_engine *e) {
                              "tensor-mode engine); lowest rejected stream %d, left reset like every rejected one", slot);
   }
   if ((e->h_status[0] & 1) && (e->flags & PNB_TRAIN_NETWORK))
-    return fail(PNB_ERR_DOMAIN, "a pnb_train_grad_* call met a non-finite gradient (non-finite records inside a window, or "
-                                "non-finite weights); the Adam step after it was skipped.  Sticky until pnb_reset");
+    return fail(PNB_ERR_DOMAIN, "a pnb_train_grad_* call or pnb_train_finish met a non-finite gradient (non-finite records "
+                                "inside a window, non-finite weights, or a non-finite imported accumulator); the Adam step "
+                                "after it was skipped.  Sticky until pnb_reset");
   if (e->h_status[0] & 1)
     return fail(PNB_ERR_DOMAIN, "tensor path: a pre-activation left the domain of the reference's tansig_approx (|x| >= 8.5e7, "
                                 "src/vec.h:63 is undefined there); results since the last pnb_reset are not the reference's -- "
@@ -1347,28 +1349,64 @@ extern "C" int pnb_train_adam(pnb_engine *e, double lr, long long step, void *cu
   { int rc = check_trainer(e); if (rc) return rc; }
   if (!(lr >= 0.0) || !isfinite(lr)) return fail(PNB_ERR_ARG, "lr = %g is not a finite number >= 0", lr);
   if (step < 1) return fail(PNB_ERR_ARG, "step = %lld, Adam counts steps from 1", step);
+  if (e->train_open)
+    return fail(PNB_ERR_ARG, "accumulated gradients are not finished: pnb_train_finish before pnb_train_adam");
   CK(cudaSetDevice(e->device));
   const int n = enqueue_ordered(e, (cudaStream_t)cuda_stream, [&] { return train_adam(e, lr, step, (cudaStream_t)cuda_stream); });
   return n < 0 ? n : PNB_OK;
 }
 
-// Export / import of the trainer's arrays as one flat float32 vector in PNBW blob order; both wait for the engine's
-// earlier work and finish before they return.
-static int train_transfer(pnb_engine *e, int what, void *host, size_t bytes, bool to_host) {
+// Accumulation: the held gradient, weighted by the hops its call counted, into the float64 accumulator; and the
+// accumulated batch's gradient back into the held gradient.  Each refuses what would count a gradient twice or step
+// on a part of the batch, before anything is enqueued.
+extern "C" int pnb_train_accumulate(pnb_engine *e, void *cuda_stream) {
   { int rc = check_trainer(e); if (rc) return rc; }
-  if (!host) return fail(PNB_ERR_ARG, "%s is NULL", to_host ? "dst" : "src");
-  if (what < PNB_TRAIN_WEIGHTS || what > PNB_TRAIN_ADAM_V) return fail(PNB_ERR_ARG, "what = %d is not a PNB_TRAIN_* array", what);
-  if (!to_host && what == PNB_TRAIN_GRADIENT) return fail(PNB_ERR_ARG, "the gradient is computed, not imported");
-  const size_t need = train_params(e) * sizeof(float);
-  if (to_host ? bytes < need : bytes != need)
+  if (!e->train_hops)
+    return fail(PNB_ERR_ARG, "no pnb_train_grad_* call since the last pnb_train_accumulate or pnb_train_finish: the "
+                             "held gradient is already counted");
+  CK(cudaSetDevice(e->device));
+  { int rc = train_accum_prepare(e); if (rc) return rc; }
+  const int n = enqueue_ordered(e, (cudaStream_t)cuda_stream, [&] { return train_accumulate(e, (cudaStream_t)cuda_stream); });
+  if (n < 0) return n;
+  e->train_hops = 0;
+  e->train_open = true;
+  return PNB_OK;
+}
+extern "C" int pnb_train_finish(pnb_engine *e, void *cuda_stream) {
+  { int rc = check_trainer(e); if (rc) return rc; }
+  if (!e->train_open)
+    return fail(PNB_ERR_ARG, "nothing was accumulated or imported since the last pnb_train_finish");
+  CK(cudaSetDevice(e->device));
+  const int n = enqueue_ordered(e, (cudaStream_t)cuda_stream, [&] { return train_finish(e, (cudaStream_t)cuda_stream); });
+  if (n < 0) return n;
+  e->train_hops = 0;
+  e->train_open = false;
+  return PNB_OK;
+}
+
+// Export / import of the trainer's arrays: weights, gradient, m and v as one flat float32 vector in PNBW blob order
+// in host memory; the accumulator as its N + 1 doubles in host memory or device memory of the engine's device.  Both
+// wait for the engine's earlier work and finish before they return.
+static int train_transfer(pnb_engine *e, int what, void *mem, size_t bytes, bool out) {
+  { int rc = check_trainer(e); if (rc) return rc; }
+  if (!mem) return fail(PNB_ERR_ARG, "%s is NULL", out ? "dst" : "src");
+  if (what < PNB_TRAIN_WEIGHTS || what > PNB_TRAIN_ACCUM) return fail(PNB_ERR_ARG, "what = %d is not a PNB_TRAIN_* array", what);
+  if (!out && what == PNB_TRAIN_GRADIENT) return fail(PNB_ERR_ARG, "the gradient is computed, not imported");
+  const bool accum = what == PNB_TRAIN_ACCUM;
+  const size_t need = accum ? (train_params(e) + 1) * sizeof(double) : train_params(e) * sizeof(float);
+  if ((out ? bytes < need : bytes != need) && accum)
+    return fail(PNB_ERR_ARG, "%zu bytes, the accumulator is %zu doubles (%zu bytes)", bytes, train_params(e) + 1, need);
+  if (out ? bytes < need : bytes != need)
     return fail(PNB_ERR_ARG, "%zu bytes, the model has %zu parameters (%zu bytes)", bytes, train_params(e), need);
   CK(cudaSetDevice(e->device));
+  if (accum) { int rc = train_accum_prepare(e); if (rc) return rc; }
   const int n = enqueue_ordered(e, e->stream, [&] {
-    const int rc = train_copy(e, what, host, to_host, e->stream);
+    const int rc = accum ? train_accum_copy(e, mem, out, e->stream) : train_copy(e, what, mem, out, e->stream);
     return rc ? rc : 0;
   });
   if (n < 0) return n;
   CK(cudaStreamSynchronize(e->stream));
+  if (accum && !out) e->train_open = true;
   return PNB_OK;
 }
 extern "C" int pnb_train_export(pnb_engine *e, int what, void *dst, size_t bytes) { return train_transfer(e, what, dst, bytes, true); }

@@ -77,6 +77,10 @@ struct pnb_engine {
   std::shared_ptr<pnb_tc_state> tc;
   std::shared_ptr<pnb_f32_state> f32;
   std::shared_ptr<pnb_train_state> train;
+  // PNB_TRAIN_NETWORK accumulation: the hops the held gradient counted while no pnb_train_accumulate has taken it yet
+  // (0: none, or taken), and whether the accumulator holds anything (accumulated or imported) not yet finished
+  long long train_hops = 0;
+  bool train_open = false;
   int last_frames = 0;
   // hops of an analysis (pnb_analyze_*) whose synthesis (pnb_synthesize_*) is still due, or 0.  Between the two halves
   // the analysed streams are mid-hop, so every call and state operation but the synthesis and network calls is refused.
@@ -171,7 +175,10 @@ int f32_state_segs(const pnb_engine *e, pnb::StateSeg *seg, int ns);
 // PNB_TRAIN_NETWORK (pnb_train.cu).  prepare: after f32_prepare, the trainer's buffers.  grad: the loss sums and the
 // gradient of a call of F hops on windows [0, n_active) (records on the device; frames: device / host copies of the
 // hops per window, or null), returns its launch count.  adam: one step with the held gradient.  copy: what = 0 weights,
-// 1 gradient, 2 m, 3 v between the device and train_params(e) floats of host memory, on st.
+// 1 gradient, 2 m, 3 v between the device and train_params(e) floats of host memory, on st.  accum_prepare: the
+// float64 accumulator, allocated once; accumulate: the held gradient times e->train_hops into it (1 launch); finish:
+// the gradient from it, the accumulator zeroed, and the non-finite check (2 launches); accum_copy: its
+// train_params(e) + 1 doubles to (out) or from mem, host or device memory, on st.
 int f32_params(const pnb_engine *e, float **p, size_t *count);
 int train_prepare(pnb_engine *e);
 int train_grad(pnb_engine *e, const float *rec, size_t rec_stride, const int *frames, const int *h_frames, double *sums,
@@ -180,6 +187,10 @@ int train_grad_launches(const pnb_engine *e);
 int train_adam(pnb_engine *e, double lr, long long step, cudaStream_t st);
 int train_copy(pnb_engine *e, int what, void *host, bool to_host, cudaStream_t st);
 size_t train_params(const pnb_engine *e);
+int train_accum_prepare(pnb_engine *e);
+int train_accumulate(pnb_engine *e, cudaStream_t st);
+int train_finish(pnb_engine *e, cudaStream_t st);
+int train_accum_copy(pnb_engine *e, void *mem, bool out, cudaStream_t st);
 
 // RAII marker used by the launch schedule: records an event pair around a launch when profiling
 struct ProfScope {

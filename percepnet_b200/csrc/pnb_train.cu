@@ -14,6 +14,9 @@
 //            (split over the rows into a fixed number of parts, then summed part by part in order).
 //   check    one pass over the gradient: a non-finite value raises the engine's domain bit and makes the next Adam
 //            step a no-op on the device
+// Between gradient calls and Adam, pnb_train_accumulate / pnb_train_finish sum several calls' gradients (micro-batches,
+// or ranks through an exported accumulator) in float64, weighted by their counted hops (train_accum_kernel,
+// train_finish_kernel), and the check runs again on the sum.
 // No floating-point atomics anywhere: every sum has one fixed order, so a call's loss and gradient are the same bits
 // whatever stream it runs on.
 #include <math.h>
@@ -335,6 +338,47 @@ __global__ void train_check_kernel(const float *__restrict__ g, size_t n, int *b
   }
 }
 
+// Accumulation of several gradient calls (micro-batches, or ranks) before one Adam step, in float64: each call's
+// gradient g_k carries 1/c_k (c_k its counted hops), so the batch's is sum c_k g_k / sum c_k.  acc[i] += g[i] * c for
+// i < n, acc[n] += c.  g * c is exact in float64 (24-bit mantissa, c < 2^29), so one call finishes to its own bits and
+// two add to the same bits in either order.  Four values per thread (n is the model's 7 962 564, a multiple of 4; the
+// tail loop covers any other n).
+__global__ void train_accum_kernel(const float *__restrict__ g, size_t n, double c, double *__restrict__ acc) {
+  const size_t n4 = n / 4, stride = (size_t)gridDim.x * blockDim.x, tid = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const float4 *g4 = reinterpret_cast<const float4 *>(g);
+  double2 *a2 = reinterpret_cast<double2 *>(acc);
+  for (size_t i = tid; i < n4; i += stride) {
+    const float4 v = __ldg(g4 + i);
+    double2 lo = a2[2 * i], hi = a2[2 * i + 1];
+    lo.x = __dadd_rn(lo.x, __dmul_rn((double)v.x, c)); lo.y = __dadd_rn(lo.y, __dmul_rn((double)v.y, c));
+    hi.x = __dadd_rn(hi.x, __dmul_rn((double)v.z, c)); hi.y = __dadd_rn(hi.y, __dmul_rn((double)v.w, c));
+    a2[2 * i] = lo;
+    a2[2 * i + 1] = hi;
+  }
+  for (size_t i = 4 * n4 + tid; i < n; i += stride) acc[i] = __dadd_rn(acc[i], __dmul_rn((double)g[i], c));
+  if (tid == 0) acc[n] = __dadd_rn(acc[n], c);
+}
+
+// g[i] = (float)(acc[i] / acc[n]) and acc[i] = 0 for i < n; acc[n] is read by every thread, so the caller zeroes it
+// after this launch
+__global__ void train_finish_kernel(double *__restrict__ acc, size_t n, float *__restrict__ g) {
+  const double C = acc[n];
+  const size_t n4 = n / 4, stride = (size_t)gridDim.x * blockDim.x, tid = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  float4 *g4 = reinterpret_cast<float4 *>(g);
+  double2 *a2 = reinterpret_cast<double2 *>(acc);
+  const double2 zero = make_double2(0.0, 0.0);
+  for (size_t i = tid; i < n4; i += stride) {
+    const double2 lo = a2[2 * i], hi = a2[2 * i + 1];
+    g4[i] = make_float4((float)__ddiv_rn(lo.x, C), (float)__ddiv_rn(lo.y, C), (float)__ddiv_rn(hi.x, C), (float)__ddiv_rn(hi.y, C));
+    a2[2 * i] = zero;
+    a2[2 * i + 1] = zero;
+  }
+  for (size_t i = 4 * n4 + tid; i < n; i += stride) {
+    g[i] = (float)__ddiv_rn(acc[i], C);
+    acc[i] = 0.0;
+  }
+}
+
 struct AdamArgs {
   float *p[kParams];
   size_t off[kParams + 1];
@@ -382,6 +426,7 @@ struct pnb_train_state {
   size_t off[kParams + 1];
   float *grad = nullptr, *m = nullptr, *v = nullptr;  // [N] flat, blob order
   float *part = nullptr;                               // partial sums of the split weight-gradient contractions
+  double *acc = nullptr;                               // [N + 1] accumulated gradients and their hops, on first use
   int *bad = nullptr;
   unsigned *cnt = nullptr;                             // [10] counters of the recurrences, zeroed per call
   // activations and gradients of one call, rows r = t*n + b; sized for S windows x Fmax hops
@@ -701,6 +746,7 @@ int train_grad(pnb_engine *e, const float *rec, size_t rec_stride, const int *fr
   TCK(L.err);
   // pnb_launches_per_call reports train_grad_launches: the schedule above and that count must agree
   if (L.n != train_grad_launches(e)) return engine_fail(PNB_ERR_CUDA, "train_grad issued a launch count train_grad_launches does not know");
+  e->train_hops = counted;
   return L.n;
 }
 
@@ -747,3 +793,41 @@ int train_copy(pnb_engine *e, int what, void *host, bool to_host, cudaStream_t s
 }
 
 size_t train_params(const pnb_engine *e) { return e->train ? e->train->off[kParams] : 0; }
+
+// The accumulator, allocated (zeroed, and zeroed again by pnb_reset) the first time an accumulation, export or import
+// needs it: engines that never accumulate do not carry its 64 MB.  engine_alloc's zeroing runs on the legacy stream,
+// so the device is synchronised once before any stream of the engine's may touch the buffer.
+int train_accum_prepare(pnb_engine *e) {
+  pnb_train_state &s = *e->train;
+  if (s.acc) return PNB_OK;
+  TCK(engine_alloc(e, &s.acc, s.off[kParams] + 1, kStreamState));
+  TCK(cudaDeviceSynchronize());
+  return PNB_OK;
+}
+
+int train_accumulate(pnb_engine *e, cudaStream_t st) {
+  const pnb_train_state &s = *e->train;
+  const size_t N = s.off[kParams];
+  train_accum_kernel<<<blocks_for(N / 4), 256, 0, st>>>(s.grad, N, (double)e->train_hops, s.acc);
+  TCK(cudaGetLastError());
+  return 1;
+}
+
+int train_finish(pnb_engine *e, cudaStream_t st) {
+  const pnb_train_state &s = *e->train;
+  const size_t N = s.off[kParams];
+  train_finish_kernel<<<blocks_for(N / 4), 256, 0, st>>>(s.acc, N, s.grad);
+  TCK(cudaMemsetAsync(s.acc + N, 0, sizeof(double), st));
+  TCK(cudaMemsetAsync(s.bad, 0, sizeof(int), st));
+  train_check_kernel<<<blocks_for(N, 1024), 256, 0, st>>>(s.grad, N, s.bad, e->d_status);
+  TCK(cudaGetLastError());
+  return 2;
+}
+
+// The accumulator's N + 1 doubles to or from mem, host memory or device memory of the engine's device, on st
+int train_accum_copy(pnb_engine *e, void *mem, bool out, cudaStream_t st) {
+  const pnb_train_state &s = *e->train;
+  const size_t bytes = (s.off[kParams] + 1) * sizeof(double);
+  TCK(out ? cudaMemcpyAsync(mem, s.acc, bytes, cudaMemcpyDefault, st) : cudaMemcpyAsync(s.acc, mem, bytes, cudaMemcpyDefault, st));
+  return PNB_OK;
+}

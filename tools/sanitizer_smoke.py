@@ -9,8 +9,8 @@ calls on the chain's anti-diagonal unit order, state export / import, a session-
 relocations, fresh starts, session export / import / reset), ragged session calls (sessions that stop early, across the
 history slide and the fp32 network's 32-hop chunk), network-only calls on features and on records (both network modes),
 the pitch-only kernel on tiny batches and the network trainer (ten windows, more than a recurrence CTA's eight warps,
-on an active range, a call shorter than max_frames_per_call, ragged frames, then one Adam step); prints a checksum per
-leg."""
+on an active range, a call shorter than max_frames_per_call, ragged frames, then one Adam step, then two micro-batches
+accumulated, exported, imported and finished before a second step); prints a checksum per leg."""
 import os
 import sys
 
@@ -137,6 +137,17 @@ def main():
         e.train_adam(1e-3, 1)
         e.wait()
         print("trainnet", float(sums.sum()), float(np.abs(e.train_export("gradient").astype(np.float64)).sum()),
+              float(e.train_export("weights").astype(np.float64).sum()))
+        # two micro-batches accumulated, the accumulator through the host and back, finished, one more Adam step
+        e.train_grad(rec, [6] * 10)
+        e.train_accumulate()
+        e.train_grad(rec, [1, 2, 3, 4, 5, 6, 5, 4, 3, 2])
+        e.train_accumulate()
+        e.train_import("accum", e.train_export("accum"))
+        e.train_finish()
+        e.train_adam(1e-3, 2)
+        e.wait()
+        print("trainaccum", float(np.abs(e.train_export("gradient").astype(np.float64)).sum()),
               float(e.train_export("weights").astype(np.float64).sum()))
         e.close()
 

@@ -330,13 +330,13 @@ int pnb_train_import(pnb_engine *e, int what, const void *src, size_t bytes);
  *   out / d_out   PCM rows as pnb_process_*_* writes them (int16: C truncation of y*32768, wrapping)
  * These are the layouts of pnb_compute_rnn_* (PNB_RNN_FEATURES in, g/r out), so the three calls chain on device
  * pointers with no reshaping; f32 and int16 forms of the two halves mix freely.
- * pnb_analyze_* advances the active slots' signal input by n_frames hops (stage-in, analysis, history bookkeeping) and
- * leaves a pending synthesis on the engine.  The next pnb_synthesize_*, with the same n_frames, completes those hops
- * with the caller's g/r in place of the network's (post-filtered on a PNB_POSTFILTER engine), writes the PCM and commits
- * the hops.  A pnb_process_* call on the same input with the same g/r produces the same output and leaves the engine in
- * the same state.  g/r are used as given: for finite values the output is the reference's synthesis arithmetic on them
- * (pitch_filter and interp_band_gain are linear in r and g; nothing is clamped); for non-finite values the affected
- * rows' output is unspecified, the call still completes and the other rows are unaffected.
+ * pnb_analyze_* advances the active slots' signal input by n_frames hops (stage-in, analysis) and leaves a pending
+ * synthesis on the engine.  The next pnb_synthesize_*, with the same n_frames, completes those hops with the caller's
+ * g/r in place of the network's (post-filtered on a PNB_POSTFILTER engine), writes the PCM, moves the history and
+ * commits the hops.  A pnb_process_* call on the same input with the same g/r produces the same output and leaves the
+ * engine in the same state.  g/r are used as given: for finite values the output is the reference's synthesis
+ * arithmetic on them (pitch_filter and interp_band_gain are linear in r and g; nothing is clamped); for non-finite
+ * values the affected rows' output is unspecified, the call still completes and the other rows are unaffected.
  * While a synthesis is pending, only pnb_synthesize_*, pnb_compute_rnn_* / pnb_score_records_* (they touch no signal
  * state), pnb_wait, pnb_check, pnb_flush, pnb_read_tap, the profile readers and pnb_reset (which cancels it) are
  * accepted.  Every other call and state operation -- another pnb_analyze_*, pnb_process_* / pnb_submit_*,
@@ -347,8 +347,9 @@ int pnb_train_import(pnb_engine *e, int what, const void *src, size_t bytes);
  * an engine in session mode, PNB_TRAIN_DATA and PNB_NETWORK_ONLY engines, NULL pointers, short strides, n_frames outside
  * [1, max_frames]; a poisoned engine returns PNB_ERR_CUDA.  Ordering, blocking and poisoning are those of
  * pnb_process_device_* / pnb_process_host_*.
- * Launches: pnb_analyze_* issues three (stage-in, analysis, feature store), plus the history move on the calls where
- * pnb_process_* would issue it; pnb_synthesize_* issues two (g/r stage-in, synthesis). */
+ * Launches:  pnb_analyze_*     stage-in + analysis + feature store
+ *            pnb_synthesize_*  g/r stage + synthesis + [history move]
+ * with the history move on the synthesis where pnb_process_* would issue it. */
 int pnb_analyze_host_f32(pnb_engine *e, const float *in, size_t in_stride, int n_frames, float *feat, size_t feat_stride);
 int pnb_analyze_host_i16(pnb_engine *e, const short *in, size_t in_stride, int n_frames, float *feat, size_t feat_stride);
 int pnb_analyze_device_f32(pnb_engine *e, const float *d_in, size_t in_stride, int n_frames, float *d_feat,

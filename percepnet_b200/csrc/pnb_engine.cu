@@ -6,13 +6,10 @@
 // The network step is the only part that is sequential in time across the batch; analysis and synthesis
 // need no network state, so hops are processed F at a time.  A network-only call (pnb_compute_rnn_*) is
 //   rows_stage (features) -> F x network step -> rows_store (g/r)
-// on caller-supplied features or training records.  The split call cuts the PCM call where the network sits:
-//   pnb_analyze_*:    stage_in -> analysis -> rows_store (features) [-> slide history]
-//   pnb_synthesize_*: rows_stage (caller g/r) -> synthesis
-// and on a session list (pnb_*_sessions_*), where the ragged fix-up and the slide follow the synthesis as in the fused
-// session call:
-//   pnb_analyze_sessions_*:    [session move] -> stage_in -> analysis -> rows_store (features)
-//   pnb_synthesize_sessions_*: rows_stage (caller g/r) -> synthesis [-> ragged fix-up] [-> slide history]
+// on caller-supplied features or training records.  The split call cuts the PCM call where the network sits, on slots
+// and on a session list (pnb_*_sessions_*) alike, each half the fused call's (analysis_half / synthesis_half):
+//   pnb_analyze_*:    [session move] -> stage_in -> analysis -> rows_store (features)
+//   pnb_synthesize_*: rows_stage (caller g/r) -> synthesis [-> ragged fix-up] [-> slide history]
 #include <math.h>
 #include <stdarg.h>
 #include <stdio.h>
@@ -320,10 +317,7 @@ extern "C" int pnb_reset(pnb_engine *e) {
   e->h_status[0] = 0;
   e->h_status[1] = kNoRejectedSlot;
   e->hop = 0;
-  e->pending = 0;
-  e->pend_ids.clear();
-  e->pend_hops.clear();
-  e->pend_up.clear();
+  e->pending = {};
   e->n_active = e->S;
   e->poisoned = false;
   e->train_open = false;  // the accumulator (stream state) was zeroed above; the held gradient stays, and stays due
@@ -571,11 +565,12 @@ static int enqueue_plan(pnb_engine *e, const int *ids, int k, const int *hops, i
   return launch_session_move(a, st);
 }
 
-// The rows of the pending session split, from its host copy (pnb_engine::pend_up): nothing is planned again.
+// The rows of the pending session split, from its host copy (pnb_engine::pending.up): nothing is planned again.
 static int stage_pending_rows(pnb_engine *e, cudaStream_t st, SessionRows *r) {
+  const pnb_engine::PendingSplit &p = e->pending;
   const int *d = nullptr;
-  { int rc = stage_ints(e, e->pend_up.data(), e->pend_up.size(), st, &d); if (rc) return rc; }
-  point_rows(d, (int)e->pend_ids.size(), true, !e->pend_hops.empty(), e->pend_up.size(), r);
+  { int rc = stage_ints(e, p.up.data(), p.up.size(), st, &d); if (rc) return rc; }
+  point_rows(d, (int)p.ids.size(), true, !p.hops.empty(), p.up.size(), r);
   return PNB_OK;
 }
 
@@ -669,25 +664,76 @@ struct Call {
   bool pool = false;   // an analysis, synthesis or network call on a session list (pnb_*_sessions_*)
 };
 
+// The rows of a call on st, *r: nothing for a slot call; on a session list the pending session split's rows staged
+// again (the same list: nothing moves mid-hop), or else the call's residency plan applied, with the slot map for a
+// split or network call.  Returns the number of launches or a negative error.
+static int call_rows(pnb_engine *e, const Call &c, cudaStream_t st, SessionRows *r) {
+  if (!c.ids) return 0;
+  if (e->pending.F) return stage_pending_rows(e, st, r);
+  return enqueue_plan(e, c.ids, c.n_ids, c.hops, c.F, c.pool, st, r);
+}
+
+// The network hook of the engine's path for a call of F hops (hops: a ragged call's per-slot hops, or null).
+static int network(pnb_engine *e, int F, const int *hops, cudaStream_t st) {
+  return (e->flags & PNB_NN_TENSOR) ? tc_network(e, F, hops, st) : f32_network(e, F, hops, st);
+}
+
+// The signal path before the network, on st: the caller's PCM rows (in) into the history line, then the analysis of F
+// hops into d_feat, over the active slots and through a session call's row map and per-slot hops (r; null for slots).
+// Returns the number of launches or a negative error.
+static int analysis_half(pnb_engine *e, const Rows &in, int F, const SessionRows &r, cudaStream_t st) {
+  const bool i16 = in.bytes == sizeof(short);
+  int n = 0;
+  {
+    ProfScope ps(e, PNB_K_STAGE_IN, st);
+    n += launch_stage_in(e->d_pcm + e->line_off, e->pcm_stride, i16 ? nullptr : static_cast<const float *>(in.p),
+                         i16 ? static_cast<const short *>(in.p) : nullptr, in.stride, e->n_active, F * kFrame, st, 32768.f,
+                         r.row, r.rg.hops);
+  }
+  {
+    AnalysisArgs aa = analysis_args(e, F);
+    aa.hops = r.rg.hops;
+    ProfScope ps(e, PNB_K_ANALYSIS, st);
+    n += launch_analysis(aa, st);
+  }
+  CK(cudaGetLastError());
+  return n;
+}
+
+// The signal path after the network, on st, from the g/r in d_gr: the synthesis of F hops into the caller's PCM rows
+// (out), through r as analysis_half, then the fix-up of the slots that stop short, then the history slide when it falls
+// due.  The fix-up runs before the slide, which moves the window the counters of hop F point at.  Returns the number of
+// launches.
+static int synthesis_half(pnb_engine *e, const Rows &out, int F, const SessionRows &r, cudaStream_t st) {
+  const bool i16 = out.bytes == sizeof(short);
+  int n = 0;
+  {
+    SynthesisArgs sa = synthesis_args(e, F, i16 ? nullptr : static_cast<float *>(out.p),
+                                      i16 ? static_cast<short *>(out.p) : nullptr, out.stride);
+    sa.row = r.row;
+    sa.hops = r.rg.hops;
+    ProfScope ps(e, PNB_K_SYNTHESIS, st);
+    n += launch_synthesis(sa, st);
+  }
+  if (r.rg.n_short) {
+    ProfScope ps(e, PNB_K_SLIDE, st);
+    n += launch_ragged_carry(e, F, r.rg.hops, r.rg.slots, r.rg.n_short, st);
+  }
+  return n + advance_line(e, F, st);
+}
+
 // A network call on st (arguments already checked): the caller's rows into the features buffer, the network hook, its
 // g/r out to the caller's rows; a score call reduces the loss from the same g/r and writes g/r only when asked.  The
 // signal state (history line, overlap-add, pitch memory, spectrum ring, hop counter, line offset) is not touched.  On a
-// session list the call first applies its residency plan like any session call, or, between the halves of a session
-// split, stages the pending split's rows again (the same list: nothing moves mid-hop); row i of the caller's arrays is
-// then ids[i]'s, and a ragged call's frozen hops stage and store zeros.
+// session list row i of the caller's arrays is ids[i]'s (call_rows), and a ragged call's frozen hops stage and store
+// zeros.
 static int enqueue_network(pnb_engine *e, const Call &c, cudaStream_t st) {
   const int F = c.F;
   const Rows &in = c.in[0], &gr = c.out[0], &sums = c.out[1];
   return enqueue_call(e, F, st, [&]() -> int {
-    int n = 0;
     SessionRows r;
-    if (c.pool && e->pending) {
-      const int rc = stage_pending_rows(e, st, &r);
-      if (rc) return rc;
-    } else if (c.pool) {
-      n = enqueue_plan(e, c.ids, c.n_ids, c.hops, F, true, st, &r);
-      if (n < 0) return n;
-    }
+    int n = call_rows(e, c, st, &r);
+    if (n < 0) return n;
     const int S = e->S, na = e->n_active;
     const int *frames = nullptr;  // a score call's per-row hop counts, staged like a ragged call's hops
     if (c.frames) { int rc = stage_ints(e, c.frames, (size_t)na, st, &frames); if (rc) return rc; }
@@ -698,7 +744,7 @@ static int enqueue_network(pnb_engine *e, const Call &c, cudaStream_t st) {
     }
     CK(cudaGetLastError());
     {
-      const int q = (e->flags & PNB_NN_TENSOR) ? tc_network(e, F, r.rg.hops, st) : f32_network(e, F, r.rg.hops, st);
+      const int q = network(e, F, r.rg.hops, st);
       if (q < 0) return q;
       n += q;
     }
@@ -751,53 +797,30 @@ static int enqueue_records(pnb_engine *e, const Call &c, cudaStream_t st) {
   });
 }
 
-// One enhancement call on st, its buffers on the device (arguments already checked).  A session call first applies its
-// residency plan, and reads input row / writes output row and g/r row row[p] for slot p.  With hops (a ragged call)
-// slot p runs the hops of its list row, and the slots that stop early are moved to the counters of hop F after
-// synthesis.
+// One enhancement call on st, its buffers on the device (arguments already checked): the analysis half, the network,
+// the synthesis half.  A session call first applies its residency plan, and reads input row / writes output row and
+// g/r row row[p] for slot p.  With hops (a ragged call) slot p runs the hops of its list row, and the slots that stop
+// early are moved to the counters of hop F after synthesis.
 static int enqueue_enhance(pnb_engine *e, const Call &c, cudaStream_t st) {
   const int F = c.F;
-  const bool i16 = c.in[0].bytes == sizeof(short);
   return enqueue_call(e, F, st, [&]() -> int {
-    int n = 0;
     SessionRows r;
-    if (c.ids) {
-      n = enqueue_plan(e, c.ids, c.n_ids, c.hops, F, false, st, &r);
-      if (n < 0) return n;
-    }
-    const int *row = r.row;
-    const RaggedSlots &rg = r.rg;
-    const int S = e->S, na = e->n_active;  // the call advances streams [0, na); per-call buffers keep the stride S
-    const float *in = i16 ? nullptr : static_cast<const float *>(c.in[0].p);
-    const short *in16 = i16 ? static_cast<const short *>(c.in[0].p) : nullptr;
-    { ProfScope ps(e, PNB_K_STAGE_IN, st); n += launch_stage_in(e->d_pcm + e->line_off, e->pcm_stride, in, in16, c.in[0].stride, na, F * kFrame, st, 32768.f, row, rg.hops); }
+    int n = call_rows(e, c, st, &r);
+    if (n < 0) return n;
     {
-      AnalysisArgs aa = analysis_args(e, F);
-      aa.hops = rg.hops;
-      ProfScope ps(e, PNB_K_ANALYSIS, st);
-      n += launch_analysis(aa, st);
-    }
-    CK(cudaGetLastError());
-    {
-      const int q = (e->flags & PNB_NN_TENSOR) ? tc_network(e, F, rg.hops, st) : f32_network(e, F, rg.hops, st);
+      const int q = analysis_half(e, c.in[0], F, r, st);
       if (q < 0) return q;
       n += q;
     }
     {
-      SynthesisArgs sa = synthesis_args(e, F, i16 ? nullptr : static_cast<float *>(c.out[0].p),
-                                        i16 ? static_cast<short *>(c.out[0].p) : nullptr, c.out[0].stride);
-      sa.row = row;
-      sa.hops = rg.hops;
-      ProfScope ps(e, PNB_K_SYNTHESIS, st);
-      n += launch_synthesis(sa, st);
+      const int q = network(e, F, r.rg.hops, st);
+      if (q < 0) return q;
+      n += q;
     }
-    if (rg.n_short) {  // before the slide: it moves the window the counters of hop F point at
-      ProfScope ps(e, PNB_K_SLIDE, st);
-      n += launch_ragged_carry(e, F, rg.hops, rg.slots, rg.n_short, st);
-    }
-    n += advance_line(e, F, st);
-    if (c.gr && row)  // [F][na][68] in list order
-      n += launch_gr_gather(e->d_gr, c.gr, row, na, S, F, st, rg.hops);
+    n += synthesis_half(e, c.out[0], F, r, st);
+    const int S = e->S, na = e->n_active;  // the call advances streams [0, na); per-call buffers keep the stride S
+    if (c.gr && r.row)  // [F][na][68] in list order
+      n += launch_gr_gather(e->d_gr, c.gr, r.row, na, S, F, st, r.rg.hops);
     else if (c.gr)  // [F][na][68] from the [F][S][68] buffer
       CK(cudaMemcpy2DAsync(c.gr, (size_t)na * 68 * sizeof(float), e->d_gr, (size_t)S * 68 * sizeof(float), (size_t)na * 68 * sizeof(float), F,
                            cudaMemcpyDeviceToDevice, st));
@@ -805,95 +828,49 @@ static int enqueue_enhance(pnb_engine *e, const Call &c, cudaStream_t st) {
   });
 }
 
-// The analysis half of a slot call on st (arguments already checked): stage-in, analysis and, when it falls due, the
-// history slide, exactly as enqueue_enhance runs them, and the features out to the caller's rows.  The hop counter stays
-// where it is (the analysis and synthesis kernels both take hop0 = e->hop); the synthesis that completes these hops
-// commits it.  The slide may run before the synthesis: synthesis reads the spectra, not the history line.
-// On a session list the call first applies its residency plan as enqueue_enhance does, stages and analyses through the
-// row map and per-slot hops, and leaves the slide to the synthesis half: there a ragged call's fix-up runs after the
-// synthesis and before the slide, the fused call's order, so this half moves nothing bound to the counters.  The pending
-// split keeps the list, the hops and the rows of its upload.
+// An analysis on st (arguments already checked): the rows of the call and the analysis half, as enqueue_enhance runs
+// them, then the features out to the caller's rows.  Nothing bound to the hop counter or the line offset moves: the
+// analysis and synthesis kernels both take hop0 = e->hop, and the synthesis that completes these hops runs the rest of
+// the fused call and commits them.  The pending split keeps the hops and, on a session list, the list and the rows of
+// its upload.
 static int enqueue_analyze(pnb_engine *e, const Call &c, cudaStream_t st) {
   const int F = c.F;
-  const Rows &in = c.in[0], &feat = c.out[0];
-  const bool i16 = in.bytes == sizeof(short);
+  const Rows &feat = c.out[0];
   SessionRows r;
   const int rc = enqueue_call(e, F, st, [&]() -> int {
-    int n = 0;
-    if (c.pool) {
-      n = enqueue_plan(e, c.ids, c.n_ids, c.hops, F, true, st, &r);
-      if (n < 0) return n;
-    }
-    const int S = e->S, na = e->n_active;
-    {
-      ProfScope ps(e, PNB_K_STAGE_IN, st);
-      n += launch_stage_in(e->d_pcm + e->line_off, e->pcm_stride, i16 ? nullptr : static_cast<const float *>(in.p),
-                           i16 ? static_cast<const short *>(in.p) : nullptr, in.stride, na, F * kFrame, st, 32768.f, r.row,
-                           r.rg.hops);
-    }
-    {
-      AnalysisArgs aa = analysis_args(e, F);
-      aa.hops = r.rg.hops;
-      ProfScope ps(e, PNB_K_ANALYSIS, st);
-      n += launch_analysis(aa, st);
-    }
-    {
-      ProfScope ps(e, PNB_K_STAGE_IN, st);
-      n += launch_rows_store(e->d_feat, kFeat, static_cast<float *>(feat.p), feat.stride, na, S, F, st, r.slot, r.rg.hops);
-    }
-    if (!c.pool) n += advance_line(e, F, st);
-    return n;
+    int n = call_rows(e, c, st, &r);
+    if (n < 0) return n;
+    const int q = analysis_half(e, c.in[0], F, r, st);
+    if (q < 0) return q;
+    ProfScope ps(e, PNB_K_STAGE_IN, st);
+    return n + q + launch_rows_store(e->d_feat, kFeat, static_cast<float *>(feat.p), feat.stride, e->n_active, e->S, F, st,
+                                     r.slot, r.rg.hops);
   }, false);
-  if (rc == PNB_OK) {
-    e->pending = F;
-    if (c.pool) {
-      e->pend_ids.assign(c.ids, c.ids + c.n_ids);
-      if (c.hops) e->pend_hops.assign(c.hops, c.hops + c.n_ids);
-      else e->pend_hops.clear();
-      e->pend_up.assign(e->plan_up.begin(), e->plan_up.begin() + r.n_up);
-    }
-  }
+  if (rc == PNB_OK)
+    e->pending = {F, std::vector<int>(c.ids, c.ids + c.n_ids),
+                  c.hops ? std::vector<int>(c.hops, c.hops + c.n_ids) : std::vector<int>(),
+                  std::vector<int>(e->plan_up.begin(), e->plan_up.begin() + r.n_up)};
   return rc;
 }
 
-// The synthesis half (arguments already checked, an analysis of F hops pending): the caller's g/r rows into d_gr where
-// the network hook would have left them, then the synthesis of enqueue_enhance, which commits the hop counter.  For a
-// session split the pending rows are staged again, and the ragged fix-up and the history slide follow the synthesis,
-// in enqueue_enhance's order.
+// A synthesis on st (arguments already checked, an analysis of F hops pending): the rows of the call, the caller's g/r
+// rows into d_gr where the network hook would have left them, then the synthesis half of enqueue_enhance, which commits
+// the hop counter.
 static int enqueue_synthesize(pnb_engine *e, const Call &c, cudaStream_t st) {
   const int F = c.F;
-  const Rows &gr = c.in[0], &out = c.out[0];
-  const bool i16 = out.bytes == sizeof(short);
+  const Rows &gr = c.in[0];
   const int rc = enqueue_call(e, F, st, [&]() -> int {
-    int n = 0;
     SessionRows r;
-    if (c.pool) { int q = stage_pending_rows(e, st, &r); if (q) return q; }
+    int n = call_rows(e, c, st, &r);
+    if (n < 0) return n;
     {
       ProfScope ps(e, PNB_K_STAGE_IN, st);
       n += launch_rows_stage(e->d_gr, 68, static_cast<const float *>(gr.p), gr.stride, 68, 0, e->n_active, e->S, F, st,
                              r.row, r.rg.hops);
     }
-    {
-      SynthesisArgs sa = synthesis_args(e, F, i16 ? nullptr : static_cast<float *>(out.p),
-                                        i16 ? static_cast<short *>(out.p) : nullptr, out.stride);
-      sa.row = r.row;
-      sa.hops = r.rg.hops;
-      ProfScope ps(e, PNB_K_SYNTHESIS, st);
-      n += launch_synthesis(sa, st);
-    }
-    if (r.rg.n_short) {  // before the slide: it moves the window the counters of hop F point at
-      ProfScope ps(e, PNB_K_SLIDE, st);
-      n += launch_ragged_carry(e, F, r.rg.hops, r.rg.slots, r.rg.n_short, st);
-    }
-    if (c.pool) n += advance_line(e, F, st);
-    return n;
+    return n + synthesis_half(e, c.out[0], F, r, st);
   });
-  if (rc == PNB_OK) {
-    e->pending = 0;
-    e->pend_ids.clear();
-    e->pend_hops.clear();
-    e->pend_up.clear();
-  }
+  if (rc == PNB_OK) e->pending = {};
   return rc;
 }
 
@@ -925,7 +902,7 @@ static int enqueue(pnb_engine *e, const Call &c, cudaStream_t st) {
 // a stream's state between the halves is mid-hop (its overlap-add memory lags its history), and no blob may capture it.
 static int refuse_pending(const pnb_engine *e) {
   return fail(PNB_ERR_ARG, "a synthesis is pending (pnb_analyze_* of %d hops): call pnb_synthesize_* with the same n_frames, or pnb_reset",
-              e->pending);
+              e->pending.F);
 }
 
 // The slot-level entry points of an engine in session mode: refused before anything is enqueued.
@@ -970,13 +947,13 @@ static int check_strides(const Rows (&a)[2], int F) {
 // A call on a session list while a session split is pending: the pending list in its order and n_frames, and for a
 // network call (which passes hops) the pending hops.
 static int check_pending_list(const pnb_engine *e, const Call &c) {
-  const std::vector<int> &ids = e->pend_ids, &hops = e->pend_hops;
-  bool same = c.n_ids == (int)ids.size() && c.F == e->pending && std::equal(ids.begin(), ids.end(), c.ids);
+  const std::vector<int> &ids = e->pending.ids, &hops = e->pending.hops;
+  bool same = c.n_ids == (int)ids.size() && c.F == e->pending.F && std::equal(ids.begin(), ids.end(), c.ids);
   if (same && c.kind == Call::kNetwork)
     same = c.hops ? !hops.empty() && std::equal(hops.begin(), hops.end(), c.hops) : hops.empty();
   if (!same)
     return fail(PNB_ERR_ARG, "a session split of %d sessions and %d hops is pending: pass its list in the same order, its n_frames%s",
-                (int)ids.size(), e->pending, c.kind == Call::kNetwork ? " and its hops" : "");
+                (int)ids.size(), e->pending.F, c.kind == Call::kNetwork ? " and its hops" : "");
   return PNB_OK;
 }
 
@@ -1031,12 +1008,12 @@ static int check_call(pnb_engine *e, Call &c) {
     return fail(PNB_ERR_ARG, "engine was created with PNB_TRAIN_AUDIO: use pnb_train_audio_*, so that its audio has no gaps");
   { int rc = check_strides(c.out, c.F); if (rc) return rc; }
   if (c.kind == Call::kSynthesize) {
-    if (!e->pending) return fail(PNB_ERR_ARG, "no analysis awaits its synthesis: call pnb_analyze_* first");
-    if (c.F != e->pending) return fail(PNB_ERR_ARG, "n_frames %d, but the pending analysis has %d hops", c.F, e->pending);
+    if (!e->pending.F) return fail(PNB_ERR_ARG, "no analysis awaits its synthesis: call pnb_analyze_* first");
+    if (c.F != e->pending.F) return fail(PNB_ERR_ARG, "n_frames %d, but the pending analysis has %d hops", c.F, e->pending.F);
     if (c.pool) { int rc = check_pending_list(e, c); if (rc) return rc; }
-  } else if (e->pending && !network) {
+  } else if (e->pending.F && !network) {
     return refuse_pending(e);
-  } else if (e->pending && c.pool) {
+  } else if (e->pending.F && c.pool) {
     int rc = check_pending_list(e, c);
     if (rc) return rc;
   }
@@ -1595,7 +1572,7 @@ static int check_blobs(const void *d_blobs, size_t blob_stride) {
 static int state_batch(pnb_engine *e, int mode, const int *streams, int n, void *d_blobs, size_t blob_stride, void *cuda_stream) {
   if (!e) return fail(PNB_ERR_ARG, "engine is NULL");
   if (e->sessions) return refuse_in_session_mode();
-  if (e->pending) return refuse_pending(e);
+  if (e->pending.F) return refuse_pending(e);
   if (n < 0) return fail(PNB_ERR_ARG, "n = %d is negative", n);
   if (n == 0) return PNB_OK;
   if (!streams) return fail(PNB_ERR_ARG, "streams is NULL");
@@ -1623,7 +1600,7 @@ extern "C" int pnb_set_active_streams(pnb_engine *e, int n, void *cuda_stream) {
   if (!e) return fail(PNB_ERR_ARG, "engine is NULL");
   if (e->flags & PNB_TRAIN_DATA) return fail(PNB_ERR_ARG, "PNB_TRAIN_DATA engines always advance all their streams");
   if (e->sessions) return refuse_in_session_mode();
-  if (e->pending) return refuse_pending(e);
+  if (e->pending.F) return refuse_pending(e);
   if (n < 1 || n > e->S) return fail(PNB_ERR_ARG, "active streams %d outside [1, %d]", n, e->S);
   if (e->poisoned) return refuse_poisoned(PNB_ERR_ARG);
   if (n > e->n_active) {
@@ -1641,7 +1618,7 @@ extern "C" int pnb_active_streams(const pnb_engine *e) { return e ? e->n_active 
 static int check_one_state(pnb_engine *e, int stream, const void *buf, size_t bytes) {
   if (!e || !buf) return fail(PNB_ERR_ARG, "NULL argument");
   if (e->sessions) return refuse_in_session_mode();
-  if (e->pending) return refuse_pending(e);
+  if (e->pending.F) return refuse_pending(e);
   { int rc = check_list(e, &stream, 1, e->S, e->n_active, "stream"); if (rc) return rc; }
   if (bytes < sizeof(StreamState)) return fail(PNB_ERR_ARG, "state buffer of %zu bytes, need pnb_state_size() = %zu", bytes, sizeof(StreamState));
   if (e->poisoned) return refuse_poisoned(PNB_ERR_CUDA);
@@ -1703,7 +1680,7 @@ extern "C" int pnb_sessions_reserve(pnb_engine *e, int n_sessions) {
   if (e->flags & PNB_TRAIN_DATA) return fail(PNB_ERR_ARG, "PNB_TRAIN_DATA engines have no session pool");
   if (e->flags & PNB_NETWORK_ONLY) return fail(PNB_ERR_ARG, "PNB_NETWORK_ONLY engines have no session pool");
   if (e->flags & PNB_SIGNAL_ONLY) return fail(PNB_ERR_ARG, "PNB_SIGNAL_ONLY engines have no session pool");
-  if (e->pending) return refuse_pending(e);
+  if (e->pending.F) return refuse_pending(e);
   if (e->poisoned) return refuse_poisoned(PNB_ERR_ARG);
   if (n_sessions < 1) return fail(PNB_ERR_ARG, "n_sessions = %d, need >= 1", n_sessions);
   if (e->sessions && n_sessions <= e->pool.capacity()) return PNB_OK;  // the pool never shrinks
@@ -1791,7 +1768,7 @@ extern "C" int pnb_process_sessions_ragged_host_i16(pnb_engine *e, const int *id
 static int session_batch(pnb_engine *e, int mode, const int *ids, int n, void *d_blobs, size_t blob_stride, void *cuda_stream) {
   if (!e) return fail(PNB_ERR_ARG, "engine is NULL");
   if (e->poisoned) return refuse_poisoned(PNB_ERR_ARG);
-  if (e->pending) return refuse_pending(e);
+  if (e->pending.F) return refuse_pending(e);
   if (n == 0 && e->sessions) return PNB_OK;
   if (mode != kStateReset) { int rc = check_blobs(d_blobs, blob_stride); if (rc) return rc; }
   { int rc = check_ids(e, ids, n, e->pool.capacity()); if (rc) return rc; }

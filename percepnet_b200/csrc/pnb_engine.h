@@ -82,15 +82,18 @@ struct pnb_engine {
   long long train_hops = 0;
   bool train_open = false;
   int last_frames = 0;
-  // hops of an analysis (pnb_analyze_*) whose synthesis (pnb_synthesize_*) is still due, or 0.  Between the two halves
-  // the analysed streams are mid-hop, so every call and state operation but the synthesis and network calls is refused.
-  int pending = 0;
-  // A session split (pnb_analyze_sessions_*) pending: its list, its hops in list order (empty when every session runs
-  // `pending` hops) and the host copy of its row upload (row map, slot map, and for a ragged call the hops of every slot
-  // and the slots that stop early).  The index staging that upload went through is reused by the next call, and the
-  // plan is already applied to the pool, so the synthesis and a network call between the halves stage this copy again.
-  // All empty for a slot split.
-  std::vector<int> pend_ids, pend_hops, pend_up;
+  // An analysis (pnb_analyze_*) whose synthesis (pnb_synthesize_*) is still due, set by the analysis and cleared by the
+  // synthesis or pnb_reset.  F: its hops, or 0 when none is pending.  Between the two halves the analysed streams are
+  // mid-hop, so every call and state operation but the synthesis and network calls is refused.  A session split
+  // (pnb_analyze_sessions_*) also keeps its list, its hops in list order (empty when every session runs F hops) and the
+  // host copy of its row upload (row map, slot map, and for a ragged call the hops of every slot and the slots that stop
+  // early).  The index staging that upload went through is reused by the next call, and the plan is already applied to
+  // the pool, so the synthesis and a network call between the halves stage this copy again.  All empty for a slot split.
+  struct PendingSplit {
+    int F = 0;
+    std::vector<int> ids, hops, up;
+  };
+  PendingSplit pending;
   long long launches = 0;
   // status word on the device: bit 0 = an activation left the domain in which the reference's tansig_approx is
   // defined (tensor path only; reported as PNB_ERR_DOMAIN by the synchronising entry points, cleared by pnb_reset);

@@ -41,22 +41,33 @@ def _blobs(eng, n):
     return b.cpu().numpy()
 
 
-def _split_device(api, eng, x, int16):
-    """analyze_device -> compute_rnn_device -> synthesize_device on torch buffers, chained with no reshaping:
-    (out [n, F*480], g/r [n, F, 68], features [n, F, 70])."""
+def _split(api, eng, x, where, int16):
+    """analyze -> compute_rnn -> synthesize through the host forms, or through the device forms on torch buffers
+    chained with no reshaping: (out [n, F*480], g/r [n, F, 68], features [n, F, 70], launches of the analysis, launches
+    of the synthesis)."""
     import torch
     n, T = x.shape
     F = T // FRAME
+    n0 = eng.launches
+    if where == "host":
+        feat = eng.analyze(x)
+        n1 = eng.launches
+        gr = eng.compute_rnn(feat)
+        n2 = eng.launches
+        out = eng.synthesize(gr, int16=int16)
+        return out, gr, feat, n1 - n0, eng.launches - n2
     d_in = torch.from_numpy(np.ascontiguousarray(x)).cuda()
     d_feat = torch.full((n, F, 70), -7.0, device="cuda")
     d_gr = torch.full((n, F, 68), -7.0, device="cuda")
     d_out = torch.empty_like(d_in)
     torch.cuda.synchronize()
     eng.analyze_device(d_in.data_ptr(), T, F, d_feat.data_ptr(), F * 70, int16=int16)
+    n1 = eng.launches
     eng.compute_rnn_device(api.RNN_FEATURES, d_feat.data_ptr(), F * 70, F, d_gr.data_ptr(), F * 68)
+    n2 = eng.launches
     eng.synthesize_device(d_gr.data_ptr(), F * 68, F, d_out.data_ptr(), T, int16=int16)
     eng.check()
-    return d_out.cpu().numpy(), d_gr.cpu().numpy(), d_feat.cpu().numpy()
+    return d_out.cpu().numpy(), d_gr.cpu().numpy(), d_feat.cpu().numpy(), n1 - n0, eng.launches - n2
 
 
 def _fused_device(eng, x, int16):
@@ -93,14 +104,8 @@ def test_split_call_is_the_fused_call(api, model0, mode, post):
     for F, where, i16 in calls:
         xin = np.ascontiguousarray((x16 if i16 else x)[:, t0 * FRAME:(t0 + F) * FRAME])
         tag = f"hops {t0}..{t0 + F - 1} {where} {'int16' if i16 else 'f32'}"
-        if where == "host":
-            want, want_gr = fused.process(xin, want_gr=True)
-            feat = split.analyze(xin)
-            gr = split.compute_rnn(feat)
-            got = split.synthesize(gr, int16=i16)
-        else:
-            want, want_gr = _fused_device(fused, xin, i16)
-            got, gr, feat = _split_device(api, split, xin, i16)
+        want, want_gr = fused.process(xin, want_gr=True) if where == "host" else _fused_device(fused, xin, i16)
+        got, gr, feat, _, _ = _split(api, split, xin, where, i16)
         assert got.dtype == want.dtype, tag
         assert (np.array_equal(got, want) if i16 else same_bits(got, want)), tag
         assert same_bits(gr, want_gr.transpose(1, 0, 2)), tag
@@ -114,6 +119,44 @@ def test_split_call_is_the_fused_call(api, model0, mode, post):
     want, _ = fused.process(np.ascontiguousarray(x[:, t0 * FRAME:]))
     got, _ = split.process(np.ascontiguousarray(x[:, t0 * FRAME:]))
     assert same_bits(got, want)
+    fused.close()
+    split.close()
+
+
+@pytest.mark.parametrize("mode", ["fp32", "tensor"])
+def test_split_call_slides_where_the_fused_call_does(api, model0, mode):
+    """Ten 2-hop split calls at max_frames 2 against a twin engine's pnb_process_* calls, through every host and device
+    form (f32 and int16), on an active range below n_streams.  The history line holds eight such calls, so the eighth
+    moves it back to the start of the rows.  After every pair the output, g/r, features and exported blobs are
+    bit-identical; the analysis issues three launches and the synthesis two plus the history move, which is whatever
+    the fused call issued beyond launches_per_call."""
+    from percepnet_b200.synth import to_int16
+    S, n, F, calls = 5, 4, 2, 10
+    x = crowd(n, (calls + 1) * F, seed=450)
+    x16 = to_int16(x)
+    fused, split = (api.Engine(S, F, model0, _flags(api, mode) | api.KEEP_TAPS) for _ in range(2))
+    for e in (fused, split):
+        e.set_active(n)
+    per_call = fused.launches_per_call(F)
+    slides = []
+    for k in range(calls):
+        where, i16 = ("host", "device")[k % 2], (k // 2) % 2 == 1
+        xin = np.ascontiguousarray((x16 if i16 else x)[:, k * F * FRAME:(k + 1) * F * FRAME])
+        tag = f"call {k} {where} {'int16' if i16 else 'f32'}"
+        n0 = fused.launches
+        want, want_gr = fused.process(xin, want_gr=True) if where == "host" else _fused_device(fused, xin, i16)
+        slide = fused.launches - n0 - per_call
+        got, gr, feat, n_analysis, n_synthesis = _split(api, split, xin, where, i16)
+        assert (np.array_equal(got, want) if i16 else same_bits(got, want)), tag
+        assert same_bits(gr, want_gr.transpose(1, 0, 2)), tag
+        assert same_bits(feat, fused.read_tap("features", F)[:, :n].transpose(1, 0, 2)), tag
+        assert np.array_equal(_blobs(split, n), _blobs(fused, n)), tag
+        assert (n_analysis, n_synthesis) == (3, 2 + slide), tag
+        if slide:
+            slides.append(k)
+    assert slides == [7]
+    rest = np.ascontiguousarray(x[:, calls * F * FRAME:])
+    assert same_bits(split.process(rest)[0], fused.process(rest)[0])
     fused.close()
     split.close()
 

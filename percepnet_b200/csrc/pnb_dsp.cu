@@ -1110,10 +1110,9 @@ cudaError_t dsp_configure() {
                               (int)synthesis_smem_bytes());
 }
 
-int launch_analysis(const AnalysisArgs &a, cudaStream_t st) {
+void launch_analysis(const AnalysisArgs &a, cudaStream_t st) {
   dim3 grid((a.n_streams + kAnaWarps - 1) / kAnaWarps);
   analysis_kernel<<<grid, kAnaWarps * 32, analysis_smem_bytes(), st>>>(a);
-  return 1;
 }
 // ------------------------------------------------------------------------------------------
 // Training-data labels (SURVEY.md 8 row f1).  One warp per (frame, pair); lane b and b+32 own a band.
@@ -1195,38 +1194,34 @@ extern "C" int pnb_debug_analysis_cycles(unsigned long long *out16, int reset) {
 }
 #endif
 
-int launch_pitch_only(const PitchOnlyArgs &a, cudaStream_t st) {
+bool launch_pitch_only(const PitchOnlyArgs &a, cudaStream_t st) {
   const size_t smem = kPitchWarps * sizeof(WarpSmem);
   static bool configured = false;
   if (!configured) {
-    if (cudaFuncSetAttribute(pitch_only_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return -1;
+    if (cudaFuncSetAttribute(pitch_only_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return false;
     configured = true;
   }
   pitch_only_kernel<<<(unsigned)((a.n_units + kPitchWarps - 1) / kPitchWarps), kPitchWarps * 32, smem, st>>>(a);
-  return 1;
+  return true;
 }
 
-int launch_train_labels(const LabelArgs &a, cudaStream_t st) {
+void launch_train_labels(const LabelArgs &a, cudaStream_t st) {
   const long total = (long)a.n_frames * a.n_pairs;
   train_labels_kernel<<<(unsigned)((total + 7) / 8), 256, 0, st>>>(a);
-  return 1;
 }
 
-int launch_synthesis(const SynthesisArgs &a, cudaStream_t st) {
+void launch_synthesis(const SynthesisArgs &a, cudaStream_t st) {
   dim3 grid((a.n_streams + kSynWarps - 1) / kSynWarps);
   if (a.clamp16) synthesis_kernel<true><<<grid, kSynWarps * 32, synthesis_smem_bytes(), st>>>(a);
   else synthesis_kernel<false><<<grid, kSynWarps * 32, synthesis_smem_bytes(), st>>>(a);
-  return 1;
 }
-int launch_stage_in(float *pcm, size_t pcm_stride, const float *in, const short *in16, size_t in_stride,
-                    int n_streams, int n_samples, cudaStream_t st, float i16_div, const int *row, const int *hops) {
+void launch_stage_in(float *pcm, size_t pcm_stride, const float *in, const short *in16, size_t in_stride,
+                     int n_streams, int n_samples, cudaStream_t st, float i16_div, const int *row, const int *hops) {
   dim3 grid(n_streams, (n_samples + 1023) / 1024 > 8 ? 8 : (n_samples + 1023) / 1024);
   stage_in_kernel<<<grid, 256, 0, st>>>(pcm, pcm_stride, in, in16, in_stride, n_streams, n_samples, i16_div, row, hops);
-  return 1;
 }
-int launch_slide_history(float *pcm, size_t pcm_stride, int n_streams, int n_samples, cudaStream_t st) {
+void launch_slide_history(float *pcm, size_t pcm_stride, int n_streams, int n_samples, cudaStream_t st) {
   slide_history_kernel<<<n_streams, 512, 0, st>>>(pcm, pcm_stride, n_samples);
-  return 1;
 }
 
 }  // namespace pnb

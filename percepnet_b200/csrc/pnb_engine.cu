@@ -338,15 +338,16 @@ static cudaEvent_t prof_event(pnb_engine *e) {
   cudaEventCreate(&ev);
   return ev;
 }
-ProfScope::ProfScope(pnb_engine *eng, int cls, cudaStream_t s) : e(eng), idx(-1), st(s) {
-  if (!e->profiling) return;
+LaunchScope::LaunchScope(pnb_engine *eng, int cls, cudaStream_t s) : e(eng), idx(-1), st(s) {
+  e->launches++;
+  if (!e->profiling || cls == kUnprofiled) return;
   pnb_engine::ProfRec r;
   r.cls = cls; r.a = prof_event(e); r.b = prof_event(e);
   cudaEventRecord(r.a, st);
   e->prof_pending.push_back(r);
   idx = (int)e->prof_pending.size() - 1;
 }
-ProfScope::~ProfScope() {
+LaunchScope::~LaunchScope() {
   if (idx >= 0) cudaEventRecord(e->prof_pending[idx].b, st);
 }
 extern "C" int pnb_profile_enable(pnb_engine *e, int on) {
@@ -402,14 +403,15 @@ extern "C" const char *pnb_kernel_class_name(int cls) {
 
 // ------------------------------------------------------------------------------------------
 // The next call's window starts n_frames*480 samples further on; when it would not fit any more, the last 5280
-// samples are moved back to the start of the rows.  Returns the number of launches.
-static int advance_line(pnb_engine *e, int F, cudaStream_t st) {
+// samples are moved back to the start of the rows.
+static void advance_line(pnb_engine *e, int F, cudaStream_t st) {
   e->line_off += (size_t)F * kFrame;
-  if (e->line_off + kKeep + (size_t)e->Fmax * kFrame <= e->pcm_stride) return 0;
-  ProfScope ps(e, PNB_K_SLIDE, st);
-  int n = launch_slide_history(e->d_pcm, e->pcm_stride, e->n_active, (int)e->line_off, st);  // inactive rows: no state to keep
+  if (e->line_off + kKeep + (size_t)e->Fmax * kFrame <= e->pcm_stride) return;
+  {
+    LaunchScope m(e, PNB_K_SLIDE, st);
+    launch_slide_history(e->d_pcm, e->pcm_stride, e->n_active, (int)e->line_off, st);  // inactive rows: no state to keep
+  }
   e->line_off = 0;
-  return n;
 }
 
 static AnalysisArgs analysis_args(pnb_engine *e, int F) {
@@ -450,26 +452,29 @@ static int mark_call_end(pnb_engine *e, cudaStream_t st) {
   return PNB_OK;
 }
 
-// The launches of one call or state operation, in ev_call's order, added to the launch count; returns their count or a
-// negative error.  The enqueue itself may move host-side stream state (advance_line the line offset, a session
-// operation the residency plan) and part of the work may already be enqueued, so a failure after it started leaves the
-// streams' state undefined: the engine is poisoned, and refuses calls and state operations until pnb_reset.
+// The launches of one call or state operation, in ev_call's order; returns PNB_OK or a negative error.  Their markers
+// count them as they are issued.  The enqueue itself may move host-side stream state (advance_line the line offset, a
+// session operation the residency plan) and part of the work may already be enqueued, so a failure after it started
+// leaves the streams' state undefined: the engine is poisoned, and refuses calls and state operations until pnb_reset.
+// A failed enqueue adds nothing to the launch count.
 template <typename Launches>
 static int enqueue_ordered(pnb_engine *e, cudaStream_t st, Launches launches) {
-  int n = wait_last_call(e, st);
-  if (n == PNB_OK) n = launches();
-  if (n >= 0) { const int rc = mark_call_end(e, st); if (rc) n = rc; }
-  if (n < 0) e->poisoned = true;
-  else e->launches += n;
-  return n;
+  const long long launches0 = e->launches;
+  int rc = wait_last_call(e, st);
+  if (rc == PNB_OK) rc = launches();
+  if (rc == PNB_OK) rc = mark_call_end(e, st);
+  if (rc != PNB_OK) {
+    e->launches = launches0;
+    e->poisoned = true;
+  }
+  return rc;
 }
 // Enqueues one call of F hops on st (arguments already checked) and commits the hop counter (unless commit_hop is false:
 // a network call, which leaves the signal state alone, or an analysis, whose synthesis commits it) and last_frames when
 // all of it was accepted.
 template <typename Launches>
 static int enqueue_call(pnb_engine *e, int F, cudaStream_t st, Launches launches, bool commit_hop = true) {
-  const int n = enqueue_ordered(e, st, launches);
-  if (n < 0) return n;
+  if (int rc = enqueue_ordered(e, st, launches)) return rc;
   if (commit_hop) e->hop += F;
   e->last_frames = F;
   return PNB_OK;
@@ -534,7 +539,7 @@ static void point_rows(const int *d, int k, bool with_slot, bool ragged, size_t 
 
 // A session call's residency plan, applied (pnb_session_plan.h), its upload (the rows of SessionRows, then the moves
 // 16-byte aligned), and its state launch when membership changed.  Sets the active range to the list; *r: the rows on
-// the device.  Returns the number of launches or a negative error.
+// the device.
 static int enqueue_plan(pnb_engine *e, const int *ids, int k, const int *hops, int F, bool with_slot, cudaStream_t st,
                         SessionRows *r) {
   StateArgs a = state_args(e);  // before the plan: parking reads the pieces where the last call left them
@@ -559,10 +564,12 @@ static int enqueue_plan(pnb_engine *e, const int *ids, int k, const int *hops, i
   const int *d = nullptr;
   { int rc = stage_ints(e, up.data(), up.size(), st, &d); if (rc) return rc; }
   point_rows(d, k, with_slot, hops != nullptr, n_up, r);
-  if (e->plan_moves.empty()) return 0;
+  if (e->plan_moves.empty()) return PNB_OK;
   a.n = (int)e->plan_moves.size();
   a.moves = d + at_moves;
-  return launch_session_move(a, st);
+  LaunchScope m(e, kUnprofiled, st);
+  launch_session_move(a, st);
+  return PNB_OK;
 }
 
 // The rows of the pending session split, from its host copy (pnb_engine::pending.up): nothing is planned again.
@@ -576,7 +583,7 @@ static int stage_pending_rows(pnb_engine *e, cudaStream_t st, SessionRows *r) {
 
 // A session export into the caller's blobs (a: their address and stride): resident sessions from their slots
 // (session_move_kernel), parked ones from their parking blobs (session_blob_kernel); nothing moves.  Its upload is
-// [moves of the resident ones][ids of the parked ones][their rows].  Returns the number of launches or a negative error.
+// [moves of the resident ones][ids of the parked ones][their rows].
 static int enqueue_session_export(pnb_engine *e, const int *ids, int n, StateArgs a, cudaStream_t st) {
   std::vector<int> &up = e->plan_up;
   up.clear();
@@ -591,10 +598,17 @@ static int enqueue_session_export(pnb_engine *e, const int *ids, int n, StateArg
   up.insert(up.end(), rows.begin(), rows.end());
   const int *d = nullptr;
   { int rc = stage_ints(e, up.data(), up.size(), st, &d); if (rc) return rc; }
-  int n_launches = 0;
-  if (r) { a.n = r; a.moves = d; n_launches += launch_session_move(a, st); }
-  if (p) { a.n = p; a.streams = d + 4 * r; a.rows = d + 4 * r + p; n_launches += launch_session_blob(a, st); }
-  return n_launches;
+  if (r) {
+    a.n = r; a.moves = d;
+    LaunchScope m(e, kUnprofiled, st);
+    launch_session_move(a, st);
+  }
+  if (p) {
+    a.n = p; a.streams = d + 4 * r; a.rows = d + 4 * r + p;
+    LaunchScope m(e, kUnprofiled, st);
+    launch_session_blob(a, st);
+  }
+  return PNB_OK;
 }
 
 // One stream-state operation (reset, export or import: mode) as its entry point received it.
@@ -612,7 +626,7 @@ struct StateOp {
 // import, the move.  Sessions: an export as enqueue_session_export; a reset or an import takes the sessions out of
 // their slots on the host, then stages the ids, checks the blobs of an import and rewrites their parking blobs.
 static int enqueue_state(pnb_engine *e, const StateOp &op, cudaStream_t st) {
-  const int n = enqueue_ordered(e, st, [&]() -> int {
+  return enqueue_ordered(e, st, [&]() -> int {
     StateArgs a = state_args(e);
     a.mode = op.mode;
     a.blobs = static_cast<char *>(op.blobs);
@@ -622,10 +636,15 @@ static int enqueue_state(pnb_engine *e, const StateOp &op, cudaStream_t st) {
       for (int i = 0; i < op.n; i++) e->pool.evict(op.list[i]);
     { int rc = stage_ints(e, op.list, (size_t)op.n, st, &a.streams); if (rc) return rc; }
     a.n = op.n;
-    const int check = op.mode == kStateImport ? launch_state_check(a, st) : 0;  // a session import reports session ids
-    return check + (op.sessions ? launch_session_blob(a, st) : launch_state_move(a, st));
+    if (op.mode == kStateImport) {  // a session import reports session ids
+      LaunchScope m(e, kUnprofiled, st);
+      launch_state_check(a, st);
+    }
+    LaunchScope m(e, kUnprofiled, st);
+    if (op.sessions) launch_session_blob(a, st);
+    else launch_state_move(a, st);
+    return PNB_OK;
   });
-  return n < 0 ? n : PNB_OK;
 }
 
 // One array of a call's rows, in host or device memory by entry point: row r at p + r * stride values of `bytes` bytes
@@ -666,9 +685,9 @@ struct Call {
 
 // The rows of a call on st, *r: nothing for a slot call; on a session list the pending session split's rows staged
 // again (the same list: nothing moves mid-hop), or else the call's residency plan applied, with the slot map for a
-// split or network call.  Returns the number of launches or a negative error.
+// split or network call.
 static int call_rows(pnb_engine *e, const Call &c, cudaStream_t st, SessionRows *r) {
-  if (!c.ids) return 0;
+  if (!c.ids) return PNB_OK;
   if (e->pending.F) return stage_pending_rows(e, st, r);
   return enqueue_plan(e, c.ids, c.n_ids, c.hops, c.F, c.pool, st, r);
 }
@@ -680,46 +699,42 @@ static int network(pnb_engine *e, int F, const int *hops, cudaStream_t st) {
 
 // The signal path before the network, on st: the caller's PCM rows (in) into the history line, then the analysis of F
 // hops into d_feat, over the active slots and through a session call's row map and per-slot hops (r; null for slots).
-// Returns the number of launches or a negative error.
 static int analysis_half(pnb_engine *e, const Rows &in, int F, const SessionRows &r, cudaStream_t st) {
   const bool i16 = in.bytes == sizeof(short);
-  int n = 0;
   {
-    ProfScope ps(e, PNB_K_STAGE_IN, st);
-    n += launch_stage_in(e->d_pcm + e->line_off, e->pcm_stride, i16 ? nullptr : static_cast<const float *>(in.p),
-                         i16 ? static_cast<const short *>(in.p) : nullptr, in.stride, e->n_active, F * kFrame, st, 32768.f,
-                         r.row, r.rg.hops);
+    LaunchScope m(e, PNB_K_STAGE_IN, st);
+    launch_stage_in(e->d_pcm + e->line_off, e->pcm_stride, i16 ? nullptr : static_cast<const float *>(in.p),
+                    i16 ? static_cast<const short *>(in.p) : nullptr, in.stride, e->n_active, F * kFrame, st, 32768.f,
+                    r.row, r.rg.hops);
   }
   {
     AnalysisArgs aa = analysis_args(e, F);
     aa.hops = r.rg.hops;
-    ProfScope ps(e, PNB_K_ANALYSIS, st);
-    n += launch_analysis(aa, st);
+    LaunchScope m(e, PNB_K_ANALYSIS, st);
+    launch_analysis(aa, st);
   }
   CK(cudaGetLastError());
-  return n;
+  return PNB_OK;
 }
 
 // The signal path after the network, on st, from the g/r in d_gr: the synthesis of F hops into the caller's PCM rows
 // (out), through r as analysis_half, then the fix-up of the slots that stop short, then the history slide when it falls
-// due.  The fix-up runs before the slide, which moves the window the counters of hop F point at.  Returns the number of
-// launches.
-static int synthesis_half(pnb_engine *e, const Rows &out, int F, const SessionRows &r, cudaStream_t st) {
+// due.  The fix-up runs before the slide, which moves the window the counters of hop F point at.
+static void synthesis_half(pnb_engine *e, const Rows &out, int F, const SessionRows &r, cudaStream_t st) {
   const bool i16 = out.bytes == sizeof(short);
-  int n = 0;
   {
     SynthesisArgs sa = synthesis_args(e, F, i16 ? nullptr : static_cast<float *>(out.p),
                                       i16 ? static_cast<short *>(out.p) : nullptr, out.stride);
     sa.row = r.row;
     sa.hops = r.rg.hops;
-    ProfScope ps(e, PNB_K_SYNTHESIS, st);
-    n += launch_synthesis(sa, st);
+    LaunchScope m(e, PNB_K_SYNTHESIS, st);
+    launch_synthesis(sa, st);
   }
   if (r.rg.n_short) {
-    ProfScope ps(e, PNB_K_SLIDE, st);
-    n += launch_ragged_carry(e, F, r.rg.hops, r.rg.slots, r.rg.n_short, st);
+    LaunchScope m(e, PNB_K_SLIDE, st);
+    launch_ragged_carry(e, F, r.rg.hops, r.rg.slots, r.rg.n_short, st);
   }
-  return n + advance_line(e, F, st);
+  advance_line(e, F, st);
 }
 
 // A network call on st (arguments already checked): the caller's rows into the features buffer, the network hook, its
@@ -732,31 +747,26 @@ static int enqueue_network(pnb_engine *e, const Call &c, cudaStream_t st) {
   const Rows &in = c.in[0], &gr = c.out[0], &sums = c.out[1];
   return enqueue_call(e, F, st, [&]() -> int {
     SessionRows r;
-    int n = call_rows(e, c, st, &r);
-    if (n < 0) return n;
+    if (int rc = call_rows(e, c, st, &r)) return rc;
     const int S = e->S, na = e->n_active;
     const int *frames = nullptr;  // a score call's per-row hop counts, staged like a ragged call's hops
     if (c.frames) { int rc = stage_ints(e, c.frames, (size_t)na, st, &frames); if (rc) return rc; }
     {
-      ProfScope ps(e, PNB_K_STAGE_IN, st);
-      n += launch_rows_stage(e->d_feat, kFeat, static_cast<const float *>(in.p), in.stride, (int)in.width,
-                             c.format == PNB_RNN_RECORDS ? 68 : 0, na, S, F, st, r.row, r.rg.hops);
+      LaunchScope m(e, PNB_K_STAGE_IN, st);
+      launch_rows_stage(e->d_feat, kFeat, static_cast<const float *>(in.p), in.stride, (int)in.width,
+                        c.format == PNB_RNN_RECORDS ? 68 : 0, na, S, F, st, r.row, r.rg.hops);
     }
     CK(cudaGetLastError());
-    {
-      const int q = network(e, F, r.rg.hops, st);
-      if (q < 0) return q;
-      n += q;
-    }
+    if (int rc = network(e, F, r.rg.hops, st)) return rc;
     if (sums.p) {
-      ProfScope ps(e, PNB_K_STAGE_IN, st);
-      n += launch_loss_sums(e->d_gr, static_cast<const float *>(in.p), in.stride, frames, static_cast<double *>(sums.p), na, S, F, st);
+      LaunchScope m(e, PNB_K_STAGE_IN, st);
+      launch_loss_sums(e->d_gr, static_cast<const float *>(in.p), in.stride, frames, static_cast<double *>(sums.p), na, S, F, st);
     }
     if (gr.p) {
-      ProfScope ps(e, PNB_K_STAGE_IN, st);
-      n += launch_rows_store(e->d_gr, 68, static_cast<float *>(gr.p), gr.stride, na, S, F, st, r.slot, r.rg.hops);
+      LaunchScope m(e, PNB_K_STAGE_IN, st);
+      launch_rows_store(e->d_gr, 68, static_cast<float *>(gr.p), gr.stride, na, S, F, st, r.slot, r.rg.hops);
     }
-    return n;
+    return PNB_OK;
   }, false);
 }
 
@@ -769,31 +779,33 @@ static int enqueue_records(pnb_engine *e, const Call &c, cudaStream_t st) {
   return enqueue_call(e, F, st, [&]() -> int {
     const int N = e->S / 2;
     float *line = e->d_pcm + e->line_off;
-    int n = 0;
     {
-      ProfScope ps(e, PNB_K_STAGE_IN, st);
-      n += launch_stage_in(line, e->pcm_stride, nullptr, static_cast<const short *>(noisy.p), noisy.stride, N, F * kFrame, st, 1.f);
-      n += launch_stage_in(line + (size_t)N * e->pcm_stride, e->pcm_stride, nullptr, static_cast<const short *>(speech.p),
-                           speech.stride, N, F * kFrame, st, 1.f);
+      LaunchScope m(e, PNB_K_STAGE_IN, st);
+      launch_stage_in(line, e->pcm_stride, nullptr, static_cast<const short *>(noisy.p), noisy.stride, N, F * kFrame, st, 1.f);
+    }
+    {
+      LaunchScope m(e, PNB_K_STAGE_IN, st);
+      launch_stage_in(line + (size_t)N * e->pcm_stride, e->pcm_stride, nullptr, static_cast<const short *>(speech.p),
+                      speech.stride, N, F * kFrame, st, 1.f);
     }
     AnalysisArgs a = analysis_args(e, F);  // all S streams: the active range of a training-data engine is always S
     a.raw = e->d_raw;
     a.P_rows = N;  // an audio engine's P: the noisy rows (the others have none)
-    { ProfScope ps(e, PNB_K_ANALYSIS, st); n += launch_analysis(a, st); }
+    { LaunchScope m(e, PNB_K_ANALYSIS, st); launch_analysis(a, st); }
     LabelArgs l;
     l.feat = e->d_feat; l.raw = e->d_raw; l.Ex = e->d_Ex; l.tab = e->d_tab; l.n_pairs = N; l.n_frames = F;
     l.records = static_cast<float *>(records.p); l.pair_stride = records.stride;
     l.gr = audio.p ? e->d_gr : nullptr;
-    { ProfScope ps(e, PNB_K_LABELS, st); n += launch_train_labels(l, st); }
+    { LaunchScope m(e, PNB_K_LABELS, st); launch_train_labels(l, st); }
     if (audio.p) {  // denoise.cpp:742-759 on the noisy rows, their labels post-filtered already (no PNB_POSTFILTER here)
       SynthesisArgs s = synthesis_args(e, F, nullptr, static_cast<short *>(audio.p), audio.stride);
       s.n_streams = N;
       s.clamp16 = 1;
-      ProfScope ps(e, PNB_K_SYNTHESIS, st);
-      n += launch_synthesis(s, st);
+      LaunchScope m(e, PNB_K_SYNTHESIS, st);
+      launch_synthesis(s, st);
     }
-    n += advance_line(e, F, st);
-    return n;
+    advance_line(e, F, st);
+    return PNB_OK;
   });
 }
 
@@ -805,26 +817,19 @@ static int enqueue_enhance(pnb_engine *e, const Call &c, cudaStream_t st) {
   const int F = c.F;
   return enqueue_call(e, F, st, [&]() -> int {
     SessionRows r;
-    int n = call_rows(e, c, st, &r);
-    if (n < 0) return n;
-    {
-      const int q = analysis_half(e, c.in[0], F, r, st);
-      if (q < 0) return q;
-      n += q;
-    }
-    {
-      const int q = network(e, F, r.rg.hops, st);
-      if (q < 0) return q;
-      n += q;
-    }
-    n += synthesis_half(e, c.out[0], F, r, st);
+    if (int rc = call_rows(e, c, st, &r)) return rc;
+    if (int rc = analysis_half(e, c.in[0], F, r, st)) return rc;
+    if (int rc = network(e, F, r.rg.hops, st)) return rc;
+    synthesis_half(e, c.out[0], F, r, st);
     const int S = e->S, na = e->n_active;  // the call advances streams [0, na); per-call buffers keep the stride S
-    if (c.gr && r.row)  // [F][na][68] in list order
-      n += launch_gr_gather(e->d_gr, c.gr, r.row, na, S, F, st, r.rg.hops);
-    else if (c.gr)  // [F][na][68] from the [F][S][68] buffer
+    if (c.gr && r.row) {  // [F][na][68] in list order
+      LaunchScope m(e, kUnprofiled, st);
+      launch_gr_gather(e->d_gr, c.gr, r.row, na, S, F, st, r.rg.hops);
+    } else if (c.gr) {  // [F][na][68] from the [F][S][68] buffer
       CK(cudaMemcpy2DAsync(c.gr, (size_t)na * 68 * sizeof(float), e->d_gr, (size_t)S * 68 * sizeof(float), (size_t)na * 68 * sizeof(float), F,
                            cudaMemcpyDeviceToDevice, st));
-    return n;
+    }
+    return PNB_OK;
   });
 }
 
@@ -838,13 +843,11 @@ static int enqueue_analyze(pnb_engine *e, const Call &c, cudaStream_t st) {
   const Rows &feat = c.out[0];
   SessionRows r;
   const int rc = enqueue_call(e, F, st, [&]() -> int {
-    int n = call_rows(e, c, st, &r);
-    if (n < 0) return n;
-    const int q = analysis_half(e, c.in[0], F, r, st);
-    if (q < 0) return q;
-    ProfScope ps(e, PNB_K_STAGE_IN, st);
-    return n + q + launch_rows_store(e->d_feat, kFeat, static_cast<float *>(feat.p), feat.stride, e->n_active, e->S, F, st,
-                                     r.slot, r.rg.hops);
+    if (int rc = call_rows(e, c, st, &r)) return rc;
+    if (int rc = analysis_half(e, c.in[0], F, r, st)) return rc;
+    LaunchScope m(e, PNB_K_STAGE_IN, st);
+    launch_rows_store(e->d_feat, kFeat, static_cast<float *>(feat.p), feat.stride, e->n_active, e->S, F, st, r.slot, r.rg.hops);
+    return PNB_OK;
   }, false);
   if (rc == PNB_OK)
     e->pending = {F, std::vector<int>(c.ids, c.ids + c.n_ids),
@@ -861,14 +864,14 @@ static int enqueue_synthesize(pnb_engine *e, const Call &c, cudaStream_t st) {
   const Rows &gr = c.in[0];
   const int rc = enqueue_call(e, F, st, [&]() -> int {
     SessionRows r;
-    int n = call_rows(e, c, st, &r);
-    if (n < 0) return n;
+    if (int rc = call_rows(e, c, st, &r)) return rc;
     {
-      ProfScope ps(e, PNB_K_STAGE_IN, st);
-      n += launch_rows_stage(e->d_gr, 68, static_cast<const float *>(gr.p), gr.stride, 68, 0, e->n_active, e->S, F, st,
-                             r.row, r.rg.hops);
+      LaunchScope m(e, PNB_K_STAGE_IN, st);
+      launch_rows_stage(e->d_gr, 68, static_cast<const float *>(gr.p), gr.stride, 68, 0, e->n_active, e->S, F, st, r.row,
+                        r.rg.hops);
     }
-    return n + synthesis_half(e, c.out[0], F, r, st);
+    synthesis_half(e, c.out[0], F, r, st);
+    return PNB_OK;
   });
   if (rc == PNB_OK) e->pending = {};
   return rc;
@@ -1148,7 +1151,7 @@ static int round_trip(pnb_engine *e, int k, bool pipelined, H2D h2d, Call call, 
 static int report_status(pnb_engine *e) {
   if (e->h_status[0] & kStatusRejected) {  // reported once: no other stream was affected
     const int slot = e->h_status[1];
-    launch_state_clear_reject(e->d_status, e->stream);
+    launch_state_clear_reject(e->d_status, e->stream);  // uncounted: part of reporting a rejection, not of a call or state operation
     CK(cudaGetLastError());
     CK(cudaStreamSynchronize(e->stream));
     e->h_status[0] &= ~kStatusRejected;
@@ -1329,8 +1332,7 @@ extern "C" int pnb_train_adam(pnb_engine *e, double lr, long long step, void *cu
   if (e->train_open)
     return fail(PNB_ERR_ARG, "accumulated gradients are not finished: pnb_train_finish before pnb_train_adam");
   CK(cudaSetDevice(e->device));
-  const int n = enqueue_ordered(e, (cudaStream_t)cuda_stream, [&] { return train_adam(e, lr, step, (cudaStream_t)cuda_stream); });
-  return n < 0 ? n : PNB_OK;
+  return enqueue_ordered(e, (cudaStream_t)cuda_stream, [&] { return train_adam(e, lr, step, (cudaStream_t)cuda_stream); });
 }
 
 // Accumulation: the held gradient, weighted by the hops its call counted, into the float64 accumulator; and the
@@ -1343,8 +1345,8 @@ extern "C" int pnb_train_accumulate(pnb_engine *e, void *cuda_stream) {
                              "held gradient is already counted");
   CK(cudaSetDevice(e->device));
   { int rc = train_accum_prepare(e); if (rc) return rc; }
-  const int n = enqueue_ordered(e, (cudaStream_t)cuda_stream, [&] { return train_accumulate(e, (cudaStream_t)cuda_stream); });
-  if (n < 0) return n;
+  if (int rc = enqueue_ordered(e, (cudaStream_t)cuda_stream, [&] { return train_accumulate(e, (cudaStream_t)cuda_stream); }))
+    return rc;
   e->train_hops = 0;
   e->train_open = true;
   return PNB_OK;
@@ -1354,8 +1356,8 @@ extern "C" int pnb_train_finish(pnb_engine *e, void *cuda_stream) {
   if (!e->train_open)
     return fail(PNB_ERR_ARG, "nothing was accumulated or imported since the last pnb_train_finish");
   CK(cudaSetDevice(e->device));
-  const int n = enqueue_ordered(e, (cudaStream_t)cuda_stream, [&] { return train_finish(e, (cudaStream_t)cuda_stream); });
-  if (n < 0) return n;
+  if (int rc = enqueue_ordered(e, (cudaStream_t)cuda_stream, [&] { return train_finish(e, (cudaStream_t)cuda_stream); }))
+    return rc;
   e->train_hops = 0;
   e->train_open = false;
   return PNB_OK;
@@ -1377,11 +1379,10 @@ static int train_transfer(pnb_engine *e, int what, void *mem, size_t bytes, bool
     return fail(PNB_ERR_ARG, "%zu bytes, the model has %zu parameters (%zu bytes)", bytes, train_params(e), need);
   CK(cudaSetDevice(e->device));
   if (accum) { int rc = train_accum_prepare(e); if (rc) return rc; }
-  const int n = enqueue_ordered(e, e->stream, [&] {
-    const int rc = accum ? train_accum_copy(e, mem, out, e->stream) : train_copy(e, what, mem, out, e->stream);
-    return rc ? rc : 0;
+  const int rc = enqueue_ordered(e, e->stream, [&] {
+    return accum ? train_accum_copy(e, mem, out, e->stream) : train_copy(e, what, mem, out, e->stream);
   });
-  if (n < 0) return n;
+  if (rc) return rc;
   CK(cudaStreamSynchronize(e->stream));
   if (accum && !out) e->train_open = true;
   return PNB_OK;
@@ -1872,7 +1873,8 @@ extern "C" int pnb_pitch_only_device(const float *d_pitch_buf, size_t stride, lo
   PitchOnlyArgs a;
   a.buf = d_pitch_buf; a.stride = stride; a.n_units = (long)n_units; a.prev_period = d_prev_period; a.prev_gain = d_prev_gain;
   a.T = d_period; a.corr = d_corr; a.gain = d_gain; a.lag = d_lag;
-  if (launch_pitch_only(a, (cudaStream_t)cuda_stream) < 0) return fail(PNB_ERR_CUDA, "pitch_only_kernel could not be configured");
+  // uncounted: there is no engine to count it
+  if (!launch_pitch_only(a, (cudaStream_t)cuda_stream)) return fail(PNB_ERR_CUDA, "pitch_only_kernel could not be configured");
   CK(cudaGetLastError());
   return PNB_OK;
 }

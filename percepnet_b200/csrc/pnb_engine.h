@@ -94,7 +94,7 @@ struct pnb_engine {
     std::vector<int> ids, hops, up;
   };
   PendingSplit pending;
-  long long launches = 0;
+  long long launches = 0;  // kernel launches of the calls and state operations so far (pnb_launch_count; LaunchScope)
   // status word on the device: bit 0 = an activation left the domain in which the reference's tansig_approx is
   // defined (tensor path only; reported as PNB_ERR_DOMAIN by the synchronising entry points, cleared by pnb_reset);
   // bit 1 = pnb_import_states rejected a blob, [1] = the lowest rejected slot (reported once, then cleared; in session
@@ -161,7 +161,7 @@ constexpr bool kStreamState = true, kScratch = false;  // engine_alloc's zero_on
 int engine_fail(int code, const char *msg);
 
 // The network paths' hooks, tensor-core (tc_*, pnb_nn_tc.cu) and fp32 FMA (f32_*, pnb_nn_f32.cu).  Return PNB_OK /
-// a negative error; the network hooks return their launch count.
+// a negative error.
 // prepare: the path's weights and buffers, and the GRU states e->h in its layout
 int tc_prepare(pnb_engine *e, const pnb_model *model);
 int f32_prepare(pnb_engine *e, const pnb_model *model);
@@ -177,7 +177,7 @@ int f32_state_segs(const pnb_engine *e, pnb::StateSeg *seg, int ns);
 
 // PNB_TRAIN_NETWORK (pnb_train.cu).  prepare: after f32_prepare, the trainer's buffers.  grad: the loss sums and the
 // gradient of a call of F hops on windows [0, n_active) (records on the device; frames: device / host copies of the
-// hops per window, or null), returns its launch count.  adam: one step with the held gradient.  copy: what = 0 weights,
+// hops per window, or null).  adam: one step with the held gradient.  copy: what = 0 weights,
 // 1 gradient, 2 m, 3 v between the device and train_params(e) floats of host memory, on st.  accum_prepare: the
 // float64 accumulator, allocated once; accumulate: the held gradient times e->train_hops into it (1 launch); finish:
 // the gradient from it, the accumulator zeroed, and the non-finite check (2 launches); accum_copy: its
@@ -195,10 +195,14 @@ int train_accumulate(pnb_engine *e, cudaStream_t st);
 int train_finish(pnb_engine *e, cudaStream_t st);
 int train_accum_copy(pnb_engine *e, void *mem, bool out, cudaStream_t st);
 
-// RAII marker used by the launch schedule: records an event pair around a launch when profiling
-struct ProfScope {
+// The marker of one kernel launch on behalf of an engine, constructed right before the launch and destroyed right
+// after it: it counts the launch in e->launches and, when profiling and cls is a kernel class, records an event pair
+// around it for that class (kUnprofiled: counted only).  Every launch of a call or state operation has its own marker,
+// and nothing else counts launches.
+constexpr int kUnprofiled = -1;
+struct LaunchScope {
   pnb_engine *e; int idx;
-  ProfScope(pnb_engine *eng, int cls, cudaStream_t st);
-  ~ProfScope();
+  LaunchScope(pnb_engine *eng, int cls, cudaStream_t st);
+  ~LaunchScope();
   cudaStream_t st;
 };

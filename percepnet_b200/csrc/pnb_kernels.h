@@ -63,10 +63,11 @@ struct LabelArgs {
   size_t pair_stride;
   float *gr;               // [F][2N][68] or null: the record's g and r of pair p, frame t at row t*2N + p (its noisy row)
 };
-int launch_train_labels(const LabelArgs &a, cudaStream_t st);
+void launch_train_labels(const LabelArgs &a, cudaStream_t st);
 
 // pitch analysis alone (BASELINE.json config 5): unit u reads buf[u*stride .. +1728), writes T/corr/gain (and the
-// pitch_search lag when lag != null); prev_period / prev_gain null = 0 (a fresh stream)
+// pitch_search lag when lag != null); prev_period / prev_gain null = 0 (a fresh stream).  Returns false, launching
+// nothing, when the kernel cannot be configured.
 struct PitchOnlyArgs {
   const float *buf;
   size_t stride;
@@ -77,33 +78,33 @@ struct PitchOnlyArgs {
   float *corr, *gain;
   int *lag;
 };
-int launch_pitch_only(const PitchOnlyArgs &a, cudaStream_t st);
+bool launch_pitch_only(const PitchOnlyArgs &a, cudaStream_t st);
 
 cudaError_t dsp_configure();
-int launch_analysis(const AnalysisArgs &a, cudaStream_t st);
-int launch_synthesis(const SynthesisArgs &a, cudaStream_t st);
+void launch_analysis(const AnalysisArgs &a, cudaStream_t st);
+void launch_synthesis(const SynthesisArgs &a, cudaStream_t st);
 // row: [n_streams] input row of each slot (session calls), or null: row s.  hops: [n_streams] hops of each slot (ragged
 // session calls), or null: slot s copies hops[s] * 480 samples instead of n_samples
-int launch_stage_in(float *pcm, size_t pcm_stride, const float *in, const short *in16, size_t in_stride,
-                    int n_streams, int n_samples, cudaStream_t st, float i16_div = 32768.f, const int *row = nullptr,
-                    const int *hops = nullptr);
-int launch_slide_history(float *pcm, size_t pcm_stride, int n_streams, int n_samples, cudaStream_t st);
+void launch_stage_in(float *pcm, size_t pcm_stride, const float *in, const short *in16, size_t in_stride,
+                     int n_streams, int n_samples, cudaStream_t st, float i16_div = 32768.f, const int *row = nullptr,
+                     const int *hops = nullptr);
+void launch_slide_history(float *pcm, size_t pcm_stride, int n_streams, int n_samples, cudaStream_t st);
 
 // ---- layout moves of the network and split calls (pnb_rnn_io.cu) ---------------------------
 // rows [0, n_streams) of `in` (n_frames hops of in_width floats each) -> dst [F][S][w], w = 70 (features, or records
 // with in_width 138) or 68 (g/r); the first n_scaled values of each hop are multiplied by 30 (records: 68, else 0).
 // row: [n_streams] the input row of each slot (session calls), or null: row s.  hops (with row only): [n_streams] hops
 // of each slot, or null: n_frames; slot s gets zeros for hops >= hops[s], whose input is not read
-int launch_rows_stage(float *dst, int w, const float *in, size_t in_stride, int in_width, int n_scaled, int n_streams,
-                      int S, int n_frames, cudaStream_t st, const int *row = nullptr, const int *hops = nullptr);
+void launch_rows_stage(float *dst, int w, const float *in, size_t in_stride, int in_width, int n_scaled, int n_streams,
+                       int S, int n_frames, cudaStream_t st, const int *row = nullptr, const int *hops = nullptr);
 // src [F][S][w] -> rows [0, n_streams) of `out`, n_frames x w floats each; w = 68 (g/r) or 70 (features).  slot:
 // [n_streams] the slot of each output row (session calls), or null: slot r.  hops (with slot only): [n_streams] hops of
 // each slot, or null: n_frames; a row is zero for the hops its slot did not run
-int launch_rows_store(const float *src, int w, float *out, size_t out_stride, int n_streams, int S, int n_frames,
-                      cudaStream_t st, const int *slot = nullptr, const int *hops = nullptr);
+void launch_rows_store(const float *src, int w, float *out, size_t out_stride, int n_streams, int S, int n_frames,
+                       cudaStream_t st, const int *slot = nullptr, const int *hops = nullptr);
 // rnn_train.py's CustomLoss sums of rows [0, n_streams): gr [F][S][68] against the labels rec[t][70..137] of row i's
 // first frames[i] hops (frames null: all n_frames) -> sums[i] = {sum dg^2, sum dg^4, sum dr^2, count} in float64
-int launch_loss_sums(const float *gr, const float *rec, size_t rec_stride, const int *frames, double *sums, int n_streams,
-                     int S, int n_frames, cudaStream_t st);
+void launch_loss_sums(const float *gr, const float *rec, size_t rec_stride, const int *frames, double *sums, int n_streams,
+                      int S, int n_frames, cudaStream_t st);
 
 }  // namespace pnb

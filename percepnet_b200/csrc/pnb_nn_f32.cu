@@ -192,14 +192,13 @@ __global__ void __launch_bounds__(256) gemm_f32_kernel(GemmArgs g) {
   }
 }
 
-int launch_gemm_f32(const GemmArgs &g, cudaStream_t st) {
+void launch_gemm_f32(const GemmArgs &g, cudaStream_t st) {
   dim3 grid((g.N + BN - 1) / BN, g.n_slots * ((g.M + BM - 1) / BM));
   bool vec = true;
   for (int i = 0; i < g.n_seg; i++)
     if ((g.seg[i].ldb & 3) || (reinterpret_cast<uintptr_t>(g.seg[i].B) & 15)) vec = false;
   if (vec) gemm_f32_kernel<true><<<grid, 256, 0, st>>>(g);
   else gemm_f32_kernel<false><<<grid, 256, 0, st>>>(g);
-  return 1;
 }
 
 // fc 70 -> 128 (+relu): one thread per (stream, output); the 70-float feature row is broadcast, the
@@ -231,10 +230,9 @@ __global__ void __launch_bounds__(128) fc_f32_kernel(const float *__restrict__ f
     if (r0 + rr < M) out[(size_t)(r0 + rr) * N + n] = a[rr] < 0.f ? 0.f : a[rr];
 }
 
-int launch_fc_f32(const float *feat, const float *W, const float *bias, float *out, int M, int K, int N, int n_slots,
-                  size_t slot_stride, cudaStream_t st) {
+void launch_fc_f32(const float *feat, const float *W, const float *bias, float *out, int M, int K, int N, int n_slots,
+                   size_t slot_stride, cudaStream_t st) {
   fc_f32_kernel<<<dim3((M + 3) / 4, n_slots), 128, 0, st>>>(feat, W, bias, out, M, K, N, slot_stride);
-  return 1;
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -413,7 +411,8 @@ __global__ void __launch_bounds__(CH_THREADS, RT == 8 ? 2 : 4) gru_chain_f32_ker
 
 size_t f32_chain_smem(int rt) { return rt == 8 ? sizeof(ChainSmem<8>) : sizeof(ChainSmem<1>); }
 
-int launch_gru_chain_f32(const F32ChainArgs &a, int rt, int sm_count, cudaStream_t st) {
+// Returns false, launching nothing, when the kernel cannot be configured.
+bool launch_gru_chain_f32(const F32ChainArgs &a, int rt, int sm_count, cudaStream_t st) {
   static int occ8 = 0, occ1 = 0;
   int &occ = rt == 8 ? occ8 : occ1;
   const size_t smem = f32_chain_smem(rt);
@@ -426,14 +425,14 @@ int launch_gru_chain_f32(const F32ChainArgs &a, int rt, int sm_count, cudaStream
       e1 = cudaFuncSetAttribute(gru_chain_f32_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
       e2 = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, gru_chain_f32_kernel<1>, CH_THREADS, smem);
     }
-    if (e1 != cudaSuccess || e2 != cudaSuccess || occ < 1) { occ = 0; return -1; }
+    if (e1 != cudaSuccess || e2 != cudaSuccess || occ < 1) { occ = 0; return false; }
   }
   // the dependency waits need every block of the grid resident: never more blocks than fit at once
   int grid = occ * sm_count;
   if (grid > a.order.units()) grid = a.order.units();
   if (rt == 8) gru_chain_f32_kernel<8><<<grid, CH_THREADS, smem, st>>>(a);
   else gru_chain_f32_kernel<1><<<grid, CH_THREADS, smem, st>>>(a);
-  return 1;
+  return true;
 }
 
 }  // namespace pnb
@@ -511,19 +510,18 @@ static int run_chunk(pnb_engine *e, int h0, int n, const int *hops, cudaStream_t
   // all streams active: the rows of the n slots are one flat range; otherwise the first na rows of each slot
   const int rows = na == S ? n * S : na, slots = na == S ? 1 : n;
   const float *tbl = e->tansig();
-  int nl = 0;
   // fc -> slots 4.. (slots 0..3 hold the last four hops' outputs)
-  { ProfScope ps(e, PNB_K_FC, st); nl += launch_fc_f32(e->d_feat + (size_t)h0 * S * kFeat, e->fc.W, e->fc.b, f.ring_fc + (size_t)4 * S * 128, rows, 70, 128, slots, S, st); }
+  { LaunchScope m(e, PNB_K_FC, st); launch_fc_f32(e->d_feat + (size_t)h0 * S * kFeat, e->fc.W, e->fc.b, f.ring_fc + (size_t)4 * S * 128, rows, 70, 128, slots, S, st); }
   GemmArgs g;
   memset(&g, 0, sizeof g);
   g.M = rows; g.n_slots = slots; g.slot_stride = S; g.tansig = tbl;
   // conv1: tap q of hop t reads fc slot t + q (oldest first, nnet.cpp:182-200; weights [tap][c][n]) -> c1 slots 2..
   for (int q = 0; q < 5; q++) g.seg[q] = seg(f.ring_fc + (size_t)q * S * 128, 128, f.conv1.W + (size_t)q * 128 * 512, 512, 128);
   g.n_seg = 5; g.N = 512; g.C = f.ring_c1 + (size_t)2 * S * 512; g.ldc = 512; g.bias = f.conv1.b; g.act = PNB_ACT_RELU;
-  { ProfScope ps(e, PNB_K_GEMM_F32, st); nl += launch_gemm_f32(g, st); }
+  { LaunchScope m(e, PNB_K_GEMM_F32, st); launch_gemm_f32(g, st); }
   for (int q = 0; q < 3; q++) g.seg[q] = seg(f.ring_c1 + (size_t)q * S * 512, 512, f.conv2.W + (size_t)q * 512 * 512, 512, 512);
   g.n_seg = 3; g.N = 512; g.C = f.c2_all; g.ldc = 512; g.bias = f.conv2.b; g.act = PNB_ACT_TANH;
-  { ProfScope ps(e, PNB_K_GEMM_F32, st); nl += launch_gemm_f32(g, st); }
+  { LaunchScope m(e, PNB_K_GEMM_F32, st); launch_gemm_f32(g, st); }
 
   // stacked GRUs: each consumes the freshly updated state of the one below (SURVEY.md App. C.10)
   F32ChainArgs a;
@@ -547,19 +545,18 @@ static int run_chunk(pnb_engine *e, int h0, int n, const int *hops, cudaStream_t
     }
   }
   {
-    ProfScope ps(e, PNB_K_GEMM_F32, st);
-    if (launch_gru_chain_f32(a, f.rt, e->sm_count, st) < 0) return engine_fail(PNB_ERR_CUDA, "cannot configure the fp32 GRU chain kernel");
-    nl++;
+    LaunchScope m(e, PNB_K_GEMM_F32, st);
+    if (!launch_gru_chain_f32(a, f.rt, e->sm_count, st)) return engine_fail(PNB_ERR_CUDA, "cannot configure the fp32 GRU chain kernel");
   }
   // fc_gb on [conv2, gru1, gru2, gru3, gru_gb] (rnn.cpp:73-78), fc_rb on gru_rb (rnn.cpp:80); state after hop t = slot t+1
   float *gr = e->d_gr + (size_t)h0 * S * 68;
   g.seg[0] = seg(f.c2_all, 512, f.fc_gb.W, 34, 512);
   for (int q = 1; q < 5; q++) g.seg[q] = seg(e->h[q - 1] + (size_t)S * 512, 512, f.fc_gb.W + (size_t)q * 512 * 34, 34, 512);
   g.n_seg = 5; g.N = 34; g.C = gr; g.ldc = 68; g.bias = f.fc_gb.b; g.act = PNB_ACT_SIGMOID;
-  { ProfScope ps(e, PNB_K_GEMM_F32, st); nl += launch_gemm_f32(g, st); }
+  { LaunchScope m(e, PNB_K_GEMM_F32, st); launch_gemm_f32(g, st); }
   g.seg[0] = seg(e->h[4] + (size_t)S * 128, 128, f.fc_rb.W, 34, 128);
   g.n_seg = 1; g.N = 34; g.C = gr + 34; g.ldc = 68; g.bias = f.fc_rb.b; g.act = PNB_ACT_SIGMOID;
-  { ProfScope ps(e, PNB_K_GEMM_F32, st); nl += launch_gemm_f32(g, st); }
+  { LaunchScope m(e, PNB_K_GEMM_F32, st); launch_gemm_f32(g, st); }
   // carry: the last 4 fc / 2 conv1 slots and the last state slot move to the front, conv2's output of the last hop is
   // kept for the tap.  In a ragged call a row that stopped inside the chunk takes its own last hop's slots, one that
   // stopped in an earlier chunk keeps its front slots
@@ -570,20 +567,16 @@ static int run_chunk(pnb_engine *e, int h0, int n, const int *hops, cudaStream_t
   add_carry_seg(c, f.ring_c1, f.ring_c1, 512 * 4, na, S, 2, n);
   for (int li = 0; li < 5; li++) add_carry_seg(c, e->h[li], e->h[li], kGruH[li] * 4, na, S, 1, n);
   add_carry_seg(c, e->c2, f.c2_all, 512 * 4, na, S, 1, n - 1);
-  { ProfScope ps(e, PNB_K_F32_CARRY, st); nl += launch_slot_carry(c, e->sm_count, st); }
-  return nl;
+  { LaunchScope m(e, PNB_K_F32_CARRY, st); launch_slot_carry(c, e->sm_count, st); }
+  return PNB_OK;
 }
 
 // The network of a call of F hops: chunks of up to chunk_hops(e) hops, in order.
 int f32_network(pnb_engine *e, int F, const int *hops, cudaStream_t st) {
   const int C = chunk_hops(e);
-  int nl = 0;
-  for (int h0 = 0; h0 < F; h0 += C) {
-    const int q = run_chunk(e, h0, F - h0 < C ? F - h0 : C, hops, st);
-    if (q < 0) return q;
-    nl += q;
-  }
-  return nl;
+  for (int h0 = 0; h0 < F; h0 += C)
+    if (int rc = run_chunk(e, h0, F - h0 < C ? F - h0 : C, hops, st)) return rc;
+  return PNB_OK;
 }
 
 int f32_network_launches(const pnb_engine *e, int F) {

@@ -1118,10 +1118,12 @@ int tc_state_segs(const pnb_engine *e, StateSeg *seg, int ns) {
   return ns;
 }
 
+// One persistent tensor-core launch: a dense layer or the GRU chain, each a tc_gemm_kernel record in the profile.
 template <typename K, typename A>
 static int tc_launch(pnb_engine *e, K kernel, const A &a, int units, size_t smem, cudaStream_t st) {
   int grid = units < e->sm_count ? units : e->sm_count;  // persistent: one CTA per SM
   if (grid < 1) grid = 1;
+  LaunchScope m(e, PNB_K_TC_GEMM, st);
   kernel<<<grid, kTcThreads, smem, st>>>(a);
   TCK(cudaGetLastError());
   return PNB_OK;
@@ -1149,20 +1151,18 @@ static TcSeg mkseg(int a_map, int b_map, int K, int a_k0, int b_k0, int a_row0, 
   return s;
 }
 
-// ---- the network of a call of F hops, in phases; each returns its number of launches or a negative error ------------
+// ---- the network of a call of F hops, in phases; each returns PNB_OK or a negative error --------------------------
 // The non-recurrent front (rnn.cpp:50-52 on F S rows): fc -> conv1 -> conv2.  Hop t of the call lives in slot t of the
 // per-call buffers.
 static int tc_front(pnb_engine *e, int F, const int *hops, cudaStream_t st) {
   pnb_tc_state *t = e->tc.get();
   const int S = e->S, Fm = e->Fmax, na = e->n_active;
   const float *tbl = e->tansig();
-  int nl = 0, rc;
   {  // fc (fp32 FMA on the CUDA cores) -> bf16 terms at slots 4 ..
     const int rows = na == S ? F * S : na, slots = na == S ? 1 : F;  // per grid.y slot
-    ProfScope ps(e, PNB_K_TC_AUX, st);
+    LaunchScope m(e, PNB_K_TC_AUX, st);
     fc_split_kernel<<<dim3((rows + FC_ROWS - 1) / FC_ROWS, slots), 128, 0, st>>>(e->d_feat, e->fc.W, e->fc.b,
                                                     t->fc_all + (size_t)4 * S * 128, rows, (size_t)(Fm + 4) * S, (size_t)S);
-    nl++;
   }
   TcArgs a;
   // conv1: tap q of hop t reads fc slot t + q (oldest first, nnet.cpp:182-200); output -> c1 slots 2 + t
@@ -1173,11 +1173,7 @@ static int tc_front(pnb_engine *e, int F, const int *hops, cudaStream_t st) {
   a.n_seg = 5; a.b_term_rows = 512; a.out_scale = 1.f; a.tansig = tbl;
   a.bias = t->bias_pad; a.act = PNB_ACT_RELU; a.N = 512;
   a.out_b = t->c1_all; a.out_row0 = 2 * S; a.out_plane_rows = (Fm + 2) * S; a.out_terms = kConvTerms; a.wide = t->wide;
-  {
-    ProfScope ps(e, PNB_K_TC_GEMM, st);
-    if ((rc = tc_launch_dense<DENSE_BN, true, DENSE_STAGES, DENSE_STAGES3>(e, a, F, 512 / DENSE_BN, st))) return rc;
-    nl++;
-  }
+  if (int rc = tc_launch_dense<DENSE_BN, true, DENSE_STAGES, DENSE_STAGES3>(e, a, F, 512 / DENSE_BN, st)) return rc;
   // conv2: three taps -> tanh -> fp16 terms (gru1 / gru_rb / fc_gb inputs); fp32 copy of the call's last hop (of each
   // row's last hop in a ragged call, whose frozen hops neither store nor raise the domain bit)
   memset(&a, 0, sizeof a);
@@ -1189,12 +1185,7 @@ static int tc_front(pnb_engine *e, int F, const int *hops, cudaStream_t st) {
   a.out_f32 = e->c2; a.ldc = 512; a.f32_row0 = (F - 1) * S;
   a.out_h = t->c2_h; a.out_row0 = 0; a.out_plane_rows = Fm * S; a.wide = t->wide;
   a.hops = hops;
-  {
-    ProfScope ps(e, PNB_K_TC_GEMM, st);
-    if ((rc = tc_launch_dense<DENSE_BN, true, DENSE_STAGES, DENSE_STAGES3>(e, a, F, 512 / DENSE_BN, st))) return rc;
-    nl++;
-  }
-  return nl;
+  return tc_launch_dense<DENSE_BN, true, DENSE_STAGES, DENSE_STAGES3>(e, a, F, 512 / DENSE_BN, st);
 }
 
 // The recurrent part: five GRUs per hop (rnn.cpp:58-71) in one persistent launch.  State slot t holds the state
@@ -1236,12 +1227,7 @@ static int tc_gru_chain(pnb_engine *e, int F, const int *hops, cudaStream_t st) 
       L.x_map[1] = 0; L.x_kb[1] = 512 / CBK; L.x_bk0[1] = 512; L.x_row1[1] = 0; L.x_term_rows[1] = c2_terms;
     }
   }
-  {
-    ProfScope ps(e, PNB_K_TC_GEMM, st);
-    int rc = tc_launch(e, gru_chain_kernel, a, a.order.units(), tc_smem_bytes<GRU_STAGES, GRU_STAGES * GruStage::kBytes>(), st);
-    if (rc) return rc;
-  }
-  return 1;
+  return tc_launch(e, gru_chain_kernel, a, a.order.units(), tc_smem_bytes<GRU_STAGES, GRU_STAGES * GruStage::kBytes>(), st);
 }
 
 // The two 34-wide output layers (rnn.cpp:73-80; N padded to 48, fp16 two-term split, sigmoid epilogue).
@@ -1250,7 +1236,6 @@ static int tc_out(pnb_engine *e, int F, const int *, cudaStream_t st) {
   const int S = e->S, Fm = e->Fmax;
   const float *tbl = e->tansig();
   const int h_terms = (Fm + 1) * S;
-  int nl = 0, rc;
   TcArgs a;
   memset(&a, 0, sizeof a);
   a.maps[0] = t->m_c2;
@@ -1260,23 +1245,14 @@ static int tc_out(pnb_engine *e, int F, const int *, cudaStream_t st) {
   for (int q = 1; q < 5; q++) a.seg[q] = mkseg(q, 5, 512, 0, q * 512, S, h_terms);  // state after hop t = slot t+1
   a.n_seg = 5; a.b_term_rows = SMALL_BN; a.out_scale = t->scale_gb; a.tansig = tbl;
   a.bias = t->bias_pad + 1024; a.act = PNB_ACT_SIGMOID; a.N = 34; a.ldc = 68; a.out_f32 = e->d_gr;
-  {
-    ProfScope ps(e, PNB_K_TC_GEMM, st);
-    if ((rc = tc_launch_dense<SMALL_BN, false, SMALL_STAGES, 0>(e, a, F, 1, st))) return rc;
-    nl++;
-  }
+  if (int rc = tc_launch_dense<SMALL_BN, false, SMALL_STAGES, 0>(e, a, F, 1, st)) return rc;
   memset(&a, 0, sizeof a);
   a.maps[0] = t->m_h[4];
   a.maps[1] = t->m_wrb;
   a.seg[0] = mkseg(0, 1, 128, 0, 0, S, h_terms);
   a.n_seg = 1; a.b_term_rows = SMALL_BN; a.out_scale = t->scale_rb; a.tansig = tbl;
   a.bias = t->bias_pad + 1072; a.act = PNB_ACT_SIGMOID; a.N = 34; a.ldc = 68; a.out_f32 = e->d_gr + 34;
-  {
-    ProfScope ps(e, PNB_K_TC_GEMM, st);
-    if ((rc = tc_launch_dense<SMALL_BN, false, SMALL_STAGES, 0>(e, a, F, 1, st))) return rc;
-    nl++;
-  }
-  return nl;
+  return tc_launch_dense<SMALL_BN, false, SMALL_STAGES, 0>(e, a, F, 1, st);
 }
 
 // End of a call of F hops: the last 4 fc / 2 conv1 hop slots and the last state slot move to the front (in a ragged
@@ -1297,18 +1273,15 @@ static int tc_carry(pnb_engine *e, int F, const int *hops, cudaStream_t st) {
       __half *b = t->h_all[li] + (size_t)tm * (Fm + 1) * S * kGruH[li];
       add_carry_seg(c, b, b, kGruH[li] * 2, na, S, 1, F);
     }
-  ProfScope ps(e, PNB_K_TC_AUX, st);
-  return launch_slot_carry(c, e->sm_count, st);
+  LaunchScope m(e, PNB_K_TC_AUX, st);
+  launch_slot_carry(c, e->sm_count, st);
+  return PNB_OK;
 }
 
 int tc_network(pnb_engine *e, int F, const int *hops, cudaStream_t st) {
-  int n = 0;
-  for (int (*phase)(pnb_engine *, int, const int *, cudaStream_t) : {tc_front, tc_gru_chain, tc_out, tc_carry}) {
-    const int q = phase(e, F, hops, st);
-    if (q < 0) return q;
-    n += q;
-  }
-  return n;
+  for (int (*phase)(pnb_engine *, int, const int *, cudaStream_t) : {tc_front, tc_gru_chain, tc_out, tc_carry})
+    if (int rc = phase(e, F, hops, st)) return rc;
+  return PNB_OK;
 }
 
 int tc_network_launches(const pnb_engine *, int) { return 7; }  // fc, conv1, conv2, GRU chain, fc_gb, fc_rb, carry

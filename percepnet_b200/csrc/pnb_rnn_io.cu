@@ -107,12 +107,11 @@ static void rows_stage(unsigned blocks, float *dst, const float *in, size_t in_s
   if (row) rows_stage_kernel<W, true><<<blocks, 256, 0, st>>>(dst, in, in_stride, in_width, n_scaled, n, S, F, row, hops);
   else rows_stage_kernel<W, false><<<blocks, 256, 0, st>>>(dst, in, in_stride, in_width, n_scaled, n, S, F, nullptr, nullptr);
 }
-int launch_rows_stage(float *dst, int w, const float *in, size_t in_stride, int in_width, int n_scaled, int n_streams,
-                      int S, int n_frames, cudaStream_t st, const int *row, const int *hops) {
+void launch_rows_stage(float *dst, int w, const float *in, size_t in_stride, int in_width, int n_scaled, int n_streams,
+                       int S, int n_frames, cudaStream_t st, const int *row, const int *hops) {
   const unsigned blocks = copy_blocks((long long)n_frames * n_streams * w);
   if (w == kFeat) rows_stage<kFeat>(blocks, dst, in, in_stride, in_width, n_scaled, n_streams, S, n_frames, row, hops, st);
   else rows_stage<68>(blocks, dst, in, in_stride, in_width, n_scaled, n_streams, S, n_frames, row, hops, st);
-  return 1;
 }
 
 template <int W>
@@ -121,19 +120,17 @@ static void rows_store(unsigned blocks, const float *src, float *out, size_t out
   if (slot) rows_store_kernel<W, true><<<blocks, 256, 0, st>>>(src, out, out_stride, n, S, F, slot, hops);
   else rows_store_kernel<W, false><<<blocks, 256, 0, st>>>(src, out, out_stride, n, S, F, nullptr, nullptr);
 }
-int launch_rows_store(const float *src, int w, float *out, size_t out_stride, int n_streams, int S, int n_frames,
-                      cudaStream_t st, const int *slot, const int *hops) {
+void launch_rows_store(const float *src, int w, float *out, size_t out_stride, int n_streams, int S, int n_frames,
+                       cudaStream_t st, const int *slot, const int *hops) {
   const unsigned blocks = copy_blocks((long long)n_frames * n_streams * w);
   if (w == kFeat) rows_store<kFeat>(blocks, src, out, out_stride, n_streams, S, n_frames, slot, hops, st);
   else rows_store<68>(blocks, src, out, out_stride, n_streams, S, n_frames, slot, hops, st);
-  return 1;
 }
 
-int launch_loss_sums(const float *gr, const float *rec, size_t rec_stride, const int *frames, double *sums, int n_streams,
-                     int S, int n_frames, cudaStream_t st) {
+void launch_loss_sums(const float *gr, const float *rec, size_t rec_stride, const int *frames, double *sums, int n_streams,
+                      int S, int n_frames, cudaStream_t st) {
   loss_sums_kernel<<<(unsigned)(((long long)n_streams * 32 + 255) / 256), 256, 0, st>>>(gr, rec, rec_stride, frames, sums,
                                                                                       n_streams, S, n_frames);
-  return 1;
 }
 
 }  // namespace pnb

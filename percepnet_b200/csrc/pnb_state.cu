@@ -361,48 +361,40 @@ int state_segs(const pnb_engine *e, StateSeg *seg) {
   return (e->flags & PNB_NN_TENSOR) ? tc_state_segs(e, seg, ns) : f32_state_segs(e, seg, ns);
 }
 
-int launch_state_check(const StateArgs &a, cudaStream_t st) {
+void launch_state_check(const StateArgs &a, cudaStream_t st) {
   state_check_kernel<<<a.n, 256, 0, st>>>(a);
-  return 1;
 }
-int launch_state_move(const StateArgs &a, cudaStream_t st) {
+void launch_state_move(const StateArgs &a, cudaStream_t st) {
   const long long warps = (long long)a.n * a.n_seg;
   state_move_kernel<<<(unsigned)((warps + kWarpsPerBlock - 1) / kWarpsPerBlock), 32 * kWarpsPerBlock, 0, st>>>(a);
-  return 1;
 }
-int launch_session_move(const StateArgs &a, cudaStream_t st) {
+void launch_session_move(const StateArgs &a, cudaStream_t st) {
   const long long warps = (long long)a.n * a.n_seg;
   session_move_kernel<<<(unsigned)((warps + kWarpsPerBlock - 1) / kWarpsPerBlock), 32 * kWarpsPerBlock, 0, st>>>(a);
-  return 1;
 }
-int launch_session_blob(const StateArgs &a, cudaStream_t st) {
+void launch_session_blob(const StateArgs &a, cudaStream_t st) {
   session_blob_kernel<<<a.n, 256, 0, st>>>(a);
-  return 1;
 }
-int launch_gr_gather(const float *src, float *dst, const int *row, int k, int S, int F, cudaStream_t st, const int *hops) {
+void launch_gr_gather(const float *src, float *dst, const int *row, int k, int S, int F, cudaStream_t st, const int *hops) {
   const long long total = (long long)F * k * 68;
   const long long blocks = (total + 255) / 256;
   gr_gather_kernel<<<(unsigned)(blocks < 4096 ? blocks : 4096), 256, 0, st>>>(src, dst, row, k, S, F, hops);
-  return 1;
 }
 
 // Beside state_segs: the same places, at the counters of the call's start.
-int launch_ragged_carry(const pnb_engine *e, int F, const int *d_hops, const int *d_slots, int n, cudaStream_t st) {
+void launch_ragged_carry(const pnb_engine *e, int F, const int *d_hops, const int *d_slots, int n, cudaStream_t st) {
   RaggedArgs a;
   memset(&a, 0, sizeof a);
   a.pcm = e->d_pcm; a.pcm_stride = e->pcm_stride; a.line_off = e->line_off;
   a.zring = e->d_zring; a.ering = e->d_ering; a.ring = e->ring; a.S = e->S; a.F = F; a.hop0 = e->hop;
   a.hops = d_hops; a.slots = d_slots;
   ragged_carry_kernel<<<n, kRaggedThreads, 0, st>>>(a);
-  return 1;
 }
-int launch_slot_carry(const SlotCarry &c, int sm_count, cudaStream_t st) {
+void launch_slot_carry(const SlotCarry &c, int sm_count, cudaStream_t st) {
   slot_carry_kernel<<<2 * sm_count, 256, 0, st>>>(c);
-  return 1;
 }
-int launch_state_clear_reject(int *status, cudaStream_t st) {
+void launch_state_clear_reject(int *status, cudaStream_t st) {
   state_clear_reject_kernel<<<1, 1, 0, st>>>(status);
-  return 1;
 }
 
 }  // namespace pnb

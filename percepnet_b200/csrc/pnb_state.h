@@ -104,21 +104,21 @@ constexpr int kNoRejectedSlot = 0x7F7F7F7F;  // status[1] when nothing was rejec
 // The pieces of a stream's state in engine e at its current hop / line offset (host counters committed when a call is
 // enqueued, so the list is right in stream order); returns their number (<= kMaxStateSegs).
 int state_segs(const pnb_engine *e, StateSeg *seg);
-int launch_state_check(const StateArgs &a, cudaStream_t st);
-int launch_state_move(const StateArgs &a, cudaStream_t st);
-int launch_state_clear_reject(int *status, cudaStream_t st);
+void launch_state_check(const StateArgs &a, cudaStream_t st);
+void launch_state_move(const StateArgs &a, cudaStream_t st);
+void launch_state_clear_reject(int *status, cudaStream_t st);
 // session pool: the state launch of a call (a.n moves), the parking-blob operations (a.n sessions), and the g/r of a
 // call in list order ([F][k][68] from the engine's [F][S][68])
-int launch_session_move(const StateArgs &a, cudaStream_t st);
-int launch_session_blob(const StateArgs &a, cudaStream_t st);
+void launch_session_move(const StateArgs &a, cudaStream_t st);
+void launch_session_blob(const StateArgs &a, cudaStream_t st);
 // hops: [k] hops of each slot in a ragged call (entries t >= hops[p] are written as zeros), or null
-int launch_gr_gather(const float *src, float *dst, const int *row, int k, int S, int F, cudaStream_t st,
-                     const int *hops = nullptr);
+void launch_gr_gather(const float *src, float *dst, const int *row, int k, int S, int F, cudaStream_t st,
+                      const int *hops = nullptr);
 // The fix-up of a ragged session call (pnb_process_sessions_ragged_*), enqueued after synthesis and before the history
 // slide, with the engine's hop counter and line offset still those of the call's start.  The n slots at d_slots stopped
 // after hops[p] < F hops; the pieces of their state that sit where the counters say (state_segs) move from where hop
 // hops[p] left them to where hop F would have put them.  One launch.
-int launch_ragged_carry(const pnb_engine *e, int F, const int *d_hops, const int *d_slots, int n, cudaStream_t st);
+void launch_ragged_carry(const pnb_engine *e, int F, const int *d_hops, const int *d_slots, int n, cudaStream_t st);
 
 // The carry at the end of a network chunk of n hops (hops [h0, h0 + n) of the call), both network paths: the hop slots
 // the next chunk reads first move to the front of their buffers, and the chain's counters return to zero.  Segment g
@@ -141,7 +141,7 @@ inline void add_carry_seg(SlotCarry &c, void *dst, const void *src, size_t row_b
   c.seg[c.n_seg++] = SlotSeg{static_cast<uint4 *>(dst), static_cast<const uint4 *>(src), n_rows * row_bytes / 16,
                              S * row_bytes / 16, row_bytes / 16, n_slots, from};
 }
-int launch_slot_carry(const SlotCarry &c, int sm_count, cudaStream_t st);
+void launch_slot_carry(const SlotCarry &c, int sm_count, cudaStream_t st);
 // Parking blobs are engine-owned: padded to 16 bytes
 constexpr size_t kParkStride = (sizeof(StreamState) + 15) / 16 * 16;
 

@@ -536,7 +536,6 @@ TSeg tseg(const float *A, size_t lda, const float *B, size_t ldb, int K) { retur
 struct Launcher {
   pnb_engine *e;
   cudaStream_t st;
-  int n = 0;
   cudaError_t err = cudaSuccess;
   void check() { if (err == cudaSuccess) err = cudaGetLastError(); }
 
@@ -549,9 +548,11 @@ struct Launcher {
     g.n_seg = n_seg; g.M = M; g.N = N; g.parts = 1; g.C = C; g.ldc = ldc; g.accumulate = acc; g.bias = bias;
     g.epi = epi; g.aux = aux; g.ld_aux = ld_aux; g.pre = pre;
     dim3 grid((N + TBN - 1) / TBN, (M + TBM - 1) / TBM, 1);
-    if (tb) train_gemm_kernel<false, true><<<grid, 256, 0, st>>>(g);
-    else train_gemm_kernel<false, false><<<grid, 256, 0, st>>>(g);
-    n++;
+    {
+      LaunchScope m(e, kUnprofiled, st);
+      if (tb) train_gemm_kernel<false, true><<<grid, 256, 0, st>>>(g);
+      else train_gemm_kernel<false, false><<<grid, 256, 0, st>>>(g);
+    }
     check();
   }
   // dst[M x N] (contiguous) = X^T dY over R rows: X [R][ldx] (null: ones, a bias gradient with M = 1), dY [R][ldy].
@@ -570,14 +571,14 @@ struct Launcher {
     g.seg[0] = tseg(X, ldx, dY, ldy, R);
     g.n_seg = 1; g.M = M; g.N = N; g.parts = parts; g.C = e->train->part; g.ldc = N;
     dim3 grid((N + TBN - 1) / TBN, (M + TBM - 1) / TBM, parts);
-    train_gemm_kernel<true, false><<<grid, 256, 0, st>>>(g);
+    { LaunchScope m(e, kUnprofiled, st); train_gemm_kernel<true, false><<<grid, 256, 0, st>>>(g); }
     const size_t cnt = (size_t)M * N;
-    train_parts_kernel<<<blocks_for(cnt), 256, 0, st>>>(e->train->part, parts, cnt, dst);
-    n += 2;
+    { LaunchScope m(e, kUnprofiled, st); train_parts_kernel<<<blocks_for(cnt), 256, 0, st>>>(e->train->part, parts, cnt, dst); }
     check();
   }
   template <int JU>
   void rec_launch(const RecArgs &a, int G, bool fwd) {
+    LaunchScope m(e, kUnprofiled, st);
     if (fwd) gru_fwd_rec_kernel<JU><<<G, 256, fwd_smem(a.H, JU), st>>>(a);
     else gru_bwd_rec_kernel<JU><<<G, 256, bwd_smem(a.H, JU), st>>>(a);
   }
@@ -590,7 +591,6 @@ struct Launcher {
       case 8: rec_launch<8>(a, G, fwd); break;
       default: rec_launch<16>(a, G, fwd); break;
     }
-    n++;
     check();
   }
 };
@@ -603,6 +603,7 @@ int train_grad(pnb_engine *e, const float *rec, size_t rec_stride, const int *fr
   pnb_train_state &s = *e->train;
   const int n = e->n_active, R = F * n;
   const size_t nb = (size_t)n;
+  const long long launches0 = e->launches;
   Launcher L{e, st};
   float *const *P = s.param;
   float *G = s.grad;
@@ -617,9 +618,8 @@ int train_grad(pnb_engine *e, const float *rec, size_t rec_stride, const int *fr
   TCK(cudaMemsetAsync(s.ea + (size_t)R * 512, 0, 4 * nb * 512 * sizeof(float), st));
 
   // ---- stage: {30 rec[0..67], rec[68], rec[69]}, zero past each window's end
-  L.n += launch_rows_stage(s.x, kFeat, rec, rec_stride, PNB_RECORD_FLOATS, 68, n, n, F, st);
-  train_mask_kernel<<<blocks_for((size_t)R * kFeat), 256, 0, st>>>(s.x, frames, n, F);
-  L.n++;
+  { LaunchScope m(e, kUnprofiled, st); launch_rows_stage(s.x, kFeat, rec, rec_stride, PNB_RECORD_FLOATS, 68, n, n, F, st); }
+  { LaunchScope m(e, kUnprofiled, st); train_mask_kernel<<<blocks_for((size_t)R * kFeat), 256, 0, st>>>(s.x, frames, n, F); }
   L.check();
 
   // ---- forward
@@ -667,12 +667,14 @@ int train_grad(pnb_engine *e, const float *rec, size_t rec_stride, const int *fr
   }
 
   // ---- loss and its gradient at the output pre-activations
-  L.n += launch_loss_sums(s.pred, rec, rec_stride, frames, sums, n, n, F, st);
+  { LaunchScope m(e, kUnprofiled, st); launch_loss_sums(s.pred, rec, rec_stride, frames, sums, n, n, F, st); }
   long long counted = 0;
   for (int i = 0; i < n; i++) counted += h_frames ? h_frames[i] : F;
-  train_dpre_kernel<<<blocks_for((size_t)R * 68), 256, 0, st>>>(s.pred, rec, rec_stride, frames, n, F,
-                                                                1.0 / ((double)counted * kBands), s.dpre);
-  L.n++;
+  {
+    LaunchScope m(e, kUnprofiled, st);
+    train_dpre_kernel<<<blocks_for((size_t)R * 68), 256, 0, st>>>(s.pred, rec, rec_stride, frames, n, F,
+                                                                  1.0 / ((double)counted * kBands), s.dpre);
+  }
   L.check();
 
   // ---- backward.  Weight gradients go straight into the flat gradient at their blob offsets.
@@ -740,14 +742,14 @@ int train_grad(pnb_engine *e, const float *rec, size_t rec_stride, const int *fr
   L.wgrad(nullptr, 0, 1, s.eb, 128, 128, R, G + O[1]);
 
   const size_t N = O[kParams];
-  train_check_kernel<<<blocks_for(N, 1024), 256, 0, st>>>(G, N, s.bad, e->d_status);
-  L.n++;
+  { LaunchScope m(e, kUnprofiled, st); train_check_kernel<<<blocks_for(N, 1024), 256, 0, st>>>(G, N, s.bad, e->d_status); }
   L.check();
   TCK(L.err);
   // pnb_launches_per_call reports train_grad_launches: the schedule above and that count must agree
-  if (L.n != train_grad_launches(e)) return engine_fail(PNB_ERR_CUDA, "train_grad issued a launch count train_grad_launches does not know");
+  if (e->launches - launches0 != train_grad_launches(e))
+    return engine_fail(PNB_ERR_CUDA, "train_grad issued a launch count train_grad_launches does not know");
   e->train_hops = counted;
-  return L.n;
+  return PNB_OK;
 }
 
 // The launches of train_grad, which does not depend on the shape of the call: stage 2; forward 3 + 5 x 2 + 2; loss 2;
@@ -769,9 +771,9 @@ int train_adam(pnb_engine *e, double lr, long long step, cudaStream_t st) {
   a.bc2_sqrt = (float)pow(bc2, 0.5);
   a.neg_step = (float)(-(lr / bc1));
   a.eps = 1e-8f;
-  train_adam_kernel<<<dim3(64, kParams), 256, 0, st>>>(a);
+  { LaunchScope m(e, kUnprofiled, st); train_adam_kernel<<<dim3(64, kParams), 256, 0, st>>>(a); }
   TCK(cudaGetLastError());
-  return 1;
+  return PNB_OK;
 }
 
 // what: 0 weights, 1 gradient, 2 Adam m, 3 Adam v; host memory of train_params(e) floats
@@ -808,20 +810,20 @@ int train_accum_prepare(pnb_engine *e) {
 int train_accumulate(pnb_engine *e, cudaStream_t st) {
   const pnb_train_state &s = *e->train;
   const size_t N = s.off[kParams];
-  train_accum_kernel<<<blocks_for(N / 4), 256, 0, st>>>(s.grad, N, (double)e->train_hops, s.acc);
+  { LaunchScope m(e, kUnprofiled, st); train_accum_kernel<<<blocks_for(N / 4), 256, 0, st>>>(s.grad, N, (double)e->train_hops, s.acc); }
   TCK(cudaGetLastError());
-  return 1;
+  return PNB_OK;
 }
 
 int train_finish(pnb_engine *e, cudaStream_t st) {
   const pnb_train_state &s = *e->train;
   const size_t N = s.off[kParams];
-  train_finish_kernel<<<blocks_for(N / 4), 256, 0, st>>>(s.acc, N, s.grad);
+  { LaunchScope m(e, kUnprofiled, st); train_finish_kernel<<<blocks_for(N / 4), 256, 0, st>>>(s.acc, N, s.grad); }
   TCK(cudaMemsetAsync(s.acc + N, 0, sizeof(double), st));
   TCK(cudaMemsetAsync(s.bad, 0, sizeof(int), st));
-  train_check_kernel<<<blocks_for(N, 1024), 256, 0, st>>>(s.grad, N, s.bad, e->d_status);
+  { LaunchScope m(e, kUnprofiled, st); train_check_kernel<<<blocks_for(N, 1024), 256, 0, st>>>(s.grad, N, s.bad, e->d_status); }
   TCK(cudaGetLastError());
-  return 2;
+  return PNB_OK;
 }
 
 // The accumulator's N + 1 doubles to or from mem, host memory or device memory of the engine's device, on st

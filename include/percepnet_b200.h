@@ -558,7 +558,14 @@ enum {
   /* network state after the last hop of the call, layout [n_streams][width] (no PNB_KEEP_TAPS needed): */
   PNB_TAP_NN_C2 = 7,    /* float[512] conv2 output                                            */
   PNB_TAP_NN_H0 = 8,    /* +0..4: float[512|128] states of gru1, gru2, gru3, gru_gb, gru_rb   */
-  PNB_TAP_G_USED = 13   /* float[34]  band gains as applied: g, post-filtered under PNB_POSTFILTER (PNB_KEEP_TAPS) */
+  PNB_TAP_G_USED = 13,  /* float[34]  band gains as applied: g, post-filtered under PNB_POSTFILTER (PNB_KEEP_TAPS) */
+  /* PNB_TRAIN_NETWORK only (no PNB_KEEP_TAPS needed): diagnostics of the last pnb_train_grad_* call, the forward values
+     its backward used.  Layout [F][n][width], F and n the hops and active rows of that call, row t*n + b; hops past a
+     window's end hold the forward of its zeroed input.  Refused before the engine's first gradient call; pnb_train_adam,
+     _accumulate and _finish leave them as they are. */
+  PNB_TAP_TRAIN_FC = 14,    /* float[128] fc output (after ReLU)                                */
+  PNB_TAP_TRAIN_C1 = 15,    /* float[512] conv1 output (after ReLU)                             */
+  PNB_TAP_TRAIN_C2PRE = 16  /* float[512] conv2 pre-activation (before tanh)                    */
 };
 int pnb_read_tap(pnb_engine *e, int what, void *dst, size_t dst_bytes);
 

@@ -26,7 +26,9 @@ RECORD = 138
 RNN_FEATURES, RNN_RECORDS = 0, 1   # pnb_compute_rnn_* formats: 70 features or 138 record floats per hop
 TAPS = {"features": (0, np.float32, 70), "pitch": (1, np.int32, 4), "pitchf": (2, np.float32, 2),
         "X": (3, np.float32, 800), "P": (4, np.float32, 800), "Ex": (5, np.float32, 34), "gr": (6, np.float32, 68),
-        "g_used": (13, np.float32, 34)}
+        "g_used": (13, np.float32, 34),
+        # TRAIN_NETWORK: fc / conv1 outputs and conv2's pre-activation of the last train_grad, [F][active rows][width]
+        "train_fc": (14, np.float32, 128), "train_c1": (15, np.float32, 512), "train_c2pre": (16, np.float32, 512)}
 
 _lib = None
 
@@ -472,9 +474,11 @@ class Engine:
         """pnb_check: waits for the engine's work (and `stream`) and raises on PNB_ERR_DOMAIN / PNB_ERR_CUDA."""
         self._ck(self.L.pnb_check(self.h, stream or None), "pnb_check")
 
-    def read_tap(self, name: str, n_frames: int) -> np.ndarray:
+    def read_tap(self, name: str, n_frames: int, rows: int = None) -> np.ndarray:
+        """pnb_read_tap: [n_frames][rows][width], rows n_streams by default; the train_* taps of a train_grad call
+        take that call's active rows."""
         code, dt, width = TAPS[name]
-        a = np.empty((n_frames, self.n_streams, width), dt)
+        a = np.empty((n_frames, self.n_streams if rows is None else rows, width), dt)
         self._ck(self.L.pnb_read_tap(self.h, code, a.ctypes.data, a.nbytes), f"pnb_read_tap({name})")
         return a
 

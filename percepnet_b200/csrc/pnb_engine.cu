@@ -1542,6 +1542,11 @@ extern "C" int pnb_read_tap(pnb_engine *e, int what, void *dst, size_t dst_bytes
       int li = what - PNB_TAP_NN_H0;
       src = e->h[li]; bytes = (size_t)e->S * kGruH[li] * 4; break;
     }
+    case PNB_TAP_TRAIN_FC: case PNB_TAP_TRAIN_C1: case PNB_TAP_TRAIN_C2PRE: {
+      int rc = train_tap(e, what, &src, &bytes);
+      if (rc) return rc;
+      break;
+    }
     default: return fail(PNB_ERR_ARG, "unknown tap %d", what);
   }
   if (!src && (e->flags & PNB_SIGNAL_ONLY) && what >= PNB_TAP_NN_C2 && what < PNB_TAP_G_USED)

@@ -194,6 +194,9 @@ int train_accum_prepare(pnb_engine *e);
 int train_accumulate(pnb_engine *e, cudaStream_t st);
 int train_finish(pnb_engine *e, cudaStream_t st);
 int train_accum_copy(pnb_engine *e, void *mem, bool out, cudaStream_t st);
+// The PNB_TAP_TRAIN_* tap `what` of the last gradient call: its device pointer and size in bytes, or PNB_ERR_ARG (set
+// as the last error) on an engine without a trainer or before its first gradient call.
+int train_tap(const pnb_engine *e, int what, const void **src, size_t *bytes);
 
 // The marker of one kernel launch on behalf of an engine, constructed right before the launch and destroyed right
 // after it: it counts the launch in e->launches and, when profiling and cls is a kernel class, records an event pair

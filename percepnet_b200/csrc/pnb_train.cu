@@ -442,6 +442,7 @@ struct pnb_train_state {
   float *dc2 = nullptr;                    // [F+2][n][512]
   float *carry = nullptr;                  // [S][512]
   int G512 = 0, G128 = 0;                  // CTAs of the recurrences (a power of two, co-resident)
+  int last_F = 0, last_n = 0;              // hops and rows of the last gradient call (0: none yet), for train_tap
 };
 
 constexpr size_t kPartFloats = (size_t)1 << 21;
@@ -749,6 +750,21 @@ int train_grad(pnb_engine *e, const float *rec, size_t rec_stride, const int *fr
   if (e->launches - launches0 != train_grad_launches(e))
     return engine_fail(PNB_ERR_CUDA, "train_grad issued a launch count train_grad_launches does not know");
   e->train_hops = counted;
+  s.last_F = F;
+  s.last_n = n;
+  return PNB_OK;
+}
+
+int train_tap(const pnb_engine *e, int what, const void **src, size_t *bytes) {
+  if (!e->train) return engine_fail(PNB_ERR_ARG, "the PNB_TAP_TRAIN_* taps need a PNB_TRAIN_NETWORK engine");
+  const pnb_train_state &s = *e->train;
+  if (!s.last_F) return engine_fail(PNB_ERR_ARG, "the PNB_TAP_TRAIN_* taps need a pnb_train_grad_* call first");
+  const size_t nb = (size_t)s.last_n, rows = (size_t)s.last_F * nb;
+  switch (what) {
+    case PNB_TAP_TRAIN_FC: *src = s.fc + 4 * nb * 128; *bytes = rows * 128 * sizeof(float); break;
+    case PNB_TAP_TRAIN_C1: *src = s.c1 + 2 * nb * 512; *bytes = rows * 512 * sizeof(float); break;
+    default: *src = s.c2p; *bytes = rows * 512 * sizeof(float); break;
+  }
   return PNB_OK;
 }
 

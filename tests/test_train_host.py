@@ -88,6 +88,50 @@ def test_closed_form_loss_gradient():
     assert np.all(np.isfinite(d)) and np.all(d == 0)
 
 
+def test_grads_at_own_values_is_grads():
+    """grads_at fed float64's own forward values (fc and conv1 outputs, conv2's pre-activation) is grads, loss and all
+    30 tensors within 1e-12, with the taps cut into chunks of windows like the records."""
+    sd = synth_state_dict(0)
+    rec = records(3, 24, 7)
+    frames = [24, 13, 24]
+    L, g = O.grads(sd, rec, frames)
+    fc, c1, c2p = O.forward_taps(sd, rec, frames)
+    assert fc.shape == (24, 3, 128) and c1.shape == (24, 3, 512) and c2p.shape == (24, 3, 512)
+    La, ga = O.grads_at(sd, rec, frames, fc, c1, c2p, chunk=2)
+    assert abs(La - L) <= 1e-12 * abs(L)
+    for k in g:
+        assert np.linalg.norm(ga[k] - g[k]) <= 1e-12 * np.linalg.norm(g[k]), k
+
+
+def test_grads_at_takes_tanh_prime_at_the_given_preactivation():
+    """Two conv2 pre-activations that differ at one unit j of one hop only, both deep in saturation (tanh = 1 exactly in
+    float64, tanh' of 1.7e-17 and 4.6e-17): every value of the network is the same, only tanh' at that unit moves.  So the
+    24 tensors above conv2 are bit-identical, conv2's bias gradient moves at unit j alone, and conv2's weight gradient in
+    row j alone, by that move times the conv1 outputs the unit sees (hops t - 2 .. t of its window)."""
+    sd = synth_state_dict(0)
+    rec = records(2, 24, 8)
+    fc, c1, c2p = O.forward_taps(sd, rec)
+    j, t, b = 37, 9, 1
+    a = c2p.copy()
+    a[:, :, j] = 20.0
+    p = a.copy()
+    p[t, b, j] = 19.5
+    assert np.tanh(20.0) == 1.0 and np.tanh(19.5) == 1.0
+    _, ga = O.grads_at(sd, rec, None, fc, c1, a)
+    _, gp = O.grads_at(sd, rec, None, fc, c1, p)
+    for k in ga:
+        if not k.startswith(("fc.", "conv1.", "conv2.")):
+            assert bits_equal(ga[k], gp[k]), k
+    moved = np.flatnonzero(ga["conv2.0.bias"] != gp["conv2.0.bias"])
+    assert moved.tolist() == [j]
+    delta = gp["conv2.0.bias"][j] - ga["conv2.0.bias"][j]
+    assert delta != 0
+    dw = gp["conv2.0.weight"] - ga["conv2.0.weight"]       # [out 512][in 512][tap 3]: tap k sees hop t - 2 + k
+    assert not np.any(np.delete(dw, j, axis=0))
+    want = delta * np.stack([c1[t - 2 + k, b] for k in range(3)], -1)
+    np.testing.assert_allclose(dw[j], want, rtol=1e-9, atol=1e-9 * np.abs(want).max())
+
+
 def test_layout_round_trips():
     sd = synth_state_dict(1, gain=2.0)
     back = unpack_state_dict(pack_state_dict(sd))

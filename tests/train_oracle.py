@@ -33,6 +33,9 @@ class Net(nn.Module):
         y = self.fc(x).permute(0, 2, 1)
         y = self.conv1(y)[:, :, :-4]                          # causal: output t sees inputs t-4 .. t
         c = self.conv2(y)[:, :, :-2].permute(0, 2, 1)
+        return self.head(c)
+
+    def head(self, c):                                        # conv2's output c [B, T, 512] -> [B, T, 68]
         h1, _ = self.gru1(c)
         h2, _ = self.gru2(h1)
         h3, _ = self.gru3(h2)
@@ -84,19 +87,99 @@ def grads(sd: dict, rec: np.ndarray, frames=None, dtype=torch.float64, device="c
     L = 0.0
     for c0 in range(0, B, chunk):
         part = slice(c0, min(B, c0 + chunk))
-        fr = None if frames is None else [int(f) for f in counts[part]]
-        x = features(rec[part])
-        if fr is not None:
-            for b, f in enumerate(fr):
-                x[b, f:] = 0
-        xt = torch.from_numpy(x).to(device=device, dtype=dtype)
-        y = torch.from_numpy(np.ascontiguousarray(rec[part, :, 70:])).to(device=device, dtype=dtype)
+        xt, y, fr = _inputs(rec, counts, part, frames, dtype, device)
         Lc = loss(m(xt), y, fr)
         if chunk < B:
             Lc = Lc * (float(counts[part].sum()) / total)
         Lc.backward()
         L += float(Lc.detach())
         del xt, y, Lc
+    return L, {k: p.grad.detach().cpu().numpy() for k, p in m.named_parameters()}
+
+
+def _inputs(rec, counts, part, frames, dtype, device):
+    """The network input and labels of windows rec[part], hops past each window's end zeroed; and their frames."""
+    fr = None if frames is None else [int(f) for f in counts[part]]
+    x = features(rec[part])
+    if fr is not None:
+        for b, f in enumerate(fr):
+            x[b, f:] = 0
+    xt = torch.from_numpy(x).to(device=device, dtype=dtype)
+    y = torch.from_numpy(np.ascontiguousarray(rec[part, :, 70:])).to(device=device, dtype=dtype)
+    return xt, y, fr
+
+
+def forward_taps(sd: dict, rec: np.ndarray, frames=None, dtype=torch.float64, device="cpu"):
+    """The fc output, conv1 output and conv2 pre-activation of the records' windows in `dtype`, as numpy arrays laid out
+    as the trainer's taps are: [T][B][width], hops past a window's end computed from its zeroed input."""
+    m = model(sd, dtype, device)
+    B, T = rec.shape[:2]
+    counts = np.full(B, T, np.int64) if frames is None else np.asarray(frames, np.int64)
+    with torch.no_grad():
+        x, _, _ = _inputs(rec, counts, slice(0, B), frames, dtype, device)
+        fc = m.fc(x)
+        c1 = m.conv1(fc.permute(0, 2, 1))[:, :, :-4]
+        c2p = m.conv2[0](c1)[:, :, :-2]
+    hop_major = lambda a: np.ascontiguousarray(a.detach().cpu().numpy().transpose(1, 0, 2))
+    return hop_major(fc), hop_major(c1.permute(0, 2, 1)), hop_major(c2p.permute(0, 2, 1))
+
+
+class TanhAtPre(torch.autograd.Function):
+    """tanh whose derivative is taken from the pre-activation a in closed form, 4 e / (1 + e)^2 with e = exp(-2|a|), as
+    the trainer's kEpiDTanh takes it: torch's 1 - y^2 of the output y loses every digit of tanh'(a) where y rounds to
+    +-1 (|a| > 19 in float64), and most of them from |a| of about 9 on.  factor: tanh'(a) given instead (same shape)."""
+
+    @staticmethod
+    def forward(ctx, a, factor=None):
+        ctx.save_for_backward(a, factor)
+        return torch.tanh(a)
+
+    @staticmethod
+    def backward(ctx, g):
+        a, factor = ctx.saved_tensors
+        if factor is None:
+            e = torch.exp(-2 * a.abs())
+            factor = 4 * e / ((1 + e) * (1 + e))
+        return g * factor, None
+
+
+def grads_at(sd: dict, rec: np.ndarray, frames, fc32, c1_32, c2p32, chunk=None, device="cpu", dtanh=None):
+    """grads at the trainer's own forward values: float64 autograd as `grads`, with fc's and conv1's outputs and conv2's
+    pre-activation pinned to fc32, c1_32 and c2p32 ([T][B][128 | 512 | 512], the PNB_TAP_TRAIN_* taps) by
+    straight-through substitution.  fc = fc64 m + (fc32 - fc64 m).detach(), m = fc32 > 0 (the saved output's sign is the
+    ReLU mask, as in kEpiDRelu), fc64 the float64 pre-activation; conv1 the same from that fc; c2p = c2p64 + (c2p32 -
+    c2p64).detach(), then c = tanh(c2p) (TanhAtPre) and the rest of Net.forward.  The values are the trainer's; the
+    gradient still flows through the float64 weights and the masks, with tanh' at the trainer's own pre-activation.
+    Hops past a window's end take the tapped values like any other.  dtanh: tanh' as [T][B][512] float64 instead of its
+    closed form at c2p32.  Returns (loss, {name: gradient})."""
+    m = model(sd, torch.float64, device)
+    B, T = rec.shape[:2]
+    chunk = chunk or B
+    counts = np.full(B, T, np.int64) if frames is None else np.asarray(frames, np.int64)
+    total = float(counts.sum())
+    L = 0.0
+    for c0 in range(0, B, chunk):
+        part = slice(c0, min(B, c0 + chunk))
+        x, y, fr = _inputs(rec, counts, part, frames, torch.float64, device)
+        # [T][B][w] taps -> [b, w, T] of this chunk, as float64
+        tap = lambda a: torch.from_numpy(np.ascontiguousarray(np.asarray(a)[:, part].transpose(1, 2, 0))).to(
+            device=device, dtype=torch.float64)
+        fc_t, c1_t, c2p_t = tap(fc32), tap(c1_32), tap(c2p32)
+        fc64 = m.fc[0](x).permute(0, 2, 1)
+        mk = (fc_t > 0).to(torch.float64)
+        fc = fc64 * mk + (fc_t - fc64 * mk).detach()
+        c1_64 = m.conv1[0](fc)[:, :, :-4]
+        mk = (c1_t > 0).to(torch.float64)
+        c1 = c1_64 * mk + (c1_t - c1_64 * mk).detach()
+        c2p64 = m.conv2[0](c1)[:, :, :-2]
+        c2p = c2p64 + (c2p_t - c2p64).detach()
+        c = TanhAtPre.apply(c2p, None if dtanh is None else tap(dtanh))
+        Lc = loss(m.head(c.permute(0, 2, 1)), y, fr)
+        if chunk < B:
+            Lc = Lc * (float(counts[part].sum()) / total)
+        Lc.backward()
+        L += float(Lc.detach())
+        del x, y, Lc
     return L, {k: p.grad.detach().cpu().numpy() for k, p in m.named_parameters()}
 
 

@@ -319,6 +319,8 @@ int pnb_train_accumulate(pnb_engine *e, void *cuda_stream);
 int pnb_train_finish(pnb_engine *e, void *cuda_stream);
 int pnb_train_export(pnb_engine *e, int what, void *dst, size_t bytes);
 int pnb_train_import(pnb_engine *e, int what, const void *src, size_t bytes);
+/* The trainer's forward and backward with the caller's loss (pnb_train_forward_device, pnb_train_backward_device) are
+ * declared in pnb_train_device.h, included at the end of this header. */
 
 /* The signal path without the network: pnb_process_* cut where the network sits, so the g/r between analysis and
  * synthesis come from the caller -- another engine's pnb_compute_rnn_*, a torch model, a records file's ideal gains,
@@ -559,13 +561,15 @@ enum {
   PNB_TAP_NN_C2 = 7,    /* float[512] conv2 output                                            */
   PNB_TAP_NN_H0 = 8,    /* +0..4: float[512|128] states of gru1, gru2, gru3, gru_gb, gru_rb   */
   PNB_TAP_G_USED = 13,  /* float[34]  band gains as applied: g, post-filtered under PNB_POSTFILTER (PNB_KEEP_TAPS) */
-  /* PNB_TRAIN_NETWORK only (no PNB_KEEP_TAPS needed): diagnostics of the last pnb_train_grad_* call, the forward values
-     its backward used.  Layout [F][n][width], F and n the hops and active rows of that call, row t*n + b; hops past a
-     window's end hold the forward of its zeroed input.  Refused before the engine's first gradient call; pnb_train_adam,
-     _accumulate and _finish leave them as they are. */
+  /* PNB_TRAIN_NETWORK only (no PNB_KEEP_TAPS needed): diagnostics of the last pnb_train_grad_* or
+     pnb_train_forward_device call, the forward values its backward uses.  Layout [F][n][width], F and n the hops and
+     active rows of that call, row t*n + b; hops past a window's end hold the forward of its zeroed input.  Refused
+     before the engine's first gradient or forward call; pnb_train_adam, _accumulate and _finish leave them as they are. */
   PNB_TAP_TRAIN_FC = 14,    /* float[128] fc output (after ReLU)                                */
   PNB_TAP_TRAIN_C1 = 15,    /* float[512] conv1 output (after ReLU)                             */
-  PNB_TAP_TRAIN_C2PRE = 16  /* float[512] conv2 pre-activation (before tanh)                    */
+  PNB_TAP_TRAIN_C2PRE = 16, /* float[512] conv2 pre-activation (before tanh)                    */
+  PNB_TAP_TRAIN_DPRE = 17   /* float[68]  dL/d(output pre-activation) of the last pnb_train_grad_* or
+                               pnb_train_backward_device call                                   */
 };
 int pnb_read_tap(pnb_engine *e, int what, void *dst, size_t dst_bytes);
 
@@ -606,4 +610,6 @@ const char *pnb_version(void);
 #ifdef __cplusplus
 }
 #endif
+#include "pnb_train_device.h"
+
 #endif /* PERCEPNET_B200_H */

@@ -1,4 +1,4 @@
-"""Python host mirror of the C-ABI in include/percepnet_b200.h (ctypes; no compute here).
+"""Python host mirror of the C-ABI in include/percepnet_b200.h and include/pnb_train_device.h (ctypes; no compute here).
 
 ``Engine`` is the batched-streams counterpart of the reference's ``DenoiseState``
 (/root/reference/src/rnnoise.h:49-60): ``Engine.process`` advances S independent 48 kHz streams by F
@@ -27,8 +27,11 @@ RNN_FEATURES, RNN_RECORDS = 0, 1   # pnb_compute_rnn_* formats: 70 features or 1
 TAPS = {"features": (0, np.float32, 70), "pitch": (1, np.int32, 4), "pitchf": (2, np.float32, 2),
         "X": (3, np.float32, 800), "P": (4, np.float32, 800), "Ex": (5, np.float32, 34), "gr": (6, np.float32, 68),
         "g_used": (13, np.float32, 34),
-        # TRAIN_NETWORK: fc / conv1 outputs and conv2's pre-activation of the last train_grad, [F][active rows][width]
-        "train_fc": (14, np.float32, 128), "train_c1": (15, np.float32, 512), "train_c2pre": (16, np.float32, 512)}
+        # TRAIN_NETWORK: fc / conv1 outputs and conv2's pre-activation of the last train_grad or train_forward_device,
+        # and the gradient at the output pre-activations of the last train_grad or train_backward_device,
+        # [F][active rows][width]
+        "train_fc": (14, np.float32, 128), "train_c1": (15, np.float32, 512), "train_c2pre": (16, np.float32, 512),
+        "train_dpre": (17, np.float32, 68)}
 # read_nn_state: the network state after the last hop, [n_streams][width] (PNB_TAP_NN_C2, PNB_TAP_NN_H0 + 0..4)
 _NN_STATE = {"c2": (7, np.float32, 512), "gru1": (8, np.float32, 512), "gru2": (9, np.float32, 512),
              "gru3": (10, np.float32, 512), "gru_gb": (11, np.float32, 512), "gru_rb": (12, np.float32, 128)}
@@ -125,6 +128,12 @@ _SIGNATURES = {
     "pnb_version": (C.c_char_p, ()),
 }
 EXPORTS = tuple(_SIGNATURES)
+# Every symbol of include/pnb_train_device.h (the trainer's calls with the caller's loss), the same way.
+_TRAIN_DEVICE_SIGNATURES = {
+    "pnb_train_forward_device": (_i, (_vp, _vp, _sz, _i, _vp, _vp, _sz, _vp)),
+    "pnb_train_backward_device": (_i, (_vp, _vp, _sz, _vp, _sz, _vp, _vp)),
+}
+TRAIN_DEVICE_EXPORTS = tuple(_TRAIN_DEVICE_SIGNATURES)
 
 
 def load_library() -> C.CDLL:
@@ -136,7 +145,7 @@ def load_library() -> C.CDLL:
         raise PnbError(f"{LIB_PATH} is missing: run `python -c 'import __graft_entry__ as g; g.build()'` "
                        "(nvcc, sm_90a).  There is no CPU implementation to fall back to.")
     L = C.CDLL(LIB_PATH)
-    for name, (restype, argtypes) in _SIGNATURES.items():
+    for name, (restype, argtypes) in {**_SIGNATURES, **_TRAIN_DEVICE_SIGNATURES}.items():
         f = getattr(L, name)
         f.restype, f.argtypes = restype, argtypes
     _lib = L
@@ -396,6 +405,20 @@ class Engine:
         """pnb_train_grad_device on raw device pointers (rec_stride in floats); frames: None or a host sequence of one
         count per active row; d_sums: [active, 4] float64."""
         self._call("pnb_train_grad_device", d_rec, rec_stride, n_frames, _ptr(self._frames(frames)), d_sums, stream)
+
+    def train_forward_device(self, d_x: int, x_stride: int, n_frames: int, d_weights: int, d_out: int, out_stride: int,
+                             stream: int = 0):
+        """pnb_train_forward_device on raw device pointers (strides in floats): features [active, n_frames, 70] (not
+        scaled) through the trainer's forward into g/r [active, n_frames, 68]; d_weights: 0, or N_PARAMS floats in blob
+        order that replace the weights first.  Its backward (train_backward_device) is then due."""
+        self._call("pnb_train_forward_device", d_x, x_stride, n_frames, d_weights, d_out, out_stride, stream)
+
+    def train_backward_device(self, d_dout: int, dout_stride: int, d_dx: int = 0, dx_stride: int = 0, d_grad: int = 0,
+                              stream: int = 0):
+        """pnb_train_backward_device on raw device pointers (strides in floats): dL/d(out) of the last
+        train_forward_device in; dL/dx (d_dx, or 0 for none) and the blob-order gradient (d_grad, or 0) out.  The
+        gradient is also the held one, for train_adam / train_accumulate."""
+        self._call("pnb_train_backward_device", d_dout, dout_stride, d_dx, dx_stride, d_grad, stream)
 
     def train_adam(self, lr: float, step: int, stream: int = 0):
         """pnb_train_adam: one torch.optim.Adam step (defaults) with the gradient of the last train_grad; step counts

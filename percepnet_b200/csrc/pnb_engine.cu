@@ -321,6 +321,7 @@ extern "C" int pnb_reset(pnb_engine *e) {
   e->n_active = e->S;
   e->poisoned = false;
   e->train_open = false;  // the accumulator (stream state) was zeroed above; the held gradient stays, and stays due
+  e->train_fwd_F = 0;
   if (e->sessions) {  // every session fresh: all parked, every blob marked fresh
     CK(cudaMemset(e->d_park, 0, (size_t)e->pool.capacity() * kParkStride));
     e->pool.init(e->S, e->pool.capacity());
@@ -666,10 +667,10 @@ static Rows pcm(const T *p, size_t stride) { return rows(p, stride, kFrame, size
 // One call as its entry point received it, its buffers as row arrays.  In / out: PCM / PCM of a slot, session or ragged
 // call; speech, noisy / records and (pnb_train_audio_*) audio of a training-record call; features or records / g/r of a
 // network call; records / g/r (when asked for) and the loss sums of a score call; PCM / features of an analysis; g/r /
-// PCM of a synthesis.  An analysis, synthesis or network call on a session list (pool) has ids too; its analysis and
+// PCM of a synthesis; features / g/r of a training forward; dL/d(out) / dL/dx (when asked for) of a training backward.  An analysis, synthesis or network call on a session list (pool) has ids too; its analysis and
 // network forms may have hops.
 struct Call {
-  enum Kind { kSlots, kSessions, kRagged, kNetwork, kRecords, kAnalyze, kSynthesize, kTrain } kind;
+  enum Kind { kSlots, kSessions, kRagged, kNetwork, kRecords, kAnalyze, kSynthesize, kTrain, kTrainForward, kTrainBackward } kind;
   Rows in[2], out[2];
   int F;           // hops; a ragged call's is max(hops), set by check_call
   float *gr;       // enhancement calls: g/r destination [F][rows][68], or null
@@ -681,6 +682,8 @@ struct Call {
   const int *frames;  // score and gradient calls: the hops each row's loss counts (host), or null for F
   bool status = true;  // a blocking host call reads back and reports the status word (rejected imports, PNB_ERR_DOMAIN)
   bool pool = false;   // an analysis, synthesis or network call on a session list (pnb_*_sessions_*)
+  const float *weights = nullptr;  // a training forward: the parameters in blob order (device), or null
+  float *grad = nullptr;           // a training backward: the gradient's destination in blob order (device), or null
 };
 
 // The rows of a call on st, *r: nothing for a slot call; on a session list the pending session split's rows staged
@@ -881,11 +884,32 @@ static int enqueue_synthesize(pnb_engine *e, const Call &c, cudaStream_t st) {
 // [0, n_active), each from zero state; the loss sums to the caller, the gradient into the engine's buffer.  Neither the
 // network state of the slots nor the signal state is touched.
 static int enqueue_train(pnb_engine *e, const Call &c, cudaStream_t st) {
+  e->train_fwd_F = 0;
   return enqueue_call(e, c.F, st, [&]() -> int {
     const int *frames = nullptr;
     if (c.frames) { int rc = stage_ints(e, c.frames, (size_t)e->n_active, st, &frames); if (rc) return rc; }
     return train_grad(e, static_cast<const float *>(c.in[0].p), c.in[0].stride, frames, c.frames,
                       static_cast<double *>(c.out[1].p), c.F, st);
+  }, false);
+}
+
+// A training forward on st (arguments already checked): the caller's features through the trainer's forward half on
+// windows [0, n_active), its g/r out; its backward becomes due.  A training backward (arguments checked, so a forward of
+// F hops is due): the caller's dL/d(out) through the backward half into the held gradient, dL/dx out when asked for.
+static int enqueue_train_forward(pnb_engine *e, const Call &c, cudaStream_t st) {
+  e->train_fwd_F = 0;
+  const int rc = enqueue_call(e, c.F, st, [&]() -> int {
+    return train_forward(e, static_cast<const float *>(c.in[0].p), c.in[0].stride, c.weights, static_cast<float *>(c.out[0].p),
+                         c.out[0].stride, c.F, st);
+  }, false);
+  if (rc == PNB_OK) e->train_fwd_F = c.F;
+  return rc;
+}
+static int enqueue_train_backward(pnb_engine *e, const Call &c, cudaStream_t st) {
+  e->train_fwd_F = 0;
+  return enqueue_call(e, c.F, st, [&]() -> int {
+    return train_backward(e, static_cast<const float *>(c.in[0].p), c.in[0].stride, static_cast<float *>(c.out[0].p),
+                          c.out[0].stride, c.grad, st);
   }, false);
 }
 
@@ -897,6 +921,8 @@ static int enqueue(pnb_engine *e, const Call &c, cudaStream_t st) {
     case Call::kAnalyze: return enqueue_analyze(e, c, st);
     case Call::kSynthesize: return enqueue_synthesize(e, c, st);
     case Call::kTrain: return enqueue_train(e, c, st);
+    case Call::kTrainForward: return enqueue_train_forward(e, c, st);
+    case Call::kTrainBackward: return enqueue_train_backward(e, c, st);
     default: return enqueue_enhance(e, c, st);
   }
 }
@@ -988,14 +1014,21 @@ static int check_call(pnb_engine *e, Call &c) {
     for (int i = 0; i < c.n_ids; i++) uniform = uniform && c.hops[i] == c.F;
     if (uniform) c.hops = nullptr;
   }
-  const bool train = c.kind == Call::kRecords, network = c.kind == Call::kNetwork || c.kind == Call::kTrain;
+  const bool trainer = c.kind == Call::kTrain || c.kind == Call::kTrainForward || c.kind == Call::kTrainBackward;
+  const bool train = c.kind == Call::kRecords, network = c.kind == Call::kNetwork || trainer;
   const bool split = c.kind == Call::kAnalyze || c.kind == Call::kSynthesize;
   if (!e) return fail(PNB_ERR_ARG, "engine is NULL");
   if (!network && (e->flags & PNB_NETWORK_ONLY))
     return fail(PNB_ERR_ARG, "engine was created with PNB_NETWORK_ONLY: use pnb_compute_rnn_* / pnb_score_records_*");
   if (!split && (e->flags & PNB_SIGNAL_ONLY))
     return fail(PNB_ERR_ARG, "engine was created with PNB_SIGNAL_ONLY: use pnb_analyze_* / pnb_synthesize_*");
-  if (c.kind == Call::kTrain && !(e->flags & PNB_TRAIN_NETWORK)) return fail(PNB_ERR_ARG, "engine was not created with PNB_TRAIN_NETWORK");
+  if (trainer && !(e->flags & PNB_TRAIN_NETWORK)) return fail(PNB_ERR_ARG, "engine was not created with PNB_TRAIN_NETWORK");
+  if (c.kind == Call::kTrainBackward) {  // the hops of the forward it differentiates
+    if (!e->train_fwd_F)
+      return fail(PNB_ERR_ARG, "no pnb_train_forward_device call awaits its backward (one backward per forward; "
+                               "pnb_reset, pnb_set_active_streams and pnb_train_grad_* end a forward's wait)");
+    c.F = e->train_fwd_F;
+  }
   if (train && !(e->flags & PNB_TRAIN_DATA)) return fail(PNB_ERR_ARG, "engine was not created with PNB_TRAIN_DATA");
   if (!train && (e->flags & PNB_TRAIN_DATA))
     return fail(PNB_ERR_ARG, "engine was created with PNB_TRAIN_DATA: use pnb_train_records_* / pnb_submit_train_records");
@@ -1317,6 +1350,23 @@ extern "C" int pnb_train_grad_host(pnb_engine *e, const float *rec, size_t rec_s
   return host_call(e, train_call(rec, rec_stride, n_frames, frames, sums), false);
 }
 
+// The trainer's forward and backward on the caller's tensors (PNB_TRAIN_NETWORK): features in, g/r out; dL/d(out) in,
+// dL/dx (when asked for) and the gradient (when asked for) out.
+extern "C" int pnb_train_forward_device(pnb_engine *e, const float *d_x, size_t x_stride, int n_frames,
+                                        const float *d_weights, float *d_out, size_t out_stride, void *cuda_stream) {
+  Call c{Call::kTrainForward, {rows(d_x, x_stride, kFeat, sizeof(float), "x_stride")},
+         {rows(d_out, out_stride, 68, sizeof(float), "out_stride")}, n_frames};
+  c.weights = d_weights;
+  return device_call(e, c, (cudaStream_t)cuda_stream);
+}
+extern "C" int pnb_train_backward_device(pnb_engine *e, const float *d_dout, size_t dout_stride, float *d_dx,
+                                         size_t dx_stride, float *d_grad, void *cuda_stream) {
+  Call c{Call::kTrainBackward, {rows(d_dout, dout_stride, 68, sizeof(float), "dout_stride")}, {}, 0};
+  if (d_dx) c.out[0] = rows(d_dx, dx_stride, kFeat, sizeof(float), "dx_stride");
+  c.grad = d_grad;
+  return device_call(e, c, (cudaStream_t)cuda_stream);
+}
+
 // The refusals every training entry point shares: an engine of its kind that no failed call has poisoned.
 static int check_trainer(pnb_engine *e) {
   if (!e) return fail(PNB_ERR_ARG, "engine is NULL");
@@ -1542,7 +1592,7 @@ extern "C" int pnb_read_tap(pnb_engine *e, int what, void *dst, size_t dst_bytes
       int li = what - PNB_TAP_NN_H0;
       src = e->h[li]; bytes = (size_t)e->S * kGruH[li] * 4; break;
     }
-    case PNB_TAP_TRAIN_FC: case PNB_TAP_TRAIN_C1: case PNB_TAP_TRAIN_C2PRE: {
+    case PNB_TAP_TRAIN_FC: case PNB_TAP_TRAIN_C1: case PNB_TAP_TRAIN_C2PRE: case PNB_TAP_TRAIN_DPRE: {
       int rc = train_tap(e, what, &src, &bytes);
       if (rc) return rc;
       break;
@@ -1617,6 +1667,7 @@ extern "C" int pnb_set_active_streams(pnb_engine *e, int n, void *cuda_stream) {
     if (rc) return rc;
   }
   e->n_active = n;
+  e->train_fwd_F = 0;  // a pending training forward ran on the old rows
   return PNB_OK;
 }
 extern "C" int pnb_active_streams(const pnb_engine *e) { return e ? e->n_active : 0; }

@@ -81,6 +81,9 @@ struct pnb_engine {
   // (0: none, or taken), and whether the accumulator holds anything (accumulated or imported) not yet finished
   long long train_hops = 0;
   bool train_open = false;
+  // the hops of the pnb_train_forward_device call whose backward is still due (0: none).  Cleared by its backward,
+  // a gradient call, pnb_set_active_streams and pnb_reset: one backward per forward, on the rows that forward ran.
+  int train_fwd_F = 0;
   int last_frames = 0;
   // An analysis (pnb_analyze_*) whose synthesis (pnb_synthesize_*) is still due, set by the analysis and cleared by the
   // synthesis or pnb_reset.  F: its hops, or 0 when none is pending.  Between the two halves the analysed streams are
@@ -187,6 +190,17 @@ int train_prepare(pnb_engine *e);
 int train_grad(pnb_engine *e, const float *rec, size_t rec_stride, const int *frames, const int *h_frames, double *sums,
                int F, cudaStream_t st);
 int train_grad_launches(const pnb_engine *e);
+// forward: the caller's network input x (rows of F x 70 floats, not scaled) of windows [0, n_active) through the
+// network, weights (device, blob order, or null) copied into the parameters first, the predictions out to the caller's
+// rows (F x 68); the activations are kept for one backward.  backward: from the caller's dL/d(out) rows (F x 68) of the
+// last forward, the held gradient (copied to grad, device, when not null) and, when dx is not null, dL/dx to the
+// caller's rows (F x 70).  Their launch counts depend on nothing but whether dx is asked for.
+int train_forward(pnb_engine *e, const float *x, size_t x_stride, const float *weights, float *out, size_t out_stride,
+                  int F, cudaStream_t st);
+int train_backward(pnb_engine *e, const float *dout, size_t dout_stride, float *dx, size_t dx_stride, float *grad,
+                   cudaStream_t st);
+int train_forward_launches(const pnb_engine *e);
+int train_backward_launches(const pnb_engine *e, bool dx);
 int train_adam(pnb_engine *e, double lr, long long step, cudaStream_t st);
 int train_copy(pnb_engine *e, int what, void *host, bool to_host, cudaStream_t st);
 size_t train_params(const pnb_engine *e);
@@ -194,7 +208,7 @@ int train_accum_prepare(pnb_engine *e);
 int train_accumulate(pnb_engine *e, cudaStream_t st);
 int train_finish(pnb_engine *e, cudaStream_t st);
 int train_accum_copy(pnb_engine *e, void *mem, bool out, cudaStream_t st);
-// The PNB_TAP_TRAIN_* tap `what` of the last gradient call: its device pointer and size in bytes, or PNB_ERR_ARG (set
+// The PNB_TAP_TRAIN_* tap `what` of the last gradient or forward call: its device pointer and size in bytes, or PNB_ERR_ARG (set
 // as the last error) on an engine without a trainer or before its first gradient call.
 int train_tap(const pnb_engine *e, int what, const void **src, size_t *bytes);
 

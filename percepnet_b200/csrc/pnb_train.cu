@@ -14,6 +14,11 @@
 //            (split over the rows into a fixed number of parts, then summed part by part in order).
 //   check    one pass over the gradient: a non-finite value raises the engine's domain bit and makes the next Adam
 //            step a no-op on the device
+// The forward and the backward are two halves (forward_half, backward_half) that train_grad runs around its loss.
+// pnb_train_forward_device runs the forward half alone on the caller's network input and weights; the backward of the
+// caller's loss (pnb_train_backward_device) seeds the output pre-activations from the caller's dL/d(out)
+// (train_seed_kernel), runs the backward half, and adds dL/dx = dA_fc W_fc^T when asked.  Its check skips the next
+// Adam step on a non-finite gradient but raises no domain bit: the caller owns that loss, as torch's autograd does.
 // Between gradient calls and Adam, pnb_train_accumulate / pnb_train_finish sum several calls' gradients (micro-batches,
 // or ranks through an exported accumulator) in float64, weighted by their counted hops (train_accum_kernel,
 // train_finish_kernel), and the check runs again on the sum.
@@ -327,14 +332,30 @@ __global__ void train_dpre_kernel(const float *__restrict__ pred, const float *_
   }
 }
 
-// bad = 1 (and the engine's domain bit) when any of the n gradient values is not finite; bad is zeroed before
+// The backward's entry point when the caller supplies dL/d(out): dout [n][F][68] rows of dout_stride floats (window-major,
+// as the caller's tensors) -> d [F][n][68] (hop-major, r = t*n + b), d = dout (1 - p) p left to right, ATen's
+// sigmoid_backward, so the seed is the same bits torch's autograd passes into the output layers.
+__global__ void train_seed_kernel(const float *__restrict__ dout, size_t dout_stride, const float *__restrict__ pred, int n,
+                                  int F, float *__restrict__ d) {
+  const size_t total = (size_t)F * n * 68;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+    const int k = (int)(i % 68);
+    const size_t row = i / 68;
+    const int b = (int)(row % n), t = (int)(row / n);
+    const float p = pred[i];
+    d[i] = __fmul_rn(__fmul_rn(dout[(size_t)b * dout_stride + (size_t)t * 68 + k], __fsub_rn(1.f, p)), p);
+  }
+}
+
+// bad = 1 (and, with a status word, the engine's domain bit) when any of the n gradient values is not finite; bad is
+// zeroed before
 __global__ void train_check_kernel(const float *__restrict__ g, size_t n, int *bad, int *status) {
   bool found = false;
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
     found |= !isfinite(g[i]);
   if (__syncthreads_or(found) && threadIdx.x == 0) {
     *bad = 1;
-    atomicOr(status, 1);
+    if (status) atomicOr(status, 1);
   }
 }
 
@@ -599,31 +620,35 @@ struct Launcher {
 
 // The parameter arrays in blob order: fc W, b (0, 1); conv1 (2, 3); conv2 (4, 5); GRU k = 0..4 (gru1, gru2, gru3,
 // gru_gb, gru_rb) W, U, b at 6 + 3k .. 8 + 3k; fc_gb (21, 22); fc_rb (23, 24).
-int train_grad(pnb_engine *e, const float *rec, size_t rec_stride, const int *frames, const int *h_frames, double *sums,
-               int F, cudaStream_t st) {
+namespace {
+// The recurrence arguments of GRU l over the rows t*n + b of an F-hop call: forward into its saved h/z/r/n/hn, backward
+// from them into g1 (dgx) and g2 (dgh).
+RecArgs rec_args(const pnb_train_state &s, int l, int n, int F, const int *frames) {
+  RecArgs a;
+  memset(&a, 0, sizeof a);
+  a.H = kGruH[l]; a.n = n; a.F = F;
+  a.U = s.param[7 + 3 * l]; a.bh = s.param[8 + 3 * l] + 3 * kGruH[l];
+  a.gx = s.g1; a.h = s.h[l]; a.z = s.z[l]; a.r = s.r[l]; a.nn = s.nn[l]; a.hn = s.hn[l];
+  a.dgx = s.g1; a.dgh = s.g2; a.carry = s.carry; a.frames = frames;
+  return a;
+}
+// GRU l's output at hop t: slot t+1 of its states
+float *out_of(const pnb_train_state &s, int l, int n) { return s.h[l] + (size_t)n * kGruH[l]; }
+}  // namespace
+
+// The forward half on the network input staged in s.x ([F][n][70]): fc, conv1, conv2, the five GRUs with everything
+// their backward needs saved, fc_gb and fc_rb into s.pred.  15 launches.
+static int forward_half(pnb_engine *e, Launcher &L, const int *frames, int F) {
   pnb_train_state &s = *e->train;
   const int n = e->n_active, R = F * n;
   const size_t nb = (size_t)n;
-  const long long launches0 = e->launches;
-  Launcher L{e, st};
+  const cudaStream_t st = L.st;
   float *const *P = s.param;
-  float *G = s.grad;
-  const size_t *O = s.off;
-  // per call: the counters, the flag and the zero slots (the row stride n changes from call to call)
-  TCK(cudaMemsetAsync(s.cnt, 0, 10 * sizeof(unsigned), st));
-  TCK(cudaMemsetAsync(s.bad, 0, sizeof(int), st));
+  // per call: the forward counters and the zero slots (the row stride n changes from call to call)
+  TCK(cudaMemsetAsync(s.cnt, 0, 5 * sizeof(unsigned), st));
   TCK(cudaMemsetAsync(s.fc, 0, 4 * nb * 128 * sizeof(float), st));
   TCK(cudaMemsetAsync(s.c1, 0, 2 * nb * 512 * sizeof(float), st));
   for (int l = 0; l < 5; l++) TCK(cudaMemsetAsync(s.h[l], 0, nb * kGruH[l] * sizeof(float), st));
-  TCK(cudaMemsetAsync(s.dc2 + (size_t)R * 512, 0, 2 * nb * 512 * sizeof(float), st));
-  TCK(cudaMemsetAsync(s.ea + (size_t)R * 512, 0, 4 * nb * 512 * sizeof(float), st));
-
-  // ---- stage: {30 rec[0..67], rec[68], rec[69]}, zero past each window's end
-  { LaunchScope m(e, kUnprofiled, st); launch_rows_stage(s.x, kFeat, rec, rec_stride, PNB_RECORD_FLOATS, 68, n, n, F, st); }
-  { LaunchScope m(e, kUnprofiled, st); train_mask_kernel<<<blocks_for((size_t)R * kFeat), 256, 0, st>>>(s.x, frames, n, F); }
-  L.check();
-
-  // ---- forward
   float *fc_out = s.fc + 4 * nb * 128, *c1_out = s.c1 + 2 * nb * 512;
   { TSeg a[1] = {tseg(s.x, kFeat, P[0], 128, kFeat)}; L.gemm(false, a, 1, R, 128, fc_out, 128, P[1], kEpiRelu); }
   {
@@ -636,58 +661,54 @@ int train_grad(pnb_engine *e, const float *rec, size_t rec_stride, const int *fr
     for (int q = 0; q < 3; q++) a[q] = tseg(s.c1 + q * nb * 512, 512, P[4] + (size_t)q * 512 * 512, 512, 512);
     L.gemm(false, a, 3, R, 512, s.c2, 512, P[5], kEpiTanh, false, nullptr, 512, s.c2p);
   }
-  auto rec_args = [&](int l) {
-    RecArgs a;
-    memset(&a, 0, sizeof a);
-    a.H = kGruH[l]; a.n = n; a.F = F;
-    a.U = P[7 + 3 * l]; a.bh = P[8 + 3 * l] + 3 * kGruH[l];
-    a.gx = s.g1; a.h = s.h[l]; a.z = s.z[l]; a.r = s.r[l]; a.nn = s.nn[l]; a.hn = s.hn[l];
-    a.dgx = s.g1; a.dgh = s.g2; a.carry = s.carry; a.frames = frames;
-    return a;
-  };
-  auto out_of = [&](int l) { return s.h[l] + nb * kGruH[l]; };  // the layer's output at hop t: slot t+1
   for (int l = 0; l < 5; l++) {
     const int H = kGruH[l], H3 = 3 * H;
     const float *W = P[6 + 3 * l], *b = P[8 + 3 * l];
     if (l == 0) { TSeg a[1] = {tseg(s.c2, 512, W, H3, 512)}; L.gemm(false, a, 1, R, H3, s.g1, H3, b); }
-    else if (l < 4) { TSeg a[1] = {tseg(out_of(l - 1), 512, W, H3, 512)}; L.gemm(false, a, 1, R, H3, s.g1, H3, b); }
+    else if (l < 4) { TSeg a[1] = {tseg(out_of(s, l - 1, n), 512, W, H3, 512)}; L.gemm(false, a, 1, R, H3, s.g1, H3, b); }
     else {
-      TSeg a[2] = {tseg(out_of(2), 512, W, H3, 512), tseg(s.c2, 512, W + (size_t)512 * H3, H3, 512)};
+      TSeg a[2] = {tseg(out_of(s, 2, n), 512, W, H3, 512), tseg(s.c2, 512, W + (size_t)512 * H3, H3, 512)};
       L.gemm(false, a, 2, R, H3, s.g1, H3, b);
     }
-    RecArgs a = rec_args(l);
+    RecArgs a = rec_args(s, l, n, F, frames);
     a.cnt = s.cnt + l;
     L.rec(a, true);
   }
   {
     TSeg a[5] = {tseg(s.c2, 512, P[21], 34, 512)};
-    for (int q = 1; q < 5; q++) a[q] = tseg(out_of(q - 1), 512, P[21] + (size_t)q * 512 * 34, 34, 512);
+    for (int q = 1; q < 5; q++) a[q] = tseg(out_of(s, q - 1, n), 512, P[21] + (size_t)q * 512 * 34, 34, 512);
     L.gemm(false, a, 5, R, 34, s.pred, 68, P[22], kEpiSigmoid);
-    TSeg c[1] = {tseg(out_of(4), 128, P[23], 34, 128)};
+    TSeg c[1] = {tseg(out_of(s, 4, n), 128, P[23], 34, 128)};
     L.gemm(false, c, 1, R, 34, s.pred + 34, 68, P[24], kEpiSigmoid);
   }
+  return PNB_OK;
+}
 
-  // ---- loss and its gradient at the output pre-activations
-  { LaunchScope m(e, kUnprofiled, st); launch_loss_sums(s.pred, rec, rec_stride, frames, sums, n, n, F, st); }
-  long long counted = 0;
-  for (int i = 0; i < n; i++) counted += h_frames ? h_frames[i] : F;
-  {
-    LaunchScope m(e, kUnprofiled, st);
-    train_dpre_kernel<<<blocks_for((size_t)R * 68), 256, 0, st>>>(s.pred, rec, rec_stride, frames, n, F,
-                                                                  1.0 / ((double)counted * kBands), s.dpre);
-  }
-  L.check();
-
-  // ---- backward.  Weight gradients go straight into the flat gradient at their blob offsets.
+// The backward half of the forward half's call, from the gradient at the output pre-activations in s.dpre: output
+// layers, then the GRUs in reverse dependency order, conv2, conv1, fc.  Weight gradients go straight into the flat
+// gradient at their blob offsets; fc's pre-activation gradient is left in s.eb.  98 launches.
+static int backward_half(pnb_engine *e, Launcher &L, const int *frames, int F) {
+  pnb_train_state &s = *e->train;
+  const int n = e->n_active, R = F * n;
+  const size_t nb = (size_t)n;
+  const cudaStream_t st = L.st;
+  float *const *P = s.param;
+  float *G = s.grad;
+  const size_t *O = s.off;
+  TCK(cudaMemsetAsync(s.cnt + 5, 0, 5 * sizeof(unsigned), st));
+  TCK(cudaMemsetAsync(s.dc2 + (size_t)R * 512, 0, 2 * nb * 512 * sizeof(float), st));
+  TCK(cudaMemsetAsync(s.ea + (size_t)R * 512, 0, 4 * nb * 512 * sizeof(float), st));
+  const float *fc_out = s.fc + 4 * nb * 128, *c1_out = s.c1 + 2 * nb * 512;
+  auto out = [&](int l) { return out_of(s, l, n); };
   const float *dg = s.dpre, *dr = s.dpre + 34;
   // fc_rb
-  L.wgrad(out_of(4), 128, 128, dr, 68, 34, R, G + O[23]);
+  L.wgrad(out(4), 128, 128, dr, 68, 34, R, G + O[23]);
   L.wgrad(nullptr, 0, 1, dr, 68, 34, R, G + O[24]);
   { TSeg a[1] = {tseg(dr, 68, P[23], 34, 34)}; L.gemm(true, a, 1, R, 128, s.ea, 128); }
   // a GRU's recurrence backwards and its weight gradients; X segments: its inputs
   auto gru_back = [&](int l, const float *ext, const float *X0, const float *X1) {
     const int H = kGruH[l], H3 = 3 * H;
-    RecArgs a = rec_args(l);
+    RecArgs a = rec_args(s, l, n, F, frames);
     a.dh_ext = ext;
     a.cnt = s.cnt + 5 + l;
     L.rec(a, false);
@@ -700,7 +721,7 @@ int train_grad(pnb_engine *e, const float *rec, size_t rec_stride, const int *fr
   const float *Wfg = P[21];
   auto fcgb_rows = [&](int q) { return tseg(dg, 68, Wfg + (size_t)q * 512 * 34, 34, 34); };  // dY_g W_fcgb[q]^T
   // gru_rb: its inputs are [gru3, conv2]
-  gru_back(4, s.ea, out_of(2), s.c2);
+  gru_back(4, s.ea, out(2), s.c2);
   {
     const float *W = P[18];
     TSeg a[1] = {tseg(s.g1, 384, W, 384, 384)};
@@ -710,17 +731,17 @@ int train_grad(pnb_engine *e, const float *rec, size_t rec_stride, const int *fr
   }
   // fc_gb
   L.wgrad(s.c2, 512, 512, dg, 68, 34, R, G + O[21]);
-  for (int q = 1; q < 5; q++) L.wgrad(out_of(q - 1), 512, 512, dg, 68, 34, R, G + O[21] + (size_t)q * 512 * 34);
+  for (int q = 1; q < 5; q++) L.wgrad(out(q - 1), 512, 512, dg, 68, 34, R, G + O[21] + (size_t)q * 512 * 34);
   L.wgrad(nullptr, 0, 1, dg, 68, 34, R, G + O[22]);
   { TSeg a[1] = {fcgb_rows(0)}; L.gemm(true, a, 1, R, 512, s.dc2, 512, nullptr, kEpiNone, true); }
   // gru_gb
   { TSeg a[1] = {fcgb_rows(4)}; L.gemm(true, a, 1, R, 512, s.ea, 512); }
-  gru_back(3, s.ea, out_of(2), nullptr);
+  gru_back(3, s.ea, out(2), nullptr);
   { TSeg a[2] = {tseg(s.g1, 1536, P[15], 1536, 1536), fcgb_rows(3)}; L.gemm(true, a, 2, R, 512, s.eb, 512, nullptr, kEpiNone, true); }
   // gru3, gru2, gru1: each one's input gradient plus fc_gb's share is the layer below's
-  gru_back(2, s.eb, out_of(1), nullptr);
+  gru_back(2, s.eb, out(1), nullptr);
   { TSeg a[2] = {tseg(s.g1, 1536, P[12], 1536, 1536), fcgb_rows(2)}; L.gemm(true, a, 2, R, 512, s.ea, 512); }
-  gru_back(1, s.ea, out_of(0), nullptr);
+  gru_back(1, s.ea, out(0), nullptr);
   { TSeg a[2] = {tseg(s.g1, 1536, P[9], 1536, 1536), fcgb_rows(1)}; L.gemm(true, a, 2, R, 512, s.eb, 512); }
   gru_back(0, s.eb, s.c2, nullptr);
   // conv2: its output gradient through tanh
@@ -741,10 +762,45 @@ int train_grad(pnb_engine *e, const float *rec, size_t rec_stride, const int *fr
   }
   L.wgrad(s.x, kFeat, kFeat, s.eb, 128, 128, R, G + O[0]);
   L.wgrad(nullptr, 0, 1, s.eb, 128, 128, R, G + O[1]);
+  return PNB_OK;
+}
 
-  const size_t N = O[kParams];
-  { LaunchScope m(e, kUnprofiled, st); train_check_kernel<<<blocks_for(N, 1024), 256, 0, st>>>(G, N, s.bad, e->d_status); }
+// The check of the held gradient: s.bad zeroed, then raised (and the domain bit in status, unless null) by a
+// non-finite value.  1 launch.
+static int check_grad(pnb_engine *e, Launcher &L, int *status) {
+  const pnb_train_state &s = *e->train;
+  const size_t N = s.off[kParams];
+  TCK(cudaMemsetAsync(s.bad, 0, sizeof(int), L.st));
+  { LaunchScope m(e, kUnprofiled, L.st); train_check_kernel<<<blocks_for(N, 1024), 256, 0, L.st>>>(s.grad, N, s.bad, status); }
   L.check();
+  return PNB_OK;
+}
+
+int train_grad(pnb_engine *e, const float *rec, size_t rec_stride, const int *frames, const int *h_frames, double *sums,
+               int F, cudaStream_t st) {
+  pnb_train_state &s = *e->train;
+  const int n = e->n_active, R = F * n;
+  const long long launches0 = e->launches;
+  Launcher L{e, st};
+  // ---- stage: {30 rec[0..67], rec[68], rec[69]}, zero past each window's end
+  { LaunchScope m(e, kUnprofiled, st); launch_rows_stage(s.x, kFeat, rec, rec_stride, PNB_RECORD_FLOATS, 68, n, n, F, st); }
+  { LaunchScope m(e, kUnprofiled, st); train_mask_kernel<<<blocks_for((size_t)R * kFeat), 256, 0, st>>>(s.x, frames, n, F); }
+  L.check();
+  if (int rc = forward_half(e, L, frames, F)) return rc;
+
+  // ---- loss and its gradient at the output pre-activations
+  { LaunchScope m(e, kUnprofiled, st); launch_loss_sums(s.pred, rec, rec_stride, frames, sums, n, n, F, st); }
+  long long counted = 0;
+  for (int i = 0; i < n; i++) counted += h_frames ? h_frames[i] : F;
+  {
+    LaunchScope m(e, kUnprofiled, st);
+    train_dpre_kernel<<<blocks_for((size_t)R * 68), 256, 0, st>>>(s.pred, rec, rec_stride, frames, n, F,
+                                                                  1.0 / ((double)counted * kBands), s.dpre);
+  }
+  L.check();
+
+  if (int rc = backward_half(e, L, frames, F)) return rc;
+  if (int rc = check_grad(e, L, e->d_status)) return rc;
   TCK(L.err);
   // pnb_launches_per_call reports train_grad_launches: the schedule above and that count must agree
   if (e->launches - launches0 != train_grad_launches(e))
@@ -755,14 +811,71 @@ int train_grad(pnb_engine *e, const float *rec, size_t rec_stride, const int *fr
   return PNB_OK;
 }
 
+// A forward of the caller's network input (70 features per hop, not scaled) on windows [0, n_active), each from zero
+// state; weights (or null) first replace the parameters, and the predictions go to the caller's rows.
+int train_forward(pnb_engine *e, const float *x, size_t x_stride, const float *weights, float *out, size_t out_stride,
+                  int F, cudaStream_t st) {
+  pnb_train_state &s = *e->train;
+  const int n = e->n_active;
+  const long long launches0 = e->launches;
+  Launcher L{e, st};
+  if (weights)
+    for (int i = 0; i < kParams; i++)
+      TCK(cudaMemcpyAsync(s.param[i], weights + s.off[i], (s.off[i + 1] - s.off[i]) * sizeof(float),
+                          cudaMemcpyDeviceToDevice, st));
+  { LaunchScope m(e, kUnprofiled, st); launch_rows_stage(s.x, kFeat, x, x_stride, kFeat, 0, n, n, F, st); }
+  L.check();
+  if (int rc = forward_half(e, L, nullptr, F)) return rc;
+  { LaunchScope m(e, kUnprofiled, st); launch_rows_store(s.pred, 68, out, out_stride, n, n, F, st); }
+  L.check();
+  TCK(L.err);
+  if (e->launches - launches0 != train_forward_launches(e))
+    return engine_fail(PNB_ERR_CUDA, "train_forward issued a launch count train_forward_launches does not know");
+  s.last_F = F;
+  s.last_n = n;
+  return PNB_OK;
+}
+
+// The backward of the last train_forward from the caller's gradient at its output: the seed, the backward half, and the
+// input gradient when asked for; the gradient becomes the held one (its check skips the next Adam step, but raises no
+// domain bit: the caller owns the loss) and, when asked for, is copied out in blob order.
+int train_backward(pnb_engine *e, const float *dout, size_t dout_stride, float *dx, size_t dx_stride, float *grad,
+                   cudaStream_t st) {
+  pnb_train_state &s = *e->train;
+  const int n = s.last_n, F = s.last_F, R = F * n;
+  const long long launches0 = e->launches;
+  Launcher L{e, st};
+  {
+    LaunchScope m(e, kUnprofiled, st);
+    train_seed_kernel<<<blocks_for((size_t)R * 68), 256, 0, st>>>(dout, dout_stride, s.pred, n, F, s.dpre);
+  }
+  L.check();
+  if (int rc = backward_half(e, L, nullptr, F)) return rc;
+  if (dx) {  // dL/dx = dA_fc W_fc^T, then out to the caller's rows
+    TSeg a[1] = {tseg(s.eb, 128, s.param[0], 128, 128)};
+    L.gemm(true, a, 1, R, kFeat, s.g1, kFeat);
+    { LaunchScope m(e, kUnprofiled, st); launch_rows_store(s.g1, kFeat, dx, dx_stride, n, n, F, st); }
+    L.check();
+  }
+  if (int rc = check_grad(e, L, nullptr)) return rc;
+  if (grad) TCK(cudaMemcpyAsync(grad, s.grad, s.off[kParams] * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  TCK(L.err);
+  if (e->launches - launches0 != train_backward_launches(e, dx != nullptr))
+    return engine_fail(PNB_ERR_CUDA, "train_backward issued a launch count train_backward_launches does not know");
+  e->train_hops = (long long)n * F;
+  return PNB_OK;
+}
+
 int train_tap(const pnb_engine *e, int what, const void **src, size_t *bytes) {
   if (!e->train) return engine_fail(PNB_ERR_ARG, "the PNB_TAP_TRAIN_* taps need a PNB_TRAIN_NETWORK engine");
   const pnb_train_state &s = *e->train;
-  if (!s.last_F) return engine_fail(PNB_ERR_ARG, "the PNB_TAP_TRAIN_* taps need a pnb_train_grad_* call first");
+  if (!s.last_F)
+    return engine_fail(PNB_ERR_ARG, "the PNB_TAP_TRAIN_* taps need a pnb_train_grad_* or pnb_train_forward_device call first");
   const size_t nb = (size_t)s.last_n, rows = (size_t)s.last_F * nb;
   switch (what) {
     case PNB_TAP_TRAIN_FC: *src = s.fc + 4 * nb * 128; *bytes = rows * 128 * sizeof(float); break;
     case PNB_TAP_TRAIN_C1: *src = s.c1 + 2 * nb * 512; *bytes = rows * 512 * sizeof(float); break;
+    case PNB_TAP_TRAIN_DPRE: *src = s.dpre; *bytes = rows * 68 * sizeof(float); break;
     default: *src = s.c2p; *bytes = rows * 512 * sizeof(float); break;
   }
   return PNB_OK;
@@ -772,6 +885,10 @@ int train_tap(const pnb_engine *e, int what, const void **src, size_t *bytes) {
 // backward 99 (fc_rb 5, gru_rb 11 + 2, fc_gb 13, gru_gb 1 + 9 + 1, gru3 and gru2 9 + 1 each, gru1 9, conv2 9, conv1 13,
 // fc 5, check 1).
 int train_grad_launches(const pnb_engine *) { return 118; }
+// train_forward: stage 1, forward 15, store 1.  train_backward: seed 1, backward 98, check 1, and with the input
+// gradient its contraction and store 2.
+int train_forward_launches(const pnb_engine *) { return 17; }
+int train_backward_launches(const pnb_engine *, bool dx) { return dx ? 102 : 100; }
 
 int train_adam(pnb_engine *e, double lr, long long step, cudaStream_t st) {
   const pnb_train_state &s = *e->train;

@@ -34,8 +34,10 @@ extern "C" {
  *                     d_grad, when not NULL, receives it in blob order (N floats).  A non-finite value in it skips the next
  *                     pnb_train_adam on the device but does not raise PNB_ERR_DOMAIN: the caller owns the loss, and
  *                     non-finite gradients pass through as torch passes them.
- * A forward waits for one backward; pnb_reset, pnb_set_active_streams, a pnb_train_grad_* call and that backward end the
- * wait.  Refused with PNB_ERR_ARG before anything is enqueued: an engine without PNB_TRAIN_NETWORK, n_frames outside
+ * A forward waits for one backward; pnb_reset, pnb_set_active_streams, a pnb_train_grad_* call, pnb_train_adam,
+ * pnb_train_import of PNB_TRAIN_WEIGHTS (the last two rewrite the weights the backward would take) and that backward
+ * end the wait; imports of the moments or the accumulator, pnb_train_accumulate and pnb_train_finish keep it.
+ * Refused with PNB_ERR_ARG before anything is enqueued: an engine without PNB_TRAIN_NETWORK, n_frames outside
  * [1, max_frames_per_call], a NULL d_x, d_out or d_dout, a short stride, a backward with no forward waiting for it, a
  * poisoned engine (PNB_ERR_CUDA).  Each call issues a fixed number of launches whatever n_frames: 17 for a forward,
  * 100 for a backward, 102 with d_dx. */

@@ -426,8 +426,8 @@ class Engine:
         self._call("pnb_train_adam", float(lr), int(step), stream)
 
     def train_accumulate(self, stream: int = 0):
-        """pnb_train_accumulate: the gradient of the last train_grad, weighted by the hops it counted, into the engine's
-        float64 accumulator (micro-batches and ranks summed before one train_adam)."""
+        """pnb_train_accumulate: the gradient of the last gradient call or backward, weighted by the hops it counted, into
+        the engine's float64 accumulator (micro-batches and ranks summed before one train_adam)."""
         self._call("pnb_train_accumulate", stream)
 
     def train_finish(self, stream: int = 0):

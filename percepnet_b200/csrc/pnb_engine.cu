@@ -1026,7 +1026,8 @@ static int check_call(pnb_engine *e, Call &c) {
   if (c.kind == Call::kTrainBackward) {  // the hops of the forward it differentiates
     if (!e->train_fwd_F)
       return fail(PNB_ERR_ARG, "no pnb_train_forward_device call awaits its backward (one backward per forward; "
-                               "pnb_reset, pnb_set_active_streams and pnb_train_grad_* end a forward's wait)");
+                               "pnb_reset, pnb_set_active_streams, pnb_train_grad_*, pnb_train_adam and "
+                               "pnb_train_import of the weights end a forward's wait)");
     c.F = e->train_fwd_F;
   }
   if (train && !(e->flags & PNB_TRAIN_DATA)) return fail(PNB_ERR_ARG, "engine was not created with PNB_TRAIN_DATA");
@@ -1382,7 +1383,10 @@ extern "C" int pnb_train_adam(pnb_engine *e, double lr, long long step, void *cu
   if (e->train_open)
     return fail(PNB_ERR_ARG, "accumulated gradients are not finished: pnb_train_finish before pnb_train_adam");
   CK(cudaSetDevice(e->device));
-  return enqueue_ordered(e, (cudaStream_t)cuda_stream, [&] { return train_adam(e, lr, step, (cudaStream_t)cuda_stream); });
+  if (int rc = enqueue_ordered(e, (cudaStream_t)cuda_stream, [&] { return train_adam(e, lr, step, (cudaStream_t)cuda_stream); }))
+    return rc;
+  e->train_fwd_F = 0;  // the step rewrote the weights a pending forward's backward would take
+  return PNB_OK;
 }
 
 // Accumulation: the held gradient, weighted by the hops its call counted, into the float64 accumulator; and the
@@ -1391,7 +1395,7 @@ extern "C" int pnb_train_adam(pnb_engine *e, double lr, long long step, void *cu
 extern "C" int pnb_train_accumulate(pnb_engine *e, void *cuda_stream) {
   { int rc = check_trainer(e); if (rc) return rc; }
   if (!e->train_hops)
-    return fail(PNB_ERR_ARG, "no pnb_train_grad_* call since the last pnb_train_accumulate or pnb_train_finish: the "
+    return fail(PNB_ERR_ARG, "no gradient call or backward since the last pnb_train_accumulate or pnb_train_finish: the "
                              "held gradient is already counted");
   CK(cudaSetDevice(e->device));
   { int rc = train_accum_prepare(e); if (rc) return rc; }
@@ -1435,6 +1439,7 @@ static int train_transfer(pnb_engine *e, int what, void *mem, size_t bytes, bool
   if (rc) return rc;
   CK(cudaStreamSynchronize(e->stream));
   if (accum && !out) e->train_open = true;
+  if (what == PNB_TRAIN_WEIGHTS && !out) e->train_fwd_F = 0;  // as after pnb_train_adam
   return PNB_OK;
 }
 extern "C" int pnb_train_export(pnb_engine *e, int what, void *dst, size_t bytes) { return train_transfer(e, what, dst, bytes, true); }

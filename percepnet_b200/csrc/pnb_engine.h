@@ -82,7 +82,8 @@ struct pnb_engine {
   long long train_hops = 0;
   bool train_open = false;
   // the hops of the pnb_train_forward_device call whose backward is still due (0: none).  Cleared by its backward,
-  // a gradient call, pnb_set_active_streams and pnb_reset: one backward per forward, on the rows that forward ran.
+  // a gradient call, pnb_set_active_streams, pnb_reset, pnb_train_adam and pnb_train_import of the weights: one
+  // backward per forward, on the rows and with the weights that forward ran.
   int train_fwd_F = 0;
   int last_frames = 0;
   // An analysis (pnb_analyze_*) whose synthesis (pnb_synthesize_*) is still due, set by the analysis and cleared by the

@@ -1,7 +1,10 @@
 """torch_module.PercepNet on the GPU: the bits of the trainer's forward and backward halves against pnb_train_grad_*
 and ATen, gradients of torch losses against float64 autograd of the torch restatement (train_oracle) at the module's
 own weights, stream order and determinism, the recompute of a forward whose engine moved on, launch counts, refusals,
-non-finite gradients, and rnn_train.py's training step closing the loop."""
+non-finite gradients, and rnn_train.py's training step closing the loop.  The halves' bits depend on the call alone
+(active rows of a larger engine, padded strides, NULL weights or gradient), their seed is ATen's at saturated outputs and
+non-finite or subnormal dL/d(out), and the module gives the plain step's bits for autocast, strided views, expanded or
+partial dL/d(out), no dL/dx and frozen parameters."""
 
 import numpy as np
 import pytest
@@ -9,7 +12,7 @@ import torch
 
 from percepnet_b200 import api, torch_module as tm
 from percepnet_b200.eval_records import loss_terms
-from percepnet_b200.weights import pack_state_dict, synth_state_dict
+from percepnet_b200.weights import N_PARAMS, pack_state_dict, synth_state_dict
 import train_oracle as O
 from test_gpu_train import LOWER, generator_records, moderate_records, trainer, windows
 
@@ -41,13 +44,15 @@ def arbitrary_loss(seed):
 
 
 def step(m, x, y, loss_fn, want_dx=True):
-    """zero_grad, forward, loss, backward: (out, loss, {name: grad}, dx)."""
+    """zero_grad, forward, loss, backward: (out, loss, {name: grad} of the parameters that require it, dx).  x keeps
+    its dtype and strides."""
     m.zero_grad(set_to_none=True)
-    x = x.clone().requires_grad_(want_dx)
+    x = x.detach().requires_grad_(want_dx)
     out = m(x)
     L = loss_fn(out, y)
     L.backward()
-    return out.detach(), float(L.detach()), {k: p.grad.detach().clone() for k, p in m.named_parameters()}, \
+    return out.detach(), float(L.detach()), \
+        {k: p.grad.detach().clone() for k, p in m.named_parameters() if p.requires_grad}, \
         (x.grad.detach().clone() if want_dx else None)
 
 
@@ -110,6 +115,121 @@ def test_halves_are_train_grads_bits():
     sb = torch.ops.aten.sigmoid_backward(dout.transpose(0, 1), out.transpose(0, 1)).cpu().numpy()
     assert np.array_equal(got.view(np.int32), np.ascontiguousarray(sb).view(np.int32))
     eng.close()
+
+
+SENTINEL = 0x7FA5A5A5   # a NaN bit pattern that no kernel writes: what a store must leave alone keeps it
+FWD_TAPS = ("train_fc", "train_c1", "train_c2pre")
+
+
+def padded(a, stride, pad=(float("nan"),)):
+    """a [n, T, w] as rows of `stride` floats, the padding cycling through `pad`."""
+    n = a.shape[0]
+    flat = a.reshape(n, -1)
+    p = torch.tensor(pad, dtype=torch.float32).repeat(stride - flat.shape[1])[:stride - flat.shape[1]]
+    return torch.cat([flat, p.to(a.device).expand(n, -1)], 1).contiguous()
+
+
+def sentinel(rows, stride):
+    return torch.full((rows, stride), SENTINEL, dtype=torch.int32, device="cuda").view(torch.float32)
+
+
+def _tbits(a):
+    return a.contiguous().view(torch.int32)
+
+
+def test_halves_bits_depend_on_the_call_alone():
+    """A 10 x 40 forward and backward on the active 10 rows of a 16 x 48 engine created with other weights, after
+    forward / backward pairs on all 16 rows and on 10 rows of 48 hops, through padded strides (x padded with NaN and
+    1e30, dL/d(out) with NaN) and the caller's blob: out, the fc / c1 / c2pre and dpre taps, dL/dx and d_grad (also the
+    exported gradient) are the bits of the same call with exact strides on a fresh 10 x 40 engine of the blob's
+    weights, whose weights the engine then holds.  The padding and rows 10..15 of out and dL/dx keep their sentinel.  A
+    forward with d_weights NULL after it, and a backward with d_grad NULL, give the same bits again."""
+    sd = synth_state_dict(1)
+    B, T, S, Fm = 10, 40, 16, 48
+    blob = torch.from_numpy(pack_state_dict(sd).flat()).cuda()
+    x = feats(moderate_records(B, T, 280))
+    dout = torch.randn((B, T, 68), generator=torch.Generator().manual_seed(281)).cuda()
+
+    base = trainer(sd, B, T)
+    out0, dx0 = torch.empty((B, T, 68), device="cuda"), torch.empty((B, T, 70), device="cuda")
+    g0 = torch.empty(N_PARAMS, device="cuda")
+    base.train_forward_device(x.data_ptr(), T * 70, T, 0, out0.data_ptr(), T * 68)
+    taps0 = {k: base.read_tap(k, T, B) for k in FWD_TAPS}
+    base.train_backward_device(dout.data_ptr(), T * 68, dx0.data_ptr(), T * 70, g0.data_ptr())
+    taps0["train_dpre"] = base.read_tap("train_dpre", T, B)
+    base.wait()
+    base.close()
+
+    eng = trainer(synth_state_dict(3), S, Fm)
+    for n in (S, B):                                 # rows and hops past the call's hold other values
+        eng.set_active(n)
+        xr = feats(moderate_records(n, Fm, 282 + n))
+        o, d = torch.empty((n, Fm, 68), device="cuda"), torch.empty((n, Fm, 70), device="cuda")
+        do = torch.rand((n, Fm, 68), device="cuda")
+        eng.train_forward_device(xr.data_ptr(), Fm * 70, Fm, 0, o.data_ptr(), Fm * 68)
+        eng.train_backward_device(do.data_ptr(), Fm * 68, d.data_ptr(), Fm * 70)
+        eng.wait()
+    xs, os_, ds, dxs = T * 70 + 5, T * 68 + 3, T * 68 + 7, T * 70 + 9
+    xp = padded(x, xs, (float("nan"), 1e30))
+    dp = padded(dout, ds)
+
+    def call(weights, want_grad):
+        out, dx = sentinel(S, os_), sentinel(S, dxs)
+        grad = sentinel(1, N_PARAMS)[0]
+        eng.train_forward_device(xp.data_ptr(), xs, T, weights, out.data_ptr(), os_)
+        taps = {k: eng.read_tap(k, T, B) for k in FWD_TAPS}
+        eng.train_backward_device(dp.data_ptr(), ds, dx.data_ptr(), dxs, grad.data_ptr() if want_grad else 0)
+        taps["train_dpre"] = eng.read_tap("train_dpre", T, B)
+        eng.wait()
+        return out, dx, grad, taps
+
+    for label, weights, want_grad in (("blob", blob.data_ptr(), True), ("d_weights NULL, d_grad NULL", 0, False)):
+        out, dx, grad, taps = call(weights, want_grad)
+        assert _bits(out[:B, :T * 68].reshape(B, T, 68), out0), (label, "out")
+        assert _bits(dx[:B, :T * 70].reshape(B, T, 70), dx0), (label, "dx")
+        for k, w in taps0.items():
+            assert np.array_equal(taps[k].view(np.int32), w.view(np.int32)), (label, k)
+        held = torch.from_numpy(eng.train_export("gradient")).cuda()
+        assert _bits(held, g0), (label, "held gradient")
+        if want_grad:
+            assert _bits(grad, g0), (label, "d_grad")
+        else:
+            assert bool((_tbits(grad) == SENTINEL).all()), (label, "d_grad NULL")
+        for name, a, w in (("out", out, T * 68), ("dx", dx, T * 70)):
+            assert bool((_tbits(a[:, w:]) == SENTINEL).all()), (label, name, "padding")
+            assert bool((_tbits(a[B:]) == SENTINEL).all()), (label, name, "rows past the active range")
+        assert np.array_equal(eng.train_export("weights").view(np.int32), blob.cpu().numpy().view(np.int32)), label
+    eng.close()
+
+
+def test_seed_at_saturated_outputs_and_edge_gradients():
+    """dL/d(out) of +-inf, NaN, +-0, +-FLT_TRUE_MIN, 1e-40 and +-3e38 (and 1) at every band, on outputs of exactly 1
+    and below 1e-12 (biases of +-30 on bands of both output layers): the seed is ATen's sigmoid_backward bit for bit,
+    the NaN of inf x 0 included."""
+    sd = synth_state_dict(0, 4.0)
+    for k in ("fc_gb.0.bias", "fc_rb.0.bias"):
+        sd[k] = sd[k].copy()
+        sd[k][:4], sd[k][4:8] = 30.0, -30.0
+    B, T = 3, 40
+    eng = trainer(sd, B, T)
+    x = feats(moderate_records(B, T, 290))
+    out = torch.empty((B, T, 68), device="cuda")
+    eng.train_forward_device(x.data_ptr(), T * 70, T, 0, out.data_ptr(), T * 68)
+    tiny = float(np.finfo(np.float32).smallest_subnormal)
+    edges = torch.tensor([float("inf"), -float("inf"), float("nan"), 0.0, -0.0, tiny, -tiny, 1e-40, 3e38, -3e38, 1.0])
+    # 11 values along the flat index: 68 hops' worth of bands step it by 68 = 2 (mod 11), so every band meets each
+    dout = edges[torch.arange(B * T * 68) % len(edges)].reshape(B, T, 68).cuda()
+    eng.train_backward_device(dout.data_ptr(), T * 68)
+    got = eng.read_tap("train_dpre", T, B)
+    eng.close()
+    want = torch.ops.aten.sigmoid_backward(dout, out).transpose(0, 1).cpu().numpy()
+    o = out.cpu().numpy()
+    print(f"\n{int((o == 1).sum())} outputs exactly 1, {int((o <= 1e-12).sum())} at or below 1e-12, "
+          f"{int((o == 0).sum())} exactly 0; {int(np.isnan(want).sum())} NaN seeds")
+    assert (o == 1).any() and (o <= 1e-12).any()
+    inf_at_one = np.isinf(dout.transpose(0, 1).cpu().numpy()) & (o.transpose(1, 0, 2) == 1)
+    assert inf_at_one.any() and np.isnan(want[inf_at_one]).all()
+    assert np.array_equal(got.view(np.int32), np.ascontiguousarray(want).view(np.int32))
 
 
 @pytest.mark.parametrize("B,T", [(3, 40), (8, 500)], ids=["3x40", "8x500"])
@@ -184,6 +304,66 @@ def test_growing_and_shrinking_shapes():
         _same_step(got, step(fresh, x, y, custom_loss), f"{B}x{T}")
         fresh.close()
     m.close()
+
+
+def test_module_edges_give_the_plain_steps_bits():
+    """fp16 and bf16 x under autocast (x.grad the plain dL/dx in that dtype), x as a strided slice and as a transposed
+    view, out.sum() (dL/d(out) expanded, stride 0) against an explicit weighting by ones, a loss of the g half only
+    against a weighting with zeros on r, x without requires_grad (100 launches in the backward, not 102) and a frozen fc
+    (the other 28 gradients): each gives the bits of the same step on float32 contiguous x."""
+    sd = synth_state_dict(1)
+    m = module(sd)
+    B, T = 4, 30
+    rec = moderate_records(B, T, 300)
+    x, y = feats(rec), torch.from_numpy(np.ascontiguousarray(rec[..., 70:])).cuda()
+    plain = step(m, x, y, custom_loss)
+    for dt in (torch.float16, torch.bfloat16):
+        xl = x.to(dt)
+        want = step(m, xl.float(), y, custom_loss)
+        with torch.autocast("cuda", dtype=dt):
+            got = step(m, xl, y, custom_loss)
+        assert got[3].dtype == dt, dt
+        _same_step(got, want[:3] + (want[3].to(dt),), str(dt))
+    wide = torch.full((B, 2 * T, 70), float("nan"), device="cuda")
+    wide[:, ::2] = x
+    for label, xv in (("[:, ::2] slice", wide[:, ::2]), ("transposed view", x.transpose(0, 1).contiguous().transpose(0, 1))):
+        assert not xv.is_contiguous() and torch.equal(xv, x)
+        _same_step(step(m, xv, y, custom_loss), plain, label)
+    _same_step(step(m, x, y, lambda o, y: o.sum()), step(m, x, y, lambda o, y: (o * torch.ones_like(o)).sum()),
+               "out.sum()")
+    w = torch.rand((B, T, 68), generator=torch.Generator().manual_seed(301)).cuda()
+    wz = w.clone()
+    wz[..., 34:] = 0
+    _same_step(step(m, x, y, lambda o, y: (o[..., :34] * w[..., :34]).sum()), step(m, x, y, lambda o, y: (o * wz).sum()),
+               "g half only")
+    tr = m._trainers[x.device]
+    m.zero_grad(set_to_none=True)
+    L = custom_loss(m(x), y)
+    n0 = tr.eng.launches
+    L.backward()
+    assert tr.eng.launches - n0 == 100
+    for k, p in m.named_parameters():
+        assert _bits(p.grad, plain[2][k]), ("x without requires_grad", k)
+    m.fc.requires_grad_(False)
+    got = step(m, x, y, custom_loss)
+    m.fc.requires_grad_(True)
+    assert sorted(got[2]) == sorted(k for k in plain[2] if not k.startswith("fc.")) and len(got[2]) == 28
+    _same_step(got, plain, "fc frozen")
+    m.close()
+
+
+def test_row_limit():
+    """B x T above 65535 x 64 rows raises ValueError before any engine exists (x an expanded zero-stride tensor, no
+    memory); pnb_create of a PNB_TRAIN_NETWORK engine one row above refuses it with PNB_ERR_ARG.  One stream of
+    4 194 241 hops: what the engine allocates before that check per stream (network state, the f32 chain's rings)
+    is then one stream's, and only the per-row feature and g/r buffers (2.3 GB) remain."""
+    m = module(synth_state_dict(0))
+    for shape in ((tm.MAX_ROWS + 1, 1, 70), (1, tm.MAX_ROWS + 1, 70), (2049, 2048, 70)):
+        with pytest.raises(ValueError, match="65535 x 64"):
+            m(torch.zeros((1, 1, 1), device="cuda").expand(*shape))
+    assert not m._trainers
+    with pytest.raises(api.PnbError, match=r"\(-1\): PNB_TRAIN_NETWORK: n_streams x max_frames_per_call above 65535 x 64"):
+        api.Engine(1, tm.MAX_ROWS + 1, pack_state_dict(synth_state_dict(0)), api.TRAIN_NETWORK)
 
 
 def test_launch_counts():
@@ -266,6 +446,47 @@ def test_refusals():
     with pytest.raises(api.PnbError, match="no pnb_train_forward_device"):
         bwd()                                        # and pnb_reset
     assert (eng.launches, n2 - n1, n3 - n2, n4 - n3) == (n5, 102, 17 + 118, 17)
+    eng.wait()
+    eng.close()
+
+    # an Adam step and an import of the weights rewrite the weights the pending forward's backward would take: both
+    # end the wait, and the refused backward changes nothing (the next step is a twin's that saw no refusal)
+    sd = synth_state_dict(0)
+    x = feats(moderate_records(B, T, 310))
+    dout = torch.rand((B, T, 68), generator=torch.Generator().manual_seed(311)).cuda()
+    w2 = pack_state_dict(synth_state_dict(2)).flat()
+    for label, change in (("train_adam", lambda e: e.train_adam(1e-3, 1)),
+                          ("train_import of the weights", lambda e: e.train_import("weights", w2))):
+        eng, twin = trainer(sd, B, T), trainer(sd, B, T)
+        runs = {}
+        for e in (eng, twin):
+            e.train_forward_device(x.data_ptr(), T * 70, T, 0, out.data_ptr(), T * 68)
+            e.train_backward_device(dout.data_ptr(), T * 68)
+        n0 = eng.launches
+        eng.train_forward_device(x.data_ptr(), T * 70, T, 0, out.data_ptr(), T * 68)
+        n1 = eng.launches
+        change(eng)
+        n2 = eng.launches
+        with pytest.raises(api.PnbError, match="no pnb_train_forward_device.*pnb_train_adam"):
+            eng.train_backward_device(dout.data_ptr(), T * 68, dx.data_ptr(), T * 70)
+        assert (n1 - n0, eng.launches) == (17, n2), label
+        change(twin)
+        for name, e in (("refused", eng), ("twin", twin)):
+            o, d = torch.empty_like(out), torch.empty_like(dx)
+            g = torch.empty(N_PARAMS, device="cuda")
+            e.train_forward_device(x.data_ptr(), T * 70, T, 0, o.data_ptr(), T * 68)
+            e.train_backward_device(dout.data_ptr(), T * 68, d.data_ptr(), T * 70, g.data_ptr())
+            e.wait()
+            runs[name] = (o, d, g, e.train_export("weights"))
+            e.close()
+        for k in range(3):
+            assert _bits(runs["refused"][k], runs["twin"][k]), (label, k)
+        assert np.array_equal(runs["refused"][3].view(np.int32), runs["twin"][3].view(np.int32)), label
+    # an import of m keeps the wait: the parameters are unchanged
+    eng = trainer(sd, B, T)
+    eng.train_forward_device(x.data_ptr(), T * 70, T, 0, out.data_ptr(), T * 68)
+    eng.train_import("m", np.zeros(N_PARAMS, np.float32))
+    eng.train_backward_device(dout.data_ptr(), T * 68, dx.data_ptr(), T * 70)
     eng.wait()
     eng.close()
 

@@ -1,5 +1,6 @@
 """Gradient accumulation on the trainer (pnb_train_accumulate / pnb_train_finish / PNB_TRAIN_ACCUM): one micro-batch
-finishes to the call's own gradient bit for bit, splits of a batch meet the float64 bars of the whole batch (and
+finishes to the call's own gradient bit for bit, splits of a batch meet the float64 bars of the whole batch (and, for
+gradients of the forward and backward halves, also split batches; and
 weighting by windows instead of hops does not), exported accumulators sum across engines bit for bit, a NaN in any
 micro-batch skips the step, and every refusal leaves every bit as it was."""
 import ctypes as C
@@ -30,10 +31,27 @@ def state(eng):
     return {k: eng.train_export(k) for k in ("weights", "m", "v", "gradient", "accum")}
 
 
-@pytest.mark.parametrize("B,T,frames", [(3, 40, [40, 23, 40]), (10, 500, "ragged")], ids=["3x40", "10x500"])
+def halves(eng, rec):
+    """pnb_train_forward_device and pnb_train_backward_device on the records' full windows, with dL/d(out) torch
+    autograd of CustomLoss (the mean over these windows) at the fp32 out: returns that out."""
+    B, T = rec.shape[:2]
+    x = torch.from_numpy(O.features(rec)).cuda()
+    y = torch.from_numpy(np.ascontiguousarray(rec[..., 70:])).cuda()
+    out = torch.empty((B, T, 68), device="cuda")
+    eng.train_forward_device(x.data_ptr(), T * 70, T, 0, out.data_ptr(), T * 68)
+    o = out.clone().requires_grad_(True)
+    O.loss(o, y).backward()
+    eng.train_backward_device(o.grad.data_ptr(), T * 68)
+    eng.wait()
+    return out.cpu().numpy()
+
+
+@pytest.mark.parametrize("B,T,frames", [(3, 40, [40, 23, 40]), (10, 500, "ragged"), (3, 40, "halves")],
+                         ids=["3x40", "10x500", "3x40-halves"])
 def test_one_micro_batch_is_the_call(B, T, frames):
     """grad -> accumulate -> finish holds the call's own gradient, bit for bit, and Adam after it gives the same
-    weights, m and v; accumulate issues one launch and finish two."""
+    weights, m and v; accumulate issues one launch and finish two.  "halves": the gradient of a backward after its
+    forward instead of a gradient call's."""
     sd = synth_state_dict(1)
     rec = moderate_records(B, T, 200 + B)
     if frames == "ragged":
@@ -41,7 +59,7 @@ def test_one_micro_batch_is_the_call(B, T, frames):
     plain, acc = trainer(sd, B, T), trainer(sd, B, T)
     out = {}
     for name, eng in (("plain", plain), ("accumulated", acc)):
-        s = eng.train_grad(rec, frames)
+        s = halves(eng, rec) if frames == "halves" else eng.train_grad(rec, frames)
         if eng is acc:
             n0 = eng.launches
             eng.train_accumulate()
@@ -54,7 +72,7 @@ def test_one_micro_batch_is_the_call(B, T, frames):
         eng.train_adam(1e-3, 1)
         eng.wait()
         out[name] = (s, g) + tuple(eng.train_export(k) for k in ("weights", "m", "v"))
-    for k, name in enumerate(("sums", "gradient", "weights", "m", "v")):
+    for k, name in enumerate(("sums or out", "gradient", "weights", "m", "v")):
         assert same_bits(out["plain"][k], out["accumulated"][k]), name
     assert np.any(out["plain"][1] != 0)
     plain.close()
@@ -80,7 +98,8 @@ def test_splits_against_float64():
     """8 x 500 moderate records split as {8}, {4, 4} and {1, 3, 4} (the 3 holding windows of 1, 7 and 30 hops): every
     finished gradient meets the float64 bars of the whole batch and is close to the one-call gradient, and equals the
     hop-weighted float64 combination of the micro-batches' own gradients bit for bit.  Weighting the same gradients by
-    windows misses the bars."""
+    windows misses the bars.  The full windows cut {4, 4} through the halves, each half seeded with CustomLoss's mean
+    over its own windows, meet the float64 bars of the whole batch."""
     sd = synth_state_dict(1)
     B, T = 8, 500
     rec = moderate_records(B, T, 210)
@@ -118,6 +137,16 @@ def test_splits_against_float64():
             wrong = failing(rel_errors(unpack_state_dict(PackedModel.from_flat(by_windows.astype(np.float32))), g64))
             print(f"  weighted by windows instead of hops: {len(wrong)} of {len(g64)} tensors miss the bars")
             assert len(wrong) > 0
+    _, g64 = O.grads(sd, rec, None, torch.float64, "cuda")
+    eng.set_active(4)
+    for b0 in (0, 4):
+        halves(eng, np.ascontiguousarray(rec[b0:b0 + 4]))
+        eng.train_accumulate()
+    eng.train_finish()
+    err = rel_errors(unpack_state_dict(PackedModel.from_flat(eng.train_export("gradient"))), g64)
+    worst = max(err, key=lambda k: err[k][0])
+    print(f"halves {{4, 4}}, full windows: worst {worst} {err[worst][0]:.2e} / {err[worst][1]:.2e} against float64")
+    assert not failing(err), failing(err)
     eng.close()
 
 

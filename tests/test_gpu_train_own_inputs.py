@@ -8,6 +8,9 @@ and conv2 to a bar.  Here the two questions are taken apart:
   FMA chain;
 * the backward: all 30 gradient tensors against float64 autograd at the trainer's own forward values
   (train_oracle.grads_at, through the PNB_TAP_TRAIN_* taps), with the bars of test_gpu_train.py.
+The same for the forward and backward halves (pnb_train_forward_device / pnb_train_backward_device), seeded with a
+torch loss's dL/d(out) at their own fp32 output: their output against float64 at the own values, and dL/dx held to the
+gradients' bars too.
 What remains is the accuracy of the trainer's own arithmetic, which is what a defect in its kernels would move."""
 import os
 
@@ -19,7 +22,8 @@ import torch.nn.functional as Fn
 from conftest import GOLDEN
 from percepnet_b200 import api
 from percepnet_b200.eval_records import loss_terms
-from percepnet_b200.weights import pack_state_dict, synth_state_dict
+from percepnet_b200.weights import N_PARAMS, PackedModel, pack_state_dict, synth_state_dict, unpack_state_dict
+from test_gpu_torch_module import arbitrary_loss
 from test_gpu_train import grads_of, ragged_frames, trainer, windows
 import train_oracle as O
 
@@ -42,6 +46,30 @@ def run_trainer(sd, rec, frames):
     taps = [eng.read_tap(name, T, B) for name in TAPS]
     eng.close()
     return loss_terms(sums.sum(0))["total"], g, taps
+
+
+def run_halves(sd, rec, engine):
+    """One forward and one backward of the halves on the first B rows of an engine of shape `engine` (active B), x the
+    records' features, dL/d(out) arbitrary_loss's at the fp32 out: (out, dout, gradients and dL/dx by name, taps)."""
+    B, T = rec.shape[:2]
+    eng = trainer(sd, *engine)
+    if engine[0] != B:
+        eng.set_active(B)
+    x = torch.from_numpy(O.features(rec)).cuda()
+    out = torch.empty((B, T, 68), device="cuda")
+    eng.train_forward_device(x.data_ptr(), T * 70, T, 0, out.data_ptr(), T * 68)
+    taps = [eng.read_tap(name, T, B) for name in TAPS]
+    o = out.clone().requires_grad_(True)
+    arbitrary_loss(B)(o, None).backward()
+    dout = o.grad.detach().contiguous()
+    dx = torch.empty((B, T, 70), device="cuda")
+    grad = torch.empty(N_PARAMS, device="cuda")
+    eng.train_backward_device(dout.data_ptr(), T * 68, dx.data_ptr(), T * 70, grad.data_ptr())
+    eng.wait()
+    g = unpack_state_dict(PackedModel.from_flat(grad.cpu().numpy()))
+    g["dL/dx"] = dx.cpu().numpy()
+    eng.close()
+    return out.cpu().numpy(), dout.cpu().numpy().astype(np.float64), g, taps
 
 
 def staged_input(rec, frames):
@@ -107,9 +135,17 @@ def misses(err):
     return sorted(k for k, e in err.items() if not (e[0] <= 1e-4 and e[1] <= 1e-3))
 
 
-def check_at_own_inputs(sd, rec, frames, label, chunk=16):
+def check_at_own_inputs(sd, rec, frames, label, chunk=16, halves=None):
+    """The forward bound on fc, conv1 and conv2, and the gradients' bars at the own forward values, of a gradient call
+    (halves None) or of the forward and backward halves on the first B rows of an engine of shape `halves` (frames
+    None), whose out is also held within 1e-5 of float64's at the own values and whose dL/dx is held like a gradient."""
     B, T = rec.shape[:2]
-    loss, g, taps = run_trainer(sd, rec, frames)
+    if halves is None:
+        loss, g, taps = run_trainer(sd, rec, frames)
+        seed = {}
+    else:
+        out, dout, g, taps = run_halves(sd, rec, halves)
+        seed = dict(dout=dout, want_dx=True)
     print(f"\n{label}:")
     fwd = forward_errors(sd, rec, frames, taps, chunk)
     for k, (worst, p999) in fwd.items():
@@ -125,12 +161,25 @@ def check_at_own_inputs(sd, rec, frames, label, chunk=16):
     print(f"  smallest |c2p| per unit over counted hops: min {lo.min():.3g}, median {np.median(lo):.3g}, "
           f"max {lo.max():.3g}; {np.count_nonzero(lo > 43.7)} of 512 units above 43.7 (fp32 tanh' subnormal there)")
 
-    L64, g64 = O.grads_at(sd, rec, frames, *taps, chunk=chunk, device=DEVICE)
-    print(f"  loss {loss:.9e}, float64 at own inputs {L64:.9e}, rel {abs(loss - L64) / abs(L64):.2e}")
-    assert abs(loss - L64) <= 1e-6 * abs(L64)
+    def reference(**kw):
+        L64, g64, out64, dx64 = O.grads_at(sd, rec, frames, *taps, chunk=chunk, device=DEVICE, **seed, **kw)
+        if dx64 is not None:
+            g64["dL/dx"] = dx64
+        return L64, g64, out64
+
+    L64, g64, out64 = reference()
+    if halves is None:
+        print(f"  loss {loss:.9e}, float64 at own inputs {L64:.9e}, rel {abs(loss - L64) / abs(L64):.2e}")
+        assert abs(loss - L64) <= 1e-6 * abs(L64)
+    else:
+        d = float(np.abs(out - out64).max())
+        print(f"  max|out - out64| at own inputs {d:.2e}")
+        assert d <= 1e-5
     err = gradient_errors(g, g64)
     for k in sorted(err, key=lambda k: -err[k][0])[:3]:
         print(f"  {k}: |g - g64| / |g64| = {err[k][0]:.2e}, max|g - g64| / max|g64| = {err[k][1]:.2e}")
+    if "dL/dx" in err:
+        print(f"  dL/dx: |g - g64| / |g64| = {err['dL/dx'][0]:.2e}, max|g - g64| / max|g64| = {err['dL/dx'][1]:.2e}")
     zero = sorted(k for k in g64 if not np.any(g64[k]))
     if zero:
         print(f"  float64's gradient is exactly zero for {zero}; the trainer's max |g| there "
@@ -147,8 +196,7 @@ def check_at_own_inputs(sd, rec, frames, label, chunk=16):
         print(f"  {bad} miss the bar; {np.count_nonzero(tiny)} of {tiny.size} tanh' factors below FLT_MIN: "
               f"the kernel's fp32 factor taken there")
         assert tiny.any(), f"{label}: {bad} miss the bar at own inputs"
-        L64, g64 = O.grads_at(sd, rec, frames, *taps, chunk=chunk, device=DEVICE,
-                              dtanh=np.where(tiny, kernel_dtanh(c2p32), exact))
+        _, g64, _ = reference(dtanh=np.where(tiny, kernel_dtanh(c2p32), exact))
         err = gradient_errors(g, g64)
         for k in bad:
             print(f"  {k} with own factors below FLT_MIN: |g - g64| / |g64| = {err[k][0]:.2e}, "
@@ -183,6 +231,23 @@ def test_own_inputs_at_training_shapes(B, T, gain):
     rec = records(B, T, 210 + B)
     frames = ragged_frames(B, T, 220 + B) if T == 500 else None
     check_at_own_inputs(synth_state_dict(0, gain), rec, frames, f"{B}x{T} seed 0 gain {gain}")
+
+
+@pytest.mark.parametrize("gain", [1.0, 4.0], ids=["gain1", "gain4"])
+def test_halves_own_inputs_3x40(gain):
+    """The halves on 3 x 40: the two tests/golden/train.npz windows and one generator window."""
+    rec = records(3, 40, 203).copy()
+    rec[:2] = np.load(os.path.join(GOLDEN, "train.npz"))["records"][:, :40]
+    check_at_own_inputs(synth_state_dict(0, gain), rec, None, f"halves 3x40 gain {gain}", halves=(3, 40))
+
+
+@pytest.mark.parametrize("B,T,engine", [(10, 500, (16, 600)), (32, 500, (32, 500))], ids=["10x500-of-16x600", "32x500"])
+def test_halves_own_inputs_at_training_shapes(B, T, engine):
+    """The halves on the CLI's batch as the active 10 rows of a 16 x 600 engine in a 500-hop call, and on 32 x 500.
+    128 x 2000 is left to test_own_inputs_at_training_shapes: its long weight-gradient sums are backward_half's, which
+    the halves share with the gradient call; the halves' own kernels (stage, seed, dL/dx, stores) are per row."""
+    check_at_own_inputs(synth_state_dict(0), records(B, T, 210 + B), None, f"halves {B}x{T} on {engine[0]}x{engine[1]}",
+                        halves=engine)
 
 
 def test_train_taps_follow_the_last_gradient_call():

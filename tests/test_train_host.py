@@ -90,17 +90,33 @@ def test_closed_form_loss_gradient():
 
 def test_grads_at_own_values_is_grads():
     """grads_at fed float64's own forward values (fc and conv1 outputs, conv2's pre-activation) is grads, loss and all
-    30 tensors within 1e-12, with the taps cut into chunks of windows like the records."""
+    30 tensors within 1e-12, with the taps cut into chunks of windows like the records; and so is it seeded with
+    dL/d(out) of that loss instead, with dL/dx and out those of plain float64 autograd of the model within 1e-12."""
     sd = synth_state_dict(0)
     rec = records(3, 24, 7)
     frames = [24, 13, 24]
     L, g = O.grads(sd, rec, frames)
     fc, c1, c2p = O.forward_taps(sd, rec, frames)
     assert fc.shape == (24, 3, 128) and c1.shape == (24, 3, 512) and c2p.shape == (24, 3, 512)
-    La, ga = O.grads_at(sd, rec, frames, fc, c1, c2p, chunk=2)
-    assert abs(La - L) <= 1e-12 * abs(L)
+    La, ga, _, dxa = O.grads_at(sd, rec, frames, fc, c1, c2p, chunk=2)
+    assert abs(La - L) <= 1e-12 * abs(L) and dxa is None
     for k in g:
         assert np.linalg.norm(ga[k] - g[k]) <= 1e-12 * np.linalg.norm(g[k]), k
+
+    m = O.model(sd, torch.float64)
+    x, y, fr = O._inputs(rec, np.asarray(frames), slice(0, 3), frames, torch.float64, "cpu")
+    x.requires_grad_(True)
+    out = m(x)
+    dout, = torch.autograd.grad(O.loss(out, y, fr), out, retain_graph=True)
+    O.loss(out, y, fr).backward()
+    Ld, gd, outd, dxd = O.grads_at(sd, rec, frames, fc, c1, c2p, chunk=2, dout=dout.numpy(), want_dx=True)
+    assert Ld is None and outd.shape == (3, 24, 68) and dxd.shape == (3, 24, 70)
+    for k in g:
+        assert np.linalg.norm(gd[k] - g[k]) <= 1e-12 * np.linalg.norm(g[k]), k
+    dx = x.grad.numpy()
+    assert np.linalg.norm(dxd - dx) <= 1e-12 * np.linalg.norm(dx)
+    want = out.detach().numpy()
+    assert np.abs(outd - want).max() <= 1e-12 * np.abs(want).max()
 
 
 def test_grads_at_takes_tanh_prime_at_the_given_preactivation():
@@ -117,8 +133,8 @@ def test_grads_at_takes_tanh_prime_at_the_given_preactivation():
     p = a.copy()
     p[t, b, j] = 19.5
     assert np.tanh(20.0) == 1.0 and np.tanh(19.5) == 1.0
-    _, ga = O.grads_at(sd, rec, None, fc, c1, a)
-    _, gp = O.grads_at(sd, rec, None, fc, c1, p)
+    _, ga, _, _ = O.grads_at(sd, rec, None, fc, c1, a)
+    _, gp, _, _ = O.grads_at(sd, rec, None, fc, c1, p)
     for k in ga:
         if not k.startswith(("fc.", "conv1.", "conv2.")):
             assert bits_equal(ga[k], gp[k]), k

@@ -143,7 +143,8 @@ class TanhAtPre(torch.autograd.Function):
         return g * factor, None
 
 
-def grads_at(sd: dict, rec: np.ndarray, frames, fc32, c1_32, c2p32, chunk=None, device="cpu", dtanh=None):
+def grads_at(sd: dict, rec: np.ndarray, frames, fc32, c1_32, c2p32, chunk=None, device="cpu", dtanh=None, dout=None,
+             want_dx=False):
     """grads at the trainer's own forward values: float64 autograd as `grads`, with fc's and conv1's outputs and conv2's
     pre-activation pinned to fc32, c1_32 and c2p32 ([T][B][128 | 512 | 512], the PNB_TAP_TRAIN_* taps) by
     straight-through substitution.  fc = fc64 m + (fc32 - fc64 m).detach(), m = fc32 > 0 (the saved output's sign is the
@@ -151,16 +152,20 @@ def grads_at(sd: dict, rec: np.ndarray, frames, fc32, c1_32, c2p32, chunk=None, 
     c2p64).detach(), then c = tanh(c2p) (TanhAtPre) and the rest of Net.forward.  The values are the trainer's; the
     gradient still flows through the float64 weights and the masks, with tanh' at the trainer's own pre-activation.
     Hops past a window's end take the tapped values like any other.  dtanh: tanh' as [T][B][512] float64 instead of its
-    closed form at c2p32.  Returns (loss, {name: gradient})."""
+    closed form at c2p32.  dout: dL/d(out) as [B][T][68] float64, seeding the backward (out.backward(dout)) instead of
+    CustomLoss, as pnb_train_backward_device takes the caller's.  want_dx: also dL/dx ([B][T][70], through the masked fc64
+    path to the network input).
+    Returns (loss or None when dout is given, {name: gradient}, out at the own values [B][T][68], dL/dx or None)."""
     m = model(sd, torch.float64, device)
     B, T = rec.shape[:2]
     chunk = chunk or B
     counts = np.full(B, T, np.int64) if frames is None else np.asarray(frames, np.int64)
     total = float(counts.sum())
-    L = 0.0
+    L, outs, dxs = 0.0, [], []
     for c0 in range(0, B, chunk):
         part = slice(c0, min(B, c0 + chunk))
         x, y, fr = _inputs(rec, counts, part, frames, torch.float64, device)
+        x.requires_grad_(want_dx)
         # [T][B][w] taps -> [b, w, T] of this chunk, as float64
         tap = lambda a: torch.from_numpy(np.ascontiguousarray(np.asarray(a)[:, part].transpose(1, 2, 0))).to(
             device=device, dtype=torch.float64)
@@ -174,13 +179,22 @@ def grads_at(sd: dict, rec: np.ndarray, frames, fc32, c1_32, c2p32, chunk=None, 
         c2p64 = m.conv2[0](c1)[:, :, :-2]
         c2p = c2p64 + (c2p_t - c2p64).detach()
         c = TanhAtPre.apply(c2p, None if dtanh is None else tap(dtanh))
-        Lc = loss(m.head(c.permute(0, 2, 1)), y, fr)
-        if chunk < B:
-            Lc = Lc * (float(counts[part].sum()) / total)
-        Lc.backward()
-        L += float(Lc.detach())
-        del x, y, Lc
-    return L, {k: p.grad.detach().cpu().numpy() for k, p in m.named_parameters()}
+        out = m.head(c.permute(0, 2, 1))
+        outs.append(out.detach().cpu().numpy())
+        if dout is None:
+            Lc = loss(out, y, fr)
+            if chunk < B:
+                Lc = Lc * (float(counts[part].sum()) / total)
+            Lc.backward()
+            L += float(Lc.detach())
+            del Lc
+        else:
+            out.backward(torch.as_tensor(np.asarray(dout)[part], dtype=torch.float64, device=device))
+        if want_dx:
+            dxs.append(x.grad.detach().cpu().numpy())
+        del x, y, out
+    return (None if dout is not None else L, {k: p.grad.detach().cpu().numpy() for k, p in m.named_parameters()},
+            np.concatenate(outs), np.concatenate(dxs) if want_dx else None)
 
 
 def dloss_dpre(p: np.ndarray, y: np.ndarray, count: int) -> np.ndarray:

@@ -611,5 +611,6 @@ const char *pnb_version(void);
 }
 #endif
 #include "pnb_train_device.h"
+#include "pnb_train_state.h"
 
 #endif /* PERCEPNET_B200_H */

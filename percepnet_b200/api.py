@@ -1,4 +1,5 @@
-"""Python host mirror of the C-ABI in include/percepnet_b200.h and include/pnb_train_device.h (ctypes; no compute here).
+"""Python host mirror of the C-ABI in include/percepnet_b200.h, include/pnb_train_device.h and include/pnb_train_state.h
+(ctypes; no compute here).
 
 ``Engine`` is the batched-streams counterpart of the reference's ``DenoiseState``
 (/root/reference/src/rnnoise.h:49-60): ``Engine.process`` advances S independent 48 kHz streams by F
@@ -134,6 +135,13 @@ _TRAIN_DEVICE_SIGNATURES = {
     "pnb_train_backward_device": (_i, (_vp, _vp, _sz, _vp, _sz, _vp, _vp)),
 }
 TRAIN_DEVICE_EXPORTS = tuple(_TRAIN_DEVICE_SIGNATURES)
+# Every symbol of include/pnb_train_state.h (the same calls with network state and per-window lengths), the same way.
+_TRAIN_STATE_SIGNATURES = {
+    "pnb_train_forward_state_device": (_i, (_vp, _vp, _sz, _i, _vp, _vp, _vp, _sz, _vp, _sz, _vp, _sz, _vp)),
+    "pnb_train_backward_state_device": (_i, (_vp, _vp, _sz, _vp, _sz, _vp, _sz, _vp, _sz, _vp, _vp)),
+}
+TRAIN_STATE_EXPORTS = tuple(_TRAIN_STATE_SIGNATURES)
+TRAIN_STATE_FLOATS = 3712   # PNB_TRAIN_STATE_FLOATS: one window's network state
 
 
 def load_library() -> C.CDLL:
@@ -145,7 +153,7 @@ def load_library() -> C.CDLL:
         raise PnbError(f"{LIB_PATH} is missing: run `python -c 'import __graft_entry__ as g; g.build()'` "
                        "(nvcc, sm_90a).  There is no CPU implementation to fall back to.")
     L = C.CDLL(LIB_PATH)
-    for name, (restype, argtypes) in {**_SIGNATURES, **_TRAIN_DEVICE_SIGNATURES}.items():
+    for name, (restype, argtypes) in {**_SIGNATURES, **_TRAIN_DEVICE_SIGNATURES, **_TRAIN_STATE_SIGNATURES}.items():
         f = getattr(L, name)
         f.restype, f.argtypes = restype, argtypes
     _lib = L
@@ -361,11 +369,11 @@ class Engine:
         """pnb_compute_rnn_device on raw device pointers (format RNN_FEATURES or RNN_RECORDS; strides in floats)."""
         self._compute_rnn_device(None, None, format, d_in, in_stride, n_frames, d_gr, gr_stride, stream)
 
-    def _frames(self, frames):
+    def _frames(self, frames, what: str = "frames"):
         """frames (None, or one count per active row) as int32 or None."""
-        fr = None if frames is None else _int32s(frames, "frames")
+        fr = None if frames is None else _int32s(frames, what)
         if fr is not None and len(fr) != self.active:
-            raise PnbError("frames needs one entry per active row")
+            raise PnbError(f"{what} needs one entry per active row")
         return fr
 
     def score_records(self, x: np.ndarray, frames=None, want_gr: bool = False):
@@ -419,6 +427,25 @@ class Engine:
         train_forward_device in; dL/dx (d_dx, or 0 for none) and the blob-order gradient (d_grad, or 0) out.  The
         gradient is also the held one, for train_adam / train_accumulate."""
         self._call("pnb_train_backward_device", d_dout, dout_stride, d_dx, dx_stride, d_grad, stream)
+
+    def train_forward_state_device(self, d_x: int, x_stride: int, n_frames: int, lengths=None, d_weights: int = 0,
+                                   d_state_in: int = 0, state_in_stride: int = TRAIN_STATE_FLOATS, d_out: int = 0,
+                                   out_stride: int = 0, d_state_out: int = 0,
+                                   state_out_stride: int = TRAIN_STATE_FLOATS, stream: int = 0):
+        """pnb_train_forward_state_device on raw device pointers (strides in floats): train_forward_device from the
+        state rows d_state_in (0: zero state), the state at each window's end out to d_state_out (0: none); lengths: None,
+        or a host sequence of one hop count in [1, n_frames] per active row."""
+        self._call("pnb_train_forward_state_device", d_x, x_stride, n_frames, _ptr(self._frames(lengths, "lengths")),
+                   d_weights, d_state_in, state_in_stride, d_out, out_stride, d_state_out, state_out_stride, stream)
+
+    def train_backward_state_device(self, d_dout: int, dout_stride: int, d_dstate_out: int = 0,
+                                    dstate_out_stride: int = TRAIN_STATE_FLOATS, d_dx: int = 0, dx_stride: int = 0,
+                                    d_dstate_in: int = 0, dstate_in_stride: int = TRAIN_STATE_FLOATS, d_grad: int = 0,
+                                    stream: int = 0):
+        """pnb_train_backward_state_device on raw device pointers (strides in floats): train_backward_device with
+        dL/d(state out) in (d_dstate_out, or 0 for none) and dL/d(state in) out (d_dstate_in, or 0 for none)."""
+        self._call("pnb_train_backward_state_device", d_dout, dout_stride, d_dstate_out, dstate_out_stride, d_dx,
+                   dx_stride, d_dstate_in, dstate_in_stride, d_grad, stream)
 
     def train_adam(self, lr: float, step: int, stream: int = 0):
         """pnb_train_adam: one torch.optim.Adam step (defaults) with the gradient of the last train_grad; step counts

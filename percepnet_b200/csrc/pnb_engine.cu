@@ -679,7 +679,8 @@ struct Call {
   const int *hops;    // ragged and pool calls: each listed session's hops (host), or null; null once check_call finds
                       // them all equal to F
   int format;         // network calls: PNB_RNN_FEATURES or PNB_RNN_RECORDS
-  const int *frames;  // score and gradient calls: the hops each row's loss counts (host), or null for F
+  const int *frames;  // score and gradient calls: the hops each row's loss counts (host), or null for F; a training
+                      // forward: each window's hops (lengths)
   bool status = true;  // a blocking host call reads back and reports the status word (rejected imports, PNB_ERR_DOMAIN)
   bool pool = false;   // an analysis, synthesis or network call on a session list (pnb_*_sessions_*)
   const float *weights = nullptr;  // a training forward: the parameters in blob order (device), or null
@@ -896,11 +897,17 @@ static int enqueue_train(pnb_engine *e, const Call &c, cudaStream_t st) {
 // A training forward on st (arguments already checked): the caller's features through the trainer's forward half on
 // windows [0, n_active), its g/r out; its backward becomes due.  A training backward (arguments checked, so a forward of
 // F hops is due): the caller's dL/d(out) through the backward half into the held gradient, dL/dx out when asked for.
+// Either may carry network state: a forward's state in / state out rows and per-window lengths (c.frames), a backward's
+// dL/d(state out) / dL/d(state in) rows (in[1] / out[1], null when absent).
 static int enqueue_train_forward(pnb_engine *e, const Call &c, cudaStream_t st) {
   e->train_fwd_F = 0;
   const int rc = enqueue_call(e, c.F, st, [&]() -> int {
-    return train_forward(e, static_cast<const float *>(c.in[0].p), c.in[0].stride, c.weights, static_cast<float *>(c.out[0].p),
-                         c.out[0].stride, c.F, st);
+    const int *lengths = nullptr;
+    if (c.frames) { int rc = stage_ints(e, c.frames, (size_t)e->n_active, st, &lengths); if (rc) return rc; }
+    return train_forward(e, static_cast<const float *>(c.in[0].p), c.in[0].stride, c.weights,
+                         static_cast<const float *>(c.in[1].p), c.in[1].stride, lengths, c.frames,
+                         static_cast<float *>(c.out[0].p), c.out[0].stride, static_cast<float *>(c.out[1].p),
+                         c.out[1].stride, c.F, st);
   }, false);
   if (rc == PNB_OK) e->train_fwd_F = c.F;
   return rc;
@@ -908,8 +915,9 @@ static int enqueue_train_forward(pnb_engine *e, const Call &c, cudaStream_t st) 
 static int enqueue_train_backward(pnb_engine *e, const Call &c, cudaStream_t st) {
   e->train_fwd_F = 0;
   return enqueue_call(e, c.F, st, [&]() -> int {
-    return train_backward(e, static_cast<const float *>(c.in[0].p), c.in[0].stride, static_cast<float *>(c.out[0].p),
-                          c.out[0].stride, c.grad, st);
+    return train_backward(e, static_cast<const float *>(c.in[0].p), c.in[0].stride,
+                          static_cast<const float *>(c.in[1].p), c.in[1].stride, static_cast<float *>(c.out[0].p),
+                          c.out[0].stride, static_cast<float *>(c.out[1].p), c.out[1].stride, c.grad, st);
   }, false);
 }
 
@@ -969,7 +977,9 @@ static int check_ids(pnb_engine *e, const int *ids, int n, int n_max) {
 // The stride refusal of each of the arrays: a row of F hops fits in its stride.
 static int check_strides(const Rows (&a)[2], int F) {
   for (const Rows &r : a)
-    if (r.width && r.stride < r.values(F)) return fail(PNB_ERR_ARG, "%s smaller than n_frames*%zu", r.name, r.width);
+    if (r.width && r.stride < r.values(F))
+      return r.per_row ? fail(PNB_ERR_ARG, "%s smaller than %zu", r.name, r.width)
+                       : fail(PNB_ERR_ARG, "%s smaller than n_frames*%zu", r.name, r.width);
   return PNB_OK;
 }
 
@@ -1058,11 +1068,13 @@ static int check_call(pnb_engine *e, Call &c) {
   if (c.kind == Call::kNetwork && c.format != PNB_RNN_FEATURES && c.format != PNB_RNN_RECORDS)
     return fail(PNB_ERR_ARG, "format %d is neither PNB_RNN_FEATURES (0) nor PNB_RNN_RECORDS (1)", c.format);
   if ((c.kind == Call::kSlots || network || split) && !c.pool && e->sessions) return refuse_in_session_mode();
-  const int fr_lo = c.kind == Call::kTrain ? 1 : 0;  // a window of a gradient call has at least one hop
+  // a window of a gradient call or a training forward has at least one hop
+  const int fr_lo = c.kind == Call::kTrain || c.kind == Call::kTrainForward ? 1 : 0;
   if (c.frames)  // every row's counted hops in [fr_lo, F]
     for (int i = 0; i < e->n_active; i++)
       if (c.frames[i] < fr_lo || c.frames[i] > c.F)
-        return fail(PNB_ERR_ARG, "frames[%d] = %d outside [%d, %d]", i, c.frames[i], fr_lo, c.F);
+        return fail(PNB_ERR_ARG, "%s[%d] = %d outside [%d, %d]", c.kind == Call::kTrainForward ? "lengths" : "frames", i,
+                    c.frames[i], fr_lo, c.F);
   return PNB_OK;
 }
 
@@ -1351,21 +1363,48 @@ extern "C" int pnb_train_grad_host(pnb_engine *e, const float *rec, size_t rec_s
   return host_call(e, train_call(rec, rec_stride, n_frames, frames, sums), false);
 }
 
-// The trainer's forward and backward on the caller's tensors (PNB_TRAIN_NETWORK): features in, g/r out; dL/d(out) in,
-// dL/dx (when asked for) and the gradient (when asked for) out.
-extern "C" int pnb_train_forward_device(pnb_engine *e, const float *d_x, size_t x_stride, int n_frames,
-                                        const float *d_weights, float *d_out, size_t out_stride, void *cuda_stream) {
-  Call c{Call::kTrainForward, {rows(d_x, x_stride, kFeat, sizeof(float), "x_stride")},
-         {rows(d_out, out_stride, 68, sizeof(float), "out_stride")}, n_frames};
+// The trainer's forward and backward on the caller's tensors (PNB_TRAIN_NETWORK): features, and the state in and
+// lengths when given, in; g/r, and the state out when asked for, out.  dL/d(out), and dL/d(state out) when given, in;
+// dL/dx, dL/d(state in) and the gradient, each when asked for, out.  The calls without state are the calls with every
+// state array and lengths NULL.
+static Rows state_rows(const float *p, size_t stride, const char *name) {
+  return p ? rows(p, stride, PNB_TRAIN_STATE_FLOATS, sizeof(float), name, true) : Rows{};
+}
+extern "C" int pnb_train_forward_state_device(pnb_engine *e, const float *d_x, size_t x_stride, int n_frames,
+                                              const int *lengths, const float *d_weights, const float *d_state_in,
+                                              size_t state_in_stride, float *d_out, size_t out_stride,
+                                              float *d_state_out, size_t state_out_stride, void *cuda_stream) {
+  Call c{Call::kTrainForward,
+         {rows(d_x, x_stride, kFeat, sizeof(float), "x_stride"), state_rows(d_state_in, state_in_stride, "state_in_stride")},
+         {rows(d_out, out_stride, 68, sizeof(float), "out_stride"),
+          state_rows(d_state_out, state_out_stride, "state_out_stride")},
+         n_frames};
   c.weights = d_weights;
+  c.frames = lengths;
   return device_call(e, c, (cudaStream_t)cuda_stream);
 }
-extern "C" int pnb_train_backward_device(pnb_engine *e, const float *d_dout, size_t dout_stride, float *d_dx,
-                                         size_t dx_stride, float *d_grad, void *cuda_stream) {
-  Call c{Call::kTrainBackward, {rows(d_dout, dout_stride, 68, sizeof(float), "dout_stride")}, {}, 0};
+extern "C" int pnb_train_backward_state_device(pnb_engine *e, const float *d_dout, size_t dout_stride,
+                                               const float *d_dstate_out, size_t dstate_out_stride, float *d_dx,
+                                               size_t dx_stride, float *d_dstate_in, size_t dstate_in_stride,
+                                               float *d_grad, void *cuda_stream) {
+  Call c{Call::kTrainBackward,
+         {rows(d_dout, dout_stride, 68, sizeof(float), "dout_stride"),
+          state_rows(d_dstate_out, dstate_out_stride, "dstate_out_stride")},
+         {Rows{}, state_rows(d_dstate_in, dstate_in_stride, "dstate_in_stride")},
+         0};
   if (d_dx) c.out[0] = rows(d_dx, dx_stride, kFeat, sizeof(float), "dx_stride");
   c.grad = d_grad;
   return device_call(e, c, (cudaStream_t)cuda_stream);
+}
+extern "C" int pnb_train_forward_device(pnb_engine *e, const float *d_x, size_t x_stride, int n_frames,
+                                        const float *d_weights, float *d_out, size_t out_stride, void *cuda_stream) {
+  return pnb_train_forward_state_device(e, d_x, x_stride, n_frames, nullptr, d_weights, nullptr, 0, d_out, out_stride,
+                                        nullptr, 0, cuda_stream);
+}
+extern "C" int pnb_train_backward_device(pnb_engine *e, const float *d_dout, size_t dout_stride, float *d_dx,
+                                         size_t dx_stride, float *d_grad, void *cuda_stream) {
+  return pnb_train_backward_state_device(e, d_dout, dout_stride, nullptr, 0, d_dx, dx_stride, nullptr, 0, d_grad,
+                                         cuda_stream);
 }
 
 // The refusals every training entry point shares: an engine of its kind that no failed call has poisoned.

@@ -192,16 +192,21 @@ int train_grad(pnb_engine *e, const float *rec, size_t rec_stride, const int *fr
                int F, cudaStream_t st);
 int train_grad_launches(const pnb_engine *e);
 // forward: the caller's network input x (rows of F x 70 floats, not scaled) of windows [0, n_active) through the
-// network, weights (device, blob order, or null) copied into the parameters first, the predictions out to the caller's
-// rows (F x 68); the activations are kept for one backward.  backward: from the caller's dL/d(out) rows (F x 68) of the
-// last forward, the held gradient (copied to grad, device, when not null) and, when dx is not null, dL/dx to the
-// caller's rows (F x 70).  Their launch counts depend on nothing but whether dx is asked for.
-int train_forward(pnb_engine *e, const float *x, size_t x_stride, const float *weights, float *out, size_t out_stride,
-                  int F, cudaStream_t st);
-int train_backward(pnb_engine *e, const float *dout, size_t dout_stride, float *dx, size_t dx_stride, float *grad,
-                   cudaStream_t st);
-int train_forward_launches(const pnb_engine *e);
-int train_backward_launches(const pnb_engine *e, bool dx);
+// network from the state rows state_in (PNB_TRAIN_STATE_FLOATS each, or null: zero state), weights (device, blob order,
+// or null) copied into the parameters first, the predictions out to the caller's rows (F x 68) and the state at each
+// window's end to state_out (or null); lengths (device, h_lengths its host copy, or null: F): each window's hops.  The
+// activations are kept for one backward.  backward: from the caller's dL/d(out) rows (F x 68) and dL/d(state out) rows
+// (or null) of the last forward, the held gradient (copied to grad, device, when not null) and, when not null, dL/dx to
+// the caller's rows (F x 70) and dL/d(state in) to its state rows.  Their launch counts depend on nothing but which of
+// the optional arrays are given.
+int train_forward(pnb_engine *e, const float *x, size_t x_stride, const float *weights, const float *state_in,
+                  size_t state_in_stride, const int *lengths, const int *h_lengths, float *out, size_t out_stride,
+                  float *state_out, size_t state_out_stride, int F, cudaStream_t st);
+int train_backward(pnb_engine *e, const float *dout, size_t dout_stride, const float *dstate_out,
+                   size_t dstate_out_stride, float *dx, size_t dx_stride, float *dstate_in, size_t dstate_in_stride,
+                   float *grad, cudaStream_t st);
+int train_forward_launches(const pnb_engine *e, bool state_in, bool lengths, bool state_out);
+int train_backward_launches(const pnb_engine *e, bool dx, bool dstate_out, bool dstate_in);
 int train_adam(pnb_engine *e, double lr, long long step, cudaStream_t st);
 int train_copy(pnb_engine *e, int what, void *host, bool to_host, cudaStream_t st);
 size_t train_params(const pnb_engine *e);

@@ -19,6 +19,9 @@
 // caller's loss (pnb_train_backward_device) seeds the output pre-activations from the caller's dL/d(out)
 // (train_seed_kernel), runs the backward half, and adds dL/dx = dA_fc W_fc^T when asked.  Its check skips the next
 // Adam step on a non-finite gradient but raises no domain bit: the caller owns that loss, as torch's autograd does.
+// Both may carry network state (pnb_train_state.h): the forward starts from the caller's state rows and gathers each
+// window's state at its end (train_state_kernel), over per-window lengths; the backward takes dL/d(state out) as seeds
+// and gives dL/d(state in).
 // Between gradient calls and Adam, pnb_train_accumulate / pnb_train_finish sum several calls' gradients (micro-batches,
 // or ranks through an exported accumulator) in float64, weighted by their counted hops (train_accum_kernel,
 // train_finish_kernel), and the check runs again on the sum.
@@ -174,6 +177,12 @@ struct RecArgs {
   float *carry;             // [n][H]: dh * z of the hop after, per unit
   const int *frames;        // [n] hops per window (device), or null: F
   unsigned *cnt;            // hops finished x CTAs, zero at launch
+  // backward, each or null: dL/d(state out) of this layer (row b at seed + b * seed_stride), added to dh at each window's
+  // last hop; dL/d(state in) (row b at dh0 + b * dh0_stride), one more step after hop 0
+  const float *seed;
+  size_t seed_stride;
+  float *dh0;
+  size_t dh0_stride;
 };
 
 __device__ __forceinline__ float sigm(float x) { return 1.f / (1.f + expf(-x)); }
@@ -276,6 +285,7 @@ __global__ void __launch_bounds__(256) gru_bwd_rec_kernel(const __grid_constant_
         }
         float dh = a.dh_ext[row * H + j];
         if (rec) dh += acc[ju] + *cr;
+        else if (a.seed) dh += a.seed[(size_t)b * a.seed_stride + j];  // t = fr - 1: the state the window ends in
         const float z = a.z[row * H + j], r = a.r[row * H + j], nv = a.nn[row * H + j], hn = a.hn[row * H + j];
         const float hp = a.h[row * H + j];  // slot t: the state before hop t
         const float dan = dh * (1.f - z) * (1.f - nv * nv);
@@ -292,15 +302,37 @@ __global__ void __launch_bounds__(256) gru_bwd_rec_kernel(const __grid_constant_
       red_release_gpu_add(a.cnt, 1u);
     }
   }
+  if (!a.dh0) return;
+  // the state before hop 0: dh0 = dgh(0) U^T + dh(0) z(0), summed as the loop's carry is (hop 0 counts in every window)
+  if (tid == 0) chain_wait(a.cnt, (unsigned)a.F * G);
+  __syncthreads();
+  for (int b = warp; b < n; b += blockDim.x >> 5) {
+    float acc[JU];
+#pragma unroll
+    for (int ju = 0; ju < JU; ju++) acc[ju] = 0.f;
+    const float *gp = a.dgh + (size_t)b * H3;
+    for (int c = lane; c < H3; c += 32) {
+      const float d = __ldcg(gp + c);
+#pragma unroll
+      for (int ju = 0; ju < JU; ju++) acc[ju] = fmaf(d, Ur[ju * H3 + c], acc[ju]);
+    }
+#pragma unroll
+    for (int ju = 0; ju < JU; ju++)
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) acc[ju] += __shfl_xor_sync(0xffffffffu, acc[ju], o);
+#pragma unroll
+    for (int ju = 0; ju < JU; ju++)
+      if (lane == ju) a.dh0[(size_t)b * a.dh0_stride + j0 + ju] = acc[ju] + a.carry[(size_t)b * H + j0 + ju];
+  }
 }
 
 // ---------------------------------------------------------------------------------------------------- elementwise
-// x [F][n][70]: the hops t >= frames[b] of window b become zeros, so that nothing past a window's end (NaN included)
-// reaches any activation the gradient multiplies
-__global__ void train_mask_kernel(float *__restrict__ x, const int *__restrict__ frames, int n, int F) {
-  const size_t total = (size_t)F * n * kFeat;
+// x [F][n][w]: the hops t >= frames[b] of window b become zeros, so that nothing past a window's end (NaN included)
+// reaches any activation the gradient multiplies (w = 70, the network input), or the caller's output rows (w = 68)
+__global__ void train_mask_kernel(float *__restrict__ x, int w, const int *__restrict__ frames, int n, int F) {
+  const size_t total = (size_t)F * n * w;
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
-    const size_t row = i / kFeat;
+    const size_t row = i / w;
     const int b = (int)(row % n), t = (int)(row / n);
     if (frames && t >= frames[b]) x[i] = 0.f;
   }
@@ -334,16 +366,66 @@ __global__ void train_dpre_kernel(const float *__restrict__ pred, const float *_
 
 // The backward's entry point when the caller supplies dL/d(out): dout [n][F][68] rows of dout_stride floats (window-major,
 // as the caller's tensors) -> d [F][n][68] (hop-major, r = t*n + b), d = dout (1 - p) p left to right, ATen's
-// sigmoid_backward, so the seed is the same bits torch's autograd passes into the output layers.
-__global__ void train_seed_kernel(const float *__restrict__ dout, size_t dout_stride, const float *__restrict__ pred, int n,
-                                  int F, float *__restrict__ d) {
+// sigmoid_backward, so the seed is the same bits torch's autograd passes into the output layers.  Hops past a window's
+// end (frames, or null: none) get zeros whatever dout holds there.
+__global__ void train_seed_kernel(const float *__restrict__ dout, size_t dout_stride, const float *__restrict__ pred,
+                                  const int *__restrict__ frames, int n, int F, float *__restrict__ d) {
   const size_t total = (size_t)F * n * 68;
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
     const int k = (int)(i % 68);
     const size_t row = i / 68;
     const int b = (int)(row % n), t = (int)(row / n);
+    if (frames && t >= frames[b]) { d[i] = 0.f; continue; }
     const float p = pred[i];
     d[i] = __fmul_rn(__fmul_rn(dout[(size_t)b * dout_stride + (size_t)t * 68 + k], __fsub_rn(1.f, p)), p);
+  }
+}
+
+// The network state of a window, PNB_TRAIN_STATE_FLOATS floats: [fc_hist 4 x 128][c1_hist 2 x 512][gru1, gru2, gru3,
+// gru_gb 512 each][gru_rb 128], histories oldest first (StreamState's fc_hist, c1_hist, h).  For a window that has run L
+// hops, value i of window b is fc slot L + k, c1 slot L + k or GRU slot L of the trainer's buffers: the state in is
+// L = 0 (the slots before hop 0), the state out L = the window's hops.
+struct StateBufs {
+  float *fc, *c1, *h[5];
+  int n;
+};
+__device__ __forceinline__ float *state_slot(const StateBufs &s, int b, int i, int L) {
+  const size_t n = s.n;
+  if (i < 512) return s.fc + ((L + i / 128) * n + b) * 128 + i % 128;
+  if (i < 1536) return s.c1 + ((L + (i - 512) / 512) * n + b) * 512 + (i - 512) % 512;
+  const int l = (i - 1536) / 512;
+  return s.h[l] + ((size_t)L * n + b) * (l < 4 ? 512 : 128) + (i - 1536) % 512;
+}
+
+// out false: the caller's state rows (row b at st + b * stride) into the slots before hop 0; out true: the slots at each
+// window's end (frames[b], or null: F) out to the rows
+__global__ void train_state_kernel(const StateBufs s, float *st, size_t stride, const int *__restrict__ frames, int F,
+                                   bool out) {
+  const size_t total = (size_t)s.n * PNB_TRAIN_STATE_FLOATS;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+    const int b = (int)(i / PNB_TRAIN_STATE_FLOATS), k = (int)(i % PNB_TRAIN_STATE_FLOATS);
+    float *row = st + (size_t)b * stride + k;
+    if (out) *row = *state_slot(s, b, k, frames ? frames[b] : F);
+    else *state_slot(s, b, k, 0) = *row;
+  }
+}
+
+// dL/d(state out) of the conv histories (row b at ds + b * ds_stride), L = frames[b] (or F): fc_hist[k] is the fc
+// output of hop L - 4 + k and c1_hist[k] conv1's of hop L - 2 + k, so its seed goes to that hop's row of dfc [F][n][128]
+// or dc1 [F][n][512] (zero elsewhere; their contractions add them before the ReLU derivative).  A slot before hop 0
+// (L < 4, L < 2) is state in slot L + k passed through, and dsi (dL/d(state in), or null) starts from those seeds:
+// every history value of it is written, zero where none passes through.
+__global__ void train_hist_seed_kernel(const float *__restrict__ ds, size_t ds_stride, float *__restrict__ dsi,
+                                       size_t dsi_stride, const int *__restrict__ frames, int n, int F,
+                                       float *__restrict__ dfc, float *__restrict__ dc1) {
+  const size_t total = (size_t)n * 1536;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+    const int b = (int)(i / 1536), k = (int)(i % 1536), L = frames ? frames[b] : F;
+    const bool fc = k < 512;
+    const int W = fc ? 128 : 512, D = fc ? 4 : 2, kk = fc ? k : k - 512, slot = kk / W, c = kk % W, t = L - D + slot;
+    const float *row = ds + (size_t)b * ds_stride;
+    if (t >= 0) (fc ? dfc : dc1)[((size_t)t * n + b) * W + c] = row[k];
+    if (dsi) dsi[(size_t)b * dsi_stride + k] = slot >= L ? row[k - L * W] : 0.f;
   }
 }
 
@@ -462,8 +544,11 @@ struct pnb_train_state {
   float *ea = nullptr, *eb = nullptr;      // [F+4][n][512]: layer gradients, trailing zero slots for the conv backward
   float *dc2 = nullptr;                    // [F+2][n][512]
   float *carry = nullptr;                  // [S][512]
+  int *lens = nullptr;                     // [S] the last train_forward's hops per window, when it had lengths
   int G512 = 0, G128 = 0;                  // CTAs of the recurrences (a power of two, co-resident)
   int last_F = 0, last_n = 0;              // hops and rows of the last gradient call (0: none yet), for train_tap
+  const int *fwd_frames = nullptr;         // the last train_forward's per-window hops (lens), or null: all F
+  long long fwd_hops = 0;                  // and the hops they count
 };
 
 constexpr size_t kPartFloats = (size_t)1 << 21;
@@ -545,6 +630,7 @@ int train_prepare(pnb_engine *e) {
   TCK(engine_alloc(e, &s.eb, (F + 4) * S * 512, kScratch));
   TCK(engine_alloc(e, &s.dc2, (F + 2) * S * 512, kScratch));
   TCK(engine_alloc(e, &s.carry, S * 512, kScratch));
+  TCK(engine_alloc(e, &s.lens, S, kScratch));
   s.G512 = rec_grid(e, 512);
   s.G128 = rec_grid(e, 128);
   if (!s.G512 || !s.G128) return engine_fail(PNB_ERR_CUDA, "cannot configure the training recurrence kernels");
@@ -634,21 +720,38 @@ RecArgs rec_args(const pnb_train_state &s, int l, int n, int F, const int *frame
 }
 // GRU l's output at hop t: slot t+1 of its states
 float *out_of(const pnb_train_state &s, int l, int n) { return s.h[l] + (size_t)n * kGruH[l]; }
+StateBufs state_bufs(const pnb_train_state &s, int n) {
+  StateBufs b;
+  b.fc = s.fc; b.c1 = s.c1; b.n = n;
+  for (int l = 0; l < 5; l++) b.h[l] = s.h[l];
+  return b;
+}
+// where GRU l's state starts in a state row
+constexpr size_t state_gru(int l) { return 1536 + 512 * (size_t)l; }
 }  // namespace
 
-// The forward half on the network input staged in s.x ([F][n][70]): fc, conv1, conv2, the five GRUs with everything
-// their backward needs saved, fc_gb and fc_rb into s.pred.  15 launches.
-static int forward_half(pnb_engine *e, Launcher &L, const int *frames, int F) {
+// The forward half on the network input staged in s.x ([F][n][70]) from the caller's state (state_in, rows of
+// state_in_stride floats) or, with state_in null, from zero state: fc, conv1, conv2, the five GRUs with everything their
+// backward needs saved, fc_gb and fc_rb into s.pred.  15 launches, 16 with a state in.
+static int forward_half(pnb_engine *e, Launcher &L, const int *frames, int F, const float *state_in,
+                        size_t state_in_stride) {
   pnb_train_state &s = *e->train;
   const int n = e->n_active, R = F * n;
   const size_t nb = (size_t)n;
   const cudaStream_t st = L.st;
   float *const *P = s.param;
-  // per call: the forward counters and the zero slots (the row stride n changes from call to call)
+  // per call: the forward counters and the slots before hop 0 (the row stride n changes from call to call)
   TCK(cudaMemsetAsync(s.cnt, 0, 5 * sizeof(unsigned), st));
-  TCK(cudaMemsetAsync(s.fc, 0, 4 * nb * 128 * sizeof(float), st));
-  TCK(cudaMemsetAsync(s.c1, 0, 2 * nb * 512 * sizeof(float), st));
-  for (int l = 0; l < 5; l++) TCK(cudaMemsetAsync(s.h[l], 0, nb * kGruH[l] * sizeof(float), st));
+  if (state_in) {
+    LaunchScope m(e, kUnprofiled, st);
+    train_state_kernel<<<blocks_for(nb * PNB_TRAIN_STATE_FLOATS), 256, 0, st>>>(
+        state_bufs(s, n), const_cast<float *>(state_in), state_in_stride, nullptr, 0, false);
+  } else {
+    TCK(cudaMemsetAsync(s.fc, 0, 4 * nb * 128 * sizeof(float), st));
+    TCK(cudaMemsetAsync(s.c1, 0, 2 * nb * 512 * sizeof(float), st));
+    for (int l = 0; l < 5; l++) TCK(cudaMemsetAsync(s.h[l], 0, nb * kGruH[l] * sizeof(float), st));
+  }
+  L.check();
   float *fc_out = s.fc + 4 * nb * 128, *c1_out = s.c1 + 2 * nb * 512;
   { TSeg a[1] = {tseg(s.x, kFeat, P[0], 128, kFeat)}; L.gemm(false, a, 1, R, 128, fc_out, 128, P[1], kEpiRelu); }
   {
@@ -686,8 +789,12 @@ static int forward_half(pnb_engine *e, Launcher &L, const int *frames, int F) {
 
 // The backward half of the forward half's call, from the gradient at the output pre-activations in s.dpre: output
 // layers, then the GRUs in reverse dependency order, conv2, conv1, fc.  Weight gradients go straight into the flat
-// gradient at their blob offsets; fc's pre-activation gradient is left in s.eb.  98 launches.
-static int backward_half(pnb_engine *e, Launcher &L, const int *frames, int F) {
+// gradient at their blob offsets; fc's pre-activation gradient is left in s.eb.  dstate_out (or null): dL/d(state out)
+// rows, which seed the GRUs' last hops and the histories' hops; dstate_in (or null): dL/d(state in) rows, written.
+// 98 launches, + 1 with dstate_out (the history seeds), + 6 with dstate_in (the history gradients, one contraction per
+// history slot).
+static int backward_half(pnb_engine *e, Launcher &L, const int *frames, int F, const float *dstate_out,
+                         size_t dstate_out_stride, float *dstate_in, size_t dstate_in_stride) {
   pnb_train_state &s = *e->train;
   const int n = e->n_active, R = F * n;
   const size_t nb = (size_t)n;
@@ -711,6 +818,8 @@ static int backward_half(pnb_engine *e, Launcher &L, const int *frames, int F) {
     RecArgs a = rec_args(s, l, n, F, frames);
     a.dh_ext = ext;
     a.cnt = s.cnt + 5 + l;
+    if (dstate_out) { a.seed = dstate_out + state_gru(l); a.seed_stride = dstate_out_stride; }
+    if (dstate_in) { a.dh0 = dstate_in + state_gru(l); a.dh0_stride = dstate_in_stride; }
     L.rec(a, false);
     L.wgrad(X0, 512, 512, s.g1, H3, H3, R, G + O[6 + 3 * l]);
     if (X1) L.wgrad(X1, 512, 512, s.g1, H3, H3, R, G + O[6 + 3 * l] + (size_t)512 * H3);
@@ -748,17 +857,37 @@ static int backward_half(pnb_engine *e, Launcher &L, const int *frames, int F) {
   { TSeg a[1] = {tseg(s.g1, 1536, P[6], 1536, 1536)}; L.gemm(true, a, 1, R, 512, s.dc2, 512, nullptr, kEpiDTanh, true, s.c2p, 512); }
   for (int q = 0; q < 3; q++) L.wgrad(s.c1 + q * nb * 512, 512, 512, s.dc2, 512, 512, R, G + O[4] + (size_t)q * 512 * 512);
   L.wgrad(nullptr, 0, 1, s.dc2, 512, 512, R, G + O[5]);
+  const bool seeded = dstate_out != nullptr;  // the conv1 / fc output gradients below add the history seeds
+  if (seeded) {
+    TCK(cudaMemsetAsync(s.ea, 0, (size_t)R * 512 * sizeof(float), st));
+    TCK(cudaMemsetAsync(s.eb, 0, (size_t)R * 128 * sizeof(float), st));
+    LaunchScope m(e, kUnprofiled, st);
+    train_hist_seed_kernel<<<blocks_for(nb * 1536), 256, 0, st>>>(dstate_out, dstate_out_stride, dstate_in,
+                                                                  dstate_in_stride, frames, n, F, s.eb, s.ea);
+  }
   {  // conv1 output gradient: hop t gets tap q of hop t + 2 - q (the trailing zero slots end the sum)
     TSeg a[3];
     for (int q = 0; q < 3; q++) a[q] = tseg(s.dc2 + (2 - q) * nb * 512, 512, P[4] + (size_t)q * 512 * 512, 512, 512);
-    L.gemm(true, a, 3, R, 512, s.ea, 512, nullptr, kEpiDRelu, false, c1_out, 512);
+    L.gemm(true, a, 3, R, 512, s.ea, 512, nullptr, kEpiDRelu, seeded, c1_out, 512);
   }
   for (int q = 0; q < 5; q++) L.wgrad(s.fc + q * nb * 128, 128, 128, s.ea, 512, 512, R, G + O[2] + (size_t)q * 128 * 512);
   L.wgrad(nullptr, 0, 1, s.ea, 512, 512, R, G + O[3]);
   {
     TSeg a[5];
     for (int q = 0; q < 5; q++) a[q] = tseg(s.ea + (4 - q) * nb * 512, 512, P[2] + (size_t)q * 128 * 512, 512, 512);
-    L.gemm(true, a, 5, R, 128, s.eb, 128, nullptr, kEpiDRelu, false, fc_out, 128);
+    L.gemm(true, a, 5, R, 128, s.eb, 128, nullptr, kEpiDRelu, seeded, fc_out, 128);
+  }
+  if (dstate_in) {  // history slot k (hop k - D) is conv tap q of hop k - q: the input gradients extended before hop 0
+    for (int k = 0; k < 2; k++) {
+      TSeg a[2];
+      for (int q = 0; q <= k; q++) a[q] = tseg(s.dc2 + (k - q) * nb * 512, 512, P[4] + (size_t)q * 512 * 512, 512, 512);
+      L.gemm(true, a, k + 1, n, 512, dstate_in + 512 + 512 * k, dstate_in_stride, nullptr, kEpiNone, seeded);
+    }
+    for (int k = 0; k < 4; k++) {
+      TSeg a[4];
+      for (int q = 0; q <= k; q++) a[q] = tseg(s.ea + (k - q) * nb * 512, 512, P[2] + (size_t)q * 128 * 512, 512, 512);
+      L.gemm(true, a, k + 1, n, 128, dstate_in + 128 * k, dstate_in_stride, nullptr, kEpiNone, seeded);
+    }
   }
   L.wgrad(s.x, kFeat, kFeat, s.eb, 128, 128, R, G + O[0]);
   L.wgrad(nullptr, 0, 1, s.eb, 128, 128, R, G + O[1]);
@@ -784,9 +913,9 @@ int train_grad(pnb_engine *e, const float *rec, size_t rec_stride, const int *fr
   Launcher L{e, st};
   // ---- stage: {30 rec[0..67], rec[68], rec[69]}, zero past each window's end
   { LaunchScope m(e, kUnprofiled, st); launch_rows_stage(s.x, kFeat, rec, rec_stride, PNB_RECORD_FLOATS, 68, n, n, F, st); }
-  { LaunchScope m(e, kUnprofiled, st); train_mask_kernel<<<blocks_for((size_t)R * kFeat), 256, 0, st>>>(s.x, frames, n, F); }
+  { LaunchScope m(e, kUnprofiled, st); train_mask_kernel<<<blocks_for((size_t)R * kFeat), 256, 0, st>>>(s.x, kFeat, frames, n, F); }
   L.check();
-  if (int rc = forward_half(e, L, frames, F)) return rc;
+  if (int rc = forward_half(e, L, frames, F, nullptr, 0)) return rc;
 
   // ---- loss and its gradient at the output pre-activations
   { LaunchScope m(e, kUnprofiled, st); launch_loss_sums(s.pred, rec, rec_stride, frames, sums, n, n, F, st); }
@@ -799,7 +928,7 @@ int train_grad(pnb_engine *e, const float *rec, size_t rec_stride, const int *fr
   }
   L.check();
 
-  if (int rc = backward_half(e, L, frames, F)) return rc;
+  if (int rc = backward_half(e, L, frames, F, nullptr, 0, nullptr, 0)) return rc;
   if (int rc = check_grad(e, L, e->d_status)) return rc;
   TCK(L.err);
   // pnb_launches_per_call reports train_grad_launches: the schedule above and that count must agree
@@ -811,12 +940,16 @@ int train_grad(pnb_engine *e, const float *rec, size_t rec_stride, const int *fr
   return PNB_OK;
 }
 
-// A forward of the caller's network input (70 features per hop, not scaled) on windows [0, n_active), each from zero
-// state; weights (or null) first replace the parameters, and the predictions go to the caller's rows.
-int train_forward(pnb_engine *e, const float *x, size_t x_stride, const float *weights, float *out, size_t out_stride,
-                  int F, cudaStream_t st) {
+// A forward of the caller's network input (70 features per hop, not scaled) on windows [0, n_active), each from the
+// caller's state rows (state_in) or from zero state; weights (or null) first replace the parameters, and the predictions
+// go to the caller's rows.  lengths (device, with h_lengths its host copy; or null): the hops of each window, whose
+// later input is zeroed and whose later output rows are zeros; the state at each window's end goes to state_out (or
+// nowhere).
+int train_forward(pnb_engine *e, const float *x, size_t x_stride, const float *weights, const float *state_in,
+                  size_t state_in_stride, const int *lengths, const int *h_lengths, float *out, size_t out_stride,
+                  float *state_out, size_t state_out_stride, int F, cudaStream_t st) {
   pnb_train_state &s = *e->train;
-  const int n = e->n_active;
+  const int n = e->n_active, R = F * n;
   const long long launches0 = e->launches;
   Launcher L{e, st};
   if (weights)
@@ -824,33 +957,57 @@ int train_forward(pnb_engine *e, const float *x, size_t x_stride, const float *w
       TCK(cudaMemcpyAsync(s.param[i], weights + s.off[i], (s.off[i + 1] - s.off[i]) * sizeof(float),
                           cudaMemcpyDeviceToDevice, st));
   { LaunchScope m(e, kUnprofiled, st); launch_rows_stage(s.x, kFeat, x, x_stride, kFeat, 0, n, n, F, st); }
+  const int *frames = nullptr;  // kept on the trainer for the backward: the staging lengths came through is reused
+  if (lengths) {
+    TCK(cudaMemcpyAsync(s.lens, lengths, (size_t)n * sizeof(int), cudaMemcpyDeviceToDevice, st));
+    frames = s.lens;
+    LaunchScope m(e, kUnprofiled, st);
+    train_mask_kernel<<<blocks_for((size_t)R * kFeat), 256, 0, st>>>(s.x, kFeat, frames, n, F);
+  }
   L.check();
-  if (int rc = forward_half(e, L, nullptr, F)) return rc;
+  if (int rc = forward_half(e, L, frames, F, state_in, state_in_stride)) return rc;
+  if (frames) {
+    LaunchScope m(e, kUnprofiled, st);
+    train_mask_kernel<<<blocks_for((size_t)R * 68), 256, 0, st>>>(s.pred, 68, frames, n, F);
+  }
   { LaunchScope m(e, kUnprofiled, st); launch_rows_store(s.pred, 68, out, out_stride, n, n, F, st); }
+  if (state_out) {
+    LaunchScope m(e, kUnprofiled, st);
+    train_state_kernel<<<blocks_for((size_t)n * PNB_TRAIN_STATE_FLOATS), 256, 0, st>>>(state_bufs(s, n), state_out,
+                                                                                       state_out_stride, frames, F, true);
+  }
   L.check();
   TCK(L.err);
-  if (e->launches - launches0 != train_forward_launches(e))
+  if (e->launches - launches0 != train_forward_launches(e, state_in, lengths, state_out))
     return engine_fail(PNB_ERR_CUDA, "train_forward issued a launch count train_forward_launches does not know");
   s.last_F = F;
   s.last_n = n;
+  s.fwd_frames = frames;
+  s.fwd_hops = (long long)n * F;
+  if (h_lengths) {
+    s.fwd_hops = 0;
+    for (int i = 0; i < n; i++) s.fwd_hops += h_lengths[i];
+  }
   return PNB_OK;
 }
 
-// The backward of the last train_forward from the caller's gradient at its output: the seed, the backward half, and the
-// input gradient when asked for; the gradient becomes the held one (its check skips the next Adam step, but raises no
-// domain bit: the caller owns the loss) and, when asked for, is copied out in blob order.
-int train_backward(pnb_engine *e, const float *dout, size_t dout_stride, float *dx, size_t dx_stride, float *grad,
-                   cudaStream_t st) {
+// The backward of the last train_forward from the caller's gradient at its output (and at its state out, when not null):
+// the seed, the backward half, and the input and state-in gradients when asked for; the gradient becomes the held one
+// (its check skips the next Adam step, but raises no domain bit: the caller owns the loss) and, when asked for, is
+// copied out in blob order.
+int train_backward(pnb_engine *e, const float *dout, size_t dout_stride, const float *dstate_out,
+                   size_t dstate_out_stride, float *dx, size_t dx_stride, float *dstate_in, size_t dstate_in_stride,
+                   float *grad, cudaStream_t st) {
   pnb_train_state &s = *e->train;
   const int n = s.last_n, F = s.last_F, R = F * n;
   const long long launches0 = e->launches;
   Launcher L{e, st};
   {
     LaunchScope m(e, kUnprofiled, st);
-    train_seed_kernel<<<blocks_for((size_t)R * 68), 256, 0, st>>>(dout, dout_stride, s.pred, n, F, s.dpre);
+    train_seed_kernel<<<blocks_for((size_t)R * 68), 256, 0, st>>>(dout, dout_stride, s.pred, s.fwd_frames, n, F, s.dpre);
   }
   L.check();
-  if (int rc = backward_half(e, L, nullptr, F)) return rc;
+  if (int rc = backward_half(e, L, s.fwd_frames, F, dstate_out, dstate_out_stride, dstate_in, dstate_in_stride)) return rc;
   if (dx) {  // dL/dx = dA_fc W_fc^T, then out to the caller's rows
     TSeg a[1] = {tseg(s.eb, 128, s.param[0], 128, 128)};
     L.gemm(true, a, 1, R, kFeat, s.g1, kFeat);
@@ -860,9 +1017,9 @@ int train_backward(pnb_engine *e, const float *dout, size_t dout_stride, float *
   if (int rc = check_grad(e, L, nullptr)) return rc;
   if (grad) TCK(cudaMemcpyAsync(grad, s.grad, s.off[kParams] * sizeof(float), cudaMemcpyDeviceToDevice, st));
   TCK(L.err);
-  if (e->launches - launches0 != train_backward_launches(e, dx != nullptr))
+  if (e->launches - launches0 != train_backward_launches(e, dx, dstate_out, dstate_in))
     return engine_fail(PNB_ERR_CUDA, "train_backward issued a launch count train_backward_launches does not know");
-  e->train_hops = (long long)n * F;
+  e->train_hops = s.fwd_hops;
   return PNB_OK;
 }
 
@@ -885,10 +1042,15 @@ int train_tap(const pnb_engine *e, int what, const void **src, size_t *bytes) {
 // backward 99 (fc_rb 5, gru_rb 11 + 2, fc_gb 13, gru_gb 1 + 9 + 1, gru3 and gru2 9 + 1 each, gru1 9, conv2 9, conv1 13,
 // fc 5, check 1).
 int train_grad_launches(const pnb_engine *) { return 118; }
-// train_forward: stage 1, forward 15, store 1.  train_backward: seed 1, backward 98, check 1, and with the input
-// gradient its contraction and store 2.
-int train_forward_launches(const pnb_engine *) { return 17; }
-int train_backward_launches(const pnb_engine *, bool dx) { return dx ? 102 : 100; }
+// train_forward: stage 1, forward 15, store 1; a state in 1 (its scatter), lengths 2 (the masks of the input and the
+// output), a state out 1 (its gather).  train_backward: seed 1, backward 98, check 1, and with the input gradient its
+// contraction and store 2; a state-out gradient 1 (the history seeds), a state-in gradient 6 (the history contractions).
+int train_forward_launches(const pnb_engine *, bool state_in, bool lengths, bool state_out) {
+  return 17 + (state_in ? 1 : 0) + (lengths ? 2 : 0) + (state_out ? 1 : 0);
+}
+int train_backward_launches(const pnb_engine *, bool dx, bool dstate_out, bool dstate_in) {
+  return (dx ? 102 : 100) + (dstate_out ? 1 : 0) + (dstate_in ? 6 : 0);
+}
 
 int train_adam(pnb_engine *e, double lr, long long step, cudaStream_t st) {
   const pnb_train_state &s = *e->train;

@@ -11,17 +11,21 @@
 //   GRUs / output layers (inputs bounded by tanh): fp16 terms, both sides pre-scaled by powers of two
 //   conv1 / conv2 (ReLU inputs, unbounded):        bf16 terms
 //
-// Two kernels, both persistent and warp-specialised, one CTA of three warpgroups per SM:
-//   tc_gemm_kernel   one dense layer over all rows (conv1, conv2, fc_gb, fc_rb run once per call over F*S rows)
+// Three kernels, all persistent and warp-specialised, one CTA of three warpgroups per SM:
+//   conv_pair_kernel conv1 or conv2 over all F hops of a call.  A tile is two neighbouring hops of 128 streams:
+//                    each weight stage feeds both hops, each input hop slot feeds tap j of the first hop and tap
+//                    j - 1 of the second.
+//   tc_gemm_kernel   one 34-wide output layer over all rows (fc_gb, fc_rb run once per call over F*S rows)
 //   gru_chain_kernel the five GRUs of all F hops of a call in ONE launch.  A tile (hop, layer, 128 streams,
 //                    64 hidden units) depends only on tiles of the same 128 streams (layer below at this hop,
 //                    own layer at the previous hop), so the recurrence is a per-(layer, row tile) counter that
 //                    the consumer warps bump (release) and the TMA producer polls (acquire) -- no grid barrier,
 //                    no launch boundary between layers or hops.
 // Warpgroup roles per CTA: warpgroup 0 = TMA producer (one thread: cp.async.bulk.tensor into a ring of stages guarded
-// by full / empty mbarriers; dense layers SWIZZLE_128B boxes of 64 k, the chain SWIZZLE_64B boxes of 32 k),
+// by full / empty mbarriers; output layers SWIZZLE_128B boxes of 64 k, the conv layers and the chain SWIZZLE_64B
+// boxes of 32 k),
 // warpgroups 1 and 2 = consumers: each issues wgmma for 64 of the tile's 128 rows (m64nNk16, fp32 accumulators in
-// registers; the dense layers take both operands from shared memory, the chain loads its activation operand into
+// registers; the conv and output layers take both operands from shared memory, the chain loads its activation operand into
 // registers with ldmatrix once per stage) and runs the epilogue of its rows.  The producer streams the next tile's
 // operands while the consumers finish the current one.
 //
@@ -51,14 +55,17 @@ using namespace pnb;
 namespace {
 
 constexpr int TM = 128;   // streams per CTA tile: two consumer warpgroups of 64 rows
-constexpr int BK = 64;    // k per pipeline stage of the dense layers: 128-byte rows, SWIZZLE_128B
-constexpr int CBK = 32;   // k per pipeline stage of the GRU chain: 64-byte rows, SWIZZLE_64B (five 40 KB stages fit)
+constexpr int BK = 64;    // k per pipeline stage of the output layers: 128-byte rows, SWIZZLE_128B
+constexpr int CBK = 32;   // k per pipeline stage of the conv layers and the GRU chain: 64-byte rows, SWIZZLE_64B
 constexpr int HT = 64;    // hidden units per GRU tile
 constexpr int GRU_BN = 3 * HT;  // weight rows per GRU tile (z|r|n)
 constexpr int kConsumerWGs = 2;
 constexpr int kTcThreads = 128 * (1 + kConsumerWGs);
 constexpr int kPubWarps = 4 * kConsumerWGs;  // warps that bump a GRU tile's completion counter
-constexpr int DENSE_BN = 128;   // output columns per dense (conv) tile
+constexpr int DENSE_BN = 128;   // output columns per conv tile
+// Registers per thread after the producer warpgroup hands its surplus to the consumers (setmaxnreg, in the conv
+// layers and the GRU chain): the launch gives 168 to each of the 384 threads; 128 x (168 - 40) = 256 x (232 - 168).
+constexpr int kProducerRegs = 40, kConsumerRegs = 232;
 constexpr float kActScale = 1024.f;  // fp16 activations are stored x 2^10 (keeps the low term normal)
 // |pre-activation| from which the reference's tansig_approx (vec.h:63) overflows its float->int conversion
 constexpr float kTanhDomain = 8.5e7f;
@@ -225,18 +232,39 @@ __device__ __forceinline__ void store_split_h2(float v0, float v1, __half *hi_p,
   *reinterpret_cast<__half2 *>(hi_p) = h;
   *reinterpret_cast<__half2 *>(lo_p) = __floats2half2_rn(s0 - hf.x, s1 - hf.y);
 }
-// bf16 split of two neighbouring values into `terms` (2 or 3) planes `plane` elements apart
-__device__ __forceinline__ void store_split_b2(float v0, float v1, __nv_bfloat16 *t0_p, size_t plane, int terms) {
-  const __nv_bfloat162 h = __floats2bfloat162_rn(v0, v1);
-  const float2 hf = __bfloat1622float2(h);
-  const float r0 = v0 - hf.x, r1 = v1 - hf.y;
-  const __nv_bfloat162 l = __floats2bfloat162_rn(r0, r1);
-  *reinterpret_cast<__nv_bfloat162 *>(t0_p) = h;
-  *reinterpret_cast<__nv_bfloat162 *>(t0_p + plane) = l;
-  if (terms == 3) {
-    const float2 lf = __bfloat1622float2(l);
-    *reinterpret_cast<__nv_bfloat162 *>(t0_p + 2 * plane) = __floats2bfloat162_rn(r0 - lf.x, r1 - lf.y);
+// The conv layers' splits of four neighbouring values, one 8-byte store per term: fp16 two-term split (x 2^10), the
+// roundings of store_split_h2, and bf16 three-term split into planes `plane` elements apart
+__device__ __forceinline__ uint32_t h2_bits(__half2 h) { return *reinterpret_cast<uint32_t *>(&h); }
+__device__ __forceinline__ uint32_t b2_bits(__nv_bfloat162 h) { return *reinterpret_cast<uint32_t *>(&h); }
+__device__ __forceinline__ void store_split_h4(const float *v, __half *hi_p, __half *lo_p) {
+  uint32_t hi[2], lo[2];
+#pragma unroll
+  for (int i = 0; i < 2; i++) {
+    const float s0 = v[2 * i] * kActScale, s1 = v[2 * i + 1] * kActScale;
+    const __half2 h = __floats2half2_rn(s0, s1);
+    const float2 hf = __half22float2(h);
+    hi[i] = h2_bits(h);
+    lo[i] = h2_bits(__floats2half2_rn(s0 - hf.x, s1 - hf.y));
   }
+  *reinterpret_cast<uint2 *>(hi_p) = make_uint2(hi[0], hi[1]);
+  *reinterpret_cast<uint2 *>(lo_p) = make_uint2(lo[0], lo[1]);
+}
+__device__ __forceinline__ void store_split_b4(const float *v, __nv_bfloat16 *t0_p, size_t plane) {
+  uint32_t t[3][2];
+#pragma unroll
+  for (int i = 0; i < 2; i++) {
+    const float v0 = v[2 * i], v1 = v[2 * i + 1];
+    const __nv_bfloat162 h = __floats2bfloat162_rn(v0, v1);
+    const float2 hf = __bfloat1622float2(h);
+    const float r0 = v0 - hf.x, r1 = v1 - hf.y;
+    const __nv_bfloat162 l = __floats2bfloat162_rn(r0, r1);
+    const float2 lf = __bfloat1622float2(l);
+    t[0][i] = b2_bits(h);
+    t[1][i] = b2_bits(l);
+    t[2][i] = b2_bits(__floats2bfloat162_rn(r0 - lf.x, r1 - lf.y));
+  }
+#pragma unroll
+  for (int k = 0; k < 3; k++) *reinterpret_cast<uint2 *>(t0_p + k * plane) = make_uint2(t[k][0], t[k][1]);
 }
 
 // ------------------------------------------------------------------------------------------ shared kernel pieces
@@ -275,12 +303,6 @@ template <int STAGES, int REGION_BYTES>
 constexpr size_t tc_smem_bytes() {
   return (size_t)REGION_BYTES + 2 * STAGES * 8 + 256 * 4 + 1024;
 }
-template <int BN, int ST2, int ST3>
-constexpr size_t dense_smem_bytes() {
-  constexpr int r2 = ST2 * StageLayout<BN, 2>::kBytes, r3 = ST3 * StageLayout<BN, 3>::kBytes;
-  return tc_smem_bytes<(ST2 > ST3 ? ST2 : ST3), (r2 > r3 ? r2 : r3)>();
-}
-
 // common prologue: barriers and the activation table
 template <int STAGES>
 __device__ __forceinline__ void tc_prologue(const SmemCarve &c, const float *tansig) {
@@ -295,38 +317,19 @@ __device__ __forceinline__ void tc_prologue(const SmemCarve &c, const float *tan
   __syncthreads();
 }
 
-// One k-block of a tile on the MMA side (one consumer warpgroup, its 64 rows): the significant products of the four
-// 16-wide k-steps.  `a_lo` is the descriptor low word of this warpgroup's rows in the stage's first A term, `b_lo` that
-// of the stage's first B term.  Two terms per operand: hi hi, hi lo, lo hi.  Three terms (t0 t1 t2, each 8 bits below
-// the previous): the six products of total order <= 2.
-// The dense layers' ReLU inputs are unbounded, so the K loop runs once per product order, smallest products first
+// The products of one pass over K, as (A term, B term) pairs in issue order.  Two terms per operand: hi hi, hi lo,
+// lo hi.  Three terms (t0 t1 t2, each 8 bits below the previous): the six products of total order <= 2.
+// The conv layers' ReLU inputs are unbounded, so the K loop runs once per product order, smallest products first
 // (three terms: PASS 0 order 2, PASS 1 order 1, PASS 2 t0 t0; two terms: PASS 1, PASS 2).  The tensor core adds
 // into the fp32 accumulator with truncation at the accumulator's magnitude, so correction products added to an already
-// large sum lose exactly the bits they were meant to supply; summed among themselves first, they do not.  (The GRU
-// chain, whose operands are bounded by 1, issues all products of a k-block at once: gru_mma_kblock.)
-template <int BN, int N, bool BF16, int NT, int PASS>
-__device__ __forceinline__ void mma_kblock(float *acc, uint32_t a_lo, uint32_t b_lo) {
-  using SL = StageLayout<BN, NT>;
-  constexpr uint32_t A = SL::kABytes >> 4, B = SL::kBBytes >> 4;
-#pragma unroll
-  for (int ks = 0; ks < BK / 16; ks++) {
-    const uint32_t a = a_lo + ks * 2, b = b_lo + ks * 2;
-    if (NT == 2 && PASS == 1) {
-      wgmma<N, BF16>(acc, desc64(a), desc64(b + B));
-      wgmma<N, BF16>(acc, desc64(a + A), desc64(b));
-    } else if (NT == 2) {
-      wgmma<N, BF16>(acc, desc64(a), desc64(b));
-    } else if (PASS == 0) {
-      wgmma<N, BF16>(acc, desc64(a + A), desc64(b + B));
-      wgmma<N, BF16>(acc, desc64(a), desc64(b + 2 * B));
-      wgmma<N, BF16>(acc, desc64(a + 2 * A), desc64(b));
-    } else if (PASS == 1) {
-      wgmma<N, BF16>(acc, desc64(a), desc64(b + B));
-      wgmma<N, BF16>(acc, desc64(a + A), desc64(b));
-    } else {
-      wgmma<N, BF16>(acc, desc64(a), desc64(b));
-    }
-  }
+// large sum lose exactly the bits they were meant to supply; summed among themselves first, they do not.  The output
+// layers use the same two passes.  (The GRU chain, whose operands are bounded by 1, issues all products of a k-block
+// at once: gru_mma_kblock.)
+template <int PASS, typename F>
+__device__ __forceinline__ void pass_products(F &&mma) {
+  if (PASS == 0) { mma(1, 1); mma(0, 2); mma(2, 0); }
+  else if (PASS == 1) { mma(0, 1); mma(1, 0); }
+  else mma(0, 0);
 }
 
 // Consumer side of one stage: wait for the operands, issue the k-block's MMAs, and free the stage the PREVIOUS k-block
@@ -359,12 +362,12 @@ struct Consumer {
   }
 };
 
-// ------------------------------------------------------------------------------------------ dense layers
+// ------------------------------------------------------------------------------------------ output layers
 struct TcSeg {
   int a_map, b_map;  // indices into TcArgs::maps
   int k_blocks;      // K / BK
   int a_k0, b_k0;    // starting k (elements) in the A / B matrices
-  int a_row0;        // row of the A matrix that holds tile row 0 (hop / tap offset inside a multi-hop buffer)
+  int a_row0;        // row of the A matrix that holds tile row 0 (hop offset inside a multi-hop buffer)
   int a_term_rows;   // row distance between the split terms inside this A buffer
 };
 
@@ -381,42 +384,28 @@ struct TcArgs {
   const float *tansig;  // 201-entry table (global)
   const float *bias;    // padded to a multiple of 16 entries
   int *status;          // engine status word: bit 0 = an activation left the reference's defined domain
-  const int *wide;      // null, or a device word: non-zero = run with three operand terms (six products) instead of two
-  int out_terms;        // bf16 terms written to out_b (2 or 3)
-  int act;
   int N;                // valid output columns
   int ldc;              // row stride of out_f32
-  float *out_f32;       // [M][ldc] or null
-  int f32_row0;         // only rows >= f32_row0 are written to out_f32, at row - f32_row0
-  const int *hops;      // ragged calls (per-slot tiling): [M] hops of each row of a slot, or null.  Row r of hop slot t is
-                        // computed but neither checked nor stored when t >= hops[r]; out_f32 takes row r of slot
-                        // hops[r] - 1, at r
-  __half *out_h;        // fp16 two-term split [2][out_plane_rows][N] (x 2^10) or null
-  __nv_bfloat16 *out_b; // bf16 two-term split [2][out_plane_rows][N] or null
-  int out_row0;         // first row written inside a term plane of out_h / out_b
-  int out_plane_rows;   // rows per term plane of out_h / out_b
+  float *out_f32;       // sigmoid outputs [rows][ldc]
 };
 
-// First row of row tile mt, the end of its hop slot's rows in *lim, and the hop slot in *slot_out
-__device__ __forceinline__ int dense_tile_row0(const TcArgs &args, int mt, int *lim, int *slot_out = nullptr) {
+// First row of row tile mt, the end of its hop slot's rows in *lim
+__device__ __forceinline__ int dense_tile_row0(const TcArgs &args, int mt, int *lim) {
   const int slot = mt / args.tiles_slot;
   *lim = slot * args.slot_stride + args.M;
-  if (slot_out) *slot_out = slot;
   return slot * args.slot_stride + (mt - slot * args.tiles_slot) * TM;
 }
 
 // ===== TMA producer (one thread): the tile's A rows and B rows, one pass over K per product order =====
-template <int BN, int NT, int STAGES>
+template <int BN, int STAGES>
 __device__ __forceinline__ void dense_producer(const TcArgs &args, const SmemCarve &c, uint32_t stage0, int total_tiles) {
-  using SL = StageLayout<BN, NT>;
+  using SL = StageLayout<BN>;
   Pipe p;
   for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
     int lim;
     const int n_tile = tile % args.tiles_n, m0 = dense_tile_row0(args, tile / args.tiles_n, &lim);
-    // one pass over K per product order (see mma_kblock); with q passes still to go after this one, the pass needs
-    // the first q + 1 terms of either operand
-    for (int pass = 0; pass < NT; pass++) {
-      const int nt = NT - pass;
+    // pass 1 (hi lo, lo hi) needs both terms of either operand, pass 2 (hi hi) the first
+    for (int nt = 2; nt > 0; nt--) {
       for (int s = 0; s < args.n_seg; s++) {
         const TcSeg &sg = args.seg[s];
         const CUtensorMap *ma = &args.maps[sg.a_map], *mb = &args.maps[sg.b_map];
@@ -426,12 +415,9 @@ __device__ __forceinline__ void dense_producer(const TcArgs &args, const SmemCar
           const uint32_t fb = c.full + 8 * p.st;
           mbar_expect_tx(fb, nt * (SL::kABytes + SL::kBBytes));
           const uint32_t sp = stage0 + p.st * SL::kBytes;
-#pragma unroll
-          for (int tm = 0; tm < NT; tm++) {
-            if (tm < nt) {
-              tma_load_2d(sp + tm * SL::kABytes, ma, fb, sg.a_k0 + kb * BK, tm * sg.a_term_rows + arow);
-              tma_load_2d(sp + NT * SL::kABytes + tm * SL::kBBytes, mb, fb, sg.b_k0 + kb * BK, tm * args.b_term_rows + brow);
-            }
+          for (int tm = 0; tm < nt; tm++) {
+            tma_load_2d(sp + tm * SL::kABytes, ma, fb, sg.a_k0 + kb * BK, tm * sg.a_term_rows + arow);
+            tma_load_2d(sp + 2 * SL::kABytes + tm * SL::kBBytes, mb, fb, sg.b_k0 + kb * BK, tm * args.b_term_rows + brow);
           }
           p.advance(STAGES);
         }
@@ -440,35 +426,48 @@ __device__ __forceinline__ void dense_producer(const TcArgs &args, const SmemCar
   }
 }
 
-// ===== consumer warpgroup: MMAs of its 64 rows, then the epilogue (bias, activation, fp32 / split stores) =====
-template <int BN, bool BF16, int NT, int STAGES>
+// One k-block of a tile on the MMA side (one consumer warpgroup, its 64 rows): the pass's products of the four 16-wide
+// k-steps.  `a_lo` is the descriptor low word of this warpgroup's rows in the stage's first A term, `b_lo` that of the
+// stage's first B term.
+template <int BN, int PASS>
+__device__ __forceinline__ void mma_kblock(float *acc, uint32_t a_lo, uint32_t b_lo) {
+  using SL = StageLayout<BN>;
+  constexpr uint32_t A = SL::kABytes >> 4, B = SL::kBBytes >> 4;
+#pragma unroll
+  for (int ks = 0; ks < BK / 16; ks++) {
+    const uint32_t a = a_lo + ks * 2, b = b_lo + ks * 2;
+    pass_products<PASS>([&](int ta, int tb) { wgmma<BN, false>(acc, desc64(a + ta * A), desc64(b + tb * B)); });
+  }
+}
+
+// ===== consumer warpgroup: MMAs of its 64 rows, then the epilogue (bias, sigmoid, fp32 stores) =====
+template <int BN, int STAGES>
 __device__ __forceinline__ void dense_consumer(const TcArgs &args, const SmemCarve &c, uint32_t stage0, int total_tiles, int wg) {
-  using SL = StageLayout<BN, NT>;
+  using SL = StageLayout<BN>;
   constexpr int R = BN / 2;  // accumulator registers per thread
   const uint32_t a_lo0 = desc_lo(stage0) + (uint32_t)(wg * 64 * 128 >> 4);
-  const uint32_t b_lo0 = desc_lo(stage0) + (uint32_t)(NT * SL::kABytes >> 4);
+  const uint32_t b_lo0 = desc_lo(stage0) + (uint32_t)(2 * SL::kABytes >> 4);
   const int warp = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
   const float sc = args.out_scale;
   const float *tbl = c.tbl;
-  const int N = args.N, act = args.act;
+  const int N = args.N;
   Pipe p;
   Consumer<R> cons;
   for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-    int lim, slot;  // rows from lim on (padding up to the tile's end) are computed but neither stored nor checked
-    const int n_tile = tile % args.tiles_n, m0 = dense_tile_row0(args, tile / args.tiles_n, &lim, &slot);
+    int lim;  // rows from lim on (padding up to the tile's end) are computed but neither stored nor checked
+    const int n_tile = tile % args.tiles_n, m0 = dense_tile_row0(args, tile / args.tiles_n, &lim);
     float acc[R];
 #pragma unroll
     for (int i = 0; i < R; i++) acc[i] = 0.f;
     int nkb = 0;
     for (int s = 0; s < args.n_seg; s++) nkb += args.seg[s].k_blocks;
 #pragma unroll
-    for (int pass = 3 - NT; pass < 3; pass++) {
+    for (int pass = 1; pass < 3; pass++) {
       for (int kb = 0; kb < nkb; kb++) {
         cons.begin(acc, c.full + 8 * p.st, p.ph);
         const uint32_t so = p.st * (SL::kBytes >> 4);
-        if (pass == 0) mma_kblock<BN, BN, BF16, NT, 0>(acc, a_lo0 + so, b_lo0 + so);
-        else if (pass == 1) mma_kblock<BN, BN, BF16, NT, 1>(acc, a_lo0 + so, b_lo0 + so);
-        else mma_kblock<BN, BN, BF16, NT, 2>(acc, a_lo0 + so, b_lo0 + so);
+        if (pass == 1) mma_kblock<BN, 1>(acc, a_lo0 + so, b_lo0 + so);
+        else mma_kblock<BN, 2>(acc, a_lo0 + so, b_lo0 + so);
         cons.end(acc, c.empty + 8 * p.st);
         p.advance(STAGES);
       }
@@ -479,65 +478,301 @@ __device__ __forceinline__ void dense_consumer(const TcArgs &args, const SmemCar
     for (int h = 0; h < 2; h++) {  // the thread's two rows of the fragment
       const int row = m0 + wg * 64 + warp * 16 + (lane >> 2) + 8 * h;
       if (row >= lim) continue;
-      const int r = row - slot * args.slot_stride;  // the row inside its hop slot
-      int f32_at = row - args.f32_row0;              // out_f32 row, or < 0
-      if (args.hops) {                               // a ragged call: the row's frozen hops are padding too
-        const int hr = __ldg(args.hops + r);
-        if (slot >= hr) continue;
-        f32_at = slot == hr - 1 ? r : -1;
-      }
-      const size_t orow = (size_t)args.out_row0 + row;
 #pragma unroll
       for (int j = 0; j < BN / 8; j++) {
         const int col = n_tile * BN + 8 * j + 2 * (lane & 3);
         if (col >= N) continue;  // N is even: a pair is entirely in or out
         const float2 bb = __ldg(reinterpret_cast<const float2 *>(args.bias + col));
-        float v[2];
+        float *op = args.out_f32 + (size_t)row * args.ldc + col;
 #pragma unroll
         for (int q = 0; q < 2; q++) {
           const float x = fmaf(acc[4 * j + 2 * h + q], sc, q ? bb.y : bb.x);
-          if (act == PNB_ACT_TANH) { v[q] = tansig_s(x, tbl); bad |= fabsf(x) >= kTanhDomain; }
-          else if (act == PNB_ACT_RELU) v[q] = x < 0.f ? 0.f : x;
-          else if (act == PNB_ACT_SIGMOID) { v[q] = sigmoid_s(x, tbl); bad |= fabsf(x) >= 2.f * kTanhDomain; }
-          else v[q] = x;
+          op[q] = sigmoid_s(x, tbl);
+          bad |= fabsf(x) >= 2.f * kTanhDomain;
         }
-        if (args.out_f32 && f32_at >= 0) {
-          float *op = args.out_f32 + (size_t)f32_at * args.ldc + col;
-          op[0] = v[0];
-          op[1] = v[1];
-        }
-        if (args.out_h)
-          store_split_h2(v[0], v[1], args.out_h + orow * N + col, args.out_h + ((size_t)args.out_plane_rows + orow) * N + col);
-        if (args.out_b) store_split_b2(v[0], v[1], args.out_b + orow * N + col, (size_t)args.out_plane_rows * N, args.out_terms);
       }
     }
     if (bad) atomicOr(args.status, 1);
   }
 }
 
-// ST2 stages of two-term operands; ST3 > 0 adds a three-term mode (ST3 stages) chosen at run time from *args.wide
-template <int BN, bool BF16, int ST2, int ST3>
+// fc_gb / fc_rb: fp16 two-term operands, STAGES stages
+template <int BN, int STAGES>
 __global__ void __launch_bounds__(kTcThreads, 1) tc_gemm_kernel(const __grid_constant__ TcArgs args) {
-  constexpr int kStagesMax = ST2 > ST3 ? ST2 : ST3;
-  constexpr int kRegion = (ST2 * StageLayout<BN, 2>::kBytes > ST3 * StageLayout<BN, 3>::kBytes) ? ST2 * StageLayout<BN, 2>::kBytes
-                                                                                               : ST3 * StageLayout<BN, 3>::kBytes;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  const SmemCarve c = carve<kStagesMax, kRegion>(smem_raw);
+  const SmemCarve c = carve<STAGES, STAGES * StageLayout<BN>::kBytes>(smem_raw);
   const int wg = threadIdx.x >> 7;
   const int total_tiles = args.tiles_m * args.tiles_n;
-  tc_prologue<kStagesMax>(c, args.tansig);
+  tc_prologue<STAGES>(c, args.tansig);
+  const uint32_t stage0 = smem_u32(c.stages);
+  if (wg == 0) {
+    if (threadIdx.x == 0) dense_producer<BN, STAGES>(args, c, stage0, total_tiles);
+  } else {
+    dense_consumer<BN, STAGES>(args, c, stage0, total_tiles, wg - 1);
+  }
+}
+
+// ------------------------------------------------------------------------------------------ conv layers
+// conv_pair_kernel<Q>: conv1 (Q = 5 taps over the fc outputs) or conv2 (Q = 3 taps over the conv1 outputs) for all F
+// hops of a call, 512 outputs, bf16 terms.  Tap q of hop t reads input slot t + q, and every hop uses the same weight
+// rows for tap q.  A tile is (hop pair t0 = 2p, t0 + 1; 128 streams; 128 output columns), with two accumulator sets:
+// acc0 for hop t0, acc1 for hop t0 + 1.  Input slot t0 + j feeds tap j of hop t0 and tap j - 1 of hop t0 + 1, and
+// weight tap q feeds both, so per pass and 32-k block the tile loads Q + 1 input slots and Q weight taps where two
+// one-hop tiles loaded 2 Q of each.
+// The ring carries, per pass and k-block, Q + 1 stages: stage j holds the pass's terms of input slot t0 + j and of
+// weight tap j (stage Q: the input slot alone).  Unit j, on the stage j barrier, issues tap j - 1 of hop t0 + 1
+// (acc1 += A_j W_{j-1}, weights of stage j - 1) and tap j of hop t0 (acc0 += A_j W_j).  Stage j - 1 is read for the
+// last time by unit j and stage Q by unit Q, so stages are freed in ring order, and the consumers hold at most three
+// at once (two for the units being issued, one for the unit in flight).
+// A tile whose second hop is past the call's end (odd F) loads stages 0 .. Q - 1 only and issues acc0 alone.
+// Tiles are walked column tile fastest, then hop pair, then row tile: the CTAs running at once read the input slots of
+// one or two row tiles, which neighbouring pairs share, so they come from L2.  (With the row tile before the pair, the
+// input slots of one pair over all rows -- 75 MB for conv1 at 16 384 streams -- overflow L2 and every pair reads its
+// slots from HBM again.)
+// Summation order, identical for every hop whichever accumulator or tile it is in: passes (pass_products), then 32-k
+// blocks, then taps, then 16-wide k-steps.  A hop's bits depend on nothing but its own row.
+struct ConvArgs {
+  CUtensorMap a_map;    // input hop slots, [3 terms][slots x S][K]: boxes of 128 rows x 32 k, SWIZZLE_64B
+  CUtensorMap w_map;    // packed weights, [3 terms][512][Q K]: the same boxes
+  int k_blocks;         // K / CBK
+  int a_term_rows;      // rows per term plane of the input
+  int S;                // rows per hop slot
+  int n;                // active streams: rows [0, n) of every slot
+  int F;                // hops of the call
+  int pairs;            // hop pairs, ceil(F / 2)
+  int tiles;            // row tiles (ceil(n / 128)) x pairs x column tiles
+  const float *tansig;
+  const float *bias;
+  int *status;          // engine status word: bit 0 = an activation left the reference's defined domain
+  const int *wide;      // device word: non-zero = three operand terms (six products) instead of two
+  const int *hops;      // ragged calls: [n] hops of each row, or null.  Hop t of row r with t >= hops[r] is computed
+                        // but neither stored nor checked; out_f32 takes the row's hop hops[r] - 1 (else F - 1)
+  int act;              // PNB_ACT_RELU (conv1) or PNB_ACT_TANH (conv2)
+  __nv_bfloat16 *out_b; // conv1: three bf16 terms, hop t at row out_row0 + t S of planes out_plane_rows apart
+  __half *out_h;        // conv2: fp16 two-term split (x 2^10), hop t at row out_row0 + t S
+  float *out_f32;       // conv2: fp32 copy of each row's last hop, [n][512], or null
+  int out_row0;
+  int out_plane_rows;
+};
+constexpr int CONV_N = 512;
+constexpr int CONV_TILES_N = CONV_N / DENSE_BN;
+// 7 stages of 32 KB (two terms) or 4 of 48 KB (three terms): three held by the consumers, the rest in flight
+constexpr int CONV_ST2 = 7, CONV_ST3 = 4;
+constexpr int kConvRegion = CONV_ST2 * StageLayout<DENSE_BN, 2, CBK>::kBytes > CONV_ST3 * StageLayout<DENSE_BN, 3, CBK>::kBytes
+                                ? CONV_ST2 * StageLayout<DENSE_BN, 2, CBK>::kBytes
+                                : CONV_ST3 * StageLayout<DENSE_BN, 3, CBK>::kBytes;
+constexpr int kConvStages = CONV_ST2 > CONV_ST3 ? CONV_ST2 : CONV_ST3;
+
+struct ConvTile {
+  int n_tile, m0, t0;
+  bool pair;  // hop t0 + 1 is inside the call
+  __device__ __forceinline__ ConvTile(const ConvArgs &a, int tile) {
+    n_tile = tile % CONV_TILES_N;
+    const int rp = tile / CONV_TILES_N;
+    t0 = 2 * (rp % a.pairs);
+    m0 = (rp / a.pairs) * TM;
+    pair = t0 + 1 < a.F;
+  }
+};
+
+// ===== TMA producer (one thread): per pass, k-block and unit j, input slot t0 + j and weight tap j =====
+template <int Q, int NT, int STAGES>
+__device__ __forceinline__ void conv_producer(const ConvArgs &args, const SmemCarve &c, uint32_t stage0) {
+  using SL = StageLayout<DENSE_BN, NT, CBK>;
+  const int K = args.k_blocks * CBK;
+  Pipe p;
+  for (int tile = blockIdx.x; tile < args.tiles; tile += gridDim.x) {
+    const ConvTile tl(args, tile);
+    const int units = tl.pair ? Q + 1 : Q;
+    const int arow = tl.t0 * args.S + tl.m0, brow = tl.n_tile * DENSE_BN;
+    // with q passes still to go after this one, the pass needs the first q + 1 terms of either operand
+    for (int nt = NT; nt > 0; nt--) {
+      for (int kb = 0; kb < args.k_blocks; kb++) {
+        for (int j = 0; j < units; j++) {
+          mbar_wait(c.empty + 8 * p.st, p.ph ^ 1);  // fresh barrier: passes immediately
+          const uint32_t fb = c.full + 8 * p.st;
+          mbar_expect_tx(fb, nt * (SL::kABytes + (j < Q ? SL::kBBytes : 0)));
+          const uint32_t sp = stage0 + p.st * SL::kBytes;
+          for (int tm = 0; tm < nt; tm++) {
+            tma_load_2d(sp + tm * SL::kABytes, &args.a_map, fb, kb * CBK, tm * args.a_term_rows + j * args.S + arow);
+            if (j < Q)
+              tma_load_2d(sp + NT * SL::kABytes + tm * SL::kBBytes, &args.w_map, fb, j * K + kb * CBK, tm * CONV_N + brow);
+          }
+          p.advance(STAGES);
+        }
+      }
+    }
+  }
+}
+
+// The consumer's side of the conv ring: `full` is the next stage to wait for, `freed` the oldest stage not yet freed,
+// `pending` the stages the unit in flight is the last reader of.
+struct ConvRing {
+  Pipe full, freed;
+  int pending = 0;
+  template <int STAGES>
+  __device__ __forceinline__ void release(const SmemCarve &c) {
+    for (; pending > 0; pending--) {
+      if (threadIdx.x % 128 == 0) mbar_arrive(c.empty + 8 * freed.st);
+      freed.advance(STAGES);
+    }
+  }
+};
+
+// One unit on one consumer warpgroup: wait for its stage, issue acc1 (if HOP1: A of this stage, weights of the
+// stage before) and acc0 (if HOP0: A and weights of this stage) per k-step and product, alternating so that
+// neighbouring MMAs do not wait on each other's accumulators, then free the stages the previous unit read last once
+// its MMAs have completed (one unit stays in flight).  RETIRE: stages this unit is the last reader of.
+template <int NT, int PASS, int STAGES, int R, bool HOP0, bool HOP1, int RETIRE>
+__device__ __forceinline__ void conv_unit(float *acc, uint32_t a_lo0, uint32_t b_lo0, const SmemCarve &c, ConvRing &ring) {
+  using SL = StageLayout<DENSE_BN, NT, CBK>;
+  constexpr uint32_t A = SL::kABytes >> 4, B = SL::kBBytes >> 4, ST = SL::kBytes >> 4;
+  const uint32_t st = ring.full.st;
+  mbar_wait(c.full + 8 * st, ring.full.ph);
+  acc_fence<R>(acc);
+  wgmma_fence();
+  const uint32_t so = st * ST, sp = (st ? st - 1 : STAGES - 1) * ST;
+#pragma unroll
+  for (int ks = 0; ks < CBK / 16; ks++) {
+    const uint32_t a = a_lo0 + so + ks * 2, b = b_lo0 + so + ks * 2, bp = b_lo0 + sp + ks * 2;
+    pass_products<PASS>([&](int ta, int tb) {
+      if (HOP1) wgmma<DENSE_BN, true>(acc + 64, desc64(a + ta * A, kDescHi64), desc64(bp + tb * B, kDescHi64));
+      if (HOP0) wgmma<DENSE_BN, true>(acc, desc64(a + ta * A, kDescHi64), desc64(b + tb * B, kDescHi64));
+    });
+  }
+  wgmma_commit();
+  wgmma_wait<1>();
+  acc_fence<R>(acc);
+  ring.release<STAGES>(c);
+  ring.pending = RETIRE;
+  ring.full.advance(STAGES);
+}
+
+// One pass over K of a tile: k-blocks, and per k-block the units in ring order
+template <int Q, int NT, int PASS, int STAGES, bool PAIR>
+__device__ __forceinline__ void conv_pass(float *acc, int k_blocks, uint32_t a_lo0, uint32_t b_lo0, const SmemCarve &c,
+                                          ConvRing &ring) {
+  constexpr int R = PAIR ? 128 : 64;
+  for (int kb = 0; kb < k_blocks; kb++) {
+    if (PAIR) {
+      conv_unit<NT, PASS, STAGES, R, true, false, 0>(acc, a_lo0, b_lo0, c, ring);
+#pragma unroll
+      for (int j = 1; j < Q; j++) conv_unit<NT, PASS, STAGES, R, true, true, 1>(acc, a_lo0, b_lo0, c, ring);
+      conv_unit<NT, PASS, STAGES, R, false, true, 2>(acc, a_lo0, b_lo0, c, ring);
+    } else {
+#pragma unroll
+      for (int j = 0; j < Q; j++) conv_unit<NT, PASS, STAGES, R, true, false, 1>(acc, a_lo0, b_lo0, c, ring);
+    }
+  }
+}
+template <int Q, int NT, int STAGES, bool PAIR>
+__device__ __forceinline__ void conv_tile_mmas(float *acc, int k_blocks, uint32_t a_lo0, uint32_t b_lo0, const SmemCarve &c,
+                                               ConvRing &ring) {
+  if (NT == 3) conv_pass<Q, NT, 0, STAGES, PAIR>(acc, k_blocks, a_lo0, b_lo0, c, ring);
+  conv_pass<Q, NT, 1, STAGES, PAIR>(acc, k_blocks, a_lo0, b_lo0, c, ring);
+  conv_pass<Q, NT, 2, STAGES, PAIR>(acc, k_blocks, a_lo0, b_lo0, c, ring);
+  wgmma_wait<0>();
+  acc_fence<PAIR ? 128 : 64>(acc);
+  ring.release<STAGES>(c);
+}
+
+// Epilogue of hop t for this thread's two rows: bias, activation, stores.  Returns whether a pre-activation left the
+// reference's tanh domain.  In the MMA fragment a lane holds two neighbouring columns of every 8-column group, so a
+// warp's stores would cover half a 32-byte sector per row; the four lanes of a row (a quad) first exchange the
+// activated values of column groups 2 jj and 2 jj + 1, after which lane q holds columns 16 jj + 4 q .. + 3 and the
+// quad writes whole sectors.  Lanes of a quad share their row, so rows that store nothing still take part in the
+// exchange.
+__device__ __forceinline__ bool conv_epilogue(const ConvArgs &args, const float *acc, const ConvTile &tl, int t, int wg,
+                                              const float *tbl) {
+  const int warp = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31, q = lane & 3;
+  const int src = (lane & ~3) | ((q & 1) << 1);  // the quad lane holding the first two of this lane's columns
+  bool bad = false;
+#pragma unroll
+  for (int h = 0; h < 2; h++) {  // the thread's two rows of the fragment
+    const int row = tl.m0 + wg * 64 + warp * 16 + (lane >> 2) + 8 * h;
+    bool ok = row < args.n;  // padding rows of the last row tile are computed only
+    bool last = t == args.F - 1;
+    if (args.hops && ok) {   // a ragged call: the row's frozen hops are padding too
+      const int hr = __ldg(args.hops + row);
+      ok = t < hr;
+      last = t == hr - 1;
+    }
+    const size_t orow = (size_t)args.out_row0 + (size_t)t * args.S + row;
+#pragma unroll
+    for (int jj = 0; jj < DENSE_BN / 16; jj++) {
+      float v[2][2];  // columns 8 j + 2 q, + 1 of j = 2 jj, 2 jj + 1
+#pragma unroll
+      for (int g = 0; g < 2; g++) {
+        const int j = 2 * jj + g;
+        const float2 bb = __ldg(reinterpret_cast<const float2 *>(args.bias + tl.n_tile * DENSE_BN + 8 * j + 2 * q));
+#pragma unroll
+        for (int e = 0; e < 2; e++) {
+          const float x = acc[4 * j + 2 * h + e] + (e ? bb.y : bb.x);
+          if (args.act == PNB_ACT_TANH) { v[g][e] = tansig_s(x, tbl); bad |= ok && fabsf(x) >= kTanhDomain; }
+          else v[g][e] = x < 0.f ? 0.f : x;
+        }
+      }
+      float w[4];  // columns 16 jj + 4 q .. + 3
+#pragma unroll
+      for (int e = 0; e < 2; e++) {
+        const float a0 = __shfl_sync(0xffffffffu, v[0][e], src), b0 = __shfl_sync(0xffffffffu, v[1][e], src);
+        const float a1 = __shfl_sync(0xffffffffu, v[0][e], src + 1), b1 = __shfl_sync(0xffffffffu, v[1][e], src + 1);
+        w[e] = q < 2 ? a0 : b0;
+        w[2 + e] = q < 2 ? a1 : b1;
+      }
+      if (!ok) continue;
+      const int col = tl.n_tile * DENSE_BN + 16 * jj + 4 * q;
+      if (args.out_f32 && last) {
+        float *op = args.out_f32 + (size_t)row * CONV_N + col;
+#pragma unroll
+        for (int e = 0; e < 4; e++) op[e] = w[e];
+      }
+      if (args.out_h)
+        store_split_h4(w, args.out_h + orow * CONV_N + col, args.out_h + ((size_t)args.out_plane_rows + orow) * CONV_N + col);
+      if (args.out_b) store_split_b4(w, args.out_b + orow * CONV_N + col, (size_t)args.out_plane_rows * CONV_N);
+    }
+  }
+  return bad;
+}
+
+// ===== consumer warpgroup: MMAs of its 64 rows of both hops, then the epilogue of each hop =====
+template <int Q, int NT, int STAGES>
+__device__ __forceinline__ void conv_consumer(const ConvArgs &args, const SmemCarve &c, uint32_t stage0, int wg) {
+  using SL = StageLayout<DENSE_BN, NT, CBK>;
+  const uint32_t a_lo0 = desc_lo(stage0) + (uint32_t)(wg * 64 * CBK * 2 >> 4);
+  const uint32_t b_lo0 = desc_lo(stage0) + (uint32_t)(NT * SL::kABytes >> 4);
+  ConvRing ring;
+  for (int tile = blockIdx.x; tile < args.tiles; tile += gridDim.x) {
+    const ConvTile tl(args, tile);
+    float acc[128];  // acc0 = acc[0, 64), acc1 = acc[64, 128)
+#pragma unroll
+    for (int i = 0; i < 128; i++) acc[i] = 0.f;
+    if (tl.pair) conv_tile_mmas<Q, NT, STAGES, true>(acc, args.k_blocks, a_lo0, b_lo0, c, ring);
+    else conv_tile_mmas<Q, NT, STAGES, false>(acc, args.k_blocks, a_lo0, b_lo0, c, ring);
+    bool bad = conv_epilogue(args, acc, tl, tl.t0, wg, c.tbl);
+    if (tl.pair) bad |= conv_epilogue(args, acc + 64, tl, tl.t0 + 1, wg, c.tbl);
+    if (bad) atomicOr(args.status, 1);
+  }
+}
+
+template <int Q>
+__global__ void __launch_bounds__(kTcThreads, 1) conv_pair_kernel(const __grid_constant__ ConvArgs args) {
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  const SmemCarve c = carve<kConvStages, kConvRegion>(smem_raw);
+  const int wg = threadIdx.x >> 7;
+  tc_prologue<kConvStages>(c, args.tansig);
   const uint32_t stage0 = smem_u32(c.stages);
   // the same word for every thread of the launch (written by an earlier launch): every role takes the same branch
-  const bool wide = ST3 > 0 && args.wide != nullptr && *args.wide != 0;
-
+  const bool wide = *args.wide != 0;
   if (wg == 0) {
-    if (threadIdx.x == 0) {
-      if (ST3 > 0 && wide) dense_producer<BN, 3, ST3 ? ST3 : 1>(args, c, stage0, total_tiles);
-      else dense_producer<BN, 2, ST2>(args, c, stage0, total_tiles);
-    }
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kProducerRegs));
+    if (threadIdx.x != 0) return;
+    if (wide) conv_producer<Q, 3, CONV_ST3>(args, c, stage0);
+    else conv_producer<Q, 2, CONV_ST2>(args, c, stage0);
   } else {
-    if (ST3 > 0 && wide) dense_consumer<BN, BF16, 3, ST3 ? ST3 : 1>(args, c, stage0, total_tiles, wg - 1);
-    else dense_consumer<BN, BF16, 2, ST2>(args, c, stage0, total_tiles, wg - 1);
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kConsumerRegs));
+    if (wide) conv_consumer<Q, 3, CONV_ST3>(args, c, stage0, wg - 1);
+    else conv_consumer<Q, 2, CONV_ST2>(args, c, stage0, wg - 1);
   }
 }
 
@@ -579,9 +814,6 @@ __device__ __forceinline__ void wait_layer(const ChainArgs &a, int layer, int rb
 
 constexpr int GRU_STAGES = 5;
 using GruStage = StageLayout<GRU_BN, 2, CBK>;  // 2 x 8 KB of A + 2 x 12 KB of B = 40 KB
-// Registers per thread after the producer warpgroup hands its surplus to the consumers (setmaxnreg): the launch
-// gives 168 to each of the 384 threads; 128 x (168 - 40) = 256 x (232 - 168).
-constexpr int kProducerRegs = 40, kConsumerRegs = 232;
 
 // A fragments of one k-block (CBK = two 16-wide k-steps, both terms of A) for one consumer warp: 16 registers,
 // fa[8 term + 4 ks + i] (wgmma_rs layout).  `a_addr[ks]` is this lane's ldmatrix row address for k-step ks in the first A term of stage
@@ -767,12 +999,15 @@ __global__ void __launch_bounds__(kTcThreads, 1) gru_chain_kernel(const __grid_c
   }
 }
 
-constexpr int DENSE_STAGES = 3, DENSE_STAGES3 = 2, SMALL_BN = 48, SMALL_STAGES = 5;
+constexpr int SMALL_BN = 48, SMALL_STAGES = 5;
 // conv layers: fc / conv1 outputs and the conv weights are stored as THREE bf16 terms.  The launches use the first
 // two (three products, corrections summed before the main product) unless the engine's `wide` word is set
 // (PNB_CONV_WIDE at pnb_create: all three terms, six products).  The mode is the same for every row of every call,
 // so a stream's result never depends on what its neighbours in the batch carry.
 constexpr int kConvTerms = 3;
+constexpr size_t kConvSmem = tc_smem_bytes<kConvStages, kConvRegion>();
+constexpr size_t kSmallSmem = tc_smem_bytes<SMALL_STAGES, SMALL_STAGES * StageLayout<SMALL_BN>::kBytes>();
+static_assert(kConvSmem <= 227 * 1024, "the conv ring fits a Hopper block's shared memory");
 
 // fc 70 -> 128 relu in fp32 FMA (0.1 % of the MACs; K = 70 is no tensor-core shape), emitting the three bf16
 // terms conv1 consumes.  One block per 16 rows, one thread per output: the 16 feature rows sit in shared memory and are
@@ -857,8 +1092,9 @@ struct pnb_tc_state {
   int *wide = nullptr;                                   // see kConvTerms
   int tiles_mp = 0;
   // tensor maps
-  CUtensorMap m_fc_all, m_c1_all, m_c2, m_h[5], m_wconv1, m_wconv2, m_wgb, m_wrb;  // dense layers: 64-k boxes, SW128
-  CUtensorMap m_c2_ch, m_h_ch[5], m_w[5], m_u[5];                                   // GRU chain: 32-k boxes, SW64
+  CUtensorMap m_c2, m_h[5], m_wgb, m_wrb;                  // output layers: 64-k boxes, SW128
+  CUtensorMap m_fc_all, m_c1_all, m_wconv1, m_wconv2;     // conv layers: 32-k boxes, SW64
+  CUtensorMap m_c2_ch, m_h_ch[5], m_w[5], m_u[5];         // GRU chain: 32-k boxes, SW64
 };
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *,
@@ -867,7 +1103,8 @@ typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t
 static EncodeTiledFn g_encode = nullptr;
 static std::string g_tc_err;
 
-// boxes of box_k x box_rows; the dense layers read 64 k (SWIZZLE_128B), the GRU chain 32 k (SWIZZLE_64B)
+// boxes of box_k x box_rows; the output layers read 64 k (SWIZZLE_128B), the conv layers and the GRU chain 32 k
+// (SWIZZLE_64B)
 static int make_map(CUtensorMap *m, const void *base, bool bf16, uint64_t rows, uint64_t cols, uint32_t box_rows,
                     uint32_t box_k = BK, CUtensorMapSwizzle swizzle = CU_TENSOR_MAP_SWIZZLE_128B) {
   cuuint64_t dims[2] = {cols, rows};
@@ -1054,15 +1291,15 @@ int tc_prepare(pnb_engine *e, const pnb_model *model) {
   int bad = 0;
   bad |= make_map(&t->m_wgb, t->w_gb, false, 2 * SMALL_BN, 2560, SMALL_BN);
   bad |= make_map(&t->m_wrb, t->w_rb, false, 2 * SMALL_BN, 128, SMALL_BN);
-  bad |= make_map(&t->m_fc_all, t->fc_all, true, kConvTerms * (Fm + 4) * S, 128, TM);
-  bad |= make_map(&t->m_c1_all, t->c1_all, true, kConvTerms * (Fm + 2) * S, 512, TM);
   bad |= make_map(&t->m_c2, t->c2_h, false, 2 * Fm * S, 512, TM);
   for (int i = 0; i < 5; i++)
     bad |= make_map(&t->m_h[i], t->h_all[i], false, 2 * (Fm + 1) * S, kGruH[i], TM);
-  bad |= make_map(&t->m_wconv1, t->w_conv1, true, kConvTerms * 512, 640, DENSE_BN);
-  bad |= make_map(&t->m_wconv2, t->w_conv2, true, kConvTerms * 512, 1536, DENSE_BN);
-  // the chain's operands: the same buffers in boxes of 32 k
+  // the conv layers' and the chain's operands: boxes of 32 k
   const CUtensorMapSwizzle sw64 = CU_TENSOR_MAP_SWIZZLE_64B;
+  bad |= make_map(&t->m_fc_all, t->fc_all, true, kConvTerms * (Fm + 4) * S, 128, TM, CBK, sw64);
+  bad |= make_map(&t->m_c1_all, t->c1_all, true, kConvTerms * (Fm + 2) * S, 512, TM, CBK, sw64);
+  bad |= make_map(&t->m_wconv1, t->w_conv1, true, kConvTerms * 512, 640, DENSE_BN, CBK, sw64);
+  bad |= make_map(&t->m_wconv2, t->w_conv2, true, kConvTerms * 512, 1536, DENSE_BN, CBK, sw64);
   bad |= make_map(&t->m_c2_ch, t->c2_h, false, 2 * Fm * S, 512, TM, CBK, sw64);
   for (int i = 0; i < 5; i++) {
     const int rows = (kGruH[i] / HT) * GRU_BN;
@@ -1073,17 +1310,17 @@ int tc_prepare(pnb_engine *e, const pnb_model *model) {
   if (bad) return engine_fail(PNB_ERR_CUDA, "cuTensorMapEncodeTiled failed");
   TCK(cudaFuncSetAttribute(gru_chain_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                            (int)tc_smem_bytes<GRU_STAGES, GRU_STAGES * GruStage::kBytes>()));
-  TCK(cudaFuncSetAttribute(tc_gemm_kernel<DENSE_BN, true, DENSE_STAGES, DENSE_STAGES3>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                           (int)dense_smem_bytes<DENSE_BN, DENSE_STAGES, DENSE_STAGES3>()));
-  TCK(cudaFuncSetAttribute(tc_gemm_kernel<SMALL_BN, false, SMALL_STAGES, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                           (int)dense_smem_bytes<SMALL_BN, SMALL_STAGES, 0>()));
+  TCK(cudaFuncSetAttribute(conv_pair_kernel<5>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kConvSmem));
+  TCK(cudaFuncSetAttribute(conv_pair_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kConvSmem));
+  TCK(cudaFuncSetAttribute(tc_gemm_kernel<SMALL_BN, SMALL_STAGES>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                           (int)kSmallSmem));
   return PNB_OK;
 }
 
 // The tensor path's part of a stream's state: the conv input histories (the last 4 fc / 2 conv1 outputs, oldest first)
 // as the three bf16 term planes of hop slots 0..3 / 0..1, and the fp16 hi / lo terms of the GRU states at slot 0.
 // Export writes the terms and their fp32 sums; import restores the raw terms, or splits blobs without them (fp32-mode
-// engines) with the roundings of store_split_b2 / store_split_h2.
+// engines) with the roundings of store_split_b4 / store_split_h2.
 int tc_state_segs(const pnb_engine *e, StateSeg *seg, int ns) {
   static_assert(kConvTerms == 3, "StreamState carries three bf16 terms per conv history value");
   const pnb_tc_state *t = e->tc.get();
@@ -1118,7 +1355,8 @@ int tc_state_segs(const pnb_engine *e, StateSeg *seg, int ns) {
   return ns;
 }
 
-// One persistent tensor-core launch: a dense layer or the GRU chain, each a tc_gemm_kernel record in the profile.
+// One persistent tensor-core launch: a conv layer, an output layer or the GRU chain, each a tc_gemm_kernel record in the
+// profile.
 template <typename K, typename A>
 static int tc_launch(pnb_engine *e, K kernel, const A &a, int units, size_t smem, cudaStream_t st) {
   int grid = units < e->sm_count ? units : e->sm_count;  // persistent: one CTA per SM
@@ -1128,20 +1366,27 @@ static int tc_launch(pnb_engine *e, K kernel, const A &a, int units, size_t smem
   TCK(cudaGetLastError());
   return PNB_OK;
 }
-// A dense layer over the active rows of `slots` hop slots.  With every stream active the rows are one flat range of
-// slots x S; otherwise, and whenever the epilogue needs each row's hop slot (a.hops), each slot has its own
-// ceil(n / 128) row tiles.
-template <int BN, bool BF16, int ST2, int ST3>
-static int tc_launch_dense(pnb_engine *e, TcArgs &a, int slots, int tiles_n, cudaStream_t st) {
+// An output layer over the active rows of `slots` hop slots.  With every stream active the rows are one flat range of
+// slots x S; otherwise each slot has its own ceil(n / 128) row tiles.
+static int tc_launch_out(pnb_engine *e, TcArgs &a, int slots, cudaStream_t st) {
   const int n = e->n_active;
-  if (n == e->S && !a.hops) {
+  if (n == e->S) {
     a.M = slots * n; a.slot_stride = 0; a.tiles_slot = (a.M + TM - 1) / TM; a.tiles_m = a.tiles_slot;
   } else {
     a.M = n; a.slot_stride = e->S; a.tiles_slot = (n + TM - 1) / TM; a.tiles_m = slots * a.tiles_slot;
   }
-  a.tiles_n = tiles_n;
+  a.tiles_n = 1;
   a.status = e->d_status;
-  return tc_launch(e, tc_gemm_kernel<BN, BF16, ST2, ST3>, a, a.tiles_m * a.tiles_n, dense_smem_bytes<BN, ST2, ST3>(), st);
+  return tc_launch(e, tc_gemm_kernel<SMALL_BN, SMALL_STAGES>, a, a.tiles_m, kSmallSmem, st);
+}
+// A conv layer over the active rows of the call's F hops: ceil(n / 128) row tiles per hop pair
+template <int Q>
+static int tc_launch_conv(pnb_engine *e, ConvArgs &a, int F, cudaStream_t st) {
+  a.S = e->S; a.n = e->n_active; a.F = F;
+  a.pairs = (F + 1) / 2;
+  a.tiles = (a.n + TM - 1) / TM * a.pairs * CONV_TILES_N;
+  a.status = e->d_status;
+  return tc_launch(e, conv_pair_kernel<Q>, a, a.tiles, kConvSmem, st);
 }
 
 static TcSeg mkseg(int a_map, int b_map, int K, int a_k0, int b_k0, int a_row0, int a_term_rows) {
@@ -1164,28 +1409,23 @@ static int tc_front(pnb_engine *e, int F, const int *hops, cudaStream_t st) {
     fc_split_kernel<<<dim3((rows + FC_ROWS - 1) / FC_ROWS, slots), 128, 0, st>>>(e->d_feat, e->fc.W, e->fc.b,
                                                     t->fc_all + (size_t)4 * S * 128, rows, (size_t)(Fm + 4) * S, (size_t)S);
   }
-  TcArgs a;
   // conv1: tap q of hop t reads fc slot t + q (oldest first, nnet.cpp:182-200); output -> c1 slots 2 + t
+  ConvArgs a;
   memset(&a, 0, sizeof a);
-  a.maps[0] = t->m_fc_all;
-  a.maps[1] = t->m_wconv1;
-  for (int q = 0; q < 5; q++) a.seg[q] = mkseg(0, 1, 128, 0, q * 128, q * S, (Fm + 4) * S);
-  a.n_seg = 5; a.b_term_rows = 512; a.out_scale = 1.f; a.tansig = tbl;
-  a.bias = t->bias_pad; a.act = PNB_ACT_RELU; a.N = 512;
-  a.out_b = t->c1_all; a.out_row0 = 2 * S; a.out_plane_rows = (Fm + 2) * S; a.out_terms = kConvTerms; a.wide = t->wide;
-  if (int rc = tc_launch_dense<DENSE_BN, true, DENSE_STAGES, DENSE_STAGES3>(e, a, F, 512 / DENSE_BN, st)) return rc;
+  a.a_map = t->m_fc_all; a.w_map = t->m_wconv1;
+  a.k_blocks = 128 / CBK; a.a_term_rows = (Fm + 4) * S;
+  a.tansig = tbl; a.bias = t->bias_pad; a.wide = t->wide; a.act = PNB_ACT_RELU;
+  a.out_b = t->c1_all; a.out_row0 = 2 * S; a.out_plane_rows = (Fm + 2) * S;
+  if (int rc = tc_launch_conv<5>(e, a, F, st)) return rc;
   // conv2: three taps -> tanh -> fp16 terms (gru1 / gru_rb / fc_gb inputs); fp32 copy of the call's last hop (of each
   // row's last hop in a ragged call, whose frozen hops neither store nor raise the domain bit)
   memset(&a, 0, sizeof a);
-  a.maps[0] = t->m_c1_all;
-  a.maps[1] = t->m_wconv2;
-  for (int q = 0; q < 3; q++) a.seg[q] = mkseg(0, 1, 512, 0, q * 512, q * S, (Fm + 2) * S);
-  a.n_seg = 3; a.b_term_rows = 512; a.out_scale = 1.f; a.tansig = tbl;
-  a.bias = t->bias_pad + 512; a.act = PNB_ACT_TANH; a.N = 512;
-  a.out_f32 = e->c2; a.ldc = 512; a.f32_row0 = (F - 1) * S;
-  a.out_h = t->c2_h; a.out_row0 = 0; a.out_plane_rows = Fm * S; a.wide = t->wide;
+  a.a_map = t->m_c1_all; a.w_map = t->m_wconv2;
+  a.k_blocks = 512 / CBK; a.a_term_rows = (Fm + 2) * S;
+  a.tansig = tbl; a.bias = t->bias_pad + 512; a.wide = t->wide; a.act = PNB_ACT_TANH;
+  a.out_h = t->c2_h; a.out_f32 = e->c2; a.out_row0 = 0; a.out_plane_rows = Fm * S;
   a.hops = hops;
-  return tc_launch_dense<DENSE_BN, true, DENSE_STAGES, DENSE_STAGES3>(e, a, F, 512 / DENSE_BN, st);
+  return tc_launch_conv<3>(e, a, F, st);
 }
 
 // The recurrent part: five GRUs per hop (rnn.cpp:58-71) in one persistent launch.  State slot t holds the state
@@ -1244,15 +1484,15 @@ static int tc_out(pnb_engine *e, int F, const int *, cudaStream_t st) {
   a.seg[0] = mkseg(0, 5, 512, 0, 0, 0, Fm * S);
   for (int q = 1; q < 5; q++) a.seg[q] = mkseg(q, 5, 512, 0, q * 512, S, h_terms);  // state after hop t = slot t+1
   a.n_seg = 5; a.b_term_rows = SMALL_BN; a.out_scale = t->scale_gb; a.tansig = tbl;
-  a.bias = t->bias_pad + 1024; a.act = PNB_ACT_SIGMOID; a.N = 34; a.ldc = 68; a.out_f32 = e->d_gr;
-  if (int rc = tc_launch_dense<SMALL_BN, false, SMALL_STAGES, 0>(e, a, F, 1, st)) return rc;
+  a.bias = t->bias_pad + 1024; a.N = 34; a.ldc = 68; a.out_f32 = e->d_gr;
+  if (int rc = tc_launch_out(e, a, F, st)) return rc;
   memset(&a, 0, sizeof a);
   a.maps[0] = t->m_h[4];
   a.maps[1] = t->m_wrb;
   a.seg[0] = mkseg(0, 1, 128, 0, 0, S, h_terms);
   a.n_seg = 1; a.b_term_rows = SMALL_BN; a.out_scale = t->scale_rb; a.tansig = tbl;
-  a.bias = t->bias_pad + 1072; a.act = PNB_ACT_SIGMOID; a.N = 34; a.ldc = 68; a.out_f32 = e->d_gr + 34;
-  return tc_launch_dense<SMALL_BN, false, SMALL_STAGES, 0>(e, a, F, 1, st);
+  a.bias = t->bias_pad + 1072; a.N = 34; a.ldc = 68; a.out_f32 = e->d_gr + 34;
+  return tc_launch_out(e, a, F, st);
 }
 
 // End of a call of F hops: the last 4 fc / 2 conv1 hop slots and the last state slot move to the front (in a ragged

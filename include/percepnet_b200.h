@@ -351,7 +351,9 @@ int pnb_train_import(pnb_engine *e, int what, const void *src, size_t bytes);
  * pnb_process_device_* / pnb_process_host_*.
  * Launches:  pnb_analyze_*     stage-in + analysis + feature store
  *            pnb_synthesize_*  g/r stage + synthesis + [history move]
- * with the history move on the synthesis where pnb_process_* would issue it. */
+ * with the history move on the synthesis where pnb_process_* would issue it.
+ * The operands of a pending synthesis and the synthesis's gradient with respect to g/r (pnb_synthesis_operands_device,
+ * pnb_synthesis_backward_device) are declared in pnb_synth_grad.h, included at the end of this header. */
 int pnb_analyze_host_f32(pnb_engine *e, const float *in, size_t in_stride, int n_frames, float *feat, size_t feat_stride);
 int pnb_analyze_host_i16(pnb_engine *e, const short *in, size_t in_stride, int n_frames, float *feat, size_t feat_stride);
 int pnb_analyze_device_f32(pnb_engine *e, const float *d_in, size_t in_stride, int n_frames, float *d_feat,
@@ -612,5 +614,6 @@ const char *pnb_version(void);
 #endif
 #include "pnb_train_device.h"
 #include "pnb_train_state.h"
+#include "pnb_synth_grad.h"
 
 #endif /* PERCEPNET_B200_H */

@@ -1,5 +1,5 @@
-"""Python host mirror of the C-ABI in include/percepnet_b200.h, include/pnb_train_device.h and include/pnb_train_state.h
-(ctypes; no compute here).
+"""Python host mirror of the C-ABI in include/percepnet_b200.h, include/pnb_train_device.h, include/pnb_train_state.h and
+include/pnb_synth_grad.h (ctypes; no compute here).
 
 ``Engine`` is the batched-streams counterpart of the reference's ``DenoiseState``
 (/root/reference/src/rnnoise.h:49-60): ``Engine.process`` advances S independent 48 kHz streams by F
@@ -142,6 +142,13 @@ _TRAIN_STATE_SIGNATURES = {
 }
 TRAIN_STATE_EXPORTS = tuple(_TRAIN_STATE_SIGNATURES)
 TRAIN_STATE_FLOATS = 3712   # PNB_TRAIN_STATE_FLOATS: one window's network state
+# Every symbol of include/pnb_synth_grad.h (the operands of a pending synthesis and its gradient), the same way.
+_SYNTH_GRAD_SIGNATURES = {
+    "pnb_synthesis_operands_device": (_i, (_vp, _vp, _sz, _vp)),
+    "pnb_synthesis_backward_device": (_i, (_vp, _sz, _vp, _sz, _ll, _i, _i, _vp, _sz, _vp, _sz, _vp)),
+}
+SYNTH_GRAD_EXPORTS = tuple(_SYNTH_GRAD_SIGNATURES)
+SYNTH_OPS_FLOATS = 1636     # PNB_SYNTH_OPS_FLOATS: one hop's synthesis operands
 
 
 def load_library() -> C.CDLL:
@@ -153,7 +160,8 @@ def load_library() -> C.CDLL:
         raise PnbError(f"{LIB_PATH} is missing: run `python -c 'import __graft_entry__ as g; g.build()'` "
                        "(nvcc, sm_90a).  There is no CPU implementation to fall back to.")
     L = C.CDLL(LIB_PATH)
-    for name, (restype, argtypes) in {**_SIGNATURES, **_TRAIN_DEVICE_SIGNATURES, **_TRAIN_STATE_SIGNATURES}.items():
+    for name, (restype, argtypes) in {**_SIGNATURES, **_TRAIN_DEVICE_SIGNATURES, **_TRAIN_STATE_SIGNATURES,
+                                    **_SYNTH_GRAD_SIGNATURES}.items():
         f = getattr(L, name)
         f.restype, f.argtypes = restype, argtypes
     _lib = L
@@ -235,6 +243,16 @@ def pitch_only_device(d_buf: int, stride: int, n_units: int, d_period: int, d_co
     """pnb_pitch_only_device on raw device pointers (BASELINE.json config 5: the pitch analysis alone)."""
     _call_lib("pnb_pitch_only_device", d_buf, stride, n_units, d_prev_period, d_prev_gain, d_period, d_corr, d_gain,
               d_lag, stream)
+
+
+def synthesis_backward_device(d_ops: int, ops_stride: int, d_gr: int, gr_stride: int, n_rows: int, n_frames: int,
+                              postfilter: bool, d_dout: int, dout_stride: int, d_dgr: int, dgr_stride: int,
+                              stream: int = 0):
+    """pnb_synthesis_backward_device on raw device pointers (strides in floats): dL/d(g, r) [n_rows, n_frames, 68] of
+    the synthesis whose operands (Engine.synthesis_operands_device) and g/r are given, from dL/d(out) [n_rows,
+    n_frames*480]; postfilter: the POSTFILTER setting of the engine that synthesised.  Needs no engine."""
+    _call_lib("pnb_synthesis_backward_device", d_ops, ops_stride, d_gr, gr_stride, n_rows, n_frames, 1 if postfilter else 0,
+              d_dout, dout_stride, d_dgr, dgr_stride, stream)
 
 
 def pitch_only(bufs: np.ndarray, prev_period=None, prev_gain=None):
@@ -536,6 +554,11 @@ class Engine:
                           int16: bool = False):
         """pnb_synthesize_device_* on raw device pointers (strides in elements)."""
         self._synthesize_device(None, d_gr, gr_stride, n_frames, d_out, out_stride, stream, int16)
+
+    def synthesis_operands_device(self, d_ops: int, ops_stride: int, stream: int = 0):
+        """pnb_synthesis_operands_device: the operands of the pending synthesis, [active, F, SYNTH_OPS_FLOATS] at d_ops
+        (ops_stride in floats); the synthesis stays pending."""
+        self._call("pnb_synthesis_operands_device", d_ops, ops_stride, stream)
 
     @property
     def device_bytes(self) -> int:

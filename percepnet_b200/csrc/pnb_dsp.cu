@@ -1034,6 +1034,172 @@ __global__ void __launch_bounds__(kSynWarps * 32) synthesis_kernel(SynthesisArgs
 }
 
 // ------------------------------------------------------------------------------------------
+// the synthesis's gradient with respect to g/r (include/pnb_synth_grad.h), one warp per (row, hop).  Hop t's output
+// is out[t][n] = x_t[n] hw[n] + x_{t-1}[480 + n] hw[479 - n], with x_t = Re(sum_i Y'_i e^{2 pi i i n / 960}) the
+// inverse transform of the Hermitian extension Y' of the gained spectrum Y (synthesis_kernel).  So, per hop:
+//   dx[n] = dout[t][n] hw[n],  dx[480 + m] = dout[t+1][m] hw[479 - m] (0 for the call's last hop: that half goes to
+//           the overlap-add memory of the next call)
+//   dY_k  = c_k sum_n dx[n] e^{-2 pi i k n / 960}, c_0 = 1, c_k = 2 (bins k and 960 - k fold onto k): one forward
+//           transform of the real vector dx
+//   Y_k = gf_k Z_k, Z_k = rfx_k X_k + rfp_k P_k (X_k on a silent hop), with gf, rfx, rfp interpolated from the band
+//           values g_used, 1 - r, r as interp_band_gain does:
+//           dgf_k = Re(conj(dY_k) Z_k),  d(rfp_k) - d(rfx_k) = gf_k Re(conj(dY_k) (P_k - X_k)) =: drf_k
+//   band b takes omf_k times the bins of band b and frac_k times the bins of band b - 1
+//   post-filter: g_used_b = G gw_b, gw_b = g_b sin(pi g_b / 2), G = sqrt((1 + beta) q / (1 + beta q^2)),
+//           q = e0 / (e1 + 1e-6), e0 = sum g_j Ey_j, e1 = sum gw_j Ey_j:
+//           dg_b = dgu_b G gw'_b + (sum_j dgu_j gw_j) dG/dq Ey_b (1 - q gw'_b) / (e1 + 1e-6)
+//           G = 0 (every g zero): g_used vanishes to second order, and dg is 0.
+// ------------------------------------------------------------------------------------------
+struct __align__(16) SynGradWarpSmem {  // 16-byte aligned: fft960_warp's first pass stores float4
+  float2 fft[kFftLine];  // the transform of dx; then the per-bin products, four arrays of kBins floats
+  float g[kBands], r[kBands], ir[kBands], gw[kBands], gu[kBands], dgu[kBands], dr[kBands];
+};
+struct SynGradBlockSmem {
+  FftTw ft;
+  float hw[kFrame];
+  float frac[kBins];
+  float omf[kBins];
+  short band_of[kBins];
+  short border[kBands + 2];
+};
+constexpr int kSgWarps = 8;
+static_assert(4 * kBins <= 2 * kFftLine, "the per-bin products do not fit the transform's line");
+static_assert(sizeof(SynGradWarpSmem) % 16 == 0, "every warp's transform line must start 16-byte aligned");
+
+__global__ void __launch_bounds__(kSgWarps * 32) synthesis_backward_kernel(SynthGradArgs A) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  SynGradBlockSmem &B = *reinterpret_cast<SynGradBlockSmem *>(smem_raw);
+  SynGradWarpSmem *Wall = reinterpret_cast<SynGradWarpSmem *>(smem_raw + ((sizeof(SynGradBlockSmem) + 15) / 16) * 16);
+  const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
+  const Tables *T = A.tab;
+  for (int i = threadIdx.x; i < kWin; i += blockDim.x) B.ft.tw[i] = T->tw[i];
+  for (int i = threadIdx.x; i < 4 * 192; i += blockDim.x) B.ft.tw5[i / 192][i % 192] = T->tw[(i / 192 + 1) * (i % 192)];
+  for (int i = threadIdx.x; i < kFrame; i += blockDim.x) B.hw[i] = T->half_window[i];
+  for (int i = threadIdx.x; i < kBins; i += blockDim.x) {
+    B.frac[i] = T->frac[i];
+    B.omf[i] = T->omf[i];
+    B.band_of[i] = T->band_of[i];
+  }
+  for (int i = threadIdx.x; i < kBands + 2; i += blockDim.x) B.border[i] = T->border[i];
+  __syncthreads();
+  SynGradWarpSmem &W = Wall[wib];
+  float *const vgf = reinterpret_cast<float *>(W.fft), *const vgo = vgf + kBins;  // dgf times frac / omf
+  float *const vrf = vgf + 2 * kBins, *const vro = vgf + 3 * kBins;               // drf times frac / omf
+  const float beta = 0.02f;
+  const long long units = A.n_rows * A.n_frames;
+  for (long long u = (long long)blockIdx.x * kSgWarps + wib; u < units; u += (long long)gridDim.x * kSgWarps) {
+    const long long row = u / A.n_frames;
+    const int t = (int)(u % A.n_frames);
+    const float *ops = A.ops + (size_t)row * A.ops_stride + (size_t)t * kSynthOps;
+    const float *Ey = ops + 4 * kBins;
+    const bool silence = ops[4 * kBins + kBands] != 0.f;
+    const float *gr = A.gr + (size_t)row * A.gr_stride + (size_t)t * 68;
+    const float *d0 = A.dout + (size_t)row * A.dout_stride + (size_t)t * kFrame;
+    const float *d1 = t + 1 < A.n_frames ? d0 + kFrame : nullptr;
+
+    // the band gains as the synthesis applied them
+    for (int b = lane; b < kBands; b += 32) {
+      const float g = gr[b], r = gr[kBands + b];
+      W.g[b] = g;
+      W.r[b] = r;
+      W.ir[b] = 1.f - r;
+      W.gw[b] = g * (float)sin((double)(float)(M_PI / 2 * (double)g));
+    }
+    __syncwarp();
+    float G = 0.f, q = 0.f, den = 0.f;
+    if (A.postfilter) {
+      if (lane == 0) {
+        float e0 = 0.f, e1 = 0.f;
+        for (int b = 0; b < kBands; b++) e0 += W.g[b] * Ey[b];
+        for (int b = 0; b < kBands; b++) e1 += W.gw[b] * Ey[b];
+        den = e1 + 1e-6f;
+        q = e0 / den;
+        G = sqrtf(((1.f + beta) * q) / (1.f + beta * (q * q)));
+      }
+      G = __shfl_sync(0xffffffffu, G, 0);
+      q = __shfl_sync(0xffffffffu, q, 0);
+      den = __shfl_sync(0xffffffffu, den, 0);
+    }
+    for (int b = lane; b < kBands; b += 32) W.gu[b] = A.postfilter ? G * W.gw[b] : W.g[b];
+
+    // dL/dY of bins 0..399: the forward transform of the windowed dL/d(out)
+    fft960_warp<false>(W.fft, B.ft, lane, [&](int i) {
+      float v;
+      if (i < kFrame) v = d0[i] * B.hw[i];
+      else v = d1 ? d1[i - kFrame] * B.hw[kWin - 1 - i] : 0.f;
+      return make_float2(v, 0.f);
+    });
+    constexpr int kPer = (kBins + 31) / 32;
+    float2 dY[kPer];
+#pragma unroll
+    for (int j = 0; j < kPer; j++) {
+      const int k = lane + 32 * j;
+      dY[j] = k < kBins ? W.fft[fpos(k)] : make_float2(0.f, 0.f);
+    }
+    __syncwarp();  // every lane has read the transform before the products overwrite it
+#pragma unroll
+    for (int j = 0; j < kPer; j++) {
+      const int k = lane + 32 * j;
+      if (k >= kBins) continue;
+      const float c = k == 0 ? 1.f : 2.f;
+      const float2 dy = make_float2(c * dY[j].x, c * dY[j].y);
+      const float2 x = make_float2(ops[2 * k], ops[2 * k + 1]);
+      const int b = B.band_of[k];
+      const float fr = B.frac[k], om = B.omf[k];
+      float2 z = x;
+      float drf = 0.f;
+      const float gf = om * W.gu[b] + fr * W.gu[b + 1];
+      if (!silence) {
+        const float2 p = make_float2(ops[2 * kBins + 2 * k], ops[2 * kBins + 2 * k + 1]);
+        const float rfx = om * W.ir[b] + fr * W.ir[b + 1], rfp = om * W.r[b] + fr * W.r[b + 1];
+        z = make_float2(rfx * x.x + rfp * p.x, rfx * x.y + rfp * p.y);
+        drf = gf * (dy.x * (p.x - x.x) + dy.y * (p.y - x.y));
+      }
+      const float dgf = dy.x * z.x + dy.y * z.y;
+      vgf[k] = fr * dgf;
+      vgo[k] = om * dgf;
+      vrf[k] = fr * drf;
+      vro[k] = om * drf;
+    }
+    __syncwarp();
+    // band b: omf-weighted bins of band b, frac-weighted bins of band b - 1
+    for (int b = lane; b < kBands; b += 32) {
+      float ag = 0.f, ar = 0.f;
+      if (b > 0)
+        for (int k = B.border[b - 1]; k < B.border[b]; k++) { ag += vgf[k]; ar += vrf[k]; }
+      if (b < kBands - 1)
+        for (int k = B.border[b]; k < B.border[b + 1]; k++) { ag += vgo[k]; ar += vro[k]; }
+      W.dgu[b] = ag;
+      W.dr[b] = ar;
+    }
+    __syncwarp();
+    float S = 0.f;  // sum_j dgu_j gw_j
+    if (A.postfilter) {
+      for (int b = lane; b < kBands; b += 32) S += W.dgu[b] * W.gw[b];
+      for (int o = 16; o > 0; o >>= 1) S += __shfl_xor_sync(0xffffffffu, S, o);
+    }
+    float *dgr = A.dgr + (size_t)row * A.dgr_stride + (size_t)t * 68;
+    for (int b = lane; b < kBands; b += 32) {
+      float dg = W.dgu[b];
+      if (A.postfilter) {
+        if (G == 0.f) {
+          dg = 0.f;
+        } else {
+          float s, c;
+          sincospif(0.5f * W.g[b], &s, &c);
+          const float gwp = s + W.g[b] * ((float)(M_PI / 2) * c);
+          const float dGdq = ((1.f + beta) * (1.f - beta * (q * q))) / (2.f * G * ((1.f + beta * (q * q)) * (1.f + beta * (q * q))));
+          dg = W.dgu[b] * (G * gwp) + S * dGdq * (Ey[b] * (1.f - q * gwp) / den);
+        }
+      }
+      dgr[b] = dg;
+      dgr[kBands + b] = silence ? 0.f : W.dr[b];
+    }
+    __syncwarp();  // the next unit overwrites the band arrays and the line
+  }
+}
+
+// ------------------------------------------------------------------------------------------
 // staging: append the new hops to each stream's PCM line / slide the history forward
 // ------------------------------------------------------------------------------------------
 __global__ void stage_in_kernel(float *pcm, size_t pcm_stride, const float *in, const short *in16, size_t in_stride,
@@ -1208,6 +1374,24 @@ bool launch_pitch_only(const PitchOnlyArgs &a, cudaStream_t st) {
 void launch_train_labels(const LabelArgs &a, cudaStream_t st) {
   const long total = (long)a.n_frames * a.n_pairs;
   train_labels_kernel<<<(unsigned)((total + 7) / 8), 256, 0, st>>>(a);
+}
+
+// a grid that fills the device once: each warp then walks units (row, hop) at a stride of the grid, so the block's
+// tables are staged once per block, not once per eight hops
+bool launch_synthesis_backward(const SynthGradArgs &a, cudaStream_t st) {
+  const size_t smem = ((sizeof(SynGradBlockSmem) + 15) / 16) * 16 + kSgWarps * sizeof(SynGradWarpSmem);
+  int dev = 0, sms = 0, per_sm = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess) return false;
+  if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) return false;
+  if (cudaFuncSetAttribute(synthesis_backward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
+    return false;
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, synthesis_backward_kernel, kSgWarps * 32, smem) != cudaSuccess ||
+      per_sm < 1)
+    return false;
+  const long long units = a.n_rows * a.n_frames, need = (units + kSgWarps - 1) / kSgWarps;
+  const long long full = (long long)sms * per_sm;
+  synthesis_backward_kernel<<<(unsigned)(need < full ? need : full), kSgWarps * 32, smem, st>>>(a);
+  return true;
 }
 
 void launch_synthesis(const SynthesisArgs &a, cudaStream_t st) {

@@ -19,6 +19,7 @@
 #include <stddef.h>
 #include <stdint.h>
 #include <algorithm>
+#include <mutex>
 #include <string>
 #include <vector>
 
@@ -667,10 +668,11 @@ static Rows pcm(const T *p, size_t stride) { return rows(p, stride, kFrame, size
 // One call as its entry point received it, its buffers as row arrays.  In / out: PCM / PCM of a slot, session or ragged
 // call; speech, noisy / records and (pnb_train_audio_*) audio of a training-record call; features or records / g/r of a
 // network call; records / g/r (when asked for) and the loss sums of a score call; PCM / features of an analysis; g/r /
-// PCM of a synthesis; features / g/r of a training forward; dL/d(out) / dL/dx (when asked for) of a training backward.  An analysis, synthesis or network call on a session list (pool) has ids too; its analysis and
+// PCM of a synthesis; - / the operands of the pending synthesis (kOperands); features / g/r of a training forward; dL/d(out) / dL/dx (when asked for) of a training backward.  An analysis, synthesis or network call on a session list (pool) has ids too; its analysis and
 // network forms may have hops.
 struct Call {
-  enum Kind { kSlots, kSessions, kRagged, kNetwork, kRecords, kAnalyze, kSynthesize, kTrain, kTrainForward, kTrainBackward } kind;
+  enum Kind { kSlots, kSessions, kRagged, kNetwork, kRecords, kAnalyze, kSynthesize, kOperands, kTrain, kTrainForward,
+              kTrainBackward } kind;
   Rows in[2], out[2];
   int F;           // hops; a ragged call's is max(hops), set by check_call
   float *gr;       // enhancement calls: g/r destination [F][rows][68], or null
@@ -881,6 +883,19 @@ static int enqueue_synthesize(pnb_engine *e, const Call &c, cudaStream_t st) {
   return rc;
 }
 
+// The operands of the pending synthesis on st (arguments already checked, an analysis of F hops pending): one launch
+// that reads what synthesis_kernel will read, through the same SynthesisArgs.  Neither the signal state, the hop counter
+// nor the pending synthesis changes, so it is ordered like a call but commits nothing.
+static int enqueue_operands(pnb_engine *e, const Call &c, cudaStream_t st) {
+  const Rows &ops = c.out[0];
+  return enqueue_ordered(e, st, [&]() -> int {
+    const SynthesisArgs sa = synthesis_args(e, c.F, nullptr, nullptr, 0);
+    LaunchScope m(e, PNB_K_STAGE_IN, st);
+    launch_synth_ops(sa, static_cast<float *>(ops.p), ops.stride, st);
+    return PNB_OK;
+  });
+}
+
 // A gradient call on st (arguments already checked): the trainer's forward, loss and backward on the records of windows
 // [0, n_active), each from zero state; the loss sums to the caller, the gradient into the engine's buffer.  Neither the
 // network state of the slots nor the signal state is touched.
@@ -928,6 +943,7 @@ static int enqueue(pnb_engine *e, const Call &c, cudaStream_t st) {
     case Call::kRecords: return enqueue_records(e, c, st);
     case Call::kAnalyze: return enqueue_analyze(e, c, st);
     case Call::kSynthesize: return enqueue_synthesize(e, c, st);
+    case Call::kOperands: return enqueue_operands(e, c, st);
     case Call::kTrain: return enqueue_train(e, c, st);
     case Call::kTrainForward: return enqueue_train_forward(e, c, st);
     case Call::kTrainBackward: return enqueue_train_backward(e, c, st);
@@ -1000,7 +1016,8 @@ static int check_pending_list(const pnb_engine *e, const Call &c) {
 // enhancement or the network alone; a PNB_NETWORK_ONLY engine runs network calls only, a PNB_SIGNAL_ONLY engine split
 // calls only) that no failed call has poisoned, 1 <= F <= Fmax, none of its arrays NULL, the input strides; a
 // training-record call then that its engine has audio exactly when the call does; every call then the output strides,
-// and the pending synthesis: a synthesis needs one of F hops (on a session list: the pending list), a network call on a
+// and the pending synthesis: a synthesis needs one of F hops (on a session list: the pending list), an operand export one
+// whose hops it takes, a network call on a
 // session list while one is pending the pending list and hops, every other call but a network call none.  After that a
 // slot or split call checks session mode, a session call its list, a network call its format, then session mode, and a
 // score call its frames.  A ragged call, and a split or network call on a session list, checks the list first (so
@@ -1026,7 +1043,7 @@ static int check_call(pnb_engine *e, Call &c) {
   }
   const bool trainer = c.kind == Call::kTrain || c.kind == Call::kTrainForward || c.kind == Call::kTrainBackward;
   const bool train = c.kind == Call::kRecords, network = c.kind == Call::kNetwork || trainer;
-  const bool split = c.kind == Call::kAnalyze || c.kind == Call::kSynthesize;
+  const bool split = c.kind == Call::kAnalyze || c.kind == Call::kSynthesize || c.kind == Call::kOperands;
   if (!e) return fail(PNB_ERR_ARG, "engine is NULL");
   if (!network && (e->flags & PNB_NETWORK_ONLY))
     return fail(PNB_ERR_ARG, "engine was created with PNB_NETWORK_ONLY: use pnb_compute_rnn_* / pnb_score_records_*");
@@ -1044,6 +1061,10 @@ static int check_call(pnb_engine *e, Call &c) {
   if (!train && (e->flags & PNB_TRAIN_DATA))
     return fail(PNB_ERR_ARG, "engine was created with PNB_TRAIN_DATA: use pnb_train_records_* / pnb_submit_train_records");
   if (e->poisoned) return refuse_poisoned(PNB_ERR_CUDA);
+  if (c.kind == Call::kOperands) {  // the hops of the pending synthesis
+    if (!e->pending.F) return fail(PNB_ERR_ARG, "no analysis awaits its synthesis: call pnb_analyze_* first");
+    c.F = e->pending.F;
+  }
   if (c.F < 1 || c.F > e->Fmax) return fail(PNB_ERR_ARG, "n_frames %d outside [1, %d]", c.F, e->Fmax);
   for (int i = 0; i < 2; i++)
     if ((c.in[i].width && !c.in[i].p) || (c.out[i].width && !c.out[i].p))
@@ -1054,7 +1075,7 @@ static int check_call(pnb_engine *e, Call &c) {
   if (train && !audio && (e->flags & PNB_TRAIN_AUDIO))
     return fail(PNB_ERR_ARG, "engine was created with PNB_TRAIN_AUDIO: use pnb_train_audio_*, so that its audio has no gaps");
   { int rc = check_strides(c.out, c.F); if (rc) return rc; }
-  if (c.kind == Call::kSynthesize) {
+  if (c.kind == Call::kSynthesize || c.kind == Call::kOperands) {
     if (!e->pending.F) return fail(PNB_ERR_ARG, "no analysis awaits its synthesis: call pnb_analyze_* first");
     if (c.F != e->pending.F) return fail(PNB_ERR_ARG, "n_frames %d, but the pending analysis has %d hops", c.F, e->pending.F);
     if (c.pool) { int rc = check_pending_list(e, c); if (rc) return rc; }
@@ -1522,6 +1543,12 @@ extern "C" int pnb_synthesize_device_i16(pnb_engine *e, const float *d_gr, size_
                                          size_t out_stride, void *cuda_stream) {
   return device_call(e, synthesize_call(d_gr, gr_stride, n_frames, d_out, sizeof(short), out_stride), (cudaStream_t)cuda_stream);
 }
+// The operands of the pending synthesis (include/pnb_synth_grad.h): a split call with no input, whose hops are the
+// pending analysis's.
+extern "C" int pnb_synthesis_operands_device(pnb_engine *e, float *d_ops, size_t ops_stride, void *cuda_stream) {
+  return device_call(e, {Call::kOperands, {}, {rows(d_ops, ops_stride, kSynthOps, sizeof(float), "ops_stride")}, 0},
+                     (cudaStream_t)cuda_stream);
+}
 
 // The split and network calls on a session list: row i of every array belongs to ids[i]; hops NULL, or each listed
 // session's own hops (ragged, n_frames = max(hops)).  The synthesis takes the list, hops and rows of the pending analysis.
@@ -1975,6 +2002,57 @@ extern "C" int pnb_pitch_only_device(const float *d_pitch_buf, size_t stride, lo
   a.T = d_period; a.corr = d_corr; a.gain = d_gain; a.lag = d_lag;
   // uncounted: there is no engine to count it
   if (!launch_pitch_only(a, (cudaStream_t)cuda_stream)) return fail(PNB_ERR_CUDA, "pitch_only_kernel could not be configured");
+  CK(cudaGetLastError());
+  return PNB_OK;
+}
+
+// ------------------------------------------------------------------------------------------
+// the synthesis's gradient with respect to g/r (include/pnb_synth_grad.h)
+// ------------------------------------------------------------------------------------------
+// The constant tables on the current device, uploaded by the first call there and kept for the process (there is no
+// engine to own them); null when the upload failed.
+static const Tables *device_tables() {
+  static std::mutex mu;
+  static std::vector<Tables *> per_device;
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess) return nullptr;
+  std::lock_guard<std::mutex> lock(mu);
+  if ((size_t)dev >= per_device.size()) per_device.resize(dev + 1, nullptr);
+  if (!per_device[dev]) {
+    Tables h;
+    build_tables(h);
+    Tables *d = nullptr;
+    if (cudaMalloc((void **)&d, sizeof(Tables)) != cudaSuccess) return nullptr;
+    if (cudaMemcpy(d, &h, sizeof(Tables), cudaMemcpyHostToDevice) != cudaSuccess) {
+      cudaFree(d);
+      return nullptr;
+    }
+    per_device[dev] = d;
+  }
+  return per_device[dev];
+}
+
+extern "C" int pnb_synthesis_backward_device(const float *d_ops, size_t ops_stride, const float *d_gr, size_t gr_stride,
+                                             long long n_rows, int n_frames, int postfilter, const float *d_dout,
+                                             size_t dout_stride, float *d_dgr, size_t dgr_stride, void *cuda_stream) {
+  if (!d_ops || !d_gr || !d_dout || !d_dgr) return fail(PNB_ERR_ARG, "NULL argument");
+  if (n_rows < 1) return fail(PNB_ERR_ARG, "n_rows %lld below 1", n_rows);
+  if (n_frames < 1) return fail(PNB_ERR_ARG, "n_frames %d below 1", n_frames);
+  if (postfilter != 0 && postfilter != 1) return fail(PNB_ERR_ARG, "postfilter %d is neither 0 nor 1", postfilter);
+  const size_t F = (size_t)n_frames;
+  if (ops_stride < F * kSynthOps) return fail(PNB_ERR_ARG, "ops_stride smaller than n_frames*%d", kSynthOps);
+  if (gr_stride < F * 68) return fail(PNB_ERR_ARG, "gr_stride smaller than n_frames*68");
+  if (dout_stride < F * kFrame) return fail(PNB_ERR_ARG, "dout_stride smaller than n_frames*%d", kFrame);
+  if (dgr_stride < F * 68) return fail(PNB_ERR_ARG, "dgr_stride smaller than n_frames*68");
+  SynthGradArgs a;
+  a.ops = d_ops; a.ops_stride = ops_stride; a.gr = d_gr; a.gr_stride = gr_stride; a.dout = d_dout;
+  a.dout_stride = dout_stride; a.dgr = d_dgr; a.dgr_stride = dgr_stride; a.n_rows = n_rows; a.n_frames = n_frames;
+  a.postfilter = postfilter;
+  a.tab = device_tables();
+  if (!a.tab) return fail(PNB_ERR_CUDA, "the constant tables could not be uploaded to the current device");
+  // uncounted: there is no engine to count it
+  if (!launch_synthesis_backward(a, (cudaStream_t)cuda_stream))
+    return fail(PNB_ERR_CUDA, "synthesis_backward_kernel could not be configured");
   CK(cudaGetLastError());
   return PNB_OK;
 }

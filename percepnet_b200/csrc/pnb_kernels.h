@@ -80,6 +80,25 @@ struct PitchOnlyArgs {
 };
 bool launch_pitch_only(const PitchOnlyArgs &a, cudaStream_t st);
 
+// The synthesis's gradient with respect to g/r (include/pnb_synth_grad.h): one warp per (row, hop) of n_rows rows of
+// n_frames hops; strides in floats.  Returns false, launching nothing, when the kernel cannot be configured.
+constexpr int kSynthOps = 1636;  // PNB_SYNTH_OPS_FLOATS: X [800], P [800], Ex [34], silence, padding
+struct SynthGradArgs {
+  const float *ops;
+  size_t ops_stride;
+  const float *gr;
+  size_t gr_stride;
+  const float *dout;
+  size_t dout_stride;
+  float *dgr;
+  size_t dgr_stride;
+  long long n_rows;
+  int n_frames;
+  int postfilter;
+  const Tables *tab;
+};
+bool launch_synthesis_backward(const SynthGradArgs &a, cudaStream_t st);
+
 cudaError_t dsp_configure();
 void launch_analysis(const AnalysisArgs &a, cudaStream_t st);
 void launch_synthesis(const SynthesisArgs &a, cudaStream_t st);
@@ -102,6 +121,9 @@ void launch_rows_stage(float *dst, int w, const float *in, size_t in_stride, int
 // each slot, or null: n_frames; a row is zero for the hops its slot did not run
 void launch_rows_store(const float *src, int w, float *out, size_t out_stride, int n_streams, int S, int n_frames,
                        cudaStream_t st, const int *slot = nullptr, const int *hops = nullptr);
+// the operands synthesis_kernel reads for the rows [0, a.n_streams) and hops [0, a.n_frames) of the synthesis `a`
+// (zring, ring, hop0, P, Ex, silence, stride) -> ops rows of n_frames x kSynthOps floats
+void launch_synth_ops(const SynthesisArgs &a, float *ops, size_t ops_stride, cudaStream_t st);
 // rnn_train.py's CustomLoss sums of rows [0, n_streams): gr [F][S][68] against the labels rec[t][70..137] of row i's
 // first frames[i] hops (frames null: all n_frames) -> sums[i] = {sum dg^2, sum dg^4, sum dr^2, count} in float64
 void launch_loss_sums(const float *gr, const float *rec, size_t rec_stride, const int *frames, double *sums, int n_streams,

@@ -1,8 +1,9 @@
 // pnb_rnn_io.cu -- the layout moves between a caller's stream-major rows and the per-call buffers [F][S][w] of the
 // engine: the network call's features or training records into d_feat and its g/r out of d_gr (pnb_compute_rnn_*), the
 // analysis half's features out of d_feat (pnb_analyze_*) and the synthesis half's caller g/r into d_gr
-// (pnb_synthesize_*), and the same on a session list (row-mapped, with per-slot hops); and the loss of a score call (pnb_score_records_*), reduced from the same g/r and the records'
-// labels.
+// (pnb_synthesize_*), and the same on a session list (row-mapped, with per-slot hops); the operands of a pending
+// synthesis out to the caller's rows (pnb_synthesis_operands_device); and the loss of a score call (pnb_score_records_*),
+// reduced from the same g/r and the records' labels.
 #include "../../include/percepnet_b200.h"
 #include "pnb_kernels.h"
 
@@ -48,6 +49,37 @@ __global__ void rows_store_kernel(const float *__restrict__ src, float *__restri
     const int t = (int)(rt % F), r = (int)(rt / F);
     const int s = kMapped ? slot[r] : r;
     out[(size_t)r * out_stride + (size_t)t * W + c] = (kMapped && hops && t >= hops[s]) ? 0.f : src[((size_t)t * S + s) * W + c];
+  }
+}
+
+// The operands of the pending synthesis (include/pnb_synth_grad.h): ops[r*ops_stride + t*1636 + j] for the rows r of
+// [0, n) and hops t of [0, F), read at exactly the addresses synthesis_kernel reads for slot r at hop t: X from the ring
+// slot of hop hop0 + t - 5 (a call's first five hops read spectra of the previous call), P, Ex and the silence flag from
+// the per-call buffers.  Threads walk the output in order: the writes are contiguous, the reads runs of 800 or 34 floats.
+__global__ void synth_ops_kernel(const float2 *__restrict__ zring, int ring, long hop0, const float2 *__restrict__ P,
+                                 const float *__restrict__ Ex, const unsigned char *__restrict__ silence,
+                                 float *__restrict__ ops, size_t ops_stride, int n, int S, int F) {
+  const long long total = (long long)n * F * kSynthOps;
+  for (long long x = (long long)blockIdx.x * blockDim.x + threadIdx.x; x < total; x += (long long)gridDim.x * blockDim.x) {
+    const int j = (int)(x % kSynthOps);
+    const long long rt = x / kSynthOps;
+    const int t = (int)(rt % F), r = (int)(rt / F);
+    const size_t fs = (size_t)t * S + r;
+    float v = 0.f;
+    if (j < 2 * kBins) {
+      const long c = hop0 + t;
+      const int slot_x = (int)(((c - 5) % ring + ring) % ring);
+      const float2 z = zring[((size_t)slot_x * S + r) * kBins + j / 2];
+      v = (j & 1) ? z.y : z.x;
+    } else if (j < 4 * kBins) {
+      const float2 p = P[fs * kBins + (j - 2 * kBins) / 2];
+      v = (j & 1) ? p.y : p.x;
+    } else if (j < 4 * kBins + kBands) {
+      v = Ex[fs * kBands + j - 4 * kBins];
+    } else if (j == 4 * kBins + kBands) {
+      v = silence[fs] != 0 ? 1.f : 0.f;
+    }
+    ops[(size_t)r * ops_stride + (size_t)t * kSynthOps + j] = v;
   }
 }
 
@@ -125,6 +157,11 @@ void launch_rows_store(const float *src, int w, float *out, size_t out_stride, i
   const unsigned blocks = copy_blocks((long long)n_frames * n_streams * w);
   if (w == kFeat) rows_store<kFeat>(blocks, src, out, out_stride, n_streams, S, n_frames, slot, hops, st);
   else rows_store<68>(blocks, src, out, out_stride, n_streams, S, n_frames, slot, hops, st);
+}
+
+void launch_synth_ops(const SynthesisArgs &a, float *ops, size_t ops_stride, cudaStream_t st) {
+  synth_ops_kernel<<<copy_blocks((long long)a.n_streams * a.n_frames * kSynthOps), 256, 0, st>>>(
+      a.zring, a.ring, a.hop0, a.P, a.Ex, a.silence, ops, ops_stride, a.n_streams, a.stride, a.n_frames);
 }
 
 void launch_loss_sums(const float *gr, const float *rec, size_t rec_stride, const int *frames, double *sums, int n_streams,

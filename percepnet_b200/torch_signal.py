@@ -162,6 +162,28 @@ class SignalPath:
             with torch.cuda.device(self.device):
                 self._eng.reset_streams(rows, torch.cuda.current_stream().cuda_stream)
 
+    def _check_states(self, what: str):
+        if self._eng is None:
+            raise RuntimeError(f"SignalPath.{what}: the path has no streams before its first analyze")
+        if self._pending is not None:
+            raise RuntimeError(f"SignalPath.{what}: an analysis is pending (its streams are mid-hop): synthesize it "
+                               "first")
+
+    def export_states(self, rows) -> torch.Tensor:
+        """The state blobs of the listed streams of the last call's [0, B): CUDA uint8 [len(rows), pnb_state_size()]
+        (pnb_export_states; the signal part, the network part zero), e.g. to checkpoint a run between windows.
+        Refused before the first analyze and while an analysis is pending."""
+        self._check_states("export_states")
+        with torch.cuda.device(self.device):
+            return self._eng.export_states(rows, None, stream=torch.cuda.current_stream().cuda_stream)
+
+    def import_states(self, rows, blobs: torch.Tensor):
+        """The listed streams continue from the blobs of export_states (CUDA uint8 [len(rows), pnb_state_size()], on
+        the path's device; pnb_import_states, the network part ignored).  Refused as export_states."""
+        self._check_states("import_states")
+        with torch.cuda.device(self.device):
+            self._eng.import_states(rows, blobs, stream=torch.cuda.current_stream().cuda_stream)
+
     def close(self):
         """Frees the engine (the next analyze creates a fresh one)."""
         if self._eng is not None:
